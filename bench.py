@@ -1,19 +1,22 @@
 #!/usr/bin/env python
 """bench.py — exact-GP log-marginal + gradient evaluations per second (fp64), the metric of BASELINE.json.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--n 16384] [--d 8]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--n 16384] [--d 8] [--dump-outputs DIR]
 
 One "step" = one evaluation (= one GP.parameters_changed(), GPy/core/gp.py:269-282): theta -> log marginal likelihood and
 its gradient w.r.t. (variance, D lengthscales, noise) for GPRegression RBF ARD on the synthetic workload of
-SURVEY.md §8(d) (BASELINE.json configs[1]: N=16384, D=8, fp64, 1xB200).
+SURVEY.md §8(d) (BASELINE.json configs[1]: N=16384, D=8, fp64, 1xH100).
 
 `value`  : evaluations/s with X, Y resident in HBM (theta in, (LML, grad) out each step), device-timed.
 `e2e`    : the same metric through the reference-facing plugin API (gpy_b200.GPRegression over the C ABI) with HOST
            buffers: every step copies X and Y host->device and reads (LML, grad) back, inside the timed region.
-`roofline`: dominant kernel = the digit-split int8 GEMM on the tcgen05 tensor cores (trailing update + K^-1); achieved = the
-           int8 tensor operations it issues / its CUDA-event time, measured live over the timed steps; peak = 2 x the
-           measured dense bf16 rate (MEASURED_PEAKS.json). On the fp64 DMMA path (option ozaki = 0, multi-GPU) the kernel
-           is the DMMA GEMM and the peak the DMMA issue rate measured in the same run.
+`roofline`: dominant kernel = the fp64 DMMA trailing-update GEMM (the default path); achieved = its flops / its CUDA-event
+           time; peak = the DMMA.16x8x4 issue rate measured in the same run. With GPX_OZAKI=1 the kernel is the digit-split
+           int8 GEMM on the wgmma tensor cores (trailing update + K^-1): achieved = the int8 tensor operations it issues /
+           its CUDA-event time, peak = the H100 SXM data-sheet dense int8 rate.
+`--dump-outputs DIR`: after the timed steps, the outputs of the last timed step (log marginal, gradient, extra jitter;
+           sparse: log marginal and the gradient vector) as DIR/<name>.npy in float64. Inputs are seeded, so two builds
+           run with the same arguments can be compared output for output.
 `cpu_baseline` / `--impl reference`: the reference's own CPU operation sequence (oracle/gpy_oracle.py: same LAPACK/BLAS
            calls incl. the wasted dtrtri, two exp passes, the serial ARD loop compiled from C) on this box's cores.
 """
@@ -55,7 +58,7 @@ def theta_for_step(D, step):
 
 
 class ClockSampler(object):
-    """nvidia-smi sampler for the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler for the timed region: SM clock, power and throttle reasons."""
 
     def __init__(self, gpu_index=0):
         self.gpu_index = gpu_index
@@ -106,15 +109,15 @@ class ClockSampler(object):
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
-def measured_peaks():
-    """dense bf16 TFLOP/s (sustained) measured by the driver on this pool (MEASURED_PEAKS.json), else the fallback of
-    B200_PROFILING.md (1.4 PFLOP/s sustained) -> (value, source)"""
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            mp = json.load(f)
-        return float(mp.get("bf16_tflops_sustained") or mp["bf16_tflops"]), "MEASURED_PEAKS.json (measured)"
-    except Exception:
-        return 1400.0, "B200_PROFILING.md fallback (1.4 PFLOP/s sustained bf16)"
+# NVIDIA H100 SXM data sheet, dense int8 tensor rate (700 W card); a card set to a lower power limit reaches less
+H100_INT8_TOPS = 1979.0
+
+
+def dump_outputs(dirname, arrays):
+    """write each output of the last timed step as DIR/<name>.npy (float64)"""
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(dirname, name + ".npy"), np.asarray(a, dtype=np.float64).reshape(-1))
 
 
 def dist_env():
@@ -163,18 +166,16 @@ def run_reference(args):
     threads, infos = cpu_threads()
     for w in range(args.warmup):
         cpu_eval_timed(min(N, 2048), D, -1 - w, native)   # warm-up on a small instance: BLAS threads, page cache
-    # Every step is one COMPLETE evaluation at the full size (no extrapolation). One such evaluation takes of the
-    # order of a minute on the host cores, so the run is time-bounded: steps stop once GPX_REF_BUDGET_S (default 240 s)
-    # is spent; at least one step always runs. `steps` in the JSON line is the number actually timed.
-    budget = float(os.environ.get("GPX_REF_BUDGET_S", "240"))
+    # Every step is one COMPLETE evaluation at the full size (no extrapolation); one such evaluation takes of the
+    # order of a minute on the host cores.
     times = []
     t_start = time.perf_counter()
     for s in range(args.steps):
         dt, lml, grad = cpu_eval_timed(N, D, s, native)
         times.append(dt)
-        if time.perf_counter() - t_start + dt > budget:
-            break
     total = time.perf_counter() - t_start
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"lml": [lml], "grad": grad})
     per = float(np.mean(times))
     blas = ", ".join(sorted({"%s %s" % (i.get("internal_api"), i.get("version")) for i in infos}))
     line = {
@@ -189,8 +190,7 @@ def run_reference(args):
                            "dpotri, dpotrs, Cython helpers (symmetrify, serial ARD loop) restated in C, paramz caching "
                            "of r and K modelled"},
         "cpu_baseline": {"value": 1.0 / per, "unit": UNIT, "cores": threads, "kind": "port",
-                         "sample": "%d of %d requested steps, each one complete evaluation at N=%d (time-bounded to %.0f s; "
-                                   "warm-up at N=2048)" % (len(times), args.steps, N, budget),
+                         "sample": "%d steps, each one complete evaluation at N=%d (warm-up at N=2048)" % (len(times), N),
                          "host_cpus": os.cpu_count(), "blas": blas},
         "e2e": {"value": 1.0 / per, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "wall_s": total,
@@ -223,8 +223,8 @@ def run_ours(args):
 
     X, Y = synthetic(N, D)
     eng = _ffi.Engine(local)
-    # N > 1 GPUs. A matrix that fits one GPU is evaluated fastest by ONE GPU (the tcgen05 path is single-GPU; at N = 16384 one
-    # B200 finishes an evaluation sooner than 2-8 GPUs sharing it, whose strong scaling is bound by the serial diagonal-block
+    # N > 1 GPUs. A matrix that fits one GPU is evaluated fastest by ONE GPU (the Ozaki path is single-GPU; at N = 16384 one
+    # GPU finishes an evaluation sooner than 2-8 GPUs sharing it, whose strong scaling is bound by the serial diagonal-block
     # chain and the per-panel collectives) — so for N <= 32768 the N GPUs run INDEPENDENT evaluations (different theta per
     # rank: multi-restart optimisation, the reference's own data-parallel pattern, paramz Model.optimize_restarts(parallel=
     # True)), no data-path collective, weak scaling; the sharded evaluation of the same size is measured and reported beside
@@ -259,6 +259,8 @@ def run_ours(args):
         upd_i8 += st.get("update_int8_ops", 0.0)
     barrier()
     wall = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"lml": [last[0]], "grad": last[1], "jitter": [last[2]]})
     launches = eng.total_launches() - launches0
     clocks = sampler.stop() if rank == 0 else None
     t_dev = float(np.sum(dev_ms)) * 1e-3          # CUDA-event time of the K evaluations on the launching stream
@@ -294,7 +296,7 @@ def run_ours(args):
         dist.all_reduce(e2e_t, op=dist.ReduceOp.MAX)
     e2e_value = (1 if sharded or world == 1 else world) * e2e_steps / float(e2e_t[0])
 
-    # ---- parity carried by the bench line itself when N > 1 (the driver's SCALE run has no other parity evidence) ---------
+    # ---- parity carried by the bench line itself when N > 1 ----------------------------------------------------------------
     parity_multi = None
     eng_s = eng if sharded else None
     if use_dist and not sharded:
@@ -357,30 +359,23 @@ def run_ours(args):
                  "share_of_step": upd_ms / (t_dev * 1e3) if t_dev else None,
                  "launches": (upd_launches / args.steps) if upd_launches else None}
         if upd_i8 > 0 and upd_ms > 0:
-            # tcgen05 path: the dominant kernel is the int8 digit-split GEMM (trailing update + K^-1 in the same launches).
+            # Ozaki path: the dominant kernel is the int8 digit-split GEMM (trailing update + K^-1 in the same launches).
             # achieved = int8 tensor operations actually issued (2 per MAC, summed over the digit pairs computed: 36 per
-            # fp64 product with 8 digits, 28 with 7) / CUDA-event time of those launches; peak = 2 x the measured dense bf16
-            # rate of MEASURED_PEAKS.json (kind::i8 issues at exactly twice the kind::f16 rate on this part:
-            # profiles/r02_microbench_tcgen05_i8_width_sweep.txt), the sustained figure because the kernel is timed inside a
-            # long step.
-            mp, src = measured_peaks()
-            i8_peak = 2.0 * mp
+            # fp64 product with 8 digits, 28 with 7) / CUDA-event time of those launches; peak = the data-sheet dense int8
+            # rate of the H100 SXM.
             ach = upd_i8 / upd_ms * 1e-9
-            roofline = {"bound": "tensor", "kernel": "oz_gemm2_kernel (tcgen05.mma kind::i8 digit-split GEMM, 128x128x32 MMAs in two "
-                                                      "passes: trailing update + K^-1)",
-                        "achieved": ach, "peak": i8_peak, "unit": "TFLOP/s", "frac": ach / i8_peak,
+            roofline = {"bound": "tensor", "kernel": "oz_gemm_kernel (wgmma s8 digit-split GEMM, 64x64x32 MMAs: trailing "
+                                                      "update + K^-1)",
+                        "achieved": ach, "peak": H100_INT8_TOPS, "unit": "TFLOP/s", "frac": ach / H100_INT8_TOPS,
                         "unit_note": "int8 tensor operations (2 per multiply-add), not floating point",
-                        "peak_source": "2 x bf16_tflops_sustained of %s" % src,
-                        # for context: the kind::i8 ISSUE rate of this part (8192 MAC/clk/SM, tools/microbench_tcgen05.cu) at the
-                        # SM clock sampled during this run; cuBLAS bf16 itself reaches ~0.73 of the corresponding bf16 issue rate
-                        "frac_of_i8_issue_rate": ach / (2 * 8192 * 148 * (clocks["sm_mhz"] or 1965.0) * 1e-6)
+                        "peak_source": "H100 SXM data sheet, dense int8 (700 W)",
+                        # for context: the dense int8 rate (4096 MAC/clk/SM x 132 SMs) at the SM clock sampled during this run
+                        "frac_of_i8_issue_rate": ach / (2 * 4096 * 132 * clocks["sm_mhz"] * 1e-6)
                         if clocks and clocks.get("sm_mhz") else None,
                         "fp64_equivalent_tflops": upd_flops / upd_ms * 1e-9,
                         "algorithmic_flops_per_step": upd_flops / args.steps,
                         "traffic": None,
-                        "traffic_note": "not measured in this run; per-launch DRAM traffic differs launch to launch (16 panels): the ncu "
-                                        "capture of the same path (profiles/r02s3_final_oz_traffic.txt) has 2.61 GB per large launch "
-                                        "(1.8 GB read + 0.9 GB written) at N=16384",
+                        "traffic_note": "not measured",
                         "grad_from_kinv_ms_per_step": lau_ms / args.steps}
         else:
             ach = upd_flops / upd_ms * 1e-9 if upd_ms > 0 else 0.0
@@ -389,8 +384,7 @@ def run_ours(args):
                         "frac": ach / peak if (peak and upd_ms > 0) else None,
                         "note": None if upd_ms > 0 else "per-kernel event accounting is single-GPU; see whole_eval_*",
                         "traffic": None,
-                        "peak_source": "fp64 DMMA.8x8x4 issue rate measured in this run (gpx_measure_fp64_peak); "
-                                       "MEASURED_PEAKS.json holds no fp64 entry",
+                        "peak_source": "fp64 DMMA.16x8x4 issue rate measured in this run (gpx_measure_fp64_peak)",
                         "lauum_tflops": lau_flops / lau_ms * 1e-9 if lau_ms else None}
         roofline.update(whole)
         line = {
@@ -437,7 +431,7 @@ def run_sparse(args):
     import torch
     rank, world, local = dist_env()
     if world > 1 and rank != 0:
-        return                                   # replicas only: the driver's line comes from rank 0 (row sharding: tools/)
+        return                                   # replicas only: the JSON line comes from rank 0
     torch.cuda.set_device(local)
     import gpy_b200
     N, M, D = args.n if args.n != 16384 else 262144, args.m, args.d if args.d != 8 else 16
@@ -471,6 +465,8 @@ def run_sparse(args):
         step(i, False)
     torch.cuda.synchronize()
     t_res = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"lml": [m.log_likelihood()], "grad": np.asarray(m.gradient)})
     launches = eng.total_launches() - l0
     clocks = sampler.stop()
     torch.cuda.synchronize()
@@ -535,6 +531,8 @@ def main():
     ap.add_argument("--workload", default="exact", choices=["exact", "sparse"],
                     help="exact = BASELINE.json configs[1] (the metric); sparse = configs[4] (VarDTC, N=262144 M=4096 D=16)")
     ap.add_argument("--m", type=int, default=4096, help="inducing points (sparse workload)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64)")
     ap.add_argument("--mode", default="auto", choices=["auto", "sharded", "replicas"],
                     help="N>1 GPUs: auto = independent evaluations per GPU while the matrix fits one GPU (N <= 32768), one "
                          "sharded evaluation beyond; or force either")

@@ -1,8 +1,8 @@
-"""gpy_b200 — B200-native exact-GP engine behind GPy's kernel / exact-inference plugin interface.
+"""gpy_b200 — H100 exact-GP engine behind GPy's kernel / exact-inference plugin interface.
 
 Host side (Python, mirrors the reference's operator interface for the hot path) over a ctypes C ABI
-(include/gpx.h) into hand-written sm_100a CUDA (gpy_b200/csrc). No CPU fallback: importing works everywhere,
-computing requires libgpx.so and a B200.
+(include/gpx.h) into hand-written sm_90a CUDA (gpy_b200/csrc). No CPU fallback: importing works everywhere,
+computing requires libgpx.so and an H100.
 """
 from . import _ffi  # noqa: F401
 from ._ffi import Engine, GpxError, kern_K, kern_Kdiag, kern_grad_full  # noqa: F401

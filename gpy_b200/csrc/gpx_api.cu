@@ -1,4 +1,4 @@
-// gpx_api.cu — C ABI (include/gpx.h) and host orchestration of the exact-GP evaluation on one B200.
+// gpx_api.cu — C ABI (include/gpx.h) and host orchestration of the exact-GP evaluation on one H100.
 //
 // One evaluation (= one GP.parameters_changed(), GPy/core/gp.py:269-282):
 //   prep_x -> kbuild (Ky into the workspace S) -> unified blocked factor-and-invert sweep (S: lower = L, upper = U = L^-T)
@@ -65,8 +65,7 @@ static long pick_nb(const gpx_ctx* c) {
   if (c->NB > 0) return std::min<long>(c->NB, c->Npad);
   const char* e = getenv("GPX_NB");
   if (e && atol(e) >= TILE && atol(e) % TILE == 0) return std::min<long>(atol(e), c->Npad);
-  // measured with the chain schedule (profiles/r02s2_chain_ab.txt): N = 16384: 1024 (66.8 ms; 512: 76.3, 2048: 73.4);
-  // N = 8192: 512 (12.65 vs 13.15 ms); N = 4096: 512 (3.27; 256: 3.80, 1024: 3.76); N = 512: one block (0.467 vs 0.506 ms)
+  // outer block by size (chosen with the chain schedule): 1024 above N = 8192, 512 from 2048, one block up to 512
   if (c->Npad > 8192) return 1024;
   if (c->Npad >= 2048) return 512;
   if (c->Npad <= 512) return c->Npad;
@@ -91,7 +90,7 @@ int gpx::fill_kp(KernParams& kp, int kind, int ard, int D, double variance, cons
 extern "C" {
 
 const char* gpx_last_error(void) { return gpx::g_err.c_str(); }
-const char* gpx_version(void) { return "gpx 0.2 (sm_100a: tcgen05 int8 digit-split GEMM + fp64 DMMA)"; }
+const char* gpx_version(void) { return "gpx 0.2 (sm_90a: wgmma int8 digit-split GEMM + fp64 DMMA)"; }
 
 int gpx_device_count(void) {
   int n = 0;
@@ -177,7 +176,6 @@ int gpx_set_option(gpx_ctx* c, const char* name, int64_t value) {
     return 0;
   }
   if (!strcmp(name, "oz_ctas")) { c->oz_ctas = (int)std::max<int64_t>(0, value); return 0; }
-  if (!strcmp(name, "oz_dbg")) { c->oz_dbg = (int)value; return 0; }
   if (!strcmp(name, "oz_tpc")) { c->oz_tpc = (int)std::max<int64_t>(0, value); return 0; }
   if (!strcmp(name, "oz_panel")) { c->oz_panel = (int)std::max<int64_t>(0, std::min<int64_t>(value, 2)); return 0; }   // 2 = at every size
   if (!strcmp(name, "oz_sched")) { c->oz_sched = value ? 1 : 0; return 0; }
@@ -306,16 +304,17 @@ static int sync_event(gpx_ctx* c, size_t idx, cudaEvent_t* out) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// tcgen05 / Ozaki path: tile lists and buffers for (Npad, NB)
+// Ozaki path: tile lists and buffers for (Npad, NB)
 // ---------------------------------------------------------------------------------------------------------------
 static bool oz_wanted(const gpx_ctx* c) {
   if (c->dist) return false;
   int on = c->ozaki;
-  if (on < 0) { const char* e = getenv("GPX_OZAKI"); on = e ? atoi(e) : 1; }
+  // off by default: on the H100 the fp64 DMMA.16x8x4 GEMMs are faster than the int8 digit split (140 vs 183 ms at
+  // N = 16384, H100 80GB HBM3 at a 400 W power limit, profiles/h100_bench_*); option "ozaki" = 1 or GPX_OZAKI=1 selects it
+  if (on < 0) { const char* e = getenv("GPX_OZAKI"); on = e ? atoi(e) : 0; }
   if (!on) return false;
   const long NB = pick_nb(c);
-  // wherever there are at least two panels (measured faster than the DMMA path from N = 700 up: 0.97 vs 1.03 ms at 700,
-  // 5.3 vs 5.9 ms at 4096, 64 vs 142 ms at 16384); a single-block matrix has no panel and stays on the DMMA path
+  // wherever there are at least two panels; a single-block matrix has no panel and stays on the DMMA path
   return c->Npad >= 2 * NB && NB % OZ_KC == 0;
 }
 
@@ -350,7 +349,7 @@ static int oz_prepare(gpx_ctx* c) {
 //   U2(k) trailing update of the remaining columns                                                      [main stream]
 // Look-ahead: D(k+1), Pn(k+1) only need U1(k), so they run on the high-priority side stream while U2(k) keeps the
 // machine busy; U1(k+1) waits for Pn(k+1). Without look-ahead everything is issued on the main stream.
-// oz: 0 = DMMA updates; 1 = trailing update on tcgen05 (Ozaki split); 2 = that + K^-1 = U U^T accumulated into c->Kinv
+// oz: 0 = DMMA updates; 1 = trailing update on the int8 tensor cores (Ozaki split); 2 = that + K^-1 = U U^T accumulated into c->Kinv
 // panel by panel inside the same launches (the panel's digit planes serve both)
 static int run_sweep_chain(gpx_ctx* c, Recorder& rec);
 
@@ -381,7 +380,7 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
     // ---- D(k): inner sweep of the nb x nb diagonal block ------------------------------------------------------
     GPX_CHECK(diag_block_sweep(c, Sblk, ld, nbt, kt0, ss));
     if (nbt == nt) break;  // single block: done
-    // tcgen05 schedule (option "oz_sched", default): the persistent U2(k-1) leaves a few SMs free, on which the serial
+    // Ozaki schedule (option "oz_sched", default): the persistent U2(k-1) leaves a few SMs free, on which the serial
     // diagonal-block chain D(k) runs meanwhile (side stream); the panel GEMM Pn(k), which needs the whole machine for half a
     // millisecond, is queued on the MAIN stream behind U2(k-1) instead of fighting it for SM slots.
     if (u1_pending) {   // (oz_u0) the panel of this step needs ALL of its block column updated, not only the diagonal block
@@ -416,8 +415,8 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
                                    (size_t)(Npad - o - nb) * 8, nb, cudaMemcpyDeviceToDevice, ss));
       return 0;
     };
-    // DMMA updates read the panel from Pb, tcgen05 updates from the digit planes: either way nothing on the main stream
-    // reads block column k of S, so on the tcgen05 path the copy-back leaves the critical chain (after the hand-over)
+    // DMMA updates read the panel from Pb, Ozaki updates from the digit planes: either way nothing on the main stream
+    // reads block column k of S, so on the Ozaki path the copy-back leaves the critical chain (after the hand-over)
     if (!oz) GPX_CHECK(copy_back());
     if (oz) {   // digit planes + row exponents of this panel (all rows: U block column | U_kk | Cholesky panel)
       GPX_CHECK(launch_oz_split(Pb, Npad, nb, c->ozp[kblk & 1], sp));
@@ -453,7 +452,7 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
           memset(&op, 0, sizeof(op));
           op.tiles = c->oz_tiles + off; op.ntiles = ntl; op.nkc = (int)(nb / OZ_KC);
           op.scale = pl.scale; op.S = c->S; op.lds = ld; op.Kinv = c->Kinv; op.ldk = ld;
-          op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.dbg = c->oz_dbg; op.wide = c->oz_wide;
+          op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.wide = c->oz_wide;
           op.tpc = c->oz_ctas > 0 ? (ntl + c->oz_ctas - 1) / c->oz_ctas : c->oz_tpc;
           if (sched2 && c->oz_ctas <= 0 && c->oz_tpc <= 0) {
             // persistent: U1 on every SM (nothing else can run before it is done), U2 on all but the reserved SMs
@@ -520,18 +519,18 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
   return 0;
 }
 
-// The tcgen05 sweep with the serial chain on its own stream (option "chain", default). Per step k:
+// The Ozaki sweep with the serial chain on its own stream (option "chain", default). Per step k:
 //   side stream  ss : D(k) -> assemble -> Pc(k): panel rows of block k+1 (fine DMMA tiles) -> U0d(k): diagonal block k+1 -= Pc Pc^T
 //                     (fine DMMA tiles, fp64 operands straight from the panel buffer) -> D(k+1) ...
 //   third stream s3 : Pr(k): the other panel rows -> digit split of the whole panel -> copy-back -> forward substitution
-//   main stream  sm : U1(k): rest of block column k+1 -> U2(k): everything else + the K^-1 tiles          (tcgen05)
+//   main stream  sm : U1(k): rest of block column k+1 -> U2(k): everything else + the K^-1 tiles          (Ozaki)
 // Dependences across streams (events):  Pc(k), Pr(k) read block column k: after U1(k-1);  U0d(k) touches tiles that U2(k-1)
 // updates: after U2(k-1);  split(k) after Pc(k);  U1(k) after split(k);  assemble(k+1) overwrites Tm and, with Pc/Pr(k+1), the
 // panel buffer of step k-1: after the forward-substitution block of step k on s3 (s3 runs in order, so everything of step
 // k-1 there is done as well);  the digit planes of step k are those of step k-2: split(k) is behind Pr(k), which waits for
 // U1(k-1), which is behind U2(k-2) on the main stream.
 // What the next diagonal block waits for is therefore D(k) + two small launches instead of D(k) + full panel + split + a
-// tcgen05 launch, and the main stream never waits for a diagonal block unless the trailing update is shorter than D.
+// Ozaki launch, and the main stream never waits for a diagonal block unless the trailing update is shorter than D.
 static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
   const long ld = c->Npad, Npad = c->Npad;
   const int nt = (int)(Npad / TILE);
@@ -591,8 +590,7 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
       c->eval_launches++;
     }
     // ---- s3: Pr(k), split, copy-back, forward substitution --------------------------------------------------------------
-    // (measured, profiles/r02s2_panel_ab.txt: +3.8 % at N = 16384, +3.1 % at 8192, even at 4096, -7 % at 1300: five launches
-    // instead of one only pay once the panel GEMM is a visible share of the step)
+    // (from N = 4096 on: five launches instead of one only pay once the panel GEMM is a visible share of the step)
     const bool oz_pan = c->oz_panel && c->oz_wide && os.pan_n > 0 && (c->oz_panel > 1 || Npad >= 4096);
     if (oz_pan) {
       // the panel GEMM itself on the tensor cores: digit planes of block column k of the workspace (A) and of L_kk^-1 (B,
@@ -605,7 +603,7 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
       op.tiles = c->oz_tiles + os.pan_off; op.ntiles = os.pan_n; op.nkc = (int)(nb / OZ_KC);
       op.scale = c->ozpA.scale; op.scaleB = c->ozpB.scale; op.P = Pb; op.ldp = Npad; op.Pfinal = c->S + o * ld;
       op.S = c->S; op.lds = ld; op.Kinv = c->Kinv; op.ldk = ld;
-      op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.dbg = c->oz_dbg; op.wide = 1;
+      op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.wide = 1;
       op.tpc = c->oz_ctas > 0 ? (os.pan_n + c->oz_ctas - 1) / c->oz_ctas : c->oz_tpc;
       GPX_CHECK(launch_oz_gemm(c->ozpA, op, c->num_sms, s3, &c->ozpB));
       c->eval_launches += 5;
@@ -639,7 +637,7 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
     GPX_CHECK(link(s3, nullptr, &ev_fw));
     GPX_CHECK(launch_fw_panel(Pb + (o + nb), Npad, Npad - o - nb, (int)nb, c->dTfw + o, Npad, c->P, c->dYres + (o + nb), s3));
     c->eval_launches++;
-    // ---- sm: U1(k), U2(k) on the tcgen05 tensor cores ---------------------------------------------------------------------
+    // ---- sm: U1(k), U2(k) on the int8 tensor cores ---------------------------------------------------------------------
     for (int part = 0; part < 2; part++) {
       const int off = part == 0 ? os.u1_off : os.u2_off;
       const int ntl = part == 0 ? os.u1_n : os.u2_n;
@@ -648,7 +646,7 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
         memset(&op, 0, sizeof(op));
         op.tiles = c->oz_tiles + off; op.ntiles = ntl; op.nkc = (int)(nb / OZ_KC);
         op.scale = pl.scale; op.S = c->S; op.lds = ld; op.Kinv = c->Kinv; op.ldk = ld;
-        op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.dbg = c->oz_dbg; op.wide = c->oz_wide;
+        op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.wide = c->oz_wide;
         op.tpc = c->oz_ctas > 0 ? (ntl + c->oz_ctas - 1) / c->oz_ctas : c->oz_tpc;
         const int tn = c->oz_wide ? 2 * OZ_TN : OZ_TN;
         const double flops = (double)ntl * 2.0 * OZ_TM * tn * (double)nb;
@@ -770,14 +768,14 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
   }
   {
     const int h = rec.begin(PH_SOLVE);
-    // alpha = U (U^T y). On the tcgen05 path t = L^-1 y = U^T y came along with the sweep (forward substitution): one mat-vec
+    // alpha = U (U^T y). On the Ozaki path t = L^-1 y = U^T y came along with the sweep (forward substitution): one mat-vec
     if (!oz) GPX_CHECK(launch_utv(c->S, ld, c->Npad, c->P, c->dY, c->dT, st));
     GPX_CHECK(launch_uv(c->S, ld, c->Npad, c->P, oz ? c->dTfw : c->dT, KSPLIT, c->dUvPart, c->dAlpha, st));
     rec.end(h);
     c->eval_launches += oz ? 2 : 3;
   }
   if (c->multi) {
-    // composite kernel: K^-1 stored (by the sweep on the tcgen05 path, else by a plain LAUUM), then one reduction pass per part
+    // composite kernel: K^-1 stored (by the sweep on the Ozaki path, else by a plain LAUUM), then one reduction pass per part
     if (!oz) {
       if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)ld * ld * 8));
       GPX_CHECK(run_lauum(c, c->Kinv, &rec, true));
@@ -809,7 +807,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
   }
   long grad_tiles = (long)nt * nt;
   if (oz) {
-    // K^-1 was accumulated panel by panel inside the sweep (tcgen05): reduce dL_dK -> gradients from the stored tiles
+    // K^-1 was accumulated panel by panel inside the sweep (Ozaki): reduce dL_dK -> gradients from the stored tiles
     const int csplit = grad_kinv_csplit(nt, nl + 2);
     grad_tiles = (long)nt * nt * csplit;
     GPX_CUDA(cudaMemsetAsync(c->partials, 0, (size_t)grad_tiles * (nl + 2) * 8, st));
@@ -827,7 +825,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
     rec.end(h);
     c->eval_launches++;
   } else if (c->fine && nt <= 8 && !c->dist) {
-    // small matrix on the DMMA path (one block, or tcgen05 switched off): the fused LAUUM kernel has one CTA per 128 x 128 tile
+    // small matrix on the DMMA path (one block, or Ozaki switched off): the fused LAUUM kernel has one CTA per 128 x 128 tile
     // -- 10 CTAs for N = 512, each walking up to 512 k alone (136 us of a 0.48 ms evaluation). K^-1 = U U^T in 64 x 32 tiles
     // (80 CTAs) into the K^-1 buffer, then the gradient pass over the stored tiles, split over the columns
     if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)ld * ld * 8));
@@ -1257,7 +1255,7 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
   PointSet& pj = X2 ? p2 : p1;
   // m is split into chunks so that ~4 waves of CTAs are in flight; partials are reduced in fixed order
   const long ntile = (N + TILE - 1) / TILE;
-  int nchunk = (int)std::max<long>(1, std::min<long>((M + 31) / 32, (4 * 148 + ntile - 1) / ntile));
+  int nchunk = (int)std::max<long>(1, std::min<long>((M + 31) / 32, (4 * c->num_sms + ntile - 1) / ntile));
   const long mchunk = ((M + nchunk - 1) / nchunk + 31) / 32 * 32;
   nchunk = (int)((M + mchunk - 1) / mchunk);
   double *dd = nullptr, *dpart = nullptr, *dout = nullptr;

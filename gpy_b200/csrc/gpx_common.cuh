@@ -1,4 +1,4 @@
-// gpx_common.cuh — shared definitions for the sm_100a exact-GP kernels (internal; the public ABI is include/gpx.h).
+// gpx_common.cuh — shared definitions for the sm_90a exact-GP kernels (internal; the public ABI is include/gpx.h).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -59,7 +59,7 @@ __device__ __forceinline__ void k_dk_of_r_unit(int kind, double r, double& k, do
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// PTX helpers: mbarrier + 1-D bulk async copy (TMA engine, SASS UBLKCP) + fp64 tensor MMA (SASS DMMA.8x8x4)
+// PTX helpers: mbarrier + 1-D bulk async copy (TMA engine, SASS UBLKCP) + fp64 tensor MMA (SASS DMMA.16x8x4)
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -92,11 +92,12 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// D(8x8) += A(8x4, row) * B(4x8, col): lane holds A[g][t], B[t][g], C[g][2t..2t+1] with g = lane>>2, t = lane&3
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
+// D(16x8) += A(16x4, row) * B(4x8, col), the sm_90 fp64 shape (SASS DMMA.16x8x4): lane holds A[g][t], A[g+8][t], B[t][g],
+// C[g][2t..2t+1], C[g+8][2t..2t+1] with g = lane>>2, t = lane&3. On the H100 it issues at twice the rate of m8n8k4.
+__device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+               : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+               : "d"(a0), "d"(a1), "d"(b));
 }
 
 __device__ __forceinline__ double warp_sum(double v) {

@@ -19,7 +19,7 @@ struct gpx_ctx {
   bool kfirst_valid = false;
   int lookahead = 1;
   int fine = 1;                 // option "fine": 64 x 64-tile DMMA kernels in the diagonal-block chain (gpx_fine.cu); 0 = 128 x 128 tiles
-  int chain = 1;                // option "chain": tcgen05 path: the chain D(k) -> panel rows of block k+1 -> update of diagonal block k+1
+  int chain = 1;                // option "chain": Ozaki path: the chain D(k) -> panel rows of block k+1 -> update of diagonal block k+1
                                 // (fp64 DMMA, fine tiles) -> D(k+1) runs alone on the side stream; 0 = round-2 schedule
   std::vector<cudaEvent_t> sync_ev;
   // data
@@ -62,20 +62,19 @@ struct gpx_ctx {
   int64_t eval_launches = 0;
   std::vector<cudaEvent_t> ev;
   int profile = 1;
-  // ---- tcgen05 / Ozaki path (gpx_ozaki.cu): trailing update and K^-1 on the INT8 tensor cores ------------------------
-  int ozaki = -1;              // option "ozaki": -1 = default (env GPX_OZAKI, else on), 0 = DMMA only, 1 = on where applicable
+  // ---- Ozaki path (gpx_ozaki.cu): trailing update and K^-1 on the INT8 tensor cores ------------------------
+  int ozaki = -1;              // option "ozaki": -1 = default (env GPX_OZAKI, else off), 0 = DMMA only, 1 = on where applicable
   int oz_dig_up = 7;           // digits per operand for the inverse-part / K^-1 tiles, which feed only the gradients
                                // (option "oz_dig_up"; 7 -> 28 digit pairs instead of 36, gradient error ~6e-10 at N = 16384)
   int oz_ctas = 0;             // option "oz_ctas": >0 = that many CTAs sharing the tile list evenly (persistent-style); 0 = default chunking
   int oz_tpc = 0;              // option "oz_tpc": consecutive tiles per CTA (0 = default 4)
-  int oz_dbg = 0;              // measurement-only kernel variants (OzParams::dbg)
   int oz_u0 = 1;               // option "oz_u0": update the NEXT diagonal block first (own small launch) so that its factorisation starts
                                // before the rest of block column k+1 is updated
   int oz_sched = 0;            // option "oz_sched": 1 = panel GEMM on the main stream + persistent U2 leaving oz_reserve SMs to the
                                // diagonal-block chain; 0 = everything of step k+1 on the side stream, U launches in chunks of tiles
   int oz_reserve = 4;          // SMs left free by the persistent U2 launch for the side stream
   int oz_wide = 1;             // option "oz_wide": 1 = two-pass kernel with 128 x 128 tiles, 0 = one-pass kernel with 128 x 64 tiles
-  int num_sms = 148;
+  int num_sms = 132;
   bool oz_ready = false;       // planes and K^-1 buffer allocated for (Npad, NB)
   bool oz_lists_ready = false; // tile lists built for (Npad, NB, oz_wide)
   gpx::OzPlanes ozp[2];        // digit planes of the current / next panel (look-ahead double buffer)

@@ -1,6 +1,6 @@
 // gpx_fine.cu — fine-grained fp64 DMMA kernels of the serial chain (see gpx_fine.cuh) and the inner sweep of a diagonal block.
 //
-//   gemm_fine_kernel<FINE_UPDATE / FINE_PANEL> : 64 x 32 output tile per CTA, 8 warps (4 x 2, 16 x 16 each, DMMA.8x8x4); 32-deep
+//   gemm_fine_kernel<FINE_UPDATE / FINE_PANEL> : 64 x 32 output tile per CTA, 8 warps (4 x 2, 16 x 16 each, DMMA.16x8x4); 32-deep
 //       k-chunks of both operands in a 4-stage cp.async ring (16-byte LDGSTS by every thread); smem pitches 68 / 36 doubles
 //       (== 4 mod 16: conflict-free fragment loads); two CTAs per SM. A 128-deep product is 4 chunks, i.e. the whole operand
 //       strip is in flight at once.
@@ -150,9 +150,12 @@ __global__ void __launch_bounds__(F_THREADS, 2) gemm_fine_kernel(const FineParam
 #pragma unroll
       for (int nb = 0; nb < 2; nb++) bf[nb] = b[k * FPB + nb * 8];
 #pragma unroll
-      for (int mb = 0; mb < 2; mb++)
+      for (int mb = 0; mb < 2; mb += 2)
 #pragma unroll
-        for (int nb = 0; nb < 2; nb++) dmma884(acc[k4 & (NS - 1)][mb][nb][0], acc[k4 & (NS - 1)][mb][nb][1], af[mb], bf[nb]);
+        for (int nb = 0; nb < 2; nb++) {
+          double (&c)[2][2][2] = acc[k4 & (NS - 1)];
+          dmma1684(c[mb][nb][0], c[mb][nb][1], c[mb + 1][nb][0], c[mb + 1][nb][1], af[mb], af[mb + 1], bf[nb]);
+        }
     }
   }
 #pragma unroll
@@ -214,9 +217,10 @@ fine_panel_inplace_kernel(double* __restrict__ Sblk, long ld, const double* __re
 #pragma unroll
     for (int ni = 0; ni < 2; ni++) bf[ni] = b[k * PITCH + ni * 8];
 #pragma unroll
-    for (int mi = 0; mi < 2; mi++)
+    for (int mi = 0; mi < 2; mi += 2)
 #pragma unroll
-      for (int ni = 0; ni < 2; ni++) dmma884(acc[mi][ni][0], acc[mi][ni][1], af[mi], bf[ni]);
+      for (int ni = 0; ni < 2; ni++) dmma1684(acc[mi][ni][0], acc[mi][ni][1], acc[mi + 1][ni][0], acc[mi + 1][ni][1],
+                                                          af[mi], af[mi + 1], bf[ni]);
   }
   // every byte of the strip is in shared memory (the mbarrier completed for the whole CTA): overwrite in place
 #pragma unroll

@@ -3,7 +3,7 @@
 // The diagonal-block chain D(k) -> panel rows of the next block -> update of the next diagonal block -> D(k+1) is latency,
 // not throughput: with 128 x 128 CTA tiles a 128-deep product keeps 3..35 SMs busy for ~22 us each (one SM's DMMA rate on a
 // 128^3 tile). The kernels here cut the same products into 64 x 32 output tiles (16-row strips for the in-place inner
-// panel), so that a chain link spreads over up to 148 SMs and lasts a few microseconds. Same arithmetic, same operand
+// panel), so that a chain link spreads over up to 132 SMs and lasts a few microseconds. Same arithmetic, same operand
 // layout (column-major, m-contiguous), same results up to the summation order inside DMMA.
 #pragma once
 #include "gpx_common.cuh"

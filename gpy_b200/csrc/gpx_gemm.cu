@@ -8,12 +8,13 @@
 //                 reduces dL_dK -> (variance, lengthscale, noise) gradients (replaces exact_gaussian_inference.py:70-72,
 //                 stationary.py:193-243, stationary_cython.pyx:53-62, likelihoods/gaussian.py:78-79) without writing K^-1.
 //
-// Machine mapping (sm_100a): tcgen05.mma has no f64 kind, so the fp64 tensor path is DMMA.8x8x4 (mma.sync m8n8k4).
+// Machine mapping (sm_90a): wgmma has no f64 kind, so the fp64 tensor path is DMMA.16x8x4 (mma.sync m16n8k4,
+// the sm_90 shape: twice the issue rate of the older m8n8k4 on the H100).
 // A 128x128 CTA tile is computed by 8 consumer warps (64x32 each, 64 fp64 accumulators per lane); a 9th producer
 // warp streams 16-deep k-slabs of both operands into a 4-stage shared-memory ring with 1-D bulk async copies
 // (cp.async.bulk -> SASS UBLKCP, the TMA engine) signalled through mbarriers. Operands are m-contiguous
 // (column-major), a slab column is one 1 KiB bulk copy; the smem pitch of 132 doubles makes the DMMA fragment
-// loads bank-conflict free. Measured DMMA issue peak on B200: 37.1 TFLOP/s (tools/microbench.cu).
+// loads bank-conflict free.
 #include <algorithm>
 #include <cstdlib>
 
@@ -31,13 +32,13 @@ static int epi_bytes(int D, int P) {
 }
 constexpr int SMEM_PIPE = BAR_BYTES + PIPE_BYTES;
 constexpr int SMEM_MAX = 227 * 1024;
-constexpr int SB = 12;   // super-block edge of the tile schedule (SB*SB = 144 <= 148 SMs)
+constexpr int SB = 11;   // super-block edge of the tile schedule (SB*SB = 121 <= 132 SMs)
 
 size_t gemm_smem_bytes() { return SMEM_PIPE; }
 
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_WARPS * 32) : "memory"); }
 
-// Tile schedule. UPDATE / LAUUM run on a 1-D grid decoded through SB x SB super-blocks so that the ~148 CTAs in flight
+// Tile schedule. UPDATE / LAUUM run on a 1-D grid decoded through SB x SB super-blocks so that the ~132 CTAs in flight
 // share <= 2*SB row panels and SB column panels (operand streams stay L2-resident). LAUUM enumerates the super-blocks of
 // the lower triangle row by row: small r first = longest k-ranges first, so the tail of the launch is made of short tiles.
 // block-mapped operand base of row tile r (see GemmParams)
@@ -200,9 +201,10 @@ __device__ __forceinline__ void gemm_nt_body(const GemmParams& p) {
 #pragma unroll
       for (int nb = 0; nb < 4; nb++) bf[nb] = b[kk + nb * 8];
 #pragma unroll
-      for (int mb = 0; mb < 8; mb++)
+      for (int mb = 0; mb < 8; mb += 2)
 #pragma unroll
-        for (int nb = 0; nb < 4; nb++) dmma884(acc[mb][nb][0], acc[mb][nb][1], af[mb], bf[nb]);
+        for (int nb = 0; nb < 4; nb++) dmma1684(acc[mb][nb][0], acc[mb][nb][1], acc[mb + 1][nb][0], acc[mb + 1][nb][1],
+                                                          af[mb], af[mb + 1], bf[nb]);
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);

@@ -286,7 +286,7 @@ base_sweep_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, d
 //       rsqrt on the serial chain, no block barrier inside),
 //   (2) all threads form the micro-panel  P = T(:, panel) W^T  (W = inverse of the micro-block) in place,
 //   (3) all 16 warps apply  T(r,c) -= P_r P_c^T  to the 16x16 micro-tiles c > panel, r in [0..panel] U [c..7] with
-//       DMMA.8x8x4 (fragments straight from shared memory, pitch 132 -> conflict-free).
+//       DMMA.16x8x4 (fragments straight from shared memory, pitch 132 -> conflict-free).
 // Three block barriers per micro-panel instead of one per column: 24 instead of 128, and the rank-16 updates run on
 // the tensor pipe. Same inputs/outputs as base_sweep_kernel.
 // =================================================================================================================
@@ -342,7 +342,7 @@ __device__ __forceinline__ void micro_diag(double* T, int c0, double* Pd, double
   }
 }
 
-// (3) one 16 x (8*NI) piece of a micro-tile update  T(rt, ct) -= P_rt P_ct^T  (k-depth 16) with DMMA.8x8x4
+// (3) one 16 x (8*NI) piece of a micro-tile update  T(rt, ct) -= P_rt P_ct^T  (k-depth 16) with DMMA.16x8x4
 template <int NI>
 __device__ __forceinline__ void micro_update(double* T, int c0, int jp, int rt, int ct, int n0, const double* Pd,
                                              int lane) {
@@ -366,9 +366,10 @@ __device__ __forceinline__ void micro_update(double* T, int c0, int jp, int rt, 
 #pragma unroll
     for (int ni = 0; ni < NI; ni++) bf[ni] = Bp[(k4 * 4 + tg) * BP + ni * 8 + g];
 #pragma unroll
-    for (int mi = 0; mi < 2; mi++)
+    for (int mi = 0; mi < 2; mi += 2)
 #pragma unroll
-      for (int ni = 0; ni < NI; ni++) dmma884(c[mi][ni][0], c[mi][ni][1], af[mi], bf[ni]);
+      for (int ni = 0; ni < NI; ni++) dmma1684(c[mi][ni][0], c[mi][ni][1], c[mi + 1][ni][0], c[mi + 1][ni][1],
+                                                          af[mi], af[mi + 1], bf[ni]);
   }
 #pragma unroll
   for (int mi = 0; mi < 2; mi++)
@@ -424,9 +425,10 @@ base_sweep16_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag,
 #pragma unroll
         for (int ni = 0; ni < 2; ni++) bf[ni] = Wm[(k4 * 4 + tg) * MP + ni * 8 + g];   // B(n = c, k) = W(c, k)
 #pragma unroll
-        for (int mi = 0; mi < 2; mi++)
+        for (int mi = 0; mi < 2; mi += 2)
 #pragma unroll
-          for (int ni = 0; ni < 2; ni++) dmma884(c[mi][ni][0], c[mi][ni][1], af[mi][k4], bf[ni]);
+          for (int ni = 0; ni < 2; ni++) dmma1684(c[mi][ni][0], c[mi][ni][1], c[mi + 1][ni][0], c[mi + 1][ni][1],
+                                                          af[mi][k4], af[mi + 1][k4], bf[ni]);
       }
       __syncwarp();                                       // every lane has read its A fragments: overwrite in place
 #pragma unroll
@@ -618,9 +620,10 @@ base_sweep3_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, 
 #pragma unroll
         for (int ni = 0; ni < 2; ni++) bf[ni] = Wm[(k4 * 4 + tg) * MP + ni * 8 + g];
 #pragma unroll
-        for (int mi = 0; mi < 2; mi++)
+        for (int mi = 0; mi < 2; mi += 2)
 #pragma unroll
-          for (int ni = 0; ni < 2; ni++) dmma884(c[mi][ni][0], c[mi][ni][1], af[mi][k4], bf[ni]);
+          for (int ni = 0; ni < 2; ni++) dmma1684(c[mi][ni][0], c[mi][ni][1], c[mi + 1][ni][0], c[mi + 1][ni][1],
+                                                          af[mi][k4], af[mi + 1][k4], bf[ni]);
       }
       __syncwarp();
 #pragma unroll
@@ -804,9 +807,10 @@ __device__ __forceinline__ void micro_panel_rows(double* T, int c0, int rt, cons
 #pragma unroll
     for (int ni = 0; ni < 2; ni++) bf[ni] = Wm[(k4 * 4 + tg) * MP + ni * 8 + g];
 #pragma unroll
-    for (int mi = 0; mi < 2; mi++)
+    for (int mi = 0; mi < 2; mi += 2)
 #pragma unroll
-      for (int ni = 0; ni < 2; ni++) dmma884(c[mi][ni][0], c[mi][ni][1], af[mi][k4], bf[ni]);
+      for (int ni = 0; ni < 2; ni++) dmma1684(c[mi][ni][0], c[mi][ni][1], c[mi + 1][ni][0], c[mi + 1][ni][1],
+                                                          af[mi][k4], af[mi + 1][k4], bf[ni]);
   }
   __syncwarp();                                       // every lane has read its A fragments: overwrite in place
 #pragma unroll
@@ -1779,21 +1783,21 @@ int launch_gradx(const GradFullParams& p, int nchunk, long mchunk, double* part,
 }
 
 // =================================================================================================================
-// roofline denominator: DMMA.8x8x4 issue rate of this device (8 independent accumulator chains per warp,
-// 8 warps per CTA, 2 CTAs per SM), timed with CUDA events. tools/microbench.cu is the stand-alone version.
+// roofline denominator: DMMA.16x8x4 issue rate of this device (8 independent accumulator chains per warp,
+// 8 warps per CTA, 2 CTAs per SM), timed with CUDA events.
 // =================================================================================================================
 __global__ void dmma_rate_kernel(double* out, int iters) {
-  double c[8][2];
+  double c[8][4];
 #pragma unroll
-  for (int i = 0; i < 8; i++) { c[i][0] = 0.0; c[i][1] = 0.0; }
+  for (int i = 0; i < 8; i++) { c[i][0] = 0.0; c[i][1] = 0.0; c[i][2] = 0.0; c[i][3] = 0.0; }
   const double a = 1.0 + threadIdx.x * 1e-9, b = 1.0 - threadIdx.x * 1e-9;
   for (int it = 0; it < iters; it++) {
 #pragma unroll
-    for (int i = 0; i < 8; i++) dmma884(c[i][0], c[i][1], a, b);
+    for (int i = 0; i < 8; i++) dmma1684(c[i][0], c[i][1], c[i][2], c[i][3], a, b, b);
   }
   double s = 0;
 #pragma unroll
-  for (int i = 0; i < 8; i++) s += c[i][0] + c[i][1];
+  for (int i = 0; i < 8; i++) s += (c[i][0] + c[i][1]) + (c[i][2] + c[i][3]);
   out[(long)blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 
@@ -1815,7 +1819,7 @@ int measure_dmma_peak(cudaStream_t st, double* tflops) {
     GPX_CUDA(cudaEventSynchronize(e1));
     float ms = 0;
     GPX_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    const double tf = (double)grid * (threads / 32) * iters * 8 * 512.0 / ms * 1e-9;
+    const double tf = (double)grid * (threads / 32) * iters * 8 * 1024.0 / ms * 1e-9;   // 2 x 16 x 8 x 4 flop per MMA
     if (rep > 0 && tf > best) best = tf;
   }
   cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(out);

@@ -1,24 +1,25 @@
-// gpx_ozaki.cu — the trailing update and K^-1 = U U^T of the factor-and-invert sweep on the 5th-generation tensor cores.
+// gpx_ozaki.cu — the trailing update and K^-1 = U U^T of the factor-and-invert sweep on the Hopper INT8 tensor cores.
 //
-// tcgen05.mma has no f64 kind, so fp64-grade products are formed by an Ozaki split on kind::i8 (exact s32 accumulation):
+// wgmma has no f64 kind, so fp64-grade products are formed by an Ozaki split on s8 x s8 -> s32 (exact integer accumulation):
 //   every row of a panel P (rows x K) is scaled by a power of two to (-1/2, 1/2) and cut into 8 signed digits of 7 bits, rounded
 //   to nearest (|digit| <= 64; int8 planes),
 //   P_r P_c^T = sum_{s+t <= 7} 2^(e_r + e_c - 7 (s+t+2)) D_s(r) D_t(c)^T; the 36 digit-pair products of a 32-deep k-chunk are
-//   36 tcgen05.mma (128 x 64 x 32) accumulated per exponent group g = s + t in its own 64 TMEM columns (8 groups = all 512
-//   columns of the SM), |digit product sum| <= 64^2 * K * 8 < 2^31 for K <= 65536; the epilogue converts the groups to
-//   fp64, sums them smallest first, rescales by the row/column exponents and applies the result to the fp64 target tile.
+//   36 wgmma.m64n64k32 accumulated per exponent group g = s + t in its own s32 register accumulator,
+//   |digit product sum| <= 64^2 * K * 8 < 2^31 for K <= 65536; the epilogue converts the groups to fp64, sums them smallest
+//   first, rescales by the row/column exponents and applies the result to the fp64 target tile.
 // Replaces the same reference work as the DMMA GEMM of gpx_gemm.cu: LAPACK dpotrf / dtrtri / dpotri behind
 // GPy/util/linalg.py:58,142,209-212 (see DESIGN.md §5 for the digit budget against the 1e-8 / 1e-6 tolerances).
 //
-// Kernel anatomy (one CTA per SM, persistent over a tile list): warp 0 = TMA producer (cp.async.bulk.tensor, 4-D tensor map
-// over the pre-tiled digit planes, 4-stage mbarrier ring of 32-deep k-chunks), warp 1 = MMA issuer (one thread, tcgen05.mma
-// from shared-memory descriptors, tcgen05.commit frees the stage / publishes the accumulators), warps 2..9 = epilogue
-// (tcgen05.ld, one TMEM lane quarter x 32 columns each).
+// Kernel anatomy (one CTA per SM over a run of consecutive tiles of the list): warpgroup 2 = TMA producer (one warp,
+// cp.async.bulk.tensor over the pre-tiled digit planes, mbarrier ring of 32-deep k-chunks), warpgroups 0 and 1 = consumers.
+// Eight exponent groups of a 64 x 64 accumulator are 256 s32 registers per thread, more than a thread has, so the two
+// consumer warpgroups compute the SAME 64 x 64 sub-tile and split the groups between them (four each, 128 registers):
+// warpgroup 0 takes the groups g with g % 4 in {0, 3}, warpgroup 1 those with g % 4 in {1, 2} (18 of the 36 digit pairs each).
+// A 128 x 64 (or 128 x 128) output tile of the list is walked as 2 (or 4) such sub-tiles.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <type_traits>
 #include <cstdlib>
 #include <cstring>
 
@@ -30,16 +31,16 @@
 
 namespace gpx {
 
-constexpr int OZ_STAGES = 4;
-constexpr int OZ_A_BYTES = OZ_TM * OZ_KC;                         // 4096: one digit plane of the A tile, one k-chunk
-constexpr int OZ_B_BYTES = OZ_TN * OZ_KC;                         // 2048
-constexpr int OZ_STAGE_BYTES = OZ_S * (OZ_A_BYTES + OZ_B_BYTES);  // 49152
-constexpr int OZ_EPI_WARPS = 8;
-constexpr int OZ_THREADS = (2 + OZ_EPI_WARPS) * 32;               // 320
-constexpr int OZ_SMEM = OZ_STAGES * OZ_STAGE_BYTES + 1024 + 256;  // ring + alignment slack + barriers
+constexpr int OZ_SUB = 64;                                        // sub-tile edge (wgmma M = N = 64)
+constexpr int OZ_STAGES = 5;
+constexpr int OZ_PLANE = OZ_SUB * OZ_KC;                          // 2048: one digit plane of a 64-row sub-tile, one k-chunk
+constexpr int OZ_STAGE_BYTES = 2 * OZ_S * OZ_PLANE;               // 32768: up to 8 A planes + 8 B planes
+constexpr int OZ_XCH_BYTES = OZ_SUB * OZ_SUB * 8;                 // 32768: fp64 partial sums handed between the consumers
+constexpr int OZ_THREADS = 384;                                   // three warpgroups (setmaxnreg works per warpgroup)
+constexpr int OZ_SMEM = OZ_STAGES * OZ_STAGE_BYTES + OZ_XCH_BYTES + 1024 + 256;   // ring + exchange + alignment + barriers
 
 // ---------------------------------------------------------------------------------------------------------------
-// PTX helpers (tcgen05 / TMA tensor copies); mbarrier helpers come from gpx_common.cuh
+// PTX helpers (wgmma / TMA tensor copies); mbarrier helpers come from gpx_common.cuh
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t* bar) {
   asm volatile(
@@ -48,8 +49,8 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, i
       "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar))
       : "memory");
 }
-// mbarrier wait with back-off: the polling loop of a waiting warp takes issue slots from the one thread that feeds the tensor
-// core, so the roles that wait for long (epilogue: a whole tile; producer: a free stage) sleep between polls
+// mbarrier wait with back-off, for the producer waiting for a free stage: its polling must not take issue slots from the
+// consumers on the same SM sub-partitions
 __device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity, unsigned ns) {
   for (;;) {
     uint32_t ok;
@@ -62,41 +63,29 @@ __device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {   // one lane of the (converged) warp
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 // shared-memory matrix descriptor: no swizzle, K-major, core matrices 8 rows x 16 B; LBO = 128 B between the two core matrices
-// along K, SBO = 256 B between 8-row groups (layout pinned by tools/tcgen05_i8_check.cu on the hardware)
+// along K, SBO = 256 B between 8-row groups (the image of gpx_ozaki.cuh)
 __device__ __forceinline__ uint64_t oz_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32);
 }
-// instruction descriptor: D = s32, A = B = signed 8-bit, both K-major, N at bit 17 (units of 8), M at bit 24 (units of 16)
-__host__ __device__ constexpr uint32_t oz_idesc(int M, int N) {
-  return (uint32_t)(2 << 4) | (uint32_t)(1 << 7) | (uint32_t)(1 << 10) | (uint32_t)((N >> 3) << 17) | (uint32_t)((M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_i8(uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-               "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t addr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D(64 x 64, s32) += A(64 x 32, s8) B(64 x 32, s8)^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_i8(uint32_t (&d)[32], uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, "
-      "%19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(addr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]),
+        "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]),
+        "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]),
+        "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "l"(da), "l"(db), "r"(1)
+      : "memory");
 }
+__device__ __forceinline__ void named_bar(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ---------------------------------------------------------------------------------------------------------------
 // 1. digit split: row exponents + 8 signed 7-bit digit planes of a panel, written in the tiled image of gpx_ozaki.cuh
@@ -195,413 +184,198 @@ int launch_oz_split(const double* P, long ld, long K, OzPlanes& pl, cudaStream_t
   return 0;
 }
 
-// apply one thread's row of an output tile to the fp64 target: NCOL columns, leading dimension ld. The loads of a group of 8
-// columns are all issued before the first store: written as `C[j * ld] -= ...` the compiler must assume that a store may
-// alias the next load (ld is a run-time value) and serialises 64 global round trips per thread (~20 us per tile, measured).
-template <int NCOL>
-__device__ __forceinline__ void oz_apply_row(double* __restrict__ C, long ld, const double (&acc)[NCOL], double si,
-                                             const double* __restrict__ scol, int kind) {
-#pragma unroll
-  for (int j0 = 0; j0 < NCOL; j0 += 8) {
-    double old[8];
-    if (kind != OZ_LAUUM_SET) {
-#pragma unroll
-      for (int j = 0; j < 8; j++) old[j] = C[(long)(j0 + j) * ld];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      const double v = acc[j0 + j] * (si * __ldg(scol + j0 + j));
-      C[(long)(j0 + j) * ld] = kind == OZ_UPDATE ? old[j] - v : (kind == OZ_LAUUM_ACC ? old[j] + v : v);
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // 2. the GEMM
 // ---------------------------------------------------------------------------------------------------------------
-// one 32-deep k-chunk: the ND (ND + 1) / 2 digit-pair products, exponent group g = s + t in TMEM columns [64 g, 64 g + 64).
-// a_lo = low descriptor word (address field) of digit plane 0 of the A tile in this stage; the B planes follow the 8 A planes.
-template <int ND, int G_BEG, int G_END>
-__device__ __forceinline__ void oz_issue_groups(uint32_t taddr, uint32_t a_lo, uint32_t acc0) {
-  constexpr uint32_t idesc = oz_idesc(OZ_TM, OZ_TN);
-  constexpr uint64_t hi = ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46);   // LBO, SBO, version
-  const uint32_t b_lo = a_lo + (uint32_t)((OZ_S * OZ_A_BYTES) >> 4);
+// exponent group of accumulator slot j of consumer warpgroup w (slots in ascending group order)
+__host__ __device__ constexpr int oz_group(int w, int j) {
+  return w == 0 ? (j == 0 ? 0 : j == 1 ? 3 : j == 2 ? 4 : 7) : (j == 0 ? 1 : j == 1 ? 2 : j == 2 ? 5 : 6);
+}
+// k-chunks of a tile: the whole panel width, except OZ_PANEL tiles (triangular B: columns of tile c' see k < (c' + 1) * 128)
+__device__ __forceinline__ int oz_tile_nkc(uint32_t t, int nkc) {
+  return ((t >> 25) & 3) == OZ_PANEL ? min(nkc, (int)(((t >> 12) & 0x1fff) + 1) * (2 * OZ_TN / OZ_KC)) : nkc;
+}
+// one 32-deep k-chunk of warpgroup W: the digit pairs (s, g - s) of its groups g < ND. a_base = shared address of digit
+// plane 0 of the A sub-tile in this stage; the B planes follow the 8 A planes.
+template <int W, int ND>
+__device__ __forceinline__ void oz_issue(uint32_t (&acc)[4][32], uint32_t a_base) {
+  const uint64_t da0 = oz_desc(a_base), db0 = oz_desc(a_base + OZ_S * OZ_PLANE);
 #pragma unroll
-  for (int g = G_BEG; g < G_END; g++) {
+  for (int j = 0; j < 4; j++) {
+    const int g = oz_group(W, j);
+    if (g < ND) {
 #pragma unroll
-    for (int s = 0; s <= g; s++) {
-      const uint64_t da = hi | (uint64_t)(a_lo + (uint32_t)(s * (OZ_A_BYTES >> 4)));
-      const uint64_t db = hi | (uint64_t)(b_lo + (uint32_t)((g - s) * (OZ_B_BYTES >> 4)));
-      umma_i8(taddr + (uint32_t)(g * OZ_TN), da, db, idesc, s > 0 ? 1u : acc0);
+      for (int s = 0; s <= g; s++) wgmma_i8(acc[j], da0 + (uint64_t)((s * OZ_PLANE) >> 4), db0 + (uint64_t)(((g - s) * OZ_PLANE) >> 4));
+    }
+  }
+}
+// the k-loop of one sub-tile, then its exponent groups summed in fp64 into f (wgmma needs the digit count at compile time:
+// a run-time branch around the instructions makes the compiler serialise them)
+template <int W, int ND>
+__device__ __forceinline__ void oz_subtile(double (&f)[32], uint32_t ring_s, uint64_t* full, uint64_t* empty, uint32_t& it,
+                                           int nkc_t, int tid) {
+  uint32_t acc[4][32];
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+#pragma unroll
+    for (int e = 0; e < 32; e++) acc[j][e] = 0u;
+  for (int kc = 0; kc < nkc_t; kc++, it++) {
+    const int st = it % OZ_STAGES;
+    mbar_wait(&full[st], (it / OZ_STAGES) & 1);
+    wg_fence();
+    oz_issue<W, ND>(acc, ring_s + (uint32_t)st * OZ_STAGE_BYTES);
+    wg_commit();
+    wg_wait<1>();   // the chunk before this one has been read: its stage may be refilled
+    if (kc > 0 && tid == 0) mbar_arrive(&empty[(it - 1) % OZ_STAGES]);
+  }
+  wg_wait<0>();
+  if (tid == 0) mbar_arrive(&empty[(it - 1) % OZ_STAGES]);
+  // s32 -> fp64 without the conversion unit (I2F.F64 runs at a few lanes per SM): the bit pattern
+  // {0x43300000, v ^ 0x80000000} is the double 2^52 + 2^31 + v, one exact DADD takes the offset off
+#pragma unroll
+  for (int e = 0; e < 32; e++) f[e] = 0.0;
+#pragma unroll
+  for (int j = 3; j >= 0; j--) {   // smallest magnitude first
+    const int g = oz_group(W, j);
+    if (g < ND) {
+      const double sc = __longlong_as_double((long long)(1023 - 7 * g) << 52);   // 2^(-7 g)
+#pragma unroll
+      for (int e = 0; e < 32; e++)
+        f[e] = fma(__hiloint2double(0x43300000, (int)(acc[j][e] ^ 0x80000000u)) - 4503601774854144.0, sc, f[e]);
     }
   }
 }
 
+template <int W>
+__device__ __forceinline__ void oz_consume(const OzParams& p, const unsigned char* ring, double* xch, uint64_t* full,
+                                           uint64_t* empty, int ti_beg, int ti_end, int tw) {
+  const int tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31;
+  const uint32_t ring_s = smem_u32(ring);
+  const int nsub = 2 * (tw / OZ_SUB);
+  uint32_t it = 0;
+  for (int ti = ti_beg; ti < ti_end; ti++) {
+    const uint32_t t = p.tiles[ti];
+    const int r = t & 0xfff, c = (t >> 12) & 0x1fff, kind = (t >> 25) & 3;
+    const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
+    const int nkc_t = oz_tile_nkc(t, p.nkc);
+    for (int sub = 0; sub < nsub; sub++) {
+      double f[32];
+      if (nd == 8) oz_subtile<W, 8>(f, ring_s, full, empty, it, nkc_t, tid);
+      else if (nd == 7) oz_subtile<W, 7>(f, ring_s, full, empty, it, nkc_t, tid);
+      else if (nd == 6) oz_subtile<W, 6>(f, ring_s, full, empty, it, nkc_t, tid);
+      else if (nd == 5) oz_subtile<W, 5>(f, ring_s, full, empty, it, nkc_t, tid);
+      else oz_subtile<W, 4>(f, ring_s, full, empty, it, nkc_t, tid);
+      // warpgroup 0 finishes columns 0..31 of the sub-tile (accumulator elements 0..15), warpgroup 1 columns 32..63: each
+      // hands the other half of its partial sums over (the two hold the same elements at the same thread index)
+      constexpr int KEEP = W == 0 ? 0 : 16, GIVE = 16 - KEEP;
+      named_bar(1, 256);   // the partner has read the previous sub-tile's exchange
+#pragma unroll
+      for (int e = 0; e < 16; e++) xch[(W * 16 + e) * 128 + tid] = f[GIVE + e];
+      named_bar(1, 256);
+#pragma unroll
+      for (int e = 0; e < 16; e++) f[KEEP + e] += xch[((1 - W) * 16 + e) * 128 + tid];
+      // element e of the accumulator: row warp * 16 + lane / 4 + 8 * ((e / 2) % 2), column (e / 4) * 8 + (lane % 4) * 2 + e % 2
+      const long gi0 = (long)r * OZ_TM + (sub & 1) * OZ_SUB + warp * 16 + (lane >> 2);
+      const long gj0 = (long)c * tw + (sub >> 1) * OZ_SUB + (lane & 3) * 2;
+      const double si[2] = {p.scale[gi0], p.scale[gi0 + 8]};
+      const double* scol = kind == OZ_PANEL ? p.scaleB : p.scale;
+      double v[16];
+#pragma unroll
+      for (int e = 0; e < 16; e++) {
+        const int ee = KEEP + e;
+        v[e] = f[ee] * (si[(ee >> 1) & 1] * __ldg(scol + gj0 + (ee >> 2) * 8 + (ee & 1)));
+      }
+      // all loads of the target before the first store: with a run-time leading dimension the compiler must otherwise assume
+      // that a store may alias the next load and serialise the global round trips
+      auto apply = [&](double* C, long ld, int how) {
+        double old[16];
+        if (how != OZ_LAUUM_SET) {
+#pragma unroll
+          for (int e = 0; e < 16; e++) {
+            const int ee = KEEP + e;
+            old[e] = C[gi0 + 8 * ((ee >> 1) & 1) + (gj0 + (ee >> 2) * 8 + (ee & 1)) * ld];
+          }
+        }
+#pragma unroll
+        for (int e = 0; e < 16; e++) {
+          const int ee = KEEP + e;
+          C[gi0 + 8 * ((ee >> 1) & 1) + (gj0 + (ee >> 2) * 8 + (ee & 1)) * ld] =
+              how == OZ_UPDATE ? old[e] - v[e] : (how == OZ_LAUUM_ACC ? old[e] + v[e] : v[e]);
+        }
+      };
+      if (kind == OZ_UPDATE) apply(p.S, p.lds, OZ_UPDATE);
+      else if (kind == OZ_PANEL) {
+        apply(p.P, p.ldp, OZ_LAUUM_SET);
+        // the panel rows also take their final place in the workspace (U block column above, L panel below the diagonal
+        // block): its digit planes were taken before this launch, nothing reads the fp64 block column any more
+        if (p.Pfinal) apply(p.Pfinal, p.lds, OZ_LAUUM_SET);
+      } else apply(p.Kinv, p.ldk, kind);
+    }
+  }
+}
+
+// Warp roles: warpgroups 0 and 1 = consumers (setmaxnreg 232: 128 s32 accumulators + 32 fp64 sums per thread), warp 8 =
+// TMA producer, warps 9..11 idle (the third warpgroup hands its registers over: 40 each).
 __global__ void __launch_bounds__(OZ_THREADS, 1)
 oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const OzParams p) {
   extern __shared__ unsigned char oz_smem_raw[];
   unsigned char* ring = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(oz_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + OZ_STAGES * OZ_STAGE_BYTES);
+  double* xch = reinterpret_cast<double*>(ring + OZ_STAGES * OZ_STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + OZ_STAGES * OZ_STAGE_BYTES + OZ_XCH_BYTES);
   uint64_t* empty = full + OZ_STAGES;
-  uint64_t* tmem_full = empty + OZ_STAGES;
-  uint64_t* tmem_empty = tmem_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
+  const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
 #pragma unroll
-    for (int s = 0; s < OZ_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
-    mbar_init(tmem_empty, OZ_EPI_WARPS);
+    for (int s = 0; s < OZ_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     fence_mbar_init();
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
   }
-  if (warp == 1) {   // the MMA warp owns the TMEM allocation: all 512 columns (8 exponent groups x 64)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t taddr = *tmem_slot;
-  const int nkc = p.nkc;
+  const int tw = p.wide ? 2 * OZ_TN : OZ_TN;
   // a CTA owns p.tpc CONSECUTIVE tiles of the list (neighbours in the banded order share operand panels in L2) and then
   // retires: SM slots come free every few tiles, so the high-priority side stream of the sweep (diagonal block, panel of the
   // next step) gets onto the machine while this launch is still running — a fully persistent grid would shut it out
   const int ti_beg = blockIdx.x * p.tpc, ti_end = min(p.ntiles, ti_beg + p.tpc);
-
-  if (warp == 0) {
+  if (wg == 2) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x >= 288) return;
     // ================= TMA producer: lane s < nd loads digit plane s of both operands ================================
-    uint32_t it = 0;
-    for (int ti = ti_beg; ti < ti_end; ti++) {
-      const uint32_t t = p.tiles[ti];
-      const int r = t & 0xfff, c64 = (t >> 12) & 0x1fff;
-      const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
-      for (int kc = 0; kc < nkc; kc++, it++) {
-        const int st = it % OZ_STAGES;
-        if (p.dbg & 16) mbar_wait(&empty[st], ((it / OZ_STAGES) & 1) ^ 1);
-        else mbar_wait_backoff(&empty[st], ((it / OZ_STAGES) & 1) ^ 1, 64);
-        if (p.dbg & 2) { if (lane == 0) mbar_arrive(&full[st]); continue; }
-        // complete_tx of a copy may precede the expect_tx below: the phase cannot complete before lane 0's arrival
-        unsigned char* dst = ring + st * OZ_STAGE_BYTES;
-        if (lane < nd) {
-          tma_load_4d(dst + lane * OZ_A_BYTES, &mapA, 0, r * (OZ_TM / 8), kc, lane, &full[st]);
-          tma_load_4d(dst + OZ_S * OZ_A_BYTES + lane * OZ_B_BYTES, &mapB, 0, c64 * (OZ_TN / 8), kc, lane, &full[st]);
-        }
-        if (lane == 0) mbar_arrive_expect_tx(&full[st], (uint32_t)nd * (OZ_A_BYTES + OZ_B_BYTES));
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer ====================================================================================
-    // The issue loop must sustain one tcgen05.mma per ~48 clk from ONE thread: descriptors are not rebuilt per instruction
-    // (the first version spent ~100 clk of uniform-datapath arithmetic per MMA and ran at half the shared-memory bound);
-    // the low descriptor word of plane s is the stage's base word + s * (plane bytes >> 4), the 36 instructions of a
-    // k-chunk are straight-line code (template on the digit count). The whole warp executes the loop convergently and an
-    // elected lane issues: inside an `if (lane == 0)` region the compiler can lose track of warp-uniformity and then
-    // feeds every MMA operand through R2UR from vector registers (measured: 1.3x slower issue).
-    {   // the WHOLE warp runs the (warp-uniform) control flow; one elected lane issues MMAs and commits
-      uint32_t it = 0, tl = 0;
-      const uint32_t ring_lo = (smem_u32(ring) & 0x3FFFF) >> 4;
-      for (int ti = ti_beg; ti < ti_end; ti++, tl++) {
-        const uint32_t t = p.tiles[ti];
-        const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
-        mbar_wait(tmem_empty, (tl & 1) ^ 1);     // the epilogue has read the previous tile out of TMEM
-        tc_fence_after();
-        for (int kc = 0; kc < nkc; kc++, it++) {
-          const int st = it % OZ_STAGES;
-          mbar_wait(&full[st], (it / OZ_STAGES) & 1);
-          tc_fence_after();
-          const uint32_t a_lo = ring_lo + (uint32_t)st * (OZ_STAGE_BYTES >> 4);
-          const uint32_t acc0 = kc > 0 ? 1u : 0u;
-          if (elect_one()) {
-            if (!(p.dbg & 1)) {
-              if (nd == 8) oz_issue_groups<8, 0, 8>(taddr, a_lo, acc0);
-              else if (nd == 7) oz_issue_groups<7, 0, 7>(taddr, a_lo, acc0);
-              else if (nd == 6) oz_issue_groups<6, 0, 6>(taddr, a_lo, acc0);
-              else if (nd == 5) oz_issue_groups<5, 0, 5>(taddr, a_lo, acc0);
-              else oz_issue_groups<4, 0, 4>(taddr, a_lo, acc0);
-            }
-            umma_commit(&empty[st]);              // the stage may be refilled once these MMAs have read it
-          }
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(tmem_full);  // accumulators of this tile complete
-        __syncwarp();
-      }
-    }
-  } else {
-    // ================= epilogue warps: TMEM lane quarter = warp % 4, column half = (warp - 2) / 4 ====================
-    const int q = warp & 3, h = (warp - 2) >> 2;
-    uint32_t tl = 0;
-    for (int ti = ti_beg; ti < ti_end; ti++, tl++) {
-      const uint32_t t = p.tiles[ti];
-      const int r = t & 0xfff, c64 = (t >> 12) & 0x1fff, kind = (t >> 25) & 3;
-      const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
-      if (p.dbg & 8) mbar_wait(tmem_full, tl & 1);
-      else mbar_wait_backoff(tmem_full, tl & 1, 128);
-      tc_fence_after();
-      double acc[32];
-#pragma unroll
-      for (int j = 0; j < 32; j++) acc[j] = 0.0;
-      for (int g = ((p.dbg & 4) ? 0 : nd) - 1; g >= 0; g--) {         // smallest magnitude first
-        uint32_t v[32];
-        tmem_ld32(taddr + ((uint32_t)(q * 32) << 16) + (uint32_t)(g * OZ_TN + h * 32), v);
-        const double sc = __longlong_as_double((long long)(1023 - 7 * g) << 52);   // 2^(-7 g)
-        // s32 -> fp64 without the conversion unit (I2F.F64 is a few lanes per SM: it made the TMEM drain ~15k clk per tile):
-        // the bit pattern {0x43300000, v ^ 0x80000000} is the double 2^52 + 2^31 + v, one exact DADD takes the offset off
-#pragma unroll
-        for (int j = 0; j < 32; j++)
-          acc[j] = fma(__hiloint2double(0x43300000, (int)(v[j] ^ 0x80000000u)) - 4503601774854144.0, sc, acc[j]);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty);     // TMEM may be overwritten by the next tile's MMAs
-      if (p.dbg & 4) continue;
-      const long gi = (long)r * OZ_TM + q * 32 + lane;
-      const long gj0 = (long)c64 * OZ_TN + h * 32;
-      const double si = p.scale[gi];
-      if (kind == OZ_UPDATE) oz_apply_row<32>(p.S + gi + gj0 * p.lds, p.lds, acc, si, p.scale + gj0, kind);
-      else oz_apply_row<32>(p.Kinv + gi + gj0 * p.ldk, p.ldk, acc, si, p.scale + gj0, kind);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(taddr));
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// 2b. the two-pass variant: 128 x 128 output tiles, tcgen05.mma 128 x 128 x 32.
-// At N = 64 the tensor core re-reads the 4 KB A plane for every 2 KB B plane and the 128 B/clk shared-memory read port
-// caps it at 2/3 of its rate (48 clk instead of 32 per MMA, tools/microbench_ozaki_pattern.cu); at N = 128 it runs at the
-// full 8192 MAC/clk. Eight exponent groups x 128 columns do not fit the 512 TMEM columns, so a tile is computed in two
-// passes over K: first the low-order groups 4..7 (26 digit pairs, all planes), drained into fp64 registers, then the
-// high-order groups 0..3 (10 pairs, planes 0..3 only). Operand traffic per output element is 1.5x that of the one-pass
-// kernel (24 instead of 16 plane-tile loads per 128 x 128 x 32), the MMA time 2/3.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int OZ2_TN = 128;
-constexpr int OZ2_STAGES = 3;
-constexpr int OZ2_PLANE = OZ_TM * OZ_KC;                          // 4096 bytes: one digit plane of a 128-row tile, one k-chunk
-constexpr int OZ2_STAGE_BYTES = 2 * OZ_S * OZ2_PLANE;             // 65536: up to 8 A planes + 8 B planes
-constexpr int OZ2_SMEM = OZ2_STAGES * OZ2_STAGE_BYTES + 1024 + 256;
-constexpr int OZ2_THREADS = 384;                                   // three warpgroups (setmaxnreg works per warpgroup)
-
-// groups [G_BEG, G_END) of one k-chunk, highest group first; group g accumulates in TMEM columns [(g - G_BASE) * 128, +128)
-template <int G, int G_BASE>
-__device__ __forceinline__ void oz2_issue_group(uint32_t taddr, uint32_t a_lo, uint32_t acc0) {
-  constexpr uint32_t idesc = oz_idesc(OZ_TM, OZ2_TN);
-  constexpr uint64_t hi = ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46);
-  const uint32_t b_lo = a_lo + (uint32_t)((OZ_S * OZ2_PLANE) >> 4);
-#pragma unroll
-  for (int s = 0; s <= G; s++) {
-    const uint64_t da = hi | (uint64_t)(a_lo + (uint32_t)(s * (OZ2_PLANE >> 4)));
-    const uint64_t db = hi | (uint64_t)(b_lo + (uint32_t)((G - s) * (OZ2_PLANE >> 4)));
-    umma_i8(taddr + (uint32_t)((G - G_BASE) * OZ2_TN), da, db, idesc, s > 0 ? 1u : acc0);
-  }
-}
-template <int G_BEG, int G_END, int G_BASE>
-__device__ __forceinline__ void oz2_issue_groups(uint32_t taddr, uint32_t a_lo, uint32_t acc0) {
-  if constexpr (G_END > G_BEG) {
-    oz2_issue_group<G_END - 1, G_BASE>(taddr, a_lo, acc0);
-    oz2_issue_groups<G_BEG, G_END - 1, G_BASE>(taddr, a_lo, acc0);
-  }
-}
-// First k-chunk of a pass: the accumulator of group g (TMEM slot g - G_BASE) is overwritten as soon as the epilogue has drained
-// THAT slot of the previous pass (it drains the slots in the same descending order), not the whole TMEM: the tensor core waits
-// for one slot's drain (~670 clk) instead of four. Bit s of usebits is the parity of the number of passes that used slot s (the mbarrier phase to wait for).
-template <int G_BEG, int G_END, int G_BASE>
-__device__ __forceinline__ void oz2_first_chunk(uint32_t taddr, uint32_t a_lo, uint64_t* tmem_empty, uint32_t& usebits, bool issue) {
-  if constexpr (G_END > G_BEG) {
-    constexpr int slot = G_END - 1 - G_BASE;
-    mbar_wait(&tmem_empty[slot], ((usebits >> slot) & 1u) ^ 1u);
-    usebits ^= 1u << slot;
-    tc_fence_after();
-    if (elect_one()) {
-      if (issue) oz2_issue_group<G_END - 1, G_BASE>(taddr, a_lo, 0u);
-    }
-    __syncwarp();
-    oz2_first_chunk<G_BEG, G_END - 1, G_BASE>(taddr, a_lo, tmem_empty, usebits, issue);
-  }
-}
-// k-chunks of a tile: the whole panel width, except OZ_PANEL tiles (triangular B: columns of tile c' see k < (c' + 1) * 128)
-__device__ __forceinline__ int oz2_tile_nkc(uint32_t t, int nkc) {
-  return ((t >> 25) & 3) == OZ_PANEL ? min(nkc, (int)(((t >> 12) & 0x1fff) + 1) * (OZ2_TN / OZ_KC)) : nkc;
-}
-// Warp roles: warps 0..7 = epilogue (TMEM lane quarter = warp % 4, column half = warp / 4; two warpgroups that raise their
-// register budget to 224 with setmaxnreg: 64 fp64 accumulators per thread live across the two passes), warp 8 = TMA
-// producer, warp 9 = MMA issuer, warps 10-11 idle (the third warpgroup hands its registers over: 56 each).
-__global__ void __launch_bounds__(OZ2_THREADS, 1)
-oz_gemm2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const OzParams p) {
-  extern __shared__ unsigned char oz_smem_raw[];
-  unsigned char* ring = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(oz_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(ring + OZ2_STAGES * OZ2_STAGE_BYTES);
-  uint64_t* empty = full + OZ2_STAGES;
-  uint64_t* tmem_full = empty + OZ2_STAGES;
-  uint64_t* tmem_empty = tmem_full + 1;                    // one per TMEM slot (128 accumulator columns)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int s = 0; s < OZ2_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
-#pragma unroll
-    for (int s = 0; s < 4; s++) mbar_init(&tmem_empty[s], OZ_EPI_WARPS);
-    fence_mbar_init();
-    tma_prefetch_desc(&mapA);
-    tma_prefetch_desc(&mapB);
-  }
-  if (warp == 9) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t taddr = *tmem_slot;
-  const int nkc = p.nkc;
-  const int ti_beg = blockIdx.x * p.tpc, ti_end = min(p.ntiles, ti_beg + p.tpc);
-
-  if (warp >= 8) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-  if (warp == 8) {
-    // ================= TMA producer =================================================================================
+    const int lane = threadIdx.x & 31;
+    const int nsub = 2 * (tw / OZ_SUB);
     uint32_t it = 0;
     for (int ti = ti_beg; ti < ti_end; ti++) {
       const uint32_t t = p.tiles[ti];
       const int r = t & 0xfff, c = (t >> 12) & 0x1fff;
-      const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;   // >= 5 here: both passes always run, so that the stage
-      const int nkc_t = oz2_tile_nkc(t, nkc);
-      for (int pass = 0; pass < 2; pass++) {                    // counter stays warp-uniform (descriptors in uniform registers)
-        const int npl = pass == 0 ? nd : 4;        // low-order groups need every plane, groups 0..3 only planes 0..3
-        for (int kc = 0; kc < nkc_t; kc++, it++) {
-          const int st = it % OZ2_STAGES;
-          if (p.dbg & 16) mbar_wait(&empty[st], ((it / OZ2_STAGES) & 1) ^ 1);
-          else mbar_wait_backoff(&empty[st], ((it / OZ2_STAGES) & 1) ^ 1, 64);
-          if (p.dbg & 2) { if (lane == 0) mbar_arrive(&full[st]); continue; }
-          unsigned char* dst = ring + st * OZ2_STAGE_BYTES;
-          if (lane < npl) {
-            tma_load_4d(dst + lane * OZ2_PLANE, &mapA, 0, r * (OZ_TM / 8), kc, lane, &full[st]);
-            tma_load_4d(dst + (OZ_S + lane) * OZ2_PLANE, &mapB, 0, c * (OZ2_TN / 8), kc, lane, &full[st]);
-          }
-          if (lane == 0) mbar_arrive_expect_tx(&full[st], (uint32_t)npl * 2 * OZ2_PLANE);
-        }
-      }
-    }
-  } else if (warp == 9) {
-    // ================= MMA issuer (one thread) ======================================================================
-    {   // the WHOLE warp runs the (warp-uniform) control flow; one elected lane issues MMAs and commits
-      uint32_t ph = 0;
-      uint32_t usebits = 0u;
-      int st = 0;
-      const uint32_t ring_lo = (smem_u32(ring) & 0x3FFFF) >> 4;
-      const bool issue = !(p.dbg & 1);
-      for (int ti = ti_beg; ti < ti_end; ti++) {
-        const uint32_t t = p.tiles[ti];
-        const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
-        const int nkc_t = oz2_tile_nkc(t, nkc);
-        // the two passes are two copies of the loop (compile-time pass): with a run-time pass variable selecting the MMA
-        // block the compiler keeps the descriptors in vector registers (R2UR per operand, ~1.3x slower issue)
-        auto run_pass = [&](auto pass_tag) {
-          constexpr int pass = decltype(pass_tag)::value;
-          for (int kc = 0; kc < nkc_t; kc++) {
-            mbar_wait(&full[st], ph);
-            tc_fence_after();
-            const uint32_t a_lo = ring_lo + (uint32_t)st * (OZ2_STAGE_BYTES >> 4);
-            if (kc == 0) {   // slot by slot behind the epilogue's drain of the previous pass
-              if (pass == 1) oz2_first_chunk<0, 4, 0>(taddr, a_lo, tmem_empty, usebits, issue);
-              else if (nd == 8) oz2_first_chunk<4, 8, 4>(taddr, a_lo, tmem_empty, usebits, issue);
-              else if (nd == 7) oz2_first_chunk<4, 7, 4>(taddr, a_lo, tmem_empty, usebits, issue);
-              else if (nd == 6) oz2_first_chunk<4, 6, 4>(taddr, a_lo, tmem_empty, usebits, issue);
-              else oz2_first_chunk<4, 5, 4>(taddr, a_lo, tmem_empty, usebits, issue);
-              if (elect_one()) umma_commit(&empty[st]);
-            } else if (elect_one()) {
-              if (issue) {
-                if (pass == 1) oz2_issue_groups<0, 4, 0>(taddr, a_lo, 1u);          // groups 0 .. 3
-                else if (nd == 8) oz2_issue_groups<4, 8, 4>(taddr, a_lo, 1u);       // low-order groups 4 .. nd-1
-                else if (nd == 7) oz2_issue_groups<4, 7, 4>(taddr, a_lo, 1u);
-                else if (nd == 6) oz2_issue_groups<4, 6, 4>(taddr, a_lo, 1u);
-                else oz2_issue_groups<4, 5, 4>(taddr, a_lo, 1u);
-              }
-              umma_commit(&empty[st]);
-            }
-            __syncwarp();
-            if (++st == OZ2_STAGES) { st = 0; ph ^= 1; }
-          }
-          if (elect_one()) umma_commit(tmem_full);
-          __syncwarp();
-        };
-        run_pass(std::integral_constant<int, 0>{});
-        run_pass(std::integral_constant<int, 1>{});
-      }
-    }
-  }
-  } else {
-    // ================= epilogue warps: TMEM lane quarter = warp % 4, 64 of the 128 columns each =======================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int q = warp & 3, h = warp >> 2;
-    uint32_t hs = 0;
-    for (int ti = ti_beg; ti < ti_end; ti++) {
-      const uint32_t t = p.tiles[ti];
-      const int r = t & 0xfff, c = (t >> 12) & 0x1fff, kind = (t >> 25) & 3;
       const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
-      double acc[64];
-#pragma unroll
-      for (int j = 0; j < 64; j++) acc[j] = 0.0;
-      for (int pass = 0; pass < 2; pass++, hs++) {
-        if (p.dbg & 8) mbar_wait(tmem_full, hs & 1);
-        else mbar_wait_backoff(tmem_full, hs & 1, 128);
-        tc_fence_after();
-        const int gbase = pass == 0 ? 4 : 0, gtop = pass == 0 ? nd : 4;
-        for (int g = gtop - 1; g >= gbase; g--) {   // smallest magnitude first (pass 0 before pass 1)
-          const double sc = __longlong_as_double((long long)(1023 - 7 * g) << 52);   // 2^(-7 g)
-          uint32_t v0[32], v1[32];
-          if (!(p.dbg & 4)) {
-            const uint32_t ta = taddr + ((uint32_t)(q * 32) << 16) + (uint32_t)((g - gbase) * OZ2_TN + h * 64);
-            tmem_ld32(ta, v0);
-            tmem_ld32(ta + 32, v1);
-          }
-          tc_fence_before();
+      const int nkc_t = oz_tile_nkc(t, p.nkc);
+      for (int sub = 0; sub < nsub; sub++) {
+        const int arow = (r * OZ_TM + (sub & 1) * OZ_SUB) / 8, brow = (c * tw + (sub >> 1) * OZ_SUB) / 8;
+        for (int kc = 0; kc < nkc_t; kc++, it++) {
+          const int st = it % OZ_STAGES;
+          mbar_wait_backoff(&empty[st], ((it / OZ_STAGES) & 1) ^ 1, 64);
+          if (lane == 0) mbar_arrive_expect_tx(&full[st], (uint32_t)nd * 2 * OZ_PLANE);
           __syncwarp();
-          if (lane == 0 && !(p.dbg & 32)) mbar_arrive(&tmem_empty[g - gbase]);   // this slot may take the next pass's MMAs: the fp64 sum follows
-          if (!(p.dbg & 4)) {
-#pragma unroll
-            for (int j = 0; j < 32; j++)
-              acc[j] = fma(__hiloint2double(0x43300000, (int)(v0[j] ^ 0x80000000u)) - 4503601774854144.0, sc, acc[j]);
-#pragma unroll
-            for (int j = 0; j < 32; j++)
-              acc[32 + j] = fma(__hiloint2double(0x43300000, (int)(v1[j] ^ 0x80000000u)) - 4503601774854144.0, sc, acc[32 + j]);
+          unsigned char* dst = ring + st * OZ_STAGE_BYTES;
+          if (lane < nd) {
+            tma_load_4d(dst + lane * OZ_PLANE, &mapA, 0, arow, kc, lane, &full[st]);
+            tma_load_4d(dst + (OZ_S + lane) * OZ_PLANE, &mapB, 0, brow, kc, lane, &full[st]);
           }
         }
-        if (p.dbg & 32) {   // measurement: release the whole TMEM only after the full drain (the behaviour before the per-slot barriers)
-          __syncwarp();
-          if (lane == 0)
-            for (int g = gtop - 1; g >= gbase; g--) mbar_arrive(&tmem_empty[g - gbase]);
-        }
       }
-      if (p.dbg & 4) continue;
-      const long gi = (long)r * OZ_TM + q * 32 + lane;
-      const long gj0 = (long)c * OZ2_TN + h * 64;
-      const double si = p.scale[gi];
-      if (kind == OZ_UPDATE) oz_apply_row<64>(p.S + gi + gj0 * p.lds, p.lds, acc, si, p.scale + gj0, kind);
-      else if (kind == OZ_PANEL) {
-        oz_apply_row<64>(p.P + gi + gj0 * p.ldp, p.ldp, acc, si, p.scaleB + gj0, OZ_LAUUM_SET);
-        // the panel rows also take their final place in the workspace (U block column above, L panel below the diagonal
-        // block): its digit planes were taken before this launch, nothing reads the fp64 block column any more
-        if (p.Pfinal) oz_apply_row<64>(p.Pfinal + gi + gj0 * p.lds, p.lds, acc, si, p.scaleB + gj0, OZ_LAUUM_SET);
-      }
-      else oz_apply_row<64>(p.Kinv + gi + gj0 * p.ldk, p.ldk, acc, si, p.scale + gj0, kind);
     }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    if (wg == 0) oz_consume<0>(p, ring, xch, full, empty, ti_beg, ti_end, tw);
+    else oz_consume<1>(p, ring, xch, full, empty, ti_beg, ti_end, tw);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(taddr));
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // tile lists of the sweep (host): per panel step the launches U0 | U1 | U2 (+ the K^-1 tiles of the step)
 // ---------------------------------------------------------------------------------------------------------------
-// tiles in bands of 8 row tiles x 16 column tiles (64 wide): the ~148 tiles in flight share 8 A panels and 16 B panels in L2
-// (column tiles: cw per 128 columns - two 64-wide tiles for the one-pass kernel, one 128-wide tile for the two-pass kernel)
+// tiles in bands of 8 row tiles x 16 column tiles (64 wide): the ~132 tiles in flight share 8 A panels and 16 B panels in L2
+// (column tiles: cw per 128 columns - two 64-wide tiles, or one 128-wide tile with option oz_wide)
 template <class Valid, class Emit>
 static void oz_banded(const std::vector<int>& rows, int ct_beg, int ct_end, int cw, Valid valid, Emit emit) {
   for (size_t b = 0; b < rows.size(); b += 8)
@@ -697,15 +471,14 @@ int oz_init() {
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   }
   GPX_CUDA(cudaFuncSetAttribute(oz_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OZ_SMEM));
-  GPX_CUDA(cudaFuncSetAttribute(oz_gemm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OZ2_SMEM));
   return 0;
 }
 
-static int oz_make_map(CUtensorMap* map, const OzPlanes& pl, int box_rows) {
+static int oz_make_map(CUtensorMap* map, const OzPlanes& pl) {
   const cuuint64_t ngrp = (cuuint64_t)(pl.rows / 8);
   cuuint64_t dims[4] = {256, ngrp, (cuuint64_t)pl.nkc, (cuuint64_t)OZ_S};
   cuuint64_t strides[3] = {256, ngrp * 256, (cuuint64_t)pl.nkc * ngrp * 256};
-  cuuint32_t box[4] = {256, (cuuint32_t)(box_rows / 8), 1, 1};
+  cuuint32_t box[4] = {256, (cuuint32_t)(OZ_SUB / 8), 1, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   const CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, pl.planes, dims, strides, box, estr,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -721,7 +494,7 @@ int oz_planes_alloc(OzPlanes& pl, long rows, long K) {
   GPX_CUDA(cudaMalloc(&pl.planes, (size_t)OZ_S * rows * K));
   GPX_CUDA(cudaMalloc(&pl.scale, (size_t)rows * 8));
   GPX_CUDA(cudaMalloc(&pl.amax_part, (size_t)rows * 8 * 8));   // SPLIT_KS partial row maxima
-  if (oz_make_map(&pl.mapA, pl, OZ_TM) || oz_make_map(&pl.mapB, pl, OZ_TN)) return -1;
+  if (oz_make_map(&pl.map, pl)) return -1;
   return 0;
 }
 
@@ -735,13 +508,11 @@ void oz_planes_free(OzPlanes& pl) {
 int launch_oz_gemm(const OzPlanes& pl, const OzParams& p_in, int num_sms, cudaStream_t st, const OzPlanes* plB) {
   if (p_in.ntiles <= 0) return 0;
   OzParams p = p_in;
-  // default: 8 narrow / 4 wide tiles per CTA when there is enough work (measured: 1 -> 2 -> 4 -> 8 tiles per CTA = 118 / 104 / 98 / 91 ms)
+  // default: 8 narrow / 4 wide tiles per CTA when there is enough work
   if (p.tpc <= 0) p.tpc = std::max(1, std::min(p.wide ? 4 : 8, p.ntiles / std::max(1, num_sms)));
   const int grid = (p.ntiles + p.tpc - 1) / p.tpc;
-  if (p.wide && (p.dig_lo < 5 || p.dig_up < 5)) { set_error("the two-pass kernel needs at least 5 digits"); return -2; }
-  if (plB && !p.wide) { set_error("OZ_PANEL tiles need the two-pass kernel"); return -2; }
-  if (p.wide) oz_gemm2_kernel<<<grid, OZ2_THREADS, OZ2_SMEM, st>>>(pl.mapA, plB ? plB->mapA : pl.mapA, p);
-  else oz_gemm_kernel<<<grid, OZ_THREADS, OZ_SMEM, st>>>(pl.mapA, pl.mapB, p);
+  if (plB && !p.wide) { set_error("OZ_PANEL tiles are listed in 128-column units (wide)"); return -2; }
+  oz_gemm_kernel<<<grid, OZ_THREADS, OZ_SMEM, st>>>(pl.map, plB ? plB->map : pl.map, p);
   GPX_CUDA(cudaGetLastError());
   return 0;
 }
@@ -876,7 +647,7 @@ __global__ void __launch_bounds__(256) grad_kinv_kernel(GradKinvParams p) {
 int grad_kinv_csplit(int nt, int nred) {
   const int tiles = nt * (nt + 1) / 2;
   int cs = 1;
-  while (cs < 8 && tiles * cs < 592 && (cs * 2) * nred <= MAX_D + 2) cs *= 2;   // ~4 waves of CTAs; partials sized for MAX_D + 2 per tile
+  while (cs < 8 && tiles * cs < 528 && (cs * 2) * nred <= MAX_D + 2) cs *= 2;   // ~4 waves of CTAs on 132 SMs; partials sized for MAX_D + 2 per tile
   return cs;
 }
 

@@ -1,4 +1,4 @@
-// gpx_ozaki.cuh — fp64-grade GEMM on the INT8 tensor path (tcgen05.mma kind::i8, TMEM accumulators, TMA-fed): internal API.
+// gpx_ozaki.cuh — fp64-grade GEMM on the INT8 tensor path (wgmma s8 x s8 -> s32, register accumulators, TMA-fed): internal API.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -12,12 +12,12 @@ struct gpx_ctx;
 namespace gpx {
 
 constexpr int OZ_S = 8;         // signed 7-bit digit planes per fp64 operand (56 bits >= the 53-bit significand)
-constexpr int OZ_TM = 128;      // output tile rows   (= MMA M, one TMEM lane per row)
-constexpr int OZ_TN = 64;       // output tile columns (= MMA N; 8 exponent groups x 64 columns = all 512 TMEM columns)
-constexpr int OZ_KC = 32;       // k-depth of one tcgen05.mma kind::i8 (32 bytes of K)
+constexpr int OZ_TM = 128;      // output tile rows   (two 64-row wgmma sub-tiles)
+constexpr int OZ_TN = 64;       // output tile columns (= wgmma N; 128 with option oz_wide)
+constexpr int OZ_KC = 32;       // k-depth of one wgmma .s8 (32 bytes of K)
 
 // Digit planes of one panel (rows x K, K = nkc * 32), stored so that every (plane, k-chunk, 8-row group) is one 256-byte
-// block in exactly the shared-memory image tcgen05 reads (no-swizzle K-major core matrices: two 8 x 16 B core matrices per
+// block in exactly the shared-memory image wgmma reads (no-swizzle K-major core matrices: two 8 x 16 B core matrices per
 // block). A tile of R rows of one (plane, k-chunk) is therefore R*32 contiguous bytes = one TMA box {256, R/8, 1, 1}.
 //   byte offset of digit s of element (row i, column k):
 //     (((s * nkc + k/32) * (rows/8) + i/8) * 256) + ((k%32)/16)*128 + (i%8)*16 + k%16
@@ -27,7 +27,7 @@ struct OzPlanes {
   double* amax_part = nullptr;  // [8][rows]: partial row maxima (scratch of the split)
   long rows = 0;
   int nkc = 0;
-  CUtensorMap mapA, mapB;       // the same tensor with a 128-row and a 64-row box
+  CUtensorMap map;              // the tensor with a 64-row box (one wgmma operand of one plane and k-chunk)
 };
 
 // one output tile: bits 0-11 row tile (128 rows), 12-24 column tile (64 columns), 25-26 kind, 27 inverse-part tile
@@ -45,15 +45,13 @@ struct OzParams {
   double* Kinv; long ldk;  // OZ_LAUUM_* target:     Kinv(r, c) (+)= P_r P_c^T   (lower tiles)
   int dig_lo, dig_up;      // digits per operand for Cholesky-part tiles / inverse-part tiles (<= OZ_S)
   int tpc;                 // consecutive tiles per CTA (0 = default)
-  int wide;                // 1: 128 x 128 tiles (two-pass kernel, column tile index in 128-column units), 0: 128 x 64 tiles
-  // OZ_PANEL tiles (two-pass kernel only): P(r, c') = A_r B_c'^T with A = digit planes of a block column of the workspace
-  // (the launch's tensor map), B = digit planes of L_kk^-1 (mapB of launch_oz_gemm), lower triangular: the k-range of output
+  int wide;                // 1: 128 x 128 tiles (column tile index in 128-column units), 0: 128 x 64 tiles
+  // OZ_PANEL tiles (wide only): P(r, c') = A_r B_c'^T with A = digit planes of a block column of the workspace
+  // (pl of launch_oz_gemm), B = digit planes of L_kk^-1 (plB of launch_oz_gemm), lower triangular: the k-range of output
   // column tile c' ends at (c' + 1) * 128. Result stored (not accumulated) into P.
   double* P; long ldp;
   double* Pfinal;          // optional second target of OZ_PANEL tiles: the block column of the workspace itself (ld = lds)
   const double* scaleB;    // row scales of the B operand's planes (= column scales of the product)
-  int dbg;                 // measurement only: 1 = no MMA issue, 2 = no TMA loads, 4 = no epilogue work (results invalid);
-                           // 8 / 16 = epilogue / producer wait WITHOUT back-off, 32 = TMEM released per pass, not per slot (results valid)
 };
 
 // one panel step of the sweep: offsets into the tile list. U0: the next diagonal block only; U1: the rest of block column k+1;

@@ -290,7 +290,7 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
   }
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
   const int nl = s->kp.ard ? D : 1, nred = nl + 1;
-  const int nchunk = (int)std::max<long>(1, std::min<long>((N + 31) / 32, (4 * 148 + mt - 1) / mt));
+  const int nchunk = (int)std::max<long>(1, std::min<long>((N + 31) / 32, (4 * c->num_sms + mt - 1) / mt));
   const long mchunk = ((N + nchunk - 1) / nchunk + 31) / 32 * 32;
   const int nch = (int)((N + mchunk - 1) / mchunk);
   const size_t part_full = (size_t)mt * ntl * nred * 8, part_x = (size_t)nch * M * D * 8 + (size_t)M * D * 8;
@@ -571,7 +571,7 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     for (int q = 0; q < nl; q++) dl_kmm[q] = -tot[1 + q] / s->kp.ls[q];
   }
   {
-    const int nchunk = (int)std::max<long>(1, std::min<long>((M + 31) / 32, (4 * 148 + mt - 1) / mt));
+    const int nchunk = (int)std::max<long>(1, std::min<long>((M + 31) / 32, (4 * c->num_sms + mt - 1) / mt));
     const long mchunk = ((M + nchunk - 1) / nchunk + 31) / 32 * 32;
     const int nch = (int)((M + mchunk - 1) / mchunk);
     GPX_CHECK(ensure_part(s, (size_t)(nch + 1) * M * D * 8));

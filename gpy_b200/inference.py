@@ -1,4 +1,4 @@
-"""Host-side mirror of GPy's exact Gaussian inference plugin, computing on the B200 through libgpx.
+"""Host-side mirror of GPy's exact Gaussian inference plugin, computing on the H100 through libgpx.
 
 Mirrors (same names, argument meaning, return structure and error behaviour):
     GPy.inference.latent_function_inference.ExactGaussianInference.inference

@@ -1,4 +1,4 @@
-"""Host-side mirror of GPy's stationary-kernel plugin interface, computing on the B200 through libgpx.
+"""Host-side mirror of GPy's stationary-kernel plugin interface, computing on the H100 through libgpx.
 
 Same names, argument meaning and error behaviour as the reference classes:
     GPy.kern.RBF           GPy/kern/src/rbf.py:13-52,177-178

@@ -1,4 +1,4 @@
-"""Host-side mirror of GPy's sparse GP regression (VarDTC), computing the N-dependent work on the B200.
+"""Host-side mirror of GPy's sparse GP regression (VarDTC), computing the N-dependent work on the H100.
 
 Mirrors:
     GPy.inference.latent_function_inference.VarDTC.inference   GPy/inference/latent_function_inference/var_dtc.py:66-215

@@ -1,11 +1,13 @@
-/* gpx.h — C ABI of the B200-native exact-GP engine (libgpx.so).
+/* gpx.h — C ABI of the H100 exact-GP engine (libgpx.so).
  *
  * This is the drop-in boundary for ONE hot path of SheffieldML/GPy:
  *     GPRegression -> GP.parameters_changed -> ExactGaussianInference.inference -> Kern.K/Kdiag/update_gradients_full
  * Each entry point names the reference interface it replaces (paths relative to the GPy repository root).
  * Plain C: pointers and sizes only, no torch / numpy types. All inputs, outputs and stored matrices are IEEE fp64; the N^3
- * products run on fp64 tensor instructions (DMMA) or, from N = 8192 on one GPU, as int8 digit-split products on the tcgen05
- * tensor cores whose exact s32 sums are recombined in fp64 (8 digits for the Cholesky part, 7 for the inverse part:
+ * products run on fp64 tensor instructions (DMMA, the default) or, with option "ozaki" on one GPU wherever the matrix has two
+ * or more outer blocks, as int8
+ * digit-split products on the wgmma tensor cores whose exact s32 sums are recombined in fp64 (8 digits for the Cholesky
+ * part, 7 for the inverse part:
  * |dLML| <= 1e-8 and 1e-6 relative on gradients against the reference, DESIGN.md section 5.1; option "ozaki" selects).
  *
  * Conventions
@@ -168,9 +170,9 @@ typedef struct {
   float total_ms;       /* whole eval, H2D of theta .. D2H of (lml, grad) */
   float kbuild_ms;      /* covariance build kernel */
   float sweep_ms;       /* blocked factor-and-invert sweep (all launches) */
-  float update_ms;      /* sum over the outer trailing-update GEMM launches (dominant kernel); on the tcgen05 path these launches
+  float update_ms;      /* sum over the outer trailing-update GEMM launches (dominant kernel); on the Ozaki path these launches
                            also accumulate K^-1 = U U^T */
-  float lauum_ms;       /* DMMA path: K^-1 = U U^T + fused gradient epilogue; tcgen05 path: gradient reductions from the stored K^-1 */
+  float lauum_ms;       /* DMMA path: K^-1 = U U^T + fused gradient epilogue; Ozaki path: gradient reductions from the stored K^-1 */
   float solve_ms;       /* alpha / quadratic form */
   double update_flops;  /* algorithmic flops executed by the outer trailing-update launches */
   double lauum_flops;
@@ -178,18 +180,18 @@ typedef struct {
   int64_t launches;     /* kernels launched by the last eval */
   int32_t update_launches;
   int32_t tries;        /* factorisation attempts (1 = no jitter ladder) */
-  double update_int8_ops; /* tcgen05 path: int8 multiply-add operations (2 per MAC) issued by the update / K^-1 launches, summed
+  double update_int8_ops; /* Ozaki path: int8 multiply-add operations (2 per MAC) issued by the update / K^-1 launches, summed
                              over the digit pairs actually computed; 0 on the DMMA path */
 } gpx_stats;
 int gpx_get_stats(gpx_ctx* ctx, gpx_stats* out);
 int64_t gpx_total_launches(gpx_ctx* ctx);
-/* Roofline denominator measured on this device: fp64 tensor (DMMA.8x8x4) issue rate in TFLOP/s, CUDA-event timed. */
+/* Roofline denominator measured on this device: fp64 tensor (DMMA.16x8x4) issue rate in TFLOP/s, CUDA-event timed. */
 int gpx_measure_fp64_peak(gpx_ctx* ctx, double* tflops);
 
 /* Tunables (block sizes etc.), mainly for tests: name in {"nb", "lookahead", "profile", "ozaki" (0 = fp64 DMMA only,
- * 1 = trailing update and K^-1 on the tcgen05 int8 path where applicable, -1 = default), "oz_dig_up" (digits per operand
- * for the inverse-part tiles, 4..8), "oz_ctas" (CTAs of the persistent tcgen05 GEMM, 0 = one per SM), "fine" (1 = 64 x 64-tile DMMA kernels inside
- * the diagonal-block chain, 0 = 128 x 128 tiles), "chain" (1 = tcgen05 path: diagonal-block chain alone on the side stream, the
+ * 1 = trailing update and K^-1 on the wgmma int8 path where applicable, -1 = default: env GPX_OZAKI, else 0), "oz_dig_up" (digits per operand
+ * for the inverse-part tiles, 4..8), "oz_ctas" (CTAs of the persistent int8 GEMM, 0 = one per SM), "fine" (1 = 64 x 64-tile DMMA kernels inside
+ * the diagonal-block chain, 0 = 128 x 128 tiles), "chain" (1 = Ozaki path: diagonal-block chain alone on the side stream, the
  * rest of the panel / digit split / forward substitution on a third stream; 0 = round-2 schedule), "base" (generation of the
  * 128 x 128 base-block kernel, process-wide: 0 = default, 1..3)}. */
 int gpx_set_option(gpx_ctx* ctx, const char* name, int64_t value);

@@ -26,16 +26,16 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(L, n), "libgpx.so does not export %s" % n
     assert set(names) == set(_ffi.EXPORTS), "ctypes table and header disagree: %s" % (set(names) ^ set(_ffi.EXPORTS))
-    assert b"sm_100a" in L.gpx_version()
+    assert b"sm_90a" in L.gpx_version()
 
 
-def test_built_for_sm_100a_only():
+def test_built_for_sm_90a_only():
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", _ffi.LIB_PATH], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out.stdout
-    assert not re.search(r"sm_(?!100a)\d+", out.stdout)
+    assert "sm_90a" in out.stdout
+    assert not re.search(r"sm_(?!90a)\d+", out.stdout)
 
 
 def test_no_gpu_fails_loudly(have_gpu):

@@ -34,7 +34,7 @@ def test_non_zero_ranks_of_the_reference_arm_exit_quietly():
 import pytest
 
 
-@pytest.mark.parametrize("name", ["r01_bench_ours_n16384.json", "r02s3_final_bench_ours.json"])
+@pytest.mark.parametrize("name", ["h100_bench_ours_n16384.json"])
 def test_committed_product_line_has_the_contract_keys(name):
     p = os.path.join(ROOT, "profiles", name)
     d = json.loads([l for l in open(p).read().splitlines() if l.startswith("{")][-1])

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 with -m gpu): the CUDA path through the C ABI against the CPU oracle on the same
+"""GPU parity tests (run on the H100 with -m gpu): the CUDA path through the C ABI against the CPU oracle on the same
 seeded inputs. Tolerances are those of BASELINE.json's north star: 1e-8 absolute on the log marginal likelihood,
 1e-6 relative on gradients (fp64 throughout)."""
 import os
@@ -491,7 +491,7 @@ def test_sparse_golden_fixtures():
         np.testing.assert_allclose(g, z["grad"], rtol=1e-6, atol=1e-8, err_msg=fn)
         # dL/dZ is the worst-conditioned output: for the Matern-5/2 fixture cond(Kmm) = 2e8 and the reference's own fp64
         # result differs from an extended-precision evaluation of the same formulas by 7.7e-8 (2e-8 of max|dL/dZ|);
-        # (reproduce: python tools/sparse_dz_extended_precision.py -> profiles/r02_sparse_dz_extended_precision.txt);
+        # (reproduce: python tools/sparse_dz_extended_precision.py);
         # hence the absolute floor relative to the largest entry
         np.testing.assert_allclose(m.Z.gradient, z["Zgrad"], rtol=1e-6, atol=1e-7 * np.abs(z["Zgrad"]).max(), err_msg=fn)
         np.testing.assert_allclose(m.posterior.woodbury_vector, z["woodbury_vector"], rtol=1e-6, atol=1e-7, err_msg=fn)
@@ -595,7 +595,7 @@ def _composite_case(D=5):
 def test_composite_kernels_on_the_fused_device_path(N):
     """Sum / product / White / Bias kernels (add.py:60-99, prod.py:59-68,377-396, static.py:63-185) through
     gpx_exact_eval_multi: LML, every part's gradient, alpha, K and predictions against the oracle; N = 700 / 1300 take the
-    tcgen05 sweep with the stored K^-1, N = 150 the DMMA sweep + plain LAUUM."""
+    int8 (Ozaki) sweep with the stored K^-1, N = 150 the DMMA sweep + plain LAUUM."""
     D = 5
     X, Y = o.synthetic(N, D, seed=N)
     k, parts = _composite_case(D)
@@ -632,7 +632,7 @@ def test_composite_kernels_on_the_fused_device_path(N):
 
 @pytest.mark.parametrize("oz", [0, 1])
 def test_tensor_path_selection_gives_the_same_answer(oz):
-    """option ozaki = 0 (fp64 DMMA GEMMs) and 1 (tcgen05 kind::i8 digit-split GEMMs) both meet the tolerances against the
+    """option ozaki = 0 (fp64 DMMA GEMMs) and 1 (wgmma int8 digit-split GEMMs) both meet the tolerances against the
     oracle, on a size with several panels, a non-multiple-of-block tail and P = 2 outputs."""
     rng = np.random.default_rng(3)
     N, D = 1700, 6

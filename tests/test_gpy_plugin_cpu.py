@@ -11,7 +11,8 @@ import pytest
 
 from oracle import gpy_oracle as o
 
-pytestmark = pytest.mark.skipif(not os.path.isdir("/root/reference/GPy"), reason="reference tree not present")
+pytestmark = pytest.mark.skipif(not os.path.isdir(os.environ.get("GPX_REFERENCE", "/root/reference") + "/GPy"),
+                                reason="reference tree not present")
 
 
 class FakeEngine(object):

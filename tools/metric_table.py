@@ -1,7 +1,7 @@
 """BASELINE.json metric in one run (SURVEY.md §8d): exact-GP log-marginal + gradient evaluations per second, fp64, RBF ARD
-D=8, on one B200 at N in {512, 4096, 16384, 65536} (median of 3 after one warm-up, CUDA-event time) as absolute numbers and
+D=8, on one GPU at N in {512, 4096, 16384, 65536} (median of 3 after one warm-up, CUDA-event time) as absolute numbers and
 as a fraction of the fp64 DMMA roofline (N^3 flops), beside the CPU oracle (GPy's operation sequence) on this host at
-N in {512, 4096} (median of 3 after one warm-up; N=16384 is the cpu_baseline leg of bench.py, 69 s per evaluation;
+N in {512, 4096} (median of 3 after one warm-up; N=16384 is the cpu_baseline leg of bench.py;
 N=65536 needs ~400 GiB of host memory with GPy's temporaries and is not run)."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,5 +1,5 @@
-"""Numerical prototype (CPU, NumPy) for the next-round kernel: the N^3 GEMMs of the factor-and-invert sweep computed by an
-Ozaki split on INT8 tensor cores (tcgen05.mma kind::i8, exact int32 accumulation in TMEM) instead of fp64 DMMA.
+"""Numerical prototype (CPU, NumPy) of the digit-split kernel: the N^3 GEMMs of the factor-and-invert sweep computed by an
+Ozaki split on INT8 tensor cores (wgmma s8 x s8 -> s32, exact int32 accumulation) instead of fp64 DMMA.
 
   * each row of an operand is scaled by a power of two to (-1, 1) and cut into S signed 7-bit digits (int8),
   * C = A B^T = sum_{s+t <= S+1} 2^(e_i + f_j - 7(s+t)) * (D_s^A D_t^B^T), every digit product accumulated EXACTLY

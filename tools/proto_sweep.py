@@ -1,4 +1,4 @@
-"""NumPy prototype of the device algorithm (design validation; mirrors gpy_b200/csrc/gpx_sweep.cu step by step).
+"""NumPy prototype of the device algorithm (design validation; mirrors run_sweep of gpy_b200/csrc/gpx_api.cu step by step).
 
 Unified in-place sweep on one n x n buffer S (column-major on device):
   lower triangle : A -> L      (Cholesky factor)
