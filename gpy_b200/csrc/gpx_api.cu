@@ -170,35 +170,6 @@ int gpx_set_option(gpx_ctx* c, const char* name, int64_t value) {
   }
   if (!strcmp(name, "profile")) { c->profile = (int)value; return 0; }
   if (!strcmp(name, "ozaki")) { c->ozaki = value < 0 ? -1 : (value ? 1 : 0); return 0; }
-  if (!strcmp(name, "oz_dig_up")) {
-    if (value < 4 || value > OZ_S) GPX_FAIL("oz_dig_up must be in [4, 8]");
-    c->oz_dig_up = (int)value;
-    return 0;
-  }
-  if (!strcmp(name, "oz_ctas")) { c->oz_ctas = (int)std::max<int64_t>(0, value); return 0; }
-  if (!strcmp(name, "oz_tpc")) { c->oz_tpc = (int)std::max<int64_t>(0, value); return 0; }
-  if (!strcmp(name, "oz_panel")) { c->oz_panel = (int)std::max<int64_t>(0, std::min<int64_t>(value, 2)); return 0; }   // 2 = at every size
-  if (!strcmp(name, "oz_sched")) { c->oz_sched = value ? 1 : 0; return 0; }
-  if (!strcmp(name, "oz_u0")) { c->oz_u0 = value ? 1 : 0; return 0; }
-  if (!strcmp(name, "oz_reserve")) { c->oz_reserve = (int)std::max<int64_t>(0, std::min<int64_t>(value, 64)); return 0; }
-  if (!strcmp(name, "oz_wide")) {
-    if ((value ? 1 : 0) != c->oz_wide && c->oz_ready) {   // the tile lists are per tile shape: rebuild at the next evaluation
-      GPX_CUDA(cudaSetDevice(c->device));
-      GPX_CUDA(cudaStreamSynchronize(c->st));
-      if (c->oz_tiles) cudaFree(c->oz_tiles);
-      c->oz_tiles = nullptr;
-      c->oz_steps.clear();
-      c->oz_lists_ready = false;
-    }
-    c->oz_wide = value ? 1 : 0;
-    return 0;
-  }
-  if (!strcmp(name, "lookahead")) { c->lookahead = value ? 1 : 0; return 0; }
-  if (!strcmp(name, "base")) { set_base_version((int)std::max<int64_t>(0, std::min<int64_t>(value, 5))); return 0; }
-  if (!strcmp(name, "base_prof")) return set_base_prof((int)value);
-  if (!strcmp(name, "base_pdl")) { set_base_pdl((int)value); return 0; }
-  if (!strcmp(name, "fine")) { c->fine = value ? 1 : 0; return 0; }
-  if (!strcmp(name, "chain")) { c->chain = value ? 1 : 0; return 0; }
   GPX_FAIL("unknown option");
 }
 
@@ -335,42 +306,34 @@ static int oz_prepare(gpx_ctx* c) {
   }
   if (c->oz_lists_ready) return 0;
   std::vector<uint32_t> tiles;
-  oz_build_lists(Npad, NB, c->oz_wide ? 1 : 2, 1, 0, tiles, c->oz_steps);
+  oz_build_lists(Npad, NB, tiles, c->oz_steps);
   GPX_CUDA(cudaMalloc(&c->oz_tiles, tiles.size() * sizeof(uint32_t)));
   GPX_CUDA(cudaMemcpy(c->oz_tiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
   c->oz_lists_ready = true;
   return 0;
 }
 
-// Step k of the sweep (block column k of width nb):
+// The DMMA sweep. Step k (block column k of width nb):
 //   D(k)  inner sweep of the diagonal block (128 columns at a time) + assemble of U_kk / Linv_kk      [side stream]
 //   Pn(k) panel GEMM  P = S(:,block k) Linv_kk^T -> Pbuf[k&1], copied back into S                     [side stream]
 //   U1(k) trailing update restricted to the columns of block k+1                                        [main stream]
 //   U2(k) trailing update of the remaining columns                                                      [main stream]
 // Look-ahead: D(k+1), Pn(k+1) only need U1(k), so they run on the high-priority side stream while U2(k) keeps the
-// machine busy; U1(k+1) waits for Pn(k+1). Without look-ahead everything is issued on the main stream.
-// oz: 0 = DMMA updates; 1 = trailing update on the int8 tensor cores (Ozaki split); 2 = that + K^-1 = U U^T accumulated into c->Kinv
-// panel by panel inside the same launches (the panel's digit planes serve both)
-static int run_sweep_chain(gpx_ctx* c, Recorder& rec);
-
-static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
+// machine busy; U1(k+1) waits for Pn(k+1). A single block is issued on the main stream.
+static int run_sweep(gpx_ctx* c, Recorder& rec) {
   const long ld = c->Npad, Npad = c->Npad;
   const int nt = (int)(Npad / TILE);
   const long NB = pick_nb(c);
-  const bool la = c->lookahead && NB < Npad;
-  if (oz >= 2 && la && c->chain && !c->oz_sched) return run_sweep_chain(c, rec);
+  const bool la = NB < Npad;
   cudaStream_t sm = c->st;
   cudaStream_t ss = la ? c->st2 : c->st;
   size_t evi = 0;
-  cudaEvent_t ev, u1_done = nullptr;
-  bool u1_pending = false;
+  cudaEvent_t ev;
   if (la) {  // side stream starts after everything queued so far on the main stream (K build)
     GPX_CHECK(sync_event(c, evi++, &ev));
     GPX_CUDA(cudaEventRecord(ev, sm));
     GPX_CUDA(cudaStreamWaitEvent(ss, ev, 0));
   }
-  if (oz >= 2)   // forward substitution t = L^-1 y rides along on the side stream (see fw_block_kernel)
-    GPX_CUDA(cudaMemcpyAsync(c->dYres, c->dY, (size_t)c->P * Npad * 8, cudaMemcpyDeviceToDevice, ss));
   int kblk = 0;
   for (long o = 0; o < Npad; o += NB, kblk++) {
     const long nb = std::min(NB, Npad - o);
@@ -380,22 +343,8 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
     // ---- D(k): inner sweep of the nb x nb diagonal block ------------------------------------------------------
     GPX_CHECK(diag_block_sweep(c, Sblk, ld, nbt, kt0, ss));
     if (nbt == nt) break;  // single block: done
-    // Ozaki schedule (option "oz_sched", default): the persistent U2(k-1) leaves a few SMs free, on which the serial
-    // diagonal-block chain D(k) runs meanwhile (side stream); the panel GEMM Pn(k), which needs the whole machine for half a
-    // millisecond, is queued on the MAIN stream behind U2(k-1) instead of fighting it for SM slots.
-    if (u1_pending) {   // (oz_u0) the panel of this step needs ALL of its block column updated, not only the diagonal block
-      GPX_CUDA(cudaStreamWaitEvent(ss, u1_done, 0));
-      u1_pending = false;
-    }
-    const bool sched2 = oz && la && c->oz_sched;
-    cudaStream_t sp = sched2 ? sm : ss;   // stream of assemble / panel / split
-    if (sched2) {
-      GPX_CHECK(sync_event(c, evi++, &ev));
-      GPX_CUDA(cudaEventRecord(ev, ss));
-      GPX_CUDA(cudaStreamWaitEvent(sm, ev, 0));
-    }
     // ---- Pn(k): P = S(:, block) * Linv_kk^T; rows of the diagonal block get U_kk ------------------------------
-    GPX_CHECK(launch_assemble(Sblk, ld, (int)nb, Pb + o, Npad, c->Tm, sp));
+    GPX_CHECK(launch_assemble(Sblk, ld, (int)nb, Pb + o, Npad, c->Tm, ss));
     c->eval_launches++;
     {
       GemmParams pp = gemm_defaults();
@@ -404,85 +353,22 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
       pp.B = c->Tm; pp.ldb = nb;
       pp.C = Pb; pp.ldc = Npad;
       pp.K = (int)nb; pp.nt = nt; pp.skip0 = kt0; pp.skip1 = kt1; pp.tri = 1;
-      GPX_CHECK(launch_gemm(pp, dim3(nbt, nt - nbt), sp));
+      GPX_CHECK(launch_gemm(pp, dim3(nbt, nt - nbt), ss));
       c->eval_launches++;
     }
-    auto copy_back = [&]() -> int {   // the panel rows take their final place in S (U block column above, L panel below)
-      if (o > 0)
-        GPX_CUDA(cudaMemcpy2DAsync(c->S + o * ld, ld * 8, Pb, Npad * 8, (size_t)o * 8, nb, cudaMemcpyDeviceToDevice, ss));
-      if (kt1 < nt)
-        GPX_CUDA(cudaMemcpy2DAsync(c->S + o * ld + (o + nb), ld * 8, Pb + (o + nb), Npad * 8,
-                                   (size_t)(Npad - o - nb) * 8, nb, cudaMemcpyDeviceToDevice, ss));
-      return 0;
-    };
-    // DMMA updates read the panel from Pb, Ozaki updates from the digit planes: either way nothing on the main stream
-    // reads block column k of S, so on the Ozaki path the copy-back leaves the critical chain (after the hand-over)
-    if (!oz) GPX_CHECK(copy_back());
-    if (oz) {   // digit planes + row exponents of this panel (all rows: U block column | U_kk | Cholesky panel)
-      GPX_CHECK(launch_oz_split(Pb, Npad, nb, c->ozp[kblk & 1], sp));
-      c->eval_launches++;
-    }
-    if (sched2) {          // the side stream (copy-back, forward substitution, later D(k+1)) continues after the panel
-      GPX_CHECK(sync_event(c, evi++, &ev));
-      GPX_CUDA(cudaEventRecord(ev, sm));
-      GPX_CUDA(cudaStreamWaitEvent(ss, ev, 0));
-    } else if (la) {
+    // the panel rows take their final place in S (U block column above, L panel below)
+    if (o > 0)
+      GPX_CUDA(cudaMemcpy2DAsync(c->S + o * ld, ld * 8, Pb, Npad * 8, (size_t)o * 8, nb, cudaMemcpyDeviceToDevice, ss));
+    if (kt1 < nt)
+      GPX_CUDA(cudaMemcpy2DAsync(c->S + o * ld + (o + nb), ld * 8, Pb + (o + nb), Npad * 8,
+                                 (size_t)(Npad - o - nb) * 8, nb, cudaMemcpyDeviceToDevice, ss));
+    if (la) {
       GPX_CHECK(sync_event(c, evi++, &ev));
       GPX_CUDA(cudaEventRecord(ev, ss));
       GPX_CUDA(cudaStreamWaitEvent(sm, ev, 0));
     }
-    if (oz) GPX_CHECK(copy_back());
-    if (oz >= 2) {   // after the hand-over to the main stream: overlaps U1(k); the panel buffer is not reused before step k+2
-      GPX_CHECK(launch_fw_block(c->Tm, (int)nb, c->dYres + o, Npad, c->P, c->dTfw + o, ss));
-      GPX_CHECK(launch_fw_panel(Pb + (o + nb), Npad, Npad - o - nb, (int)nb, c->dTfw + o, Npad, c->P, c->dYres + (o + nb), ss));
-      c->eval_launches += 2;
-    }
     // ---- trailing update: S(r,c) -= P_r P_c^T for c >= kt1, r in [0,kt1) U [c,nt), split U1 | U2 ---------------
-    if (oz) {
-      const gpx_ctx::OzStep& os = c->oz_steps[kblk];
-      const OzPlanes& pl = c->ozp[kblk & 1];
-      // U0 (next diagonal block) | U1 (rest of block column k+1) | U2 (everything else + K^-1 tiles). With option oz_u0 = 0
-      // U0 and U1 are one launch (their lists are adjacent).
-      const bool u0 = c->oz_u0 && la && os.u0_n > 0;
-      for (int part = u0 ? -1 : 0; part < 2; part++) {
-        const int off = part < 0 ? os.u0_off : (part == 0 ? (u0 ? os.u1_off : os.u0_off) : os.u2_off);
-        const int ntl = part < 0 ? os.u0_n : (part == 0 ? (u0 ? os.u1_n : os.u0_n + os.u1_n) : (oz >= 2 ? os.u2_n : os.u2_upd));
-        if (ntl > 0) {
-          OzParams op;
-          memset(&op, 0, sizeof(op));
-          op.tiles = c->oz_tiles + off; op.ntiles = ntl; op.nkc = (int)(nb / OZ_KC);
-          op.scale = pl.scale; op.S = c->S; op.lds = ld; op.Kinv = c->Kinv; op.ldk = ld;
-          op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.wide = c->oz_wide;
-          op.tpc = c->oz_ctas > 0 ? (ntl + c->oz_ctas - 1) / c->oz_ctas : c->oz_tpc;
-          if (sched2 && c->oz_ctas <= 0 && c->oz_tpc <= 0) {
-            // persistent: U1 on every SM (nothing else can run before it is done), U2 on all but the reserved SMs
-            const int ctas = std::max(1, c->num_sms - (part == 1 ? c->oz_reserve : 0));   // (part <= 0: every SM)
-            op.tpc = (ntl + ctas - 1) / ctas;
-          }
-          const int tn = c->oz_wide ? 2 * OZ_TN : OZ_TN;
-          const double flops = (double)ntl * 2.0 * OZ_TM * tn * (double)nb;
-          const int nup = part < 0 ? 0 : (part == 0 ? os.u1_up : (oz >= 2 ? os.u2_up : os.u2_upd_up));
-          const int du = c->oz_dig_up;
-          c->stats.update_int8_ops += ((double)nup * (du * (du + 1) / 2) + (double)(ntl - nup) * (OZ_S * (OZ_S + 1) / 2)) * 2.0 *
-                                      OZ_TM * tn * (double)nb;
-          const int h = rec.begin(PH_UPDATE, flops);
-          GPX_CHECK(launch_oz_gemm(pl, op, c->num_sms, sm));
-          rec.end(h);
-          c->eval_launches++;
-          c->stats.update_launches++;
-        }
-        if (la && kt1 < nt && part == (u0 ? -1 : 0)) {   // the next diagonal block is final: D(k+1) may start on the side stream
-          GPX_CHECK(sync_event(c, evi++, &ev));
-          GPX_CUDA(cudaEventRecord(ev, sm));
-          GPX_CUDA(cudaStreamWaitEvent(ss, ev, 0));
-        }
-        if (u0 && part == 0 && kt1 < nt) {               // block column k+1 is final: the panel GEMM of step k+1 may read it
-          GPX_CHECK(sync_event(c, evi++, &u1_done));
-          GPX_CUDA(cudaEventRecord(u1_done, sm));
-          u1_pending = true;
-        }
-      }
-    } else if (kt1 < nt) {
+    if (kt1 < nt) {
       const int next_nbt = (int)(std::min(NB, Npad - (o + nb)) / TILE);
       for (int part = 0; part < 2; part++) {
         const int cbeg = part == 0 ? kt1 : kt1 + next_nbt;
@@ -519,7 +405,8 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
   return 0;
 }
 
-// The Ozaki sweep with the serial chain on its own stream (option "chain", default). Per step k:
+// The Ozaki sweep: trailing update and K^-1 = U U^T (accumulated into c->Kinv panel by panel, the panel's digit planes serve
+// both) on the int8 tensor cores, the serial chain on its own stream. Per step k:
 //   side stream  ss : D(k) -> assemble -> Pc(k): panel rows of block k+1 (fine DMMA tiles) -> U0d(k): diagonal block k+1 -= Pc Pc^T
 //                     (fine DMMA tiles, fp64 operands straight from the panel buffer) -> D(k+1) ...
 //   third stream s3 : Pr(k): the other panel rows -> digit split of the whole panel -> copy-back -> forward substitution
@@ -529,8 +416,8 @@ static int run_sweep(gpx_ctx* c, Recorder& rec, int oz = 0) {
 // panel buffer of step k-1: after the forward-substitution block of step k on s3 (s3 runs in order, so everything of step
 // k-1 there is done as well);  the digit planes of step k are those of step k-2: split(k) is behind Pr(k), which waits for
 // U1(k-1), which is behind U2(k-2) on the main stream.
-// What the next diagonal block waits for is therefore D(k) + two small launches instead of D(k) + full panel + split + a
-// Ozaki launch, and the main stream never waits for a diagonal block unless the trailing update is shorter than D.
+// What the next diagonal block waits for is therefore D(k) + two small launches, and the main stream never waits for a
+// diagonal block unless the trailing update is shorter than D.
 static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
   const long ld = c->Npad, Npad = c->Npad;
   const int nt = (int)(Npad / TILE);
@@ -591,11 +478,11 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
     }
     // ---- s3: Pr(k), split, copy-back, forward substitution --------------------------------------------------------------
     // (from N = 4096 on: five launches instead of one only pay once the panel GEMM is a visible share of the step)
-    const bool oz_pan = c->oz_panel && c->oz_wide && os.pan_n > 0 && (c->oz_panel > 1 || Npad >= 4096);
+    const bool oz_pan = os.pan_n > 0 && Npad >= 4096;
     if (oz_pan) {
       // the panel GEMM itself on the tensor cores: digit planes of block column k of the workspace (A) and of L_kk^-1 (B,
       // lower triangular: per-tile k-range), P = A B^T stored into the panel buffer. 8 digits for the Cholesky rows (they feed
-      // the log-determinant), oz_dig_up for the rows above (finished block column of U: gradients only)
+      // the log-determinant), 7 for the rows above (finished block column of U: gradients only)
       GPX_CHECK(launch_oz_split(c->S + o * ld, ld, nb, c->ozpA, s3));
       GPX_CHECK(launch_oz_split(c->Tm, nb, nb, c->ozpB, s3));
       OzParams op;
@@ -603,8 +490,6 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
       op.tiles = c->oz_tiles + os.pan_off; op.ntiles = os.pan_n; op.nkc = (int)(nb / OZ_KC);
       op.scale = c->ozpA.scale; op.scaleB = c->ozpB.scale; op.P = Pb; op.ldp = Npad; op.Pfinal = c->S + o * ld;
       op.S = c->S; op.lds = ld; op.Kinv = c->Kinv; op.ldk = ld;
-      op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.wide = 1;
-      op.tpc = c->oz_ctas > 0 ? (os.pan_n + c->oz_ctas - 1) / c->oz_ctas : c->oz_tpc;
       GPX_CHECK(launch_oz_gemm(c->ozpA, op, c->num_sms, s3, &c->ozpB));
       c->eval_launches += 5;
     } else if (nt - nbt - next_nbt > 0) {
@@ -646,14 +531,10 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
         memset(&op, 0, sizeof(op));
         op.tiles = c->oz_tiles + off; op.ntiles = ntl; op.nkc = (int)(nb / OZ_KC);
         op.scale = pl.scale; op.S = c->S; op.lds = ld; op.Kinv = c->Kinv; op.ldk = ld;
-        op.dig_lo = OZ_S; op.dig_up = c->oz_dig_up; op.wide = c->oz_wide;
-        op.tpc = c->oz_ctas > 0 ? (ntl + c->oz_ctas - 1) / c->oz_ctas : c->oz_tpc;
-        const int tn = c->oz_wide ? 2 * OZ_TN : OZ_TN;
-        const double flops = (double)ntl * 2.0 * OZ_TM * tn * (double)nb;
+        const double flops = (double)ntl * 2.0 * OZ_TM * OZ_TN * (double)nb;
         const int nup = part == 0 ? os.u1_up : os.u2_up;
-        const int du = c->oz_dig_up;
-        c->stats.update_int8_ops += ((double)nup * (du * (du + 1) / 2) + (double)(ntl - nup) * (OZ_S * (OZ_S + 1) / 2)) * 2.0 *
-                                    OZ_TM * tn * (double)nb;
+        c->stats.update_int8_ops += ((double)nup * (OZ_S_UP * (OZ_S_UP + 1) / 2) + (double)(ntl - nup) * (OZ_S * (OZ_S + 1) / 2)) *
+                                    2.0 * OZ_TM * OZ_TN * (double)nb;
         const int h = rec.begin(PH_UPDATE, flops);
         GPX_CHECK(launch_oz_gemm(pl, op, c->num_sms, sm));
         rec.end(h);
@@ -701,6 +582,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
   const long ld = c->Npad;
   const int nt = (int)(c->Npad / TILE);
   const int nl = c->kp.ard ? c->D : 1;
+  const bool oz = oz_wanted(c);
   GPX_CUDA(cudaMemsetAsync(c->info, 0, sizeof(int), st));
   if (c->multi) {
     if (c->m_cap != c->Npad) {
@@ -739,11 +621,11 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
     kb.diag_vec = c->het ? c->dNoiseVec : nullptr;
     kb.kp = c->kp;
     const int h = rec.begin(PH_KBUILD);
-    // chain schedule: the first block row goes first and is announced by an event, so that the factorisation of the first
+    // Ozaki sweep: the first block row goes first and is announced by an event, so that the factorisation of the first
     // diagonal block runs beside the rest of the covariance build
     const int nbt0 = (int)(pick_nb(c) / TILE);
     c->kfirst_valid = false;
-    if (oz_wanted(c) && c->lookahead && c->chain && !c->oz_sched && nbt0 < nt) {
+    if (oz) {
       GPX_CHECK(launch_kbuild(kb, nbt0, nt, st));
       if (!c->ev_kfirst) GPX_CUDA(cudaEventCreateWithFlags(&c->ev_kfirst, cudaEventDisableTiming));
       GPX_CUDA(cudaEventRecord(c->ev_kfirst, st));
@@ -758,12 +640,11 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
     c->eval_launches++;
   }
   }
-  const bool oz = oz_wanted(c);
   if (oz) GPX_CHECK(oz_prepare(c));
   c->oz_last = oz;
   {
     const int h = rec.begin(PH_SWEEP);
-    GPX_CHECK(run_sweep(c, rec, oz ? 2 : 0));
+    GPX_CHECK(oz ? run_sweep_chain(c, rec) : run_sweep(c, rec));
     rec.end(h);
   }
   {
@@ -824,7 +705,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
     GPX_CHECK(launch_grad_kinv(gk, st));
     rec.end(h);
     c->eval_launches++;
-  } else if (c->fine && nt <= 8 && !c->dist) {
+  } else if (nt <= 8 && !c->dist) {
     // small matrix on the DMMA path (one block, or Ozaki switched off): the fused LAUUM kernel has one CTA per 128 x 128 tile
     // -- 10 CTAs for N = 512, each walking up to 512 k alone (136 us of a 0.48 ms evaluation). K^-1 = U U^T in 64 x 32 tiles
     // (80 CTAs) into the K^-1 buffer, then the gradient pass over the stored tiles, split over the columns

@@ -267,7 +267,7 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
   // Look-ahead (when a second communicator is available): D(k), the broadcast of L_kk^-1, the panel product, the
   // all-gather and the copy-back of step k run on the high-priority side stream (own NCCL communicator) as soon as
   // the columns of block k have received update k-1 (U1); the main stream meanwhile finishes U2(k-1).
-  const bool la = c->lookahead && d->comm2 != nullptr && d->nblk > 1;
+  const bool la = d->comm2 != nullptr && d->nblk > 1;
   cudaStream_t sm = st, ss = la ? c->st2 : st;
   ncclComm_t cs = la ? d->comm2 : d->comm;
   size_t evi = 0;

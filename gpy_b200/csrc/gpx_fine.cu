@@ -6,8 +6,7 @@
 //       strip is in flight at once.
 //   fine_panel_inplace_kernel : the in-place inner panel  S(r, d) <- S(r, d) L_dd^-T  in 16-row strips (a CTA owns a full row
 //       strip, reads it completely into shared memory before it writes), 8 warps x 16 output columns, triangular k-range.
-// Replaces (for the diagonal-block chain only) the 128 x 128-tile launches of gemm_panel_kernel / gemm_update_kernel, i.e. the
-// same share of lapack.dpotrf / dtrtri (GPy/util/linalg.py:58,227) as before.
+// Reference work: the diagonal-block share of lapack.dpotrf / dtrtri (GPy/util/linalg.py:58,227).
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -239,7 +238,7 @@ int fine_init() {
   return 0;
 }
 
-// launched with the programmatic-stream-serialization attribute (option "base_pdl"): behind a kernel that issues
+// p.pdl: launched with the programmatic-stream-serialization attribute: behind a kernel that issues
 // griddepcontrol.launch_dependents (the in-place inner panel, another fine GEMM) the CTAs become resident early and block in
 // griddepcontrol.wait; behind any other kernel or an event wait this is an ordinary launch
 template <int MODE>
@@ -250,7 +249,7 @@ static int launch_fine_pdl(const FineParams& p, unsigned grid, cudaStream_t st) 
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = (p.pdl && get_base_pdl()) ? 1 : 0;
+  cfg.attrs = at; cfg.numAttrs = p.pdl ? 1 : 0;
   GPX_CUDA(cudaLaunchKernelEx(&cfg, gemm_fine_kernel<MODE>, p));
   return 0;
 }
@@ -295,39 +294,18 @@ int diag_block_sweep(gpx_ctx* c, double* Sblk, long ld, int nbt, int g0, cudaStr
                             c->info, g * TILE, st));
     c->eval_launches++;
     if (nbt == 1) break;
-    if (c->fine) {
-      GPX_CHECK_F(launch_fine_panel_inplace(Sblk, ld, c->Dinv + (long)g * TILE * TILE, nbt, d, st));
+    GPX_CHECK_F(launch_fine_panel_inplace(Sblk, ld, c->Dinv + (long)g * TILE * TILE, nbt, d, st));
+    c->eval_launches++;
+    if (d + 1 < nbt) {
+      FineParams pu{};
+      pu.mode = FINE_UPDATE;
+      pu.A = Sblk + (long)d * TILE * ld; pu.lda = ld;
+      pu.B = pu.A; pu.ldb = ld;
+      pu.C = Sblk; pu.ldc = ld;
+      pu.K = TILE; pu.nt = nbt; pu.c0 = d + 1; pu.ncols = nbt - d - 1; pu.rlow = d + 1;
+      pu.pdl = 1;
+      GPX_CHECK_F(launch_fine(pu, st));
       c->eval_launches++;
-      if (d + 1 < nbt) {
-        FineParams pu{};
-        pu.mode = FINE_UPDATE;
-        pu.A = Sblk + (long)d * TILE * ld; pu.lda = ld;
-        pu.B = pu.A; pu.ldb = ld;
-        pu.C = Sblk; pu.ldc = ld;
-        pu.K = TILE; pu.nt = nbt; pu.c0 = d + 1; pu.ncols = nbt - d - 1; pu.rlow = d + 1;
-        pu.pdl = 1;
-        GPX_CHECK_F(launch_fine(pu, st));
-        c->eval_launches++;
-      }
-    } else {   // option "fine" = 0: the 128 x 128-tile kernels (round-1 form)
-      GemmParams pp = gemm_defaults();
-      pp.mode = GEMM_PANEL;
-      pp.A = Sblk + (long)d * TILE * ld; pp.lda = ld;
-      pp.B = c->Dinv + (long)g * TILE * TILE; pp.ldb = TILE;
-      pp.C = Sblk + (long)d * TILE * ld; pp.ldc = ld;      // in place: one k-tile deep, tile-local dependence only
-      pp.K = TILE; pp.nt = nbt; pp.skip0 = d; pp.skip1 = d + 1; pp.tri = 0;
-      GPX_CHECK_F(launch_gemm(pp, dim3(1, nbt - 1), st));
-      c->eval_launches++;
-      if (d + 1 < nbt) {
-        GemmParams pu = gemm_defaults();
-        pu.mode = GEMM_UPDATE;
-        pu.A = Sblk + (long)d * TILE * ld; pu.lda = ld;
-        pu.B = pu.A; pu.ldb = ld;
-        pu.C = Sblk; pu.ldc = ld;
-        pu.K = TILE; pu.nt = nbt; pu.c0 = d + 1; pu.rlow = d + 1;
-        GPX_CHECK_F(launch_gemm(pu, dim3(1, 1), st));
-        c->eval_launches++;
-      }
     }
   }
   return 0;

@@ -1,9 +1,7 @@
 // gpx_kernels.cu — the non-GEMM kernels of the exact-GP path: input scaling, covariance build, the 128x128 base
 // factor-and-invert block, triangular matrix-vector products, block assembly, result extraction, final reduction.
 #include "gpx_common.cuh"
-#include <cstdlib>
 
-#include <cstdio>
 #include <cstring>
 
 #include "gpx_kernels.cuh"
@@ -172,175 +170,20 @@ int launch_kbuild(const KBuildParams& p, int row_tiles, int col_tiles, cudaStrea
 }
 
 // =================================================================================================================
-// base block: unified factor-and-invert sweep of one 128x128 diagonal tile, register resident.
-// 512 threads; lane a owns rows a+32s (s<4), warp b owns columns b+16t (t<8): 32 fp64 values per thread.
-// Column j: the owner warp turns column j of the tile (lower part = A, upper part = inverse region) into the vector
-// p = column / l_jj with p_j = 1/l_jj, publishes it through a double-buffered shared vector (ONE barrier per column),
-// and every thread applies  v(row,col) -= p_row p_col  for col > j and (row >= col or row <= j).
+// base block: unified factor-and-invert sweep of one 128x128 diagonal tile by one CTA of 512 threads, the tile resident
+// in shared memory.
 // On exit: lower = L_dd (to the Ldiag strip), strict upper + reciprocal diagonal = U_dd = L_dd^-T (written back to
 // the tile itself: the diagonal tiles of the workspace hold U), Dinv strip = L_dd^-1 (lower, column-major).
 // Replaces, for one block: lapack.dpotrf (GPy/util/linalg.py:58) and lapack.dtrtri (:227) incl. the
 // "not positive definite" detection that drives jitchol (:59-75).
-// =================================================================================================================
-__global__ void __launch_bounds__(512, 1)
-base_sweep_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, double* __restrict__ Dinv,
-                  double* __restrict__ logdet_part, int* __restrict__ info, int gcol0) {
-  __shared__ double pbuf[2][TILE];
-  __shared__ double ldiag[TILE];
-  const int a = threadIdx.x & 31, b = threadIdx.x >> 5;
-  double v[4][8];
-#pragma unroll
-  for (int t = 0; t < 8; t++)
-#pragma unroll
-    for (int s = 0; s < 4; s++) {
-      const int row = a + 32 * s, col = b + 16 * t;
-      v[s][t] = row >= col ? S[row + (long)col * ld] : 0.0;
-    }
-  // software pipeline: while every warp applies column j, the owner warp of column j+1 first brings its own column
-  // up to date, turns it into p_{j+1} and publishes it -- the serial sqrt/divide chain overlaps the rank-1 update.
-#define GPX_APPLY(T2, J)                                                       \
-  {                                                                            \
-    const int col_ = b + 16 * (T2);                                            \
-    const double pc_ = p[col_];                                                \
-    _Pragma("unroll") for (int s = 0; s < 4; s++) {                            \
-      const int row_ = a + 32 * s;                                             \
-      if (row_ >= col_ || row_ <= (J)) v[s][T2] = fma(-pr[s], pc_, v[s][T2]);  \
-    }                                                                          \
-  }
-#define GPX_MAKE_P(T, J)                                                                   \
-  {                                                                                        \
-    const double d_ = __shfl_sync(0xffffffffu, v[(T) >> 1][T], (J) & 31);                  \
-    if (!(d_ > 0.0) && a == 0) atomicCAS(info, 0, gcol0 + (J) + 1);                        \
-    const double inv_ = rsqrt(d_);      /* one MUFU + Newton steps instead of sqrt + divide on the serial chain */ \
-    const double l_ = d_ * inv_;                                                           \
-    _Pragma("unroll") for (int s = 0; s < 4; s++) {                                        \
-      const int row_ = a + 32 * s;                                                         \
-      const double val_ = (row_ == (J)) ? inv_ : v[s][T] * inv_;                           \
-      pbuf[(J) & 1][row_] = val_;                                                          \
-      v[s][T] = (row_ == (J)) ? l_ : val_;                                                 \
-    }                                                                                      \
-    if (a == ((J) & 31)) ldiag[J] = l_;                                                    \
-  }
-  if (b == 0) GPX_MAKE_P(0, 0);
-  __syncthreads();
-#pragma unroll
-  for (int t = 0; t < 8; t++) {
-    for (int jb = 0; jb < 16; jb++) {
-      const int j = t * 16 + jb;
-      const double* p = pbuf[j & 1];
-      double pr[4];
-#pragma unroll
-      for (int s = 0; s < 4; s++) pr[s] = p[a + 32 * s];
-      if (jb < 15) {
-        if (b == jb + 1) { GPX_APPLY(t, j); GPX_MAKE_P(t, j + 1); }
-      } else if (t < 7) {
-        if (b == 0) { GPX_APPLY(t + 1, j); GPX_MAKE_P(t + 1, j + 1); }
-      }
-#pragma unroll
-      for (int t2 = 0; t2 < 8; t2++) {
-        if (t2 < t) continue;
-        if (t2 == t && b <= jb + 1) continue;              // columns <= j, and column j+1 (done by its owner above)
-        if (t2 == t + 1 && jb == 15 && b == 0) continue;   // column j+1 when it starts the next slot
-        GPX_APPLY(t2, j);
-      }
-      __syncthreads();
-    }
-  }
-#undef GPX_APPLY
-#undef GPX_MAKE_P
-  __syncthreads();
-  // outputs
-#pragma unroll
-  for (int t = 0; t < 8; t++)
-#pragma unroll
-    for (int s = 0; s < 4; s++) {
-      const int row = a + 32 * s, col = b + 16 * t;
-      const double x = v[s][t];
-      if (row > col) {
-        Ldiag[row + col * TILE] = x;          // L_dd strictly lower
-        S[row + (long)col * ld] = 0.0;        // U_dd is upper triangular
-        Dinv[col + row * TILE] = 0.0;         // L_dd^-1 is lower triangular: (col,row) above the diagonal
-      } else if (row == col) {
-        const double inv = 1.0 / x;
-        Ldiag[row + col * TILE] = x;
-        S[row + (long)col * ld] = inv;
-        Dinv[row + col * TILE] = inv;
-      } else {
-        Ldiag[row + col * TILE] = 0.0;
-        S[row + (long)col * ld] = x;          // U_dd(row,col) = (L_dd^-1)(col,row)
-        Dinv[col + row * TILE] = x;
-      }
-    }
-  if (threadIdx.x < 32) {
-    double s = 0.0;
-    for (int j = threadIdx.x; j < TILE; j += 32) s += log(ldiag[j]);
-    s = warp_sum(s);
-    if (threadIdx.x == 0) *logdet_part = 2.0 * s;
-  }
-}
-
-// =================================================================================================================
-// base block, second generation: the same unified factor-and-invert sweep carried one level further down. The 128x128
-// tile lives in shared memory; it is processed in eight 16-column micro-panels:
-//   (1) ONE WARP factor-and-inverts the 16x16 diagonal micro-block in registers (8 values per lane, shuffles only,
-//       rsqrt on the serial chain, no block barrier inside),
-//   (2) all threads form the micro-panel  P = T(:, panel) W^T  (W = inverse of the micro-block) in place,
-//   (3) all 16 warps apply  T(r,c) -= P_r P_c^T  to the 16x16 micro-tiles c > panel, r in [0..panel] U [c..7] with
-//       DMMA.16x8x4 (fragments straight from shared memory, pitch 132 -> conflict-free).
-// Three block barriers per micro-panel instead of one per column: 24 instead of 128, and the rank-16 updates run on
-// the tensor pipe. Same inputs/outputs as base_sweep_kernel.
+// The tile is processed in eight 16-column micro-panels jp:
+//   (1) one warp factor-and-inverts the 16x16 diagonal micro-block in registers (micro_diag_row),
+//   (2) the micro-panel  P = T(:, panel) W^T  (W = inverse of the micro-block) is formed in place with DMMA.16x8x4,
+//   (3) T(r,c) -= P_r P_c^T  for the 16x16 micro-tiles c > jp, r in [0..jp] U [c..7] with DMMA.16x8x4 (fragments straight
+//       from shared memory, pitch 132 -> conflict-free).
 // =================================================================================================================
 constexpr int BP = 132;   // pitch (doubles) of the shared tile, column-major: (row, col) at col*BP + row
 constexpr int MP = 20;    // pitch of the 16x16 micro operand buffers
-
-// (1) one warp: factor-and-invert the 16x16 diagonal micro-block at (c0, c0); values in registers (8 per lane), the
-// pivot column is exchanged through a 2 x 16 shared scratch. Writes the micro-block back (lower = L, strict upper = U),
-// the operand copies Pd = U micro-block ((r,k) at k*MP+r) and Wm = U^T ((c,k) at k*MP+c), and the pivots.
-__device__ __forceinline__ void micro_diag(double* T, int c0, double* Pd, double* Wm, double* psh, double* dinv,
-                                           double* ldg, int* info, int gcol0, int lane) {
-  const int rr = lane & 15, ch = (lane >> 4) * 8;   // lane owns row rr, columns ch..ch+7 of the micro-block
-  double v[8];
-#pragma unroll
-  for (int q = 0; q < 8; q++) v[q] = (rr >= ch + q) ? T[(c0 + ch + q) * BP + c0 + rr] : 0.0;
-  double my_inv = 0.0, my_l = 0.0;
-#pragma unroll
-  for (int j = 0; j < 16; j++) {
-    const int ob = (j >> 3) * 16;                   // first lane of the half-warp that owns column j
-    const double d = __shfl_sync(0xffffffffu, v[j & 7], ob + j);
-    if (!(d > 0.0) && lane == 0) atomicCAS(info, 0, gcol0 + c0 + j + 1);
-    const double inv = rsqrt(d);
-    const double l = d * inv;
-    double* pj = psh + (j & 1) * 16;
-    if ((lane >> 4) == (j >> 3)) {                  // owner half-warp: finalize column j, publish p
-      const double pown = (rr == j) ? inv : v[j & 7] * inv;
-      pj[rr] = pown;
-      v[j & 7] = (rr == j) ? l : pown;
-      if (rr == j) { my_inv = inv; my_l = l; }
-    }
-    __syncwarp();
-    const double prow = pj[rr];
-#pragma unroll
-    for (int q = 0; q < 8; q++) {
-      const int col = ch + q;
-      if (col > j && (rr >= col || rr <= j)) v[q] = fma(-prow, pj[col], v[q]);
-    }
-  }
-  __syncwarp();
-#pragma unroll
-  for (int q = 0; q < 8; q++) {
-    const int col = ch + q;
-    T[(c0 + col) * BP + c0 + rr] = v[q];
-    const double u = rr < col ? v[q] : 0.0;          // U(rr, col) strictly above the diagonal
-    Pd[col * MP + rr] = u;
-    Wm[rr * MP + col] = u;                            // W(col, rr) = U(rr, col); zeros above W's diagonal
-  }
-  __syncwarp();
-  if (rr >= ch && rr < ch + 8) {                      // this lane produced pivot rr
-    dinv[c0 + rr] = my_inv; ldg[c0 + rr] = my_l;
-    Pd[rr * MP + rr] = my_inv;
-    Wm[rr * MP + rr] = my_inv;
-  }
-}
 
 // (3) one 16 x (8*NI) piece of a micro-tile update  T(rt, ct) -= P_rt P_ct^T  (k-depth 16) with DMMA.16x8x4
 template <int NI>
@@ -379,126 +222,8 @@ __device__ __forceinline__ void micro_update(double* T, int c0, int jp, int rt, 
       for (int e = 0; e < 2; e++) Cp[(ni * 8 + 2 * tg + e) * BP + mi * 8 + g] = c[mi][ni][e];
 }
 
-// Schedule per micro-panel jp (look-ahead inside the tile): panel(jp) | update of column block jp+1 by all warps |
-// warp 0 factors micro-block jp+1 WHILE warps 1..15 update the column blocks > jp+1. The serial chain is therefore
-// micro_diag + panel + one column block, the rest of the rank-16 update hides behind the next micro_diag.
-__global__ void __launch_bounds__(512, 1)
-base_sweep16_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, double* __restrict__ Dinv,
-                    double* __restrict__ logdet_part, int* __restrict__ info, int gcol0) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  double* T = reinterpret_cast<double*>(smem_raw);   // [128][BP]
-  double* PdB = T + TILE * BP;                       // 2 x U micro-block of a panel: (r, k) at k*MP + r
-  double* WmB = PdB + 2 * 16 * MP;                   // 2 x W = U^T micro-block (lower): (c, k) at k*MP + c
-  double* psh = WmB + 2 * 16 * MP;                   // 2 x 16 pivot-column scratch of micro_diag
-  double* dinv = psh + 32;                           // [128] reciprocal pivots
-  double* ldg = dinv + TILE;                         // [128] pivots
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int idx = tid; idx < TILE * TILE; idx += 512) {
-    const int row = idx & (TILE - 1), col = idx >> 7;
-    T[col * BP + row] = row >= col ? S[row + (long)col * ld] : 0.0;
-  }
-  __syncthreads();
-  if (warp == 0) micro_diag(T, 0, PdB, WmB, psh, dinv, ldg, info, gcol0, lane);
-  __syncthreads();
-
-  for (int jp = 0; jp < 8; jp++) {
-    const int c0 = jp * 16;
-    double* Pd = PdB + (jp & 1) * 16 * MP;
-    double* Wm = WmB + (jp & 1) * 16 * MP;
-    // ---- (2) micro-panel with DMMA: P(rows, :) = T(rows, panel) W^T for the 7 row blocks outside the micro-block -----
-    if (warp < 7) {
-      const int g = lane >> 2, tg = lane & 3;
-      const int rt = warp < jp ? warp : warp + 1;        // row micro-block, skipping jp
-      double* Ap = T + c0 * BP + rt * 16;
-      double af[2][4], c[2][2][2];
-#pragma unroll
-      for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-        for (int k4 = 0; k4 < 4; k4++) af[mi][k4] = Ap[(k4 * 4 + tg) * BP + mi * 8 + g];
-#pragma unroll
-      for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-        for (int ni = 0; ni < 2; ni++) { c[mi][ni][0] = 0.0; c[mi][ni][1] = 0.0; }
-#pragma unroll
-      for (int k4 = 0; k4 < 4; k4++) {
-        double bf[2];
-#pragma unroll
-        for (int ni = 0; ni < 2; ni++) bf[ni] = Wm[(k4 * 4 + tg) * MP + ni * 8 + g];   // B(n = c, k) = W(c, k)
-#pragma unroll
-        for (int mi = 0; mi < 2; mi += 2)
-#pragma unroll
-          for (int ni = 0; ni < 2; ni++) dmma1684(c[mi][ni][0], c[mi][ni][1], c[mi + 1][ni][0], c[mi + 1][ni][1],
-                                                          af[mi][k4], af[mi + 1][k4], bf[ni]);
-      }
-      __syncwarp();                                       // every lane has read its A fragments: overwrite in place
-#pragma unroll
-      for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-        for (int ni = 0; ni < 2; ni++)
-#pragma unroll
-          for (int e = 0; e < 2; e++) Ap[(ni * 8 + 2 * tg + e) * BP + mi * 8 + g] = c[mi][ni][e];
-    }
-    __syncthreads();
-    if (jp == 7) break;
-    // ---- (3a) column block jp+1 (8 micro-tiles, rows 0..7), two warps per micro-tile ---------------------------------
-    micro_update<1>(T, c0, jp, warp >> 1, jp + 1, (warp & 1) * 8, Pd, lane);
-    __syncthreads();
-    // ---- (1') warp 0: next diagonal micro-block  ||  (3b) warps 1..15: column blocks jp+2..7 -------------------------
-    if (warp == 0) {
-      micro_diag(T, c0 + 16, PdB + ((jp + 1) & 1) * 16 * MP, WmB + ((jp + 1) & 1) * 16 * MP, psh, dinv, ldg, info, gcol0,
-                 lane);
-    } else {
-      int lin = 0;
-      for (int ct = jp + 2; ct < 8; ct++) {
-        const int nslot = jp + 1 + 8 - ct;   // rows [0..jp] and [ct..7]
-        for (int slot = 0; slot < nslot; slot++, lin++) {
-          if (lin % 15 != warp - 1) continue;
-          const int rt = slot <= jp ? slot : ct + slot - (jp + 1);
-          micro_update<2>(T, c0, jp, rt, ct, 0, Pd, lane);
-        }
-      }
-    }
-    __syncthreads();
-  }
-  // ---- outputs ----------------------------------------------------------------------------------------------------
-  for (int idx = tid; idx < TILE * TILE; idx += 512) {
-    const int row = idx & (TILE - 1), col = idx >> 7;
-    const double x = T[col * BP + row];
-    Ldiag[row + col * TILE] = row > col ? x : (row == col ? ldg[row] : 0.0);
-    S[row + (long)col * ld] = row > col ? 0.0 : (row == col ? dinv[row] : x);   // U(row, col) above the diagonal
-  }
-  // Dinv = W = U^T needs T read transposed: lanes take consecutive rows and a column that rotates with lane/4, which
-  // spreads the 32 shared-memory reads over all banks (a plain column walk is a 16-way conflict) while every group of
-  // four lanes still writes one full 32-byte sector of Dinv.
-  for (int blk = warp; blk < 64; blk += 16) {
-    const int row = (blk & 3) * 32 + lane, cbase = (blk >> 2) * 8;
-#pragma unroll
-    for (int it = 0; it < 8; it++) {
-      const int col = cbase + (((lane >> 2) + it) & 7);
-      const double v = row > col ? T[row * BP + col] : (row == col ? dinv[row] : 0.0);   // W(row, col) = U(col, row)
-      Dinv[row + col * TILE] = v;
-    }
-  }
-  if (tid < 32) {
-    double s = 0.0;
-    for (int j = tid; j < TILE; j += 32) s += log(ldg[j]);
-    s = warp_sum(s);
-    if (tid == 0) *logdet_part = 2.0 * s;
-  }
-}
-
-// =================================================================================================================
-// base block, third generation (default). Same algorithm and outputs as base_sweep16_kernel; what changed is the serial part:
-//   * micro_diag_row: lane r of the chain warp holds ROW r of the 16 x 16 micro-block (both half-warps mirror each other), so a
-//     lane scales its own pivot-column entry without any exchange, and the NEXT pivot  d_{j+1} = v(j+1,j+1) - p_{j+1}^2  is
-//     formed locally in lane j+1 before the column is published: the serial chain per column is shuffle -> reciprocal square
-//     root -> multiply -> fused multiply-add, and the publish / read-back of the column through shared memory runs beside it.
-//     The reciprocal square root is MUFU.RSQ64H + one third-order correction (branch-free, ~1 ulp; the library rsqrt has a
-//     special-case branch that splits the basic block the scheduler can interleave).
-//   * the tile comes in by bulk async copies (lower part only, one copy per column, one mbarrier) instead of a load loop;
-//   * a column block is final as soon as its micro-panel is done: warps 1..15 stream it out (Ldiag, U into the workspace tile,
-//     the rows of L^-1) while warp 0 is busy with the next micro-block; only the last column block is written at the end.
-// =================================================================================================================
+// reciprocal square root on the pivot chain: MUFU.RSQ64H + one third-order correction (branch-free, ~1 ulp; the library
+// rsqrt has a special-case branch that splits the basic block the scheduler can interleave)
 __device__ __forceinline__ double rsqrt_fast(double x) {
   double y;
   asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));   // relative error ~2^-22
@@ -507,45 +232,6 @@ __device__ __forceinline__ double rsqrt_fast(double x) {
   const double c = fma(0.375, e, 0.5);
   const double ye = y * e;
   return fma(ye, c, y);                                      // y (1 + e/2 + 3 e^2/8): error O(e^3)
-}
-
-__device__ __forceinline__ void micro_diag_row(double* T, int c0, double* Pd, double* Wm, double* psh, double* dinv,
-                                               double* ldg, int* info, int gcol0, int lane) {
-  const int rr = lane & 15;
-  double v[16];
-#pragma unroll
-  for (int q = 0; q < 16; q++) v[q] = (rr >= q) ? T[(c0 + q) * BP + c0 + rr] : 0.0;
-  double my_inv = 0.0, my_l = 0.0;
-  double d = __shfl_sync(0xffffffffu, v[0], 0);
-#pragma unroll
-  for (int j = 0; j < 16; j++) {
-    if (!(d > 0.0) && lane == 0) atomicCAS(info, 0, gcol0 + c0 + j + 1);
-    const double inv = rsqrt_fast(d);
-    const double l = d * inv;
-    const double p = (rr == j) ? inv : v[j] * inv;
-    if (rr == j) { my_inv = inv; my_l = l; }
-    v[j] = (rr == j) ? l : p;
-    if (j < 15) {                                     // next pivot, formed where it lives (lane j+1 owns row j+1)
-      const double dn = fma(-p, p, v[j + 1]);
-      d = __shfl_sync(0xffffffffu, dn, j + 1);
-    }
-    double* pj = psh + (j & 1) * 16;
-    pj[rr] = p;
-    __syncwarp();
-    const bool up = rr <= j;
-#pragma unroll
-    for (int col = j + 1; col < 16; col++)
-      if (up || rr >= col) v[col] = fma(-p, pj[col], v[col]);
-  }
-  __syncwarp();
-#pragma unroll
-  for (int col = 0; col < 16; col++) {
-    T[(c0 + col) * BP + c0 + rr] = v[col];
-    const double u = rr < col ? v[col] : (rr == col ? my_inv : 0.0);   // U(rr, col), reciprocal pivot on the diagonal
-    Pd[col * MP + rr] = u;
-    Wm[rr * MP + col] = u;                                               // W(col, rr) = U(rr, col)
-  }
-  if (lane < 16) { dinv[c0 + rr] = my_inv; ldg[c0 + rr] = my_l; }
 }
 
 // stream out the finished column block cb (16 columns): Ldiag and U columns, and rows [16cb, 16cb+16) of Dinv = L^-1 = U^T
@@ -565,129 +251,21 @@ __device__ __forceinline__ void base_out_block(const double* T, const double* di
   }
 }
 
-__global__ void __launch_bounds__(512, 1)
-base_sweep3_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, double* __restrict__ Dinv,
-                   double* __restrict__ logdet_part, int* __restrict__ info, int gcol0) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  double* T = reinterpret_cast<double*>(smem_raw);   // [128][BP]
-  double* PdB = T + TILE * BP;
-  double* WmB = PdB + 2 * 16 * MP;
-  double* psh = WmB + 2 * 16 * MP;
-  double* dinv = psh + 32;
-  double* ldg = dinv + TILE;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(ldg + TILE);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) { mbar_init(bar, 1); fence_mbar_init(); }
-  // the inverse region starts from zero; column c is copied from row (c & ~1) down (16-byte granularity of the bulk copy)
-  for (int idx = tid; idx < TILE * TILE; idx += 512) {
-    const int row = idx & (TILE - 1), col = idx >> 7;
-    if (row < (col & ~1)) T[col * BP + row] = 0.0;
-  }
-  __syncthreads();
-  if (tid == 0) mbar_arrive_expect_tx(bar, 8320 * 8);   // sum over columns of (128 - (c & ~1)) doubles
-  __syncthreads();
-  if (tid < TILE) {
-    const int r0 = tid & ~1;
-    bulk_g2s(T + tid * BP + r0, S + r0 + (long)tid * ld, (TILE - r0) * 8, bar);
-  }
-  mbar_wait(bar, 0);
-  if (tid < TILE && (tid & 1)) T[tid * BP + tid - 1] = 0.0;   // the one element above the diagonal that came along
-  __syncthreads();
-  if (warp == 0) micro_diag_row(T, 0, PdB, WmB, psh, dinv, ldg, info, gcol0, lane);
-  __syncthreads();
-
-  for (int jp = 0; jp < 8; jp++) {
-    const int c0 = jp * 16;
-    double* Pd = PdB + (jp & 1) * 16 * MP;
-    double* Wm = WmB + (jp & 1) * 16 * MP;
-    // ---- micro-panel with DMMA: P(rows, :) = T(rows, panel) W^T for the 7 row blocks outside the micro-block -------------
-    if (warp < 7) {
-      const int g = lane >> 2, tg = lane & 3;
-      const int rt = warp < jp ? warp : warp + 1;
-      double* Ap = T + c0 * BP + rt * 16;
-      double af[2][4], c[2][2][2];
-#pragma unroll
-      for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-        for (int k4 = 0; k4 < 4; k4++) af[mi][k4] = Ap[(k4 * 4 + tg) * BP + mi * 8 + g];
-#pragma unroll
-      for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-        for (int ni = 0; ni < 2; ni++) { c[mi][ni][0] = 0.0; c[mi][ni][1] = 0.0; }
-#pragma unroll
-      for (int k4 = 0; k4 < 4; k4++) {
-        double bf[2];
-#pragma unroll
-        for (int ni = 0; ni < 2; ni++) bf[ni] = Wm[(k4 * 4 + tg) * MP + ni * 8 + g];
-#pragma unroll
-        for (int mi = 0; mi < 2; mi += 2)
-#pragma unroll
-          for (int ni = 0; ni < 2; ni++) dmma1684(c[mi][ni][0], c[mi][ni][1], c[mi + 1][ni][0], c[mi + 1][ni][1],
-                                                          af[mi][k4], af[mi + 1][k4], bf[ni]);
-      }
-      __syncwarp();
-#pragma unroll
-      for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-        for (int ni = 0; ni < 2; ni++)
-#pragma unroll
-          for (int e = 0; e < 2; e++) Ap[(ni * 8 + 2 * tg + e) * BP + mi * 8 + g] = c[mi][ni][e];
-    }
-    __syncthreads();
-    if (jp == 7) break;
-    // ---- column block jp+1 (8 micro-tiles, rows 0..7), two warps per micro-tile ------------------------------------------
-    micro_update<1>(T, c0, jp, warp >> 1, jp + 1, (warp & 1) * 8, Pd, lane);
-    __syncthreads();
-    // ---- warp 0: next diagonal micro-block  ||  warps 1..15: column blocks jp+2..7, then column block jp goes out --------
-    if (warp == 0) {
-      micro_diag_row(T, c0 + 16, PdB + ((jp + 1) & 1) * 16 * MP, WmB + ((jp + 1) & 1) * 16 * MP, psh, dinv, ldg, info, gcol0,
-                     lane);
-    } else {
-      int lin = 0;
-      for (int ct = jp + 2; ct < 8; ct++) {
-        const int nslot = jp + 1 + 8 - ct;
-        for (int slot = 0; slot < nslot; slot++, lin++) {
-          if (lin % 15 != warp - 1) continue;
-          const int rt = slot <= jp ? slot : ct + slot - (jp + 1);
-          micro_update<2>(T, c0, jp, rt, ct, 0, Pd, lane);
-        }
-      }
-      base_out_block(T, dinv, ldg, jp, tid - 32, 480, S, ld, Ldiag, Dinv);
-    }
-    __syncthreads();
-  }
-  base_out_block(T, dinv, ldg, 7, tid, 512, S, ld, Ldiag, Dinv);
-  if (tid < 32) {
-    double s = 0.0;
-    for (int j = tid; j < TILE; j += 32) s += log(ldg[j]);
-    s = warp_sum(s);
-    if (tid == 0) *logdet_part = 2.0 * s;
-  }
-}
-
-// =================================================================================================================
-// base block, fourth generation (default): the chain warp RUNS AHEAD of the other fifteen.
-// The serial part of a 128 x 128 factor-and-invert is the chain of the eight 16 x 16 diagonal micro-blocks. In generations 2/3
-// every micro-block waited for two block-wide phases (micro-panel, update of the next column block) with a barrier each. Here
-// warp 0 does, by itself, the only pieces of those phases the next micro-block needs -- P(jp+1, jp) = T(jp+1, jp) W^T and
-// T(jp+1, jp+1) -= P P^T, 32 DMMAs -- and goes straight on to micro-block jp+1, while warps 1..15 do the rest of the
-// micro-panel and of the rank-16 update of step jp and stream the finished column block out. Producer / consumer hand-overs
-// through named barriers (bar.arrive / bar.sync, two of each kind alternating by step parity):
-//   A[jp&1]: warp 0 -> bulk : W(jp), U micro-block and P(jp+1, jp) are in shared memory
-//   D[jp&1]: bulk -> warp 0 : the rank-16 update of step jp is done (warp 0 needs it before it touches row block jp+2)
-//   barrier 7: bulk only, between its micro-panel and its update.
-// micro_diag_row2: the pivot chain per column is multiply -> fused multiply-add -> shuffle -> MUFU.RSQ64H + 4 dependent fp64
-// operations; p_j(j+1), which the next column needs from lane j+1, travels by shuffle, the rest of the column through
-// shared memory (vector loads issued together, off the chain).
-// =================================================================================================================
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void named_arrive(int id, int count) {
   __threadfence_block();
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-__device__ __noinline__ void micro_diag_row2(double* T, int c0, double* Pd, double* Wm, double* psh, double* dinv,
-                                                double* ldg, int* info, int gcol0, int lane) {
+// (1) the chain warp: factor-and-invert the 16x16 diagonal micro-block at (c0, c0). Lane r holds ROW r (both half-warps
+// mirror each other), so a lane scales its own pivot-column entry without any exchange, and the next pivot
+// d_{j+1} = v(j+1,j+1) - p_{j+1}^2 is formed locally in lane j+1: the pivot chain per column is multiply -> fused
+// multiply-add -> shuffle -> MUFU.RSQ64H + 4 dependent fp64 operations. p_j(j+1), which the next column needs from lane j+1,
+// travels by shuffle, the rest of the column through shared memory (vector loads issued together, off the chain). Writes
+// the micro-block back (lower = L, strict upper = U), the operand copies Pd = U micro-block ((r,k) at k*MP+r) and
+// Wm = U^T ((c,k) at k*MP+c), and the pivots.
+__device__ __noinline__ void micro_diag_row(double* T, int c0, double* Pd, double* Wm, double* psh, double* dinv,
+                                            double* ldg, int* info, int gcol0, int lane) {
   const int rr = lane & 15;
   double v[16];
 #pragma unroll
@@ -739,55 +317,6 @@ __device__ __noinline__ void micro_diag_row2(double* T, int c0, double* Pd, doub
   __syncwarp();
 }
 
-// micro_diag_roll: the same column step as micro_diag_row2 as a ROLLED loop. The unrolled form is 16 x ~80 instructions of
-// straight-line code executed once per call: measured in situ (option "base_prof") the first call of a launch took 30 000
-// cycles (instruction fetch from L2 with a cold instruction cache, this is a one-CTA kernel on a fresh SM every time) and the
-// later ones 6 000-7 000 (~400 cycles per column). Here lane r keeps row r of the ACTIVE columns in v[0..15] with the current
-// column always in v[0]: the rank-1 update writes v[k-1] from v[k] (the shift costs nothing), finished columns go straight to
-// shared memory, so every column runs the same ~2 KB of code. The reciprocal square root of the NEXT pivot is started before
-// the update of the current column, in the same basic block, so that the scheduler interleaves the two.
-__device__ __forceinline__ void micro_diag_roll(double* T, int c0, double* Pd, double* Wm, double* psh, double* dinv,
-                                                double* ldg, int* info, int gcol0, int lane) {
-  const int rr = lane & 15;
-  double v[16];
-#pragma unroll
-  for (int q = 0; q < 16; q++) v[q] = (rr >= q) ? T[(c0 + q) * BP + c0 + rr] : 0.0;
-  int badcol = -1;
-  double d = __shfl_sync(0xffffffffu, v[0], 0);
-  double inv = rsqrt_fast(d);
-#pragma unroll 1
-  for (int j = 0; j < 16; j++) {
-    if (!(d > 0.0) && badcol < 0) badcol = j;
-    const double l = d * inv;
-    const bool diag = rr == j;
-    const double p = diag ? inv : v[0] * inv;
-    const double dn = fma(-p, p, v[1]);                       // lane j+1: the next pivot, from its own data only
-    const double dnext = __shfl_sync(0xffffffffu, dn, (j + 1) & 15);
-    const double inv_next = rsqrt_fast(dnext);                // (j = 15: unused)
-    double* pj = psh + (j & 1) * 32;                          // [0..15] = p_j, [16..31] = 0
-    pj[rr] = p;
-    if (lane < 16) {
-      T[(c0 + j) * BP + c0 + rr] = diag ? l : p;
-      const double u = rr < j ? p : (diag ? inv : 0.0);       // U(rr, j), reciprocal pivot on the diagonal
-      Pd[j * MP + rr] = u;
-      Wm[rr * MP + j] = u;                                    // W(j, rr) = U(rr, j)
-      if (diag) { dinv[c0 + j] = inv; ldg[c0 + j] = l; }
-    }
-    __syncwarp();
-    const bool up = rr <= j;
-    const double* pc = pj + j;                                // pc[k] = p_j(j + k)
-#pragma unroll
-    for (int k = 1; k < 16; k++) {
-      const double t = fma(-p, pc[k], v[k]);
-      v[k - 1] = (up || rr >= j + k) ? t : v[k];
-    }
-    v[15] = 0.0;
-    d = dnext; inv = inv_next;
-  }
-  if (badcol >= 0 && lane == 0) atomicCAS(info, 0, gcol0 + c0 + badcol + 1);
-  __syncwarp();
-}
-
 // one row block of the micro-panel: T(rt, panel jp) <- T(rt, panel jp) W^T (in place), one warp
 __device__ __forceinline__ void micro_panel_rows(double* T, int c0, int rt, const double* Wm, int lane) {
   const int g = lane >> 2, tg = lane & 3;
@@ -822,10 +351,18 @@ __device__ __forceinline__ void micro_panel_rows(double* T, int c0, int rt, cons
   __syncwarp();
 }
 
-template <bool ROLL>
+// The serial part of the tile is the chain of its eight diagonal micro-blocks, so the chain warp (warp 0) RUNS AHEAD of the
+// other fifteen: it does by itself the only pieces of (2) and (3) the next micro-block needs -- P(jp+1, jp) = T(jp+1, jp) W^T
+// and T(jp+1, jp+1) -= P P^T, 32 DMMAs -- and goes straight on to micro-block jp+1, while warps 1..15 do the rest of the
+// micro-panel and of the rank-16 update of step jp and stream the finished column block out (Ldiag, U into the workspace
+// tile, the rows of L^-1). Producer / consumer hand-overs through named barriers (bar.arrive / bar.sync, two of each kind
+// alternating by step parity):
+//   A[jp&1]: warp 0 -> bulk : W(jp), U micro-block and P(jp+1, jp) are in shared memory
+//   D[jp&1]: bulk -> warp 0 : the rank-16 update of step jp is done (warp 0 needs it before it touches row block jp+2)
+//   barrier 7: bulk only, between its micro-panel and its update.
 __global__ void __launch_bounds__(512, 1)
 base_sweep4_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, double* __restrict__ Dinv,
-                   double* __restrict__ logdet_part, int* __restrict__ info, int gcol0, long long* __restrict__ prof, int warm) {
+                   double* __restrict__ logdet_part, int* __restrict__ info, int gcol0) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   double* T = reinterpret_cast<double*>(smem_raw);   // [128][BP]
   double* PdB = T + TILE * BP;
@@ -835,24 +372,19 @@ base_sweep4_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, 
   double* ldg = dinv + TILE;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int BAR_A = 1, BAR_D = 3, BAR_BULK = 7;
-  // measurement (option "base_prof"): SM clock at the phase boundaries of the chain warp, slots 0..; see gpx_set_option
-#define GPX_STAMP(i) do { if (prof && tid == 0) prof[i] = clock64(); } while (0)
-  GPX_STAMP(0);
   if (tid < 64) psh[tid] = 0.0;
-  // Launched as a programmatic dependent of the kernel before it (warm != 0): this CTA is resident while that kernel still
-  // runs. The time is used to pull the chain warp's code into the instruction cache: one column sweep on an identity block
-  // in the (still unused) tile buffer -- measured in situ, the first micro-block of a launch costs 25 000-30 000 cycles against
-  // 6 500 for the later ones. griddepcontrol.wait then blocks until the preceding kernel has completed and flushed.
-  if (warm) {
-    if (warp == 0) {
-      for (int q = lane; q < 16 * 16; q += 32) T[(q >> 4) * BP + (q & 15)] = (q >> 4) == (q & 15) ? 1.0 : 0.0;
-      __syncwarp();
-      if (ROLL) micro_diag_roll(T, 0, PdB, WmB, psh, dinv, ldg, info, gcol0, lane);
-      else micro_diag_row2(T, 0, PdB, WmB, psh, dinv, ldg, info, gcol0, lane);
-    }
-    __syncthreads();
-    if (tid < 64) psh[tid] = 0.0;
+  // Launched as a programmatic dependent of the kernel before it: this CTA is resident while that kernel still runs. The
+  // time is used to pull the chain warp's code into the instruction cache: one column sweep on an identity block in the
+  // (still unused) tile buffer -- measured in situ, the first micro-block of a launch costs 25 000-30 000 cycles against
+  // 6 500 for the later ones (cold instruction cache: a one-CTA kernel lands on a fresh SM). griddepcontrol.wait then blocks
+  // until the preceding kernel has completed and flushed.
+  if (warp == 0) {
+    for (int q = lane; q < 16 * 16; q += 32) T[(q >> 4) * BP + (q & 15)] = (q >> 4) == (q & 15) ? 1.0 : 0.0;
+    __syncwarp();
+    micro_diag_row(T, 0, PdB, WmB, psh, dinv, ldg, info, gcol0, lane);
   }
+  __syncthreads();
+  if (tid < 64) psh[tid] = 0.0;
   asm volatile("griddepcontrol.wait;" ::: "memory");
   // lower part of the tile -> shared memory, zeros above the diagonal (the inverse region starts from zero); 16-byte pieces
 #pragma unroll 8
@@ -864,7 +396,6 @@ base_sweep4_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, 
     *reinterpret_cast<double2*>(T + col * BP + row) = v;
   }
   __syncthreads();
-  GPX_STAMP(1);
   if (warp == 0) {
     // ================= chain warp ======================================================================================
     for (int jp = 0; jp < 8; jp++) {
@@ -872,16 +403,11 @@ base_sweep4_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, 
       if (jp > 0) {
         micro_update<2>(T, c0 - 16, jp - 1, jp, jp, 0, PdB + ((jp - 1) & 1) * 16 * MP, lane);   // T(jp, jp) -= P(jp, jp-1) P(jp, jp-1)^T
         __syncwarp();
-        GPX_STAMP(1 + 4 * jp);
       }
-      if (ROLL) micro_diag_roll(T, c0, PdB + (jp & 1) * 16 * MP, WmB + (jp & 1) * 16 * MP, psh, dinv, ldg, info, gcol0, lane);
-      else micro_diag_row2(T, c0, PdB + (jp & 1) * 16 * MP, WmB + (jp & 1) * 16 * MP, psh, dinv, ldg, info, gcol0, lane);
-      GPX_STAMP(2 + 4 * jp);
+      micro_diag_row(T, c0, PdB + (jp & 1) * 16 * MP, WmB + (jp & 1) * 16 * MP, psh, dinv, ldg, info, gcol0, lane);
       if (jp > 0) named_sync(BAR_D + ((jp - 1) & 1), 512);               // update of step jp-1 done: row block jp+1 is current
-      GPX_STAMP(3 + 4 * jp);
       if (jp < 7) micro_panel_rows(T, c0, jp + 1, WmB + (jp & 1) * 16 * MP, lane);
       named_arrive(BAR_A + (jp & 1), 512);
-      GPX_STAMP(4 + 4 * jp);
     }
   } else {
     // ================= bulk warps 1..15 =================================================================================
@@ -919,7 +445,6 @@ base_sweep4_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, 
     }
   }
   __syncthreads();
-  GPX_STAMP(40);
   base_out_block(T, dinv, ldg, 7, tid, 512, S, ld, Ldiag, Dinv);
   if (tid < 32) {
     double s = 0.0;
@@ -927,77 +452,27 @@ base_sweep4_kernel(double* __restrict__ S, long ld, double* __restrict__ Ldiag, 
     s = warp_sum(s);
     if (tid == 0) *logdet_part = 2.0 * s;
   }
-  GPX_STAMP(41);
-#undef GPX_STAMP
-}
-
-static int g_base_version = 0;   // option "base" (process-wide): 0 = default / environment
-void set_base_version(int v) { g_base_version = v; }
-// option "base_prof": 1 = the fourth-generation base kernel stamps clock64() at its phase boundaries into a device buffer (the
-// last launch wins); 2 = print them (cycles since the kernel's start) to stderr. Measurement only.
-static int g_base_pdl = 1;        // option "base_pdl"
-void set_base_pdl(int v) { g_base_pdl = v ? 1 : 0; }
-int get_base_pdl() { return g_base_pdl; }
-static long long* g_base_prof = nullptr;
-static bool g_base_prof_on = false;
-int set_base_prof(int v) {
-  if (v == 1) {
-    if (!g_base_prof) { GPX_CUDA(cudaMalloc(&g_base_prof, 64 * sizeof(long long))); GPX_CUDA(cudaMemset(g_base_prof, 0, 64 * sizeof(long long))); }
-    g_base_prof_on = true;
-  } else if (v == 2 && g_base_prof) {
-    long long h[64];
-    GPX_CUDA(cudaDeviceSynchronize());
-    GPX_CUDA(cudaMemcpy(h, g_base_prof, sizeof(h), cudaMemcpyDeviceToHost));
-    fprintf(stderr, "base_sweep4 phases (SM cycles since kernel start): prologue + load %lld |", h[1] - h[0]);
-    for (int jp = 0; jp < 8; jp++) {
-      const long long t0 = jp ? h[4 * jp] : h[1];
-      if (jp) fprintf(stderr, " [jp %d: update-piece %lld micro-block %lld", jp, h[1 + 4 * jp] - t0, h[2 + 4 * jp] - h[1 + 4 * jp]);
-      else fprintf(stderr, " [jp 0: micro-block %lld", h[2] - t0);
-      fprintf(stderr, " wait %lld panel-piece %lld]", h[3 + 4 * jp] - h[2 + 4 * jp], h[4 + 4 * jp] - h[3 + 4 * jp]);
-    }
-    fprintf(stderr, " | join %lld | last column block + logdet %lld | total %lld\n", h[40] - h[32], h[41] - h[40], h[41] - h[0]);
-  } else {
-    g_base_prof_on = false;
-  }
-  return 0;
 }
 
 int launch_base(double* S, long ld, double* Ldiag, double* Dinv, double* logdet_part, int* info, int gcol0,
                 cudaStream_t st) {
   static bool ready = false;
-  constexpr int smem16 = (TILE * BP + 4 * 16 * MP + 64 + 2 * TILE) * 8 + 16;
-  int which = g_base_version;
-  if (which <= 0) {
-    const char* e = getenv("GPX_BASE");          // 4 (default) = chain warp runs ahead, 5 = that with the rolled column loop (slower:
-    which = e ? atoi(e) : (getenv("GPX_BASE_V1") ? 1 : 4);   // ~600 instead of ~400 cycles per column), 3 = row-per-lane chain warp with
-    if (which < 1 || which > 5) which = 4;                   // block barriers, 2 = round-2 kernel, 1 = round-1 kernel
-  }
+  constexpr int smem = (TILE * BP + 4 * 16 * MP + 64 + 2 * TILE) * 8 + 16;
   if (!ready) {
     ready = true;
-    GPX_CUDA(cudaFuncSetAttribute(base_sweep16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16));
-    GPX_CUDA(cudaFuncSetAttribute(base_sweep3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16));
-    GPX_CUDA(cudaFuncSetAttribute(base_sweep4_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16));
-    GPX_CUDA(cudaFuncSetAttribute(base_sweep4_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16));
+    GPX_CUDA(cudaFuncSetAttribute(base_sweep4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   }
-  if (which == 1) base_sweep_kernel<<<1, 512, 0, st>>>(S, ld, Ldiag, Dinv, logdet_part, info, gcol0);
-  else if (which == 2) base_sweep16_kernel<<<1, 512, smem16, st>>>(S, ld, Ldiag, Dinv, logdet_part, info, gcol0);
-  else if (which == 3) base_sweep3_kernel<<<1, 512, smem16, st>>>(S, ld, Ldiag, Dinv, logdet_part, info, gcol0);
-  else {
-    // programmatic dependent launch (option "base_pdl", default on): the CTA becomes resident as soon as every CTA of the kernel
-    // before it in the stream has started (the fine GEMM issues griddepcontrol.launch_dependents first thing) and warms its
-    // instruction cache until that kernel is done; after any other kernel the launch behaves like a plain one
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(1); cfg.blockDim = dim3(512); cfg.dynamicSmemBytes = smem16; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = g_base_pdl ? 1 : 0;
-    long long* pr = g_base_prof_on ? g_base_prof : nullptr;
-    const int warm = g_base_pdl ? 1 : 0;
-    if (which == 5) GPX_CUDA(cudaLaunchKernelEx(&cfg, base_sweep4_kernel<true>, S, ld, Ldiag, Dinv, logdet_part, info, gcol0, pr, warm));
-    else GPX_CUDA(cudaLaunchKernelEx(&cfg, base_sweep4_kernel<false>, S, ld, Ldiag, Dinv, logdet_part, info, gcol0, pr, warm));
-  }
+  // programmatic dependent launch: the CTA becomes resident as soon as every CTA of the kernel before it in the stream has
+  // started (the fine GEMM issues griddepcontrol.launch_dependents first thing) and warms its instruction cache until that
+  // kernel is done; after any other kernel the launch behaves like a plain one
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(1); cfg.blockDim = dim3(512); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  GPX_CUDA(cudaLaunchKernelEx(&cfg, base_sweep4_kernel, S, ld, Ldiag, Dinv, logdet_part, info, gcol0));
   GPX_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1660,6 +1135,164 @@ int launch_grad_full(const GradFullParams& p, int tiles_j, int tiles_i, cudaStre
   if (D <= 16) return launch_grad_full_t<16>(p, grid, smem, st);
   if (D <= 32) return launch_grad_full_t<32>(p, grid, smem, st);
   return launch_grad_full_t<64>(p, grid, smem, st);
+}
+
+// =================================================================================================================
+// gradient reductions from the stored K^-1 (same sums as the fused LAUUM epilogue of gpx_gemm.cu):
+//    dL_dK = 1/2 (alpha alpha^T - P K^-1)  (exact_gaussian_inference.py:70), tr -> noise (:72, gaussian.py:78-79),
+//    sum K o dL_dK / variance (stationary.py:199), ARD / iso lengthscale sums (:202-213, 225-243). One CTA per lower
+//    128 x 128 tile; the thread-mapped index is the ROW (contiguous in the column-major K^-1), 64 columns per thread.
+// =================================================================================================================
+template <int DREG>
+__global__ void __launch_bounds__(256) grad_kinv_kernel(GradKinvParams p) {
+  extern __shared__ __align__(128) unsigned char gk_smem[];
+  const int D = p.kp.D, P = p.P;
+  double* sXc = reinterpret_cast<double*>(gk_smem);   // [D][128] column points
+  double* sSc = sXc + (size_t)D * TILE;               // [128]
+  double* sAc = sSc + TILE;                           // [P][128]
+  double* sRed = sAc + (size_t)P * TILE;              // [8 warps][nred]
+  // lower tiles only: blockIdx.x enumerates (r, c), c <= r
+  const int csplit = p.csplit, tileidx = (int)blockIdx.x / csplit, sidx = (int)blockIdx.x % csplit;
+  int r = (int)((sqrtf(8.f * (float)tileidx + 1.f) - 1.f) * 0.5f);
+  while (r * (r + 1) / 2 > tileidx) --r;
+  while ((r + 1) * (r + 2) / 2 <= tileidx) ++r;
+  const int c = tileidx - r * (r + 1) / 2;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  for (int idx = tid; idx < D * TILE; idx += 256) sXc[idx] = p.XsT[(long)(idx / TILE) * p.ldx + (long)c * TILE + idx % TILE];
+  for (int idx = tid; idx < P * TILE; idx += 256) sAc[idx] = p.alpha[(long)(idx / TILE) * p.ldx + (long)c * TILE + idx % TILE];
+  if (tid < TILE) sSc[tid] = p.sq[(long)c * TILE + tid];
+  __syncthreads();
+  const int il = tid & (TILE - 1), half = tid >> 7;
+  const long gi = (long)r * TILE + il;
+  const bool ard = p.kp.ard != 0;
+  const int nl = ard ? D : 1, nred = nl + 2;
+  double xi[DREG], gq[DREG], ai[MAX_P];
+#pragma unroll
+  for (int q = 0; q < DREG; q++) { gq[q] = 0.0; xi[q] = q < D ? p.XsT[(long)q * p.ldx + gi] : 0.0; }
+#pragma unroll
+  for (int q = 0; q < MAX_P; q++) ai[q] = q < P ? p.alpha[(long)q * p.ldx + gi] : 0.0;
+  const double si = p.sq[gi];
+  const double w = (r > c) ? 2.0 : 1.0;               // strictly-lower tiles stand for their mirror image as well
+  const double variance = p.kp.variance, inv_ls = p.kp.inv_ls_iso;
+  const int kind = p.kp.kind;
+  double gvar = 0.0, giso = 0.0, gnoise = 0.0;
+  const double* kcol = p.Kinv + gi + ((long)c * TILE + half * 64) * p.ld;
+  if (gi < p.N) {
+    const int jj_beg = sidx * (64 / csplit);
+    const int jj_end = (int)min((long)(jj_beg + 64 / csplit), p.N - (long)c * TILE - half * 64);   // columns beyond N are padding
+    // two columns in flight per thread: one column is a single dependent chain (dot product -> exp -> reductions) and the
+    // 16 warps an SM holds at 92 registers leave the fp64 pipe mostly idle (1.8 ms for the 134 M elements of N = 16384)
+#pragma unroll 2
+    for (int jj = jj_beg; jj < jj_end; jj++) {
+      const int jl = half * 64 + jj;
+      const long gj = (long)c * TILE + jl;
+      const double kinv = kcol[(long)jj * p.ld];
+      double dot = 0.0;
+#pragma unroll
+      for (int q = 0; q < DREG; q++)
+        if (q < D) dot = fma(xi[q], sXc[q * TILE + jl], dot);
+      double r2 = si + sSc[jl] - 2.0 * dot;
+      if (gi == gj) r2 = 0.0;
+      r2 = fmax(r2, 0.0);
+      double aa = 0.0;
+#pragma unroll
+      for (int q = 0; q < MAX_P; q++)
+        if (q < P) aa = fma(ai[q], sAc[q * TILE + jl], aa);
+      const double dl = 0.5 * (aa - (double)P * kinv);
+      if (gi == gj) {
+        gnoise += dl;
+        if (p.dnoise_out) p.dnoise_out[gi] = dl;
+      }
+      if (kind == GPX_RBF) {
+        // dK/dr / r = -K for the RBF kernel (rbf.py:177-178 over stationary.py:205): neither the square root nor the division
+        // of the general form is needed; at r = 0 the reference's 1/0 := 0 multiplies (x_i - x_j)^2 = 0 either way
+        const double r2s = r2 * (inv_ls * inv_ls);
+        const double k = exp(-0.5 * r2s);
+        const double kd = w * k * dl;
+        gvar += kd;
+        const double tmpv = -variance * kd;
+        if (ard) {
+#pragma unroll
+          for (int q = 0; q < DREG; q++)
+            if (q < D) {
+              const double df = xi[q] - sXc[q * TILE + jl];
+              gq[q] = fma(tmpv, df * df, gq[q]);
+            }
+        } else {
+          giso = fma(tmpv, r2s, giso);
+        }
+        continue;
+      }
+      const double rr = sqrt(r2) * inv_ls;
+      double k, dk;
+      k_dk_of_r_unit(kind, rr, k, dk);
+      gvar = fma(w * k, dl, gvar);
+      const double G = variance * dk * dl;
+      if (ard) {
+        const double tmpv = (rr != 0.0) ? w * G / rr : 0.0;     // stationary.py:205,225-232: 1/r with 1/0 := 0
+#pragma unroll
+        for (int q = 0; q < DREG; q++)
+          if (q < D) {
+            const double df = xi[q] - sXc[q * TILE + jl];
+            gq[q] = fma(tmpv, df * df, gq[q]);
+          }
+      } else {
+        giso = fma(w * G, rr, giso);
+      }
+    }
+  }
+  gvar = warp_sum(gvar);
+  gnoise = warp_sum(gnoise);
+  if (lane == 0) { sRed[warp * nred] = gvar; sRed[warp * nred + nred - 1] = gnoise; }
+  if (ard) {
+#pragma unroll
+    for (int q = 0; q < DREG; q++)
+      if (q < D) {
+        const double s = warp_sum(gq[q]);
+        if (lane == 0) sRed[warp * nred + 1 + q] = s;
+      }
+  } else {
+    giso = warp_sum(giso);
+    if (lane == 0) sRed[warp * nred + 1] = giso;
+  }
+  __syncthreads();
+  if (tid < nred) {
+    double s = 0.0;
+#pragma unroll
+    for (int wdx = 0; wdx < 8; wdx++) s += sRed[wdx * nred + tid];
+    p.partials[(((long)r * p.nt + c) * csplit + sidx) * nred + tid] = s;
+  }
+}
+
+int grad_kinv_csplit(int nt, int nred) {
+  const int tiles = nt * (nt + 1) / 2;
+  int cs = 1;
+  while (cs < 8 && tiles * cs < 528 && (cs * 2) * nred <= MAX_D + 2) cs *= 2;   // ~4 waves of CTAs on 132 SMs; partials sized for MAX_D + 2 per tile
+  return cs;
+}
+
+template <int DREG>
+static int launch_grad_kinv_t(const GradKinvParams& p, unsigned grid, size_t smem, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    GPX_CUDA(cudaFuncSetAttribute(grad_kinv_kernel<DREG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)((MAX_D + 1 + MAX_P) * TILE * 8 + 8 * (MAX_D + 2) * 8)));
+    attr_set = true;
+  }
+  grad_kinv_kernel<DREG><<<grid, 256, smem, st>>>(p);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int launch_grad_kinv(const GradKinvParams& p, cudaStream_t st) {
+  const int D = p.kp.D;
+  const size_t smem = (size_t)(D + 1 + p.P) * TILE * 8 + 8 * (MAX_D + 2) * 8;
+  if (p.csplit != 1 && p.csplit != 2 && p.csplit != 4 && p.csplit != 8) { set_error("grad_kinv: csplit must be 1, 2, 4 or 8"); return -2; }
+  const unsigned grid = (unsigned)(p.nt * (p.nt + 1) / 2 * p.csplit);
+  if (D <= 8) return launch_grad_kinv_t<8>(p, grid, smem, st);
+  if (D <= 16) return launch_grad_kinv_t<16>(p, grid, smem, st);
+  if (D <= 32) return launch_grad_kinv_t<32>(p, grid, smem, st);
+  return launch_grad_kinv_t<64>(p, grid, smem, st);
 }
 
 

@@ -45,10 +45,6 @@ int launch_prep_x(const double* X, long N, long ldx, const KernParams& kp, doubl
 int launch_kbuild(const KBuildParams& p, int row_tiles, int col_tiles, cudaStream_t st);
 int launch_base(double* S, long ld, double* Ldiag, double* Dinv, double* logdet_part, int* info, int gcol0,
                 cudaStream_t st);
-void set_base_version(int v);   // 0 = default (3), 1..3 = generation of the base-block kernel (measurement / regression)
-int get_base_pdl();
-void set_base_pdl(int v);      // 1 (default) = base kernel launched as a programmatic dependent with an instruction-cache warm-up
-int set_base_prof(int v);       // measurement: phase clocks of the base-block kernel (option "base_prof")
 int launch_assemble(const double* Sblk, long ld, int nb, double* Prows, long ldp, double* Tm, cudaStream_t st);
 int launch_fw_block(const double* Tm, int nb, const double* yres, long ld, int P, double* t, cudaStream_t st);
 int launch_fw_panel(const double* Pb, long ldp, long rows, int nb, const double* t, long ld, int P, double* yres,
@@ -78,5 +74,20 @@ int launch_row_dot(const double* A, long lda, long rows_pad, long ncols, int P, 
 int launch_load_sym(const double* A, long lda, long N, double* S, long ld, double jitter, cudaStream_t st);
 int measure_dmma_peak(cudaStream_t st, double* tflops);
 int launch_grad_full(const GradFullParams& p, int tiles_j, int tiles_i, cudaStream_t st);
+
+// gradient reductions from a stored K^-1 (lower 128 x 128 tiles, column-major, leading dimension ld): same partial sums as
+// the fused epilogue of gemm_lauum_kernel, consumed by finalize_kernel
+struct GradKinvParams {
+  const double* Kinv; long ld;
+  const double* XsT; const double* sq; const double* alpha; long ldx;
+  long N; int P; int nt;
+  double* partials;        // [nt*nt*csplit][nl+2], zeroed by the caller
+  int csplit;              // CTAs per tile (each takes 64/csplit columns of both column halves): 1, 2, 4 or 8 -- small matrices
+                           // have too few tiles to fill the machine, and a thread's 64 columns are a serial chain
+  double* dnoise_out;      // optional diag(dL_dK)
+  KernParams kp;
+};
+int launch_grad_kinv(const GradKinvParams& p, cudaStream_t st);
+int grad_kinv_csplit(int nt, int nred);   // the split launch_grad_kinv expects for this matrix (partials: nt*nt*(MAX_D+2) doubles)
 
 }  // namespace gpx

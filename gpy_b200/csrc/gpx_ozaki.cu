@@ -15,7 +15,7 @@
 // Eight exponent groups of a 64 x 64 accumulator are 256 s32 registers per thread, more than a thread has, so the two
 // consumer warpgroups compute the SAME 64 x 64 sub-tile and split the groups between them (four each, 128 registers):
 // warpgroup 0 takes the groups g with g % 4 in {0, 3}, warpgroup 1 those with g % 4 in {1, 2} (18 of the 36 digit pairs each).
-// A 128 x 64 (or 128 x 128) output tile of the list is walked as 2 (or 4) such sub-tiles.
+// A 128 x 128 output tile of the list is walked as 4 such sub-tiles.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -32,6 +32,7 @@
 namespace gpx {
 
 constexpr int OZ_SUB = 64;                                        // sub-tile edge (wgmma M = N = 64)
+constexpr int OZ_NSUB = (OZ_TM / OZ_SUB) * (OZ_TN / OZ_SUB);      // sub-tiles per output tile (bit 0: row half, bit 1: column half)
 constexpr int OZ_STAGES = 5;
 constexpr int OZ_PLANE = OZ_SUB * OZ_KC;                          // 2048: one digit plane of a 64-row sub-tile, one k-chunk
 constexpr int OZ_STAGE_BYTES = 2 * OZ_S * OZ_PLANE;               // 32768: up to 8 A planes + 8 B planes
@@ -193,7 +194,7 @@ __host__ __device__ constexpr int oz_group(int w, int j) {
 }
 // k-chunks of a tile: the whole panel width, except OZ_PANEL tiles (triangular B: columns of tile c' see k < (c' + 1) * 128)
 __device__ __forceinline__ int oz_tile_nkc(uint32_t t, int nkc) {
-  return ((t >> 25) & 3) == OZ_PANEL ? min(nkc, (int)(((t >> 12) & 0x1fff) + 1) * (2 * OZ_TN / OZ_KC)) : nkc;
+  return ((t >> 25) & 3) == OZ_PANEL ? min(nkc, (int)(((t >> 12) & 0x1fff) + 1) * (OZ_TN / OZ_KC)) : nkc;
 }
 // one 32-deep k-chunk of warpgroup W: the digit pairs (s, g - s) of its groups g < ND. a_base = shared address of digit
 // plane 0 of the A sub-tile in this stage; the B planes follow the 8 A planes.
@@ -248,23 +249,19 @@ __device__ __forceinline__ void oz_subtile(double (&f)[32], uint32_t ring_s, uin
 
 template <int W>
 __device__ __forceinline__ void oz_consume(const OzParams& p, const unsigned char* ring, double* xch, uint64_t* full,
-                                           uint64_t* empty, int ti_beg, int ti_end, int tw) {
+                                           uint64_t* empty, int ti_beg, int ti_end) {
   const int tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31;
   const uint32_t ring_s = smem_u32(ring);
-  const int nsub = 2 * (tw / OZ_SUB);
   uint32_t it = 0;
   for (int ti = ti_beg; ti < ti_end; ti++) {
     const uint32_t t = p.tiles[ti];
     const int r = t & 0xfff, c = (t >> 12) & 0x1fff, kind = (t >> 25) & 3;
-    const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
+    const bool up = (t >> 27) & 1;
     const int nkc_t = oz_tile_nkc(t, p.nkc);
-    for (int sub = 0; sub < nsub; sub++) {
+    for (int sub = 0; sub < OZ_NSUB; sub++) {
       double f[32];
-      if (nd == 8) oz_subtile<W, 8>(f, ring_s, full, empty, it, nkc_t, tid);
-      else if (nd == 7) oz_subtile<W, 7>(f, ring_s, full, empty, it, nkc_t, tid);
-      else if (nd == 6) oz_subtile<W, 6>(f, ring_s, full, empty, it, nkc_t, tid);
-      else if (nd == 5) oz_subtile<W, 5>(f, ring_s, full, empty, it, nkc_t, tid);
-      else oz_subtile<W, 4>(f, ring_s, full, empty, it, nkc_t, tid);
+      if (up) oz_subtile<W, OZ_S_UP>(f, ring_s, full, empty, it, nkc_t, tid);
+      else oz_subtile<W, OZ_S>(f, ring_s, full, empty, it, nkc_t, tid);
       // warpgroup 0 finishes columns 0..31 of the sub-tile (accumulator elements 0..15), warpgroup 1 columns 32..63: each
       // hands the other half of its partial sums over (the two hold the same elements at the same thread index)
       constexpr int KEEP = W == 0 ? 0 : 16, GIVE = 16 - KEEP;
@@ -276,7 +273,7 @@ __device__ __forceinline__ void oz_consume(const OzParams& p, const unsigned cha
       for (int e = 0; e < 16; e++) f[KEEP + e] += xch[((1 - W) * 16 + e) * 128 + tid];
       // element e of the accumulator: row warp * 16 + lane / 4 + 8 * ((e / 2) % 2), column (e / 4) * 8 + (lane % 4) * 2 + e % 2
       const long gi0 = (long)r * OZ_TM + (sub & 1) * OZ_SUB + warp * 16 + (lane >> 2);
-      const long gj0 = (long)c * tw + (sub >> 1) * OZ_SUB + (lane & 3) * 2;
+      const long gj0 = (long)c * OZ_TN + (sub >> 1) * OZ_SUB + (lane & 3) * 2;
       const double si[2] = {p.scale[gi0], p.scale[gi0 + 8]};
       const double* scol = kind == OZ_PANEL ? p.scaleB : p.scale;
       double v[16];
@@ -332,7 +329,6 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     tma_prefetch_desc(&mapB);
   }
   __syncthreads();
-  const int tw = p.wide ? 2 * OZ_TN : OZ_TN;
   // a CTA owns p.tpc CONSECUTIVE tiles of the list (neighbours in the banded order share operand panels in L2) and then
   // retires: SM slots come free every few tiles, so the high-priority side stream of the sweep (diagonal block, panel of the
   // next step) gets onto the machine while this launch is still running — a fully persistent grid would shut it out
@@ -342,15 +338,14 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     if (threadIdx.x >= 288) return;
     // ================= TMA producer: lane s < nd loads digit plane s of both operands ================================
     const int lane = threadIdx.x & 31;
-    const int nsub = 2 * (tw / OZ_SUB);
     uint32_t it = 0;
     for (int ti = ti_beg; ti < ti_end; ti++) {
       const uint32_t t = p.tiles[ti];
       const int r = t & 0xfff, c = (t >> 12) & 0x1fff;
-      const int nd = ((t >> 27) & 1) ? p.dig_up : p.dig_lo;
+      const int nd = ((t >> 27) & 1) ? OZ_S_UP : OZ_S;
       const int nkc_t = oz_tile_nkc(t, p.nkc);
-      for (int sub = 0; sub < nsub; sub++) {
-        const int arow = (r * OZ_TM + (sub & 1) * OZ_SUB) / 8, brow = (c * tw + (sub >> 1) * OZ_SUB) / 8;
+      for (int sub = 0; sub < OZ_NSUB; sub++) {
+        const int arow = (r * OZ_TM + (sub & 1) * OZ_SUB) / 8, brow = (c * OZ_TN + (sub >> 1) * OZ_SUB) / 8;
         for (int kc = 0; kc < nkc_t; kc++, it++) {
           const int st = it % OZ_STAGES;
           mbar_wait_backoff(&empty[st], ((it / OZ_STAGES) & 1) ^ 1, 64);
@@ -366,30 +361,26 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    if (wg == 0) oz_consume<0>(p, ring, xch, full, empty, ti_beg, ti_end, tw);
-    else oz_consume<1>(p, ring, xch, full, empty, ti_beg, ti_end, tw);
+    if (wg == 0) oz_consume<0>(p, ring, xch, full, empty, ti_beg, ti_end);
+    else oz_consume<1>(p, ring, xch, full, empty, ti_beg, ti_end);
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// tile lists of the sweep (host): per panel step the launches U0 | U1 | U2 (+ the K^-1 tiles of the step)
+// tile lists of the sweep (host): per panel step the launches U1 | U2 (+ the K^-1 tiles of the step) and the panel GEMM
 // ---------------------------------------------------------------------------------------------------------------
-// tiles in bands of 8 row tiles x 16 column tiles (64 wide): the ~132 tiles in flight share 8 A panels and 16 B panels in L2
-// (column tiles: cw per 128 columns - two 64-wide tiles, or one 128-wide tile with option oz_wide)
+// tiles in bands of 8 row tiles x 8 column tiles: the CTAs in flight share a few operand panels in L2
 template <class Valid, class Emit>
-static void oz_banded(const std::vector<int>& rows, int ct_beg, int ct_end, int cw, Valid valid, Emit emit) {
+static void oz_banded(const std::vector<int>& rows, int ct_beg, int ct_end, Valid valid, Emit emit) {
   for (size_t b = 0; b < rows.size(); b += 8)
-    for (int cc = ct_beg; cc < ct_end; cc += 8 * cw)
+    for (int cc = ct_beg; cc < ct_end; cc += 8)
       for (size_t i = b; i < std::min(rows.size(), b + 8); i++)
-        for (int ct = cc; ct < std::min(ct_end, cc + 8 * cw); ct++)
-          if (valid(rows[i], ct / cw)) emit(rows[i], ct);
+        for (int ct = cc; ct < std::min(ct_end, cc + 8); ct++)
+          if (valid(rows[i], ct)) emit(rows[i], ct);
 }
 
-// own_G > 1 (memory-distributed multi-GPU sweep): only the row tiles of the block rows this rank owns (block-cyclic over the
-// panels of NB rows, like the DMMA update of gpx_dist.cu) are listed; every tile of the matrix is in exactly one rank's list.
-void oz_build_lists(long Npad, long NB, int cw, int own_G, int own_g, std::vector<uint32_t>& tiles, std::vector<OzStep>& steps) {
-  const int nt = (int)(Npad / TILE), nbt_full = (int)(NB / TILE);
-  auto mine = [&](int r) { return own_G <= 1 || ((r / nbt_full) % own_G) == own_g; };
+void oz_build_lists(long Npad, long NB, std::vector<uint32_t>& tiles, std::vector<OzStep>& steps) {
+  const int nt = (int)(Npad / TILE);
   tiles.clear();
   steps.clear();
   for (long o = 0; o < Npad; o += NB) {
@@ -397,44 +388,29 @@ void oz_build_lists(long Npad, long NB, int cw, int own_G, int own_g, std::vecto
     const int kt0 = (int)(o / TILE), kt1 = kt0 + (int)(nb / TILE);
     const int next_nbt = kt1 < nt ? (int)(std::min(NB, Npad - (o + nb)) / TILE) : 0;
     OzStep st;
-    auto emit_update = [&](int cbeg, int cend) {   // S(r, c) -= P_r P_c^T, c in [cbeg, cend), r in [0, kt1) U [c, nt)
-      std::vector<int> rows;
-      for (int r = 0; r < kt1; r++) if (mine(r)) rows.push_back(r);
-      for (int r = cbeg; r < nt; r++) if (mine(r)) rows.push_back(r);
-      oz_banded(rows, cw * cbeg, cw * cend, cw, [&](int r, int cc) { return r < kt1 || cc <= r; },
-                [&](int r, int ct) { tiles.push_back(oz_tile(r, ct, OZ_UPDATE, r < kt1 ? 1 : 0)); });
+    // S(r, c) -= P_r P_c^T, c in [cbeg, cend), r in [0, kt1) U [c, nt) outside block k+1: the next diagonal block is updated
+    // in fp64 by the serial chain of the sweep
+    std::vector<int> urows;
+    for (int r = 0; r < kt1; r++) urows.push_back(r);
+    for (int r = kt1 + next_nbt; r < nt; r++) urows.push_back(r);
+    auto emit_update = [&](int cbeg, int cend) {
+      oz_banded(urows, cbeg, cend, [&](int r, int c) { return r < kt1 || c <= r; },
+                [&](int r, int c) { tiles.push_back(oz_tile(r, c, OZ_UPDATE, r < kt1 ? 1 : 0)); });
     };
     auto count_up = [&](int off, int n) { int u = 0; for (int i = off; i < off + n; i++) u += (tiles[i] >> 27) & 1; return u; };
-    // U0: the tiles of the NEXT diagonal block (rows and columns of block k+1): all that D(k+1) waits for
-    st.u0_off = (int)tiles.size();
-    if (kt1 < nt) {
-      std::vector<int> rows;
-      for (int r = kt1; r < kt1 + next_nbt; r++) if (mine(r)) rows.push_back(r);
-      oz_banded(rows, cw * kt1, cw * (kt1 + next_nbt), cw, [&](int r, int cc) { return cc <= r; },
-                [&](int r, int ct) { tiles.push_back(oz_tile(r, ct, OZ_UPDATE, 0)); });
-    }
-    st.u0_n = (int)tiles.size() - st.u0_off;
-    st.u0_up = 0;
     // U1: the rest of block column k+1 (rows above the block and below it)
     st.u1_off = (int)tiles.size();
-    if (kt1 < nt) {
-      std::vector<int> rows;
-      for (int r = 0; r < kt1; r++) if (mine(r)) rows.push_back(r);
-      for (int r = kt1 + next_nbt; r < nt; r++) if (mine(r)) rows.push_back(r);
-      oz_banded(rows, cw * kt1, cw * (kt1 + next_nbt), cw, [&](int r, int cc) { return r < kt1 || cc <= r; },
-                [&](int r, int ct) { tiles.push_back(oz_tile(r, ct, OZ_UPDATE, r < kt1 ? 1 : 0)); });
-    }
+    emit_update(kt1, kt1 + next_nbt);
     st.u1_n = (int)tiles.size() - st.u1_off;
     st.u1_up = count_up(st.u1_off, st.u1_n);
+    // U2: the columns after block k+1, then the K^-1 tiles
     st.u2_off = (int)tiles.size();
-    if (kt1 + next_nbt < nt) emit_update(kt1 + next_nbt, nt);
-    st.u2_upd = (int)tiles.size() - st.u2_off;
-    st.u2_upd_up = count_up(st.u2_off, st.u2_upd);
+    emit_update(kt1 + next_nbt, nt);
     {   // K^-1(r, c) (+)= P_r P_c^T for c <= r < kt1: rows of block k see their first contribution at this step
       std::vector<int> rows;
-      for (int r = 0; r < kt1; r++) if (mine(r)) rows.push_back(r);
-      oz_banded(rows, 0, cw * kt1, cw, [&](int r, int cc) { return cc <= r; },
-                [&](int r, int ct) { tiles.push_back(oz_tile(r, ct, r >= kt0 ? OZ_LAUUM_SET : OZ_LAUUM_ACC, 1)); });
+      for (int r = 0; r < kt1; r++) rows.push_back(r);
+      oz_banded(rows, 0, kt1, [&](int r, int c) { return c <= r; },
+                [&](int r, int c) { tiles.push_back(oz_tile(r, c, r >= kt0 ? OZ_LAUUM_SET : OZ_LAUUM_ACC, 1)); });
     }
     st.u2_n = (int)tiles.size() - st.u2_off;
     st.u2_up = count_up(st.u2_off, st.u2_n);
@@ -442,13 +418,12 @@ void oz_build_lists(long Npad, long NB, int cw, int own_G, int own_g, std::vecto
       st.pan_off = (int)tiles.size();
       const int nbt = kt1 - kt0;
       std::vector<int> rows;
-      for (int r = 0; r < kt0; r++) if (mine(r)) rows.push_back(r);
-      for (int r = kt1 + next_nbt; r < nt; r++) if (mine(r)) rows.push_back(r);
+      for (int r = 0; r < kt0; r++) rows.push_back(r);
+      for (int r = kt1 + next_nbt; r < nt; r++) rows.push_back(r);
       for (size_t b = 0; b < rows.size(); b += 8)              // bands of 8 row tiles; longest k-range (last column tile) first
         for (int cc = nbt - 1; cc >= 0; cc--)
           for (size_t i = b; i < std::min(rows.size(), b + 8); i++) tiles.push_back(oz_tile(rows[i], cc, OZ_PANEL, rows[i] < kt0 ? 1 : 0));
       st.pan_n = (int)tiles.size() - st.pan_off;
-      st.pan_up = count_up(st.pan_off, st.pan_n);
     }
     steps.push_back(st);
   }
@@ -508,171 +483,12 @@ void oz_planes_free(OzPlanes& pl) {
 int launch_oz_gemm(const OzPlanes& pl, const OzParams& p_in, int num_sms, cudaStream_t st, const OzPlanes* plB) {
   if (p_in.ntiles <= 0) return 0;
   OzParams p = p_in;
-  // default: 8 narrow / 4 wide tiles per CTA when there is enough work
-  if (p.tpc <= 0) p.tpc = std::max(1, std::min(p.wide ? 4 : 8, p.ntiles / std::max(1, num_sms)));
+  // default: 4 tiles per CTA when there is enough work
+  if (p.tpc <= 0) p.tpc = std::max(1, std::min(4, p.ntiles / std::max(1, num_sms)));
   const int grid = (p.ntiles + p.tpc - 1) / p.tpc;
-  if (plB && !p.wide) { set_error("OZ_PANEL tiles are listed in 128-column units (wide)"); return -2; }
   oz_gemm_kernel<<<grid, OZ_THREADS, OZ_SMEM, st>>>(pl.map, plB ? plB->map : pl.map, p);
   GPX_CUDA(cudaGetLastError());
   return 0;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// 3. gradient reductions from the stored K^-1 (same sums as the fused LAUUM epilogue of gpx_gemm.cu):
-//    dL_dK = 1/2 (alpha alpha^T - P K^-1)  (exact_gaussian_inference.py:70), tr -> noise (:72, gaussian.py:78-79),
-//    sum K o dL_dK / variance (stationary.py:199), ARD / iso lengthscale sums (:202-213, 225-243). One CTA per lower
-//    128 x 128 tile; the thread-mapped index is the ROW (contiguous in the column-major K^-1), 64 columns per thread.
-// ---------------------------------------------------------------------------------------------------------------
-template <int DREG>
-__global__ void __launch_bounds__(256) grad_kinv_kernel(GradKinvParams p) {
-  extern __shared__ __align__(128) unsigned char gk_smem[];
-  const int D = p.kp.D, P = p.P;
-  double* sXc = reinterpret_cast<double*>(gk_smem);   // [D][128] column points
-  double* sSc = sXc + (size_t)D * TILE;               // [128]
-  double* sAc = sSc + TILE;                           // [P][128]
-  double* sRed = sAc + (size_t)P * TILE;              // [8 warps][nred]
-  // lower tiles only: blockIdx.x enumerates (r, c), c <= r
-  const int csplit = p.csplit, tileidx = (int)blockIdx.x / csplit, sidx = (int)blockIdx.x % csplit;
-  int r = (int)((sqrtf(8.f * (float)tileidx + 1.f) - 1.f) * 0.5f);
-  while (r * (r + 1) / 2 > tileidx) --r;
-  while ((r + 1) * (r + 2) / 2 <= tileidx) ++r;
-  const int c = tileidx - r * (r + 1) / 2;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int idx = tid; idx < D * TILE; idx += 256) sXc[idx] = p.XsT[(long)(idx / TILE) * p.ldx + (long)c * TILE + idx % TILE];
-  for (int idx = tid; idx < P * TILE; idx += 256) sAc[idx] = p.alpha[(long)(idx / TILE) * p.ldx + (long)c * TILE + idx % TILE];
-  if (tid < TILE) sSc[tid] = p.sq[(long)c * TILE + tid];
-  __syncthreads();
-  const int il = tid & (TILE - 1), half = tid >> 7;
-  const long gi = (long)r * TILE + il;
-  const bool ard = p.kp.ard != 0;
-  const int nl = ard ? D : 1, nred = nl + 2;
-  double xi[DREG], gq[DREG], ai[MAX_P];
-#pragma unroll
-  for (int q = 0; q < DREG; q++) { gq[q] = 0.0; xi[q] = q < D ? p.XsT[(long)q * p.ldx + gi] : 0.0; }
-#pragma unroll
-  for (int q = 0; q < MAX_P; q++) ai[q] = q < P ? p.alpha[(long)q * p.ldx + gi] : 0.0;
-  const double si = p.sq[gi];
-  const double w = (r > c) ? 2.0 : 1.0;               // strictly-lower tiles stand for their mirror image as well
-  const double variance = p.kp.variance, inv_ls = p.kp.inv_ls_iso;
-  const int kind = p.kp.kind;
-  double gvar = 0.0, giso = 0.0, gnoise = 0.0;
-  const double* kcol = p.Kinv + gi + ((long)c * TILE + half * 64) * p.ld;
-  if (gi < p.N) {
-    const int jj_beg = sidx * (64 / csplit);
-    const int jj_end = (int)min((long)(jj_beg + 64 / csplit), p.N - (long)c * TILE - half * 64);   // columns beyond N are padding
-    // two columns in flight per thread: one column is a single dependent chain (dot product -> exp -> reductions) and the
-    // 16 warps an SM holds at 92 registers leave the fp64 pipe mostly idle (1.8 ms for the 134 M elements of N = 16384)
-#pragma unroll 2
-    for (int jj = jj_beg; jj < jj_end; jj++) {
-      const int jl = half * 64 + jj;
-      const long gj = (long)c * TILE + jl;
-      const double kinv = kcol[(long)jj * p.ld];
-      double dot = 0.0;
-#pragma unroll
-      for (int q = 0; q < DREG; q++)
-        if (q < D) dot = fma(xi[q], sXc[q * TILE + jl], dot);
-      double r2 = si + sSc[jl] - 2.0 * dot;
-      if (gi == gj) r2 = 0.0;
-      r2 = fmax(r2, 0.0);
-      double aa = 0.0;
-#pragma unroll
-      for (int q = 0; q < MAX_P; q++)
-        if (q < P) aa = fma(ai[q], sAc[q * TILE + jl], aa);
-      const double dl = 0.5 * (aa - (double)P * kinv);
-      if (gi == gj) {
-        gnoise += dl;
-        if (p.dnoise_out) p.dnoise_out[gi] = dl;
-      }
-      if (kind == GPX_RBF) {
-        // dK/dr / r = -K for the RBF kernel (rbf.py:177-178 over stationary.py:205): neither the square root nor the division
-        // of the general form is needed; at r = 0 the reference's 1/0 := 0 multiplies (x_i - x_j)^2 = 0 either way
-        const double r2s = r2 * (inv_ls * inv_ls);
-        const double k = exp(-0.5 * r2s);
-        const double kd = w * k * dl;
-        gvar += kd;
-        const double tmpv = -variance * kd;
-        if (ard) {
-#pragma unroll
-          for (int q = 0; q < DREG; q++)
-            if (q < D) {
-              const double df = xi[q] - sXc[q * TILE + jl];
-              gq[q] = fma(tmpv, df * df, gq[q]);
-            }
-        } else {
-          giso = fma(tmpv, r2s, giso);
-        }
-        continue;
-      }
-      const double rr = sqrt(r2) * inv_ls;
-      double k, dk;
-      k_dk_of_r_unit(kind, rr, k, dk);
-      gvar = fma(w * k, dl, gvar);
-      const double G = variance * dk * dl;
-      if (ard) {
-        const double tmpv = (rr != 0.0) ? w * G / rr : 0.0;     // stationary.py:205,225-232: 1/r with 1/0 := 0
-#pragma unroll
-        for (int q = 0; q < DREG; q++)
-          if (q < D) {
-            const double df = xi[q] - sXc[q * TILE + jl];
-            gq[q] = fma(tmpv, df * df, gq[q]);
-          }
-      } else {
-        giso = fma(w * G, rr, giso);
-      }
-    }
-  }
-  gvar = warp_sum(gvar);
-  gnoise = warp_sum(gnoise);
-  if (lane == 0) { sRed[warp * nred] = gvar; sRed[warp * nred + nred - 1] = gnoise; }
-  if (ard) {
-#pragma unroll
-    for (int q = 0; q < DREG; q++)
-      if (q < D) {
-        const double s = warp_sum(gq[q]);
-        if (lane == 0) sRed[warp * nred + 1 + q] = s;
-      }
-  } else {
-    giso = warp_sum(giso);
-    if (lane == 0) sRed[warp * nred + 1] = giso;
-  }
-  __syncthreads();
-  if (tid < nred) {
-    double s = 0.0;
-#pragma unroll
-    for (int wdx = 0; wdx < 8; wdx++) s += sRed[wdx * nred + tid];
-    p.partials[(((long)r * p.nt + c) * csplit + sidx) * nred + tid] = s;
-  }
-}
-
-int grad_kinv_csplit(int nt, int nred) {
-  const int tiles = nt * (nt + 1) / 2;
-  int cs = 1;
-  while (cs < 8 && tiles * cs < 528 && (cs * 2) * nred <= MAX_D + 2) cs *= 2;   // ~4 waves of CTAs on 132 SMs; partials sized for MAX_D + 2 per tile
-  return cs;
-}
-
-template <int DREG>
-static int launch_grad_kinv_t(const GradKinvParams& p, unsigned grid, size_t smem, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    GPX_CUDA(cudaFuncSetAttribute(grad_kinv_kernel<DREG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)((MAX_D + 1 + MAX_P) * TILE * 8 + 8 * (MAX_D + 2) * 8)));
-    attr_set = true;
-  }
-  grad_kinv_kernel<DREG><<<grid, 256, smem, st>>>(p);
-  GPX_CUDA(cudaGetLastError());
-  return 0;
-}
-
-int launch_grad_kinv(const GradKinvParams& p, cudaStream_t st) {
-  const int D = p.kp.D;
-  const size_t smem = (size_t)(D + 1 + p.P) * TILE * 8 + 8 * (MAX_D + 2) * 8;
-  if (p.csplit != 1 && p.csplit != 2 && p.csplit != 4 && p.csplit != 8) { set_error("grad_kinv: csplit must be 1, 2, 4 or 8"); return -2; }
-  const unsigned grid = (unsigned)(p.nt * (p.nt + 1) / 2 * p.csplit);
-  if (D <= 8) return launch_grad_kinv_t<8>(p, grid, smem, st);
-  if (D <= 16) return launch_grad_kinv_t<16>(p, grid, smem, st);
-  if (D <= 32) return launch_grad_kinv_t<32>(p, grid, smem, st);
-  return launch_grad_kinv_t<64>(p, grid, smem, st);
 }
 
 }  // namespace gpx

@@ -11,9 +11,12 @@ struct gpx_ctx;
 
 namespace gpx {
 
-constexpr int OZ_S = 8;         // signed 7-bit digit planes per fp64 operand (56 bits >= the 53-bit significand)
-constexpr int OZ_TM = 128;      // output tile rows   (two 64-row wgmma sub-tiles)
-constexpr int OZ_TN = 64;       // output tile columns (= wgmma N; 128 with option oz_wide)
+constexpr int OZ_S = 8;         // signed 7-bit digit planes per fp64 operand (56 bits >= the 53-bit significand); digits used
+                                // for Cholesky-part tiles
+constexpr int OZ_S_UP = 7;      // digits used for inverse-part / K^-1 tiles, which feed only the gradients (28 digit pairs
+                                // instead of 36, gradient error ~6e-10 at N = 16384; DESIGN.md §5.1)
+constexpr int OZ_TM = 128;      // output tile rows    (two 64-row wgmma sub-tiles)
+constexpr int OZ_TN = 128;      // output tile columns (two 64-column wgmma sub-tiles)
 constexpr int OZ_KC = 32;       // k-depth of one wgmma .s8 (32 bytes of K)
 
 // Digit planes of one panel (rows x K, K = nkc * 32), stored so that every (plane, k-chunk, 8-row group) is one 256-byte
@@ -30,10 +33,10 @@ struct OzPlanes {
   CUtensorMap map;              // the tensor with a 64-row box (one wgmma operand of one plane and k-chunk)
 };
 
-// one output tile: bits 0-11 row tile (128 rows), 12-24 column tile (64 columns), 25-26 kind, 27 inverse-part tile
+// one output tile: bits 0-11 row tile, 12-24 column tile, 25-26 kind, 27 inverse-part tile
 enum OzKind { OZ_UPDATE = 0, OZ_LAUUM_ACC = 1, OZ_LAUUM_SET = 2, OZ_PANEL = 3 };
-inline uint32_t oz_tile(int r, int c64, int kind, int upper) {
-  return (uint32_t)r | ((uint32_t)c64 << 12) | ((uint32_t)kind << 25) | ((uint32_t)upper << 27);
+inline uint32_t oz_tile(int r, int c, int kind, int upper) {
+  return (uint32_t)r | ((uint32_t)c << 12) | ((uint32_t)kind << 25) | ((uint32_t)upper << 27);
 }
 
 struct OzParams {
@@ -43,43 +46,25 @@ struct OzParams {
   const double* scale;     // row scales of the panel (shared by both operands: C (op)= P_r P_c^T)
   double* S; long lds;     // OZ_UPDATE target:      S(r, c)    -= P_r P_c^T
   double* Kinv; long ldk;  // OZ_LAUUM_* target:     Kinv(r, c) (+)= P_r P_c^T   (lower tiles)
-  int dig_lo, dig_up;      // digits per operand for Cholesky-part tiles / inverse-part tiles (<= OZ_S)
   int tpc;                 // consecutive tiles per CTA (0 = default)
-  int wide;                // 1: 128 x 128 tiles (column tile index in 128-column units), 0: 128 x 64 tiles
-  // OZ_PANEL tiles (wide only): P(r, c') = A_r B_c'^T with A = digit planes of a block column of the workspace
-  // (pl of launch_oz_gemm), B = digit planes of L_kk^-1 (plB of launch_oz_gemm), lower triangular: the k-range of output
-  // column tile c' ends at (c' + 1) * 128. Result stored (not accumulated) into P.
+  // OZ_PANEL tiles: P(r, c') = A_r B_c'^T with A = digit planes of a block column of the workspace (pl of launch_oz_gemm),
+  // B = digit planes of L_kk^-1 (plB of launch_oz_gemm), lower triangular: the k-range of output column tile c' ends at
+  // (c' + 1) * 128. Result stored (not accumulated) into P.
   double* P; long ldp;
   double* Pfinal;          // optional second target of OZ_PANEL tiles: the block column of the workspace itself (ld = lds)
   const double* scaleB;    // row scales of the B operand's planes (= column scales of the product)
 };
 
-// one panel step of the sweep: offsets into the tile list. U0: the next diagonal block only; U1: the rest of block column k+1;
-// U2 list: u2_upd update tiles, then the K^-1 tiles; *_up = inverse-part tiles among them
-struct OzStep { int u0_off, u0_n, u1_off, u1_n, u2_off, u2_n, u2_upd, u0_up, u1_up, u2_up, u2_upd_up;
-                // panel GEMM of the step on the tensor cores: rows outside the diagonal block and the next block
-                int pan_off, pan_n, pan_up; };
-void oz_build_lists(long Npad, long NB, int cw, int own_G, int own_g, std::vector<uint32_t>& tiles, std::vector<OzStep>& steps);
+// one panel step of the sweep: offsets into the tile list. U1: block column k+1 outside its diagonal block; U2: the other
+// update tiles, then the K^-1 tiles; pan: the panel GEMM rows outside the diagonal block and block k+1; *_up = inverse-part
+// tiles among them
+struct OzStep { int u1_off, u1_n, u1_up, u2_off, u2_n, u2_up, pan_off, pan_n; };
+void oz_build_lists(long Npad, long NB, std::vector<uint32_t>& tiles, std::vector<OzStep>& steps);
 
 int oz_init();                                                          // driver entry point + kernel attributes
 int oz_planes_alloc(OzPlanes& pl, long rows, long K);                    // buffers + tensor maps
 void oz_planes_free(OzPlanes& pl);
 int launch_oz_split(const double* P, long ld, long K, OzPlanes& pl, cudaStream_t st);   // P: rows x K column-major, K <= layout
 int launch_oz_gemm(const OzPlanes& pl, const OzParams& p, int num_sms, cudaStream_t st, const OzPlanes* plB = nullptr);
-
-// gradient reductions from a stored K^-1 (lower 128 x 128 tiles, column-major, leading dimension ld): same partial sums as
-// the fused epilogue of gemm_lauum_kernel, consumed by finalize_kernel
-struct GradKinvParams {
-  const double* Kinv; long ld;
-  const double* XsT; const double* sq; const double* alpha; long ldx;
-  long N; int P; int nt;
-  double* partials;        // [nt*nt*csplit][nl+2], zeroed by the caller
-  int csplit;              // CTAs per tile (each takes 64/csplit columns of both column halves): 1, 2, 4 or 8 -- small matrices
-                           // have too few tiles to fill the machine, and a thread's 64 columns are a serial chain
-  double* dnoise_out;      // optional diag(dL_dK)
-  KernParams kp;
-};
-int launch_grad_kinv(const GradKinvParams& p, cudaStream_t st);
-int grad_kinv_csplit(int nt, int nred);   // the split launch_grad_kinv expects for this matrix (partials: nt*nt*(MAX_D+2) doubles)
 
 }  // namespace gpx

@@ -188,12 +188,12 @@ int64_t gpx_total_launches(gpx_ctx* ctx);
 /* Roofline denominator measured on this device: fp64 tensor (DMMA.16x8x4) issue rate in TFLOP/s, CUDA-event timed. */
 int gpx_measure_fp64_peak(gpx_ctx* ctx, double* tflops);
 
-/* Tunables (block sizes etc.), mainly for tests: name in {"nb", "lookahead", "profile", "ozaki" (0 = fp64 DMMA only,
- * 1 = trailing update and K^-1 on the wgmma int8 path where applicable, -1 = default: env GPX_OZAKI, else 0), "oz_dig_up" (digits per operand
- * for the inverse-part tiles, 4..8), "oz_ctas" (CTAs of the persistent int8 GEMM, 0 = one per SM), "fine" (1 = 64 x 64-tile DMMA kernels inside
- * the diagonal-block chain, 0 = 128 x 128 tiles), "chain" (1 = Ozaki path: diagonal-block chain alone on the side stream, the
- * rest of the panel / digit split / forward substitution on a third stream; 0 = round-2 schedule), "base" (generation of the
- * 128 x 128 base-block kernel, process-wide: 0 = default, 1..3)}. */
+/* Tunables, mainly for tests. name is one of
+ *   "nb"      outer block size: a multiple of 128, 0 = default: env GPX_NB, else by matrix size,
+ *   "profile" 1 (default) = per-phase times in gpx_stats, 0 = total_ms only,
+ *   "ozaki"   0 = fp64 DMMA only, 1 = trailing update and K^-1 on the wgmma int8 path where applicable,
+ *             -1 = default: env GPX_OZAKI, else 0.
+ * Any other name fails with "unknown option". */
 int gpx_set_option(gpx_ctx* ctx, const char* name, int64_t value);
 
 /* Multi-GPU (one process per GPU). The caller obtains a 128-byte NCCL unique id on rank 0 (gpx_comm_unique_id),

@@ -73,17 +73,21 @@ def test_block_size_does_not_change_the_answer(nb):
 
 
 def test_metric_size_n4096_against_oracle():
-    """N=4096, D=8 (the smallest size of the BASELINE.json metric): LML, gradient and alpha against the oracle."""
+    """N=4096, D=8 (the smallest size of the BASELINE.json metric): LML, gradient and alpha against the oracle, on both
+    tensor paths (option ozaki = 0 and 1). N = 4096 is the smallest size at which the int8 path also runs the panel GEMM
+    on the tensor cores."""
     X, Y = o.synthetic(4096, 8, seed=3)
     var, ls, noise = o.theta_bench(8, True)
     lml0, g0, res = o.eval_lml_grad(X, Y, "matern32", True, var, ls, noise)
-    e = _ffi.Engine(0)
-    e.set_data(X, Y)
-    lml, g, _ = e.exact_eval("matern32", True, var, ls, noise)
-    assert abs(lml - lml0) <= LML_ATOL
-    np.testing.assert_allclose(g, g0, rtol=GRAD_RTOL)
-    assert rel(e.get("alpha"), res["alpha"]) < 1e-9
-    e.close()
+    for oz in (0, 1):
+        e = _ffi.Engine(0)
+        e.set_option("ozaki", oz)
+        e.set_data(X, Y)
+        lml, g, _ = e.exact_eval("matern32", True, var, ls, noise)
+        assert abs(lml - lml0) <= LML_ATOL, (oz, lml, lml0)
+        np.testing.assert_allclose(g, g0, rtol=GRAD_RTOL, err_msg="ozaki = %d" % oz)
+        assert rel(e.get("alpha"), res["alpha"]) < 1e-9, oz
+        e.close()
 
 
 def test_config3_kernel_matern52_d32_n4096_against_oracle():
