@@ -9,6 +9,8 @@
  * digit-split products on the wgmma tensor cores whose exact s32 sums are recombined in fp64 (8 digits for the Cholesky
  * part, 7 for the inverse part:
  * |dLML| <= 1e-8 and 1e-6 relative on gradients against the reference, DESIGN.md section 5.1; option "ozaki" selects).
+ * The gradient bound is checked on the GPU up to cond(Ky) = 4.6e8. Above cond(Ky) ~ 1e8 the LML and alpha of both paths
+ * are less accurate than LAPACK's (DESIGN.md section 5.1).
  *
  * Conventions
  *   - Return value: 0 ok; >0 "matrix not positive definite, leading minor <ret>" (the caller raises

@@ -598,8 +598,9 @@ def _composite_case(D=5):
 @pytest.mark.parametrize("N", [150, 700, 1300])
 def test_composite_kernels_on_the_fused_device_path(N):
     """Sum / product / White / Bias kernels (add.py:60-99, prod.py:59-68,377-396, static.py:63-185) through
-    gpx_exact_eval_multi: LML, every part's gradient, alpha, K and predictions against the oracle; N = 700 / 1300 take the
-    int8 (Ozaki) sweep with the stored K^-1, N = 150 the DMMA sweep + plain LAUUM."""
+    gpx_exact_eval_multi: LML, every part's gradient, alpha, K and predictions against the oracle. N = 700 / 1300 force
+    option ozaki = 1 and take the int8 (Ozaki) sweep with the stored K^-1; N = 150 is a single block and takes the DMMA
+    sweep + plain LAUUM. The default (DMMA) path on several blocks is tests/test_gpu_routes.py::test_route_matrix_composite."""
     D = 5
     X, Y = o.synthetic(N, D, seed=N)
     k, parts = _composite_case(D)
