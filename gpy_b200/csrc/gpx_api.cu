@@ -25,11 +25,6 @@ void set_error(const std::string& msg) { g_err = msg; }
 
 using namespace gpx;
 
-#define GPX_CHECK(x)        \
-  do {                      \
-    int rc__ = (x);         \
-    if (rc__ != 0) return rc__; \
-  } while (0)
 #define GPX_FAIL(msg)       \
   do {                      \
     gpx::set_error(msg);    \
@@ -37,7 +32,7 @@ using namespace gpx;
   } while (0)
 
 
-static void free_data(gpx_ctx* c) {
+void gpx::free_data(gpx_ctx* c) {
   double** ptrs[] = {&c->dX, &c->dXsT, &c->dsq, &c->dY, &c->dT, &c->dAlpha, &c->dUvPart, &c->S, &c->Pbuf, &c->Tm,
                      &c->Ldiag, &c->Dinv, &c->logdet_part, &c->partials, &c->Kinv, &c->staging};
   for (auto p : ptrs) {
@@ -59,6 +54,27 @@ static void free_data(gpx_ctx* c) {
   c->oz_steps.clear();
   c->oz_ready = false;
   c->oz_lists_ready = false;
+}
+
+int gpx::alloc_data(gpx_ctx* c, long NB) {
+  const long Npad = c->Npad, nt = Npad / TILE;
+  GPX_CUDA(cudaMalloc(&c->dX, (size_t)Npad * c->D * 8));
+  GPX_CUDA(cudaMalloc(&c->dXsT, (size_t)Npad * c->D * 8));
+  GPX_CUDA(cudaMalloc(&c->dsq, (size_t)Npad * 8));
+  GPX_CUDA(cudaMalloc(&c->dY, (size_t)Npad * c->P * 8));
+  GPX_CUDA(cudaMalloc(&c->dT, (size_t)Npad * c->P * 8));
+  GPX_CUDA(cudaMalloc(&c->dAlpha, (size_t)Npad * c->P * 8));
+  GPX_CUDA(cudaMalloc(&c->Tm, (size_t)NB * NB * 8));
+  GPX_CUDA(cudaMalloc(&c->Ldiag, (size_t)Npad * TILE * 8));
+  GPX_CUDA(cudaMalloc(&c->Dinv, (size_t)Npad * TILE * 8));
+  GPX_CUDA(cudaMalloc(&c->logdet_part, (size_t)nt * 8));
+  GPX_CUDA(cudaMalloc(&c->partials, (size_t)nt * nt * (MAX_D + 2) * 8));
+  return 0;
+}
+
+static int ensure_kinv(gpx_ctx* c) {
+  if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)c->Npad * c->Npad * 8));
+  return 0;
 }
 
 static long pick_nb(const gpx_ctx* c) {
@@ -179,28 +195,18 @@ int gpx_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y,
   if (D < 1 || D > MAX_D) GPX_FAIL("input dimension must be in [1, 64]");
   if (P < 1 || P > MAX_P) GPX_FAIL("number of output columns must be in [1, 8]");
   GPX_CUDA(cudaSetDevice(c->device));
-  if (c->dist) return dist_set_data(c, X, N, D, Y, P);
   const long Npad = (N + TILE - 1) / TILE * TILE;
-  if (Npad != c->Npad || D != c->D || P != c->P) {
+  if (c->dist) {
+    GPX_CHECK(dist_set_data(c, N, D, P));
+  } else if (Npad != c->Npad || D != c->D || P != c->P) {
     GPX_CUDA(cudaStreamSynchronize(c->st));
     free_data(c);
     c->Npad = Npad; c->D = D; c->P = P;
-    const long nt = Npad / TILE;
     const long NB = pick_nb(c);
-    GPX_CUDA(cudaMalloc(&c->dX, (size_t)Npad * D * 8));
-    GPX_CUDA(cudaMalloc(&c->dXsT, (size_t)Npad * D * 8));
-    GPX_CUDA(cudaMalloc(&c->dsq, (size_t)Npad * 8));
-    GPX_CUDA(cudaMalloc(&c->dY, (size_t)Npad * P * 8));
-    GPX_CUDA(cudaMalloc(&c->dT, (size_t)Npad * P * 8));
-    GPX_CUDA(cudaMalloc(&c->dAlpha, (size_t)Npad * P * 8));
+    GPX_CHECK(alloc_data(c, NB));
     GPX_CUDA(cudaMalloc(&c->dUvPart, (size_t)KSPLIT * Npad * P * 8));
     GPX_CUDA(cudaMalloc(&c->S, (size_t)Npad * Npad * 8));
     GPX_CUDA(cudaMalloc(&c->Pbuf, (size_t)2 * Npad * NB * 8));   // double-buffered for the look-ahead
-    GPX_CUDA(cudaMalloc(&c->Tm, (size_t)NB * NB * 8));
-    GPX_CUDA(cudaMalloc(&c->Ldiag, (size_t)Npad * TILE * 8));
-    GPX_CUDA(cudaMalloc(&c->Dinv, (size_t)Npad * TILE * 8));
-    GPX_CUDA(cudaMalloc(&c->logdet_part, (size_t)nt * 8));
-    GPX_CUDA(cudaMalloc(&c->partials, (size_t)nt * nt * (MAX_D + 2) * 8));
   }
   c->N = N;
   c->have_eval = false;
@@ -208,7 +214,7 @@ int gpx_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y,
   // X: keep the caller's row-major layout on device; Y: SoA [P][Npad] zero padded (staged through dT)
   GPX_CUDA(cudaMemcpyAsync(c->dX, X, (size_t)N * D * 8, cudaMemcpyHostToDevice, c->st));
   GPX_CUDA(cudaMemcpyAsync(c->dT, Y, (size_t)N * P * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(launch_transpose_pad(c->dT, N, P, Npad, c->dY, c->st));
+  GPX_CHECK(launch_transpose_pad(c->dT, N, P, c->Npad, c->dY, c->st));
   c->total_launches += 1;
   GPX_CUDA(cudaStreamSynchronize(c->st));
   return 0;
@@ -278,7 +284,6 @@ static int sync_event(gpx_ctx* c, size_t idx, cudaEvent_t* out) {
 // Ozaki path: tile lists and buffers for (Npad, NB)
 // ---------------------------------------------------------------------------------------------------------------
 static bool oz_wanted(const gpx_ctx* c) {
-  if (c->dist) return false;
   int on = c->ozaki;
   // off by default: on the H100 the fp64 DMMA.16x8x4 GEMMs are faster than the int8 digit split (140 vs 183 ms at
   // N = 16384, H100 80GB HBM3 at a 400 W power limit, profiles/h100_bench_*); option "ozaki" = 1 or GPX_OZAKI=1 selects it
@@ -298,7 +303,6 @@ static int oz_prepare(gpx_ctx* c) {
     GPX_CHECK(oz_planes_alloc(c->ozp[1], Npad, NB));
     GPX_CHECK(oz_planes_alloc(c->ozpA, Npad, NB));
     GPX_CHECK(oz_planes_alloc(c->ozpB, NB, NB));
-    if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)Npad * Npad * 8));
     GPX_CUDA(cudaMalloc(&c->dYres, (size_t)MAX_P * Npad * 8));
     GPX_CUDA(cudaMalloc(&c->dTfw, (size_t)MAX_P * Npad * 8));
     c->oz_ready = true;
@@ -417,8 +421,9 @@ static int run_sweep(gpx_ctx* c, Recorder& rec) {
 // k-1 there is done as well);  the digit planes of step k are those of step k-2: split(k) is behind Pr(k), which waits for
 // U1(k-1), which is behind U2(k-2) on the main stream.
 // What the next diagonal block waits for is therefore D(k) + two small launches, and the main stream never waits for a
-// diagonal block unless the trailing update is shorter than D.
-static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
+// diagonal block unless the trailing update is shorter than D. D(0) waits for `first_rows` (the first block row of Ky,
+// recorded by this evaluation's build_Ky) if given, else for the whole build.
+static int run_sweep_chain(gpx_ctx* c, Recorder& rec, cudaEvent_t first_rows) {
   const long ld = c->Npad, Npad = c->Npad;
   const int nt = (int)(Npad / TILE);
   const long NB = pick_nb(c);
@@ -434,8 +439,7 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
     return 0;
   };
   GPX_CHECK(link(sm, s3, &ev));                      // K build (all of it); it also stands in for "U1(-1)": block column 0 is final
-  if (c->kfirst_valid) GPX_CUDA(cudaStreamWaitEvent(ss, c->ev_kfirst, 0));   // D(0) needs the first block row only
-  else GPX_CUDA(cudaStreamWaitEvent(ss, ev, 0));
+  GPX_CUDA(cudaStreamWaitEvent(ss, first_rows ? first_rows : ev, 0));
   ev_u1 = ev;
   GPX_CUDA(cudaMemcpyAsync(c->dYres, c->dY, (size_t)c->P * Npad * 8, cudaMemcpyDeviceToDevice, s3));
   int kblk = 0;
@@ -549,25 +553,31 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec) {
   return 0;
 }
 
-// plain: store K^-1 (lower tiles) only, no gradient reductions (composite kernels reduce from the stored matrix)
-static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec, bool plain = false) {
+// K^-1 = U U^T on gemm_lauum_kernel, in one of two modes:
+//   fused (kinv_out == nullptr): the epilogue reduces dL_dK straight into the gradient partials of the context's single
+//     kernel (and diag(dL_dK) for per-point noise); K^-1 is not stored
+//   plain store: the lower tiles of K^-1 go to kinv_out (leading dimension Npad); no reductions
+static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec) {
   const long ld = c->Npad;
   const int nt = (int)(c->Npad / TILE);
-  const int nl = c->kp.ard ? c->D : 1;
-  GPX_CUDA(cudaMemsetAsync(c->partials, 0, (size_t)nt * nt * (nl + 2) * 8, c->st));
   GemmParams pl = gemm_defaults();
   pl.mode = GEMM_LAUUM;
   pl.A = c->S; pl.lda = ld;
   pl.B = c->S; pl.ldb = ld;
-  pl.C = nullptr; pl.ldc = ld;
+  pl.ldc = ld;
   pl.K = (int)c->Npad; pl.nt = nt;
-  pl.XsT = c->dXsT; pl.sq = c->dsq; pl.alpha = c->dAlpha; pl.ldx = c->Npad;
-  pl.N = (int)c->N; pl.P = c->P;
-  pl.partials = plain ? nullptr : c->partials;
-  pl.kinv_out = kinv_out;
-  pl.dnoise_out = (c->het && rec && !plain) ? c->dDnoise : nullptr;
-  pl.kp = c->kp;
-  if (plain) { pl.kp.D = 1; pl.P = 1; }
+  if (kinv_out) {
+    pl.kinv_out = kinv_out;
+    pl.kp.D = 1; pl.P = 1;   // the smallest epilogue staging: the plain store does not use it
+  } else {
+    const int nl = c->kp.ard ? c->D : 1;
+    GPX_CUDA(cudaMemsetAsync(c->partials, 0, (size_t)nt * nt * (nl + 2) * 8, c->st));
+    pl.XsT = c->dXsT; pl.sq = c->dsq; pl.alpha = c->dAlpha; pl.ldx = c->Npad;
+    pl.N = (int)c->N; pl.P = c->P;
+    pl.partials = c->partials;
+    pl.dnoise_out = c->het ? c->dDnoise : nullptr;
+    pl.kp = c->kp;
+  }
   double flops = 0;
   for (int r = 0; r < nt; r++) flops += (double)(r + 1) * 2.0 * TILE * TILE * (double)(c->Npad - (long)r * TILE);
   int h = rec ? rec->begin(PH_LAUUM, flops) : -1;
@@ -577,182 +587,216 @@ static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec, bool plain = f
   return 0;
 }
 
-static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec) {
+// ---------------------------------------------------------------------------------------------------------------
+// point sets and K-builds, for either kind of covariance function: a single stationary kernel (`const KernParams* kp`) or
+// the context's composite kernel c->mk (kp == nullptr)
+// ---------------------------------------------------------------------------------------------------------------
+// Temporaries of the stand-alone kernel calls and of gpx_predict: stream-ordered allocations from the device's default memory
+// pool (cudaMallocAsync / cudaFreeAsync on the context's stream; gpx_create raises the pool's release threshold so that freed
+// blocks stay cached). A plain cudaMalloc / cudaFree pair per call is a device-wide synchronisation point inside any
+// optimiser loop that uses foreign inference (round-1 review).
+#define GPX_TMP_ALLOC(ptr, bytes, st) GPX_CUDA(cudaMallocAsync((void**)(ptr), (bytes), (st)))
+#define GPX_TMP_FREE(p, st) do { if (p) cudaFreeAsync((p), (st)); } while (0)
+
+// n points prepared for a kernel: scaled coordinates xT, SoA [D][ld] (composite: [sumD][ld]), and their squared norms sq,
+// [ld] (composite: [nparts][ld])
+struct Points { double* xT = nullptr; double* sq = nullptr; long n = 0, ld = 0; };
+
+// the kernel of the context's last evaluation, and its training points as build_Ky prepared them
+static const KernParams* ctx_kern(const gpx_ctx* c) { return c->multi ? nullptr : &c->kp; }
+static Points train_points(const gpx_ctx* c) {
+  return c->multi ? Points{c->mXsT, c->msq, c->N, c->Npad} : Points{c->dXsT, c->dsq, c->N, c->Npad};
+}
+
+static int prep_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, long ld, double* xT, double* sq) {
+  return kp ? launch_prep_x(X, n, ld, *kp, xT, sq, c->st) : launch_prep_multi(X, n, c->D, ld, c->mk, xT, sq, c->st);
+}
+
+struct PointSet : Points {   // host points uploaded and prepared in temporaries it owns
+  double* raw = nullptr;
+  cudaStream_t st = nullptr;
+  ~PointSet() { GPX_TMP_FREE(raw, st); GPX_TMP_FREE(xT, st); GPX_TMP_FREE(sq, st); }
+};
+// X: n points, row-major with kp->D columns (composite kernel: the context's D)
+static int upload_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, PointSet& ps) {
+  const int D = kp ? kp->D : c->D;
+  ps.n = n; ps.ld = (n + TILE - 1) / TILE * TILE; ps.st = c->st;
+  GPX_TMP_ALLOC(&ps.raw, (size_t)n * D * 8, c->st);
+  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * (kp ? kp->D : std::max(1, c->mk.sumD)) * 8, c->st);
+  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * (kp ? 1 : c->mk.nparts) * 8, c->st);
+  GPX_CUDA(cudaMemcpyAsync(ps.raw, X, (size_t)n * D * 8, cudaMemcpyHostToDevice, c->st));
+  GPX_CHECK(prep_points(c, kp, ps.raw, n, ps.ld, ps.xT, ps.sq));
+  c->total_launches++;
+  return 0;
+}
+
+struct KyDiag { double add; const double* vec; };   // added to the diagonal of Ky: a constant, and per-point values (or null)
+
+// K(rows, cols) into out[i + j * ld] (i: row point, j: column point), row tiles [rt0, rt0 + nrt) (nrt = 0: all of them;
+// a part of the rows: single kernel only). ky != nullptr: the factor workspace form of Ky (lower tiles, zero upper tiles,
+// identity padding, ky's diagonal terms).
+static int build_K(gpx_ctx* c, const KernParams* kp, const Points& rows, const Points& cols, double* out, long ld,
+                   const KyDiag* ky = nullptr, int rt0 = 0, int nrt = 0) {
+  const int row_tiles = nrt ? nrt : (int)(rows.ld / TILE), col_tiles = (int)(cols.ld / TILE);
+  const int same = rows.xT == cols.xT;   // one point set on both sides: exact zero distance on the diagonal
+  if (!kp) {
+    KBuildMultiParams kb;
+    memset(&kb, 0, sizeof(kb));
+    kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
+    kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
+    kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.mk = c->mk;
+    if (ky) { kb.sym = 1; kb.diag_add = ky->add; }
+    return launch_kbuild_multi(kb, row_tiles, col_tiles, c->st);
+  }
+  KBuildParams kb;
+  memset(&kb, 0, sizeof(kb));
+  kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
+  kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
+  kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.rt0 = rt0; kb.kp = *kp;
+  if (ky) { kb.sym = 1; kb.diag_add = ky->add; kb.diag_vec = ky->vec; }
+  return launch_kbuild(kb, row_tiles, col_tiles, c->st);
+}
+
+// Ky = K(X, X) + noise + jitter (+ the per-point noise) of the context's kernel into the workspace, training points
+// prepared first. On the int8 sweep a single kernel's first block row goes first and *first_rows is the event after it, so
+// that the factorisation of the first diagonal block runs beside the rest of the build; otherwise *first_rows = nullptr.
+static int build_Ky(gpx_ctx* c, double extra_jitter, bool int8, Recorder& rec, cudaEvent_t* first_rows) {
+  const int nt = (int)(c->Npad / TILE);
+  *first_rows = nullptr;
+  if (c->multi && c->m_cap != c->Npad) {
+    for (double** mp : {&c->mXsT, &c->msq, &c->mpartials}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
+    GPX_CUDA(cudaMalloc(&c->mXsT, (size_t)MAX_D * c->Npad * 8));
+    GPX_CUDA(cudaMalloc(&c->msq, (size_t)MAX_PARTS * c->Npad * 8));
+    GPX_CUDA(cudaMalloc(&c->mpartials, (size_t)MAX_PARTS * nt * nt * (MAX_D + 2) * 8));
+    c->m_cap = c->Npad;
+  }
+  const Points tr = train_points(c);
+  GPX_CHECK(prep_points(c, ctx_kern(c), c->dX, c->N, c->Npad, tr.xT, tr.sq));
+  c->eval_launches++;
+  const KyDiag ky{((c->het ? 0.0 : c->noise) + c->jitter) + extra_jitter, c->het ? c->dNoiseVec : nullptr};
+  const int h = rec.begin(PH_KBUILD);
+  if (int8 && !c->multi) {
+    const int nbt0 = (int)(pick_nb(c) / TILE);
+    GPX_CHECK(build_K(c, &c->kp, tr, tr, c->S, c->Npad, &ky, 0, nbt0));
+    if (!c->ev_kfirst) GPX_CUDA(cudaEventCreateWithFlags(&c->ev_kfirst, cudaEventDisableTiming));
+    GPX_CUDA(cudaEventRecord(c->ev_kfirst, c->st));
+    *first_rows = c->ev_kfirst;
+    GPX_CHECK(build_K(c, &c->kp, tr, tr, c->S, c->Npad, &ky, nbt0, nt - nbt0));
+    c->eval_launches++;
+  } else {
+    GPX_CHECK(build_K(c, ctx_kern(c), tr, tr, c->S, c->Npad, &ky));
+  }
+  rec.end(h);
+  c->eval_launches++;
+  return 0;
+}
+
+// Where K^-1 of one evaluation comes from; the gradient reductions follow from it
+enum KinvRoute {
+  KINV_FUSED,   // DMMA sweep, single kernel, nt > 8: the fused LAUUM epilogue reduces it, nothing is stored
+  KINV_FINE,    // DMMA sweep, single kernel, nt <= 8: fine LAUUM into c->Kinv
+  KINV_PLAIN,   // DMMA sweep, composite kernel (any nt): plain LAUUM into c->Kinv
+  KINV_SWEEP,   // int8 sweep: accumulated into c->Kinv panel by panel
+};
+
+// One evaluation on a single GPU (the sharded path is dist_exact_eval): build Ky -> sweep -> solve -> K^-1 per the route ->
+// gradient reductions (fused, or from the stored K^-1: grad_kinv, grad_kinv_multi per part) -> finalize. The results land
+// in c->h_res, the info flag in *c->h_info; *kinv_stored tells whether c->Kinv now holds K^-1.
+static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_stored) {
   cudaStream_t st = c->st;
   const long ld = c->Npad;
   const int nt = (int)(c->Npad / TILE);
   const int nl = c->kp.ard ? c->D : 1;
-  const bool oz = oz_wanted(c);
+  const bool int8 = oz_wanted(c);
+  const KinvRoute route = int8 ? KINV_SWEEP : c->multi ? KINV_PLAIN : nt <= 8 ? KINV_FINE : KINV_FUSED;
+  *kinv_stored = route != KINV_FUSED;
   GPX_CUDA(cudaMemsetAsync(c->info, 0, sizeof(int), st));
-  if (c->multi) {
-    if (c->m_cap != c->Npad) {
-      for (double** mp : {&c->mXsT, &c->msq, &c->mpartials}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
-      GPX_CUDA(cudaMalloc(&c->mXsT, (size_t)MAX_D * c->Npad * 8));
-      GPX_CUDA(cudaMalloc(&c->msq, (size_t)MAX_PARTS * c->Npad * 8));
-      GPX_CUDA(cudaMalloc(&c->mpartials, (size_t)MAX_PARTS * nt * nt * (MAX_D + 2) * 8));
-      c->m_cap = c->Npad;
-    }
-    GPX_CHECK(launch_prep_multi(c->dX, c->N, c->D, c->Npad, c->mk, c->mXsT, c->msq, st));
-    c->eval_launches++;
-    KBuildMultiParams kb;
-    memset(&kb, 0, sizeof(kb));
-    kb.rowsT = c->mXsT; kb.ld_rows = c->Npad; kb.sq_rows = c->msq;
-    kb.colsT = c->mXsT; kb.ld_cols = c->Npad; kb.sq_cols = c->msq;
-    kb.out = c->S; kb.ld = ld; kb.nrows = c->N; kb.ncols = c->N; kb.sym = 1; kb.same = 1;
-    kb.diag_add = (c->noise + c->jitter) + extra_jitter;
-    kb.mk = c->mk;
-    const int h = rec.begin(PH_KBUILD);
-    GPX_CHECK(launch_kbuild_multi(kb, nt, nt, st));
-    rec.end(h);
-    c->eval_launches++;
-  } else {
-  GPX_CHECK(launch_prep_x(c->dX, c->N, c->Npad, c->kp, c->dXsT, c->dsq, st));
-  c->eval_launches++;
-  {
-    KBuildParams kb;
-    memset(&kb, 0, sizeof(kb));
-    kb.rowsT = c->dXsT; kb.ld_rows = c->Npad;
-    kb.colsT = c->dXsT; kb.ld_cols = c->Npad;
-    kb.sq_rows = c->dsq; kb.sq_cols = c->dsq;
-    kb.out = c->S; kb.ld = ld;
-    kb.nrows = c->N; kb.ncols = c->N;
-    kb.sym = 1; kb.same = 1;
-    kb.diag_add = ((c->het ? 0.0 : c->noise) + c->jitter) + extra_jitter;
-    kb.diag_vec = c->het ? c->dNoiseVec : nullptr;
-    kb.kp = c->kp;
-    const int h = rec.begin(PH_KBUILD);
-    // Ozaki sweep: the first block row goes first and is announced by an event, so that the factorisation of the first
-    // diagonal block runs beside the rest of the covariance build
-    const int nbt0 = (int)(pick_nb(c) / TILE);
-    c->kfirst_valid = false;
-    if (oz) {
-      GPX_CHECK(launch_kbuild(kb, nbt0, nt, st));
-      if (!c->ev_kfirst) GPX_CUDA(cudaEventCreateWithFlags(&c->ev_kfirst, cudaEventDisableTiming));
-      GPX_CUDA(cudaEventRecord(c->ev_kfirst, st));
-      c->kfirst_valid = true;
-      kb.rt0 = nbt0;
-      GPX_CHECK(launch_kbuild(kb, nt - nbt0, nt, st));
-      c->eval_launches++;
-    } else {
-      GPX_CHECK(launch_kbuild(kb, nt, nt, st));
-    }
-    rec.end(h);
-    c->eval_launches++;
-  }
-  }
-  if (oz) GPX_CHECK(oz_prepare(c));
-  c->oz_last = oz;
+  cudaEvent_t first_rows;
+  GPX_CHECK(build_Ky(c, extra_jitter, int8, rec, &first_rows));
+  if (*kinv_stored) GPX_CHECK(ensure_kinv(c));
+  if (int8) GPX_CHECK(oz_prepare(c));
   {
     const int h = rec.begin(PH_SWEEP);
-    GPX_CHECK(oz ? run_sweep_chain(c, rec) : run_sweep(c, rec));
+    GPX_CHECK(int8 ? run_sweep_chain(c, rec, first_rows) : run_sweep(c, rec));
     rec.end(h);
   }
+  // alpha = U (U^T y). On the int8 sweep t = L^-1 y = U^T y came along with the sweep (forward substitution): one mat-vec
+  const double* T = int8 ? c->dTfw : c->dT;
   {
     const int h = rec.begin(PH_SOLVE);
-    // alpha = U (U^T y). On the Ozaki path t = L^-1 y = U^T y came along with the sweep (forward substitution): one mat-vec
-    if (!oz) GPX_CHECK(launch_utv(c->S, ld, c->Npad, c->P, c->dY, c->dT, st));
-    GPX_CHECK(launch_uv(c->S, ld, c->Npad, c->P, oz ? c->dTfw : c->dT, KSPLIT, c->dUvPart, c->dAlpha, st));
+    if (!int8) GPX_CHECK(launch_utv(c->S, ld, c->Npad, c->P, c->dY, c->dT, st));
+    GPX_CHECK(launch_uv(c->S, ld, c->Npad, c->P, T, KSPLIT, c->dUvPart, c->dAlpha, st));
     rec.end(h);
-    c->eval_launches += oz ? 2 : 3;
+    c->eval_launches += int8 ? 2 : 3;
+  }
+  auto mpart = [&](int q) { return c->mpartials + (size_t)q * nt * nt * (MAX_D + 2); };
+  long grad_tiles = (long)nt * nt;
+  if (route == KINV_FUSED) {
+    GPX_CHECK(run_lauum(c, nullptr, &rec));
+  } else {
+    if (route == KINV_PLAIN) GPX_CHECK(run_lauum(c, c->Kinv, &rec));
+    const int h = rec.begin(PH_LAUUM, 0.0);
+    if (route == KINV_FINE) {
+      // the fused LAUUM kernel has one CTA per 128 x 128 tile -- 10 CTAs for N = 512, each walking up to 512 k alone (136 us
+      // of a 0.48 ms evaluation); the fine LAUUM computes K^-1 = U U^T in 64 x 32 tiles (80 CTAs)
+      FineParams fl{};
+      fl.mode = FINE_LAUUM;
+      fl.A = c->S; fl.lda = ld; fl.B = c->S; fl.ldb = ld; fl.C = c->Kinv; fl.ldc = ld; fl.K = (int)c->Npad; fl.nt = nt;
+      GPX_CHECK(launch_fine(fl, st));
+      c->eval_launches++;
+    }
+    if (c->multi) {   // one reduction pass per part
+      for (int q = 0; q < c->mk.nparts; q++) {
+        const int nred = std::max(1, part_nl(c->mk.part[q])) + 2;
+        GPX_CUDA(cudaMemsetAsync(mpart(q), 0, (size_t)nt * nt * nred * 8, st));
+        GradKinvMultiParams gm;
+        memset(&gm, 0, sizeof(gm));
+        gm.Kinv = c->Kinv; gm.ld = ld; gm.XsT = c->mXsT; gm.sq = c->msq; gm.ldx = c->Npad; gm.alpha = c->dAlpha;
+        gm.N = c->N; gm.P = c->P; gm.nt = nt; gm.part = q; gm.want_noise = q == 0; gm.partials = mpart(q); gm.mk = c->mk;
+        GPX_CHECK(launch_grad_kinv_multi(gm, st));
+        c->eval_launches++;
+      }
+    } else {
+      const int csplit = grad_kinv_csplit(nt, nl + 2);
+      grad_tiles = (long)nt * nt * csplit;
+      GPX_CUDA(cudaMemsetAsync(c->partials, 0, (size_t)grad_tiles * (nl + 2) * 8, st));
+      GradKinvParams gk;
+      memset(&gk, 0, sizeof(gk));
+      gk.csplit = csplit;
+      gk.Kinv = c->Kinv; gk.ld = ld;
+      gk.XsT = c->dXsT; gk.sq = c->dsq; gk.alpha = c->dAlpha; gk.ldx = c->Npad;
+      gk.N = c->N; gk.P = c->P; gk.nt = nt;
+      gk.partials = c->partials;
+      gk.dnoise_out = c->het ? c->dDnoise : nullptr;
+      gk.kp = c->kp;
+      GPX_CHECK(launch_grad_kinv(gk, st));
+      c->eval_launches++;
+    }
+    rec.end(h);
   }
   if (c->multi) {
-    // composite kernel: K^-1 stored (by the sweep on the Ozaki path, else by a plain LAUUM), then one reduction pass per part
-    if (!oz) {
-      if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)ld * ld * 8));
-      GPX_CHECK(run_lauum(c, c->Kinv, &rec, true));
-    }
     FinalizeMultiParams fm;
     memset(&fm, 0, sizeof(fm));
-    const int h = rec.begin(PH_LAUUM, 0.0);
-    for (int q = 0; q < c->mk.nparts; q++) {
-      double* part = c->mpartials + (size_t)q * nt * nt * (MAX_D + 2);
-      const int nred = std::max(1, part_nl(c->mk.part[q])) + 2;
-      GPX_CUDA(cudaMemsetAsync(part, 0, (size_t)nt * nt * nred * 8, st));
-      GradKinvMultiParams gm;
-      memset(&gm, 0, sizeof(gm));
-      gm.Kinv = c->Kinv; gm.ld = ld; gm.XsT = c->mXsT; gm.sq = c->msq; gm.ldx = c->Npad; gm.alpha = c->dAlpha;
-      gm.N = c->N; gm.P = c->P; gm.nt = nt; gm.part = q; gm.want_noise = q == 0; gm.partials = part; gm.mk = c->mk;
-      GPX_CHECK(launch_grad_kinv_multi(gm, st));
-      c->eval_launches++;
-      fm.partials[q] = part;
-    }
-    rec.end(h);
+    for (int q = 0; q < c->mk.nparts; q++) fm.partials[q] = mpart(q);
     fm.ntiles = (long)nt * nt; fm.logdet_part = c->logdet_part; fm.nt = nt;
-    fm.T = oz ? c->dTfw : c->dT; fm.ld = ld; fm.N = c->N; fm.P = c->P; fm.mk = c->mk; fm.res = c->res;
+    fm.T = T; fm.ld = ld; fm.N = c->N; fm.P = c->P; fm.mk = c->mk; fm.res = c->res;
     GPX_CHECK(launch_finalize_multi(fm, st));
-    c->eval_launches++;
-    GPX_CUDA(cudaMemcpyAsync(c->h_res, c->res, (MAX_D + 2 * MAX_PARTS + 8) * sizeof(double), cudaMemcpyDeviceToHost, st));
-    GPX_CUDA(cudaMemcpyAsync(c->h_info, c->info, sizeof(int), cudaMemcpyDeviceToHost, st));
-    c->oz_last = true;   // K^-1 is stored either way
-    return 0;
-  }
-  long grad_tiles = (long)nt * nt;
-  if (oz) {
-    // K^-1 was accumulated panel by panel inside the sweep (Ozaki): reduce dL_dK -> gradients from the stored tiles
-    const int csplit = grad_kinv_csplit(nt, nl + 2);
-    grad_tiles = (long)nt * nt * csplit;
-    GPX_CUDA(cudaMemsetAsync(c->partials, 0, (size_t)grad_tiles * (nl + 2) * 8, st));
-    GradKinvParams gk;
-    memset(&gk, 0, sizeof(gk));
-    gk.csplit = csplit;
-    gk.Kinv = c->Kinv; gk.ld = ld;
-    gk.XsT = c->dXsT; gk.sq = c->dsq; gk.alpha = c->dAlpha; gk.ldx = c->Npad;
-    gk.N = c->N; gk.P = c->P; gk.nt = nt;
-    gk.partials = c->partials;
-    gk.dnoise_out = c->het ? c->dDnoise : nullptr;
-    gk.kp = c->kp;
-    const int h = rec.begin(PH_LAUUM, 0.0);
-    GPX_CHECK(launch_grad_kinv(gk, st));
-    rec.end(h);
-    c->eval_launches++;
-  } else if (nt <= 8 && !c->dist) {
-    // small matrix on the DMMA path (one block, or Ozaki switched off): the fused LAUUM kernel has one CTA per 128 x 128 tile
-    // -- 10 CTAs for N = 512, each walking up to 512 k alone (136 us of a 0.48 ms evaluation). K^-1 = U U^T in 64 x 32 tiles
-    // (80 CTAs) into the K^-1 buffer, then the gradient pass over the stored tiles, split over the columns
-    if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)ld * ld * 8));
-    const int h = rec.begin(PH_LAUUM, 0.0);
-    FineParams fl{};
-    fl.mode = FINE_LAUUM;
-    fl.A = c->S; fl.lda = ld; fl.B = c->S; fl.ldb = ld; fl.C = c->Kinv; fl.ldc = ld; fl.K = (int)c->Npad; fl.nt = nt;
-    GPX_CHECK(launch_fine(fl, st));
-    const int csplit = grad_kinv_csplit(nt, nl + 2);
-    grad_tiles = (long)nt * nt * csplit;
-    GPX_CUDA(cudaMemsetAsync(c->partials, 0, (size_t)grad_tiles * (nl + 2) * 8, st));
-    GradKinvParams gk;
-    memset(&gk, 0, sizeof(gk));
-    gk.csplit = csplit;
-    gk.Kinv = c->Kinv; gk.ld = ld;
-    gk.XsT = c->dXsT; gk.sq = c->dsq; gk.alpha = c->dAlpha; gk.ldx = c->Npad;
-    gk.N = c->N; gk.P = c->P; gk.nt = nt;
-    gk.partials = c->partials;
-    gk.dnoise_out = c->het ? c->dDnoise : nullptr;
-    gk.kp = c->kp;
-    GPX_CHECK(launch_grad_kinv(gk, st));
-    rec.end(h);
-    c->eval_launches += 2;
-    c->oz_last = true;   // K^-1 is stored
   } else {
-    GPX_CHECK(run_lauum(c, nullptr, &rec));
-  }
-  {
     FinalizeParams f;
     memset(&f, 0, sizeof(f));
     f.partials = c->partials; f.ntiles = grad_tiles; f.nl = nl;
     f.logdet_part = c->logdet_part; f.nt = nt;
-    f.T = oz ? c->dTfw : c->dT; f.ld = ld; f.N = c->N; f.P = c->P;
+    f.T = T; f.ld = ld; f.N = c->N; f.P = c->P;
     f.kp = c->kp;
     f.res = c->res;
     GPX_CHECK(launch_finalize(f, st));
-    c->eval_launches++;
   }
-  GPX_CUDA(cudaMemcpyAsync(c->h_res, c->res, (nl + 5) * sizeof(double), cudaMemcpyDeviceToHost, st));
+  c->eval_launches++;
+  const size_t nres = c->multi ? MAX_D + 2 * MAX_PARTS + 8 : nl + 5;
+  GPX_CUDA(cudaMemcpyAsync(c->h_res, c->res, nres * sizeof(double), cudaMemcpyDeviceToHost, st));
   GPX_CUDA(cudaMemcpyAsync(c->h_info, c->info, sizeof(int), cudaMemcpyDeviceToHost, st));
   return 0;
 }
-
-extern "C" {
-
-}  // extern "C"
 
 // noise_vec == nullptr: homoscedastic (`noise`); else N per-point variances (`noise` = their mean, used by the ladder)
 static int fill_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double* kdiag_total) {
@@ -831,12 +875,13 @@ static int exact_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const
   double extra = 0.0;
   int tries = 0;
   int info = 0;
+  bool kinv_stored = false;
   for (;;) {
     tries++;
     if (c->dist) {
       GPX_CHECK(dist_exact_eval(c, extra));
     } else {
-      GPX_CHECK(eval_once(c, extra, rec));
+      GPX_CHECK(eval_once(c, extra, rec, &kinv_stored));
       GPX_CUDA(cudaStreamSynchronize(c->st));
     }
     info = *c->h_info;
@@ -887,7 +932,7 @@ static int exact_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const
     GPX_CUDA(cudaStreamSynchronize(c->st));
   }
   c->have_eval = true;
-  c->have_kinv = c->oz_last;   // the Ozaki path leaves K^-1 (lower tiles) in c->Kinv
+  c->have_kinv = kinv_stored;
   return 0;
 }
 
@@ -960,27 +1005,16 @@ int gpx_get(gpx_ctx* c, int which, double* out) {
     return 0;
   }
   GPX_CHECK(ensure_staging(c));
-  if (which == GPX_GET_K && c->multi) {
-    KBuildMultiParams kb;
-    memset(&kb, 0, sizeof(kb));
-    kb.rowsT = c->mXsT; kb.ld_rows = ld; kb.sq_rows = c->msq; kb.colsT = c->mXsT; kb.ld_cols = ld; kb.sq_cols = c->msq;
-    kb.out = c->staging; kb.ld = N; kb.nrows = N; kb.ncols = N; kb.sym = 0; kb.same = 1; kb.mk = c->mk;
-    GPX_CHECK(launch_kbuild_multi(kb, (int)(ld / TILE), (int)(ld / TILE), st));
-    c->total_launches++;
-  } else if (which == GPX_GET_K) {
-    KBuildParams kb;
-    memset(&kb, 0, sizeof(kb));
-    kb.rowsT = c->dXsT; kb.ld_rows = ld; kb.colsT = c->dXsT; kb.ld_cols = ld;
-    kb.sq_rows = c->dsq; kb.sq_cols = c->dsq;
-    kb.out = c->staging; kb.ld = N; kb.nrows = N; kb.ncols = N; kb.sym = 0; kb.same = 1; kb.kp = c->kp;
-    GPX_CHECK(launch_kbuild(kb, (int)(ld / TILE), (int)(ld / TILE), st));
+  if (which == GPX_GET_K) {
+    const Points tr = train_points(c);
+    GPX_CHECK(build_K(c, ctx_kern(c), tr, tr, c->staging, N));
     c->total_launches++;
   } else if (which == GPX_GET_L || which == GPX_GET_LINV) {
     GPX_CHECK(launch_extract(which, c->S, ld, c->Ldiag, nullptr, nullptr, 0, N, c->staging, st));
     c->total_launches++;
   } else if (which == GPX_GET_KINV || which == GPX_GET_DLDK) {
-    if (!c->have_kinv) {
-      if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)ld * ld * 8));
+    if (!c->have_kinv) {   // the fused route reduced K^-1 without storing it: the plain LAUUM stores the same tiles
+      GPX_CHECK(ensure_kinv(c));
       const int64_t keep = c->eval_launches;
       GPX_CHECK(run_lauum(c, c->Kinv, nullptr));
       c->total_launches += c->eval_launches - keep;
@@ -1013,29 +1047,6 @@ static int scratch_ctx(gpx_ctx** out) {
   return 0;
 }
 
-// Temporaries of the stand-alone kernel calls and of gpx_predict: stream-ordered allocations from the device's default memory
-// pool (cudaMallocAsync / cudaFreeAsync on the context's stream; gpx_create raises the pool's release threshold so that freed
-// blocks stay cached). A plain cudaMalloc / cudaFree pair per call is a device-wide synchronisation point inside any
-// optimiser loop that uses foreign inference (round-1 review).
-#define GPX_TMP_ALLOC(ptr, bytes, st) GPX_CUDA(cudaMallocAsync((void**)(ptr), (bytes), (st)))
-#define GPX_TMP_FREE(p, st) do { if (p) cudaFreeAsync((p), (st)); } while (0)
-
-struct PointSet {
-  double* raw = nullptr; double* xT = nullptr; double* sq = nullptr; long n = 0, ld = 0;
-  cudaStream_t st = nullptr;
-  ~PointSet() { GPX_TMP_FREE(raw, st); GPX_TMP_FREE(xT, st); GPX_TMP_FREE(sq, st); }
-};
-static int upload_points(gpx_ctx* c, const double* X, long n, const KernParams& kp, PointSet& ps) {
-  ps.n = n; ps.ld = (n + TILE - 1) / TILE * TILE; ps.st = c->st;
-  GPX_TMP_ALLOC(&ps.raw, (size_t)n * kp.D * 8, c->st);
-  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * kp.D * 8, c->st);
-  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * 8, c->st);
-  GPX_CUDA(cudaMemcpyAsync(ps.raw, X, (size_t)n * kp.D * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(launch_prep_x(ps.raw, n, ps.ld, kp, ps.xT, ps.sq, c->st));
-  c->total_launches++;
-  return 0;
-}
-
 int gpx_kern_K(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
                const double* X2, int64_t M, int D, double* out) {
   if (!X || !lengthscale) GPX_FAIL("null argument");
@@ -1046,23 +1057,18 @@ int gpx_kern_K(gpx_ctx* c, int kind, int ard, double variance, const double* len
   if (!X2) M = N;
   if (N < 1 || M < 1) GPX_FAIL("empty input");
   PointSet p1, p2;
-  GPX_CHECK(upload_points(c, X, N, kp, p1));
-  if (X2) GPX_CHECK(upload_points(c, X2, M, kp, p2));
+  GPX_CHECK(upload_points(c, &kp, X, N, p1));
+  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
   PointSet& pj = X2 ? p2 : p1;   // thread-mapped operand = X2 points (contiguous index of the row-major output)
   double* dout = nullptr;
   GPX_TMP_ALLOC(&dout, (size_t)N * M * 8, c->st);
-  KBuildParams kb;
-  memset(&kb, 0, sizeof(kb));
-  kb.rowsT = pj.xT; kb.ld_rows = pj.ld; kb.sq_rows = pj.sq;
-  kb.colsT = p1.xT; kb.ld_cols = p1.ld; kb.sq_cols = p1.sq;
-  kb.out = dout; kb.ld = M; kb.nrows = M; kb.ncols = N; kb.sym = 0; kb.same = X2 ? 0 : 1; kb.kp = kp;
   // out == NULL: build on the device only (the result is dropped) and report the kernel time through gpx_get_stats
   // (kbuild_ms / kbuild_bytes) — used to measure the rectangular K(X, Z) build of the sparse model at full size.
   cudaEvent_t e0, e1;
   int rc = ev_get(c, 0, &e0) || ev_get(c, 1, &e1);
   if (rc == 0) {
     cudaEventRecord(e0, c->st);
-    rc = launch_kbuild(kb, (int)(pj.ld / TILE), (int)(p1.ld / TILE), c->st);
+    rc = build_K(c, &kp, pj, p1, dout, M);
     cudaEventRecord(e1, c->st);
   }
   c->total_launches++;
@@ -1093,8 +1099,8 @@ int gpx_kern_grad_full(gpx_ctx* c, int kind, int ard, double variance, const dou
   GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
   if (!X2) M = N;
   PointSet p1, p2;
-  GPX_CHECK(upload_points(c, X, N, kp, p1));
-  if (X2) GPX_CHECK(upload_points(c, X2, M, kp, p2));
+  GPX_CHECK(upload_points(c, &kp, X, N, p1));
+  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
   PointSet& pj = X2 ? p2 : p1;
   double* dd = nullptr; double* dpart = nullptr;
   const int tj = (int)(pj.ld / TILE), ti = (int)(p1.ld / TILE);
@@ -1131,8 +1137,8 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
   GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
   if (!X2) M = N;
   PointSet p1, p2;
-  GPX_CHECK(upload_points(c, X, N, kp, p1));
-  if (X2) GPX_CHECK(upload_points(c, X2, M, kp, p2));
+  GPX_CHECK(upload_points(c, &kp, X, N, p1));
+  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
   PointSet& pj = X2 ? p2 : p1;
   // m is split into chunks so that ~4 waves of CTAs are in flight; partials are reduced in fixed order
   const long ntile = (N + TILE - 1) / TILE;
@@ -1162,15 +1168,19 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
 // ---------------------------------------------------------------------------------------------------------------
 }  // extern "C"
 
+// size the workspace of c for an N x N matrix: bind N dummy points (D = 1, P = 1) unless such a data set is bound already
+static int bind_dummy_data(gpx_ctx* c, long N) {
+  if (c->N == N && c->D == 1 && c->P == 1 && c->S) return 0;
+  std::vector<double> zx((size_t)N, 0.0);
+  return gpx_set_data(c, zx.data(), N, 1, zx.data(), 1);
+}
+
 // Factor-and-invert a dense symmetric matrix that already lives on the device (dA, leading dimension lda, order N) into
 // the workspace of context c (lower = L, upper = U = L^-T), with jitchol's ladder (GPy/util/linalg.py:56-75):
 // jitter0 is always added; on failure mean(diag)*1e-6*10^k. Returns 0, or the failing minor (>0) / an error (<0).
 int gpx::factor_device(gpx_ctx* c, const double* dA, long lda, long N, double jitter0, int max_tries, double* logdet,
                        double* jitter_used) {
-  {
-    std::vector<double> zx((size_t)N, 0.0);
-    if (c->N != N || c->D != 1 || c->P != 1 || !c->S) GPX_CHECK(gpx_set_data(c, zx.data(), N, 1, zx.data(), 1));
-  }
+  GPX_CHECK(bind_dummy_data(c, N));
   c->have_eval = false;
   c->have_kinv = false;
   cudaStream_t st = c->st;
@@ -1225,15 +1235,12 @@ int gpx_pdinv(gpx_ctx* c, const double* A, int64_t N, int max_tries, double* Ai,
   if (c->dist) GPX_FAIL("gpx_pdinv is single-GPU");
   if (N < 1) GPX_FAIL("N must be positive");
   GPX_CUDA(cudaSetDevice(c->device));
-  {
-    std::vector<double> zx((size_t)N, 0.0);
-    if (c->N != N || c->D != 1 || c->P != 1 || !c->S) GPX_CHECK(gpx_set_data(c, zx.data(), N, 1, zx.data(), 1));
-  }
+  GPX_CHECK(bind_dummy_data(c, N));
   cudaStream_t st = c->st;
   const long ld = c->Npad;
   GPX_CHECK(ensure_staging(c));
   GPX_CUDA(cudaMemcpyAsync(c->staging, A, (size_t)N * N * 8, cudaMemcpyHostToDevice, st));
-  if (!c->Kinv) GPX_CUDA(cudaMalloc(&c->Kinv, (size_t)ld * ld * 8));
+  GPX_CHECK(ensure_kinv(c));
   // the factorisation reads the staged copy; the staging buffer is reused for the results afterwards
   double* dA = c->Kinv;   // park A in the K^-1 buffer (same size class) so that staging stays free for extraction
   GPX_CUDA(cudaMemcpyAsync(dA, c->staging, (size_t)N * N * 8, cudaMemcpyDeviceToDevice, st));
@@ -1243,15 +1250,7 @@ int gpx_pdinv(gpx_ctx* c, const double* A, int64_t N, int max_tries, double* Ai,
   }
   const int64_t l0 = c->eval_launches;
   if (Ai) {
-    const long ntl = ld / TILE;
-    GemmParams pl = gemm_defaults();
-    pl.mode = GEMM_LAUUM;
-    pl.A = c->S; pl.lda = ld; pl.B = c->S; pl.ldb = ld; pl.ldc = ld;
-    pl.K = (int)ld; pl.nt = (int)ntl; pl.N = (int)N; pl.P = 1;
-    pl.partials = nullptr; pl.kinv_out = c->Kinv;
-    pl.kp.D = 1;
-    GPX_CHECK(launch_gemm(pl, dim3(1, 1), st));
-    c->eval_launches++;
+    GPX_CHECK(run_lauum(c, c->Kinv, nullptr));
     GPX_CHECK(launch_extract(GPX_GET_KINV, c->S, ld, c->Ldiag, c->Kinv, nullptr, 0, N, c->staging, st));
     c->eval_launches++;
     GPX_CUDA(cudaMemcpyAsync(Ai, c->staging, (size_t)N * N * 8, cudaMemcpyDeviceToHost, st));
@@ -1290,36 +1289,14 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
   cudaStream_t st = c->st;
   const long ld = c->Npad, N = c->N;
   PointSet pn;
-  if (c->multi) {   // composite kernel: stacked per-part scaled coordinates of the new points
-    pn.n = M; pn.ld = (M + TILE - 1) / TILE * TILE; pn.st = c->st;
-    GPX_TMP_ALLOC(&pn.raw, (size_t)M * c->D * 8, c->st);
-    GPX_TMP_ALLOC(&pn.xT, (size_t)pn.ld * std::max(1, c->mk.sumD) * 8, c->st);
-    GPX_TMP_ALLOC(&pn.sq, (size_t)pn.ld * c->mk.nparts * 8, c->st);
-    GPX_CUDA(cudaMemcpyAsync(pn.raw, Xnew, (size_t)M * c->D * 8, cudaMemcpyHostToDevice, st));
-    GPX_CHECK(launch_prep_multi(pn.raw, M, c->D, pn.ld, c->mk, pn.xT, pn.sq, st));
-    c->total_launches++;
-  } else
-  GPX_CHECK(upload_points(c, Xnew, M, c->kp, pn));
+  GPX_CHECK(upload_points(c, ctx_kern(c), Xnew, M, pn));
   // Kx as [M][ld] (each new point one zero-padded column of length ld): thread-mapped operand = training points
   double* Kx = nullptr; double* Tx = nullptr;
   GPX_TMP_ALLOC(&Kx, (size_t)pn.ld * ld * 8, c->st);
   GPX_TMP_ALLOC(&Tx, (size_t)pn.ld * ld * 8, c->st);
   GPX_CUDA(cudaMemsetAsync(Kx, 0, (size_t)pn.ld * ld * 8, st));
   if (dG > 1) GPX_CUDA(cudaMemsetAsync(Tx, 0, (size_t)pn.ld * ld * 8, st));   // columns of other ranks stay zero
-  KBuildParams kb;
-  memset(&kb, 0, sizeof(kb));
-  kb.rowsT = c->dXsT; kb.ld_rows = ld; kb.sq_rows = c->dsq;
-  kb.colsT = pn.xT; kb.ld_cols = pn.ld; kb.sq_cols = pn.sq;
-  kb.out = Kx; kb.ld = ld; kb.nrows = N; kb.ncols = M; kb.sym = 0; kb.same = 0; kb.kp = c->kp;
-  int rc;
-  if (c->multi) {
-    KBuildMultiParams km;
-    memset(&km, 0, sizeof(km));
-    km.rowsT = c->mXsT; km.ld_rows = ld; km.sq_rows = c->msq; km.colsT = pn.xT; km.ld_cols = pn.ld; km.sq_cols = pn.sq;
-    km.out = Kx; km.ld = ld; km.nrows = N; km.ncols = M; km.sym = 0; km.same = 0; km.mk = c->mk;
-    rc = launch_kbuild_multi(km, (int)(ld / TILE), (int)(pn.ld / TILE), st);
-  } else
-  rc = launch_kbuild(kb, (int)(ld / TILE), (int)(pn.ld / TILE), st);
+  int rc = build_K(c, ctx_kern(c), train_points(c), pn, Kx, ld);
   c->total_launches++;
   // tmp = L^-1 Kx = U^T Kx, MAX_P columns per pass
   for (long m0 = 0; rc == 0 && m0 < M; m0 += MAX_P) {
@@ -1385,30 +1362,15 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
       for (long i = 0; i < N; i++) s += hK[m * ld + i] * hA[(size_t)q * ld + i];
       mu[m * c->P + q] = s;
     }
+  // K(Xnew, Xnew), built on the device from the prepared new points
   std::vector<double> kxx((size_t)M * M);
-  double lsv[MAX_D];
-  for (int q = 0; q < MAX_D; q++) lsv[q] = c->kp.ls[q];
-  if (c->multi) {   // K(Xnew, Xnew) of the composite kernel, built on the device
-    PointSet pm;
-    pm.n = M; pm.ld = (M + TILE - 1) / TILE * TILE; pm.st = c->st;
-    double* dk = nullptr;
-    GPX_TMP_ALLOC(&pm.raw, (size_t)M * c->D * 8, c->st);
-    GPX_TMP_ALLOC(&pm.xT, (size_t)pm.ld * std::max(1, c->mk.sumD) * 8, c->st);
-    GPX_TMP_ALLOC(&pm.sq, (size_t)pm.ld * c->mk.nparts * 8, c->st);
-    GPX_TMP_ALLOC(&dk, (size_t)M * M * 8, c->st);
-    GPX_CUDA(cudaMemcpyAsync(pm.raw, Xnew, (size_t)M * c->D * 8, cudaMemcpyHostToDevice, st));
-    rc = launch_prep_multi(pm.raw, M, c->D, pm.ld, c->mk, pm.xT, pm.sq, st);
-    KBuildMultiParams km;
-    memset(&km, 0, sizeof(km));
-    km.rowsT = pm.xT; km.ld_rows = pm.ld; km.sq_rows = pm.sq; km.colsT = pm.xT; km.ld_cols = pm.ld; km.sq_cols = pm.sq;
-    km.out = dk; km.ld = M; km.nrows = M; km.ncols = M; km.sym = 0; km.same = 1; km.mk = c->mk;
-    if (rc == 0) rc = launch_kbuild_multi(km, (int)(pm.ld / TILE), (int)(pm.ld / TILE), st);
-    c->total_launches += 2;
-    if (rc == 0 && cudaMemcpyAsync(kxx.data(), dk, (size_t)M * M * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) rc = -1;
-    if (cudaStreamSynchronize(st) != cudaSuccess) { gpx::set_error("gpx_predict: device failure"); rc = -1; }
-    GPX_TMP_FREE(dk, c->st);
-  } else
-  rc = gpx_kern_K(c, c->kp.kind, c->kp.ard, c->kp.variance, lsv, Xnew, M, nullptr, M, c->D, kxx.data());
+  double* dk = nullptr;
+  GPX_TMP_ALLOC(&dk, (size_t)M * M * 8, c->st);
+  rc = build_K(c, ctx_kern(c), pn, pn, dk, M);
+  c->total_launches++;
+  if (rc == 0 && cudaMemcpyAsync(kxx.data(), dk, (size_t)M * M * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) rc = -1;
+  if (cudaStreamSynchronize(st) != cudaSuccess) { gpx::set_error("gpx_predict: device failure"); rc = -1; }
+  GPX_TMP_FREE(dk, c->st);
   if (rc) return rc;
   for (long a = 0; a < M; a++)
     for (long b = 0; b < M; b++) var[a + b * M] = kxx[a * M + b] - ssq[a + b * M];

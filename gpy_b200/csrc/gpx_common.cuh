@@ -119,6 +119,12 @@ void set_error(const std::string& msg);
       return -1;                                                                                        \
     }                                                                                                   \
   } while (0)
+// propagate the non-zero return code of a host call
+#define GPX_CHECK(x)            \
+  do {                          \
+    int rc__ = (x);             \
+    if (rc__ != 0) return rc__; \
+  } while (0)
 
 // GEMM launch descriptor (see gpx_gemm.cu)
 enum GemmMode { GEMM_UPDATE = 0, GEMM_PANEL = 1, GEMM_LAUUM = 2 };

@@ -15,8 +15,8 @@ struct gpx_ctx {
   cudaStream_t st2 = nullptr;   // high-priority side stream: diagonal-block work + panel of the NEXT step (look-ahead)
   cudaStream_t st3 = nullptr;   // high-priority third stream of the Ozaki sweep: rest of the panel, digit split, copy-back, forward
                                 // substitution -- everything of step k that the NEXT diagonal block does not wait for
-  cudaEvent_t ev_kfirst = nullptr;   // Ozaki sweep: the first block row of the covariance build is done (D(0) may start)
-  bool kfirst_valid = false;
+  cudaEvent_t ev_kfirst = nullptr;   // int8 sweep, single kernel: recorded by the Ky build after its first block row, which
+                                     // is all D(0) needs; passed on to the sweep by the evaluation that recorded it
   std::vector<cudaEvent_t> sync_ev;
   // data
   long N = 0, Npad = 0;
@@ -40,13 +40,13 @@ struct gpx_ctx {
   double* res = nullptr;     // device result vector
   double* h_res = nullptr;   // pinned
   int* h_info = nullptr;     // pinned
-  double* Kinv = nullptr;    // lazy, Npad x Npad (lower tiles)
+  double* Kinv = nullptr;    // lazy (ensure_kinv), Npad x Npad (lower tiles)
   double* staging = nullptr; // lazy, N x N dense
   size_t staging_cap = 0;
   long NB = 0;               // outer block (0 = auto)
   // last evaluation
   bool have_eval = false;
-  bool have_kinv = false;
+  bool have_kinv = false;    // c->Kinv holds K^-1 of the last evaluation (its route stored it, or gpx_get made it)
   gpx::KernParams kp{};
   double noise = 0, jitter = 0, jitter_extra = 0;
   // heteroscedastic evaluation (gpx_exact_eval_het): per-point noise variances in, diag(dL_dK) out
@@ -61,7 +61,7 @@ struct gpx_ctx {
   // ---- Ozaki path (gpx_ozaki.cu): trailing update and K^-1 on the INT8 tensor cores ------------------------
   int ozaki = -1;              // option "ozaki": -1 = default (env GPX_OZAKI, else off), 0 = DMMA only, 1 = on where applicable
   int num_sms = 132;
-  bool oz_ready = false;       // planes and K^-1 buffer allocated for (Npad, NB)
+  bool oz_ready = false;       // planes and right-hand-side buffers allocated for (Npad, NB)
   bool oz_lists_ready = false; // tile lists built for (Npad, NB)
   gpx::OzPlanes ozp[2];        // digit planes of the current / next panel (look-ahead double buffer)
   gpx::OzPlanes ozpA, ozpB;    // operands of the panel GEMM P = S(:, block) L_kk^-T on the tensor cores (from N = 4096): block
@@ -71,9 +71,8 @@ struct gpx_ctx {
   double* dTfw = nullptr;      // [P][Npad] t = L^-1 y from that substitution (quadratic form of the LML)
   using OzStep = gpx::OzStep;
   std::vector<OzStep> oz_steps;
-  bool oz_last = false;        // the last evaluation went through the Ozaki path (K^-1 already stored)
-  // ---- composite kernels (gpx_multi.cu): the last evaluation used gpx_exact_eval_multi --------------------------------
-  bool multi = false;
+  // ---- composite kernels (gpx_multi.cu) ---------------------------------------------------------------------------------
+  bool multi = false;          // the last evaluation used gpx_exact_eval_multi: K-builds use mk, mXsT and msq
   gpx::MultiKern mk{};
   double* mXsT = nullptr;      // [sumD][Npad] stacked scaled inputs of the parts
   double* msq = nullptr;       // [nparts][Npad]
@@ -87,8 +86,10 @@ struct gpx_ctx {
 namespace gpx {
 constexpr int KSPLIT = 32;
 GemmParams gemm_defaults();
+void free_data(gpx_ctx* c);                                  // every buffer sized by the data set
+int alloc_data(gpx_ctx* c, long NB);                         // those of them whose size does not depend on the layout
 // multi-GPU hooks implemented in gpx_dist.cu
-int dist_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y, int P);
+int dist_set_data(gpx_ctx* c, int64_t N, int D, int P);      // (re)allocates the sharded layout for N points
 int dist_exact_eval(gpx_ctx* c, double extra_jitter);
 void dist_free(gpx_ctx* c);
 int dist_get_L(gpx_ctx* c, double* out);                                       // collective: sharded woodbury_chol

@@ -92,11 +92,6 @@ int load_nccl() {
       return -4;                                                                                             \
     }                                                                                                        \
   } while (0)
-#define GPX_CHECK(x)            \
-  do {                          \
-    int rc__ = (x);             \
-    if (rc__ != 0) return rc__; \
-  } while (0)
 
 struct DistState {
   ncclComm_t comm = nullptr;
@@ -190,52 +185,29 @@ static long dist_pick_nb(const gpx_ctx* c, long N) {
   return 256;
 }
 
-int dist_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y, int P) {
+int dist_set_data(gpx_ctx* c, int64_t N, int D, int P) {
   DistState* d = c->dist;
   const long NB = std::min<long>(dist_pick_nb(c, N), (N + TILE - 1) / TILE * TILE);
   const long Npad = (N + NB - 1) / NB * NB;      // whole blocks: every rank sees the same block structure
   const long nblk = Npad / NB, npr = (nblk + d->G - 1) / d->G;
   if (Npad != c->Npad || D != c->D || P != c->P || NB != d->NB) {
     GPX_CUDA(cudaStreamSynchronize(c->st));
-    // release the single-GPU style allocations of this context
-    double** ptrs[] = {&c->dX, &c->dXsT, &c->dsq, &c->dY, &c->dT, &c->dAlpha, &c->dUvPart, &c->S, &c->Pbuf, &c->Tm,
-                       &c->Ldiag, &c->Dinv, &c->logdet_part, &c->partials, &c->Kinv, &c->staging};
-    for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
-    c->staging_cap = 0;
+    free_data(c);   // also whatever single-GPU work allocated on this context before the communicator came
     dist_free(c);
     c->Npad = Npad; c->D = D; c->P = P;
     d->NB = NB; d->nblk = nblk; d->npr = npr;
-    const long nt = Npad / TILE;
-    GPX_CUDA(cudaMalloc(&c->dX, (size_t)Npad * D * 8));
-    GPX_CUDA(cudaMalloc(&c->dXsT, (size_t)Npad * D * 8));
-    GPX_CUDA(cudaMalloc(&c->dsq, (size_t)Npad * 8));
-    GPX_CUDA(cudaMalloc(&c->dY, (size_t)Npad * P * 8));
-    GPX_CUDA(cudaMalloc(&c->dT, (size_t)Npad * P * 8));
-    GPX_CUDA(cudaMalloc(&c->dAlpha, (size_t)Npad * P * 8));
+    GPX_CHECK(alloc_data(c, NB));
     GPX_CUDA(cudaMalloc(&c->dUvPart, (size_t)Npad * P * 8));
     d->ldl = npr * NB;
     GPX_CUDA(cudaMalloc(&c->S, (size_t)d->ldl * Npad * 8));       // owned block rows only
     GPX_CUDA(cudaMalloc(&d->SU, (size_t)Npad * d->ldl * 8));      // owned column blocks of U only
     GPX_CUDA(cudaMemsetAsync(d->SU, 0, (size_t)Npad * d->ldl * 8, c->st));
     GPX_CUDA(cudaMalloc(&c->Pbuf, (size_t)2 * d->G * npr * NB * NB * 8));   // double-buffered (look-ahead)
-    GPX_CUDA(cudaMalloc(&c->Tm, (size_t)NB * NB * 8));
     GPX_CUDA(cudaMalloc(&d->Bc, (size_t)NB * NB * 8));
     GPX_CUDA(cudaMalloc(&d->Bc2, (size_t)NB * NB * 8));
-    GPX_CUDA(cudaMalloc(&c->Ldiag, (size_t)Npad * TILE * 8));
-    GPX_CUDA(cudaMalloc(&c->Dinv, (size_t)Npad * TILE * 8));
-    GPX_CUDA(cudaMalloc(&c->logdet_part, (size_t)nt * 8));
-    GPX_CUDA(cudaMalloc(&c->partials, (size_t)nt * nt * (MAX_D + 2) * 8));
     GPX_CUDA(cudaMalloc(&d->blkpart, (size_t)nblk * P * Npad * 8));
     GPX_CUDA(cudaMemsetAsync(c->Pbuf, 0, (size_t)2 * d->G * npr * NB * NB * 8, c->st));
   }
-  c->N = N;
-  c->have_eval = false;
-  c->have_kinv = false;
-  GPX_CUDA(cudaMemcpyAsync(c->dX, X, (size_t)N * D * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CUDA(cudaMemcpyAsync(c->dT, Y, (size_t)N * P * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(launch_transpose_pad(c->dT, N, P, Npad, c->dY, c->st));
-  c->total_launches += 1;
-  GPX_CUDA(cudaStreamSynchronize(c->st));
   return 0;
 }
 

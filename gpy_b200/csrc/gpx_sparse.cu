@@ -25,11 +25,6 @@ using namespace gpx;
 static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double* dvariance, double* dlengthscale,
                             double* dZ);
 
-#define GPX_CHECK(x)            \
-  do {                          \
-    int rc__ = (x);             \
-    if (rc__ != 0) return rc__; \
-  } while (0)
 #define GPX_FAIL(msg)       \
   do {                      \
     gpx::set_error(msg);    \

@@ -23,7 +23,8 @@ change of a threshold fails here instead of quietly moving a case to another rou
 | multi-dmma: composite kernel, plain LAUUM + `grad_kinv_multi`  | 700, 2049                                              |
 | multi-int8: composite kernel, int8 sweep + `grad_kinv_multi`   | 2049                                                   |
 | jitter ladder, first failing minor in block k > 0           | test_ladder_fails_in_a_later_block (both paths)         |
-| context reuse                                                | N 1700 -> 1650 (same Npad), ozaki 1 -> 0 -> 1, P 1 -> 3 |
+| context reuse                                                | N 1700 -> 1650 (same Npad), ozaki 1 -> 0 -> 1, P 1 -> 3, |
+|                                                              | int8 single kernel -> int8 composite kernel            |
 | `gpx_pdinv` multi-block                                      | 2049, 4097: noisy kernel, graded D A D, non-PD tail    |
 
 The fine-LAUUM route with one block (N <= 512) is covered by tests/test_gpu_parity.py.
@@ -335,6 +336,41 @@ def test_reuse_with_more_outputs(oz):
         st = check_eval(e, X, Y[:, :P], "exponential", True, var, ls, noise, oz == 1)
         assert_route(st, "int8-dmmapanel" if oz else "dmma-fused", 6)
     e.close()
+
+
+@pytest.mark.gpu
+def test_composite_after_single_kernel_on_the_int8_path():
+    """A single-kernel evaluation on the int8 path, then a composite one on the same engine and data: the composite result
+    must be bit for bit that of a fresh engine. The single-kernel build of Ky announces its first block row by an event, and
+    the first diagonal block of the int8 sweep starts after it; the composite build is one launch, and the sweep after it
+    must wait for all of it. An engine that kept the earlier evaluation's event would start D(0) while block row 0 is still
+    being written; this test may still pass there by timing luck. What rules the race out is that the event is handed from
+    the build to the sweep of the same evaluation."""
+    from test_gpu_parity import _composite_case
+    N, D = 2049, 5
+    X, Y = o.synthetic(N, D, seed=N)
+    _, parts = _composite_case(D)
+    tup = [(p["kind"], p.get("ARD", False), p["term"], p["dims"], p["variance"], p.get("lengthscale")) for p in parts]
+    fresh = engine(1, 0)
+    fresh.set_data(X, Y)
+    lml_f, g_f, _ = fresh.exact_eval_multi(tup, 0.04)
+    assert_route(fresh.stats(), "multi-int8", 5)
+    kinv_f = fresh.get("Kinv")
+    fresh.close()
+    e = engine(1, 0)
+    e.set_data(X, Y)
+    var, ls, noise = theta(D, True, 3)
+    e.exact_eval("rbf", True, var, ls, noise)
+    assert_route(e.stats(), "int8-dmmapanel", 5)
+    lml, g, _ = e.exact_eval_multi(tup, 0.04)
+    assert_route(e.stats(), "multi-int8", 5)
+    assert lml == lml_f and np.array_equal(g, g_f)
+    assert np.array_equal(e.get("Kinv"), kinv_f)
+    e.close()
+    lml0, g0, res = o.composite_eval_lml_grad(X, Y, parts, 0.04)
+    assert abs(lml - lml0) <= LML_ATOL
+    np.testing.assert_allclose(g, g0, rtol=GRAD_RTOL, atol=1e-9)
+    assert rel(kinv_f, res["Wi"]) < 1e-8
 
 
 @pytest.mark.gpu
