@@ -25,13 +25,6 @@ void set_error(const std::string& msg) { g_err = msg; }
 
 using namespace gpx;
 
-#define GPX_FAIL(msg)       \
-  do {                      \
-    gpx::set_error(msg);    \
-    return -2;              \
-  } while (0)
-
-
 void gpx::free_data(gpx_ctx* c) {
   double** ptrs[] = {&c->dX, &c->dXsT, &c->dsq, &c->dY, &c->dT, &c->dAlpha, &c->dUvPart, &c->S, &c->Pbuf, &c->Tm,
                      &c->Ldiag, &c->Dinv, &c->logdet_part, &c->partials, &c->Kinv, &c->staging};
@@ -587,74 +580,10 @@ static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec) {
   return 0;
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// point sets and K-builds, for either kind of covariance function: a single stationary kernel (`const KernParams* kp`) or
-// the context's composite kernel c->mk (kp == nullptr)
-// ---------------------------------------------------------------------------------------------------------------
-// Temporaries of the stand-alone kernel calls and of gpx_predict: stream-ordered allocations from the device's default memory
-// pool (cudaMallocAsync / cudaFreeAsync on the context's stream; gpx_create raises the pool's release threshold so that freed
-// blocks stay cached). A plain cudaMalloc / cudaFree pair per call is a device-wide synchronisation point inside any
-// optimiser loop that uses foreign inference (round-1 review).
-#define GPX_TMP_ALLOC(ptr, bytes, st) GPX_CUDA(cudaMallocAsync((void**)(ptr), (bytes), (st)))
-#define GPX_TMP_FREE(p, st) do { if (p) cudaFreeAsync((p), (st)); } while (0)
-
-// n points prepared for a kernel: scaled coordinates xT, SoA [D][ld] (composite: [sumD][ld]), and their squared norms sq,
-// [ld] (composite: [nparts][ld])
-struct Points { double* xT = nullptr; double* sq = nullptr; long n = 0, ld = 0; };
-
 // the kernel of the context's last evaluation, and its training points as build_Ky prepared them
 static const KernParams* ctx_kern(const gpx_ctx* c) { return c->multi ? nullptr : &c->kp; }
 static Points train_points(const gpx_ctx* c) {
   return c->multi ? Points{c->mXsT, c->msq, c->N, c->Npad} : Points{c->dXsT, c->dsq, c->N, c->Npad};
-}
-
-static int prep_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, long ld, double* xT, double* sq) {
-  return kp ? launch_prep_x(X, n, ld, *kp, xT, sq, c->st) : launch_prep_multi(X, n, c->D, ld, c->mk, xT, sq, c->st);
-}
-
-struct PointSet : Points {   // host points uploaded and prepared in temporaries it owns
-  double* raw = nullptr;
-  cudaStream_t st = nullptr;
-  ~PointSet() { GPX_TMP_FREE(raw, st); GPX_TMP_FREE(xT, st); GPX_TMP_FREE(sq, st); }
-};
-// X: n points, row-major with kp->D columns (composite kernel: the context's D)
-static int upload_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, PointSet& ps) {
-  const int D = kp ? kp->D : c->D;
-  ps.n = n; ps.ld = (n + TILE - 1) / TILE * TILE; ps.st = c->st;
-  GPX_TMP_ALLOC(&ps.raw, (size_t)n * D * 8, c->st);
-  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * (kp ? kp->D : std::max(1, c->mk.sumD)) * 8, c->st);
-  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * (kp ? 1 : c->mk.nparts) * 8, c->st);
-  GPX_CUDA(cudaMemcpyAsync(ps.raw, X, (size_t)n * D * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(prep_points(c, kp, ps.raw, n, ps.ld, ps.xT, ps.sq));
-  c->total_launches++;
-  return 0;
-}
-
-struct KyDiag { double add; const double* vec; };   // added to the diagonal of Ky: a constant, and per-point values (or null)
-
-// K(rows, cols) into out[i + j * ld] (i: row point, j: column point), row tiles [rt0, rt0 + nrt) (nrt = 0: all of them;
-// a part of the rows: single kernel only). ky != nullptr: the factor workspace form of Ky (lower tiles, zero upper tiles,
-// identity padding, ky's diagonal terms).
-static int build_K(gpx_ctx* c, const KernParams* kp, const Points& rows, const Points& cols, double* out, long ld,
-                   const KyDiag* ky = nullptr, int rt0 = 0, int nrt = 0) {
-  const int row_tiles = nrt ? nrt : (int)(rows.ld / TILE), col_tiles = (int)(cols.ld / TILE);
-  const int same = rows.xT == cols.xT;   // one point set on both sides: exact zero distance on the diagonal
-  if (!kp) {
-    KBuildMultiParams kb;
-    memset(&kb, 0, sizeof(kb));
-    kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
-    kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
-    kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.mk = c->mk;
-    if (ky) { kb.sym = 1; kb.diag_add = ky->add; }
-    return launch_kbuild_multi(kb, row_tiles, col_tiles, c->st);
-  }
-  KBuildParams kb;
-  memset(&kb, 0, sizeof(kb));
-  kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
-  kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
-  kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.rt0 = rt0; kb.kp = *kp;
-  if (ky) { kb.sym = 1; kb.diag_add = ky->add; kb.diag_vec = ky->vec; }
-  return launch_kbuild(kb, row_tiles, col_tiles, c->st);
 }
 
 // Ky = K(X, X) + noise + jitter (+ the per-point noise) of the context's kernel into the workspace, training points
@@ -1101,31 +1030,14 @@ int gpx_kern_grad_full(gpx_ctx* c, int kind, int ard, double variance, const dou
   PointSet p1, p2;
   GPX_CHECK(upload_points(c, &kp, X, N, p1));
   if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
-  PointSet& pj = X2 ? p2 : p1;
-  double* dd = nullptr; double* dpart = nullptr;
-  const int tj = (int)(pj.ld / TILE), ti = (int)(p1.ld / TILE);
-  const int nl = ard ? D : 1, nred = nl + 1;
+  double *dd = nullptr, *dpart = nullptr;
   GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
-  GPX_TMP_ALLOC(&dpart, (size_t)tj * ti * nred * 8, c->st);
+  const GradFullParams gp = grad_params(kp, p1, X2 ? p2 : p1, dd, 0);
+  GPX_TMP_ALLOC(&dpart, grad_full_doubles(gp) * 8, c->st);
   GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
-  GradFullParams gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.x1T = p1.xT; gp.ld1 = p1.ld; gp.sq1 = p1.sq; gp.N = N;
-  gp.x2T = pj.xT; gp.ld2 = pj.ld; gp.sq2 = pj.sq; gp.M = M;
-  gp.dL_dK = dd; gp.same = X2 ? 0 : 1; gp.partials = dpart; gp.kp = kp;
-  int rc = launch_grad_full(gp, tj, ti, c->st);
-  c->total_launches++;
-  std::vector<double> hp((size_t)tj * ti * nred);
-  if (rc == 0 && cudaMemcpyAsync(hp.data(), dpart, hp.size() * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
-  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error("gpx_kern_grad_full: device failure"); rc = -1; }
+  const int rc = grad_full_sum(c, gp, dpart, dvariance, dlengthscale);
   GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
-  if (rc) return rc;
-  std::vector<double> tot(nred, 0.0);
-  for (size_t t = 0; t < (size_t)tj * ti; t++)
-    for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
-  *dvariance = tot[0];
-  for (int q = 0; q < nl; q++) dlengthscale[q] = -tot[1 + q] / lengthscale[q];
-  return 0;
+  return rc;
 }
 
 int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
@@ -1139,27 +1051,13 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
   PointSet p1, p2;
   GPX_CHECK(upload_points(c, &kp, X, N, p1));
   if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
-  PointSet& pj = X2 ? p2 : p1;
-  // m is split into chunks so that ~4 waves of CTAs are in flight; partials are reduced in fixed order
-  const long ntile = (N + TILE - 1) / TILE;
-  int nchunk = (int)std::max<long>(1, std::min<long>((M + 31) / 32, (4 * c->num_sms + ntile - 1) / ntile));
-  const long mchunk = ((M + nchunk - 1) / nchunk + 31) / 32 * 32;
-  nchunk = (int)((M + mchunk - 1) / mchunk);
-  double *dd = nullptr, *dpart = nullptr, *dout = nullptr;
+  double *dd = nullptr, *dpart = nullptr;
   GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
-  GPX_TMP_ALLOC(&dpart, (size_t)nchunk * N * D * 8, c->st);
-  GPX_TMP_ALLOC(&dout, (size_t)N * D * 8, c->st);
+  const GradFullParams gp = grad_params(kp, p1, X2 ? p2 : p1, dd, 0);
+  GPX_TMP_ALLOC(&dpart, grad_X_doubles(c, gp) * 8, c->st);
   GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
-  GradFullParams gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.x1T = p1.xT; gp.ld1 = p1.ld; gp.sq1 = p1.sq; gp.N = N;
-  gp.x2T = pj.xT; gp.ld2 = pj.ld; gp.sq2 = pj.sq; gp.M = M;
-  gp.dL_dK = dd; gp.same = X2 ? 0 : 1; gp.kp = kp;
-  int rc = launch_gradx(gp, nchunk, mchunk, dpart, dout, c->st);
-  c->total_launches += 2;
-  if (rc == 0 && cudaMemcpyAsync(grad, dout, (size_t)N * D * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
-  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error("gpx_kern_grad_X: device failure"); rc = -1; }
-  GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st); GPX_TMP_FREE(dout, c->st);
+  const int rc = grad_X(c, gp, dpart, grad);
+  GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
   return rc;
 }
 

@@ -125,6 +125,12 @@ void set_error(const std::string& msg);
     int rc__ = (x);             \
     if (rc__ != 0) return rc__; \
   } while (0)
+// reject an argument: the message goes to gpx_last_error, the call returns -2
+#define GPX_FAIL(msg)       \
+  do {                      \
+    gpx::set_error(msg);    \
+    return -2;              \
+  } while (0)
 
 // GEMM launch descriptor (see gpx_gemm.cu)
 enum GemmMode { GEMM_UPDATE = 0, GEMM_PANEL = 1, GEMM_LAUUM = 2 };

@@ -3,6 +3,7 @@
 #include <vector>
 
 #include "gpx_common.cuh"
+#include "gpx_kernels.cuh"
 #include "gpx_ozaki.cuh"
 #include "gpx_multi.cuh"
 
@@ -101,4 +102,43 @@ void sparse_free(gpx_ctx* c);
 int factor_device(gpx_ctx* c, const double* dA, long lda, long N, double jitter0, int max_tries, double* logdet,
                   double* jitter_used);
 int fill_kp(KernParams& kp, int kind, int ard, int D, double variance, const double* ls);
+
+// ---- point sets, K-builds and kernel-gradient reductions (gpx_points.cu) ----------------------------------------------
+// Temporaries of the stand-alone kernel calls and of gpx_predict: stream-ordered allocations from the device's default memory
+// pool (cudaMallocAsync / cudaFreeAsync on the context's stream; gpx_create raises the pool's release threshold so that freed
+// blocks stay cached). A plain cudaMalloc / cudaFree pair per call is a device-wide synchronisation point inside any
+// optimiser loop that uses foreign inference.
+#define GPX_TMP_ALLOC(ptr, bytes, st) GPX_CUDA(cudaMallocAsync((void**)(ptr), (bytes), (st)))
+#define GPX_TMP_FREE(p, st) do { if (p) cudaFreeAsync((p), (st)); } while (0)
+
+// n points prepared for a kernel: scaled coordinates xT, SoA [D][ld] (composite: [sumD][ld]), and their squared norms sq,
+// [ld] (composite: [nparts][ld])
+struct Points { double* xT = nullptr; double* sq = nullptr; long n = 0, ld = 0; };
+struct PointSet : Points {   // host points uploaded and prepared in temporaries it owns
+  double* raw = nullptr;
+  cudaStream_t st = nullptr;
+  ~PointSet() { GPX_TMP_FREE(raw, st); GPX_TMP_FREE(xT, st); GPX_TMP_FREE(sq, st); }
+};
+struct KyDiag { double add; const double* vec; };   // added to the diagonal of Ky: a constant, and per-point values (or null)
+
+// The K-build and prep launches are counted by the caller (into eval_launches inside an exact evaluation); the other
+// helpers count theirs into c->total_launches.
+int prep_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, long ld, double* xT, double* sq);
+// X: n points, row-major with kp->D columns (composite kernel: the context's D)
+int upload_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, PointSet& ps);
+// K(rows, cols) into out[i + j * ld] (i: row point, j: column point), row tiles [rt0, rt0 + nrt) (nrt = 0: all of them;
+// a part of the rows: single kernel only). ky != nullptr: the factor workspace form of Ky (lower tiles, zero upper tiles,
+// identity padding, ky's diagonal terms).
+int build_K(gpx_ctx* c, const KernParams* kp, const Points& rows, const Points& cols, double* out, long ld,
+            const KyDiag* ky = nullptr, int rt0 = 0, int nrt = 0);
+// dL_dK (device; element (i, j) of rows x cols at dL_dK[i * ldd + j], ldd = 0: cols.n) for the reductions below; the caller
+// may add the rank-P term or the transposed read
+GradFullParams grad_params(const KernParams& kp, const Points& rows, const Points& cols, const double* dL_dK, long ldd);
+// update_gradients_full: one row of partial sums per tile into `part` (grad_full_doubles), summed on the host in tile order
+size_t grad_full_doubles(const GradFullParams& gp);
+int grad_full_sum(gpx_ctx* c, GradFullParams gp, double* part, double* dvariance, double* dlengthscale);
+// gradients_X w.r.t. the row points: chunk partials and the N x D result in `part` (grad_X_doubles); the result is copied
+// to `out` on the host
+size_t grad_X_doubles(const gpx_ctx* c, const GradFullParams& gp);
+int grad_X(gpx_ctx* c, const GradFullParams& gp, double* part, double* out);
 }  // namespace gpx

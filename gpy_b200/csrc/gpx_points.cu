@@ -1,0 +1,108 @@
+// gpx_points.cu — point sets, K-builds and the kernel-gradient reductions shared by the exact evaluation, the sparse
+// evaluation and the stand-alone kernel calls, for either kind of covariance function: a single stationary kernel
+// (`const KernParams* kp`) or the context's composite kernel c->mk (kp == nullptr).
+#include <algorithm>
+#include <cstring>
+#include <vector>
+
+#include "gpx_common.cuh"
+#include "gpx_ctx.cuh"
+#include "gpx_kernels.cuh"
+
+namespace gpx {
+
+int prep_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, long ld, double* xT, double* sq) {
+  return kp ? launch_prep_x(X, n, ld, *kp, xT, sq, c->st) : launch_prep_multi(X, n, c->D, ld, c->mk, xT, sq, c->st);
+}
+
+int upload_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, PointSet& ps) {
+  const int D = kp ? kp->D : c->D;
+  ps.n = n; ps.ld = (n + TILE - 1) / TILE * TILE; ps.st = c->st;
+  GPX_TMP_ALLOC(&ps.raw, (size_t)n * D * 8, c->st);
+  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * (kp ? kp->D : std::max(1, c->mk.sumD)) * 8, c->st);
+  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * (kp ? 1 : c->mk.nparts) * 8, c->st);
+  GPX_CUDA(cudaMemcpyAsync(ps.raw, X, (size_t)n * D * 8, cudaMemcpyHostToDevice, c->st));
+  GPX_CHECK(prep_points(c, kp, ps.raw, n, ps.ld, ps.xT, ps.sq));
+  c->total_launches++;
+  return 0;
+}
+
+int build_K(gpx_ctx* c, const KernParams* kp, const Points& rows, const Points& cols, double* out, long ld, const KyDiag* ky,
+            int rt0, int nrt) {
+  const int row_tiles = nrt ? nrt : (int)(rows.ld / TILE), col_tiles = (int)(cols.ld / TILE);
+  const int same = rows.xT == cols.xT;   // one point set on both sides: exact zero distance on the diagonal
+  if (!kp) {
+    KBuildMultiParams kb;
+    memset(&kb, 0, sizeof(kb));
+    kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
+    kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
+    kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.mk = c->mk;
+    if (ky) { kb.sym = 1; kb.diag_add = ky->add; }
+    return launch_kbuild_multi(kb, row_tiles, col_tiles, c->st);
+  }
+  KBuildParams kb;
+  memset(&kb, 0, sizeof(kb));
+  kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
+  kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
+  kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.rt0 = rt0; kb.kp = *kp;
+  if (ky) { kb.sym = 1; kb.diag_add = ky->add; kb.diag_vec = ky->vec; }
+  return launch_kbuild(kb, row_tiles, col_tiles, c->st);
+}
+
+GradFullParams grad_params(const KernParams& kp, const Points& rows, const Points& cols, const double* dL_dK, long ldd) {
+  GradFullParams gp;
+  memset(&gp, 0, sizeof(gp));
+  gp.x1T = rows.xT; gp.ld1 = rows.ld; gp.sq1 = rows.sq; gp.N = rows.n;
+  gp.x2T = cols.xT; gp.ld2 = cols.ld; gp.sq2 = cols.sq; gp.M = cols.n;
+  gp.dL_dK = dL_dK; gp.ldd = ldd; gp.same = rows.xT == cols.xT; gp.kp = kp;
+  return gp;
+}
+
+size_t grad_full_doubles(const GradFullParams& gp) {
+  return (size_t)(gp.ld1 / TILE) * (gp.ld2 / TILE) * ((gp.kp.ard ? gp.kp.D : 1) + 1);
+}
+
+int grad_full_sum(gpx_ctx* c, GradFullParams gp, double* part, double* dvariance, double* dlengthscale) {
+  const int nl = gp.kp.ard ? gp.kp.D : 1, nred = nl + 1;
+  gp.partials = part;
+  GPX_CHECK(launch_grad_full(gp, (int)(gp.ld2 / TILE), (int)(gp.ld1 / TILE), c->st));
+  c->total_launches++;
+  std::vector<double> hp(grad_full_doubles(gp));
+  GPX_CUDA(cudaMemcpyAsync(hp.data(), part, hp.size() * 8, cudaMemcpyDeviceToHost, c->st));
+  GPX_CUDA(cudaStreamSynchronize(c->st));
+  std::vector<double> tot(nred, 0.0);
+  for (size_t t = 0; t < hp.size() / nred; t++)
+    for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
+  *dvariance = tot[0];
+  for (int q = 0; q < nl; q++) dlengthscale[q] = -tot[1 + q] / gp.kp.ls[q];
+  return 0;
+}
+
+// the columns are split into chunks so that ~4 waves of CTAs are in flight; the chunks' partials are reduced in fixed order
+static void gradx_chunks(const gpx_ctx* c, const GradFullParams& gp, int* nchunk, long* mchunk) {
+  const long ntile = (gp.N + TILE - 1) / TILE;
+  const int n = (int)std::max<long>(1, std::min<long>((gp.M + 31) / 32, (4 * c->num_sms + ntile - 1) / ntile));
+  *mchunk = ((gp.M + n - 1) / n + 31) / 32 * 32;
+  *nchunk = (int)((gp.M + *mchunk - 1) / *mchunk);
+}
+
+size_t grad_X_doubles(const gpx_ctx* c, const GradFullParams& gp) {
+  int nchunk;
+  long mchunk;
+  gradx_chunks(c, gp, &nchunk, &mchunk);
+  return (size_t)(nchunk + 1) * gp.N * gp.kp.D;
+}
+
+int grad_X(gpx_ctx* c, const GradFullParams& gp, double* part, double* out) {
+  int nchunk;
+  long mchunk;
+  gradx_chunks(c, gp, &nchunk, &mchunk);
+  double* dout = part + (size_t)nchunk * gp.N * gp.kp.D;
+  GPX_CHECK(launch_gradx(gp, nchunk, mchunk, part, dout, c->st));
+  c->total_launches += 2;
+  GPX_CUDA(cudaMemcpyAsync(out, dout, (size_t)gp.N * gp.kp.D * 8, cudaMemcpyDeviceToHost, c->st));
+  GPX_CUDA(cudaStreamSynchronize(c->st));
+  return 0;
+}
+
+}  // namespace gpx

@@ -22,15 +22,6 @@
 
 using namespace gpx;
 
-static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double* dvariance, double* dlengthscale,
-                            double* dZ);
-
-#define GPX_FAIL(msg)       \
-  do {                      \
-    gpx::set_error(msg);    \
-    return -2;              \
-  } while (0)
-
 struct SparseState {
   long N = 0, Npad = 0, M = 0, Mpad = 0;   // N: rows held by THIS rank (all of them on one GPU)
   long Ntot = 0;                           // rows over all ranks (var_dtc.py num_data)
@@ -55,6 +46,8 @@ struct SparseState {
   double trYYT = 0.0;
   bool have_eval = false;
   double noise = 0.0;
+  Points xpts() const { return Points{XsT, sqX, N, Npad}; }   // this rank's data points, prepared
+  Points zpts() const { return Points{ZsT, sqZ, M, Mpad}; }   // the inducing points, prepared
 };
 
 namespace {
@@ -140,6 +133,12 @@ __global__ void __launch_bounds__(256) trace_dot_kernel(const double* __restrict
     __syncthreads();
   }
   if (threadIdx.x == 0) { r[2 * blockIdx.x] = sh[0][0]; r[2 * blockIdx.x + 1] = sh[1][0]; }
+}
+// n kernels just issued for context c (on its stream or on a child context's): counted on c, a launch error surfaced
+int launched(gpx_ctx* c, int n = 1) {
+  c->total_launches += n;
+  GPX_CUDA(cudaGetLastError());
+  return 0;
 }
 }  // namespace
 
@@ -238,20 +237,21 @@ static int psi_device(gpx_ctx* c, int kind, int ard, double variance, const doub
   GPX_CUDA(cudaMemcpyAsync(s->Z, Z, (size_t)M * s->D * 8, cudaMemcpyHostToDevice, st));
   GPX_CHECK(launch_prep_x(s->X, N, Npad, s->kp, s->XsT, s->sqX, st));
   GPX_CHECK(launch_prep_x(s->Z, M, Mpad, s->kp, s->ZsT, s->sqZ, st));
-  const int mt = (int)(Mpad / TILE), ntl = (int)(Npad / TILE);
-  KBuildParams kb;
-  memset(&kb, 0, sizeof(kb));
-  kb.kp = s->kp; kb.sym = 0; kb.same = 0;
-  // psi1^T: thread-mapped operand = inducing points
-  kb.rowsT = s->ZsT; kb.ld_rows = Mpad; kb.sq_rows = s->sqZ; kb.colsT = s->XsT; kb.ld_cols = Npad; kb.sq_cols = s->sqX;
-  kb.out = s->Kuf; kb.ld = Mpad; kb.nrows = M; kb.ncols = N;
-  GPX_CHECK(launch_kbuild(kb, mt, ntl, st));
-  // psi1: thread-mapped operand = data points
-  kb.rowsT = s->XsT; kb.ld_rows = Npad; kb.sq_rows = s->sqX; kb.colsT = s->ZsT; kb.ld_cols = Mpad; kb.sq_cols = s->sqZ;
-  kb.out = s->Kfu; kb.ld = Npad; kb.nrows = N; kb.ncols = M;
-  GPX_CHECK(launch_kbuild(kb, ntl, mt, st));
-  c->total_launches += 4;
-  return 0;
+  GPX_CHECK(launched(c, 2));
+  GPX_CHECK(build_K(c, &s->kp, s->zpts(), s->xpts(), s->Kuf, Mpad));   // psi1^T: thread-mapped operand = inducing points
+  GPX_CHECK(build_K(c, &s->kp, s->xpts(), s->zpts(), s->Kfu, Npad));   // psi1: thread-mapped operand = data points
+  return launched(c, 2);
+}
+
+// C = A psi1^T (M x N) on the DMMA GEMM; tri = 2: A is lower triangular (k-range <= row tile)
+static int mul_psi1T(gpx_ctx* c, const double* A, double* C, int tri) {
+  SparseState* s = c->sparse;
+  GemmParams pg = gemm_defaults();
+  pg.mode = GEMM_PANEL; pg.plain = 1; pg.tri = tri;
+  pg.A = A; pg.lda = s->Mpad; pg.B = s->Kfu; pg.ldb = s->Npad; pg.C = C; pg.ldc = s->Mpad;
+  pg.K = (int)s->Mpad; pg.nt = (int)(s->Mpad / TILE); pg.ncols = (int)(s->Npad / TILE);
+  GPX_CHECK(launch_gemm(pg, dim3(1, 1), c->st));
+  return launched(c);
 }
 
 // dL_dKnm^T = W2 psi1^T (+ rank-P term on the fly) reduced to kernel-parameter gradients and dL/dZ; W2 (device, s->W2)
@@ -262,64 +262,28 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
                             double* dZ) {
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
-  const long M = s->M, Mpad = s->Mpad, N = s->N, Npad = s->Npad;
-  const int D = s->D, P = s->P;
-  const int mt = (int)(Mpad / TILE), ntl = (int)(Npad / TILE);
+  const long Mpad = s->Mpad, N = s->N, Npad = s->Npad;
+  const int P = s->P;
   if (bvec)
     ymul_kernel<<<(unsigned)((Npad * P + 255) / 256), 256, 0, st>>>(s->Y, bvec, Npad, P, s->Yb);
   else
     scale_kernel<<<(unsigned)((Npad * P + 255) / 256), 256, 0, st>>>(s->Y, beta, Npad * P, s->Yb);
-  GPX_CUDA(cudaGetLastError());
-  // dLt = W2 * psi1^T  (M x N), W2 symmetric
-  {
-    GemmParams pg = gemm_defaults();
-    pg.mode = GEMM_PANEL; pg.plain = 1;
-    pg.A = s->W2; pg.lda = Mpad; pg.B = s->Kfu; pg.ldb = Npad; pg.C = s->dLt; pg.ldc = Mpad;
-    pg.K = (int)Mpad; pg.nt = mt; pg.ncols = ntl;
-    GPX_CHECK(launch_gemm(pg, dim3(1, 1), st));
-  }
+  GPX_CHECK(launched(c));
+  GPX_CHECK(mul_psi1T(c, s->W2, s->dLt, 0));   // dLt = W2 * psi1^T  (M x N), W2 symmetric
   if (bvec) {
     scale_cols_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(s->dLt, Mpad, N, bvec);
-    GPX_CUDA(cudaGetLastError());
-    c->total_launches++;
+    GPX_CHECK(launched(c));
   }
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
-  const int nl = s->kp.ard ? D : 1, nred = nl + 1;
-  const int nchunk = (int)std::max<long>(1, std::min<long>((N + 31) / 32, (4 * c->num_sms + mt - 1) / mt));
-  const long mchunk = ((N + nchunk - 1) / nchunk + 31) / 32 * 32;
-  const int nch = (int)((N + mchunk - 1) / mchunk);
-  const size_t part_full = (size_t)mt * ntl * nred * 8, part_x = (size_t)nch * M * D * 8 + (size_t)M * D * 8;
-  GPX_CHECK(ensure_part(s, std::max(part_full, part_x)));
-  GradFullParams gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.x1T = s->XsT; gp.ld1 = Npad; gp.sq1 = s->sqX; gp.N = N;
-  gp.x2T = s->ZsT; gp.ld2 = Mpad; gp.sq2 = s->sqZ; gp.M = M;
-  gp.dL_dK = s->dLt; gp.ldd = Mpad; gp.same = 0; gp.partials = s->part; gp.kp = s->kp;
+  GradFullParams gp = grad_params(s->kp, s->xpts(), s->zpts(), s->dLt, Mpad);
   gp.ci = s->Yb; gp.ldci = Npad; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = P;
-  GPX_CHECK(launch_grad_full(gp, mt, ntl, st));
-  std::vector<double> hp((size_t)mt * ntl * nred);
-  GPX_CUDA(cudaMemcpyAsync(hp.data(), s->part, hp.size() * 8, cudaMemcpyDeviceToHost, st));
-  GPX_CUDA(cudaStreamSynchronize(st));
-  {
-    std::vector<double> tot(nred, 0.0);
-    for (size_t t = 0; t < (size_t)mt * ntl; t++)
-      for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
-    *dvariance = tot[0];
-    for (int q = 0; q < nl; q++) dlengthscale[q] = -tot[1 + q] / s->kp.ls[q];
-  }
+  GPX_CHECK(ensure_part(s, grad_full_doubles(gp) * 8));
+  GPX_CHECK(grad_full_sum(c, gp, s->part, dvariance, dlengthscale));
   // dL/dZ: gradients_X(dL_dKnm^T, Z, X): rows = inducing points, columns = data points, dL read transposed
-  GradFullParams gx;
-  memset(&gx, 0, sizeof(gx));
-  gx.x1T = s->ZsT; gx.ld1 = Mpad; gx.sq1 = s->sqZ; gx.N = M;
-  gx.x2T = s->XsT; gx.ld2 = Npad; gx.sq2 = s->sqX; gx.M = N;
-  gx.dL_dK = s->dLt; gx.ldd = Mpad; gx.transposed = 1; gx.same = 0; gx.kp = s->kp;
-  gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = s->Yb; gx.ldcj = Npad; gx.cP = P;
-  double* dout = s->part + (size_t)nch * M * D;
-  GPX_CHECK(launch_gradx(gx, nch, mchunk, s->part, dout, st));
-  GPX_CUDA(cudaMemcpyAsync(dZ, dout, (size_t)M * D * 8, cudaMemcpyDeviceToHost, st));
-  GPX_CUDA(cudaStreamSynchronize(st));
-  c->total_launches += 5;
-  return 0;
+  GradFullParams gx = grad_params(s->kp, s->zpts(), s->xpts(), s->dLt, Mpad);
+  gx.transposed = 1; gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = s->Yb; gx.ldcj = Npad; gx.cP = P;
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, gx) * 8));
+  return grad_X(c, gx, s->part, dZ);
 }
 
 // =================================================================================================================
@@ -329,20 +293,54 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
 //   A = beta (Lmi G) Lmi^T;  B = I + A -> LB, UB;  Q = LBi Um^T (= LBi Lmi);  v = Q psi1Vf;  C = Q^T v;  w = UB v
 //   B^-1 = UB UB^T;  DBi = P B^-1 + w w^T;  dL_dKmm = Um (..) Um^T;  dL_dpsi2 = beta/2 Um (P I - DBi) Um^T
 // =================================================================================================================
-static int mm_nt(gpx_ctx* c, const double* A, const double* B, double* C, long Mpad, int plain = 1) {
+static int mm_nt(gpx_ctx* c, const double* A, const double* B, double* C, int plain = 1) {
+  const long Mpad = c->sparse->Mpad;
   GemmParams pg = gemm_defaults();
   pg.mode = GEMM_PANEL; pg.plain = plain;
   pg.A = A; pg.lda = Mpad; pg.B = B; pg.ldb = Mpad; pg.C = C; pg.ldc = Mpad;
   pg.K = (int)Mpad; pg.nt = (int)(Mpad / TILE); pg.ncols = (int)(Mpad / TILE);
-  c->total_launches++;
-  return launch_gemm(pg, dim3(1, 1), c->st);
+  GPX_CHECK(launch_gemm(pg, dim3(1, 1), c->st));
+  return launched(c);
 }
-static int combine(gpx_ctx* c, double* out, long Mpad, long n, double a, const double* X, double b, const double* Y,
-                   double cdiag, double d = 0.0, const double* U = nullptr, int P = 0) {
+static int combine(gpx_ctx* c, double* out, long n, double a, const double* X, double b, const double* Y, double cdiag,
+                   double d = 0.0, const double* U = nullptr, int P = 0) {
+  const long Mpad = c->sparse->Mpad;
   dim3 grid((unsigned)((n + 255) / 256), (unsigned)n);
   combine_kernel<<<grid, 256, 0, c->st>>>(out, Mpad, n, a, X, b, Y, cdiag, d, U, Mpad, P);
-  GPX_CUDA(cudaGetLastError());
-  c->total_launches++;
+  return launched(c);
+}
+// out = Um E Um^T (T: scratch; out may be E)
+static int sandwich(gpx_ctx* c, const double* Um, const double* E, double* T, double* out) {
+  GPX_CHECK(mm_nt(c, Um, E, T));
+  return mm_nt(c, T, Um, out);
+}
+// B^-1 = UB UB^T: lower tiles, mirrored
+static int binv(gpx_ctx* c, const double* UB, double* out) {
+  const long Mpad = c->sparse->Mpad;
+  GPX_CHECK(mm_nt(c, UB, UB, out, 2));
+  mirror_tiles_kernel<<<dim3((unsigned)((Mpad + 255) / 256), (unsigned)Mpad), 256, 0, c->st>>>(out, Mpad, Mpad);
+  return launched(c);
+}
+// Kmm = K(Z, Z), dense and zero padded
+static int build_Kmm(gpx_ctx* c, double* Kd) {
+  SparseState* s = c->sparse;
+  GPX_CUDA(cudaMemsetAsync(Kd, 0, (size_t)s->Mpad * s->Mpad * 8, c->st));
+  GPX_CHECK(build_K(c, &s->kp, s->zpts(), s->zpts(), Kd, s->Mpad));
+  return launched(c);
+}
+// factor-and-invert the M x M matrix A (written on c's stream) on the child context ch, then U (clean upper) and
+// Linv = U^T out of its factor; the child's launches count on c as well
+static int factor_child(gpx_ctx* c, gpx_ctx* ch, const double* A, double jitter, double* logdet, double* U, double* Linv) {
+  const long Mpad = c->sparse->Mpad;
+  GPX_CUDA(cudaStreamSynchronize(c->st));
+  const int64_t l0 = ch->total_launches;
+  const int rc = factor_device(ch, A, Mpad, c->sparse->M, jitter, 5, logdet, nullptr);
+  c->total_launches += ch->total_launches - l0;
+  if (rc) return rc;
+  if (ch->Npad != Mpad) GPX_FAIL("internal: child workspace size");
+  GPX_CHECK(launch_assemble(ch->S, Mpad, (int)Mpad, U, Mpad, Linv, ch->st));
+  GPX_CHECK(launched(c));
+  GPX_CUDA(cudaStreamSynchronize(ch->st));
   return 0;
 }
 
@@ -382,7 +380,7 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   }
   GPX_CHECK(psi_device(c, kind, ard, variance, lengthscale, Z, M));
   const long Mpad = s->Mpad, N = s->Ntot, Npad = s->Npad;
-  const int D = s->D, P = s->P, mt = (int)(Mpad / TILE), ntl = (int)(Npad / TILE);
+  const int D = s->D, P = s->P, mt = (int)(Mpad / TILE);
   const int nl = s->kp.ard ? D : 1;
   constexpr int RSPLIT = 64;
   if (!s->mm[0]) {
@@ -404,44 +402,23 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   s->noise = het ? 0.0 : noise;
   const double *sbv = het ? s->hb : nullptr, *bvec = het ? s->hb + Npad : nullptr;
   // Kmm (dense, zero padded), factor-and-invert with const_jitter (var_dtc.py:93-95)
-  GPX_CUDA(cudaMemsetAsync(Kd, 0, (size_t)Mpad * Mpad * 8, st));
-  {
-    KBuildParams kb;
-    memset(&kb, 0, sizeof(kb));
-    kb.kp = s->kp; kb.sym = 0; kb.same = 1;
-    kb.rowsT = s->ZsT; kb.ld_rows = Mpad; kb.sq_rows = s->sqZ; kb.colsT = s->ZsT; kb.ld_cols = Mpad; kb.sq_cols = s->sqZ;
-    kb.out = Kd; kb.ld = Mpad; kb.nrows = M; kb.ncols = M;
-    GPX_CHECK(launch_kbuild(kb, mt, mt, st));
-  }
-  GPX_CUDA(cudaStreamSynchronize(st));
-  {
-    const int rc = factor_device(s->cK, Kd, Mpad, M, 1e-8, 5, nullptr, nullptr);
-    if (rc) return rc;
-  }
-  if (s->cK->Npad != Mpad) GPX_FAIL("internal: child workspace size");
-  GPX_CHECK(launch_assemble(s->cK->S, Mpad, (int)Mpad, Um, Mpad, Lmi, s->cK->st));      // Um (clean upper), Lmi = Um^T
-  GPX_CUDA(cudaStreamSynchronize(s->cK->st));
+  GPX_CHECK(build_Kmm(c, Kd));
+  GPX_CHECK(factor_child(c, s->cK, Kd, 1e-8, nullptr, Um, Lmi));                      // Um (clean upper), Lmi = Um^T
   // tmp = Lm^-1 psi1^T (M x N; var_dtc.py:131,139 dtrtrs) as a product with the triangular inverse, k-range <= row tile.
   // A = tmp tmp^T is then formed from O(1) entries. (Forming G = psi1^T psi1 first and sandwiching it, Lm^-1 G Lm^-T,
   // saves 2 M^2 N flops but cancels ~cond(Kmm) digits: measured 1e-4 instead of 1e-8 on dL/dZ at cond(Kmm) = 2e8.)
   double* Tuf = s->dLt;   // the dL_dKnm^T buffer is free until knm_grads_device
-  {
-    GemmParams pg = gemm_defaults();
-    pg.mode = GEMM_PANEL; pg.plain = 1; pg.tri = 2;
-    pg.A = Lmi; pg.lda = Mpad; pg.B = s->Kfu; pg.ldb = Npad; pg.C = Tuf; pg.ldc = Mpad;
-    pg.K = (int)Mpad; pg.nt = mt; pg.ncols = ntl;
-    GPX_CHECK(launch_gemm(pg, dim3(1, 1), st));
-  }
+  GPX_CHECK(mul_psi1T(c, Lmi, Tuf, 2));
   const double* Yrow = s->Y;   // right-hand side of t = tmp Y
   if (het) {
     // s1_n = sum_a tmp[a, n]^2 (var_dtc.py:249, before the scaling); then tmp[:, n] *= sqrt(beta_n) (:127,131), Y_n likewise
     GPX_CHECK(launch_col_sqnorm(Tuf, Mpad, M, s->N, s->hs, st));
+    GPX_CHECK(launched(c));
     scale_cols_kernel<<<(unsigned)((Mpad * s->N + 255) / 256), 256, 0, st>>>(Tuf, Mpad, s->N, sbv);
-    GPX_CUDA(cudaGetLastError());
+    GPX_CHECK(launched(c));
     ymul_kernel<<<(unsigned)((Npad * P + 255) / 256), 256, 0, st>>>(s->Y, sbv, Npad, P, s->Yb);
-    GPX_CUDA(cudaGetLastError());
+    GPX_CHECK(launched(c));
     Yrow = s->Yb;
-    c->total_launches += 3;
   }
   {
     GemmParams pg = gemm_defaults();   // A_raw = tmp tmp^T (lower tiles), k-depth = Npad
@@ -449,8 +426,10 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     pg.A = Tuf; pg.lda = Mpad; pg.B = Tuf; pg.ldb = Mpad; pg.C = Ar; pg.ldc = Mpad;
     pg.K = (int)Npad; pg.nt = mt; pg.ncols = mt;
     GPX_CHECK(launch_gemm(pg, dim3(1, 1), st));
+    GPX_CHECK(launched(c));
   }
   GPX_CHECK(launch_row_dot(Tuf, Mpad, Mpad, s->N, P, Yrow, Npad, RSPLIT, rpart, tv, st));   // t = tmp Y  ([P][Mpad])
+  GPX_CHECK(launched(c, 2));
   // row shards: A_raw and t are sums over data points -> one M x M and one M x P all-reduce
   // (the pattern of var_dtc_parallel.py:113-131 with NCCL instead of mpi4py)
   GPX_CHECK(dist_allreduce_sum(c, Ar, (size_t)Mpad * Mpad, st));
@@ -458,25 +437,19 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   {
     dim3 grid((unsigned)((Mpad + 255) / 256), (unsigned)Mpad);
     mirror_tiles_kernel<<<grid, 256, 0, st>>>(Ar, Mpad, Mpad);
-    GPX_CUDA(cudaGetLastError());
+    GPX_CHECK(launched(c));
   }
-  c->total_launches += 6;
   // B = I + beta A_raw  (var_dtc.py:135-136)
-  GPX_CHECK(combine(c, Bd, Mpad, Mpad, beta, Ar, 0.0, nullptr, 1.0));
-  GPX_CUDA(cudaStreamSynchronize(st));
+  GPX_CHECK(combine(c, Bd, Mpad, beta, Ar, 0.0, nullptr, 1.0));
   double logdetB = 0.0;
-  {
-    const int rc = factor_device(s->cB, Bd, Mpad, M, 0.0, 5, &logdetB, nullptr);
-    if (rc) return rc;
-  }
-  GPX_CHECK(launch_assemble(s->cB->S, Mpad, (int)Mpad, UB, Mpad, LBi, s->cB->st));
-  GPX_CUDA(cudaStreamSynchronize(s->cB->st));
+  GPX_CHECK(factor_child(c, s->cB, Bd, 0.0, &logdetB, UB, LBi));
   // v = LB^-1 (beta t) (:139-141) ; w = LB^-T v ; C = Lm^-T w (:142-143)   [col_dot(A, y) = A^T y]
   scale_kernel<<<(unsigned)((Mpad * P + 255) / 256), 256, 0, st>>>(tv, beta, Mpad * P, xv);
-  GPX_CUDA(cudaGetLastError());
+  GPX_CHECK(launched(c));
   GPX_CHECK(launch_col_dot(UB, Mpad, Mpad, Mpad, P, xv, Mpad, vv, Mpad, st));           // v = UB^T x = LBi x
   GPX_CHECK(launch_col_dot(LBi, Mpad, Mpad, Mpad, P, vv, Mpad, wv, Mpad, st));          // w = LBi^T v
   GPX_CHECK(launch_col_dot(Lmi, Mpad, Mpad, Mpad, P, wv, Mpad, Cv, Mpad, st));          // C = Lmi^T w
+  GPX_CHECK(launched(c, 3));
   std::vector<double> hstat, hY;
   if (het) {
     // _compute_dL_dR, het_noise (var_dtc.py:241-257): per data point
@@ -484,45 +457,33 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     //   s2_n = |LB^-1 Lm^-1 psi1^T[:, n]|^2 = |(Q psi1^T)[:, n]|^2,  Q = LB^-1 Lm^-1 (lower triangular)
     double *s2v = s->hs + Npad, *rv = s->hs + 2 * Npad;
     GPX_CHECK(launch_col_dot(Tuf, Mpad, M, s->N, P, wv, Mpad, rv, Npad, st));
-    GPX_CHECK(mm_nt(c, LBi, Um, T, Mpad));                                                // Q = LBi Um^T = LBi Lmi
-    {
-      GemmParams pg = gemm_defaults();
-      pg.mode = GEMM_PANEL; pg.plain = 1; pg.tri = 2;
-      pg.A = T; pg.lda = Mpad; pg.B = s->Kfu; pg.ldb = Npad; pg.C = s->dLt; pg.ldc = Mpad;
-      pg.K = (int)Mpad; pg.nt = mt; pg.ncols = ntl;
-      GPX_CHECK(launch_gemm(pg, dim3(1, 1), st));
-    }
+    GPX_CHECK(launched(c));
+    GPX_CHECK(mm_nt(c, LBi, Um, T));                                                      // Q = LBi Um^T = LBi Lmi
+    GPX_CHECK(mul_psi1T(c, T, s->dLt, 2));
     GPX_CHECK(launch_col_sqnorm(s->dLt, Mpad, M, s->N, s2v, st));
+    GPX_CHECK(launched(c));
     hstat.resize((size_t)(2 + P) * Npad);
     hY.resize((size_t)P * Npad);
     GPX_CUDA(cudaMemcpyAsync(hstat.data(), s->hs, hstat.size() * 8, cudaMemcpyDeviceToHost, st));
     GPX_CUDA(cudaMemcpyAsync(hY.data(), s->Y, hY.size() * 8, cudaMemcpyDeviceToHost, st));
-    c->total_launches += 3;
   }
-  // Binv = UB UB^T (lower tiles, mirrored) ; DBi = P Binv + w w^T
-  GPX_CHECK(mm_nt(c, UB, UB, DB, Mpad, 2));
-  {
-    dim3 grid((unsigned)((Mpad + 255) / 256), (unsigned)Mpad);
-    mirror_tiles_kernel<<<grid, 256, 0, st>>>(DB, Mpad, Mpad);
-    GPX_CUDA(cudaGetLastError());
-  }
-  GPX_CHECK(combine(c, DB, Mpad, Mpad, (double)P, DB, 0.0, nullptr, 0.0, 1.0, wv, P));
+  // DBi = P B^-1 + w w^T
+  GPX_CHECK(binv(c, UB, DB));
+  GPX_CHECK(combine(c, DB, Mpad, (double)P, DB, 0.0, nullptr, 0.0, 1.0, wv, P));
   // scalars: trace(A_raw), sum(A_raw .* DBi), |v|^2
   const int RB = 64;
   trace_dot_kernel<<<RB, 256, 0, st>>>(Ar, DB, Mpad, M, s->red);
-  GPX_CUDA(cudaGetLastError());
+  GPX_CHECK(launched(c));
   GPX_CUDA(cudaMemcpyAsync(s->h_red, s->red, 2 * RB * 8, cudaMemcpyDeviceToHost, st));
   std::vector<double> hv((size_t)P * Mpad);
   GPX_CUDA(cudaMemcpyAsync(hv.data(), vv, hv.size() * 8, cudaMemcpyDeviceToHost, st));
   // dL_dKmm = Um (-0.5 DBi - 0.5 P B + P I) Um^T   (var_dtc.py:152-156)
-  GPX_CHECK(combine(c, E, Mpad, Mpad, -0.5, DB, -0.5 * P, Bd, (double)P));
-  GPX_CHECK(mm_nt(c, Um, E, T, Mpad));
-  GPX_CHECK(mm_nt(c, T, Um, Kd, Mpad));                                                  // Kd now holds dL_dKmm
+  GPX_CHECK(combine(c, E, Mpad, -0.5, DB, -0.5 * P, Bd, (double)P));
+  GPX_CHECK(sandwich(c, Um, E, T, Kd));                                                   // Kd now holds dL_dKmm
   // W2 = 2 dL_dpsi2 = beta Um (P I - DBi) Um^T     (var_dtc.py:221,231-233)
-  GPX_CHECK(combine(c, E, Mpad, Mpad, -1.0, DB, 0.0, nullptr, (double)P));
-  GPX_CHECK(mm_nt(c, Um, E, T, Mpad));
-  GPX_CHECK(mm_nt(c, T, Um, E, Mpad));
-  GPX_CHECK(combine(c, s->W2, Mpad, Mpad, beta, E, 0.0, nullptr, 0.0));
+  GPX_CHECK(combine(c, E, Mpad, -1.0, DB, 0.0, nullptr, (double)P));
+  GPX_CHECK(sandwich(c, Um, E, T, E));
+  GPX_CHECK(combine(c, s->W2, Mpad, beta, E, 0.0, nullptr, 0.0));
   // Knm part: needs C in s->Cm
   GPX_CUDA(cudaMemcpyAsync(s->Cm, Cv, (size_t)P * Mpad * 8, cudaMemcpyDeviceToDevice, st));
   double dv_knm = 0.0;
@@ -546,40 +507,14 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     }
   }
   // Kmm part: kern.update_gradients_full(dL_dKmm, Z) and kern.gradients_X(dL_dKmm, Z)  (sparse_gp.py:114,117)
-  const int nred = nl + 1;
-  GradFullParams gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.x1T = s->ZsT; gp.ld1 = Mpad; gp.sq1 = s->sqZ; gp.N = M;
-  gp.x2T = s->ZsT; gp.ld2 = Mpad; gp.sq2 = s->sqZ; gp.M = M;
-  gp.dL_dK = Kd; gp.ldd = Mpad; gp.same = 1; gp.partials = s->part; gp.kp = s->kp;
-  GPX_CHECK(launch_grad_full(gp, mt, mt, st));
-  std::vector<double> hp((size_t)mt * mt * nred);
-  GPX_CUDA(cudaMemcpyAsync(hp.data(), s->part, hp.size() * 8, cudaMemcpyDeviceToHost, st));
-  GPX_CUDA(cudaStreamSynchronize(st));
+  const GradFullParams gk = grad_params(s->kp, s->zpts(), s->zpts(), Kd, Mpad);
   double dv_kmm = 0.0;
-  std::vector<double> dl_kmm(nl, 0.0);
-  {
-    std::vector<double> tot(nred, 0.0);
-    for (size_t t = 0; t < (size_t)mt * mt; t++)
-      for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
-    dv_kmm = tot[0];
-    for (int q = 0; q < nl; q++) dl_kmm[q] = -tot[1 + q] / s->kp.ls[q];
-  }
-  {
-    const int nchunk = (int)std::max<long>(1, std::min<long>((M + 31) / 32, (4 * c->num_sms + mt - 1) / mt));
-    const long mchunk = ((M + nchunk - 1) / nchunk + 31) / 32 * 32;
-    const int nch = (int)((M + mchunk - 1) / mchunk);
-    GPX_CHECK(ensure_part(s, (size_t)(nch + 1) * M * D * 8));
-    GradFullParams gx = gp;
-    gx.partials = nullptr;
-    double* dout = s->part + (size_t)nch * M * D;
-    GPX_CHECK(launch_gradx(gx, nch, mchunk, s->part, dout, st));
-    std::vector<double> hz((size_t)M * D);
-    GPX_CUDA(cudaMemcpyAsync(hz.data(), dout, hz.size() * 8, cudaMemcpyDeviceToHost, st));
-    GPX_CUDA(cudaStreamSynchronize(st));
-    for (size_t i = 0; i < hz.size(); i++) dZ[i] += hz[i];
-  }
-  c->total_launches += 8;
+  std::vector<double> dl_kmm(nl, 0.0), hz((size_t)M * D);
+  GPX_CHECK(ensure_part(s, grad_full_doubles(gk) * 8));
+  GPX_CHECK(grad_full_sum(c, gk, s->part, &dv_kmm, dl_kmm.data()));
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, gk) * 8));
+  GPX_CHECK(grad_X(c, gk, s->part, hz.data()));
+  for (size_t i = 0; i < hz.size(); i++) dZ[i] += hz[i];
   // ---- scalars on the host (var_dtc.py:237-276, homoscedastic) -----------------------------------------------------
   double trAr = 0.0, sumAD = 0.0, data_fit = 0.0;
   for (int b = 0; b < RB; b++) { trAr += s->h_red[2 * b]; sumAD += s->h_red[2 * b + 1]; }
@@ -673,36 +608,22 @@ int gpx_sparse_get(gpx_ctx* c, int which, double* out) {
     return 0;
   }
   double* src = nullptr;
-  if (which == 1) {   // woodbury_inv = Um (I - B^-1) Um^T   (var_dtc.py:207-210); B^-1 = (DBi - w w^T) / P is rebuilt
+  if (which == 1) {   // woodbury_inv = Um (I - B^-1) Um^T   (var_dtc.py:207-210); B^-1 is rebuilt from UB
     double *Um = s->mm[1], *UB = s->mm[6], *T = s->mm[3], *E = s->mm[9], *DB = s->mm[8];
-    GPX_CHECK(mm_nt(c, UB, UB, DB, Mpad, 2));
-    dim3 grid((unsigned)((Mpad + 255) / 256), (unsigned)Mpad);
-    mirror_tiles_kernel<<<grid, 256, 0, st>>>(DB, Mpad, Mpad);
-    GPX_CUDA(cudaGetLastError());
-    GPX_CHECK(combine(c, E, Mpad, Mpad, -1.0, DB, 0.0, nullptr, 1.0));
-    GPX_CHECK(mm_nt(c, Um, E, T, Mpad));
-    GPX_CHECK(mm_nt(c, T, Um, E, Mpad));
+    GPX_CHECK(binv(c, UB, DB));
+    GPX_CHECK(combine(c, E, Mpad, -1.0, DB, 0.0, nullptr, 1.0));
+    GPX_CHECK(sandwich(c, Um, E, T, E));
     src = E;
-  } else if (which == 2 || which == 3) {
-    // Kmm / Lm from the child context's factor: rebuild Kmm by the kernel build, Lm by extraction
-    if (which == 2) {
-      double* Kd = s->mm[3];
-      GPX_CUDA(cudaMemsetAsync(Kd, 0, (size_t)Mpad * Mpad * 8, st));
-      KBuildParams kb;
-      memset(&kb, 0, sizeof(kb));
-      kb.kp = s->kp; kb.sym = 0; kb.same = 1;
-      kb.rowsT = s->ZsT; kb.ld_rows = Mpad; kb.sq_rows = s->sqZ; kb.colsT = s->ZsT; kb.ld_cols = Mpad; kb.sq_cols = s->sqZ;
-      kb.out = Kd; kb.ld = Mpad; kb.nrows = M; kb.ncols = M;
-      GPX_CHECK(launch_kbuild(kb, (int)(Mpad / TILE), (int)(Mpad / TILE), st));
-      GPX_CHECK(combine(c, Kd, Mpad, M, 1.0, Kd, 0.0, nullptr, 1e-8));
-      src = Kd;
-    } else {
-      double* Ld = s->mm[3];
-      GPX_CUDA(cudaStreamSynchronize(st));
-      GPX_CHECK(launch_extract(GPX_GET_L, s->cK->S, Mpad, s->cK->Ldiag, nullptr, nullptr, 0, Mpad, Ld, s->cK->st));
-      GPX_CUDA(cudaStreamSynchronize(s->cK->st));
-      src = Ld;
-    }
+  } else if (which == 2) {   // Kmm, rebuilt by the kernel build, + const_jitter
+    src = s->mm[3];
+    GPX_CHECK(build_Kmm(c, src));
+    GPX_CHECK(combine(c, src, M, 1.0, src, 0.0, nullptr, 1e-8));
+  } else if (which == 3) {   // Lm, extracted from the child context's factor
+    src = s->mm[3];
+    GPX_CUDA(cudaStreamSynchronize(st));
+    GPX_CHECK(launch_extract(GPX_GET_L, s->cK->S, Mpad, s->cK->Ldiag, nullptr, nullptr, 0, Mpad, src, s->cK->st));
+    GPX_CHECK(launched(c));
+    GPX_CUDA(cudaStreamSynchronize(s->cK->st));
   } else {
     GPX_FAIL("unknown gpx_sparse_get selector");
   }
