@@ -33,6 +33,7 @@ void gpx::free_data(gpx_ctx* c) {
     *p = nullptr;
   }
   c->staging_cap = 0;
+  c->NBw = 0;
   c->have_eval = false;
   c->have_kinv = false;
   for (double** mp : {&c->mXsT, &c->msq, &c->mpartials}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
@@ -70,7 +71,8 @@ static int ensure_kinv(gpx_ctx* c) {
   return 0;
 }
 
-static long pick_nb(const gpx_ctx* c) {
+// the outer block for a new workspace of Npad rows: option "nb", else env GPX_NB, else by size
+static long choose_nb(const gpx_ctx* c) {
   if (c->NB > 0) return std::min<long>(c->NB, c->Npad);
   const char* e = getenv("GPX_NB");
   if (e && atol(e) >= TILE && atol(e) % TILE == 0) return std::min<long>(atol(e), c->Npad);
@@ -80,6 +82,8 @@ static long pick_nb(const gpx_ctx* c) {
   if (c->Npad <= 512) return c->Npad;
   return 256;
 }
+// the outer block of the allocated workspace, fixed until the next allocation
+static long pick_nb(const gpx_ctx* c) { return c->NBw > 0 ? c->NBw : choose_nb(c); }
 
 int gpx::fill_kp(KernParams& kp, int kind, int ard, int D, double variance, const double* ls) {
   if (kind < 0 || kind > 3) GPX_FAIL("unknown kernel kind");
@@ -195,7 +199,8 @@ int gpx_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y,
     GPX_CUDA(cudaStreamSynchronize(c->st));
     free_data(c);
     c->Npad = Npad; c->D = D; c->P = P;
-    const long NB = pick_nb(c);
+    const long NB = choose_nb(c);
+    c->NBw = NB;
     GPX_CHECK(alloc_data(c, NB));
     GPX_CUDA(cudaMalloc(&c->dUvPart, (size_t)KSPLIT * Npad * P * 8));
     GPX_CUDA(cudaMalloc(&c->S, (size_t)Npad * Npad * 8));
@@ -1110,6 +1115,7 @@ int gpx::factor_device(gpx_ctx* c, const double* dA, long lda, long N, double ji
     if (!std::isfinite(extra)) break;
   }
   c->total_launches += c->eval_launches - l0;
+  c->stats.tries = tries;
   if (jitter_used) *jitter_used = extra;
   if (info != 0) { gpx::set_error("not positive definite, even with jitter."); return info; }
   if (logdet) {   // 2 sum log diag(L) (linalg.py:208): per-tile partials summed in fixed order

@@ -45,6 +45,8 @@ struct gpx_ctx {
   double* staging = nullptr; // lazy, N x N dense
   size_t staging_cap = 0;
   long NB = 0;               // outer block (0 = auto)
+  long NBw = 0;              // outer block the workspace was allocated for (Pbuf, Tm, the int8 planes): chosen once per
+                             // allocation, so that a later change of GPX_NB cannot run a sweep on buffers sized for another
   // last evaluation
   bool have_eval = false;
   bool have_kinv = false;    // c->Kinv holds K^-1 of the last evaluation (its route stored it, or gpx_get made it)

@@ -329,13 +329,15 @@ static int build_Kmm(gpx_ctx* c, double* Kd) {
   return launched(c);
 }
 // factor-and-invert the M x M matrix A (written on c's stream) on the child context ch, then U (clean upper) and
-// Linv = U^T out of its factor; the child's launches count on c as well
+// Linv = U^T out of its factor; the child's launches count on c as well, its trailing updates in c's stats
 static int factor_child(gpx_ctx* c, gpx_ctx* ch, const double* A, double jitter, double* logdet, double* U, double* Linv) {
   const long Mpad = c->sparse->Mpad;
   GPX_CUDA(cudaStreamSynchronize(c->st));
   const int64_t l0 = ch->total_launches;
+  const int32_t u0 = ch->stats.update_launches;
   const int rc = factor_device(ch, A, Mpad, c->sparse->M, jitter, 5, logdet, nullptr);
   c->total_launches += ch->total_launches - l0;
+  c->stats.update_launches += ch->stats.update_launches - u0;
   if (rc) return rc;
   if (ch->Npad != Mpad) GPX_FAIL("internal: child workspace size");
   GPX_CHECK(launch_assemble(ch->S, Mpad, (int)Mpad, U, Mpad, Linv, ch->st));
@@ -358,6 +360,7 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
   s->have_eval = false;
+  memset(&c->stats, 0, sizeof(c->stats));   // filled below: Kmm's attempts, the trailing updates of both factorisations
   // per-point precisions beta_n = 1 / max(variance_n, const_jitter) (var_dtc.py:79-84) and the sums over n the bound needs
   std::vector<double> hbeta, hsb;
   double sum_log_beta = 0.0, sum_beta = 0.0;
@@ -392,6 +395,9 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     GPX_CUDA(cudaMallocHost(&s->h_red, 4096 * 8));
   }
   if (!s->cK) { GPX_CHECK(gpx_create(c->device, &s->cK)); GPX_CHECK(gpx_create(c->device, &s->cB)); }
+  // the factorisations of Kmm and B run with the parent's option "nb" (a change re-sizes the child's workspace)
+  for (gpx_ctx* ch : {s->cK, s->cB})
+    if (ch->NB != c->NB) GPX_CHECK(gpx_set_option(ch, "nb", c->NB));
   double *Kd = s->mm[0], *Um = s->mm[1], *Lmi = s->mm[2], *T = s->mm[3], *Ar = s->mm[4], *Bd = s->mm[5], *UB = s->mm[6],
          *LBi = s->mm[7], *DB = s->mm[8], *E = s->mm[9];
   double *tv = s->vec, *vv = tv + (size_t)P * Mpad, *Cv = vv + (size_t)P * Mpad, *wv = Cv + (size_t)P * Mpad,
@@ -404,6 +410,7 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   // Kmm (dense, zero padded), factor-and-invert with const_jitter (var_dtc.py:93-95)
   GPX_CHECK(build_Kmm(c, Kd));
   GPX_CHECK(factor_child(c, s->cK, Kd, 1e-8, nullptr, Um, Lmi));                      // Um (clean upper), Lmi = Um^T
+  c->stats.tries = s->cK->stats.tries;
   // tmp = Lm^-1 psi1^T (M x N; var_dtc.py:131,139 dtrtrs) as a product with the triangular inverse, k-range <= row tile.
   // A = tmp tmp^T is then formed from O(1) entries. (Forming G = psi1^T psi1 first and sandwiching it, Lm^-1 G Lm^-T,
   // saves 2 M^2 N flops but cancels ~cond(Kmm) digits: measured 1e-4 instead of 1e-8 on dL/dZ at cond(Kmm) = 2e8.)

@@ -10,7 +10,8 @@
  * part, 7 for the inverse part:
  * |dLML| <= 1e-8 and 1e-6 relative on gradients against the reference, DESIGN.md section 5.1; option "ozaki" selects).
  * The gradient bound is checked on the GPU up to cond(Ky) = 4.6e8. Above cond(Ky) ~ 1e8 the LML and alpha of both paths
- * are less accurate than LAPACK's (DESIGN.md section 5.1).
+ * are less accurate than LAPACK's (DESIGN.md section 5.1). The sparse evaluation stays within 4x the fp64 reference's
+ * error up to cond(Kmm + 1e-8 I) = 3e10, the jitter floor (same section).
  *
  * Conventions
  *   - Return value: 0 ok; >0 "matrix not positive definite, leading minor <ret>" (the caller raises
@@ -182,6 +183,8 @@ typedef struct {
   int64_t launches;     /* kernels launched by the last eval */
   int32_t update_launches;
   int32_t tries;        /* factorisation attempts (1 = no jitter ladder) */
+                        /* after a sparse evaluation only update_launches (both M x M factorisations, Kmm's failed attempts
+                           included) and tries (of Kmm) are set, the other fields are 0 */
   double update_int8_ops; /* Ozaki path: int8 multiply-add operations (2 per MAC) issued by the update / K^-1 launches, summed
                              over the digit pairs actually computed; 0 on the DMMA path */
 } gpx_stats;
@@ -191,7 +194,9 @@ int64_t gpx_total_launches(gpx_ctx* ctx);
 int gpx_measure_fp64_peak(gpx_ctx* ctx, double* tflops);
 
 /* Tunables, mainly for tests. name is one of
- *   "nb"      outer block size: a multiple of 128, 0 = default: env GPX_NB, else by matrix size,
+ *   "nb"      outer block size: a multiple of 128, 0 = default: env GPX_NB, else by matrix size. The block is fixed
+ *             when the workspace is allocated (gpx_set_data); a later change of GPX_NB takes effect at the next
+ *             allocation. The sparse evaluation factors Kmm and B = I + A with the same option,
  *   "profile" 1 (default) = per-phase times in gpx_stats, 0 = total_ms only,
  *   "ozaki"   0 = fp64 DMMA only, 1 = trailing update and K^-1 on the wgmma int8 path where applicable,
  *             -1 = default: env GPX_OZAKI, else 0.
