@@ -7,8 +7,8 @@ computing requires libgpx.so and an H100.
 from . import _ffi  # noqa: F401
 from ._ffi import Engine, GpxError, kern_K, kern_Kdiag, kern_grad_full  # noqa: F401
 
-from .kern import (RBF, Exponential, Matern32, Matern52, Stationary, DeviceGradient, Add, Prod, White, Bias,  # noqa: F401
-                   Kern, CombinationKernel)
+from .kern import (RBF, Exponential, Matern32, Matern52, RatQuad, StdPeriodic, Stationary, DeviceGradient,  # noqa: F401
+                   Add, Prod, White, Bias, Kern, CombinationKernel)
 from .inference import (ExactGaussianInference, Gaussian, HeteroscedasticGaussian, MixedNoise,  # noqa: F401
                         PosteriorExact)
 from .model import GP, GPHeteroscedasticRegression, GPRegression  # noqa: F401

@@ -8,7 +8,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libgpx.so")
 
-KIND = {"rbf": 0, "exponential": 1, "matern32": 2, "matern52": 3, "white": 4, "bias": 5}
+KIND = {"rbf": 0, "exponential": 1, "matern32": 2, "matern52": 3, "white": 4, "bias": 5, "ratquad": 6, "stdperiodic": 7}
 GET = {"L": 0, "alpha": 1, "Kinv": 2, "dL_dK": 3, "K": 4, "Linv": 5}
 
 _dp = ctypes.POINTER(ctypes.c_double)
@@ -29,7 +29,38 @@ class GpxStats(ctypes.Structure):
 class GpxKernPart(ctypes.Structure):
     """gpx_kern_part of include/gpx.h: one factor of a composite kernel."""
     _fields_ = [("kind", ctypes.c_int), ("ard", ctypes.c_int), ("term", ctypes.c_int), ("ndims", ctypes.c_int),
-                ("dims", ctypes.POINTER(ctypes.c_int)), ("variance", ctypes.c_double), ("lengthscale", _dp)]
+                ("dims", ctypes.POINTER(ctypes.c_int)), ("variance", ctypes.c_double), ("lengthscale", _dp),
+                ("power", ctypes.c_double), ("ard_period", ctypes.c_int), ("period", _dp)]
+
+
+def _fill_part(slot, desc, keep, i=0):
+    """one part descriptor (kind, ARD, term, dims, variance, lengthscale[, extra]) -> the gpx_kern_part `slot`; the arrays it
+    points at are appended to `keep`. extra: {"power": a} (RatQuad) or {"period": T, "ARD_period": bool} (StdPeriodic).
+    -> number of gradient entries of the part."""
+    kind, ard, term, dims, variance, lengthscale = desc[:6]
+    extra = desc[6] if len(desc) > 6 else {}
+    static = kind in ("white", "bias")
+    d = np.ascontiguousarray([] if static else dims, dtype=np.int32)
+    ls = np.ascontiguousarray([1.0] if static else np.atleast_1d(lengthscale), dtype=np.float64).reshape(-1)
+    if not static and ls.size != (d.size if ard else 1):
+        raise ValueError("part %d: lengthscale does not match its active dims" % i)
+    keep += [d, ls]
+    slot.kind, slot.ard, slot.term, slot.ndims = KIND[kind], int(bool(ard)), int(term), int(d.size)
+    slot.dims = d.ctypes.data_as(ctypes.POINTER(ctypes.c_int))
+    slot.variance, slot.lengthscale = float(variance), _ptr(ls)
+    n = 1 + (0 if static else ls.size)
+    if kind == "ratquad":
+        slot.power = float(extra["power"])
+        n += 1
+    elif kind == "stdperiodic":
+        ard_p = bool(extra.get("ARD_period", False))
+        T = np.ascontiguousarray(np.atleast_1d(extra["period"]), dtype=np.float64).reshape(-1)
+        if T.size != (d.size if ard_p else 1):
+            raise ValueError("part %d: period does not match its active dims" % i)
+        keep.append(T)
+        slot.ard_period, slot.period = int(ard_p), _ptr(T)
+        n += T.size
+    return n
 
 
 EXPORTS = {
@@ -51,6 +82,10 @@ EXPORTS = {
     "gpx_kern_K": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64, _dp,
                                   ctypes.c_int64, ctypes.c_int, _dp]),
     "gpx_kern_Kdiag": (ctypes.c_int, [ctypes.c_int, ctypes.c_double, ctypes.c_int64, _dp]),
+    "gpx_kern_part_K": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), _dp, ctypes.c_int64, _dp, ctypes.c_int64,
+                                       ctypes.c_int, _dp]),
+    "gpx_kern_part_grad_full": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), _dp, ctypes.c_int64, _dp, ctypes.c_int64,
+                                               ctypes.c_int, _dp, _dp]),
     "gpx_kern_grad_full": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64,
                                           _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp]),
     "gpx_kern_grad_X": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64, _dp,
@@ -192,21 +227,14 @@ class Engine(object):
         return lml.value, grad, dnoise, jit.value
 
     def exact_eval_multi(self, parts, noise, jitter=1e-8, max_tries=5):
-        """composite kernel: parts = [(kind, ARD, term, dims, variance, lengthscale)], ordered by term ->
-        (log_marginal, gradient [per part: variance, lengthscale.. (none for white / bias); then noise], extra_jitter)"""
+        """composite kernel: parts = [(kind, ARD, term, dims, variance, lengthscale)], ordered by term; a "ratquad" part
+        appends {"power": a}, a "stdperiodic" part {"period": T, "ARD_period": bool} (ARD then refers to its lengthscale) ->
+        (log_marginal, gradient [per part: variance, lengthscale.. (none for white / bias), power (ratquad); stdperiodic:
+        variance, period.., lengthscale..; then noise], extra_jitter)"""
         arr = (GpxKernPart * len(parts))()
         keep, ngrad = [], 1
-        for i, (kind, ard, term, dims, variance, lengthscale) in enumerate(parts):
-            static = kind in ("white", "bias")
-            d = np.ascontiguousarray([] if static else dims, dtype=np.int32)
-            ls = np.ascontiguousarray([1.0] if static else np.atleast_1d(lengthscale), dtype=np.float64).reshape(-1)
-            if not static and ls.size != (d.size if ard else 1):
-                raise ValueError("part %d: lengthscale does not match its active dims" % i)
-            keep += [d, ls]
-            arr[i].kind, arr[i].ard, arr[i].term, arr[i].ndims = KIND[kind], int(bool(ard)), int(term), int(d.size)
-            arr[i].dims = d.ctypes.data_as(ctypes.POINTER(ctypes.c_int))
-            arr[i].variance, arr[i].lengthscale = float(variance), _ptr(ls)
-            ngrad += 1 + (0 if static else ls.size)
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
         lml, jit = ctypes.c_double(), ctypes.c_double()
         grad = np.zeros(ngrad)
         rc = self._L.gpx_exact_eval_multi(self._h, arr, len(parts), float(noise), float(jitter), int(max_tries),
@@ -317,6 +345,36 @@ def kern_K(kind, ARD, variance, lengthscale, X, X2=None):
     out = np.empty((N, M))
     check(lib().gpx_kern_K(None, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2), M, D, _ptr(out)), "gpx_kern_K")
     return out
+
+
+def _part_inputs(desc, X, X2):
+    part, keep = GpxKernPart(), []
+    n = _fill_part(part, desc, keep)
+    X = _f64(X)
+    N, D = X.shape
+    X2c = None if X2 is None else _f64(X2)
+    M = N if X2 is None else X2c.shape[0]
+    return part, keep, n, X, N, X2c, M, D
+
+
+def kern_part_K(desc, X, X2=None):
+    """K(X, X2) (N x M) of one composite part descriptor (as Engine.exact_eval_multi takes it; dims index X's columns)."""
+    part, keep, _, X, N, X2c, M, D = _part_inputs(desc, X, X2)
+    out = np.empty((N, M))
+    check(lib().gpx_kern_part_K(None, ctypes.byref(part), _ptr(X), N, _ptr(X2c), M, D, _ptr(out)), "gpx_kern_part_K")
+    return out
+
+
+def kern_part_grad_full(desc, X, dL_dK, X2=None):
+    """update_gradients_full of one composite part for a dense dL_dK (N x M) -> its gradient block."""
+    part, keep, n, X, N, X2c, M, D = _part_inputs(desc, X, X2)
+    dL_dK = _f64(dL_dK)
+    if dL_dK.shape != (N, M):
+        raise ValueError("dL_dK must be %d x %d" % (N, M))
+    grad = np.zeros(n)
+    check(lib().gpx_kern_part_grad_full(None, ctypes.byref(part), _ptr(X), N, _ptr(X2c), M, D, _ptr(dL_dK), _ptr(grad)),
+          "gpx_kern_part_grad_full")
+    return grad
 
 
 def kern_Kdiag(kind, variance, N):

@@ -38,6 +38,7 @@ void gpx::free_data(gpx_ctx* c) {
   c->have_kinv = false;
   for (double** mp : {&c->mXsT, &c->msq, &c->mpartials}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
   c->m_cap = 0;
+  c->mpart_cap = 0;
   oz_planes_free(c->ozp[0]);
   oz_planes_free(c->ozp[1]);
   oz_planes_free(c->ozpA);
@@ -125,9 +126,9 @@ int gpx_create(int device, gpx_ctx** out) {
   GPX_CUDA(cudaStreamCreateWithPriority(&c->st2, cudaStreamNonBlocking, prio_hi));
   // between the two: the big panel GEMM on st3 must not hold back the small launches of the diagonal-block chain on st2
   GPX_CUDA(cudaStreamCreateWithPriority(&c->st3, cudaStreamNonBlocking, prio_hi < prio_lo - 1 ? prio_hi + 1 : prio_hi));
-  GPX_CUDA(cudaMalloc(&c->res, (MAX_D + 2 * MAX_PARTS + 8) * sizeof(double)));
+  GPX_CUDA(cudaMalloc(&c->res, RES_DOUBLES * sizeof(double)));
   GPX_CUDA(cudaMalloc(&c->info, sizeof(int)));
-  GPX_CUDA(cudaMallocHost(&c->h_res, (MAX_D + 2 * MAX_PARTS + 8) * sizeof(double)));
+  GPX_CUDA(cudaMallocHost(&c->h_res, RES_DOUBLES * sizeof(double)));
   GPX_CUDA(cudaMallocHost(&c->h_info, sizeof(int)));
   {   // keep freed temporaries of the stand-alone calls cached in the device's default pool
     cudaMemPool_t pool;
@@ -598,11 +599,21 @@ static int build_Ky(gpx_ctx* c, double extra_jitter, bool int8, Recorder& rec, c
   const int nt = (int)(c->Npad / TILE);
   *first_rows = nullptr;
   if (c->multi && c->m_cap != c->Npad) {
-    for (double** mp : {&c->mXsT, &c->msq, &c->mpartials}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
+    for (double** mp : {&c->mXsT, &c->msq}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
     GPX_CUDA(cudaMalloc(&c->mXsT, (size_t)MAX_D * c->Npad * 8));
     GPX_CUDA(cudaMalloc(&c->msq, (size_t)MAX_PARTS * c->Npad * 8));
-    GPX_CUDA(cudaMalloc(&c->mpartials, (size_t)MAX_PARTS * nt * nt * (MAX_D + 2) * 8));
     c->m_cap = c->Npad;
+  }
+  if (c->multi) {   // the parts' reduction partials, sized by the parts of this evaluation
+    size_t need = 0;
+    for (int q = 0; q < c->mk.nparts; q++) need += (size_t)nt * nt * part_nred(c->mk.part[q]);
+    if (need > c->mpart_cap) {
+      if (c->mpartials) cudaFree(c->mpartials);
+      c->mpartials = nullptr;
+      c->mpart_cap = 0;
+      GPX_CUDA(cudaMalloc(&c->mpartials, need * 8));
+      c->mpart_cap = need;
+    }
   }
   const Points tr = train_points(c);
   GPX_CHECK(prep_points(c, ctx_kern(c), c->dX, c->N, c->Npad, tr.xT, tr.sq));
@@ -663,7 +674,11 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
     rec.end(h);
     c->eval_launches += int8 ? 2 : 3;
   }
-  auto mpart = [&](int q) { return c->mpartials + (size_t)q * nt * nt * (MAX_D + 2); };
+  auto mpart = [&](int q) {
+    size_t off = 0;
+    for (int p = 0; p < q; p++) off += (size_t)nt * nt * part_nred(c->mk.part[p]);
+    return c->mpartials + off;
+  };
   long grad_tiles = (long)nt * nt;
   if (route == KINV_FUSED) {
     GPX_CHECK(run_lauum(c, nullptr, &rec));
@@ -681,8 +696,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
     }
     if (c->multi) {   // one reduction pass per part
       for (int q = 0; q < c->mk.nparts; q++) {
-        const int nred = std::max(1, part_nl(c->mk.part[q])) + 2;
-        GPX_CUDA(cudaMemsetAsync(mpart(q), 0, (size_t)nt * nt * nred * 8, st));
+        GPX_CUDA(cudaMemsetAsync(mpart(q), 0, (size_t)nt * nt * part_nred(c->mk.part[q]) * 8, st));
         GradKinvMultiParams gm;
         memset(&gm, 0, sizeof(gm));
         gm.Kinv = c->Kinv; gm.ld = ld; gm.XsT = c->mXsT; gm.sq = c->msq; gm.ldx = c->Npad; gm.alpha = c->dAlpha;
@@ -726,16 +740,19 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
     GPX_CHECK(launch_finalize(f, st));
   }
   c->eval_launches++;
-  const size_t nres = c->multi ? MAX_D + 2 * MAX_PARTS + 8 : nl + 5;
+  size_t nres = nl + 5;
+  if (c->multi) {
+    nres = 4;
+    for (int q = 0; q < c->mk.nparts; q++) nres += part_ngrad(c->mk.part[q]);
+  }
   GPX_CUDA(cudaMemcpyAsync(c->h_res, c->res, nres * sizeof(double), cudaMemcpyDeviceToHost, st));
   GPX_CUDA(cudaMemcpyAsync(c->h_info, c->info, sizeof(int), cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
-// noise_vec == nullptr: homoscedastic (`noise`); else N per-point variances (`noise` = their mean, used by the ladder)
-static int fill_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double* kdiag_total) {
+// the parts of a composite kernel -> mk (validated), *kdiag_total = Kdiag of the composite kernel. Dfull: columns of X.
+static int fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Dfull, double* kdiag_total) {
   if (!parts || nparts < 1 || nparts > MAX_PARTS) GPX_FAIL("number of kernel parts must be in [1, 8]");
-  MultiKern& mk = c->mk;
   memset(&mk, 0, sizeof(mk));
   mk.nparts = nparts;
   int off = 0;
@@ -743,25 +760,35 @@ static int fill_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double
   for (int p = 0; p < nparts; p++) {
     const gpx_kern_part& in = parts[p];
     PartDev& pd = mk.part[p];
-    if (in.kind < 0 || in.kind > GPX_BIAS) GPX_FAIL("unknown kernel kind");
+    if (!is_known(in.kind)) GPX_FAIL("unknown kernel kind");
     if (!(in.variance > 0)) GPX_FAIL("variance must be positive");
     if (p > 0 && in.term < parts[p - 1].term) GPX_FAIL("kernel parts must be ordered by term");
-    const bool stat = in.kind >= GPX_WHITE;
+    const bool stat = is_static(in.kind), periodic = in.kind == GPX_STDPERIODIC;
     if (!stat && (in.ndims < 1 || !in.dims || !in.lengthscale)) GPX_FAIL("a stationary part needs active dims and a lengthscale");
-    pd.kind = in.kind; pd.ard = (!stat && in.ard) ? 1 : 0; pd.term = in.term; pd.D = stat ? 0 : in.ndims; pd.xoff = off;
-    pd.variance = in.variance; pd.inv_ls_iso = 1.0;
+    if (periodic && !in.period) GPX_FAIL("a StdPeriodic part needs a period");
+    if (in.kind == GPX_RATQUAD && !(in.power > 0)) GPX_FAIL("power must be positive");
+    pd.kind = in.kind; pd.ard = (!stat && in.ard) ? 1 : 0; pd.ard_period = (periodic && in.ard_period) ? 1 : 0;
+    pd.term = in.term; pd.D = stat ? 0 : in.ndims; pd.xoff = off;
+    pd.variance = in.variance; pd.inv_ls_iso = 1.0; pd.power = in.kind == GPX_RATQUAD ? in.power : 0.0;
     if (off + pd.D > MAX_D) GPX_FAIL("the parts' active dims add up to more than 64");
+    if (part_nacc(pd) > MAX_D) GPX_FAIL("a StdPeriodic part on more than 32 active dims: its gradient reduction does not fit");
     for (int q = 0; q < pd.D; q++) {
-      if (in.dims[q] < 0 || in.dims[q] >= c->D) GPX_FAIL("active dim outside the data");
+      if (in.dims[q] < 0 || in.dims[q] >= Dfull) GPX_FAIL("active dim outside the data");
       const double l = in.lengthscale[pd.ard ? q : 0];
       if (!(l > 0)) GPX_FAIL("lengthscale must be positive");
       mk.dims[off + q] = in.dims[q];
       mk.ls[off + q] = l;
+      if (periodic) {
+        const double T = in.period[pd.ard_period ? q : 0];
+        if (!(T > 0)) GPX_FAIL("period must be positive");
+        mk.period[off + q] = T;
+      }
     }
-    if (!stat && !pd.ard) pd.inv_ls_iso = 1.0 / in.lengthscale[0];
+    if (is_stationary(pd.kind) && !pd.ard) pd.inv_ls_iso = 1.0 / in.lengthscale[0];
     off += pd.D;
     if (p > 0 && in.term != parts[p - 1].term) { total += prod; prod = 1.0; }
-    prod *= in.variance;                      // every kind has Kdiag = variance (stationary.py:170-173, static.py:30-33)
+    prod *= in.variance;      // every kind has Kdiag = variance (stationary.py:170-173, static.py:30-33,
+                              // standard_periodic.py:134-138)
   }
   total += prod;
   mk.sumD = off;
@@ -769,6 +796,11 @@ static int fill_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double
   return 0;
 }
 
+static int fill_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double* kdiag_total) {
+  return fill_mk(c->mk, parts, nparts, c->D, kdiag_total);
+}
+
+// noise_vec == nullptr: homoscedastic (`noise`); else N per-point variances (`noise` = their mean, used by the ladder)
 static int exact_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, double noise,
                            const double* noise_vec, double jitter, int max_tries, double* lml, double* grad,
                            double* dnoise, double* jitter_used, const gpx_kern_part* parts = nullptr, int nparts = 0) {
@@ -856,7 +888,7 @@ static int exact_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const
   *lml = c->h_res[0];
   if (c->multi) {
     int n = 0;
-    for (int p = 0; p < c->mk.nparts; p++) n += 1 + part_nl(c->mk.part[p]);
+    for (int p = 0; p < c->mk.nparts; p++) n += part_ngrad(c->mk.part[p]);
     for (int q = 0; q < n; q++) grad[q] = c->h_res[4 + q];
     grad[n] = c->h_res[3];
   } else
@@ -1066,10 +1098,109 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
   return rc;
 }
 
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// stand-alone K / update_gradients_full of one composite part (kinds 0-3, 6, 7) with the K-build and the per-pair gradient
+// terms of the composite evaluation; the context's own kernel (c->mk, c->kp) is left alone
+// ---------------------------------------------------------------------------------------------------------------
+static int fill_one_part(const gpx_kern_part* part, int D, MultiKern& mk) {
+  if (!part) GPX_FAIL("null argument");
+  if (is_known(part->kind) && is_static(part->kind)) GPX_FAIL("White / Bias parts have no stand-alone entry");
+  if (D < 1 || D > MAX_D) GPX_FAIL("input dimension must be in [1, 64]");
+  gpx_kern_part one = *part;
+  one.term = 0;
+  double kdiag;
+  return fill_mk(mk, &one, 1, D, &kdiag);
+}
+
+// n host points (n x D row-major) stacked for the one-part kernel mk into temporaries owned by ps
+static int upload_part_points(gpx_ctx* c, const MultiKern& mk, int D, const double* X, long n, PointSet& ps) {
+  ps.n = n; ps.ld = (n + TILE - 1) / TILE * TILE; ps.st = c->st;
+  GPX_TMP_ALLOC(&ps.raw, (size_t)n * D * 8, c->st);
+  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * mk.sumD * 8, c->st);
+  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * 8, c->st);
+  GPX_CUDA(cudaMemcpyAsync(ps.raw, X, (size_t)n * D * 8, cudaMemcpyHostToDevice, c->st));
+  GPX_CHECK(launch_prep_multi(ps.raw, n, D, ps.ld, mk, ps.xT, ps.sq, c->st));
+  c->total_launches++;
+  return 0;
+}
+
+extern "C" {
+
+int gpx_kern_part_K(gpx_ctx* c, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M, int D,
+                    double* out) {
+  if (!X || !out) GPX_FAIL("null argument");
+  MultiKern mk;
+  GPX_CHECK(fill_one_part(part, D, mk));
+  if (!X2) M = N;
+  if (N < 1 || M < 1) GPX_FAIL("empty input");
+  if (!c) GPX_CHECK(scratch_ctx(&c));
+  GPX_CUDA(cudaSetDevice(c->device));
+  PointSet p1, p2;
+  GPX_CHECK(upload_part_points(c, mk, D, X, N, p1));
+  if (X2) GPX_CHECK(upload_part_points(c, mk, D, X2, M, p2));
+  const PointSet& pj = X2 ? p2 : p1;   // thread-mapped operand = X2 points (contiguous index of the row-major output)
+  double* dout = nullptr;
+  GPX_TMP_ALLOC(&dout, (size_t)N * M * 8, c->st);
+  KBuildMultiParams kb;
+  memset(&kb, 0, sizeof(kb));
+  kb.rowsT = pj.xT; kb.ld_rows = pj.ld; kb.sq_rows = pj.sq;
+  kb.colsT = p1.xT; kb.ld_cols = p1.ld; kb.sq_cols = p1.sq;
+  kb.out = dout; kb.ld = M; kb.nrows = M; kb.ncols = N; kb.same = X2 == nullptr; kb.mk = mk;
+  int rc = launch_kbuild_multi(kb, (int)(pj.ld / TILE), (int)(p1.ld / TILE), c->st);
+  c->total_launches++;
+  if (rc == 0 && cudaMemcpyAsync(out, dout, (size_t)N * M * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
+  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error("gpx_kern_part_K: device failure"); rc = -1; }
+  GPX_TMP_FREE(dout, c->st);
+  return rc;
+}
+
+int gpx_kern_part_grad_full(gpx_ctx* c, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M,
+                            int D, const double* dL_dK, double* grad) {
+  if (!X || !dL_dK || !grad) GPX_FAIL("null argument");
+  MultiKern mk;
+  GPX_CHECK(fill_one_part(part, D, mk));
+  if (!X2) M = N;
+  if (N < 1 || M < 1) GPX_FAIL("empty input");
+  if (!c) GPX_CHECK(scratch_ctx(&c));
+  GPX_CUDA(cudaSetDevice(c->device));
+  PointSet p1, p2;
+  GPX_CHECK(upload_part_points(c, mk, D, X, N, p1));
+  if (X2) GPX_CHECK(upload_part_points(c, mk, D, X2, M, p2));
+  const PointSet& pj = X2 ? p2 : p1;
+  const int rtiles = (int)(pj.ld / TILE), ctiles = (int)(p1.ld / TILE), nred = part_nred(mk.part[0]);
+  double *dd = nullptr, *dpart = nullptr;
+  GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
+  GPX_TMP_ALLOC(&dpart, (size_t)rtiles * ctiles * nred * 8, c->st);
+  GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
+  GradFullMultiParams gf;
+  memset(&gf, 0, sizeof(gf));
+  gf.rowsT = pj.xT; gf.ld_rows = pj.ld; gf.sq_rows = pj.sq;
+  gf.colsT = p1.xT; gf.ld_cols = p1.ld; gf.sq_cols = p1.sq;
+  gf.nrows = M; gf.ncols = N; gf.same = X2 == nullptr; gf.dL = dd; gf.partials = dpart; gf.mk = mk;
+  int rc = launch_grad_full_multi(gf, rtiles, ctiles, c->st);
+  c->total_launches++;
+  std::vector<double> hp((size_t)rtiles * ctiles * nred);
+  if (rc == 0 && cudaMemcpyAsync(hp.data(), dpart, hp.size() * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
+  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error("gpx_kern_part_grad_full: device failure"); rc = -1; }
+  GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
+  if (rc) return rc;
+  std::vector<double> tot(nred, 0.0);   // the tiles' partials in fixed order
+  for (size_t t = 0; t < hp.size() / nred; t++)
+    for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
+  for (int t = 0; t < nred; t++) {
+    double v;
+    if (part_grad_entry(mk, 0, t, tot[t], &v)) grad[t] = v;
+  }
+  return 0;
+}
+
+}  // extern "C"
+
 // ---------------------------------------------------------------------------------------------------------------
 // stand-alone pdinv / jitchol for a caller-supplied symmetric matrix (GPy/util/linalg.py:56-75,193-214)
 // ---------------------------------------------------------------------------------------------------------------
-}  // extern "C"
 
 // size the workspace of c for an N x N matrix: bind N dummy points (D = 1, P = 1) unless such a data set is bound already
 static int bind_dummy_data(gpx_ctx* c, long N) {

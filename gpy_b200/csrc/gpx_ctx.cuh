@@ -79,8 +79,9 @@ struct gpx_ctx {
   gpx::MultiKern mk{};
   double* mXsT = nullptr;      // [sumD][Npad] stacked scaled inputs of the parts
   double* msq = nullptr;       // [nparts][Npad]
-  double* mpartials = nullptr; // [MAX_PARTS][nt*nt][MAX_D+2]
-  long m_cap = 0;              // Npad the three buffers were sized for
+  double* mpartials = nullptr; // per part p in turn: [nt*nt][part_nred(p)]
+  long m_cap = 0;              // Npad mXsT and msq were sized for
+  size_t mpart_cap = 0;        // doubles mpartials holds
   struct DistState* dist = nullptr;   // multi-GPU state (gpx_dist.cu), null on a single GPU
   struct SparseState* sparse = nullptr;   // sparse-GP (VarDTC) state (gpx_sparse.cu)
 };

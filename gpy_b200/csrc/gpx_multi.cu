@@ -1,4 +1,4 @@
-// gpx_multi.cu — composite kernels (sums of products of stationary / White / Bias parts) evaluated on the device:
+// gpx_multi.cu — composite kernels (sums of products of stationary / StdPeriodic / White / Bias parts) evaluated on the device:
 // covariance build, gradient reductions from the stored K^-1 and the final assembly. See gpx_multi.cuh for the references.
 #include <algorithm>
 #include <cstring>
@@ -9,8 +9,10 @@
 namespace gpx {
 
 // ---------------------------------------------------------------------------------------------------------------
-// prep: every part's active dims scaled the way its own Stationary._scaled_dist does (stationary.py:151-168: ARD divides
-// by the lengthscale before the expansion, iso afterwards), stacked as SoA rows, plus per-part squared norms
+// prep: every part's active dims stacked as SoA rows, plus per-part squared norms. A stationary part's dims are scaled the
+// way its own Stationary._scaled_dist does (stationary.py:151-168: ARD divides by the lengthscale before the expansion, iso
+// afterwards). A StdPeriodic part's dims stay unscaled: its argument pi (x - x') / T is formed from raw differences like
+// standard_periodic.py:130 does, so that time-like inputs (years near 2000, period 1) keep the digits the reference keeps.
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void prep_multi_kernel(const double* __restrict__ X, long N, int Dfull, long ld, MultiKern mk,
                                   double* __restrict__ XsT, double* __restrict__ sq) {
@@ -18,12 +20,13 @@ __global__ void prep_multi_kernel(const double* __restrict__ X, long N, int Dful
   if (i >= ld) return;
   for (int p = 0; p < mk.nparts; p++) {
     const PartDev& pd = mk.part[p];
+    const bool scale = pd.ard && is_stationary(pd.kind);
     double s = 0.0;
     for (int q = 0; q < pd.D; q++) {
       double v = 0.0;
       if (i < N) {
         v = X[i * Dfull + mk.dims[pd.xoff + q]];
-        if (pd.ard) v = v / mk.ls[pd.xoff + q];
+        if (scale) v = v / mk.ls[pd.xoff + q];
       }
       XsT[(long)(pd.xoff + q) * ld + i] = v;
       s += v * v;
@@ -39,25 +42,50 @@ int launch_prep_multi(const double* X, long N, int Dfull, long ld, const MultiKe
   return 0;
 }
 
-// value of one part at a pair of points held in shared-memory tiles (row point il, column point jl), unit handling of the
-// static kinds: White = variance on coincident points of the SAME set (static.py:75-79), Bias = variance (static.py:155-157)
-__device__ __forceinline__ double part_value(const MultiKern& mk, int p, const double* sR, const double* sC, const double* sSr,
-                                             const double* sSc, int il, int jl, bool samept, double* r_out, double* dk_out) {
+// scaled distance r of a stationary part at a pair of points held in shared-memory tiles (row point il, column point jl)
+__device__ __forceinline__ double part_r(const MultiKern& mk, int p, const double* sR, const double* sC, const double* sSr,
+                                         const double* sSc, int il, int jl, bool samept) {
   const PartDev& pd = mk.part[p];
-  if (pd.kind == GPX_BIAS) { if (r_out) { *r_out = 0.0; *dk_out = 0.0; } return 1.0; }
-  if (pd.kind == GPX_WHITE) { if (r_out) { *r_out = 0.0; *dk_out = 0.0; } return samept ? 1.0 : 0.0; }
   double dot = 0.0;
   for (int q = 0; q < pd.D; q++) dot = fma(sR[(pd.xoff + q) * TILE + il], sC[(pd.xoff + q) * TILE + jl], dot);
   double r2 = sSr[p * TILE + il] + sSc[p * TILE + jl] - 2.0 * dot;
   if (samept) r2 = 0.0;
   r2 = fmax(r2, 0.0);
-  const double rr = sqrt(r2) * pd.inv_ls_iso;
-  if (r_out) {
-    double k, dk;
-    k_dk_of_r_unit(pd.kind, rr, k, dk);
-    *r_out = rr; *dk_out = dk;
-    return k;
+  return sqrt(r2) * pd.inv_ls_iso;
+}
+
+// RatQuad at unit variance: k = (1 + r^2/2)^-power, dk/dr = -power r (1 + r^2/2)^(-power-1) (stationary.py:785-793);
+// lg = log1p(r^2/2) is what the power gradient needs (:797)
+__device__ __forceinline__ void ratquad_k_dk(double power, double r, double& k, double& dk, double& lg) {
+  lg = log1p(0.5 * r * r);
+  k = exp(-power * lg);
+  dk = -power * r * exp(-(power + 1.0) * lg);
+}
+
+// StdPeriodic at unit variance (standard_periodic.py:125-132): exp(-1/2 sum_q (sin(pi d_q / T_q) / l_q)^2)
+__device__ __forceinline__ double periodic_k(const MultiKern& mk, const PartDev& pd, const double* sR, const double* sC, int il,
+                                             int jl) {
+  double arg = 0.0;
+  for (int q = 0; q < pd.D; q++) {
+    const double d = sR[(pd.xoff + q) * TILE + il] - sC[(pd.xoff + q) * TILE + jl];
+    const double t = sinpi(d / mk.period[pd.xoff + q]) / mk.ls[pd.xoff + q];
+    arg = fma(t, t, arg);
   }
+  return exp(-0.5 * arg);
+}
+
+// value of one part at unit variance, static kinds: White = variance on coincident points of the SAME set
+// (static.py:75-79), Bias = variance (static.py:155-157). EXT: the kernel may contain RatQuad / StdPeriodic parts; the
+// instantiations without them keep the code (and the register budget) of the kinds RBF .. Matern52, White, Bias.
+template <bool EXT>
+__device__ __forceinline__ double part_value(const MultiKern& mk, int p, const double* sR, const double* sC, const double* sSr,
+                                             const double* sSc, int il, int jl, bool samept) {
+  const PartDev& pd = mk.part[p];
+  if (pd.kind == GPX_BIAS) return 1.0;
+  if (pd.kind == GPX_WHITE) return samept ? 1.0 : 0.0;
+  if (EXT && pd.kind == GPX_STDPERIODIC) return periodic_k(mk, pd, sR, sC, il, jl);
+  const double rr = part_r(mk, p, sR, sC, sSr, sSc, il, jl, samept);
+  if (EXT && pd.kind == GPX_RATQUAD) return exp(-pd.power * log1p(0.5 * rr * rr));
   return k_of_r_unit(pd.kind, rr);
 }
 
@@ -80,6 +108,7 @@ __device__ __forceinline__ void load_tiles(const MultiKern& mk, const double* ro
 // covariance build: K = sum_t prod_{p in t} k_p (add.py:60-74, prod.py:59-68), `sym` mode = factor workspace image
 // (lower tiles, zero upper tiles, identity padding, + (noise + jitter) on the diagonal: exact_gaussian_inference.py:55-56)
 // ---------------------------------------------------------------------------------------------------------------
+template <bool EXT>
 __global__ void __launch_bounds__(256) kbuild_multi_kernel(KBuildMultiParams p) {
   extern __shared__ __align__(128) unsigned char km_smem[];
   const MultiKern& mk = p.mk;
@@ -107,7 +136,7 @@ __global__ void __launch_bounds__(256) kbuild_multi_kernel(KBuildMultiParams p) 
     int cur = mk.part[0].term;
     for (int q = 0; q < mk.nparts; q++) {
       if (mk.part[q].term != cur) { val += prod; prod = 1.0; cur = mk.part[q].term; }
-      prod *= mk.part[q].variance * part_value(mk, q, sR, sC, sSr, sSc, il, jl, samept, nullptr, nullptr);
+      prod *= mk.part[q].variance * part_value<EXT>(mk, q, sR, sC, sSr, sSc, il, jl, samept);
     }
     val += prod;
     if (p.sym) {
@@ -120,28 +149,161 @@ __global__ void __launch_bounds__(256) kbuild_multi_kernel(KBuildMultiParams p) 
   }
 }
 
-static size_t multi_tile_smem(const MultiKern& mk) { return (size_t)(2 * mk.sumD + 2 * mk.nparts) * TILE * 8 + 8 * (MAX_D + 2) * 8; }
+constexpr int MAX_NRED = MAX_D + 3;   // largest part_nred: an ARD RatQuad part on 64 dims
 
-int launch_kbuild_multi(const KBuildMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st) {
+// any RatQuad / StdPeriodic part: the kernels' EXT instantiation
+static bool has_ext(const MultiKern& mk) {
+  for (int q = 0; q < mk.nparts; q++)
+    if (mk.part[q].kind == GPX_RATQUAD || mk.part[q].kind == GPX_STDPERIODIC) return true;
+  return false;
+}
+
+static int max_nred(const MultiKern& mk) {
+  int m = 0;
+  for (int q = 0; q < mk.nparts; q++) m = std::max(m, part_nred(mk.part[q]));
+  return m;
+}
+static size_t multi_tile_smem(const MultiKern& mk) {
+  return (size_t)(2 * mk.sumD + 2 * mk.nparts) * TILE * 8 + 8 * (size_t)max_nred(mk) * 8;
+}
+static constexpr int MAX_MULTI_SMEM = (2 * MAX_D + 2 * MAX_PARTS) * TILE * 8 + 8 * MAX_NRED * 8;
+
+template <bool EXT>
+static int launch_kbm_t(const KBuildMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    GPX_CUDA(cudaFuncSetAttribute(kbuild_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)((2 * MAX_D + 2 * MAX_PARTS) * TILE * 8 + 8 * (MAX_D + 2) * 8)));
+    GPX_CUDA(cudaFuncSetAttribute(kbuild_multi_kernel<EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_MULTI_SMEM));
     attr_set = true;
   }
-  kbuild_multi_kernel<<<dim3(col_tiles, row_tiles), 256, multi_tile_smem(p.mk), st>>>(p);
+  kbuild_multi_kernel<EXT><<<dim3(col_tiles, row_tiles), 256, multi_tile_smem(p.mk), st>>>(p);
   GPX_CUDA(cudaGetLastError());
   return 0;
 }
 
+int launch_kbuild_multi(const KBuildMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st) {
+  return has_ext(p.mk) ? launch_kbm_t<true>(p, row_tiles, col_tiles, st) : launch_kbm_t<false>(p, row_tiles, col_tiles, st);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
-// gradient reductions of ONE part from the stored K^-1: with dL_dK = 1/2 (alpha alpha^T - P K^-1) the part sees
-// dL_dK o prod(other factors of its term) (prod.py:377-396; add.py:76-99 passes dL_dK through unchanged) and reduces it
-// exactly like Stationary.update_gradients_full (stationary.py:193-243), White (static.py:88-92: trace) or Bias
-// (static.py:172-173: sum). One CTA per lower 128 x 128 tile, thread-mapped index = row (contiguous in K^-1).
+// gradient reductions of ONE part: the part sees dL_dK o prod(other factors of its term) (prod.py:377-396; add.py:76-99
+// passes dL_dK through unchanged) and reduces it exactly like Stationary.update_gradients_full (stationary.py:193-243),
+// RatQuad's (stationary.py:795-798: power sum of dL * -k log1p(r^2/2)), StdPeriodic's (standard_periodic.py:501-526),
+// White (static.py:88-92: trace) or Bias (static.py:172-173: sum). Two sources of dL_dK share the per-pair work below:
+// 1/2 (alpha alpha^T - P K^-1) from the stored K^-1 (grad_kinv_multi) and a caller's dense matrix (grad_full_multi).
 // ---------------------------------------------------------------------------------------------------------------
-template <int DREG>
-__global__ void __launch_bounds__(256) grad_kinv_multi_kernel(GradKinvMultiParams p) {
+struct PairSums {   // per-thread sums of one part, besides the per-dim accumulators
+  double var = 0.0, iso = 0.0, power = 0.0, noise = 0.0;
+};
+
+// one pair (row point il, column point jl) with dL_dK entry dl and weight w (2 for an off-diagonal tile of a symmetric
+// sweep). xi: the row point's stacked inputs of the part. gq: ARD lengthscale sums of a stationary part; a StdPeriodic part
+// keeps its period sums in gq[0, DREG/2) and its lengthscale sums in gq[DREG/2, DREG) (the launch picks DREG >= 2 D).
+template <int DREG, bool EXT>
+__device__ __forceinline__ void pair_accumulate(const MultiKern& mk, int pidx, const PartDev& me, const double* sR,
+                                                const double* sC, const double* sSr, const double* sSc, int il, int jl,
+                                                bool samept, double w, double dl, const double (&xi)[DREG],
+                                                double (&gq)[DREG], PairSums& s) {
+  for (int q = 0; q < mk.nparts; q++)       // the other factors of this part's term
+    if (q != pidx && mk.part[q].term == me.term)
+      dl *= mk.part[q].variance * part_value<EXT>(mk, q, sR, sC, sSr, sSc, il, jl, samept);
+  if (EXT && me.kind == GPX_STDPERIODIC) {
+    constexpr int H = DREG / 2;
+    const double k = periodic_k(mk, me, sR, sC, il, jl);
+    s.var = fma(w * k, dl, s.var);
+    const double W = w * me.variance * k * dl;
+#pragma unroll
+    for (int q = 0; q < H; q++)
+      if (q < me.D) {
+        const double T = mk.period[me.xoff + q], l = mk.ls[me.xoff + q];
+        const double u = (xi[q] - sC[(me.xoff + q) * TILE + jl]) / T;
+        double sn, cs;
+        sincospi(u, &sn, &cs);
+        const double base = 3.141592653589793 * u;
+        gq[q] = fma(W, sn * cs * (base / T) / (l * l), gq[q]);          // standard_periodic.py:511,518-521
+        gq[H + q] = fma(W, sn * sn / (l * l * l), gq[H + q]);            // :513,523-526
+      }
+    return;
+  }
+  double rr = 0.0, k, dk = 0.0;
+  if (is_static(me.kind)) {
+    k = part_value<EXT>(mk, pidx, sR, sC, sSr, sSc, il, jl, samept);
+  } else {
+    rr = part_r(mk, pidx, sR, sC, sSr, sSc, il, jl, samept);
+    if (EXT && me.kind == GPX_RATQUAD) {
+      double lg;
+      ratquad_k_dk(me.power, rr, k, dk, lg);
+      s.power = fma(w * dl, -me.variance * k * lg, s.power);
+    } else {
+      k_dk_of_r_unit(me.kind, rr, k, dk);
+    }
+  }
+  s.var = fma(w * k, dl, s.var);
+  const double G = me.variance * dk * dl;
+  if (me.ard && is_stationary(me.kind)) {
+    const double tmpv = (rr != 0.0) ? w * G / rr : 0.0;     // stationary.py:205,225-232: 1/r with 1/0 := 0
+#pragma unroll
+    for (int q = 0; q < DREG; q++)
+      if (q < me.D) {
+        const double df = xi[q] - sC[(me.xoff + q) * TILE + jl];
+        gq[q] = fma(tmpv, df * df, gq[q]);
+      }
+  } else {
+    s.iso = fma(w * G, rr, s.iso);
+  }
+}
+
+// the CTA's sums of one part into out[part_nred], in the order of its gradient block, tr(dL_dK) last. All threads call it.
+template <int DREG, bool EXT>
+__device__ __forceinline__ void store_part_sums(const PartDev& me, PairSums s, double (&gq)[DREG], double* sRed, double* out) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int nred = part_nred(me);
+  const int nl = me.ard ? me.D : 1;
+  double* red = sRed + warp * nred;
+  s.var = warp_sum(s.var);
+  s.noise = warp_sum(s.noise);
+  if (lane == 0) { red[0] = s.var; red[nred - 1] = s.noise; }
+  if (EXT && me.kind == GPX_STDPERIODIC) {
+    constexpr int H = DREG / 2;
+    const int np = me.ard_period ? me.D : 1;
+    double tp = 0.0, tl = 0.0;
+#pragma unroll
+    for (int q = 0; q < H; q++)
+      if (q < me.D) {
+        const double a = warp_sum(gq[q]), b = warp_sum(gq[H + q]);
+        tp += a; tl += b;
+        if (lane == 0 && me.ard_period) red[1 + q] = a;
+        if (lane == 0 && me.ard) red[1 + np + q] = b;
+      }
+    if (lane == 0 && !me.ard_period) red[1] = tp;                 // isotropic: summed over the dims (:520-521,:525-526)
+    if (lane == 0 && !me.ard) red[1 + np] = tl;
+  } else if (me.ard && is_stationary(me.kind)) {
+#pragma unroll
+    for (int q = 0; q < DREG; q++)
+      if (q < me.D) {
+        const double v = warp_sum(gq[q]);
+        if (lane == 0) red[1 + q] = v;
+      }
+  } else {
+    s.iso = warp_sum(s.iso);
+    if (lane == 0) red[1] = s.iso;
+  }
+  if (EXT && me.kind == GPX_RATQUAD) {
+    s.power = warp_sum(s.power);
+    if (lane == 0) red[1 + nl] = s.power;
+  }
+  __syncthreads();
+  if (tid < nred) {
+    double v = 0.0;
+#pragma unroll
+    for (int wdx = 0; wdx < 8; wdx++) v += sRed[wdx * nred + tid];
+    out[tid] = v;
+  }
+}
+
+// One CTA per lower 128 x 128 tile of the stored K^-1, thread-mapped index = row (contiguous in K^-1). The narrowest
+// instantiation without RatQuad / StdPeriodic parts keeps three CTAs per SM, as before those kinds existed.
+template <int DREG, bool EXT>
+__global__ void __launch_bounds__(256, DREG == 8 ? (EXT ? 2 : 3) : 1) grad_kinv_multi_kernel(GradKinvMultiParams p) {
   extern __shared__ __align__(128) unsigned char gm_smem[];
   const MultiKern& mk = p.mk;
   const int P = p.P;
@@ -154,20 +316,17 @@ __global__ void __launch_bounds__(256) grad_kinv_multi_kernel(GradKinvMultiParam
   while (r * (r + 1) / 2 > (int)blockIdx.x) --r;
   while ((r + 1) * (r + 2) / 2 <= (int)blockIdx.x) ++r;
   const int c = blockIdx.x - r * (r + 1) / 2;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   load_tiles(mk, p.XsT, p.ldx, p.sq, r, p.XsT, p.ldx, p.sq, c, sR, sC, sSr, sSc);
   __syncthreads();
   const PartDev me = mk.part[p.part];
-  const int D = me.D;
-  const bool ard = me.ard != 0 && me.kind < GPX_WHITE;
-  const int nl = me.kind >= GPX_WHITE ? 1 : (ard ? D : 1), nred = nl + 2;
   const int il = tid & (TILE - 1), half = tid >> 7;
   const long gi = (long)r * TILE + il;
   double xi[DREG], gq[DREG];
 #pragma unroll
-  for (int q = 0; q < DREG; q++) { gq[q] = 0.0; xi[q] = q < D ? sR[(me.xoff + q) * TILE + il] : 0.0; }
+  for (int q = 0; q < DREG; q++) { gq[q] = 0.0; xi[q] = q < me.D ? sR[(me.xoff + q) * TILE + il] : 0.0; }
   const double w = (r > c) ? 2.0 : 1.0;
-  double gvar = 0.0, giso = 0.0, gnoise = 0.0;
+  PairSums s;
   const double* kcol = p.Kinv + gi + ((long)c * TILE + half * 64) * p.ld;
   if (gi < p.N) {
     for (int jj = 0; jj < 64; jj++) {
@@ -178,72 +337,104 @@ __global__ void __launch_bounds__(256) grad_kinv_multi_kernel(GradKinvMultiParam
       const double kinv = kcol[(long)jj * p.ld];
       double aa = 0.0;
       for (int q = 0; q < P; q++) aa = fma(p.alpha[(long)q * p.ldx + gi], p.alpha[(long)q * p.ldx + gj], aa);
-      double dl = 0.5 * (aa - (double)P * kinv);
-      if (samept) gnoise += dl;
-      for (int q = 0; q < mk.nparts; q++)       // the other factors of this part's term
-        if (q != p.part && mk.part[q].term == me.term)
-          dl *= mk.part[q].variance * part_value(mk, q, sR, sC, sSr, sSc, il, jl, samept, nullptr, nullptr);
-      double rr, dk;
-      const double k = part_value(mk, p.part, sR, sC, sSr, sSc, il, jl, samept, &rr, &dk);
-      gvar = fma(w * k, dl, gvar);
-      const double G = me.variance * dk * dl;
-      if (ard) {
-        const double tmpv = (rr != 0.0) ? w * G / rr : 0.0;     // stationary.py:205,225-232: 1/r with 1/0 := 0
-#pragma unroll
-        for (int q = 0; q < DREG; q++)
-          if (q < D) {
-            const double df = xi[q] - sC[(me.xoff + q) * TILE + jl];
-            gq[q] = fma(tmpv, df * df, gq[q]);
-          }
-      } else {
-        giso = fma(w * G, rr, giso);
-      }
+      const double dl = 0.5 * (aa - (double)P * kinv);
+      if (samept) s.noise += dl;
+      pair_accumulate<DREG, EXT>(mk, p.part, me, sR, sC, sSr, sSc, il, jl, samept, w, dl, xi, gq, s);
     }
   }
-  gvar = warp_sum(gvar);
-  gnoise = warp_sum(gnoise);
-  if (lane == 0) { sRed[warp * nred] = gvar; sRed[warp * nred + nred - 1] = p.want_noise ? gnoise : 0.0; }
-  if (ard) {
-#pragma unroll
-    for (int q = 0; q < DREG; q++)
-      if (q < D) {
-        const double s = warp_sum(gq[q]);
-        if (lane == 0) sRed[warp * nred + 1 + q] = s;
-      }
-  } else {
-    giso = warp_sum(giso);
-    if (lane == 0) sRed[warp * nred + 1] = giso;
-  }
-  __syncthreads();
-  if (tid < nred) {
-    double s = 0.0;
-#pragma unroll
-    for (int wdx = 0; wdx < 8; wdx++) s += sRed[wdx * nred + tid];
-    p.partials[((long)r * p.nt + c) * nred + tid] = s;
-  }
+  if (!p.want_noise) s.noise = 0.0;
+  store_part_sums<DREG, EXT>(me, s, gq, sRed, p.partials + ((long)r * p.nt + c) * part_nred(me));
 }
 
-template <int DREG>
+// One CTA per 128 x 128 tile of a caller's dense dL_dK: thread-mapped index = row point (contiguous in dL_dK).
+template <int DREG, bool EXT>
+__global__ void __launch_bounds__(256) grad_full_multi_kernel(GradFullMultiParams p) {
+  extern __shared__ __align__(128) unsigned char gf_smem[];
+  const MultiKern& mk = p.mk;
+  double* sR = reinterpret_cast<double*>(gf_smem);
+  double* sC = sR + (size_t)mk.sumD * TILE;
+  double* sSr = sC + (size_t)mk.sumD * TILE;
+  double* sSc = sSr + (size_t)mk.nparts * TILE;
+  double* sRed = sSc + (size_t)mk.nparts * TILE;
+  const int ct = blockIdx.x, rt = blockIdx.y;
+  const int tid = threadIdx.x;
+  load_tiles(mk, p.rowsT, p.ld_rows, p.sq_rows, rt, p.colsT, p.ld_cols, p.sq_cols, ct, sR, sC, sSr, sSc);
+  __syncthreads();
+  const PartDev me = mk.part[0];
+  const int il = tid & (TILE - 1), half = tid >> 7;
+  const long gi = (long)rt * TILE + il;
+  double xi[DREG], gq[DREG];
+#pragma unroll
+  for (int q = 0; q < DREG; q++) { gq[q] = 0.0; xi[q] = q < me.D ? sR[(me.xoff + q) * TILE + il] : 0.0; }
+  PairSums s;
+  if (gi < p.nrows) {
+    for (int jj = 0; jj < 64; jj++) {
+      const int jl = half * 64 + jj;
+      const long gj = (long)ct * TILE + jl;
+      if (gj >= p.ncols) break;
+      pair_accumulate<DREG, EXT>(mk, 0, me, sR, sC, sSr, sSc, il, jl, p.same && gi == gj, 1.0, p.dL[gj * p.nrows + gi], xi, gq, s);
+    }
+  }
+  store_part_sums<DREG, EXT>(me, s, gq, sRed, p.partials + ((long)ct * gridDim.y + rt) * part_nred(me));
+}
+
+// register accumulators for a part: its active dims and its per-dim sums (part_nacc <= MAX_D, checked by the caller)
+static int dreg_for(const PartDev& pd) { return std::max(pd.D, part_nacc(pd)); }
+
+template <int DREG, bool EXT>
 static int launch_gkm_t(const GradKinvMultiParams& p, unsigned grid, size_t smem, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    GPX_CUDA(cudaFuncSetAttribute(grad_kinv_multi_kernel<DREG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)((2 * MAX_D + 2 * MAX_PARTS) * TILE * 8 + 8 * (MAX_D + 2) * 8)));
+    GPX_CUDA(cudaFuncSetAttribute(grad_kinv_multi_kernel<DREG, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_MULTI_SMEM));
     attr_set = true;
   }
-  grad_kinv_multi_kernel<DREG><<<grid, 256, smem, st>>>(p);
+  grad_kinv_multi_kernel<DREG, EXT><<<grid, 256, smem, st>>>(p);
   GPX_CUDA(cudaGetLastError());
   return 0;
 }
 
 int launch_grad_kinv_multi(const GradKinvMultiParams& p, cudaStream_t st) {
-  const int D = p.mk.part[p.part].D;
+  const int D = dreg_for(p.mk.part[p.part]);
   const unsigned grid = (unsigned)(p.nt * (p.nt + 1) / 2);
   const size_t smem = multi_tile_smem(p.mk);
-  if (D <= 8) return launch_gkm_t<8>(p, grid, smem, st);
-  if (D <= 16) return launch_gkm_t<16>(p, grid, smem, st);
-  if (D <= 32) return launch_gkm_t<32>(p, grid, smem, st);
-  return launch_gkm_t<64>(p, grid, smem, st);
+  if (has_ext(p.mk)) {
+    if (D <= 8) return launch_gkm_t<8, true>(p, grid, smem, st);
+    if (D <= 16) return launch_gkm_t<16, true>(p, grid, smem, st);
+    if (D <= 32) return launch_gkm_t<32, true>(p, grid, smem, st);
+    return launch_gkm_t<64, true>(p, grid, smem, st);
+  }
+  if (D <= 8) return launch_gkm_t<8, false>(p, grid, smem, st);
+  if (D <= 16) return launch_gkm_t<16, false>(p, grid, smem, st);
+  if (D <= 32) return launch_gkm_t<32, false>(p, grid, smem, st);
+  return launch_gkm_t<64, false>(p, grid, smem, st);
+}
+
+template <int DREG, bool EXT>
+static int launch_gfm_t(const GradFullMultiParams& p, dim3 grid, size_t smem, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    GPX_CUDA(cudaFuncSetAttribute(grad_full_multi_kernel<DREG, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_MULTI_SMEM));
+    attr_set = true;
+  }
+  grad_full_multi_kernel<DREG, EXT><<<grid, 256, smem, st>>>(p);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int launch_grad_full_multi(const GradFullMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st) {
+  const int D = dreg_for(p.mk.part[0]);
+  const dim3 grid(col_tiles, row_tiles);
+  const size_t smem = multi_tile_smem(p.mk);
+  if (has_ext(p.mk)) {
+    if (D <= 8) return launch_gfm_t<8, true>(p, grid, smem, st);
+    if (D <= 16) return launch_gfm_t<16, true>(p, grid, smem, st);
+    if (D <= 32) return launch_gfm_t<32, true>(p, grid, smem, st);
+    return launch_gfm_t<64, true>(p, grid, smem, st);
+  }
+  if (D <= 8) return launch_gfm_t<8, false>(p, grid, smem, st);
+  if (D <= 16) return launch_gfm_t<16, false>(p, grid, smem, st);
+  if (D <= 32) return launch_gfm_t<32, false>(p, grid, smem, st);
+  return launch_gfm_t<64, false>(p, grid, smem, st);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -275,20 +466,18 @@ __global__ void __launch_bounds__(256) finalize_multi_kernel(FinalizeMultiParams
   }
   int off = 4;
   for (int p = 0; p < f.mk.nparts; p++) {
-    const PartDev& pd = f.mk.part[p];
-    const bool stat = pd.kind >= GPX_WHITE;
-    const int nl = stat ? 1 : (pd.ard ? pd.D : 1), nred = nl + 2;
+    const int nred = part_nred(f.mk.part[p]);
     for (int t = 0; t < nred; t++) {
       s = 0.0;
       for (long i = tid; i < f.ntiles; i += 256) s += f.partials[p][i * nred + t];
       const double tot = block_sum(s);
+      double v;
       if (tid == 0) {
-        if (t == 0) f.res[off] = tot;                                                 // d/d variance (stationary.py:199)
-        else if (t == nred - 1) { if (p == 0) f.res[3] = tot; }                        // tr(dL_dK) -> noise (gaussian.py:78-79)
-        else if (!stat) f.res[off + t] = -tot / f.mk.ls[pd.xoff + (pd.ard ? t - 1 : 0)];   // stationary.py:210,213
+        if (t == nred - 1) { if (p == 0) f.res[3] = tot; }                             // tr(dL_dK) -> noise (gaussian.py:78-79)
+        else if (part_grad_entry(f.mk, p, t, tot, &v)) f.res[off + t] = v;
       }
     }
-    off += 1 + (stat ? 0 : nl);
+    off += part_ngrad(f.mk.part[p]);
   }
 }
 

@@ -1,22 +1,27 @@
 // gpx_multi.cuh — composite kernels on the device (internal): K = sum over terms of products of parts, each part a
-// stationary kernel on its own active dims, a White or a Bias kernel. Mirrors GPy/kern/src/add.py:60-99 (Add.K /
-// update_gradients_full), prod.py:59-68,377-396 (Prod.K; each factor's gradient sees dL_dK times the other factors) and
-// static.py:63-185 (White, Bias).
+// stationary kernel (RBF .. Matern52, RatQuad) or a StdPeriodic kernel on its own active dims, a White or a Bias kernel.
+// Mirrors GPy/kern/src/add.py:60-99 (Add.K / update_gradients_full), prod.py:59-68,377-396 (Prod.K; each factor's gradient
+// sees dL_dK times the other factors), static.py:63-185 (White, Bias), stationary.py:747-802 (RatQuad) and
+// standard_periodic.py:56-94,125-139,501-548 (StdPeriodic).
 #pragma once
 #include "gpx_common.cuh"
 
 namespace gpx {
 
 constexpr int MAX_PARTS = 8;
+// largest result vector of an evaluation: 4 scalars, then every part's gradient block (at most 2 + 2 D entries per part)
+constexpr int RES_DOUBLES = 4 + 2 * MAX_D + 2 * MAX_PARTS;
 
 struct PartDev {
-  int kind;          // GPX_RBF .. GPX_MATERN52, GPX_WHITE, GPX_BIAS
-  int ard;
+  int kind;          // GPX_RBF .. GPX_MATERN52, GPX_WHITE, GPX_BIAS, GPX_RATQUAD, GPX_STDPERIODIC
+  int ard;           // lengthscale per dim (StdPeriodic: GPy's ARD2)
+  int ard_period;    // StdPeriodic: period per dim (GPy's ARD1)
   int term;          // parts with equal `term` are multiplied, terms are summed (parts sorted by term)
   int D;             // active dims (0 for the static kinds)
-  int xoff;          // first row of this part inside the stacked scaled-input SoA [sumD][ld]
+  int xoff;          // first row of this part inside the stacked input SoA [sumD][ld]
   double variance;
   double inv_ls_iso;
+  double power;      // RatQuad
 };
 
 struct MultiKern {
@@ -25,7 +30,32 @@ struct MultiKern {
   PartDev part[MAX_PARTS];
   int dims[MAX_D];       // column of X behind stacked row (xoff + q)
   double ls[MAX_D];      // its lengthscale (ARD: per dim; iso: the part's single lengthscale repeated)
+  double period[MAX_D];  // StdPeriodic: its period (ARD1: per dim; iso: repeated)
 };
+
+__host__ __device__ __forceinline__ bool is_static(int kind) { return kind == GPX_WHITE || kind == GPX_BIAS; }
+__host__ __device__ __forceinline__ bool is_known(int kind) { return kind >= GPX_RBF && kind <= GPX_STDPERIODIC; }
+// a function of the scaled distance r (stationary.py:23-243): RBF .. Matern52 and RatQuad
+__host__ __device__ __forceinline__ bool is_stationary(int kind) { return (kind >= GPX_RBF && kind <= GPX_MATERN52) || kind == GPX_RATQUAD; }
+
+// gradient entries of a part (its block of the result vector)
+__host__ __device__ inline int part_ngrad(const PartDev& pd) {
+  const int nl = pd.ard ? pd.D : 1;
+  switch (pd.kind) {
+    case GPX_WHITE: case GPX_BIAS: return 1;
+    case GPX_RATQUAD: return 2 + nl;                                   // variance, lengthscale(s), power
+    case GPX_STDPERIODIC: return 1 + (pd.ard_period ? pd.D : 1) + nl;  // variance, period(s), lengthscale(s)
+    default: return 1 + nl;
+  }
+}
+// per-tile partial sums of a part's reduction pass: its gradient entries and tr(dL_dK) (static kinds keep one unused slot)
+__host__ __device__ inline int part_nred(const PartDev& pd) { return is_static(pd.kind) ? 3 : part_ngrad(pd) + 1; }
+// per-dimension register accumulators of the reduction pass: ARD lengthscales of a stationary part, period and lengthscale
+// of every dim of a StdPeriodic part. Must not exceed MAX_D.
+__host__ __device__ inline int part_nacc(const PartDev& pd) {
+  if (pd.kind == GPX_STDPERIODIC) return 2 * pd.D;
+  return (is_stationary(pd.kind) && pd.ard) ? pd.D : 0;
+}
 
 struct KBuildMultiParams {
   const double* rowsT; long ld_rows; const double* sq_rows;    // stacked SoA [sumD][ld] and [nparts][ld] of the ROW points
@@ -44,7 +74,19 @@ struct GradKinvMultiParams {
   long N; int P; int nt;
   int part;                                                    // the part whose parameter sums are reduced by this launch
   int want_noise;                                              // also reduce tr(dL_dK) (done by the first launch only)
-  double* partials;                                            // [nt*nt][nl+2] of THIS part, zeroed by the caller
+  double* partials;                                            // [nt*nt][part_nred] of THIS part, zeroed by the caller
+  MultiKern mk;
+};
+
+// update_gradients_full of part 0 of mk for a dense dL_dK: rows = thread-mapped points (X2 of the call), cols = the X
+// points; dL_dK element (col point i, row point j) at dL[i * nrows + j]
+struct GradFullMultiParams {
+  const double* rowsT; long ld_rows; const double* sq_rows;
+  const double* colsT; long ld_cols; const double* sq_cols;
+  long nrows, ncols;
+  int same;
+  const double* dL;
+  double* partials;                                            // [col tiles][row tiles][part_nred]
   MultiKern mk;
 };
 
@@ -53,14 +95,23 @@ struct FinalizeMultiParams {
   const double* logdet_part; long nt;
   const double* T; long ld; long N; int P;
   MultiKern mk;
-  double* res;   // [0] lml, [1] logdet, [2] quad, [3] d/d noise, then per part [d/d variance, d/d lengthscale(s)] (static: variance only)
+  double* res;   // [0] lml, [1] logdet, [2] quad, [3] d/d noise, then every part's gradient block (part_ngrad entries)
 };
 
 int launch_prep_multi(const double* X, long N, int Dfull, long ld, const MultiKern& mk, double* XsT, double* sq, cudaStream_t st);
 int launch_kbuild_multi(const KBuildMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st);
 int launch_grad_kinv_multi(const GradKinvMultiParams& p, cudaStream_t st);
+int launch_grad_full_multi(const GradFullMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st);
 int launch_finalize_multi(const FinalizeMultiParams& f, cudaStream_t st);
-
-inline int part_nl(const PartDev& pd) { return pd.kind >= GPX_WHITE ? 0 : (pd.ard ? pd.D : 1); }
+// entry t of part p's reduced sums -> entry t of its gradient block: the stationary lengthscale rule -tot/l
+// (stationary.py:210,213) for RBF .. Matern52 and RatQuad; RatQuad's power and StdPeriodic's sums are the gradient as they
+// are (stationary.py:797-798, standard_periodic.py:518-526). false: the trace slot (last) or a static part's unused slot.
+__host__ __device__ inline bool part_grad_entry(const MultiKern& mk, int p, int t, double tot, double* val) {
+  const PartDev& pd = mk.part[p];
+  if (t >= part_ngrad(pd)) return false;
+  const int nl = pd.ard ? pd.D : 1;
+  *val = (t >= 1 && t <= nl && is_stationary(pd.kind)) ? -tot / mk.ls[pd.xoff + (pd.ard ? t - 1 : 0)] : tot;
+  return true;
+}
 
 }  // namespace gpx

@@ -3,7 +3,8 @@ path through libgpx (see INTEGRATION.md). Use where GPy (+ paramz) is importable
 
     import GPy
     from gpy_b200 import gpy_plugin
-    B = gpy_plugin.load()                       # subclasses of GPy.kern.RBF/Matern32/Matern52/Exponential + inference
+    B = gpy_plugin.load()                       # subclasses of GPy.kern.RBF/Matern32/Matern52/Exponential/RatQuad/StdPeriodic,
+                                                # Add, Prod + inference
     m = GPy.models.GPRegression(X, Y, kernel=B.RBF(D, ARD=True))
     m.inference_method = B.ExactGaussianInference()      # same hook the reference's tests use (GPy/testing/fitc.py:31)
     m.optimize()                                # paramz loop unchanged; one gpx_exact_eval per iterate
@@ -33,6 +34,7 @@ from .inference import PosteriorExact, _DataKey, _LazyAlpha
 from .kern import DeviceGradient
 
 _KINDS = {"RBF": "rbf", "Exponential": "exponential", "Matern32": "matern32", "Matern52": "matern52"}
+_PART_KINDS = {"RatQuad": "ratquad", "StdPeriodic": "stdperiodic"}
 
 
 class SparseDeviceGradient(object):
@@ -119,6 +121,72 @@ def _make_kernel(base, kind, ffi):
     return B200Kernel
 
 
+def _make_part_kernel(base, kind, ffi):
+    """GPy.kern.RatQuad (stationary.py:747-802) / GPy.kern.StdPeriodic (standard_periodic.py:21-548) with K, Kdiag and
+    update_gradients_full on the device (gpx_kern_part_K / gpx_kern_part_grad_full, or the block a fused composite evaluation
+    already reduced); gradients_X and update_gradients_diag stay GPy's."""
+
+    class B200PartKernel(base):
+        _gpx_part_kind = kind
+
+        def _gpx_desc(self, dims, term):
+            """(kind, ARD, term, dims, variance, lengthscale, extra) for ffi.Engine.exact_eval_multi / kern_part_*"""
+            var = float(np.asarray(self.variance).reshape(-1)[0])
+            ls = np.array(self.lengthscale, dtype=np.float64).reshape(-1)
+            if kind == "ratquad":
+                ard, extra = bool(self.ARD), {"power": float(np.asarray(self.power).reshape(-1)[0])}
+            else:
+                T = np.array(self.period, dtype=np.float64).reshape(-1)
+                ard, extra = bool(self.ARD2), {"period": T if self.ARD1 else float(T[0]), "ARD_period": bool(self.ARD1)}
+            return (kind, ard, term, [int(d) for d in dims], var, ls if ard else float(ls[0]), extra)
+
+        def _gpx_state_key(self):
+            return _composite_key(self)
+
+        def K(self, X, X2=None):
+            X = np.asarray(X, dtype=np.float64)
+            return ffi.kern_part_K(self._gpx_desc(range(X.shape[1]), 0), X,
+                                   None if X2 is None else np.asarray(X2, dtype=np.float64))
+
+        def Kdiag(self, X):
+            return ffi.kern_Kdiag(kind, float(np.asarray(self.variance).reshape(-1)[0]), int(np.asarray(X).shape[0]))
+
+        def update_gradients_full(self, dL_dK, X, X2=None, reset=True):
+            if isinstance(dL_dK, DeviceGradient) and X2 is None and dL_dK.part_grads is not None \
+                    and dL_dK.matches(_composite_key(self)):
+                _set_part_gradients(self, dL_dK.part_grads[0])
+                return
+            X = np.asarray(X, dtype=np.float64)
+            _set_part_gradients(self, ffi.kern_part_grad_full(self._gpx_desc(range(X.shape[1]), 0), X,
+                                                              np.asarray(dL_dK, dtype=np.float64),
+                                                              None if X2 is None else np.asarray(X2, dtype=np.float64)))
+
+    B200PartKernel.__name__ = B200PartKernel.__qualname__ = base.__name__
+    return B200PartKernel
+
+
+def _set_part_gradients(leaf, g):
+    """a RatQuad [variance, lengthscale.., power] / StdPeriodic [variance, period.., lengthscale..] gradient block -> the
+    leaf's parameters (scalars for the isotropic ones, as GPy's own update_gradients_full assigns them)"""
+    g = np.asarray(g, dtype=np.float64)
+    nl = np.asarray(leaf.lengthscale).size
+    leaf.variance.gradient = g[0]
+    if leaf._gpx_part_kind == "ratquad":
+        leaf.lengthscale.gradient = g[1:1 + nl] if leaf.ARD else g[1]
+        leaf.power.gradient = g[1 + nl]
+    else:
+        npd = np.asarray(leaf.period).size
+        leaf.period.gradient = g[1:1 + npd] if leaf.ARD1 else g[1]
+        leaf.lengthscale.gradient = g[1 + npd:] if leaf.ARD2 else g[1 + npd]
+
+
+def _leaf_ngrad(leaf):
+    """entries of one leaf's block in the gradient of exact_eval_multi"""
+    if hasattr(leaf, "_gpx_part_kind"):
+        return 1 + np.asarray(leaf.lengthscale).size + (1 if leaf._gpx_part_kind == "ratquad" else np.asarray(leaf.period).size)
+    return 1 + (np.asarray(leaf.lengthscale).size if hasattr(leaf, "lengthscale") else 0)
+
+
 def _make_combination(base, is_prod):
     """Add / Prod over GPy's own class: K, Kdiag, gradients_X ... stay the reference's; update_gradients_full recognises the
     handle of a fused composite evaluation and hands every leaf the gradient the device already reduced for it (the stock
@@ -129,6 +197,9 @@ def _make_combination(base, is_prod):
             if isinstance(dL_dK, DeviceGradient) and X2 is None and dL_dK.part_grads is not None \
                     and dL_dK.matches(_composite_key(self)):
                 for (leaf, _), g in zip(_flatten(self), dL_dK.part_grads):
+                    if hasattr(leaf, "_gpx_part_kind"):
+                        _set_part_gradients(leaf, g)
+                        continue
                     leaf.variance.gradient = g[0]
                     if hasattr(leaf, "lengthscale"):
                         leaf.lengthscale.gradient = g[1:] if leaf.ARD else g[1]
@@ -141,7 +212,7 @@ def _make_combination(base, is_prod):
 
 
 def _is_leaf(k):
-    return hasattr(k, "_gpx_kind") or type(k).__name__ in ("White", "Bias")
+    return hasattr(k, "_gpx_kind") or hasattr(k, "_gpx_part_kind") or type(k).__name__ in ("White", "Bias")
 
 
 def _flatten(kern):
@@ -165,6 +236,8 @@ def _flatten(kern):
 
 
 def _leaf_descriptor(leaf, term):
+    if hasattr(leaf, "_gpx_part_kind"):
+        return leaf._gpx_desc(np.atleast_1d(leaf.active_dims).astype(int).tolist(), term)
     var = float(np.asarray(leaf.variance).reshape(-1)[0])
     if not hasattr(leaf, "_gpx_kind"):
         return (type(leaf).__name__.lower(), False, term, [], var, None)
@@ -255,12 +328,17 @@ def _make_vardtc(base, kernel_types, ffi):
     return B200VarDTC
 
 
-def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None):
+def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None,
+         RatQuad=None, StdPeriodic=None):
     """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC
-    optional: the sparse model)."""
+    optional: the sparse model; RatQuad / StdPeriodic optional: leaves the composite evaluation knows, alone or inside
+    Add / Prod)."""
     kernels = {n: _make_kernel(b, _KINDS[n], ffi) for n, b in
                (("RBF", RBF), ("Exponential", Exponential), ("Matern32", Matern32), ("Matern52", Matern52))}
-    kernel_types = tuple(kernels.values())
+    kernel_types = tuple(kernels.values())      # the single-kernel evaluations (exact and VarDTC) take these only
+    for n, b in (("RatQuad", RatQuad), ("StdPeriodic", StdPeriodic)):
+        if b is not None:
+            kernels[n] = _make_part_kernel(b, _PART_KINDS[n], ffi)
     if Add is not None and Prod is not None:
         kernels["Add"], kernels["Prod"] = _make_combination(Add, False), _make_combination(Prod, True)
 
@@ -293,7 +371,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
                       Z_tilde=None):
             parts = None
             if mean_function is None and K is None and not isinstance(kern, kernel_types):
-                parts = _flatten(kern) if hasattr(kern, "_gpx_is_prod") else None
+                # sums / products, and a lone RatQuad / StdPeriodic (a one-part composite)
+                parts = _flatten(kern) if hasattr(kern, "_gpx_is_prod") or hasattr(kern, "_gpx_part_kind") else None
             if parts is None and (mean_function is not None or K is not None or not isinstance(kern, kernel_types)):
                 return super(B200ExactGaussianInference, self).inference(kern, X, likelihood, Y, mean_function,
                                                                          Y_metadata, K, variance, Z_tilde)
@@ -317,7 +396,7 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
                     lml += Z_tilde
                 pg, i = [], 0
                 for (leaf, _) in parts:
-                    n = 1 + (np.asarray(leaf.lengthscale).size if hasattr(leaf, "lengthscale") else 0)
+                    n = _leaf_ngrad(leaf)
                     pg.append(grad[i:i + n])
                     i += n
                 key = _composite_key(kern)
@@ -363,4 +442,4 @@ def load():
     import GPy
     from GPy.inference.latent_function_inference import ExactGaussianInference, VarDTC
     return make(GPy.kern.RBF, GPy.kern.Exponential, GPy.kern.Matern32, GPy.kern.Matern52, ExactGaussianInference,
-                Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC)
+                Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic)

@@ -11,7 +11,7 @@ Mirrors (same names, argument meaning, return structure and error behaviour):
 import numpy as np
 
 from . import _ffi
-from .kern import (DeviceGradient, Stationary, White, Bias, composite_state_key, flatten_parts, part_descriptor)
+from .kern import (DeviceGradient, composite_state_key, flatten_parts, part_descriptor, part_ngrad, single_kernel)
 from .param import Param, Parameterized
 
 
@@ -241,11 +241,13 @@ class ExactGaussianInference(object):
         nvec = np.asarray(variance, dtype=np.float64).reshape(-1)
         het = nvec.size > 1                          # HeteroscedasticGaussian: a vector reaches diag.add (:55-56)
         noise = nvec if het else float(nvec[0])
-        if mean_function is None and K is None and not het and not isinstance(kern, Stationary):
+        # RBF .. Matern52 alone take the single-kernel evaluation; sums / products and the leaves only the composite
+        # evaluation knows (RatQuad, StdPeriodic) take gpx_exact_eval_multi
+        if mean_function is None and K is None and not het and not single_kernel(kern):
             parts = flatten_parts(kern)
             if parts is not None:
                 return self._composite_inference(kern, parts, X, Y, noise, Z_tilde)
-        if mean_function is not None or K is not None or not isinstance(kern, Stationary):
+        if mean_function is not None or K is not None or not single_kernel(kern):
             return self._generic_inference(kern, X, Y, noise, mean_function, K, Z_tilde, likelihood, Y_metadata)
         Xs = kern._slice_X(X)
         Y = np.ascontiguousarray(Y, dtype=np.float64)
@@ -285,7 +287,7 @@ class ExactGaussianInference(object):
             lml += Z_tilde
         part_grads, i = [], 0
         for (leaf, _) in parts:
-            n = 1 + (leaf.lengthscale.size if isinstance(leaf, Stationary) else 0)
+            n = part_ngrad(leaf)
             part_grads.append(grad[i:i + n])
             i += n
         N, P = Y.shape

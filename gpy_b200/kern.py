@@ -5,6 +5,8 @@ Same names, argument meaning and error behaviour as the reference classes:
     GPy.kern.Exponential   GPy/kern/src/stationary.py:378-386
     GPy.kern.Matern32      GPy/kern/src/stationary.py:457-492
     GPy.kern.Matern52      GPy/kern/src/stationary.py:556-589
+    GPy.kern.RatQuad       GPy/kern/src/stationary.py:747-802
+    GPy.kern.StdPeriodic   GPy/kern/src/standard_periodic.py:21-94,125-139,501-548
 base: GPy.kern.src.stationary.Stationary (stationary.py:23-243) and GPy.kern.Kern (kern.py:12-145).
 `K`, `Kdiag`, `update_gradients_full`, `update_gradients_diag` take/return NumPy arrays exactly like the reference;
 there is no NumPy implementation behind them — every call goes through the C ABI (include/gpx.h).
@@ -214,6 +216,157 @@ class Matern52(Stationary):
         super(Matern52, self).__init__(input_dim, variance, lengthscale, ARD, active_dims, name)
 
 
+class _PartKern(object):
+    """RatQuad and StdPeriodic: evaluated on the device as composite parts (gpx_exact_eval_multi inside a model,
+    gpx_kern_part_K / gpx_kern_part_grad_full stand-alone). Subclasses give their descriptor extra and gradient block."""
+
+    def part_desc(self, dims, term):
+        """(kind, ARD, term, dims, variance, lengthscale, extra) for Engine.exact_eval_multi"""
+        ls = self.lengthscale.values if self._ard_ls() else self.lengthscale.values[0]
+        return (self._kind, self._ard_ls(), term, list(dims), float(self.variance[0]), ls, self._extra())
+
+    def K(self, X, X2=None):
+        X = self._slice_X(X)
+        X2 = None if X2 is None else self._slice_X(X2)
+        return _ffi.kern_part_K(self.part_desc(range(self.input_dim), 0), X, X2)
+
+    def Kdiag(self, X):
+        return _ffi.kern_Kdiag(self._kind, float(self.variance[0]), int(np.asarray(X).shape[0]))
+
+    def update_gradients_full(self, dL_dK, X, X2=None, reset=True):
+        """A DeviceGradient handle of a fused evaluation of this kernel hands over the block the device reduced; any other
+        dL_dK goes through gpx_kern_part_grad_full."""
+        if X2 is None and scatter_part_gradients(self, dL_dK):
+            return
+        Xs = self._slice_X(X)
+        X2s = None if X2 is None else self._slice_X(X2)
+        self._set_gradients(_ffi.kern_part_grad_full(self.part_desc(range(self.input_dim), 0), Xs,
+                                                     np.asarray(dL_dK, dtype=np.float64), X2s))
+
+    def gradients_X(self, dL_dK, X, X2=None):
+        raise NotImplementedError("%s.gradients_X: the device has no input-gradient kernel for this kind yet" % type(self).__name__)
+
+    def gradients_X_diag(self, dL_dKdiag, X):
+        return np.zeros(np.asarray(X).shape)
+
+
+class RatQuad(_PartKern, Stationary):
+    """GPy.kern.RatQuad (stationary.py:747-802): k(r) = variance (1 + r^2/2)^-power."""
+    _kind = "ratquad"
+
+    def __init__(self, input_dim, variance=1., lengthscale=None, power=2., ARD=False, active_dims=None, name="RatQuad"):
+        super(RatQuad, self).__init__(input_dim, variance, lengthscale, ARD, active_dims, name)
+        self.power = Param("power", power)
+        self.link_parameter(self.power)                   # stationary.py:760: after variance, lengthscale
+
+    def _ard_ls(self):
+        return self.ARD
+
+    def _extra(self):
+        return {"power": float(self.power[0])}
+
+    def _state_key(self):
+        return Stationary._state_key(self) + (float(self.power[0]),)
+
+    def _set_gradients(self, g):
+        self.variance.gradient = np.atleast_1d(g[0])
+        self.lengthscale.gradient = np.atleast_1d(g[1:-1]).copy()
+        self.power.gradient = np.atleast_1d(g[-1])
+
+    def update_gradients_diag(self, dL_dKdiag, X):
+        """stationary.py:800-802."""
+        Stationary.update_gradients_diag(self, dL_dKdiag, X)
+        self.power.gradient = np.zeros(1)
+
+    def reset_gradients(self):
+        Stationary.reset_gradients(self)
+        self.power.gradient = np.zeros(1)
+
+
+class StdPeriodic(_PartKern, Kern):
+    """GPy.kern.StdPeriodic (standard_periodic.py:21-94): k = variance exp(-1/2 sum_q (sin(pi (x_q - x'_q) / T_q) / l_q)^2).
+    ARD1: one period per dim; ARD2: one lengthscale per dim."""
+    _kind = "stdperiodic"
+
+    def __init__(self, input_dim, variance=1., period=None, lengthscale=None, ARD1=False, ARD2=False, active_dims=None,
+                 name="std_periodic"):
+        super(StdPeriodic, self).__init__(input_dim, active_dims, name)
+        self.ARD1, self.ARD2 = bool(ARD1), bool(ARD2)
+        # standard_periodic.py:62-84
+        if not self.ARD1:
+            if period is not None:
+                period = np.asarray(period, dtype=np.float64)
+                assert period.size == 1, "Only one period needed for non-ARD kernel"
+            else:
+                period = np.ones(1)
+        else:
+            if period is not None:
+                period = np.asarray(period, dtype=np.float64)
+                assert period.size == input_dim, "bad number of periods"
+            else:
+                period = np.ones(input_dim)
+        if not self.ARD2:
+            if lengthscale is not None:
+                lengthscale = np.asarray(lengthscale, dtype=np.float64)
+                assert lengthscale.size == 1, "Only one lengthscale needed for non-ARD kernel"
+            else:
+                lengthscale = np.ones(1)
+        else:
+            if lengthscale is not None:
+                lengthscale = np.asarray(lengthscale, dtype=np.float64)
+                assert lengthscale.size == input_dim, "bad number of lengthscales"
+            else:
+                lengthscale = np.ones(input_dim)
+        self.variance = Param("variance", variance)
+        assert self.variance.size == 1, "Variance size must be one"
+        self.period = Param("period", period)
+        self.lengthscale = Param("lengthscale", lengthscale)
+        self.link_parameters(self.variance, self.period, self.lengthscale)   # standard_periodic.py:94
+
+    def _ard_ls(self):
+        return self.ARD2
+
+    def _extra(self):
+        return {"period": self.period.values.copy() if self.ARD1 else float(self.period[0]), "ARD_period": self.ARD1}
+
+    def _state_key(self):
+        return (self._kind, self.ARD1, self.ARD2, float(self.variance[0]), tuple(self.period.values.tolist()),
+                tuple(self.lengthscale.values.tolist()), tuple(self.active_dims.tolist()))
+
+    def _set_gradients(self, g):
+        npd = self.period.size
+        self.variance.gradient = np.atleast_1d(g[0])
+        self.period.gradient = np.atleast_1d(g[1:1 + npd]).copy()
+        self.lengthscale.gradient = np.atleast_1d(g[1 + npd:]).copy()
+
+    def update_gradients_diag(self, dL_dKdiag, X):
+        """standard_periodic.py:544-548."""
+        self.variance.gradient = np.atleast_1d(np.sum(dL_dKdiag))
+        self.period.gradient = np.zeros_like(self.period.values)
+        self.lengthscale.gradient = np.zeros_like(self.lengthscale.values)
+
+    def reset_gradients(self):
+        self.variance.gradient = np.zeros(1)
+        self.period.gradient = np.zeros_like(self.period.values)
+        self.lengthscale.gradient = np.zeros_like(self.lengthscale.values)
+
+
+SINGLE_KINDS = ("rbf", "exponential", "matern32", "matern52")
+
+
+def single_kernel(kern):
+    """True for a kernel the single-kernel device evaluation takes (gpx_exact_eval and friends): RBF .. Matern52. RatQuad is
+    a Stationary too, but only the composite evaluation knows it."""
+    return isinstance(kern, Stationary) and kern._kind in SINGLE_KINDS
+
+
+def part_ngrad(leaf):
+    """gradient entries of one flattened leaf in the result of Engine.exact_eval_multi"""
+    if isinstance(leaf, _PartKern):
+        return sum(p.size for p in leaf.flattened_parameters())
+    return 1 + (leaf.lengthscale.size if isinstance(leaf, Stationary) else 0)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # combination / static kernels (SURVEY.md §8f item 4). Mirrors GPy/kern/src/add.py:60-99, prod.py:59-68,377-396,
 # static.py:63-185. A GP whose kernel is a sum of products of stationary / White / Bias leaves is evaluated by ONE device
@@ -226,7 +379,7 @@ def flatten_parts(kern):
     """-> list of (leaf kernel, term index) for a kernel that is a leaf, a product of leaves, or a sum of those; None for
     anything else (e.g. a product containing a sum), which then takes the generic inference path."""
     def leaf(k):
-        return isinstance(k, (Stationary, White, Bias))
+        return isinstance(k, (Stationary, StdPeriodic, White, Bias))
 
     def product(k, term):
         if leaf(k):
@@ -247,7 +400,9 @@ def flatten_parts(kern):
 
 
 def part_descriptor(leaf, term):
-    """(kind, ARD, term, dims, variance, lengthscale) of one leaf for Engine.exact_eval_multi"""
+    """(kind, ARD, term, dims, variance, lengthscale[, extra]) of one leaf for Engine.exact_eval_multi"""
+    if isinstance(leaf, _PartKern):
+        return leaf.part_desc(leaf.active_dims.tolist(), term)
     if isinstance(leaf, White):
         return ("white", False, term, [], float(leaf.variance[0]), None)
     if isinstance(leaf, Bias):
@@ -262,7 +417,7 @@ def composite_state_key(kern):
         return None
     return tuple((t, type(k).__name__, float(k.variance[0]),
                   tuple(k.lengthscale.values.tolist()) if isinstance(k, Stationary) else (),
-                  tuple(k.active_dims.tolist())) for (k, t) in fl)
+                  tuple(k.active_dims.tolist())) + ((k._state_key(),) if isinstance(k, _PartKern) else ()) for (k, t) in fl)
 
 
 def scatter_part_gradients(kern, dL_dK):
@@ -271,6 +426,9 @@ def scatter_part_gradients(kern, dL_dK):
     if not (isinstance(dL_dK, DeviceGradient) and dL_dK.part_grads is not None and dL_dK.matches(composite_state_key(kern))):
         return False
     for (leaf, _), g in zip(flatten_parts(kern), dL_dK.part_grads):
+        if isinstance(leaf, _PartKern):
+            leaf._set_gradients(g)
+            continue
         leaf.variance.gradient = np.atleast_1d(g[0])
         if isinstance(leaf, Stationary):
             leaf.lengthscale.gradient = np.atleast_1d(g[1:]).copy()

@@ -18,7 +18,7 @@ import numpy as np
 
 from . import _ffi
 from .inference import Gaussian, HeteroscedasticGaussian, _DataKey
-from .kern import RBF, Stationary
+from .kern import RBF, RatQuad, StdPeriodic, Stationary
 from .param import Logexp, Param, Parameterized
 
 CONST_JITTER = 1e-8  # var_dtc.py:24
@@ -93,6 +93,9 @@ class VarDTC(object):
     def inference(self, kern, X, Z, likelihood, Y, Y_metadata=None, mean_function=None, precision=None):
         if mean_function is not None:
             raise NotImplementedError("sparse GP with a mean function is not on the accelerated path")
+        if isinstance(kern, (RatQuad, StdPeriodic)):
+            raise NotImplementedError("gpy_b200.VarDTC: %s is not on the device's sparse evaluation (RBF, Exponential, "
+                                      "Matern32, Matern52 are)" % type(kern).__name__)
         if not isinstance(kern, Stationary):
             raise TypeError("gpy_b200.VarDTC accelerates gpy_b200.kern stationary kernels")
         eng = self.engine

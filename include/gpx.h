@@ -37,7 +37,9 @@ extern "C" {
 typedef struct gpx_ctx gpx_ctx;
 
 enum { GPX_RBF = 0, GPX_EXPONENTIAL = 1, GPX_MATERN32 = 2, GPX_MATERN52 = 3,
-       GPX_WHITE = 4, GPX_BIAS = 5 /* static parts of a composite kernel only (GPy/kern/src/static.py:63-99,142-185) */ };
+       GPX_WHITE = 4, GPX_BIAS = 5, /* static parts of a composite kernel only (GPy/kern/src/static.py:63-99,142-185) */
+       GPX_RATQUAD = 6,              /* RatQuad (stationary.py:747-802), composite parts and gpx_kern_part_* only */
+       GPX_STDPERIODIC = 7 };        /* StdPeriodic (standard_periodic.py:56-94,125-139,501-548), likewise */
 
 /* gpx_get selectors */
 enum {
@@ -89,20 +91,41 @@ int gpx_exact_eval_het(gpx_ctx* ctx, int kind, int ard, double variance, const d
  * the X of gpx_set_data; kernel_slice_operations.py:59-79), a White or a Bias kernel. Parts with the same `term` are
  * multiplied, terms are summed; parts must be ordered by term. The whole evaluation runs on the device like
  * gpx_exact_eval (K-build, factor-and-invert sweep, K^-1, one gradient-reduction pass per part over the stored K^-1).
- *   grad: out, concatenation over the parts in the given order of [d/d variance, d/d lengthscale (1 or ndims; none for
- *         White / Bias)], then d/d noise — the order paramz gives Add/Prod parameters (kern.py:363-451 link order).
+ *   grad: out, concatenation over the parts in the given order of each part's gradient block, then d/d noise — the order
+ *         paramz gives Add/Prod parameters (kern.py:363-451 link order). Blocks:
+ *           RBF .. Matern52   [variance, lengthscale (1 or ndims)]                     (stationary.py:81)
+ *           White, Bias       [variance]
+ *           RatQuad           [variance, lengthscale (1 or ndims), power]              (stationary.py:81, then :760)
+ *           StdPeriodic       [variance, period (1 or ndims), lengthscale (1 or ndims)] (standard_periodic.py:94)
+ *         A StdPeriodic part keeps one sum per active dim for its period and one for its lengthscale: 2 ndims <= 64, else
+ *         the call fails with -2 (the reduction does not fit).
  * gpx_get / gpx_predict afterwards use the composite kernel. Single-GPU. */
 typedef struct {
-  int kind;                  /* GPX_RBF .. GPX_MATERN52, GPX_WHITE, GPX_BIAS */
-  int ard;                   /* stationary kinds: 0 -> lengthscale points at 1 double, 1 -> at ndims doubles */
+  int kind;                  /* GPX_RBF .. GPX_MATERN52, GPX_WHITE, GPX_BIAS, GPX_RATQUAD, GPX_STDPERIODIC */
+  int ard;                   /* lengthscale: 0 -> points at 1 double, 1 -> at ndims doubles (StdPeriodic: GPy's ARD2) */
   int term;                  /* additive term this factor belongs to */
   int ndims;                 /* number of active dims (0 for White / Bias) */
   const int* dims;           /* column indices into X, ndims entries */
   double variance;
   const double* lengthscale;
+  double power;              /* RatQuad: k = variance (1 + r^2/2)^-power, power > 0 (stationary.py:785-788) */
+  int ard_period;            /* StdPeriodic (GPy's ARD1): 0 -> period points at 1 double, 1 -> at ndims doubles */
+  const double* period;      /* StdPeriodic: k = variance exp(-1/2 sum_q (sin(pi (x_q - x'_q) / T_q) / l_q)^2), T_q > 0
+                                (standard_periodic.py:125-132) */
 } gpx_kern_part;
 int gpx_exact_eval_multi(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, double noise, double jitter, int max_tries,
                          double* lml, double* grad, double* jitter_used);
+
+/* Stand-alone K and update_gradients_full of ONE part (kinds 0-3, 6, 7; White / Bias are rejected) on the given inputs,
+ * for callers that hold a kernel object outside an evaluation (PosteriorExact._raw_predict, the generic inference path).
+ * X (N x D) and X2 (M x D) are row-major with the D columns `part->dims` index into; X2 == NULL -> X2 = X with exact zero
+ * distance on the diagonal. The K-build and the per-pair gradient terms are those of gpx_exact_eval_multi.
+ *   gpx_kern_part_K         : out, N x M row-major (like gpx_kern_K).
+ *   gpx_kern_part_grad_full : dL_dK N x M row-major in; grad out, the part's gradient block (as above). */
+int gpx_kern_part_K(gpx_ctx* ctx, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M, int D,
+                    double* out);
+int gpx_kern_part_grad_full(gpx_ctx* ctx, const gpx_kern_part* part, const double* X, int64_t N, const double* X2,
+                            int64_t M, int D, const double* dL_dK, double* grad);
 
 /* Lazy device->host fetch of N^2 / N*P results of the last gpx_exact_eval (Posterior / grad_dict consumers:
  * GPy/inference/latent_function_inference/posterior.py:21-77; exact_gaussian_inference.py:74). */
@@ -118,7 +141,8 @@ int gpx_predict(gpx_ctx* ctx, const double* Xnew, int64_t M, int full_cov, doubl
  * out == NULL: build on the device only and report the kernel time via gpx_get_stats (kbuild_ms, kbuild_bytes). */
 int gpx_kern_K(gpx_ctx* ctx, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
                const double* X2 /* NULL -> K(X,X) with exact zero-distance diagonal */, int64_t M, int D, double* out);
-/* Replaces Stationary.Kdiag (stationary.py:170-173). */
+/* Replaces Stationary.Kdiag (stationary.py:170-173); kinds 0-3, 6 and 7 (StdPeriodic.Kdiag, standard_periodic.py:134-138,
+ * is the variance as well). */
 int gpx_kern_Kdiag(int kind, double variance, int64_t N, double* out);
 /* Replaces Stationary.update_gradients_full (stationary.py:193-243) for a caller-supplied dL_dK (N x M row-major). */
 int gpx_kern_grad_full(gpx_ctx* ctx, int kind, int ard, double variance, const double* lengthscale, const double* X,
