@@ -154,6 +154,20 @@ def check(rc, what):
     raise GpxError("%s failed (%d): %s" % (what, rc, msg))
 
 
+def _inputs(X, X2=None, dL_dK=None):
+    """inputs of a stand-alone kernel call: X (N x D), X2 (M x D, or None: X itself) and, if given, dL_dK (N x M) as
+    contiguous float64 arrays -> (X, N, D, X2, M, dL_dK)"""
+    X = _f64(X)
+    N, D = X.shape
+    X2 = None if X2 is None else _f64(X2)
+    M = N if X2 is None else X2.shape[0]
+    if dL_dK is not None:
+        dL_dK = _f64(dL_dK)
+        if dL_dK.shape != (N, M):
+            raise ValueError("dL_dK must be %d x %d" % (N, M))
+    return X, N, D, X2, M, dL_dK
+
+
 def _theta(kind, ARD, lengthscale, D):
     ls = _f64(np.atleast_1d(lengthscale)).reshape(-1)
     if ARD:
@@ -261,12 +275,9 @@ class Engine(object):
 
     def kern_K_device_only(self, kind, ARD, variance, lengthscale, X, X2=None):
         """build K(X, X2) on the device without bringing it back; -> (kernel ms, algorithmic GB/s)."""
-        X = _f64(X)
-        N, D = X.shape
+        X, N, D, X2, M, _ = _inputs(X, X2)
         k, a, ls = _theta(kind, ARD, lengthscale, D)
-        X2c = None if X2 is None else _f64(X2)
-        M = N if X2 is None else X2c.shape[0]
-        check(self._L.gpx_kern_K(self._h, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2c), M, D, None), "gpx_kern_K")
+        check(self._L.gpx_kern_K(self._h, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2), M, D, None), "gpx_kern_K")
         st = self.stats()
         return st["kbuild_ms"], st["kbuild_bytes"] / st["kbuild_ms"] * 1e-6
 
@@ -334,45 +345,30 @@ class Engine(object):
 
 
 def kern_K(kind, ARD, variance, lengthscale, X, X2=None):
-    X = _f64(X)
-    N, D = X.shape
+    X, N, D, X2, M, _ = _inputs(X, X2)
     k, a, ls = _theta(kind, ARD, lengthscale, D)
-    if X2 is not None:
-        X2 = _f64(X2)
-        M = X2.shape[0]
-    else:
-        M = N
     out = np.empty((N, M))
     check(lib().gpx_kern_K(None, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2), M, D, _ptr(out)), "gpx_kern_K")
     return out
 
 
-def _part_inputs(desc, X, X2):
-    part, keep = GpxKernPart(), []
-    n = _fill_part(part, desc, keep)
-    X = _f64(X)
-    N, D = X.shape
-    X2c = None if X2 is None else _f64(X2)
-    M = N if X2 is None else X2c.shape[0]
-    return part, keep, n, X, N, X2c, M, D
-
-
 def kern_part_K(desc, X, X2=None):
     """K(X, X2) (N x M) of one composite part descriptor (as Engine.exact_eval_multi takes it; dims index X's columns)."""
-    part, keep, _, X, N, X2c, M, D = _part_inputs(desc, X, X2)
+    part, keep = GpxKernPart(), []
+    _fill_part(part, desc, keep)
+    X, N, D, X2, M, _ = _inputs(X, X2)
     out = np.empty((N, M))
-    check(lib().gpx_kern_part_K(None, ctypes.byref(part), _ptr(X), N, _ptr(X2c), M, D, _ptr(out)), "gpx_kern_part_K")
+    check(lib().gpx_kern_part_K(None, ctypes.byref(part), _ptr(X), N, _ptr(X2), M, D, _ptr(out)), "gpx_kern_part_K")
     return out
 
 
 def kern_part_grad_full(desc, X, dL_dK, X2=None):
     """update_gradients_full of one composite part for a dense dL_dK (N x M) -> its gradient block."""
-    part, keep, n, X, N, X2c, M, D = _part_inputs(desc, X, X2)
-    dL_dK = _f64(dL_dK)
-    if dL_dK.shape != (N, M):
-        raise ValueError("dL_dK must be %d x %d" % (N, M))
+    part, keep = GpxKernPart(), []
+    n = _fill_part(part, desc, keep)
+    X, N, D, X2, M, dL_dK = _inputs(X, X2, dL_dK)
     grad = np.zeros(n)
-    check(lib().gpx_kern_part_grad_full(None, ctypes.byref(part), _ptr(X), N, _ptr(X2c), M, D, _ptr(dL_dK), _ptr(grad)),
+    check(lib().gpx_kern_part_grad_full(None, ctypes.byref(part), _ptr(X), N, _ptr(X2), M, D, _ptr(dL_dK), _ptr(grad)),
           "gpx_kern_part_grad_full")
     return grad
 
@@ -385,16 +381,10 @@ def kern_Kdiag(kind, variance, N):
 
 def kern_grad_X(kind, ARD, variance, lengthscale, X, dL_dK, X2=None):
     """Stationary.gradients_X (stationary.py:245-252) on the device -> N x D."""
-    X = _f64(X)
-    N, D = X.shape
+    X, N, D, X2, M, dL_dK = _inputs(X, X2, dL_dK)
     k, a, ls = _theta(kind, ARD, lengthscale, D)
-    X2c = None if X2 is None else _f64(X2)
-    M = N if X2 is None else X2c.shape[0]
-    dL_dK = _f64(dL_dK)
-    if dL_dK.shape != (N, M):
-        raise ValueError("dL_dK must be %d x %d" % (N, M))
     out = np.empty((N, D))
-    check(lib().gpx_kern_grad_X(None, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2c), M, D, _ptr(dL_dK), _ptr(out)),
+    check(lib().gpx_kern_grad_X(None, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2), M, D, _ptr(dL_dK), _ptr(out)),
           "gpx_kern_grad_X")
     return out
 
@@ -423,17 +413,8 @@ def jitchol(A, maxtries=5, engine=None):
 
 
 def kern_grad_full(kind, ARD, variance, lengthscale, X, dL_dK, X2=None):
-    X = _f64(X)
-    N, D = X.shape
+    X, N, D, X2, M, dL_dK = _inputs(X, X2, dL_dK)
     k, a, ls = _theta(kind, ARD, lengthscale, D)
-    if X2 is not None:
-        X2 = _f64(X2)
-        M = X2.shape[0]
-    else:
-        M = N
-    dL_dK = _f64(dL_dK)
-    if dL_dK.shape != (N, M):
-        raise ValueError("dL_dK must be %d x %d" % (N, M))
     dv = ctypes.c_double()
     dl = np.zeros(ls.size)
     check(lib().gpx_kern_grad_full(None, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2), M, D, _ptr(dL_dK),

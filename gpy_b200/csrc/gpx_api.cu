@@ -587,7 +587,7 @@ static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec) {
 }
 
 // the kernel of the context's last evaluation, and its training points as build_Ky prepared them
-static const KernParams* ctx_kern(const gpx_ctx* c) { return c->multi ? nullptr : &c->kp; }
+static Kern ctx_kern(const gpx_ctx* c) { return c->multi ? Kern(&c->mk) : Kern(&c->kp); }
 static Points train_points(const gpx_ctx* c) {
   return c->multi ? Points{c->mXsT, c->msq, c->N, c->Npad} : Points{c->dXsT, c->dsq, c->N, c->Npad};
 }
@@ -616,7 +616,7 @@ static int build_Ky(gpx_ctx* c, double extra_jitter, bool int8, Recorder& rec, c
     }
   }
   const Points tr = train_points(c);
-  GPX_CHECK(prep_points(c, ctx_kern(c), c->dX, c->N, c->Npad, tr.xT, tr.sq));
+  GPX_CHECK(prep_points(c, ctx_kern(c), c->dX, c->N, c->D, c->Npad, tr.xT, tr.sq));
   c->eval_launches++;
   const KyDiag ky{((c->het ? 0.0 : c->noise) + c->jitter) + extra_jitter, c->het ? c->dNoiseVec : nullptr};
   const int h = rec.begin(PH_KBUILD);
@@ -796,25 +796,20 @@ static int fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Df
   return 0;
 }
 
-static int fill_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double* kdiag_total) {
-  return fill_mk(c->mk, parts, nparts, c->D, kdiag_total);
-}
-
-// noise_vec == nullptr: homoscedastic (`noise`); else N per-point variances (`noise` = their mean, used by the ladder)
-static int exact_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, double noise,
-                           const double* noise_vec, double jitter, int max_tries, double* lml, double* grad,
-                           double* dnoise, double* jitter_used, const gpx_kern_part* parts = nullptr, int nparts = 0) {
-  if (!c || !lml || !grad || (!parts && !lengthscale)) GPX_FAIL("null argument");
+// the checks every exact-evaluation entry makes before it reads its kernel (`kern`: the lengthscale or the parts, read
+// against the data's D)
+static int eval_args(const gpx_ctx* c, const void* kern, const double* lml, const double* grad, double noise) {
+  if (!c || !kern || !lml || !grad) GPX_FAIL("null argument");
   if (!c->S) GPX_FAIL("gpx_set_data has not been called");
   if (!(noise >= 0)) GPX_FAIL("noise variance must be non-negative");
+  return 0;
+}
+
+// One evaluation of the validated kernel k (Kdiag = kdiag), which becomes the context's kernel. noise_vec == nullptr:
+// homoscedastic (`noise`); else N per-point variances (`noise` = their mean, used by the ladder)
+static int exact_eval_impl(gpx_ctx* c, Kern k, double kdiag, double noise, const double* noise_vec, double jitter,
+                           int max_tries, double* lml, double* grad, double* dnoise, double* jitter_used) {
   GPX_CUDA(cudaSetDevice(c->device));
-  c->multi = parts != nullptr;
-  if (c->multi) {
-    if (c->dist) GPX_FAIL("composite kernels are single-GPU");
-    GPX_CHECK(fill_multi(c, parts, nparts, &variance));     // `variance` = Kdiag of the composite kernel (jitter ladder)
-    c->kp.variance = variance;
-  } else
-  GPX_CHECK(fill_kp(c->kp, kind, ard, c->D, variance, lengthscale));
   c->het = noise_vec != nullptr;
   if (c->het) {
     if (c->dist) GPX_FAIL("heteroscedastic evaluation is single-GPU");
@@ -829,11 +824,14 @@ static int exact_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const
     }
     GPX_CUDA(cudaMemcpyAsync(c->dNoiseVec, noise_vec, (size_t)c->N * 8, cudaMemcpyHostToDevice, c->st));
   }
+  c->multi = k.mk != nullptr;
+  if (c->multi) c->mk = *k.mk; else c->kp = *k.kp;
+  c->kdiag = kdiag;
   c->noise = noise;
   c->jitter = jitter;
   c->have_eval = false;
   c->have_kinv = false;
-  const int nl = ard ? c->D : 1;
+  const int nl = c->kp.ard ? c->D : 1;
   memset(&c->stats, 0, sizeof(c->stats));
   c->eval_launches = 0;
   Recorder rec{c};
@@ -855,7 +853,7 @@ static int exact_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const
     // jitchol ladder (GPy/util/linalg.py:61-75): the diagonal of Ky is variance + noise + jitter (> 0 here),
     // extra jitter = mean(diag) * 1e-6 * 10^k for k = 0 .. max_tries-1
     if (tries > max_tries) break;
-    const double mean_diag = variance + (noise + jitter);
+    const double mean_diag = kdiag + (noise + jitter);
     extra = mean_diag * 1e-6 * pow(10.0, tries - 1);
     if (!std::isfinite(extra)) break;
   }
@@ -906,15 +904,20 @@ extern "C" {
 
 int gpx_exact_eval(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, double noise,
                    double jitter, int max_tries, double* lml, double* grad, double* jitter_used) {
-  return exact_eval_impl(c, kind, ard, variance, lengthscale, noise, nullptr, jitter, max_tries, lml, grad, nullptr,
-                         jitter_used);
+  GPX_CHECK(eval_args(c, lengthscale, lml, grad, noise));
+  KernParams kp{};
+  GPX_CHECK(fill_kp(kp, kind, ard, c->D, variance, lengthscale));
+  return exact_eval_impl(c, &kp, variance, noise, nullptr, jitter, max_tries, lml, grad, nullptr, jitter_used);
 }
 
 int gpx_exact_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double noise, double jitter, int max_tries,
                          double* lml, double* grad, double* jitter_used) {
-  if (!parts) GPX_FAIL("null argument");
-  return exact_eval_impl(c, 0, 0, 1.0, nullptr, noise, nullptr, jitter, max_tries, lml, grad, nullptr, jitter_used, parts,
-                         nparts);
+  GPX_CHECK(eval_args(c, parts, lml, grad, noise));
+  if (c->dist) GPX_FAIL("composite kernels are single-GPU");
+  MultiKern mk;
+  double kdiag;
+  GPX_CHECK(fill_mk(mk, parts, nparts, c->D, &kdiag));
+  return exact_eval_impl(c, &mk, kdiag, noise, nullptr, jitter, max_tries, lml, grad, nullptr, jitter_used);
 }
 
 int gpx_exact_eval_het(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale,
@@ -927,8 +930,10 @@ int gpx_exact_eval_het(gpx_ctx* c, int kind, int ard, double variance, const dou
     mean += noise_variances[i];
   }
   mean /= (double)std::max<int64_t>(c->N, 1);
-  return exact_eval_impl(c, kind, ard, variance, lengthscale, mean, noise_variances, jitter, max_tries, lml, grad, dnoise,
-                         jitter_used);
+  GPX_CHECK(eval_args(c, lengthscale, lml, grad, mean));
+  KernParams kp{};
+  GPX_CHECK(fill_kp(kp, kind, ard, c->D, variance, lengthscale));
+  return exact_eval_impl(c, &kp, variance, mean, noise_variances, jitter, max_tries, lml, grad, dnoise, jitter_used);
 }
 
 int gpx_measure_fp64_peak(gpx_ctx* c, double* tflops) {
@@ -997,8 +1002,12 @@ int gpx_get(gpx_ctx* c, int which, double* out) {
   return 0;
 }
 
+}  // extern "C"
+
 // ---------------------------------------------------------------------------------------------------------------
-// standalone kernel-plugin calls
+// stand-alone kernel calls: K and update_gradients_full of a single kernel (kinds 0-3) or of one composite part (kinds 0-3,
+// 6, 7: the K-build and the per-pair gradient terms of the composite evaluation), gradients_X of a single kernel. Each works
+// with the kernel it is given; the context's own (that of its last evaluation) is left alone.
 // ---------------------------------------------------------------------------------------------------------------
 static std::mutex g_scratch_mu;
 static gpx_ctx* g_scratch = nullptr;
@@ -1013,39 +1022,85 @@ static int scratch_ctx(gpx_ctx** out) {
   return 0;
 }
 
-int gpx_kern_K(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
-               const double* X2, int64_t M, int D, double* out) {
-  if (!X || !lengthscale) GPX_FAIL("null argument");
+static int fill_one_part(const gpx_kern_part* part, int D, MultiKern& mk) {
+  if (!part) GPX_FAIL("null argument");
+  if (is_known(part->kind) && is_static(part->kind)) GPX_FAIL("White / Bias parts have no stand-alone entry");
+  if (D < 1 || D > MAX_D) GPX_FAIL("input dimension must be in [1, 64]");
+  gpx_kern_part one = *part;
+  one.term = 0;
+  double kdiag;
+  return fill_mk(mk, &one, 1, D, &kdiag);
+}
+
+// K(X, X2) of k into out (N x M row-major; X2 == NULL: K(X, X)) on c (NULL: the scratch context), timed into c's kbuild_ms /
+// kbuild_bytes. out == NULL: built on the device only (the result is dropped) -- used to measure the rectangular K(X, Z)
+// build of the sparse model at full size.
+static int kern_K(gpx_ctx* c, Kern k, const double* X, int64_t N, const double* X2, int64_t M, int D, double* out,
+                  const char* what) {
   if (!c) GPX_CHECK(scratch_ctx(&c));
   GPX_CUDA(cudaSetDevice(c->device));
-  KernParams kp;
-  GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
-  if (!X2) M = N;
-  if (N < 1 || M < 1) GPX_FAIL("empty input");
   PointSet p1, p2;
-  GPX_CHECK(upload_points(c, &kp, X, N, p1));
-  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
+  GPX_CHECK(upload_points(c, k, X, N, D, p1));
+  if (X2) GPX_CHECK(upload_points(c, k, X2, M, D, p2));
   PointSet& pj = X2 ? p2 : p1;   // thread-mapped operand = X2 points (contiguous index of the row-major output)
   double* dout = nullptr;
   GPX_TMP_ALLOC(&dout, (size_t)N * M * 8, c->st);
-  // out == NULL: build on the device only (the result is dropped) and report the kernel time through gpx_get_stats
-  // (kbuild_ms / kbuild_bytes) — used to measure the rectangular K(X, Z) build of the sparse model at full size.
   cudaEvent_t e0, e1;
   int rc = ev_get(c, 0, &e0) || ev_get(c, 1, &e1);
   if (rc == 0) {
     cudaEventRecord(e0, c->st);
-    rc = build_K(c, &kp, pj, p1, dout, M);
+    rc = build_K(c, k, pj, p1, dout, M);
     cudaEventRecord(e1, c->st);
   }
   c->total_launches++;
   if (rc == 0 && out && cudaMemcpyAsync(out, dout, (size_t)N * M * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
-  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error("gpx_kern_K: device failure"); rc = -1; }
+  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error(std::string(what) + ": device failure"); rc = -1; }
   if (rc == 0) {
     cudaEventElapsedTime(&c->stats.kbuild_ms, e0, e1);
     c->stats.kbuild_bytes = 8.0 * (double)N * M + 8.0 * (double)(N + M) * D;
   }
   GPX_TMP_FREE(dout, c->st);
   return rc;
+}
+
+// update_gradients_full of k for a caller's dL_dK (N x M row-major) on c (NULL: the scratch context) -> k's gradient block
+static int kern_grad_full(gpx_ctx* c, Kern k, const double* X, int64_t N, const double* X2, int64_t M, int D,
+                          const double* dL_dK, double* grad) {
+  if (!c) GPX_CHECK(scratch_ctx(&c));
+  GPX_CUDA(cudaSetDevice(c->device));
+  PointSet p1, p2;
+  GPX_CHECK(upload_points(c, k, X, N, D, p1));
+  if (X2) GPX_CHECK(upload_points(c, k, X2, M, D, p2));
+  double *dd = nullptr, *dpart = nullptr;
+  GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
+  const GradFullParams gp = grad_params(k, p1, X2 ? p2 : p1, dd, 0);
+  GPX_TMP_ALLOC(&dpart, grad_full_doubles(k, gp) * 8, c->st);
+  GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
+  const int rc = grad_full_sum(c, k, gp, dpart, grad);
+  GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
+  return rc;
+}
+
+extern "C" {
+
+int gpx_kern_K(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
+               const double* X2, int64_t M, int D, double* out) {
+  if (!X || !lengthscale) GPX_FAIL("null argument");
+  KernParams kp{};
+  GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
+  if (!X2) M = N;
+  if (N < 1 || M < 1) GPX_FAIL("empty input");
+  return kern_K(c, &kp, X, N, X2, M, D, out, "gpx_kern_K");
+}
+
+int gpx_kern_part_K(gpx_ctx* c, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M, int D,
+                    double* out) {
+  if (!X || !out) GPX_FAIL("null argument");
+  MultiKern mk;
+  GPX_CHECK(fill_one_part(part, D, mk));
+  if (!X2) M = N;
+  if (N < 1 || M < 1) GPX_FAIL("empty input");
+  return kern_K(c, &mk, X, N, X2, M, D, out, "gpx_kern_part_K");
 }
 
 int gpx_kern_Kdiag(int kind, double variance, int64_t N, double* out) {
@@ -1059,22 +1114,24 @@ int gpx_kern_grad_full(gpx_ctx* c, int kind, int ard, double variance, const dou
                        int64_t N, const double* X2, int64_t M, int D, const double* dL_dK, double* dvariance,
                        double* dlengthscale) {
   if (!X || !dL_dK || !lengthscale || !dvariance || !dlengthscale) GPX_FAIL("null argument");
-  if (!c) GPX_CHECK(scratch_ctx(&c));
-  GPX_CUDA(cudaSetDevice(c->device));
-  KernParams kp;
+  KernParams kp{};
   GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
   if (!X2) M = N;
-  PointSet p1, p2;
-  GPX_CHECK(upload_points(c, &kp, X, N, p1));
-  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
-  double *dd = nullptr, *dpart = nullptr;
-  GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
-  const GradFullParams gp = grad_params(kp, p1, X2 ? p2 : p1, dd, 0);
-  GPX_TMP_ALLOC(&dpart, grad_full_doubles(gp) * 8, c->st);
-  GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
-  const int rc = grad_full_sum(c, gp, dpart, dvariance, dlengthscale);
-  GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
-  return rc;
+  double g[MAX_D + 1];
+  GPX_CHECK(kern_grad_full(c, &kp, X, N, X2, M, D, dL_dK, g));
+  *dvariance = g[0];
+  for (int q = 0; q < (kp.ard ? D : 1); q++) dlengthscale[q] = g[1 + q];
+  return 0;
+}
+
+int gpx_kern_part_grad_full(gpx_ctx* c, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M,
+                            int D, const double* dL_dK, double* grad) {
+  if (!X || !dL_dK || !grad) GPX_FAIL("null argument");
+  MultiKern mk;
+  GPX_CHECK(fill_one_part(part, D, mk));
+  if (!X2) M = N;
+  if (N < 1 || M < 1) GPX_FAIL("empty input");
+  return kern_grad_full(c, &mk, X, N, X2, M, D, dL_dK, grad);
 }
 
 int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
@@ -1086,114 +1143,16 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
   GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
   if (!X2) M = N;
   PointSet p1, p2;
-  GPX_CHECK(upload_points(c, &kp, X, N, p1));
-  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, p2));
+  GPX_CHECK(upload_points(c, &kp, X, N, D, p1));
+  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, D, p2));
   double *dd = nullptr, *dpart = nullptr;
   GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
-  const GradFullParams gp = grad_params(kp, p1, X2 ? p2 : p1, dd, 0);
+  const GradFullParams gp = grad_params(&kp, p1, X2 ? p2 : p1, dd, 0);
   GPX_TMP_ALLOC(&dpart, grad_X_doubles(c, gp) * 8, c->st);
   GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
   const int rc = grad_X(c, gp, dpart, grad);
   GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
   return rc;
-}
-
-}  // extern "C"
-
-// ---------------------------------------------------------------------------------------------------------------
-// stand-alone K / update_gradients_full of one composite part (kinds 0-3, 6, 7) with the K-build and the per-pair gradient
-// terms of the composite evaluation; the context's own kernel (c->mk, c->kp) is left alone
-// ---------------------------------------------------------------------------------------------------------------
-static int fill_one_part(const gpx_kern_part* part, int D, MultiKern& mk) {
-  if (!part) GPX_FAIL("null argument");
-  if (is_known(part->kind) && is_static(part->kind)) GPX_FAIL("White / Bias parts have no stand-alone entry");
-  if (D < 1 || D > MAX_D) GPX_FAIL("input dimension must be in [1, 64]");
-  gpx_kern_part one = *part;
-  one.term = 0;
-  double kdiag;
-  return fill_mk(mk, &one, 1, D, &kdiag);
-}
-
-// n host points (n x D row-major) stacked for the one-part kernel mk into temporaries owned by ps
-static int upload_part_points(gpx_ctx* c, const MultiKern& mk, int D, const double* X, long n, PointSet& ps) {
-  ps.n = n; ps.ld = (n + TILE - 1) / TILE * TILE; ps.st = c->st;
-  GPX_TMP_ALLOC(&ps.raw, (size_t)n * D * 8, c->st);
-  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * mk.sumD * 8, c->st);
-  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * 8, c->st);
-  GPX_CUDA(cudaMemcpyAsync(ps.raw, X, (size_t)n * D * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(launch_prep_multi(ps.raw, n, D, ps.ld, mk, ps.xT, ps.sq, c->st));
-  c->total_launches++;
-  return 0;
-}
-
-extern "C" {
-
-int gpx_kern_part_K(gpx_ctx* c, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M, int D,
-                    double* out) {
-  if (!X || !out) GPX_FAIL("null argument");
-  MultiKern mk;
-  GPX_CHECK(fill_one_part(part, D, mk));
-  if (!X2) M = N;
-  if (N < 1 || M < 1) GPX_FAIL("empty input");
-  if (!c) GPX_CHECK(scratch_ctx(&c));
-  GPX_CUDA(cudaSetDevice(c->device));
-  PointSet p1, p2;
-  GPX_CHECK(upload_part_points(c, mk, D, X, N, p1));
-  if (X2) GPX_CHECK(upload_part_points(c, mk, D, X2, M, p2));
-  const PointSet& pj = X2 ? p2 : p1;   // thread-mapped operand = X2 points (contiguous index of the row-major output)
-  double* dout = nullptr;
-  GPX_TMP_ALLOC(&dout, (size_t)N * M * 8, c->st);
-  KBuildMultiParams kb;
-  memset(&kb, 0, sizeof(kb));
-  kb.rowsT = pj.xT; kb.ld_rows = pj.ld; kb.sq_rows = pj.sq;
-  kb.colsT = p1.xT; kb.ld_cols = p1.ld; kb.sq_cols = p1.sq;
-  kb.out = dout; kb.ld = M; kb.nrows = M; kb.ncols = N; kb.same = X2 == nullptr; kb.mk = mk;
-  int rc = launch_kbuild_multi(kb, (int)(pj.ld / TILE), (int)(p1.ld / TILE), c->st);
-  c->total_launches++;
-  if (rc == 0 && cudaMemcpyAsync(out, dout, (size_t)N * M * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
-  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error("gpx_kern_part_K: device failure"); rc = -1; }
-  GPX_TMP_FREE(dout, c->st);
-  return rc;
-}
-
-int gpx_kern_part_grad_full(gpx_ctx* c, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M,
-                            int D, const double* dL_dK, double* grad) {
-  if (!X || !dL_dK || !grad) GPX_FAIL("null argument");
-  MultiKern mk;
-  GPX_CHECK(fill_one_part(part, D, mk));
-  if (!X2) M = N;
-  if (N < 1 || M < 1) GPX_FAIL("empty input");
-  if (!c) GPX_CHECK(scratch_ctx(&c));
-  GPX_CUDA(cudaSetDevice(c->device));
-  PointSet p1, p2;
-  GPX_CHECK(upload_part_points(c, mk, D, X, N, p1));
-  if (X2) GPX_CHECK(upload_part_points(c, mk, D, X2, M, p2));
-  const PointSet& pj = X2 ? p2 : p1;
-  const int rtiles = (int)(pj.ld / TILE), ctiles = (int)(p1.ld / TILE), nred = part_nred(mk.part[0]);
-  double *dd = nullptr, *dpart = nullptr;
-  GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
-  GPX_TMP_ALLOC(&dpart, (size_t)rtiles * ctiles * nred * 8, c->st);
-  GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
-  GradFullMultiParams gf;
-  memset(&gf, 0, sizeof(gf));
-  gf.rowsT = pj.xT; gf.ld_rows = pj.ld; gf.sq_rows = pj.sq;
-  gf.colsT = p1.xT; gf.ld_cols = p1.ld; gf.sq_cols = p1.sq;
-  gf.nrows = M; gf.ncols = N; gf.same = X2 == nullptr; gf.dL = dd; gf.partials = dpart; gf.mk = mk;
-  int rc = launch_grad_full_multi(gf, rtiles, ctiles, c->st);
-  c->total_launches++;
-  std::vector<double> hp((size_t)rtiles * ctiles * nred);
-  if (rc == 0 && cudaMemcpyAsync(hp.data(), dpart, hp.size() * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
-  if (cudaStreamSynchronize(c->st) != cudaSuccess) { gpx::set_error("gpx_kern_part_grad_full: device failure"); rc = -1; }
-  GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
-  if (rc) return rc;
-  std::vector<double> tot(nred, 0.0);   // the tiles' partials in fixed order
-  for (size_t t = 0; t < hp.size() / nred; t++)
-    for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
-  for (int t = 0; t < nred; t++) {
-    double v;
-    if (part_grad_entry(mk, 0, t, tot[t], &v)) grad[t] = v;
-  }
-  return 0;
 }
 
 }  // extern "C"
@@ -1324,7 +1283,7 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
   cudaStream_t st = c->st;
   const long ld = c->Npad, N = c->N;
   PointSet pn;
-  GPX_CHECK(upload_points(c, ctx_kern(c), Xnew, M, pn));
+  GPX_CHECK(upload_points(c, ctx_kern(c), Xnew, M, c->D, pn));
   // Kx as [M][ld] (each new point one zero-padded column of length ld): thread-mapped operand = training points
   double* Kx = nullptr; double* Tx = nullptr;
   GPX_TMP_ALLOC(&Kx, (size_t)pn.ld * ld * 8, c->st);
@@ -1358,7 +1317,7 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
     if (rc) return rc;
     for (long m = 0; m < M; m++) {
       for (int q = 0; q < c->P; q++) mu[m * c->P + q] = h[(size_t)q * M + m];
-      var[m] = c->kp.variance - h[(size_t)c->P * M + m];
+      var[m] = c->kdiag - h[(size_t)c->P * M + m];
     }
     return 0;
   }

@@ -50,7 +50,8 @@ struct gpx_ctx {
   // last evaluation
   bool have_eval = false;
   bool have_kinv = false;    // c->Kinv holds K^-1 of the last evaluation (its route stored it, or gpx_get made it)
-  gpx::KernParams kp{};
+  gpx::KernParams kp{};      // the single kernel of the last evaluation (unused after a composite one: see `multi`)
+  double kdiag = 0;          // Kdiag of the last evaluation's kernel (jitter ladder, gpx_predict)
   double noise = 0, jitter = 0, jitter_extra = 0;
   // heteroscedastic evaluation (gpx_exact_eval_het): per-point noise variances in, diag(dL_dK) out
   bool het = false;
@@ -114,8 +115,16 @@ int fill_kp(KernParams& kp, int kind, int ard, int D, double variance, const dou
 #define GPX_TMP_ALLOC(ptr, bytes, st) GPX_CUDA(cudaMallocAsync((void**)(ptr), (bytes), (st)))
 #define GPX_TMP_FREE(p, st) do { if (p) cudaFreeAsync((p), (st)); } while (0)
 
-// n points prepared for a kernel: scaled coordinates xT, SoA [D][ld] (composite: [sumD][ld]), and their squared norms sq,
-// [ld] (composite: [nparts][ld])
+// The covariance function a helper below works with: a single stationary kernel or a composite one (exactly one is set)
+struct Kern {
+  const KernParams* kp = nullptr;
+  const MultiKern* mk = nullptr;
+  Kern(const KernParams* k) : kp(k) {}
+  Kern(const MultiKern* m) : mk(m) {}
+  int coord_rows() const { return kp ? kp->D : mk->sumD; }   // rows of a point set's stacked coordinates
+  int norm_rows() const { return kp ? 1 : mk->nparts; }      // rows of its squared norms
+};
+// n points prepared for a kernel: scaled coordinates xT, SoA [coord_rows][ld], and their squared norms sq, [norm_rows][ld]
 struct Points { double* xT = nullptr; double* sq = nullptr; long n = 0, ld = 0; };
 struct PointSet : Points {   // host points uploaded and prepared in temporaries it owns
   double* raw = nullptr;
@@ -126,21 +135,24 @@ struct KyDiag { double add; const double* vec; };   // added to the diagonal of 
 
 // The K-build and prep launches are counted by the caller (into eval_launches inside an exact evaluation); the other
 // helpers count theirs into c->total_launches.
-int prep_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, long ld, double* xT, double* sq);
-// X: n points, row-major with kp->D columns (composite kernel: the context's D)
-int upload_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, PointSet& ps);
+// X: n points, row-major with D columns (a single kernel's D; a composite's dims index them)
+int prep_points(gpx_ctx* c, Kern k, const double* X, long n, int D, long ld, double* xT, double* sq);
+int upload_points(gpx_ctx* c, Kern k, const double* X, long n, int D, PointSet& ps);
 // K(rows, cols) into out[i + j * ld] (i: row point, j: column point), row tiles [rt0, rt0 + nrt) (nrt = 0: all of them;
 // a part of the rows: single kernel only). ky != nullptr: the factor workspace form of Ky (lower tiles, zero upper tiles,
 // identity padding, ky's diagonal terms).
-int build_K(gpx_ctx* c, const KernParams* kp, const Points& rows, const Points& cols, double* out, long ld,
-            const KyDiag* ky = nullptr, int rt0 = 0, int nrt = 0);
-// dL_dK (device; element (i, j) of rows x cols at dL_dK[i * ldd + j], ldd = 0: cols.n) for the reductions below; the caller
-// may add the rank-P term or the transposed read
-GradFullParams grad_params(const KernParams& kp, const Points& rows, const Points& cols, const double* dL_dK, long ldd);
-// update_gradients_full: one row of partial sums per tile into `part` (grad_full_doubles), summed on the host in tile order
-size_t grad_full_doubles(const GradFullParams& gp);
-int grad_full_sum(gpx_ctx* c, GradFullParams gp, double* part, double* dvariance, double* dlengthscale);
-// gradients_X w.r.t. the row points: chunk partials and the N x D result in `part` (grad_X_doubles); the result is copied
+int build_K(gpx_ctx* c, Kern k, const Points& rows, const Points& cols, double* out, long ld, const KyDiag* ky = nullptr,
+            int rt0 = 0, int nrt = 0);
+// dL_dK (device; element (i, j) of rows x cols at dL_dK[i * ldd + j], ldd = 0: cols.n) for the reductions below. For a single
+// kernel the caller may add the rank-P term or the transposed read (gradients_X); a composite's reduction reads dL_dK with
+// ldd = cols.n and adds neither.
+GradFullParams grad_params(Kern k, const Points& rows, const Points& cols, const double* dL_dK, long ldd);
+// update_gradients_full: one reduction launch writes a row of partial sums per tile into `part` (grad_full_doubles); they are
+// summed on the host in tile order and mapped to k's gradient block in paramz order into grad (a single kernel: variance,
+// lengthscale(s); a composite: the block of its part 0, as part_grad_entry maps it)
+size_t grad_full_doubles(Kern k, const GradFullParams& gp);
+int grad_full_sum(gpx_ctx* c, Kern k, GradFullParams gp, double* part, double* grad);
+// gradients_X of a single kernel w.r.t. the row points: chunk partials and the N x D result in `part` (grad_X_doubles); the result is copied
 // to `out` on the host
 size_t grad_X_doubles(const gpx_ctx* c, const GradFullParams& gp);
 int grad_X(gpx_ctx* c, const GradFullParams& gp, double* part, double* out);

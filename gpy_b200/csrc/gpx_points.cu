@@ -1,6 +1,6 @@
 // gpx_points.cu — point sets, K-builds and the kernel-gradient reductions shared by the exact evaluation, the sparse
-// evaluation and the stand-alone kernel calls, for either kind of covariance function: a single stationary kernel
-// (`const KernParams* kp`) or the context's composite kernel c->mk (kp == nullptr).
+// evaluation and the stand-alone kernel calls, for either kind of covariance function: each helper is told which one it
+// works with (Kern: a single stationary kernel or a composite) and never falls back on the context's own.
 #include <algorithm>
 #include <cstring>
 #include <vector>
@@ -11,32 +11,31 @@
 
 namespace gpx {
 
-int prep_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, long ld, double* xT, double* sq) {
-  return kp ? launch_prep_x(X, n, ld, *kp, xT, sq, c->st) : launch_prep_multi(X, n, c->D, ld, c->mk, xT, sq, c->st);
+int prep_points(gpx_ctx* c, Kern k, const double* X, long n, int D, long ld, double* xT, double* sq) {
+  return k.kp ? launch_prep_x(X, n, ld, *k.kp, xT, sq, c->st) : launch_prep_multi(X, n, D, ld, *k.mk, xT, sq, c->st);
 }
 
-int upload_points(gpx_ctx* c, const KernParams* kp, const double* X, long n, PointSet& ps) {
-  const int D = kp ? kp->D : c->D;
+int upload_points(gpx_ctx* c, Kern k, const double* X, long n, int D, PointSet& ps) {
   ps.n = n; ps.ld = (n + TILE - 1) / TILE * TILE; ps.st = c->st;
   GPX_TMP_ALLOC(&ps.raw, (size_t)n * D * 8, c->st);
-  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * (kp ? kp->D : std::max(1, c->mk.sumD)) * 8, c->st);
-  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * (kp ? 1 : c->mk.nparts) * 8, c->st);
+  GPX_TMP_ALLOC(&ps.xT, (size_t)ps.ld * std::max(1, k.coord_rows()) * 8, c->st);   // static parts alone stack no rows
+  GPX_TMP_ALLOC(&ps.sq, (size_t)ps.ld * k.norm_rows() * 8, c->st);
   GPX_CUDA(cudaMemcpyAsync(ps.raw, X, (size_t)n * D * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(prep_points(c, kp, ps.raw, n, ps.ld, ps.xT, ps.sq));
+  GPX_CHECK(prep_points(c, k, ps.raw, n, D, ps.ld, ps.xT, ps.sq));
   c->total_launches++;
   return 0;
 }
 
-int build_K(gpx_ctx* c, const KernParams* kp, const Points& rows, const Points& cols, double* out, long ld, const KyDiag* ky,
-            int rt0, int nrt) {
+int build_K(gpx_ctx* c, Kern k, const Points& rows, const Points& cols, double* out, long ld, const KyDiag* ky, int rt0,
+            int nrt) {
   const int row_tiles = nrt ? nrt : (int)(rows.ld / TILE), col_tiles = (int)(cols.ld / TILE);
   const int same = rows.xT == cols.xT;   // one point set on both sides: exact zero distance on the diagonal
-  if (!kp) {
+  if (k.mk) {
     KBuildMultiParams kb;
     memset(&kb, 0, sizeof(kb));
     kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
     kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
-    kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.mk = c->mk;
+    kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.mk = *k.mk;
     if (ky) { kb.sym = 1; kb.diag_add = ky->add; }
     return launch_kbuild_multi(kb, row_tiles, col_tiles, c->st);
   }
@@ -44,37 +43,54 @@ int build_K(gpx_ctx* c, const KernParams* kp, const Points& rows, const Points& 
   memset(&kb, 0, sizeof(kb));
   kb.rowsT = rows.xT; kb.ld_rows = rows.ld; kb.sq_rows = rows.sq;
   kb.colsT = cols.xT; kb.ld_cols = cols.ld; kb.sq_cols = cols.sq;
-  kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.rt0 = rt0; kb.kp = *kp;
+  kb.out = out; kb.ld = ld; kb.nrows = rows.n; kb.ncols = cols.n; kb.same = same; kb.rt0 = rt0; kb.kp = *k.kp;
   if (ky) { kb.sym = 1; kb.diag_add = ky->add; kb.diag_vec = ky->vec; }
   return launch_kbuild(kb, row_tiles, col_tiles, c->st);
 }
 
-GradFullParams grad_params(const KernParams& kp, const Points& rows, const Points& cols, const double* dL_dK, long ldd) {
+GradFullParams grad_params(Kern k, const Points& rows, const Points& cols, const double* dL_dK, long ldd) {
   GradFullParams gp;
   memset(&gp, 0, sizeof(gp));
   gp.x1T = rows.xT; gp.ld1 = rows.ld; gp.sq1 = rows.sq; gp.N = rows.n;
   gp.x2T = cols.xT; gp.ld2 = cols.ld; gp.sq2 = cols.sq; gp.M = cols.n;
-  gp.dL_dK = dL_dK; gp.ldd = ldd; gp.same = rows.xT == cols.xT; gp.kp = kp;
+  gp.dL_dK = dL_dK; gp.ldd = ldd; gp.same = rows.xT == cols.xT;
+  if (k.kp) gp.kp = *k.kp;
   return gp;
 }
 
-size_t grad_full_doubles(const GradFullParams& gp) {
-  return (size_t)(gp.ld1 / TILE) * (gp.ld2 / TILE) * ((gp.kp.ard ? gp.kp.D : 1) + 1);
+// partial sums per tile of the update_gradients_full reduction: a single kernel's variance and lengthscale(s); a part's
+// gradient entries and tr(dL_dK)
+static int grad_full_nred(Kern k) { return k.kp ? (k.kp->ard ? k.kp->D : 1) + 1 : part_nred(k.mk->part[0]); }
+
+size_t grad_full_doubles(Kern k, const GradFullParams& gp) {
+  return (size_t)(gp.ld1 / TILE) * (gp.ld2 / TILE) * grad_full_nred(k);
 }
 
-int grad_full_sum(gpx_ctx* c, GradFullParams gp, double* part, double* dvariance, double* dlengthscale) {
-  const int nl = gp.kp.ard ? gp.kp.D : 1, nred = nl + 1;
-  gp.partials = part;
-  GPX_CHECK(launch_grad_full(gp, (int)(gp.ld2 / TILE), (int)(gp.ld1 / TILE), c->st));
+int grad_full_sum(gpx_ctx* c, Kern k, GradFullParams gp, double* part, double* grad) {
+  const int nred = grad_full_nred(k), tiles_j = (int)(gp.ld2 / TILE), tiles_i = (int)(gp.ld1 / TILE);
+  if (k.kp) {
+    gp.partials = part;
+    GPX_CHECK(launch_grad_full(gp, tiles_j, tiles_i, c->st));
+  } else {   // the composite reduction maps the column points to threads: rows and columns trade places
+    GradFullMultiParams gf;
+    memset(&gf, 0, sizeof(gf));
+    gf.rowsT = gp.x2T; gf.ld_rows = gp.ld2; gf.sq_rows = gp.sq2;
+    gf.colsT = gp.x1T; gf.ld_cols = gp.ld1; gf.sq_cols = gp.sq1;
+    gf.nrows = gp.M; gf.ncols = gp.N; gf.same = gp.same; gf.dL = gp.dL_dK; gf.partials = part; gf.mk = *k.mk;
+    GPX_CHECK(launch_grad_full_multi(gf, tiles_j, tiles_i, c->st));
+  }
   c->total_launches++;
-  std::vector<double> hp(grad_full_doubles(gp));
+  std::vector<double> hp(grad_full_doubles(k, gp));
   GPX_CUDA(cudaMemcpyAsync(hp.data(), part, hp.size() * 8, cudaMemcpyDeviceToHost, c->st));
   GPX_CUDA(cudaStreamSynchronize(c->st));
   std::vector<double> tot(nred, 0.0);
   for (size_t t = 0; t < hp.size() / nred; t++)
     for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
-  *dvariance = tot[0];
-  for (int q = 0; q < nl; q++) dlengthscale[q] = -tot[1 + q] / gp.kp.ls[q];
+  double v;
+  for (int q = 0; q < nred; q++) {
+    if (k.kp) grad[q] = q ? -tot[q] / k.kp->ls[q - 1] : tot[0];   // stationary.py:210,213
+    else if (part_grad_entry(*k.mk, 0, q, tot[q], &v)) grad[q] = v;
+  }
   return 0;
 }
 

@@ -258,8 +258,7 @@ static int mul_psi1T(gpx_ctx* c, const double* A, double* C, int tri) {
 // and C (device, s->Cm as [P][Mpad]) must be in place. Results on the host.
 // bvec (device, [Npad], per-point precisions) selects the heteroscedastic form: VVT_factor = beta_n Y_n and the columns of
 // W2 psi1^T scaled by beta_n (var_dtc.py:226); W2 is then 2 dL_dpsi2_beta without the scalar beta.
-static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double* dvariance, double* dlengthscale,
-                            double* dZ) {
+static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double* grad, double* dZ) {
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
   const long Mpad = s->Mpad, N = s->N, Npad = s->Npad;
@@ -275,12 +274,12 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
     GPX_CHECK(launched(c));
   }
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
-  GradFullParams gp = grad_params(s->kp, s->xpts(), s->zpts(), s->dLt, Mpad);
+  GradFullParams gp = grad_params(&s->kp, s->xpts(), s->zpts(), s->dLt, Mpad);
   gp.ci = s->Yb; gp.ldci = Npad; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = P;
-  GPX_CHECK(ensure_part(s, grad_full_doubles(gp) * 8));
-  GPX_CHECK(grad_full_sum(c, gp, s->part, dvariance, dlengthscale));
+  GPX_CHECK(ensure_part(s, grad_full_doubles(&s->kp, gp) * 8));
+  GPX_CHECK(grad_full_sum(c, &s->kp, gp, s->part, grad));
   // dL/dZ: gradients_X(dL_dKnm^T, Z, X): rows = inducing points, columns = data points, dL read transposed
-  GradFullParams gx = grad_params(s->kp, s->zpts(), s->xpts(), s->dLt, Mpad);
+  GradFullParams gx = grad_params(&s->kp, s->zpts(), s->xpts(), s->dLt, Mpad);
   gx.transposed = 1; gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = s->Yb; gx.ldcj = Npad; gx.cP = P;
   GPX_CHECK(ensure_part(s, grad_X_doubles(c, gx) * 8));
   return grad_X(c, gx, s->part, dZ);
@@ -493,32 +492,28 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   GPX_CHECK(combine(c, s->W2, Mpad, beta, E, 0.0, nullptr, 0.0));
   // Knm part: needs C in s->Cm
   GPX_CUDA(cudaMemcpyAsync(s->Cm, Cv, (size_t)P * Mpad * 8, cudaMemcpyDeviceToDevice, st));
-  double dv_knm = 0.0;
-  std::vector<double> dl_knm(nl, 0.0);
-  GPX_CHECK(knm_grads_device(c, beta, bvec, &dv_knm, dl_knm.data(), dZ));               // dZ <- Knm part
+  std::vector<double> g_knm(1 + nl, 0.0);
+  GPX_CHECK(knm_grads_device(c, beta, bvec, g_knm.data(), dZ));                         // dZ <- Knm part
   {
     int rank = 0, G = 1;
     dist_world(c, &rank, &G);
     if (G > 1) {   // sums over this rank's data points -> totals
       std::vector<double> h((size_t)1 + nl + (size_t)M * D);
-      h[0] = dv_knm;
-      for (int q = 0; q < nl; q++) h[1 + q] = dl_knm[q];
+      memcpy(h.data(), g_knm.data(), (size_t)(1 + nl) * 8);
       memcpy(h.data() + 1 + nl, dZ, (size_t)M * D * 8);
       GPX_CUDA(cudaMemcpyAsync(s->gsum, h.data(), h.size() * 8, cudaMemcpyHostToDevice, st));
       GPX_CHECK(dist_allreduce_sum(c, s->gsum, h.size(), st));
       GPX_CUDA(cudaMemcpyAsync(h.data(), s->gsum, h.size() * 8, cudaMemcpyDeviceToHost, st));
       GPX_CUDA(cudaStreamSynchronize(st));
-      dv_knm = h[0];
-      for (int q = 0; q < nl; q++) dl_knm[q] = h[1 + q];
+      memcpy(g_knm.data(), h.data(), (size_t)(1 + nl) * 8);
       memcpy(dZ, h.data() + 1 + nl, (size_t)M * D * 8);
     }
   }
   // Kmm part: kern.update_gradients_full(dL_dKmm, Z) and kern.gradients_X(dL_dKmm, Z)  (sparse_gp.py:114,117)
-  const GradFullParams gk = grad_params(s->kp, s->zpts(), s->zpts(), Kd, Mpad);
-  double dv_kmm = 0.0;
-  std::vector<double> dl_kmm(nl, 0.0), hz((size_t)M * D);
-  GPX_CHECK(ensure_part(s, grad_full_doubles(gk) * 8));
-  GPX_CHECK(grad_full_sum(c, gk, s->part, &dv_kmm, dl_kmm.data()));
+  const GradFullParams gk = grad_params(&s->kp, s->zpts(), s->zpts(), Kd, Mpad);
+  std::vector<double> g_kmm(1 + nl, 0.0), hz((size_t)M * D);
+  GPX_CHECK(ensure_part(s, grad_full_doubles(&s->kp, gk) * 8));
+  GPX_CHECK(grad_full_sum(c, &s->kp, gk, s->part, g_kmm.data()));
   GPX_CHECK(ensure_part(s, grad_X_doubles(c, gk) * 8));
   GPX_CHECK(grad_X(c, gk, s->part, hz.data()));
   for (size_t i = 0; i < hz.size(); i++) dZ[i] += hz[i];
@@ -564,8 +559,8 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     const double lik_1h = -0.5 * nd * od * log2pi + 0.5 * od * sums[0] - 0.5 * sums[2];
     const double lik_2h = -0.5 * od * (variance * sums[1] - trA);
     *lml = lik_1h + lik_2h + lik_3 + lik_4;
-    grad[0] = -0.5 * od * sums[1] + dv_knm + dv_kmm;                                       // update_gradients_diag (:110)
-    for (int q = 0; q < nl; q++) grad[1 + q] = dl_knm[q] + dl_kmm[q];
+    grad[0] = -0.5 * od * sums[1] + g_knm[0] + g_kmm[0];                                   // update_gradients_diag (:110)
+    for (int q = 0; q < nl; q++) grad[1 + q] = g_knm[1 + q] + g_kmm[1 + q];
     s->have_eval = true;
     return 0;
   }
@@ -578,8 +573,8 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   // d beta / d noise is folded by the reference into dL_dR (gradient wrt the noise VARIANCE): exact_inference_gradients
   // sums dL_dR as is (var_dtc.py:176, gaussian.py:78-79)
   const double dvar_diag = -0.5 * od * beta * nd;                                          // update_gradients_diag (:110)
-  grad[0] = dvar_diag + dv_knm + dv_kmm;
-  for (int q = 0; q < nl; q++) grad[1 + q] = dl_knm[q] + dl_kmm[q];
+  grad[0] = dvar_diag + g_knm[0] + g_kmm[0];
+  for (int q = 0; q < nl; q++) grad[1 + q] = g_knm[1 + q] + g_kmm[1 + q];
   grad[1 + nl] = dL_dR;
   s->have_eval = true;
   return 0;

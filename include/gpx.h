@@ -120,7 +120,8 @@ int gpx_exact_eval_multi(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, d
  * for callers that hold a kernel object outside an evaluation (PosteriorExact._raw_predict, the generic inference path).
  * X (N x D) and X2 (M x D) are row-major with the D columns `part->dims` index into; X2 == NULL -> X2 = X with exact zero
  * distance on the diagonal. The K-build and the per-pair gradient terms are those of gpx_exact_eval_multi.
- *   gpx_kern_part_K         : out, N x M row-major (like gpx_kern_K).
+ *   gpx_kern_part_K         : out, N x M row-major (like gpx_kern_K; it reports kbuild_ms and kbuild_bytes through
+ *                             gpx_get_stats as well, but out must not be NULL).
  *   gpx_kern_part_grad_full : dL_dK N x M row-major in; grad out, the part's gradient block (as above). */
 int gpx_kern_part_K(gpx_ctx* ctx, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M, int D,
                     double* out);

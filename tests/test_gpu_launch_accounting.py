@@ -2,6 +2,7 @@
 kernels the sparse evaluation runs on its child contexts (the factorisations of Kmm and of B = I + A) and the assembles
 it issues on their streams. Around each call, the CUDA kernel activities recorded by torch.profiler are counted (copies
 and memsets are not kernels) and compared with the call's total_launches() delta."""
+import ctypes
 import json
 import os
 import tempfile
@@ -80,6 +81,8 @@ def test_kernel_calls_pdinv_and_exact_evaluation_count_every_launch():
     rng, X, Y = _problem(1100, 3, 1, 3)
     X2 = rng.uniform(-3, 3, (260, 3))
     ls = np.array([1.2, 1.6, 2.1])
+    part, keep = _ffi.GpxKernPart(), []   # the same kernel as one composite part
+    _ffi._fill_part(part, ("matern52", True, 0, [0, 1, 2], 1.3, ls), keep)
     e = _ffi.Engine(0)
     L, h, p = _ffi.lib(), e._h, _ffi._ptr
     try:
@@ -87,18 +90,23 @@ def test_kernel_calls_pdinv_and_exact_evaluation_count_every_launch():
             M = 1100 if x2 is None else 260
             dL = rng.standard_normal((1100, M))
             out, gx = np.empty((1100, M)), np.empty((1100, 3))
-            dv, dl = np.zeros(1), np.zeros(3)
+            dv, dl, g = np.zeros(1), np.zeros(3), np.zeros(4)
             calls = {
                 "kern_K": lambda: L.gpx_kern_K(h, 3, 1, 1.3, p(ls), p(X), 1100, p(x2), M, 3, p(out)),
                 "kern_grad_full": lambda: L.gpx_kern_grad_full(h, 3, 1, 1.3, p(ls), p(X), 1100, p(x2), M, 3, p(dL), p(dv),
                                                                p(dl)),
                 "kern_grad_X": lambda: L.gpx_kern_grad_X(h, 3, 1, 1.3, p(ls), p(X), 1100, p(x2), M, 3, p(dL), p(gx)),
+                "kern_part_K": lambda: L.gpx_kern_part_K(h, ctypes.byref(part), p(X), 1100, p(x2), M, 3, p(out)),
+                "kern_part_grad_full": lambda: L.gpx_kern_part_grad_full(h, ctypes.byref(part), p(X), 1100, p(x2), M, 3, p(dL),
+                                                                         p(g)),
             }
             for name, call in calls.items():
                 assert call() == 0
                 rc = []
-                _counted(e, lambda: rc.append(call()), "%s X2=%s" % (name, x2 is not None))
+                names = _counted(e, lambda: rc.append(call()), "%s X2=%s" % (name, x2 is not None))
                 assert rc == [0]
+                if name.startswith("kern_part"):   # a part of kind 0-3 runs the composite kernels
+                    assert all("multi" in k for k in names), names
         e.set_data(X, Y)
         e.exact_eval("matern32", True, 1.3, ls, 0.05)
         _counted(e, lambda: e.exact_eval("rbf", True, 1.3, ls, 0.05), "exact_eval (5 blocks)")
