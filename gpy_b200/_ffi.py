@@ -94,6 +94,8 @@ EXPORTS = {
     "gpx_sparse_eval": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64,
                                        ctypes.c_double, _dp, _dp, _dp]),
     "gpx_sparse_get": (ctypes.c_int, [_vp, ctypes.c_int, _dp]),
+    "gpx_sparse_eval_multi": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64,
+                                             ctypes.c_double, _dp, _dp, _dp, _dp, _dp]),
     "gpx_sparse_eval_het": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64,
                                            _dp, _dp, _dp, _dp, _dp]),
     "gpx_pdinv": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
@@ -320,6 +322,32 @@ class Engine(object):
         self.sM, self._snl = M, ls.size
         self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
         return lml.value, grad, dZ, dR
+
+    def sparse_eval_multi(self, parts, Z, noise):
+        """VarDTC with a composite kernel (parts as exact_eval_multi takes them; RBF .. Matern52, White, Bias). noise: a
+        scalar variance -> (lml, grad [every part's block, noise], dZ (M x D)); one variance per data point ->
+        (lml, grad [every part's block], dZ, dL_dR (N x P))"""
+        Z = _f64(Z)
+        M = Z.shape[0]
+        arr = (GpxKernPart * len(parts))()
+        keep, ngrad = [], 0
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
+        nv = np.asarray(noise, dtype=np.float64).reshape(-1)
+        het = nv.size > 1 or np.ndim(noise) > 0
+        if het and nv.size != self.sN:
+            raise ValueError("one noise variance per data point expected (%d given, N = %d)" % (nv.size, self.sN))
+        nv = _f64(nv)
+        lml = ctypes.c_double()
+        grad = np.zeros(ngrad + (0 if het else 1))
+        dZ = np.empty((M, self.sD))
+        dR = np.empty((self.sN, self.sP)) if het else None
+        check(self._L.gpx_sparse_eval_multi(self._h, arr, len(parts), _ptr(Z), M, 0.0 if het else float(nv[0]),
+                                            _ptr(nv) if het else None, ctypes.byref(lml), _ptr(grad), _ptr(dZ), _ptr(dR)),
+              "gpx_sparse_eval_multi")
+        self.sM = M
+        self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
+        return (lml.value, grad, dZ, dR) if het else (lml.value, grad, dZ)
 
     SPARSE_GET = {"woodbury_vector": 0, "woodbury_inv": 1, "Kmm": 2, "Lm": 3}
 

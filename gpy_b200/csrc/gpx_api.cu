@@ -751,7 +751,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
 }
 
 // the parts of a composite kernel -> mk (validated), *kdiag_total = Kdiag of the composite kernel. Dfull: columns of X.
-static int fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Dfull, double* kdiag_total) {
+int gpx::fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Dfull, double* kdiag_total) {
   if (!parts || nparts < 1 || nparts > MAX_PARTS) GPX_FAIL("number of kernel parts must be in [1, 8]");
   memset(&mk, 0, sizeof(mk));
   mk.nparts = nparts;
@@ -1148,9 +1148,9 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
   double *dd = nullptr, *dpart = nullptr;
   GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
   const GradFullParams gp = grad_params(&kp, p1, X2 ? p2 : p1, dd, 0);
-  GPX_TMP_ALLOC(&dpart, grad_X_doubles(c, gp) * 8, c->st);
+  GPX_TMP_ALLOC(&dpart, grad_X_doubles(c, &kp, gp, D) * 8, c->st);
   GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
-  const int rc = grad_X(c, gp, dpart, grad);
+  const int rc = grad_X(c, &kp, gp, D, dpart, grad);
   GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
   return rc;
 }

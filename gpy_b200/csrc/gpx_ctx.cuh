@@ -143,17 +143,19 @@ int upload_points(gpx_ctx* c, Kern k, const double* X, long n, int D, PointSet& 
 // identity padding, ky's diagonal terms).
 int build_K(gpx_ctx* c, Kern k, const Points& rows, const Points& cols, double* out, long ld, const KyDiag* ky = nullptr,
             int rt0 = 0, int nrt = 0);
-// dL_dK (device; element (i, j) of rows x cols at dL_dK[i * ldd + j], ldd = 0: cols.n) for the reductions below. For a single
-// kernel the caller may add the rank-P term or the transposed read (gradients_X); a composite's reduction reads dL_dK with
-// ldd = cols.n and adds neither.
+// dL_dK (device; element (i, j) of rows x cols at dL_dK[i * ldd + j], ldd = 0: cols.n) for the reductions below. The caller
+// may add the rank-P term (ci, cj, cP) and, for gradients_X, the transposed read.
 GradFullParams grad_params(Kern k, const Points& rows, const Points& cols, const double* dL_dK, long ldd);
-// update_gradients_full: one reduction launch writes a row of partial sums per tile into `part` (grad_full_doubles); they are
-// summed on the host in tile order and mapped to k's gradient block in paramz order into grad (a single kernel: variance,
-// lengthscale(s); a composite: the block of its part 0, as part_grad_entry maps it)
+// update_gradients_full: one reduction launch per part (a single kernel: one) writes a row of partial sums per tile into
+// `part` (grad_full_doubles); they are summed on the host in tile order and mapped to k's gradient block in paramz order
+// into grad (a single kernel: variance, lengthscale(s); a composite: every part's block in turn, as part_grad_entry maps it)
 size_t grad_full_doubles(Kern k, const GradFullParams& gp);
 int grad_full_sum(gpx_ctx* c, Kern k, GradFullParams gp, double* part, double* grad);
-// gradients_X of a single kernel w.r.t. the row points: chunk partials and the N x D result in `part` (grad_X_doubles); the result is copied
-// to `out` on the host
-size_t grad_X_doubles(const gpx_ctx* c, const GradFullParams& gp);
-int grad_X(gpx_ctx* c, const GradFullParams& gp, double* part, double* out);
+// gradients_X w.r.t. the row points (D: columns of their host X; a single kernel's own D): chunk partials and the N x D
+// result in `part` (grad_X_doubles); the result is copied to `out` on the host. A composite's RatQuad / StdPeriodic parts
+// have no device gradients_X (rc -2).
+size_t grad_X_doubles(const gpx_ctx* c, Kern k, const GradFullParams& gp, int D);
+int grad_X(gpx_ctx* c, Kern k, const GradFullParams& gp, int D, double* part, double* out);
+// the parts of a composite kernel -> mk (validated against Dfull columns of X), *kdiag_total = its Kdiag (gpx_api.cu)
+int fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Dfull, double* kdiag_total);
 }  // namespace gpx

@@ -360,7 +360,7 @@ __global__ void __launch_bounds__(256) grad_full_multi_kernel(GradFullMultiParam
   const int tid = threadIdx.x;
   load_tiles(mk, p.rowsT, p.ld_rows, p.sq_rows, rt, p.colsT, p.ld_cols, p.sq_cols, ct, sR, sC, sSr, sSc);
   __syncthreads();
-  const PartDev me = mk.part[0];
+  const PartDev me = mk.part[p.part];
   const int il = tid & (TILE - 1), half = tid >> 7;
   const long gi = (long)rt * TILE + il;
   double xi[DREG], gq[DREG];
@@ -372,7 +372,8 @@ __global__ void __launch_bounds__(256) grad_full_multi_kernel(GradFullMultiParam
       const int jl = half * 64 + jj;
       const long gj = (long)ct * TILE + jl;
       if (gj >= p.ncols) break;
-      pair_accumulate<DREG, EXT>(mk, 0, me, sR, sC, sSr, sSc, il, jl, p.same && gi == gj, 1.0, p.dL[gj * p.nrows + gi], xi, gq, s);
+      pair_accumulate<DREG, EXT>(mk, p.part, me, sR, sC, sSr, sSc, il, jl, p.same && gi == gj, 1.0, p.dL[gj * p.ldd + gi], xi,
+                                 gq, s);
     }
   }
   store_part_sums<DREG, EXT>(me, s, gq, sRed, p.partials + ((long)ct * gridDim.y + rt) * part_nred(me));
@@ -422,7 +423,7 @@ static int launch_gfm_t(const GradFullMultiParams& p, dim3 grid, size_t smem, cu
 }
 
 int launch_grad_full_multi(const GradFullMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st) {
-  const int D = dreg_for(p.mk.part[0]);
+  const int D = dreg_for(p.mk.part[p.part]);
   const dim3 grid(col_tiles, row_tiles);
   const size_t smem = multi_tile_smem(p.mk);
   if (has_ext(p.mk)) {
@@ -435,6 +436,160 @@ int launch_grad_full_multi(const GradFullMultiParams& p, int row_tiles, int col_
   if (D <= 16) return launch_gfm_t<16, false>(p, grid, smem, st);
   if (D <= 32) return launch_gfm_t<32, false>(p, grid, smem, st);
   return launch_gfm_t<64, false>(p, grid, smem, st);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// gradients_X of a composite kernel: Add.gradients_X sums the parts' (add.py:88-100), Prod.gradients_X hands each factor
+// dL_dK times the other factors (prod.py:397-407), and a stationary factor reduces it like Stationary.gradients_X
+// (stationary.py:325-345): tmp = variance (1/r) dk/dr dL (1/0 := 0), grad[n, d] = sum_m tmp (x_n,d - x_m,d) / l^2. White
+// and Bias have no input gradient and enter as factors only. The layout is gradx_kernel's: one CTA = 128 row points x one
+// column chunk, dL_dK tiles of 128 x 32 through shared memory, per-chunk partials per stacked row reduced in fixed order.
+// The row points' stacked inputs sit in shared memory (each thread reads its own column), the chunk's 32 column points
+// beside them. Kinds RBF .. Matern52, White and Bias only: the caller rejects RatQuad / StdPeriodic parts.
+// ---------------------------------------------------------------------------------------------------------------
+// scaled distance of stationary part p between row point il (stride TILE) and chunk column point mm (stride 32)
+__device__ __forceinline__ double gx_part_r(const PartDev& pd, int p, const double* sR, const double* sC, const double* sSr,
+                                            const double* sSc, int il, int mm, bool samept) {
+  double dot = 0.0;
+  for (int q = 0; q < pd.D; q++) dot = fma(sR[(pd.xoff + q) * TILE + il], sC[(pd.xoff + q) * 32 + mm], dot);
+  double r2 = sSr[p * TILE + il] + sSc[p * 32 + mm] - 2.0 * dot;
+  if (samept) r2 = 0.0;
+  return sqrt(fmax(r2, 0.0)) * pd.inv_ls_iso;
+}
+
+template <int DREG>
+__global__ void __launch_bounds__(TILE) gradx_multi_kernel(GradXMultiParams p, long mchunk, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char gxm_smem[];
+  const MultiKern& mk = p.mk;
+  double (*sdl)[33] = reinterpret_cast<double (*)[33]>(gxm_smem);   // [128][33] dL_dK tile
+  double* sR = reinterpret_cast<double*>(gxm_smem) + TILE * 33;     // [sumD][128] row points
+  double* sSr = sR + (size_t)mk.sumD * TILE;                        // [nparts][128]
+  double* sC = sSr + (size_t)mk.nparts * TILE;                      // [sumD][32] column chunk
+  double* sSc = sC + (size_t)mk.sumD * 32;                          // [nparts][32]
+  const int tid = threadIdx.x;
+  const long r0 = (long)blockIdx.x * TILE, n = r0 + tid;
+  const long m_beg = (long)blockIdx.y * mchunk;
+  const long m_end = m_beg + mchunk < p.ncols ? m_beg + mchunk : p.ncols;
+  for (int q = 0; q < mk.sumD; q++) sR[q * TILE + tid] = p.rowsT[(long)q * p.ld_rows + n];
+  for (int q = 0; q < mk.nparts; q++) sSr[q * TILE + tid] = p.sq_rows[(long)q * p.ld_rows + n];
+  double acc[DREG];
+#pragma unroll
+  for (int q = 0; q < DREG; q++) acc[q] = 0.0;
+  for (long m0 = m_beg; m0 < m_end; m0 += 32) {
+    __syncthreads();
+    if (!p.transposed) {
+      for (int rr = tid >> 5; rr < TILE; rr += TILE / 32) {
+        const long gn = r0 + rr, gm = m0 + (tid & 31);
+        double dv = 0.0;
+        if (gn < p.nrows && gm < m_end) dv = p.dL[gn * p.ldd + gm];
+        sdl[rr][tid & 31] = dv;
+      }
+    } else {
+      for (int mm = 0; mm < 32; mm++) {
+        const long gm = m0 + mm;
+        double dv = 0.0;
+        if (n < p.nrows && gm < m_end) dv = p.dL[gm * p.ldd + n];
+        sdl[tid][mm] = dv;
+      }
+    }
+    for (int idx = tid; idx < mk.sumD * 32; idx += TILE) {
+      const int q = idx >> 5, mm = idx & 31;
+      sC[idx] = (m0 + mm < p.ncols) ? p.colsT[(long)q * p.ld_cols + m0 + mm] : 0.0;
+    }
+    for (int idx = tid; idx < mk.nparts * 32; idx += TILE) {
+      const int q = idx >> 5, mm = idx & 31;
+      sSc[idx] = (m0 + mm < p.ncols) ? p.sq_cols[(long)q * p.ld_cols + m0 + mm] : 0.0;
+    }
+    __syncthreads();
+    if (n < p.nrows) {
+      const int mlim = (int)((m_end - m0) < 32 ? (m_end - m0) : 32);
+      for (int mm = 0; mm < mlim; mm++) {
+        const long gm = m0 + mm;
+        const bool samept = p.same && n == gm;
+        double dl = sdl[tid][mm];
+        if (p.same) dl += p.dL[gm * p.ldd + n];                  // tmp + tmp^T (stationary.py:334-336)
+        for (int pi = 0; pi < mk.nparts; pi++) {
+          const PartDev& pd = mk.part[pi];
+          if (!is_stationary(pd.kind)) continue;
+          const double rr = gx_part_r(pd, pi, sR, sC, sSr, sSc, tid, mm, samept);
+          if (rr == 0.0) continue;
+          double kk, dk;
+          k_dk_of_r_unit(pd.kind, rr, kk, dk);
+          double t = pd.variance * dk * dl / rr;
+          for (int q = 0; q < mk.nparts; q++) {          // the other factors of this part's term
+            const PartDev& o = mk.part[q];
+            if (q == pi || o.term != pd.term) continue;
+            const double v = o.kind == GPX_BIAS ? 1.0
+                             : o.kind == GPX_WHITE ? (samept ? 1.0 : 0.0)
+                             : k_of_r_unit(o.kind, gx_part_r(o, q, sR, sC, sSr, sSc, tid, mm, samept));
+            t *= o.variance * v;
+          }
+#pragma unroll
+          for (int q = 0; q < DREG; q++)
+            if (q >= pd.xoff && q < pd.xoff + pd.D) acc[q] = fma(t, sR[q * TILE + tid] - sC[q * 32 + mm], acc[q]);
+        }
+      }
+    }
+  }
+  if (n < p.nrows) {
+#pragma unroll
+    for (int q = 0; q < DREG; q++)
+      if (q < mk.sumD) part[((long)blockIdx.y * p.nrows + n) * mk.sumD + q] = acc[q];
+  }
+}
+
+// out[n, d] = sum over the stationary parts' stacked rows q on data column d, in part order, of the chunk sums (fixed order)
+// divided by l_q (ARD: the points were scaled) or l^2 (iso)
+__global__ void gradx_multi_reduce_kernel(const double* __restrict__ part, long N, int nchunk, int Dfull, MultiKern mk,
+                                          double* __restrict__ out) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N * Dfull) return;
+  const long n = i / Dfull;
+  const int d = (int)(i % Dfull);
+  double s = 0.0;
+  for (int pi = 0; pi < mk.nparts; pi++) {
+    const PartDev& pd = mk.part[pi];
+    if (!is_stationary(pd.kind)) continue;
+    for (int q = pd.xoff; q < pd.xoff + pd.D; q++) {
+      if (mk.dims[q] != d) continue;
+      double t = 0.0;
+      for (int c = 0; c < nchunk; c++) t += part[((long)c * N + n) * mk.sumD + q];
+      const double l = mk.ls[q];
+      s += pd.ard ? t / l : t / (l * l);
+    }
+  }
+  out[i] = s;
+}
+
+template <int DREG>
+static int launch_gxm_t(const GradXMultiParams& p, dim3 grid, size_t smem, long mchunk, double* part, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    const int mx = (TILE * 33 + (MAX_D + MAX_PARTS) * (TILE + 32)) * 8;
+    GPX_CUDA(cudaFuncSetAttribute(gradx_multi_kernel<DREG>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx));
+    attr_set = true;
+  }
+  gradx_multi_kernel<DREG><<<grid, TILE, smem, st>>>(p, mchunk, part);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int launch_gradx_multi(const GradXMultiParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st) {
+  const MultiKern& mk = p.mk;
+  if (has_ext(mk)) { set_error("gradients_X: RatQuad / StdPeriodic parts have no input gradient on the device"); return -2; }
+  const size_t smem = (size_t)(TILE * 33 + (mk.sumD + mk.nparts) * (TILE + 32)) * 8;
+  const dim3 grid((unsigned)((p.nrows + TILE - 1) / TILE), nchunk);
+  const int D = mk.sumD;
+  int rc;
+  if (D <= 8) rc = launch_gxm_t<8>(p, grid, smem, mchunk, part, st);
+  else if (D <= 16) rc = launch_gxm_t<16>(p, grid, smem, mchunk, part, st);
+  else if (D <= 32) rc = launch_gxm_t<32>(p, grid, smem, mchunk, part, st);
+  else rc = launch_gxm_t<64>(p, grid, smem, mchunk, part, st);
+  if (rc) return rc;
+  gradx_multi_reduce_kernel<<<(unsigned)((p.nrows * p.Dfull + 255) / 256), 256, 0, st>>>(part, p.nrows, nchunk, p.Dfull, mk,
+                                                                                         out);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------

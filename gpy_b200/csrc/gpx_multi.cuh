@@ -78,15 +78,28 @@ struct GradKinvMultiParams {
   MultiKern mk;
 };
 
-// update_gradients_full of part 0 of mk for a dense dL_dK: rows = thread-mapped points (X2 of the call), cols = the X
-// points; dL_dK element (col point i, row point j) at dL[i * nrows + j]
+// update_gradients_full of one part of mk for a dense dL_dK: rows = thread-mapped points (X2 of the call), cols = the X
+// points; dL_dK element (col point i, row point j) at dL[i * ldd + j]
 struct GradFullMultiParams {
   const double* rowsT; long ld_rows; const double* sq_rows;
   const double* colsT; long ld_cols; const double* sq_cols;
   long nrows, ncols;
   int same;
-  const double* dL;
+  int part;                                                    // the part whose parameter sums this launch reduces
+  const double* dL; long ldd;
   double* partials;                                            // [col tiles][row tiles][part_nred]
+  MultiKern mk;
+};
+
+// gradients_X of the composite (add.py:88-100, prod.py:397-407) w.r.t. the row points, over its stationary parts (kinds
+// RBF .. Matern52; White / Bias enter as factors only): element (row n, col m) of dL_dK at dL[n * ldd + m], or at
+// dL[m * ldd + n] when `transposed`. same: the columns are the rows (dL + dL^T, stationary.py:334-336). Output: nrows x Dfull row-major, the parts' sums added per data column in
+// part order.
+struct GradXMultiParams {
+  const double* rowsT; long ld_rows; const double* sq_rows; long nrows;
+  const double* colsT; long ld_cols; const double* sq_cols; long ncols;
+  const double* dL; long ldd; int transposed; int same;
+  int Dfull;
   MultiKern mk;
 };
 
@@ -102,6 +115,8 @@ int launch_prep_multi(const double* X, long N, int Dfull, long ld, const MultiKe
 int launch_kbuild_multi(const KBuildMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st);
 int launch_grad_kinv_multi(const GradKinvMultiParams& p, cudaStream_t st);
 int launch_grad_full_multi(const GradFullMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st);
+// two launches: chunk partials [nchunk][nrows][sumD] into part, then their fixed-order sum into out (device, nrows x Dfull)
+int launch_gradx_multi(const GradXMultiParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st);
 int launch_finalize_multi(const FinalizeMultiParams& f, cudaStream_t st);
 // entry t of part p's reduced sums -> entry t of its gradient block: the stationary lengthscale rule -tot/l
 // (stationary.py:210,213) for RBF .. Matern52 and RatQuad; RatQuad's power and StdPeriodic's sums are the gradient as they

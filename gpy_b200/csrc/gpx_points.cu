@@ -58,38 +58,56 @@ GradFullParams grad_params(Kern k, const Points& rows, const Points& cols, const
   return gp;
 }
 
-// partial sums per tile of the update_gradients_full reduction: a single kernel's variance and lengthscale(s); a part's
+// partial sums per tile of the update_gradients_full reduction: a single kernel's variance and lengthscale(s); part p's
 // gradient entries and tr(dL_dK)
-static int grad_full_nred(Kern k) { return k.kp ? (k.kp->ard ? k.kp->D : 1) + 1 : part_nred(k.mk->part[0]); }
+static int grad_full_nred(Kern k, int p = 0) { return k.kp ? (k.kp->ard ? k.kp->D : 1) + 1 : part_nred(k.mk->part[p]); }
 
 size_t grad_full_doubles(Kern k, const GradFullParams& gp) {
-  return (size_t)(gp.ld1 / TILE) * (gp.ld2 / TILE) * grad_full_nred(k);
+  int nred = 0;
+  for (int p = 0; p < (k.kp ? 1 : k.mk->nparts); p++) nred += grad_full_nred(k, p);
+  return (size_t)(gp.ld1 / TILE) * (gp.ld2 / TILE) * nred;
 }
 
 int grad_full_sum(gpx_ctx* c, Kern k, GradFullParams gp, double* part, double* grad) {
-  const int nred = grad_full_nred(k), tiles_j = (int)(gp.ld2 / TILE), tiles_i = (int)(gp.ld1 / TILE);
+  const int tiles_j = (int)(gp.ld2 / TILE), tiles_i = (int)(gp.ld1 / TILE), nparts = k.kp ? 1 : k.mk->nparts;
+  const size_t ntile = (size_t)tiles_j * tiles_i;
   if (k.kp) {
     gp.partials = part;
     GPX_CHECK(launch_grad_full(gp, tiles_j, tiles_i, c->st));
+    c->total_launches++;
   } else {   // the composite reduction maps the column points to threads: rows and columns trade places
     GradFullMultiParams gf;
     memset(&gf, 0, sizeof(gf));
     gf.rowsT = gp.x2T; gf.ld_rows = gp.ld2; gf.sq_rows = gp.sq2;
     gf.colsT = gp.x1T; gf.ld_cols = gp.ld1; gf.sq_cols = gp.sq1;
-    gf.nrows = gp.M; gf.ncols = gp.N; gf.same = gp.same; gf.dL = gp.dL_dK; gf.partials = part; gf.mk = *k.mk;
-    GPX_CHECK(launch_grad_full_multi(gf, tiles_j, tiles_i, c->st));
+    if (gp.cP) GPX_FAIL("internal: a composite's reduction takes a complete dL_dK (no rank-P term)");
+    gf.nrows = gp.M; gf.ncols = gp.N; gf.same = gp.same; gf.dL = gp.dL_dK; gf.ldd = gp.ldd > 0 ? gp.ldd : gp.M;
+    gf.mk = *k.mk;
+    size_t off = 0;
+    for (int p = 0; p < nparts; p++) {   // one launch per part, each into its own block of partials
+      gf.part = p; gf.partials = part + off;
+      GPX_CHECK(launch_grad_full_multi(gf, tiles_j, tiles_i, c->st));
+      c->total_launches++;
+      off += ntile * grad_full_nred(k, p);
+    }
   }
-  c->total_launches++;
   std::vector<double> hp(grad_full_doubles(k, gp));
   GPX_CUDA(cudaMemcpyAsync(hp.data(), part, hp.size() * 8, cudaMemcpyDeviceToHost, c->st));
   GPX_CUDA(cudaStreamSynchronize(c->st));
-  std::vector<double> tot(nred, 0.0);
-  for (size_t t = 0; t < hp.size() / nred; t++)
-    for (int q = 0; q < nred; q++) tot[q] += hp[t * nred + q];
-  double v;
-  for (int q = 0; q < nred; q++) {
-    if (k.kp) grad[q] = q ? -tot[q] / k.kp->ls[q - 1] : tot[0];   // stationary.py:210,213
-    else if (part_grad_entry(*k.mk, 0, q, tot[q], &v)) grad[q] = v;
+  size_t off = 0;
+  int g = 0;
+  for (int p = 0; p < nparts; p++) {
+    const int nred = grad_full_nred(k, p);
+    std::vector<double> tot(nred, 0.0);
+    for (size_t t = 0; t < ntile; t++)
+      for (int q = 0; q < nred; q++) tot[q] += hp[off + t * nred + q];
+    double v;
+    for (int q = 0; q < nred; q++) {
+      if (k.kp) grad[q] = q ? -tot[q] / k.kp->ls[q - 1] : tot[0];   // stationary.py:210,213
+      else if (part_grad_entry(*k.mk, p, q, tot[q], &v)) grad[g + q] = v;
+    }
+    if (!k.kp) g += part_ngrad(k.mk->part[p]);
+    off += ntile * nred;
   }
   return 0;
 }
@@ -102,21 +120,36 @@ static void gradx_chunks(const gpx_ctx* c, const GradFullParams& gp, int* nchunk
   *nchunk = (int)((gp.M + *mchunk - 1) / *mchunk);
 }
 
-size_t grad_X_doubles(const gpx_ctx* c, const GradFullParams& gp) {
+// doubles of one chunk's partials: a single kernel's D columns, a composite's stacked rows
+static int gradx_width(Kern k) { return k.kp ? k.kp->D : std::max(1, k.mk->sumD); }
+
+size_t grad_X_doubles(const gpx_ctx* c, Kern k, const GradFullParams& gp, int D) {
   int nchunk;
   long mchunk;
   gradx_chunks(c, gp, &nchunk, &mchunk);
-  return (size_t)(nchunk + 1) * gp.N * gp.kp.D;
+  return (size_t)nchunk * gp.N * gradx_width(k) + (size_t)gp.N * (k.kp ? k.kp->D : D);
 }
 
-int grad_X(gpx_ctx* c, const GradFullParams& gp, double* part, double* out) {
+int grad_X(gpx_ctx* c, Kern k, const GradFullParams& gp, int D, double* part, double* out) {
   int nchunk;
   long mchunk;
   gradx_chunks(c, gp, &nchunk, &mchunk);
-  double* dout = part + (size_t)nchunk * gp.N * gp.kp.D;
-  GPX_CHECK(launch_gradx(gp, nchunk, mchunk, part, dout, c->st));
+  double* dout = part + (size_t)nchunk * gp.N * gradx_width(k);
+  if (k.kp) {
+    D = k.kp->D;
+    GPX_CHECK(launch_gradx(gp, nchunk, mchunk, part, dout, c->st));
+  } else {
+    GradXMultiParams gx;
+    memset(&gx, 0, sizeof(gx));
+    gx.rowsT = gp.x1T; gx.ld_rows = gp.ld1; gx.sq_rows = gp.sq1; gx.nrows = gp.N;
+    gx.colsT = gp.x2T; gx.ld_cols = gp.ld2; gx.sq_cols = gp.sq2; gx.ncols = gp.M;
+    if (gp.cP) GPX_FAIL("internal: a composite's reduction takes a complete dL_dK (no rank-P term)");
+    gx.dL = gp.dL_dK; gx.ldd = gp.ldd > 0 ? gp.ldd : gp.M; gx.transposed = gp.transposed; gx.same = gp.same;
+    gx.Dfull = D; gx.mk = *k.mk;
+    GPX_CHECK(launch_gradx_multi(gx, nchunk, mchunk, part, dout, c->st));
+  }
   c->total_launches += 2;
-  GPX_CUDA(cudaMemcpyAsync(out, dout, (size_t)gp.N * gp.kp.D * 8, cudaMemcpyDeviceToHost, c->st));
+  GPX_CUDA(cudaMemcpyAsync(out, dout, (size_t)gp.N * D * 8, cudaMemcpyDeviceToHost, c->st));
   GPX_CUDA(cudaStreamSynchronize(c->st));
   return 0;
 }

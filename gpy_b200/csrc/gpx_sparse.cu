@@ -34,7 +34,12 @@ struct SparseState {
   double *dLt = nullptr;   // Mpad x Npad: dL_dKnm^T
   double *Gm = nullptr, *W2 = nullptr, *Cm = nullptr;   // Mpad x Mpad, Mpad x Mpad, [P][Mpad]
   double *part = nullptr; size_t part_cap = 0;
+  int rows_cap = 0, norm_cap = 0;          // stacked coordinate rows of XsT / ZsT, squared-norm rows of sqX / sqZ
+  // the kernel of the last evaluation: a single stationary kernel (kp) or a composite (mk), and its Kdiag (psi0 per point)
   KernParams kp{};
+  MultiKern mk{};
+  bool multi = false;
+  double kdiag = 0.0;
   // full-device evaluation (gpx_sparse_eval)
   gpx_ctx *cK = nullptr, *cB = nullptr;             // child contexts holding the factors of Kmm and of B = I + A
   double *mm[10] = {nullptr};                        // Mpad x Mpad work matrices
@@ -46,6 +51,7 @@ struct SparseState {
   double trYYT = 0.0;
   bool have_eval = false;
   double noise = 0.0;
+  Kern kern() const { return multi ? Kern(&mk) : Kern(&kp); }
   Points xpts() const { return Points{XsT, sqX, N, Npad}; }   // this rank's data points, prepared
   Points zpts() const { return Points{ZsT, sqZ, M, Mpad}; }   // the inducing points, prepared
 };
@@ -67,6 +73,7 @@ void free_all(SparseState* s) {
   if (s->cK) { gpx_destroy(s->cK); s->cK = nullptr; }
   if (s->cB) { gpx_destroy(s->cB); s->cB = nullptr; }
   s->part_cap = 0;
+  s->rows_cap = s->norm_cap = 0;
   s->N = s->Npad = 0;
 }
 int ensure_part(SparseState* s, size_t bytes) {
@@ -94,6 +101,18 @@ __global__ void ymul_kernel(const double* __restrict__ Y, const double* __restri
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= ld * P) return;
   out[i] = f[i % ld] * Y[i];
+}
+// composite route: dL_dKnm^T (a, n) += sum_q C[q][a] (beta Y)[q][n] over the valid entries, so that the composite
+// reductions read a complete dL_dKnm (the single-kernel ones add this rank-P term on the fly)
+__global__ void add_rank_p_kernel(double* __restrict__ dLt, long ld, long M, long N, const double* __restrict__ C,
+                                  const double* __restrict__ Yb, long ldy, int P) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ld * N) return;
+  const long a = i % ld, n = i / ld;
+  if (a >= M) return;
+  double v = dLt[i];
+  for (int q = 0; q < P; q++) v = fma(C[(long)q * ld + a], Yb[(long)q * ldy + n], v);
+  dLt[i] = v;
 }
 // out = a X + b Y + cdiag I + d sum_p u_p u_p^T   (n x n, leading dimension ld; X, Y, U may be null)
 __global__ void combine_kernel(double* __restrict__ out, long ld, long n, double a, const double* __restrict__ X, double b,
@@ -140,6 +159,23 @@ int launched(gpx_ctx* c, int n = 1) {
   GPX_CUDA(cudaGetLastError());
   return 0;
 }
+// XsT / ZsT hold rows_cap stacked coordinate rows and sqX / sqZ norm_cap rows: grown when kernel k needs more (a composite
+// stacks every part's active dims, which can exceed D when parts share columns, and keeps one norm row per part)
+int ensure_rows(gpx_ctx* c, SparseState* s, Kern k) {
+  const int rows = std::max(s->rows_cap, std::max(1, k.coord_rows())), norms = std::max(s->norm_cap, k.norm_rows());
+  if (rows == s->rows_cap && norms == s->norm_cap) return 0;
+  GPX_CUDA(cudaStreamSynchronize(c->st));
+  double** ptrs[] = {&s->XsT, &s->sqX, &s->ZsT, &s->sqZ};
+  for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
+  s->rows_cap = rows; s->norm_cap = norms;
+  GPX_CUDA(cudaMalloc(&s->XsT, (size_t)s->Npad * rows * 8));
+  GPX_CUDA(cudaMalloc(&s->sqX, (size_t)s->Npad * norms * 8));
+  if (s->Mpad) {
+    GPX_CUDA(cudaMalloc(&s->ZsT, (size_t)s->Mpad * rows * 8));
+    GPX_CUDA(cudaMalloc(&s->sqZ, (size_t)s->Mpad * norms * 8));
+  }
+  return 0;
+}
 }  // namespace
 
 namespace gpx {
@@ -167,6 +203,7 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
     GPX_CUDA(cudaMalloc(&s->X, (size_t)Npad * D * 8));
     GPX_CUDA(cudaMalloc(&s->XsT, (size_t)Npad * D * 8));
     GPX_CUDA(cudaMalloc(&s->sqX, (size_t)Npad * 8));
+    s->rows_cap = D; s->norm_cap = 1;
     GPX_CUDA(cudaMalloc(&s->Y, (size_t)Npad * P * 8));
     GPX_CUDA(cudaMalloc(&s->Yb, (size_t)Npad * P * 8));
   }
@@ -203,20 +240,20 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
 
 }  // extern "C"
 
-// psi1 = K(X, Z) in both layouts (Kuf: M x N, Kfu: N x M), left on the device
-static int psi_device(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* Z,
-                      int64_t M) {
+// psi1 = K(X, Z) of the state's kernel in both layouts (Kuf: M x N, Kfu: N x M), left on the device
+static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
-  GPX_CHECK(fill_kp(s->kp, kind, ard, s->D, variance, lengthscale));
+  const Kern k = s->kern();
+  GPX_CHECK(ensure_rows(c, s, k));
   const long Mpad = (M + TILE - 1) / TILE * TILE, Npad = s->Npad, N = s->N;
   if (Mpad != s->Mpad) {
     GPX_CUDA(cudaStreamSynchronize(st));
     free_m(s);
     s->Mpad = Mpad;
     GPX_CUDA(cudaMalloc(&s->Z, (size_t)Mpad * s->D * 8));
-    GPX_CUDA(cudaMalloc(&s->ZsT, (size_t)Mpad * s->D * 8));
-    GPX_CUDA(cudaMalloc(&s->sqZ, (size_t)Mpad * 8));
+    GPX_CUDA(cudaMalloc(&s->ZsT, (size_t)Mpad * s->rows_cap * 8));
+    GPX_CUDA(cudaMalloc(&s->sqZ, (size_t)Mpad * s->norm_cap * 8));
     GPX_CUDA(cudaMalloc(&s->Kuf, (size_t)Mpad * Npad * 8));
     GPX_CUDA(cudaMalloc(&s->Kfu, (size_t)Mpad * Npad * 8));
     GPX_CUDA(cudaMalloc(&s->dLt, (size_t)Mpad * Npad * 8));
@@ -235,11 +272,11 @@ static int psi_device(gpx_ctx* c, int kind, int ard, double variance, const doub
   }
   s->Nw = N; s->Mw = M;
   GPX_CUDA(cudaMemcpyAsync(s->Z, Z, (size_t)M * s->D * 8, cudaMemcpyHostToDevice, st));
-  GPX_CHECK(launch_prep_x(s->X, N, Npad, s->kp, s->XsT, s->sqX, st));
-  GPX_CHECK(launch_prep_x(s->Z, M, Mpad, s->kp, s->ZsT, s->sqZ, st));
+  GPX_CHECK(prep_points(c, k, s->X, N, s->D, Npad, s->XsT, s->sqX));
+  GPX_CHECK(prep_points(c, k, s->Z, M, s->D, Mpad, s->ZsT, s->sqZ));
   GPX_CHECK(launched(c, 2));
-  GPX_CHECK(build_K(c, &s->kp, s->zpts(), s->xpts(), s->Kuf, Mpad));   // psi1^T: thread-mapped operand = inducing points
-  GPX_CHECK(build_K(c, &s->kp, s->xpts(), s->zpts(), s->Kfu, Npad));   // psi1: thread-mapped operand = data points
+  GPX_CHECK(build_K(c, k, s->zpts(), s->xpts(), s->Kuf, Mpad));   // psi1^T: thread-mapped operand = inducing points
+  GPX_CHECK(build_K(c, k, s->xpts(), s->zpts(), s->Kfu, Npad));   // psi1: thread-mapped operand = data points
   return launched(c, 2);
 }
 
@@ -254,8 +291,9 @@ static int mul_psi1T(gpx_ctx* c, const double* A, double* C, int tri) {
   return launched(c);
 }
 
-// dL_dKnm^T = W2 psi1^T (+ rank-P term on the fly) reduced to kernel-parameter gradients and dL/dZ; W2 (device, s->W2)
-// and C (device, s->Cm as [P][Mpad]) must be in place. Results on the host.
+// dL_dKnm^T = W2 psi1^T (+ rank-P term: on the fly for a single kernel, added in one pass for a composite) reduced to
+// kernel-parameter gradients and dL/dZ; W2 (device, s->W2) and C (device, s->Cm as [P][Mpad]) must be in place. Results on
+// the host.
 // bvec (device, [Npad], per-point precisions) selects the heteroscedastic form: VVT_factor = beta_n Y_n and the columns of
 // W2 psi1^T scaled by beta_n (var_dtc.py:226); W2 is then 2 dL_dpsi2_beta without the scalar beta.
 static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double* grad, double* dZ) {
@@ -274,15 +312,21 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
     GPX_CHECK(launched(c));
   }
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
-  GradFullParams gp = grad_params(&s->kp, s->xpts(), s->zpts(), s->dLt, Mpad);
-  gp.ci = s->Yb; gp.ldci = Npad; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = P;
-  GPX_CHECK(ensure_part(s, grad_full_doubles(&s->kp, gp) * 8));
-  GPX_CHECK(grad_full_sum(c, &s->kp, gp, s->part, grad));
+  const Kern k = s->kern();
+  if (s->multi) {
+    add_rank_p_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(s->dLt, Mpad, s->M, N, s->Cm, s->Yb, Npad, P);
+    GPX_CHECK(launched(c));
+  }
+  const int cP = s->multi ? 0 : P;
+  GradFullParams gp = grad_params(k, s->xpts(), s->zpts(), s->dLt, Mpad);
+  gp.ci = s->Yb; gp.ldci = Npad; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = cP;
+  GPX_CHECK(ensure_part(s, grad_full_doubles(k, gp) * 8));
+  GPX_CHECK(grad_full_sum(c, k, gp, s->part, grad));
   // dL/dZ: gradients_X(dL_dKnm^T, Z, X): rows = inducing points, columns = data points, dL read transposed
-  GradFullParams gx = grad_params(&s->kp, s->zpts(), s->xpts(), s->dLt, Mpad);
-  gx.transposed = 1; gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = s->Yb; gx.ldcj = Npad; gx.cP = P;
-  GPX_CHECK(ensure_part(s, grad_X_doubles(c, gx) * 8));
-  return grad_X(c, gx, s->part, dZ);
+  GradFullParams gx = grad_params(k, s->zpts(), s->xpts(), s->dLt, Mpad);
+  gx.transposed = 1; gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = s->Yb; gx.ldcj = Npad; gx.cP = cP;
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, k, gx, s->D) * 8));
+  return grad_X(c, k, gx, s->D, s->part, dZ);
 }
 
 // =================================================================================================================
@@ -324,7 +368,7 @@ static int binv(gpx_ctx* c, const double* UB, double* out) {
 static int build_Kmm(gpx_ctx* c, double* Kd) {
   SparseState* s = c->sparse;
   GPX_CUDA(cudaMemsetAsync(Kd, 0, (size_t)s->Mpad * s->Mpad * 8, c->st));
-  GPX_CHECK(build_K(c, &s->kp, s->zpts(), s->zpts(), Kd, s->Mpad));
+  GPX_CHECK(build_K(c, s->kern(), s->zpts(), s->zpts(), Kd, s->Mpad));
   return launched(c);
 }
 // factor-and-invert the M x M matrix A (written on c's stream) on the child context ch, then U (clean upper) and
@@ -345,20 +389,53 @@ static int factor_child(gpx_ctx* c, gpx_ctx* ch, const double* A, double jitter,
   return 0;
 }
 
-// noise_vec == nullptr: scalar noise variance `noise` (grad = [variance, lengthscale.., noise variance]);
-// noise_vec (host, one variance per row held by this rank): grad = [variance, lengthscale..], dL_dR (host, N x P row-major)
-static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* Z,
-                            int64_t M, double noise, const double* noise_vec, double* lml, double* grad, double* dZ,
-                            double* dL_dR_out) {
+// the checks every sparse entry makes before it reads its kernel (`kern`: the lengthscale or the parts, read against the
+// data's D; het: per-point noise, dL_dR required)
+static int sparse_args(const gpx_ctx* c, const void* kern, const double* Z, int64_t M, const double* lml, const double* grad,
+                       const double* dZ, bool het, const double* dL_dR) {
   if (!c || !c->sparse || !c->sparse->X) GPX_FAIL("gpx_sparse_set_data has not been called");
-  if (!Z || !lml || !grad || !dZ || !lengthscale) GPX_FAIL("null argument");
+  if (!Z || !lml || !grad || !dZ || !kern) GPX_FAIL("null argument");
   if (M < 1) GPX_FAIL("M must be positive");
+  if (het && !dL_dR) GPX_FAIL("null argument");
+  return 0;
+}
+
+// the kernel's gradient block: sum(dL_dKdiag) = ddiag through update_gradients_diag (sparse_gp.py:110), plus the Knm and
+// Kmm reductions (:112-115). A composite's parts see ddiag times the product of the other variances of their term
+// (prod.py:386-394, Kdiag = variance for every leaf kind); only the variance entry of a block depends on Kdiag.
+static void kern_grads(const SparseState* s, double ddiag, const std::vector<double>& g_knm, const std::vector<double>& g_kmm,
+                       double* grad) {
+  if (!s->multi) {
+    grad[0] = ddiag + g_knm[0] + g_kmm[0];
+    for (size_t q = 1; q < g_knm.size(); q++) grad[q] = g_knm[q] + g_kmm[q];
+    return;
+  }
+  const MultiKern& mk = s->mk;
+  int g = 0;
+  for (int p = 0; p < mk.nparts; p++) {
+    double other = 1.0;
+    for (int q = 0; q < mk.nparts; q++)
+      if (q != p && mk.part[q].term == mk.part[p].term) other *= mk.part[q].variance;
+    const int n = part_ngrad(mk.part[p]);
+    for (int t = 0; t < n; t++) grad[g + t] = (t == 0 ? ddiag * other : 0.0) + g_knm[g + t] + g_kmm[g + t];
+    g += n;
+  }
+}
+
+// One evaluation of the validated kernel k (Kdiag = kdiag, psi0 of every data point), which becomes the state's kernel.
+// noise_vec == nullptr: scalar noise variance `noise` (grad = [k's gradient block, noise variance]);
+// noise_vec (host, one variance per row held by this rank): grad = [k's gradient block], dL_dR (host, N x P row-major).
+// k's block: a single kernel's [variance, lengthscale..]; a composite's part blocks in order (part_ngrad entries each).
+static int sparse_eval_impl(gpx_ctx* c, Kern k, double kdiag, const double* Z, int64_t M, double noise,
+                            const double* noise_vec, double* lml, double* grad, double* dZ, double* dL_dR_out) {
   const bool het = noise_vec != nullptr;
-  if (het && !dL_dR_out) GPX_FAIL("null argument");
   GPX_CUDA(cudaSetDevice(c->device));
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
   s->have_eval = false;
+  s->multi = k.mk != nullptr;
+  if (s->multi) s->mk = *k.mk; else s->kp = *k.kp;
+  s->kdiag = kdiag;
   memset(&c->stats, 0, sizeof(c->stats));   // filled below: Kmm's attempts, the trailing updates of both factorisations
   // per-point precisions beta_n = 1 / max(variance_n, const_jitter) (var_dtc.py:79-84) and the sums over n the bound needs
   std::vector<double> hbeta, hsb;
@@ -380,10 +457,17 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     GPX_CUDA(cudaMemcpyAsync(s->hb + Npd, hbeta.data(), (size_t)Npd * 8, cudaMemcpyHostToDevice, st));
     GPX_CUDA(cudaStreamSynchronize(st));   // the host vectors are pageable
   }
-  GPX_CHECK(psi_device(c, kind, ard, variance, lengthscale, Z, M));
+  GPX_CHECK(psi_device(c, Z, M));
   const long Mpad = s->Mpad, N = s->Ntot, Npad = s->Npad;
   const int D = s->D, P = s->P, mt = (int)(Mpad / TILE);
+  // entries of the kernel's gradient block (a single kernel: variance and nl lengthscales; the row-shard all-reduce below
+  // is single-kernel only)
   const int nl = s->kp.ard ? D : 1;
+  int ngk = 1 + nl;
+  if (s->multi) {
+    ngk = 0;
+    for (int p = 0; p < s->mk.nparts; p++) ngk += part_ngrad(s->mk.part[p]);
+  }
   constexpr int RSPLIT = 64;
   if (!s->mm[0]) {
     for (auto& p : s->mm) GPX_CUDA(cudaMalloc(&p, (size_t)Mpad * Mpad * 8));
@@ -492,7 +576,7 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   GPX_CHECK(combine(c, s->W2, Mpad, beta, E, 0.0, nullptr, 0.0));
   // Knm part: needs C in s->Cm
   GPX_CUDA(cudaMemcpyAsync(s->Cm, Cv, (size_t)P * Mpad * 8, cudaMemcpyDeviceToDevice, st));
-  std::vector<double> g_knm(1 + nl, 0.0);
+  std::vector<double> g_knm(ngk, 0.0);
   GPX_CHECK(knm_grads_device(c, beta, bvec, g_knm.data(), dZ));                         // dZ <- Knm part
   {
     int rank = 0, G = 1;
@@ -510,12 +594,12 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     }
   }
   // Kmm part: kern.update_gradients_full(dL_dKmm, Z) and kern.gradients_X(dL_dKmm, Z)  (sparse_gp.py:114,117)
-  const GradFullParams gk = grad_params(&s->kp, s->zpts(), s->zpts(), Kd, Mpad);
-  std::vector<double> g_kmm(1 + nl, 0.0), hz((size_t)M * D);
-  GPX_CHECK(ensure_part(s, grad_full_doubles(&s->kp, gk) * 8));
-  GPX_CHECK(grad_full_sum(c, &s->kp, gk, s->part, g_kmm.data()));
-  GPX_CHECK(ensure_part(s, grad_X_doubles(c, gk) * 8));
-  GPX_CHECK(grad_X(c, gk, s->part, hz.data()));
+  const GradFullParams gk = grad_params(s->kern(), s->zpts(), s->zpts(), Kd, Mpad);
+  std::vector<double> g_kmm(ngk, 0.0), hz((size_t)M * D);
+  GPX_CHECK(ensure_part(s, grad_full_doubles(s->kern(), gk) * 8));
+  GPX_CHECK(grad_full_sum(c, s->kern(), gk, s->part, g_kmm.data()));
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, s->kern(), gk, D) * 8));
+  GPX_CHECK(grad_X(c, s->kern(), gk, D, s->part, hz.data()));
   for (size_t i = 0; i < hz.size(); i++) dZ[i] += hz[i];
   // ---- scalars on the host (var_dtc.py:237-276, homoscedastic) -----------------------------------------------------
   double trAr = 0.0, sumAD = 0.0, data_fit = 0.0;
@@ -523,6 +607,7 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   for (int q = 0; q < P; q++)
     for (long i = 0; i < M; i++) data_fit += hv[(size_t)q * Mpad + i] * hv[(size_t)q * Mpad + i];
   const double trA = beta * trAr, sumADB = beta * sumAD;
+  const double variance = s->kdiag;                                                           // psi0 per point
   const double psi0_sum = variance * (double)N;
   const double nd = (double)N, od = (double)P;
   const double log2pi = 1.8378770664093453;
@@ -559,8 +644,7 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
     const double lik_1h = -0.5 * nd * od * log2pi + 0.5 * od * sums[0] - 0.5 * sums[2];
     const double lik_2h = -0.5 * od * (variance * sums[1] - trA);
     *lml = lik_1h + lik_2h + lik_3 + lik_4;
-    grad[0] = -0.5 * od * sums[1] + g_knm[0] + g_kmm[0];                                   // update_gradients_diag (:110)
-    for (int q = 0; q < nl; q++) grad[1 + q] = g_knm[1 + q] + g_kmm[1 + q];
+    kern_grads(s, -0.5 * od * sums[1], g_knm, g_kmm, grad);                                 // update_gradients_diag (:110)
     s->have_eval = true;
     return 0;
   }
@@ -573,9 +657,8 @@ static int sparse_eval_impl(gpx_ctx* c, int kind, int ard, double variance, cons
   // d beta / d noise is folded by the reference into dL_dR (gradient wrt the noise VARIANCE): exact_inference_gradients
   // sums dL_dR as is (var_dtc.py:176, gaussian.py:78-79)
   const double dvar_diag = -0.5 * od * beta * nd;                                          // update_gradients_diag (:110)
-  grad[0] = dvar_diag + g_knm[0] + g_kmm[0];
-  for (int q = 0; q < nl; q++) grad[1 + q] = g_knm[1 + q] + g_kmm[1 + q];
-  grad[1 + nl] = dL_dR;
+  kern_grads(s, dvar_diag, g_knm, g_kmm, grad);
+  grad[ngk] = dL_dR;
   s->have_eval = true;
   return 0;
 }
@@ -584,13 +667,34 @@ extern "C" {
 
 int gpx_sparse_eval(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* Z, int64_t M,
                     double noise, double* lml, double* grad, double* dZ) {
-  return sparse_eval_impl(c, kind, ard, variance, lengthscale, Z, M, noise, nullptr, lml, grad, dZ, nullptr);
+  GPX_CHECK(sparse_args(c, lengthscale, Z, M, lml, grad, dZ, false, nullptr));
+  KernParams kp{};
+  GPX_CHECK(fill_kp(kp, kind, ard, c->sparse->D, variance, lengthscale));
+  return sparse_eval_impl(c, &kp, variance, Z, M, noise, nullptr, lml, grad, dZ, nullptr);
 }
 
 int gpx_sparse_eval_het(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* Z,
                         int64_t M, const double* noise_variances, double* lml, double* grad, double* dZ, double* dL_dR) {
   if (!noise_variances) GPX_FAIL("null argument");
-  return sparse_eval_impl(c, kind, ard, variance, lengthscale, Z, M, 0.0, noise_variances, lml, grad, dZ, dL_dR);
+  GPX_CHECK(sparse_args(c, lengthscale, Z, M, lml, grad, dZ, true, dL_dR));
+  KernParams kp{};
+  GPX_CHECK(fill_kp(kp, kind, ard, c->sparse->D, variance, lengthscale));
+  return sparse_eval_impl(c, &kp, variance, Z, M, 0.0, noise_variances, lml, grad, dZ, dL_dR);
+}
+
+int gpx_sparse_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
+                          double noise_variance, const double* noise_variances, double* lml, double* grad, double* dZ,
+                          double* dL_dR) {
+  const bool het = noise_variances != nullptr;
+  GPX_CHECK(sparse_args(c, parts, Z, M, lml, grad, dZ, het, dL_dR));
+  if (c->dist) GPX_FAIL("composite kernels are single-GPU");
+  MultiKern mk;
+  double kdiag;
+  GPX_CHECK(fill_mk(mk, parts, nparts, c->sparse->D, &kdiag));
+  for (int p = 0; p < mk.nparts; p++)   // dL/dZ needs every part's gradients_X
+    if (mk.part[p].kind == GPX_RATQUAD || mk.part[p].kind == GPX_STDPERIODIC)
+      GPX_FAIL("RatQuad and StdPeriodic parts are not on the sparse evaluation (no device gradients_X)");
+  return sparse_eval_impl(c, &mk, kdiag, Z, M, het ? 0.0 : noise_variance, noise_variances, lml, grad, dZ, dL_dR);
 }
 
 /* which: 0 woodbury_vector (M x P row-major), 1 woodbury_inv (M x M), 2 Kmm (+1e-8 I), 3 Lm (lower, col-major) */

@@ -16,10 +16,11 @@ The sparse model is a drop-in the same way — the reference's own `GPy.core.Spa
 
     m = GPy.core.SparseGP(X, Y, Z, B.RBF(D, ARD=True), GPy.likelihoods.Gaussian(), inference_method=B.VarDTC())
 
-`B.VarDTC.inference` makes ONE `gpx_sparse_eval` (or `gpx_sparse_eval_het`) and returns a grad_dict whose `dL_dKnm` /
-`dL_dKmm` are handles carrying the gradients the device already reduced; `SparseGP._update_gradients`
-(core/sparse_gp.py:108-119) then calls the plugin kernel's `update_gradients_diag / update_gradients_full / gradients_X`
-exactly as written there and gets those numbers back (the N x M matrix dL_dKnm never exists).
+`B.VarDTC.inference` makes ONE `gpx_sparse_eval` (or `gpx_sparse_eval_het`; `gpx_sparse_eval_multi` for a `B.Add` /
+`B.Prod` over plugin stationary leaves and GPy's own White / Bias) and returns a grad_dict whose `dL_dKnm` / `dL_dKmm` are
+handles carrying the gradients the device already reduced; `SparseGP._update_gradients` (core/sparse_gp.py:108-119) then
+calls the kernel's `update_gradients_diag / update_gradients_full / gradients_X` exactly as written there and gets those
+numbers back (the N x M matrix dL_dKnm never exists).
 
 The methods `K`, `Kdiag`, `update_gradients_full`, `update_gradients_diag`, `gradients_X` are defined in the class bodies on purpose:
 `KernCallsViaSlicerMeta` only wraps names it finds in the class dict (GPy/kern/src/kernel_slice_operations.py:14-57), and
@@ -42,11 +43,13 @@ class SparseDeviceGradient(object):
     (var_dtc.py:178-188). The device evaluation has already reduced both to d/d(variance, lengthscale) and dL/dZ
     (core/sparse_gp.py:110-118); the handle carries its share, keyed by the kernel state and the inducing inputs they were
     computed for. `.T` is the same handle (SparseGP passes `dL_dKnm.T` to `gradients_X`, :118). It cannot turn into an
-    ndarray: the N x M matrix is never formed."""
+    ndarray: the N x M matrix is never formed. A composite kernel's handle carries one gradient block per flattened leaf
+    (`part_grads`) instead of dvariance / dlengthscale."""
 
-    def __init__(self, key, role, shape, dvariance, dlengthscale, dZ):
+    def __init__(self, key, role, shape, dvariance, dlengthscale, dZ, part_grads=None):
         self._key, self.role, self.shape = key, role, shape
         self.dvariance, self.dlengthscale, self.dZ = dvariance, dlengthscale, dZ
+        self.part_grads = part_grads
         self.ndim, self.dtype = 2, np.dtype(np.float64)
 
     def matches(self, key):
@@ -54,7 +57,8 @@ class SparseDeviceGradient(object):
 
     @property
     def T(self):
-        h = SparseDeviceGradient(self._key, self.role, self.shape[::-1], self.dvariance, self.dlengthscale, self.dZ)
+        h = SparseDeviceGradient(self._key, self.role, self.shape[::-1], self.dvariance, self.dlengthscale, self.dZ,
+                                 self.part_grads)
         return h
 
     def __array__(self, dtype=None, copy=None):
@@ -187,24 +191,47 @@ def _leaf_ngrad(leaf):
     return 1 + (np.asarray(leaf.lengthscale).size if hasattr(leaf, "lengthscale") else 0)
 
 
+def _set_leaf_gradients(kern, part_grads):
+    """every flattened leaf of kern gets its block of a composite device evaluation"""
+    for (leaf, _), g in zip(_flatten(kern), part_grads):
+        if hasattr(leaf, "_gpx_part_kind"):
+            _set_part_gradients(leaf, g)
+            continue
+        leaf.variance.gradient = g[0]
+        if hasattr(leaf, "lengthscale"):
+            leaf.lengthscale.gradient = g[1:] if leaf.ARD else g[1]
+
+
+def _check_sparse_handle(kern, h):
+    if h.part_grads is None or not h.matches(_composite_key(kern)):
+        raise ValueError("stale gradient handle: the kernel parameters changed since the sparse evaluation")
+
+
 def _make_combination(base, is_prod):
-    """Add / Prod over GPy's own class: K, Kdiag, gradients_X ... stay the reference's; update_gradients_full recognises the
-    handle of a fused composite evaluation and hands every leaf the gradient the device already reduced for it (the stock
-    methods would build every factor's N x N matrix on the host: add.py:76-77, prod.py:377-385)."""
+    """Add / Prod over GPy's own class: K, Kdiag ... stay the reference's; update_gradients_full recognises the handle of
+    a fused composite evaluation and hands every leaf the gradient the device already reduced for it (the stock methods
+    would build every factor's N x N matrix on the host: add.py:76-77, prod.py:377-385). The handles of the device VarDTC
+    are recognised by update_gradients_full and gradients_X (core/sparse_gp.py:112-118): the stock Prod.gradients_X would
+    multiply a handle by an ndarray (prod.py:397-407), the stock Add.gradients_X would count dZ once per leaf
+    (add.py:88-100)."""
 
     class B200Combination(base):
         def update_gradients_full(self, dL_dK, X, X2=None):
+            if isinstance(dL_dK, SparseDeviceGradient):
+                _check_sparse_handle(self, dL_dK)
+                _set_leaf_gradients(self, dL_dK.part_grads)
+                return
             if isinstance(dL_dK, DeviceGradient) and X2 is None and dL_dK.part_grads is not None \
                     and dL_dK.matches(_composite_key(self)):
-                for (leaf, _), g in zip(_flatten(self), dL_dK.part_grads):
-                    if hasattr(leaf, "_gpx_part_kind"):
-                        _set_part_gradients(leaf, g)
-                        continue
-                    leaf.variance.gradient = g[0]
-                    if hasattr(leaf, "lengthscale"):
-                        leaf.lengthscale.gradient = g[1:] if leaf.ARD else g[1]
+                _set_leaf_gradients(self, dL_dK.part_grads)
                 return
             return super(B200Combination, self).update_gradients_full(np.asarray(dL_dK, dtype=np.float64), X, X2)
+
+        def gradients_X(self, dL_dK, X, X2=None):
+            if isinstance(dL_dK, SparseDeviceGradient):
+                _check_sparse_handle(self, dL_dK)
+                return dL_dK.dZ
+            return super(B200Combination, self).gradients_X(dL_dK, X, X2)
 
     B200Combination.__name__ = B200Combination.__qualname__ = base.__name__
     B200Combination._gpx_is_prod = is_prod
@@ -257,8 +284,9 @@ def _make_vardtc(base, kernel_types, ffi):
 
     class B200VarDTC(base):
         """GPy.inference.latent_function_inference.VarDTC with the whole evaluation on the device (gpx_sparse_eval /
-        gpx_sparse_eval_het). Certain inputs, Gaussian / HeteroscedasticGaussian noise, a plugin stationary kernel, no mean
-        function; anything else goes to the stock method (var_dtc.py:66-215)."""
+        gpx_sparse_eval_het; gpx_sparse_eval_multi for a B.Add / B.Prod over plugin stationary leaves and GPy's own White /
+        Bias). Certain inputs, Gaussian / HeteroscedasticGaussian noise, no mean function; anything else goes to the stock
+        method (var_dtc.py:66-215)."""
 
         def __init__(self, limit=1, device=0, engine=None):
             super(B200VarDTC, self).__init__(limit)
@@ -285,8 +313,12 @@ def _make_vardtc(base, kernel_types, ffi):
         def inference(self, kern, X, Z, likelihood, Y, Y_metadata=None, mean_function=None, precision=None, Lm=None,
                       dL_dKmm=None, psi0=None, psi1=None, psi2=None, Z_tilde=None):
             plain_X = isinstance(X, np.ndarray)                    # a VariationalPosterior is not an ndarray subclass
-            if (not isinstance(kern, kernel_types) or not plain_X or mean_function is not None or Lm is not None
-                    or dL_dKmm is not None or psi0 is not None or psi1 is not None or psi2 is not None):
+            leaves = _flatten(kern) if hasattr(kern, "_gpx_is_prod") else None
+            if leaves is not None and any(not (hasattr(l, "_gpx_kind") or type(l).__name__ in ("White", "Bias"))
+                                          for l, _ in leaves):
+                leaves = None                                      # RatQuad / StdPeriodic: no device gradients_X
+            if ((leaves is None and not isinstance(kern, kernel_types)) or not plain_X or mean_function is not None
+                    or Lm is not None or dL_dKmm is not None or psi0 is not None or psi1 is not None or psi2 is not None):
                 return super(B200VarDTC, self).inference(kern, X, Z, likelihood, Y, Y_metadata, mean_function, precision,
                                                          Lm, dL_dKmm, psi0, psi1, psi2, Z_tilde)
             if precision is None:                                  # var_dtc.py:78-80
@@ -302,6 +334,8 @@ def _make_vardtc(base, kernel_types, ffi):
             if not self._data_key.matches(Xs, Yc):
                 eng.sparse_set_data(Xs, Yc)
                 self._data_key.remember(Xs, Yc)
+            if leaves is not None:
+                return self._inference_multi(eng, kern, leaves, Zs, likelihood, variance, N, P, M, Y_metadata, Z_tilde)
             k, ard, var, ls = kern._gpx_theta()
             if variance.size > 1:                                  # het_noise (var_dtc.py:82-84)
                 lml, grad, dZ, dR = eng.sparse_eval_het(k, ard, var, ls, Zs, variance)
@@ -323,6 +357,42 @@ def _make_vardtc(base, kernel_types, ffi):
             post = LazySparsePosterior(eng)
             return post, lml, {"dL_dKmm": kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": knm, "dL_dthetaL": dL_dthetaL,
                                "dL_dm": None}
+
+        def _inference_multi(self, eng, kern, leaves, Zs, likelihood, variance, N, P, M, Y_metadata, Z_tilde):
+            """a sum / product kernel: ONE gpx_sparse_eval_multi. GPy's stock update_gradients_diag runs first
+            (sparse_gp.py:110) and gives each leaf sum(dL_dKdiag) times the other variances of its term (add.py:79-80,
+            prod.py:386-394); the dL_dKnm handle carries each leaf's total minus that share, the dL_dKmm handle zeros."""
+            het = variance.size > 1
+            out = eng.sparse_eval_multi([_leaf_descriptor(l, t) for (l, t) in leaves], Zs,
+                                        variance if het else float(variance[0]))
+            lml, grad, dZ = out[:3]
+            if het:
+                beta = 1.0 / np.fmax(variance, self.const_jitter)
+                dL_dthetaL = likelihood.exact_inference_gradients(out[3], Y_metadata)     # var_dtc.py:176
+            else:
+                beta = np.full(N, 1.0 / max(float(variance[0]), self.const_jitter))
+                dL_dthetaL = likelihood.exact_inference_gradients(np.atleast_1d(grad[-1]), Y_metadata)
+            if Z_tilde is not None:
+                lml += Z_tilde                                     # var_dtc.py:166-170
+            dL_dKdiag = -0.5 * P * beta                            # _compute_dL_dpsi: dL_dpsi0 (:218)
+            diag = dL_dKdiag.sum()
+            knm, zeros, i = [], [], 0
+            for j, (leaf, t) in enumerate(leaves):
+                n = _leaf_ngrad(leaf)
+                g = np.array(grad[i:i + n], dtype=np.float64)
+                other = 1.0
+                for q, (l2, t2) in enumerate(leaves):
+                    if q != j and t2 == t:
+                        other *= float(np.asarray(l2.variance).reshape(-1)[0])
+                g[0] -= diag * other
+                knm.append(g)
+                zeros.append(np.zeros(n))
+                i += n
+            key = _composite_key(kern)
+            h_knm = SparseDeviceGradient(key, "knm", (N, M), None, None, dZ, part_grads=knm)
+            h_kmm = SparseDeviceGradient(key, "kmm", (M, M), None, None, np.zeros_like(dZ), part_grads=zeros)
+            return LazySparsePosterior(eng), lml, {"dL_dKmm": h_kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": h_knm,
+                                                   "dL_dthetaL": dL_dthetaL, "dL_dm": None}
 
     B200VarDTC.__name__ = B200VarDTC.__qualname__ = "VarDTC"
     return B200VarDTC

@@ -425,14 +425,19 @@ def scatter_part_gradients(kern, dL_dK):
     with a dense dL_dK); -> False if the handle does not belong to this kernel state"""
     if not (isinstance(dL_dK, DeviceGradient) and dL_dK.part_grads is not None and dL_dK.matches(composite_state_key(kern))):
         return False
-    for (leaf, _), g in zip(flatten_parts(kern), dL_dK.part_grads):
+    scatter_leaf_gradients(flatten_parts(kern), dL_dK.part_grads)
+    return True
+
+
+def scatter_leaf_gradients(leaves, part_grads):
+    """set each flattened leaf's gradient from its block of a composite device evaluation (paramz order)"""
+    for (leaf, _), g in zip(leaves, part_grads):
         if isinstance(leaf, _PartKern):
             leaf._set_gradients(g)
             continue
         leaf.variance.gradient = np.atleast_1d(g[0])
         if isinstance(leaf, Stationary):
             leaf.lengthscale.gradient = np.atleast_1d(g[1:]).copy()
-    return True
 
 
 

@@ -6,7 +6,8 @@ Mirrors:
     GPy.models.SparseGPRegression                              GPy/models/sparse_gp_regression.py:33-59
 (Gaussian likelihood, certain inputs, no mean function — BASELINE.json configs[4]; scalar noise through gpx_sparse_eval,
 one noise variance per data point — the `het_noise` branches var_dtc.py:127-128,221-227,241-257,267-269 with a
-HeteroscedasticGaussian likelihood — through gpx_sparse_eval_het.)
+HeteroscedasticGaussian likelihood — through gpx_sparse_eval_het. A sum of products of RBF .. Matern52, White and Bias
+leaves (kern.flatten_parts) goes through gpx_sparse_eval_multi, with either noise form.)
 
 ONE call, gpx_sparse_eval, does the whole evaluation on the device — psi1 = K(X, Z), tmp = Lm^-1 psi1^T, A = beta tmp
 tmp^T, the two M x M factor-and-invert sweeps (Kmm, B = I + A), every M x M product, dL_dKnm = (beta Y) C^T + 2 psi1
@@ -18,7 +19,8 @@ import numpy as np
 
 from . import _ffi
 from .inference import Gaussian, HeteroscedasticGaussian, _DataKey
-from .kern import RBF, RatQuad, StdPeriodic, Stationary
+from .kern import (RBF, RatQuad, StdPeriodic, Stationary, flatten_parts, part_descriptor, part_ngrad,
+                   scatter_leaf_gradients, single_kernel)
 from .param import Logexp, Param, Parameterized
 
 CONST_JITTER = 1e-8  # var_dtc.py:24
@@ -67,8 +69,9 @@ class LazySparsePosterior(object):
 
 class VarDTC(object):
     """Drop-in for GPy's VarDTC: inference(kern, X, Z, likelihood, Y) -> (posterior, log_marginal, grad_dict).
-    `grad_dict['dL_dKnm']` is never materialised (N x M); instead the dict carries the already-reduced contributions
-    `Knm_dvariance`, `Knm_dlengthscale`, `Knm_dZ`, which SparseGP._update_gradients adds (sparse_gp.py:112,118)."""
+    `grad_dict['dL_dKnm']` is never materialised (N x M); instead the dict carries the kernel's gradients already summed
+    over sparse_gp.py:110-115 (`dvariance` / `dlengthscale` for a single kernel, `part_grads`, one block per flattened
+    leaf, for a composite), `dZ` (:117-118) and `dL_dthetaL`."""
 
     const_jitter = CONST_JITTER
 
@@ -93,12 +96,18 @@ class VarDTC(object):
     def inference(self, kern, X, Z, likelihood, Y, Y_metadata=None, mean_function=None, precision=None):
         if mean_function is not None:
             raise NotImplementedError("sparse GP with a mean function is not on the accelerated path")
-        if isinstance(kern, (RatQuad, StdPeriodic)):
-            raise NotImplementedError("gpy_b200.VarDTC: %s is not on the device's sparse evaluation (RBF, Exponential, "
-                                      "Matern32, Matern52 are)" % type(kern).__name__)
-        if not isinstance(kern, Stationary):
-            raise TypeError("gpy_b200.VarDTC accelerates gpy_b200.kern stationary kernels")
+        leaves = None if single_kernel(kern) else flatten_parts(kern)
+        for k in ([kern] if leaves is None else [q for q, _ in leaves]):
+            if isinstance(k, (RatQuad, StdPeriodic)):
+                raise NotImplementedError("gpy_b200.VarDTC: %s is not on the device's sparse evaluation (RBF, Exponential, "
+                                          "Matern32, Matern52, White, Bias and their sums and products are)"
+                                          % type(k).__name__)
+        if leaves is None and not isinstance(kern, Stationary):
+            raise TypeError("gpy_b200.VarDTC accelerates gpy_b200.kern stationary kernels and sums / products of them "
+                            "with White and Bias")
         eng = self.engine
+        if leaves is not None:
+            return self._inference_multi(eng, kern, leaves, X, Z, likelihood, Y, Y_metadata, precision)
         Xs = kern._slice_X(X)
         Zs = kern._slice_X(Z)
         Y = np.ascontiguousarray(Y, dtype=np.float64)
@@ -134,9 +143,44 @@ class VarDTC(object):
                                   "dL_dthetaL": float(grad[-1]), "num_data": num_data}
 
 
+    def _inference_multi(self, eng, kern, leaves, X, Z, likelihood, Y, Y_metadata, precision):
+        """a composite kernel: one gpx_sparse_eval_multi; gradients returned per leaf (`part_grads`)"""
+        Xs = np.ascontiguousarray(X, dtype=np.float64)
+        Zs = np.ascontiguousarray(Z, dtype=np.float64)
+        Y = np.ascontiguousarray(Y, dtype=np.float64)
+        if not self._data_key.matches(Xs, Y):
+            eng.sparse_set_data(Xs, Y)
+            self._data_key.remember(Xs, Y)
+        num_data = Y.shape[0]
+        parts = [part_descriptor(k, t) for k, t in leaves]
+        if precision is None:
+            gv = np.asarray(likelihood.gaussian_variance(Y_metadata), dtype=np.float64)
+            noise = gv.reshape(-1) if gv.size > 1 else float(np.squeeze(gv))                 # het_noise: var_dtc.py:82-84
+        elif np.size(precision) > 1:
+            noise = 1.0 / np.asarray(precision, dtype=np.float64).reshape(-1)
+        else:
+            noise = 1.0 / float(precision)
+        het = np.ndim(noise) > 0
+        if het and noise.size != num_data:
+            raise ValueError("one noise variance per data point expected")
+        out = eng.sparse_eval_multi(parts, Zs, noise)
+        lml, grad, dZ = out[:3]
+        blocks, i = [], 0
+        for k, _ in leaves:
+            blocks.append(grad[i:i + part_ngrad(k)])
+            i += part_ngrad(k)
+        if het:
+            dL_dthetaL = likelihood.exact_inference_gradients(out[3], Y_metadata) if precision is None else out[3]
+        else:
+            dL_dthetaL = float(grad[-1])
+        return LazySparsePosterior(eng), float(lml), {"part_grads": blocks, "dZ": dZ, "dL_dthetaL": dL_dthetaL,
+                                                      "num_data": num_data}
+
+
 class SparseGPRegression(Parameterized):
     """GPy.models.SparseGPRegression (sparse_gp_regression.py:33-59) / GPy.core.SparseGP (sparse_gp.py:38-119).
-    Parameter (and gradient) order as in the reference: [inducing inputs, kern.variance, kern.lengthscale, noise]."""
+    Parameter (and gradient) order as in the reference: [inducing inputs, the kernel's parameters in link order (a single
+    kernel: variance, lengthscale), the likelihood's]."""
 
     def __init__(self, X, Y, kernel=None, Z=None, num_inducing=10, device=0, engine=None, name="sparse_gp", likelihood=None,
                  Y_metadata=None):
@@ -174,8 +218,11 @@ class SparseGPRegression(Parameterized):
             self.kern, self.X, Z, self.likelihood, self.Y, self.Y_metadata)
         self.grad_dict = gd
         self.likelihood.update_gradients(gd["dL_dthetaL"])                                     # :84
-        self.kern.variance.gradient = np.atleast_1d(gd["dvariance"])          # :110-114 summed on the device
-        self.kern.lengthscale.gradient = np.atleast_1d(gd["dlengthscale"])
+        if "part_grads" in gd:                                                 # :110-115 summed on the device, per leaf
+            scatter_leaf_gradients(flatten_parts(self.kern), gd["part_grads"])
+        else:
+            self.kern.variance.gradient = np.atleast_1d(gd["dvariance"])
+            self.kern.lengthscale.gradient = np.atleast_1d(gd["dlengthscale"])
         self.Z.gradient = gd["dZ"]                                             # :117-118
 
     def log_likelihood(self):
@@ -186,7 +233,7 @@ class SparseGPRegression(Parameterized):
 
     # ---- optimizer space: Z unconstrained, the positive parameters through Logexp ---------------------------------------
     def _flat(self):
-        return [self.Z, self.kern.variance, self.kern.lengthscale, self.likelihood.variance]
+        return self.flattened_parameters()      # Z, then the kernel's and the likelihood's parameters in link order
 
     @property
     def optimizer_array(self):

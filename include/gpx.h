@@ -191,6 +191,18 @@ int gpx_sparse_get(gpx_ctx* ctx, int which, double* out);
  * the posterior of this evaluation as well. */
 int gpx_sparse_eval_het(gpx_ctx* ctx, int kind, int ard, double variance, const double* lengthscale, const double* Z,
                         int64_t M, const double* noise_variances, double* lml, double* grad, double* dZ, double* dL_dR);
+/* The same evaluation with a COMPOSITE KERNEL: a sum of products of RBF, Exponential, Matern32, Matern52 (each on its own
+ * active dims), White and Bias parts, described as for gpx_exact_eval_multi and validated against the D of
+ * gpx_sparse_set_data. psi0 is the composite's Kdiag (the sum over terms of the product of the part variances); White is
+ * zero in psi1 and the trace of dL_dKmm in the Kmm gradient (static.py:77-93); dL/dZ is Add / Prod.gradients_X
+ * (add.py:88-100, prod.py:397-407). noise_variances == NULL: scalar noise, grad = every part's block in order (part_ngrad
+ * entries each) then d/d noise variance. noise_variances != NULL: N per-point variances as gpx_sparse_eval_het, grad = the
+ * part blocks only, dL_dR (N x P row-major) required. RatQuad / StdPeriodic parts are rejected (-2: they have no device
+ * gradients_X), and so is a context with a communicator attached (single-GPU). gpx_sparse_get serves this evaluation's
+ * posterior; its Kmm is rebuilt with the composite. */
+int gpx_sparse_eval_multi(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
+                          double noise_variance, const double* noise_variances, double* lml, double* grad, double* dZ,
+                          double* dL_dR);
 
 /* Measurement hooks (bench.py): device time of the last eval between CUDA events on the launching stream, the number
  * of kernels this library launched since creation, and per-phase accounting of the last eval. */
