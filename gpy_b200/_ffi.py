@@ -79,6 +79,8 @@ EXPORTS = {
                                             ctypes.c_int, _dp, _dp, _dp]),
     "gpx_get": (ctypes.c_int, [_vp, ctypes.c_int, _dp]),
     "gpx_predict": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
+    "gpx_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
+    "gpx_sparse_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
     "gpx_kern_K": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64, _dp,
                                   ctypes.c_int64, ctypes.c_int, _dp]),
     "gpx_kern_Kdiag": (ctypes.c_int, [ctypes.c_int, ctypes.c_double, ctypes.c_int64, _dp]),
@@ -188,6 +190,7 @@ class Engine(object):
         self._L = lib()
         check(self._L.gpx_create(int(device), ctypes.byref(self._h)), "gpx_create")
         self.N = self.D = self.P = 0
+        self.sN = self.sD = self.sP = self.sM = 0   # shape of the sparse data set and of Z (sparse_set_data, sparse_eval*)
         self.device = device
         self.eval_serial = 0      # bumped by every evaluation: lazy posterior views check it before fetching
 
@@ -274,6 +277,24 @@ class Engine(object):
         var = np.empty((M, M), order="F") if full_cov else np.empty(M)
         check(self._L.gpx_predict(self._h, _ptr(Xnew), M, int(full_cov), _ptr(mu), _ptr(var)), "gpx_predict")
         return mu, (var if full_cov else var[:, None])
+
+    def _pred_grads(self, fn, name, Xnew, D, P):
+        Xnew = _f64(Xnew)
+        if Xnew.ndim != 2 or (D and Xnew.shape[1] != D):   # D == 0: no data yet, the entry rejects the call (-2)
+            raise ValueError("Xnew must be M x %d" % D)
+        M = Xnew.shape[0]
+        dmu, dvar = np.empty((M, D, P)), np.empty((M, D))
+        check(fn(self._h, _ptr(Xnew), M, _ptr(dmu), _ptr(dvar)), name)
+        return dmu, dvar
+
+    def predictive_gradients(self, Xnew):
+        """GP.predictive_gradients (gp.py:418-474) with the last exact evaluation -> (dmu (M, D, P), dvar (M, D))"""
+        return self._pred_grads(self._L.gpx_predictive_gradients, "gpx_predictive_gradients", Xnew, self.D, self.P)
+
+    def sparse_predictive_gradients(self, Xnew):
+        """the same with the last sparse evaluation (predictive variable Z) -> (dmu (M, D, P), dvar (M, D))"""
+        return self._pred_grads(self._L.gpx_sparse_predictive_gradients, "gpx_sparse_predictive_gradients", Xnew,
+                                self.sD, self.sP)
 
     def kern_K_device_only(self, kind, ARD, variance, lengthscale, X, X2=None):
         """build K(X, X2) on the device without bringing it back; -> (kernel ms, algorithmic GB/s)."""

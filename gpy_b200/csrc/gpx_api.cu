@@ -1371,4 +1371,40 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// predictive gradients with the factor of the last evaluation (gp.py:438-474): V = Ky^-1 K(X, Xnew) = U (U^T Kx), MAX_P
+// test points per pass over U, then one fused Jacobian reduction; K^-1 is never formed
+// ---------------------------------------------------------------------------------------------------------------
+int gpx_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t M, double* dmu, double* dvar) {
+  if (!c || !Xnew || !dmu || !dvar) GPX_FAIL("null argument");
+  if (!c->have_eval) GPX_FAIL("no successful gpx_exact_eval to differentiate the prediction of");
+  if (M < 1) GPX_FAIL("empty Xnew");
+  if (c->dist) GPX_FAIL("predictive gradients are single-GPU");
+  const Kern k = ctx_kern(c);
+  GPX_CHECK(pred_grad_check(k));
+  GPX_CUDA(cudaSetDevice(c->device));
+  cudaStream_t st = c->st;
+  const long ld = c->Npad;
+  PointSet pn;
+  GPX_CHECK(upload_points(c, k, Xnew, M, c->D, pn));
+  // Kx as [M][ld] (as in gpx_predict); T = U^T Kx, then V = U T over Kx in place (a pass reads only its own columns)
+  double *Kx = nullptr, *Tx = nullptr, *uvp = nullptr;
+  GPX_TMP_ALLOC(&Kx, (size_t)pn.ld * ld * 8, st);
+  GPX_TMP_ALLOC(&Tx, (size_t)pn.ld * ld * 8, st);
+  GPX_TMP_ALLOC(&uvp, (size_t)KSPLIT * MAX_P * ld * 8, st);
+  int rc = 0;
+  if (cudaMemsetAsync(Kx, 0, (size_t)pn.ld * ld * 8, st) != cudaSuccess) { gpx::set_error("gpx_predictive_gradients: device failure"); rc = -1; }
+  if (rc == 0) rc = build_K(c, k, train_points(c), pn, Kx, ld);
+  c->total_launches++;
+  for (long m0 = 0; rc == 0 && m0 < M; m0 += MAX_P) {
+    const int pc = (int)std::min<long>(MAX_P, M - m0);
+    rc = launch_utv(c->S, ld, c->Npad, pc, Kx + m0 * ld, Tx + m0 * ld, st);
+    if (rc == 0) rc = launch_uv(c->S, ld, c->Npad, pc, Tx + m0 * ld, KSPLIT, uvp, Kx + m0 * ld, st);
+    c->total_launches += 3;
+  }
+  if (rc == 0) rc = pred_grad(c, k, pn, train_points(c), c->dAlpha, ld, c->P, Kx, ld, c->D, dmu, dvar);
+  GPX_TMP_FREE(Kx, st); GPX_TMP_FREE(Tx, st); GPX_TMP_FREE(uvp, st);
+  return rc;
+}
+
 }  // extern "C"

@@ -156,6 +156,13 @@ int grad_full_sum(gpx_ctx* c, Kern k, GradFullParams gp, double* part, double* g
 // have no device gradients_X (rc -2).
 size_t grad_X_doubles(const gpx_ctx* c, Kern k, const GradFullParams& gp, int D);
 int grad_X(gpx_ctx* c, Kern k, const GradFullParams& gp, int D, double* part, double* out);
+// predictive gradients (gp.py:438-474) of k at the prepared test points against `train`, for the woodbury vector alpha
+// ([P][lda], device) and V = woodbury_inv K(train, test) (V[n + m * ldv], device): dmu (n x D x P) and dvar (n x D), host,
+// row-major, D the columns of the host X. pred_grad_check: -2 for a kernel without a device input gradient (RatQuad /
+// StdPeriodic parts), before anything is launched.
+int pred_grad_check(Kern k);
+int pred_grad(gpx_ctx* c, Kern k, const Points& test, const Points& train, const double* alpha, long lda, int P,
+              const double* V, long ldv, int D, double* dmu, double* dvar);
 // the parts of a composite kernel -> mk (validated against Dfull columns of X), *kdiag_total = its Kdiag (gpx_api.cu)
 int fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Dfull, double* kdiag_total);
 }  // namespace gpx

@@ -593,6 +593,169 @@ int launch_gradx_multi(const GradXMultiParams& p, int nchunk, long mchunk, doubl
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// predictive gradients (GPy/core/gp.py:438-474): the Jacobians of the predictive mean and variance at the test points,
+// in gradx_multi_kernel's layout and with its per-pair rules. Row points (one per thread, 128 per CTA) are the test
+// points, column points the training / inducing points in chunks of 32. Each pair forms r and dk/dr of every stationary
+// part once and feeds up to NCH channels: channel c < P is the mean of output c (the pair weighted by alpha[c][n], a
+// broadcast column), channel P the Schur term of the variance (weighted by V[n, m], a 128 x 32 tile through shared
+// memory). White is zero between the test and the training set (static.py:75-79), so a term holding it contributes
+// nothing; Bias enters as its variance. A launch covers channels [c0, c0 + NCH); its per-chunk partials are reduced in
+// fixed order by pred_grad_reduce_kernel.
+// ---------------------------------------------------------------------------------------------------------------
+template <int DREG, int NCH>
+__global__ void __launch_bounds__(TILE) pred_grad_kernel(PredGradParams p, int c0, long mchunk, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char pg_smem[];
+  const MultiKern& mk = p.mk;
+  double (*sv)[33] = reinterpret_cast<double (*)[33]>(pg_smem);     // [128][33] V tile
+  double* sR = reinterpret_cast<double*>(pg_smem) + TILE * 33;      // [sumD][128] test points
+  double* sSr = sR + (size_t)mk.sumD * TILE;                        // [nparts][128]
+  double* sC = sSr + (size_t)mk.nparts * TILE;                      // [sumD][32] column chunk
+  double* sSc = sC + (size_t)mk.sumD * 32;                          // [nparts][32]
+  double* sA = sSc + (size_t)mk.nparts * 32;                        // [NCH][32] alpha of the chunk's points
+  const int tid = threadIdx.x;
+  const long r0 = (long)blockIdx.x * TILE, m = r0 + tid;
+  const long n_beg = (long)blockIdx.y * mchunk;
+  const long n_end = n_beg + mchunk < p.ncols ? n_beg + mchunk : p.ncols;
+  const int nch = NCH < p.P + 1 - c0 ? NCH : p.P + 1 - c0;
+  const bool has_var = c0 + nch == p.P + 1;                         // the variance channel is the last one
+  for (int q = 0; q < mk.sumD; q++) sR[q * TILE + tid] = p.rowsT[(long)q * p.ld_rows + m];
+  for (int q = 0; q < mk.nparts; q++) sSr[q * TILE + tid] = p.sq_rows[(long)q * p.ld_rows + m];
+  double acc[NCH][DREG];
+#pragma unroll
+  for (int c = 0; c < NCH; c++)
+#pragma unroll
+    for (int q = 0; q < DREG; q++) acc[c][q] = 0.0;
+  for (long n0 = n_beg; n0 < n_end; n0 += 32) {
+    __syncthreads();
+    if (has_var) {
+      for (int rr = tid >> 5; rr < TILE; rr += TILE / 32) {
+        const long gm = r0 + rr, gn = n0 + (tid & 31);
+        sv[rr][tid & 31] = (gm < p.nrows && gn < n_end) ? p.V[gm * p.ldv + gn] : 0.0;
+      }
+    }
+    for (int idx = tid; idx < mk.sumD * 32; idx += TILE) {
+      const int q = idx >> 5, mm = idx & 31;
+      sC[idx] = (n0 + mm < p.ncols) ? p.colsT[(long)q * p.ld_cols + n0 + mm] : 0.0;
+    }
+    for (int idx = tid; idx < mk.nparts * 32; idx += TILE) {
+      const int q = idx >> 5, mm = idx & 31;
+      sSc[idx] = (n0 + mm < p.ncols) ? p.sq_cols[(long)q * p.ld_cols + n0 + mm] : 0.0;
+    }
+    for (int idx = tid; idx < NCH * 32; idx += TILE) {
+      const int c = c0 + (idx >> 5), mm = idx & 31;
+      sA[idx] = (c < p.P && n0 + mm < n_end) ? p.alpha[(long)c * p.lda + n0 + mm] : 0.0;
+    }
+    __syncthreads();
+    if (m < p.nrows) {
+      const int mlim = (int)((n_end - n0) < 32 ? (n_end - n0) : 32);
+      for (int mm = 0; mm < mlim; mm++) {
+        for (int pi = 0; pi < mk.nparts; pi++) {
+          const PartDev& pd = mk.part[pi];
+          if (!is_stationary(pd.kind)) continue;
+          const double rr = gx_part_r(pd, pi, sR, sC, sSr, sSc, tid, mm, false);
+          if (rr == 0.0) continue;
+          double kk, dk;
+          k_dk_of_r_unit(pd.kind, rr, kk, dk);
+          double t = pd.variance * dk / rr;
+          for (int q = 0; q < mk.nparts; q++) {          // the other factors of this part's term
+            const PartDev& o = mk.part[q];
+            if (q == pi || o.term != pd.term) continue;
+            const double v = o.kind == GPX_BIAS ? 1.0
+                             : o.kind == GPX_WHITE ? 0.0
+                             : k_of_r_unit(o.kind, gx_part_r(o, q, sR, sC, sSr, sSc, tid, mm, false));
+            t *= o.variance * v;
+          }
+#pragma unroll
+          for (int c = 0; c < NCH; c++) {
+            if (c >= nch) break;
+            const double w = t * (c0 + c < p.P ? sA[c * 32 + mm] : sv[tid][mm]);
+#pragma unroll
+            for (int q = 0; q < DREG; q++)
+              if (q >= pd.xoff && q < pd.xoff + pd.D) acc[c][q] = fma(w, sR[q * TILE + tid] - sC[q * 32 + mm], acc[c][q]);
+          }
+        }
+      }
+    }
+  }
+  if (m < p.nrows) {
+#pragma unroll
+    for (int c = 0; c < NCH; c++) {
+      if (c >= nch) break;
+#pragma unroll
+      for (int q = 0; q < DREG; q++)
+        if (q < mk.sumD) part[(((long)(c0 + c) * gridDim.y + blockIdx.y) * p.nrows + m) * mk.sumD + q] = acc[c][q];
+    }
+  }
+}
+
+// out: dmu[m, d, c] (nrows x Dfull x P row-major), then dvar[m, d] (nrows x Dfull): per channel and data column the
+// chunk sums of the stacked rows on that column, in part order, divided by l_q or l^2 as gradx_multi_reduce_kernel does;
+// the variance channel times -2 (gp.py:460-462; gradients_X_diag is zero for these kinds, stationary.py:360-361)
+__global__ void pred_grad_reduce_kernel(const double* __restrict__ part, long M, int nchunk, int P, int Dfull, MultiKern mk,
+                                        double* __restrict__ out) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M * Dfull * (P + 1)) return;
+  const long m = i / ((long)Dfull * (P + 1));
+  const int d = (int)((i / (P + 1)) % Dfull), c = (int)(i % (P + 1));
+  double s = 0.0;
+  for (int pi = 0; pi < mk.nparts; pi++) {
+    const PartDev& pd = mk.part[pi];
+    if (!is_stationary(pd.kind)) continue;
+    for (int q = pd.xoff; q < pd.xoff + pd.D; q++) {
+      if (mk.dims[q] != d) continue;
+      double t = 0.0;
+      for (int ch = 0; ch < nchunk; ch++) t += part[(((long)c * nchunk + ch) * M + m) * mk.sumD + q];
+      const double l = mk.ls[q];
+      s += pd.ard ? t / l : t / (l * l);
+    }
+  }
+  if (c < P) out[(m * Dfull + d) * P + c] = s;
+  else out[M * Dfull * P + m * Dfull + d] = -2.0 * s;
+}
+
+// channels per launch: (P + 1) x DREG accumulators where up to 32 fit, else channel groups (one launch each)
+static int pred_grad_nch(int sumD) { return sumD <= 8 ? 4 : sumD <= 16 ? 2 : 1; }
+
+int pred_grad_launches(const MultiKern& mk, int P) {
+  const int g = pred_grad_nch(mk.sumD);
+  return (P + 1 + g - 1) / g + 1;
+}
+
+template <int DREG, int NCH>
+static int launch_pg_t(const PredGradParams& p, dim3 grid, size_t smem, long mchunk, double* part, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    const int mx = (TILE * 33 + (MAX_D + MAX_PARTS) * (TILE + 32) + NCH * 32) * 8;
+    GPX_CUDA(cudaFuncSetAttribute(pred_grad_kernel<DREG, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx));
+    attr_set = true;
+  }
+  for (int c0 = 0; c0 < p.P + 1; c0 += NCH) {
+    pred_grad_kernel<DREG, NCH><<<grid, TILE, smem, st>>>(p, c0, mchunk, part);
+    GPX_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+int launch_pred_grad(const PredGradParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st) {
+  const MultiKern& mk = p.mk;
+  if (has_ext(mk)) { set_error("gradients_X: RatQuad / StdPeriodic parts have no input gradient on the device"); return -2; }
+  const int nch = pred_grad_nch(mk.sumD);
+  const size_t smem = (size_t)(TILE * 33 + (mk.sumD + mk.nparts) * (TILE + 32) + nch * 32) * 8;
+  const dim3 grid((unsigned)((p.nrows + TILE - 1) / TILE), nchunk);
+  const int D = mk.sumD;
+  int rc;
+  if (D <= 8) rc = launch_pg_t<8, 4>(p, grid, smem, mchunk, part, st);
+  else if (D <= 16) rc = launch_pg_t<16, 2>(p, grid, smem, mchunk, part, st);
+  else if (D <= 32) rc = launch_pg_t<32, 1>(p, grid, smem, mchunk, part, st);
+  else rc = launch_pg_t<64, 1>(p, grid, smem, mchunk, part, st);
+  if (rc) return rc;
+  const long tot = p.nrows * p.Dfull * (p.P + 1);
+  pred_grad_reduce_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(part, p.nrows, nchunk, p.P, p.Dfull, mk, out);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // final assembly: fixed-order sums of the per-tile partials of every part, log-determinant, quadratic form
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) finalize_multi_kernel(FinalizeMultiParams f) {

@@ -103,6 +103,18 @@ struct GradXMultiParams {
   MultiKern mk;
 };
 
+// predictive gradients (GPy/core/gp.py:438-474) at the row points (the test points) against the column points (training
+// or inducing points), with gradx_multi_kernel's rules: channel c < P weights a pair by alpha[c * lda + n] (the mean
+// Jacobian of output c), channel P by V[m * ldv + n] with V = W K(X, X*) (the variance Jacobian's Schur term).
+struct PredGradParams {
+  const double* rowsT; long ld_rows; const double* sq_rows; long nrows;
+  const double* colsT; long ld_cols; const double* sq_cols; long ncols;
+  const double* alpha; long lda; int P;
+  const double* V; long ldv;
+  int Dfull;
+  MultiKern mk;
+};
+
 struct FinalizeMultiParams {
   const double* partials[MAX_PARTS]; long ntiles;
   const double* logdet_part; long nt;
@@ -118,6 +130,11 @@ int launch_grad_full_multi(const GradFullMultiParams& p, int row_tiles, int col_
 // two launches: chunk partials [nchunk][nrows][sumD] into part, then their fixed-order sum into out (device, nrows x Dfull)
 int launch_gradx_multi(const GradXMultiParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st);
 int launch_finalize_multi(const FinalizeMultiParams& f, cudaStream_t st);
+// one reduction launch per group of channels (as many channels per group as the accumulators allow), partials
+// [P + 1][nchunk][nrows][sumD] into part, then their fixed-order sum into out (device): dmu (nrows x Dfull x P row-major),
+// followed by dvar (nrows x Dfull). RatQuad / StdPeriodic parts: -2.
+int launch_pred_grad(const PredGradParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st);
+int pred_grad_launches(const MultiKern& mk, int P);   // kernels launch_pred_grad issues
 // entry t of part p's reduced sums -> entry t of its gradient block: the stationary lengthscale rule -tot/l
 // (stationary.py:210,213) for RBF .. Matern52 and RatQuad; RatQuad's power and StdPeriodic's sums are the gradient as they
 // are (stationary.py:797-798, standard_periodic.py:518-526). false: the trace slot (last) or a static part's unused slot.

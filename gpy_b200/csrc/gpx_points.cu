@@ -154,4 +154,48 @@ int grad_X(gpx_ctx* c, Kern k, const GradFullParams& gp, int D, double* part, do
   return 0;
 }
 
+int pred_grad_check(Kern k) {
+  for (int p = 0; k.mk && p < k.mk->nparts; p++)
+    if (k.mk->part[p].kind == GPX_RATQUAD || k.mk->part[p].kind == GPX_STDPERIODIC)
+      GPX_FAIL("gradients_X: RatQuad / StdPeriodic parts have no input gradient on the device");
+  return 0;
+}
+
+int pred_grad(gpx_ctx* c, Kern k, const Points& test, const Points& train, const double* alpha, long lda, int P,
+              const double* V, long ldv, int D, double* dmu, double* dvar) {
+  GPX_CHECK(pred_grad_check(k));
+  PredGradParams pp;
+  memset(&pp, 0, sizeof(pp));
+  if (k.mk) {
+    pp.mk = *k.mk;
+  } else {   // a single kernel is the one-part composite on the same prepared points (prep_x_kernel = prep_multi_kernel)
+    const KernParams& kp = *k.kp;
+    pp.mk.nparts = 1; pp.mk.sumD = kp.D;
+    pp.mk.part[0] = PartDev{kp.kind, kp.ard, 0, 0, kp.D, 0, kp.variance, kp.inv_ls_iso, 0.0};
+    for (int q = 0; q < kp.D; q++) { pp.mk.dims[q] = q; pp.mk.ls[q] = kp.ls[kp.ard ? q : 0]; }
+  }
+  pp.rowsT = test.xT; pp.ld_rows = test.ld; pp.sq_rows = test.sq; pp.nrows = test.n;
+  pp.colsT = train.xT; pp.ld_cols = train.ld; pp.sq_cols = train.sq; pp.ncols = train.n;
+  pp.alpha = alpha; pp.lda = lda; pp.P = P; pp.V = V; pp.ldv = ldv; pp.Dfull = D;
+  GradFullParams gp;   // only its extents: test points x training points
+  memset(&gp, 0, sizeof(gp));
+  gp.N = test.n; gp.M = train.n;
+  int nchunk;
+  long mchunk;
+  gradx_chunks(c, gp, &nchunk, &mchunk);
+  const size_t npart = (size_t)(P + 1) * nchunk * test.n * std::max(1, pp.mk.sumD), nout = (size_t)test.n * D * (P + 1);
+  double* buf = nullptr;
+  GPX_TMP_ALLOC(&buf, (npart + nout) * 8, c->st);
+  int rc = launch_pred_grad(pp, nchunk, mchunk, buf, buf + npart, c->st);
+  c->total_launches += pred_grad_launches(pp.mk, P);
+  const size_t nmu = (size_t)test.n * D * P;
+  if (rc == 0 && cudaMemcpyAsync(dmu, buf + npart, nmu * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
+  if (rc == 0 && cudaMemcpyAsync(dvar, buf + npart + nmu, (size_t)test.n * D * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess)
+    rc = -1;
+  if (cudaStreamSynchronize(c->st) != cudaSuccess && rc == 0) rc = -1;
+  GPX_TMP_FREE(buf, c->st);
+  if (rc == -1) set_error("predictive gradients: device failure");
+  return rc;
+}
+
 }  // namespace gpx

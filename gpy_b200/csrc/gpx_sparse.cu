@@ -50,6 +50,8 @@ struct SparseState {
   double *hs = nullptr;                              // het noise: [2 + P][Npad] column reductions s1, s2, r (see eval)
   double trYYT = 0.0;
   bool have_eval = false;
+  bool w_ready = false;                              // mm[9] holds woodbury_inv of the current evaluation (formed by
+                                                     // gpx_sparse_predictive_gradients, kept for its later calls)
   double noise = 0.0;
   Kern kern() const { return multi ? Kern(&mk) : Kern(&kp); }
   Points xpts() const { return Points{XsT, sqX, N, Npad}; }   // this rank's data points, prepared
@@ -62,6 +64,7 @@ void free_m(SparseState* s) {
   for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
   for (auto& p : s->mm) { if (p) cudaFree(p); p = nullptr; }
   s->have_eval = false;
+  s->w_ready = false;
   s->M = s->Mpad = 0;
   s->Nw = s->Mw = 0;
 }
@@ -209,6 +212,7 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
   }
   s->N = N;
   s->have_eval = false;
+  s->w_ready = false;
   {   // trYYT = sum(Y .* Y) (var_dtc.py:37,90); with row shards: summed over the ranks, like num_data
     double t = 0.0;
     for (int64_t i = 0; i < N * (int64_t)P; i++) t += Y[i] * Y[i];
@@ -433,6 +437,7 @@ static int sparse_eval_impl(gpx_ctx* c, Kern k, double kdiag, const double* Z, i
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
   s->have_eval = false;
+  s->w_ready = false;
   s->multi = k.mk != nullptr;
   if (s->multi) s->mk = *k.mk; else s->kp = *k.kp;
   s->kdiag = kdiag;
@@ -736,6 +741,50 @@ int gpx_sparse_get(gpx_ctx* c, int which, double* out) {
   GPX_CUDA(cudaMemcpy2DAsync(out, M * 8, src, Mpad * 8, (size_t)M * 8, M, cudaMemcpyDeviceToHost, st));
   GPX_CUDA(cudaStreamSynchronize(st));
   return 0;
+}
+
+/* predictive gradients of the last sparse evaluation (gp.py:438-474 with the predictive variable Z, sparse_gp.py:52-54):
+ * woodbury_inv W as gpx_sparse_get(1) forms it, into the same scratch and once per evaluation (an optimiser asks for one
+ * batch after another on the same posterior), then V = W K(Z, Xnew) on the DMMA GEMM and one fused Jacobian reduction */
+int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, double* dmu, double* dvar) {
+  if (!c || !Xnew || !dmu || !dvar) GPX_FAIL("null argument");
+  if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to differentiate the prediction of");
+  if (Mn < 1) GPX_FAIL("empty Xnew");
+  if (c->dist) GPX_FAIL("predictive gradients are single-GPU");
+  SparseState* s = c->sparse;
+  const Kern k = s->kern();
+  GPX_CHECK(pred_grad_check(k));
+  GPX_CUDA(cudaSetDevice(c->device));
+  cudaStream_t st = c->st;
+  const long Mpad = s->Mpad;
+  PointSet pn;
+  GPX_CHECK(upload_points(c, k, Xnew, Mn, s->D, pn));
+  double *Um = s->mm[1], *UB = s->mm[6], *T = s->mm[3], *W = s->mm[9], *DB = s->mm[8];
+  if (!s->w_ready) {   // once per evaluation: gpx_sparse_get(1) writes the same W into mm[9], nothing else writes it
+    GPX_CHECK(binv(c, UB, DB));
+    GPX_CHECK(combine(c, W, Mpad, -1.0, DB, 0.0, nullptr, 1.0));
+    GPX_CHECK(sandwich(c, Um, W, T, W));
+    s->w_ready = true;
+  }
+  // K(Xnew, Z) with element (m, a) at m + a * pn.ld (the GEMM's B operand, zero padded), V (Mpad x pn.ld) = W K(Xnew, Z)^T
+  double *Kxz = nullptr, *V = nullptr;
+  GPX_TMP_ALLOC(&Kxz, (size_t)pn.ld * Mpad * 8, st);
+  GPX_TMP_ALLOC(&V, (size_t)Mpad * pn.ld * 8, st);
+  int rc = 0;
+  if (cudaMemsetAsync(Kxz, 0, (size_t)pn.ld * Mpad * 8, st) != cudaSuccess) { gpx::set_error("gpx_sparse_predictive_gradients: device failure"); rc = -1; }
+  if (rc == 0) rc = build_K(c, k, pn, s->zpts(), Kxz, pn.ld);
+  if (rc == 0) rc = launched(c);
+  if (rc == 0) {
+    GemmParams pg = gemm_defaults();
+    pg.mode = GEMM_PANEL; pg.plain = 1;
+    pg.A = W; pg.lda = Mpad; pg.B = Kxz; pg.ldb = pn.ld; pg.C = V; pg.ldc = Mpad;
+    pg.K = (int)Mpad; pg.nt = (int)(Mpad / TILE); pg.ncols = (int)(pn.ld / TILE);
+    rc = launch_gemm(pg, dim3(1, 1), st);
+    if (rc == 0) rc = launched(c);
+  }
+  if (rc == 0) rc = pred_grad(c, k, pn, s->zpts(), s->Cm, Mpad, s->P, V, Mpad, s->D, dmu, dvar);
+  GPX_TMP_FREE(Kxz, st); GPX_TMP_FREE(V, st);
+  return rc;
 }
 
 }  // extern "C"

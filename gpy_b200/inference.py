@@ -11,7 +11,8 @@ Mirrors (same names, argument meaning, return structure and error behaviour):
 import numpy as np
 
 from . import _ffi
-from .kern import (DeviceGradient, composite_state_key, flatten_parts, part_descriptor, part_ngrad, single_kernel)
+from .kern import (DeviceGradient, _PartKern, composite_state_key, flatten_parts, part_descriptor, part_ngrad,
+                   single_kernel)
 from .param import Param, Parameterized
 
 
@@ -156,19 +157,37 @@ class PosteriorExact(object):
         """posterior.py:98-110: K alpha."""
         return np.dot(self.K, self.woodbury_vector)
 
-    def _raw_predict(self, kern, Xnew, pred_var=None, full_cov=False):
-        """posterior.py:273-302 on the device (gpx_predict). `pred_var` (the training inputs) is what the engine holds."""
+    def _is_evaluated(self, kern):
+        """kern is the kernel of the evaluation this posterior describes"""
         key = kern._state_key() if hasattr(kern, "_state_key") else (
             kern._gpx_state_key() if hasattr(kern, "_gpx_state_key") else composite_state_key(kern))
-        if self._kern_key is not None and key != self._kern_key:
+        return self._kern_key is None or key == self._kern_key
+
+    @staticmethod
+    def _engine_X(kern, Xnew):
+        Xn = kern._slice_X(Xnew) if hasattr(kern, "_slice_X") else np.asarray(Xnew, dtype=np.float64)
+        if isinstance(Xn, tuple):
+            Xn = Xn[0]
+        return np.ascontiguousarray(Xn, dtype=np.float64)
+
+    def _raw_predict(self, kern, Xnew, pred_var=None, full_cov=False):
+        """posterior.py:273-302 on the device (gpx_predict). `pred_var` (the training inputs) is what the engine holds."""
+        if not self._is_evaluated(kern):
             # a different kernel than the one evaluated (GP.predict(Xnew, kern=sub_kernel)): the reference's formula with
             # the kernel it is given (posterior.py:276-295), on the factor fetched from the device
             return HostPosterior(self.woodbury_chol, self.woodbury_vector, None)._raw_predict(kern, Xnew, pred_var, full_cov)
         self._check_fresh()
-        Xn = kern._slice_X(Xnew) if hasattr(kern, "_slice_X") else np.asarray(Xnew, dtype=np.float64)
-        if isinstance(Xn, tuple):
-            Xn = Xn[0]
-        return self._engine.predict(np.ascontiguousarray(Xn, dtype=np.float64), full_cov=full_cov)
+        return self._engine.predict(self._engine_X(kern, Xnew), full_cov=full_cov)
+
+    def _predictive_gradients(self, kern, Xnew):
+        """gp.py:438-462 on the device (gpx_predictive_gradients) -> (dmu (M, D, P), dvar (M, D)) over the columns the
+        engine holds (a single kernel's active dims), or None when kern is not the evaluated kernel or has a leaf without
+        a device input gradient (RatQuad, StdPeriodic)"""
+        leaves = flatten_parts(kern)
+        if not self._is_evaluated(kern) or leaves is None or any(isinstance(k, _PartKern) for k, _ in leaves):
+            return None
+        self._check_fresh()
+        return self._engine.predictive_gradients(self._engine_X(kern, Xnew))
 
 
 class _DataKey(object):
@@ -327,6 +346,12 @@ class HostPosterior(object):
 
     def __init__(self, woodbury_chol, woodbury_vector, K):
         self.woodbury_chol, self.woodbury_vector, self.K = woodbury_chol, woodbury_vector, K
+
+    @property
+    def woodbury_inv(self):
+        """posterior.py:183-203: (K + noise)^-1 from the factor (dpotri)"""
+        from scipy.linalg import cho_solve
+        return cho_solve((self.woodbury_chol, True), np.eye(self.woodbury_chol.shape[0]))
 
     def _raw_predict(self, kern, Xnew, pred_var, full_cov=False):
         from scipy.linalg import solve_triangular

@@ -490,6 +490,13 @@ class Add(CombinationKernel):
     def gradients_X(self, dL_dK, X, X2=None):
         return sum(p.gradients_X(dL_dK, X, X2) for p in self.parts)
 
+    def gradients_X_diag(self, dL_dKdiag, X):
+        """add.py:102-105"""
+        target = np.zeros(np.asarray(X).shape)
+        for p in self.parts:
+            target += p.gradients_X_diag(dL_dKdiag, X)
+        return target
+
 
 class Prod(CombinationKernel):
     """GPy.kern.Prod (prod.py:23-110)."""
@@ -539,6 +546,18 @@ class Prod(CombinationKernel):
             out = out + p.gradients_X(dL_dK * other if other is not None else dL_dK, X, X2)
         return out
 
+    def gradients_X_diag(self, dL_dKdiag, X):
+        """prod.py:409-418"""
+        target = np.zeros(np.asarray(X).shape)
+        if len(self.parts) == 2:
+            target += self.parts[0].gradients_X_diag(dL_dKdiag * self.parts[1].Kdiag(X), X)
+            target += self.parts[1].gradients_X_diag(dL_dKdiag * self.parts[0].Kdiag(X), X)
+        else:
+            k = self.Kdiag(X) * dL_dKdiag
+            for p in self.parts:
+                target += p.gradients_X_diag(k / p.Kdiag(X), X)
+        return target
+
 
 class Static(Kern):
     """GPy.kern.src.static.Static (static.py:11-61): a variance parameter, no dependence on X."""
@@ -554,6 +573,10 @@ class Static(Kern):
         return ret
 
     def gradients_X(self, dL_dK, X, X2=None):
+        return np.zeros(np.asarray(X).shape)
+
+    def gradients_X_diag(self, dL_dKdiag, X):
+        """static.py:30-31"""
         return np.zeros(np.asarray(X).shape)
 
     def update_gradients_diag(self, dL_dKdiag, X):

@@ -12,7 +12,7 @@ paramz are importable, use the real GPy model with the plugin classes of gpy_b20
 """
 import numpy as np
 
-from .inference import ExactGaussianInference, Gaussian, HeteroscedasticGaussian
+from .inference import ExactGaussianInference, Gaussian, HeteroscedasticGaussian, PosteriorExact
 from .kern import RBF
 from .param import Logexp, Parameterized
 
@@ -243,6 +243,52 @@ class GP(Parameterized):
 
     def predict_noiseless(self, Xnew, full_cov=False, Y_metadata=None, kern=None):
         return self.predict(Xnew, full_cov, Y_metadata, kern, None, False)
+
+    def predictive_gradients(self, Xnew, kern=None):
+        """gp.py:418-474: derivatives of the predictive mean (N*, Q, P) and variance (N*, Q) with respect to Xnew. With
+        the evaluated kernel on a device posterior this is one gpx_predictive_gradients call (nothing of size N^2 reaches
+        the host); any other kernel, the generic inference path and kernels without a device input gradient take the
+        reference's formula with the stand-alone kernel calls."""
+        Xnew = np.asarray(Xnew, dtype=np.float64)
+        kern = self.kern if kern is None else kern
+        dev = self.posterior._predictive_gradients(kern, Xnew) if isinstance(self.posterior, PosteriorExact) else None
+        if dev is not None:
+            mean_jac, var_jac = (scatter_active_dims(kern, g, Xnew.shape[1]) for g in dev)
+        else:
+            mean_jac, var_jac = host_predictive_gradients(kern, self.posterior, Xnew, self.X)
+        if self.normalizer is not None:                             # gp.py:466-472
+            mean_jac = self.normalizer.inverse_mean(mean_jac) - self.normalizer.inverse_mean(0.)
+            if self.output_dim > 1:
+                var_jac = self.normalizer.inverse_covariance(var_jac)
+            else:
+                var_jac = self.normalizer.inverse_variance(var_jac)
+        return mean_jac, var_jac
+
+
+def scatter_active_dims(kern, g, Q):
+    """a single kernel's gradient over its active dims (axis 1) -> the full Q input columns, zero elsewhere, as
+    Stationary.gradients_X scatters (kernel_slice_operations.py:138-150); a composite's already spans them"""
+    if g.shape[1] == Q:
+        return g
+    full = np.zeros((g.shape[0], Q) + g.shape[2:])
+    full[:, kern.active_dims] = g
+    return full
+
+
+def host_predictive_gradients(kern, posterior, Xnew, Xpred):
+    """gp.py:438-462 with the kernel's own K / gradients_X / gradients_X_diag. The 1 x N row woodbury_vector[:, p].T the
+    reference hands gradients_X is broadcast over the N* rows here, because the stand-alone kernel calls take a full
+    dL_dK. woodbury_inv is read after the mean Jacobian, as in the reference, so a kernel without gradients_X raises
+    before it is fetched."""
+    wv = np.asarray(posterior.woodbury_vector, dtype=np.float64)
+    mean_jac = np.empty((Xnew.shape[0], Xnew.shape[1], wv.shape[1]))
+    for i in range(wv.shape[1]):
+        dL = np.ascontiguousarray(np.broadcast_to(wv[:, i][None, :], (Xnew.shape[0], wv.shape[0])))
+        mean_jac[:, :, i] = kern.gradients_X(dL, Xnew, Xpred)
+    var_jac = kern.gradients_X_diag(np.ones(Xnew.shape[0]), Xnew)
+    alpha = -2. * np.dot(kern.K(Xnew, Xpred), np.asarray(posterior.woodbury_inv, dtype=np.float64))
+    var_jac = var_jac + kern.gradients_X(alpha, Xnew, Xpred)
+    return mean_jac, var_jac
 
 
 class GPHeteroscedasticRegression(GP):

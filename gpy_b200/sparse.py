@@ -19,6 +19,7 @@ import numpy as np
 
 from . import _ffi
 from .inference import Gaussian, HeteroscedasticGaussian, _DataKey
+from .model import host_predictive_gradients, scatter_active_dims
 from .kern import (RBF, RatQuad, StdPeriodic, Stationary, flatten_parts, part_descriptor, part_ngrad,
                    scatter_leaf_gradients, single_kernel)
 from .param import Logexp, Param, Parameterized
@@ -58,6 +59,12 @@ class LazySparsePosterior(object):
     woodbury_inv = property(lambda self: self._get("woodbury_inv"))
     K = property(lambda self: self._get("Kmm"))
     K_chol = property(lambda self: self._get("Lm"))
+
+    def _predictive_gradients(self, Xnew):
+        """gp.py:438-462 with the predictive variable Z on the device (gpx_sparse_predictive_gradients)"""
+        if self._eng.sparse_serial != self._serial:
+            raise RuntimeError("stale sparse posterior: the engine has evaluated other parameters since")
+        return self._eng.sparse_predictive_gradients(Xnew)
 
     def materialise(self):
         for w in ("woodbury_vector", "woodbury_inv"):
@@ -304,3 +311,13 @@ class SparseGPRegression(Parameterized):
                                  "include_likelihood=False (gp_heteroscedastic_regression.py:13-15)")
             mu, var = self.likelihood.predictive_values(mu, var, full_cov, Y_metadata=Y_metadata)
         return mu, var
+
+    def predictive_gradients(self, Xnew, kern=None):
+        """gp.py:418-474 with the predictive variable Z (sparse_gp.py:52-54): with the evaluated kernel one
+        gpx_sparse_predictive_gradients call, with any other kernel the reference's formula on the stand-alone calls"""
+        Xnew = np.asarray(Xnew, dtype=np.float64)
+        if kern is None or kern is self.kern:
+            Xs = self.kern._slice_X(Xnew) if single_kernel(self.kern) else np.ascontiguousarray(Xnew)
+            return tuple(scatter_active_dims(self.kern, g, Xnew.shape[1])
+                         for g in self.posterior._predictive_gradients(Xs))
+        return host_predictive_gradients(kern, self.posterior, Xnew, self.Z.values)

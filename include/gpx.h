@@ -137,6 +137,27 @@ int gpx_get(gpx_ctx* ctx, int which, double* out_host);
  * or var (M x M col-major) = K(Xnew) - tmp^T tmp                                                 [full_cov = 1]. */
 int gpx_predict(gpx_ctx* ctx, const double* Xnew, int64_t M, int full_cov, double* mu, double* var);
 
+/* GP.predictive_gradients (GPy/core/gp.py:418-474) on the device with the posterior of the last evaluation:
+ *   dmu  (M x D x P row-major): dmu[m, q, p] = sum_n alpha[n, p] dk(x*_m, x_n)/dx*_mq
+ *        (kern.gradients_X(woodbury_vector[:, p:p+1].T, Xnew, X), gp.py:442-446)
+ *   dvar (M x D row-major):     dvar[m, q] = -2 sum_n V[n, m] dk(x*_m, x_n)/dx*_mq, V = woodbury_inv K(X, Xnew)
+ *        (gp.py:448-462; gradients_X_diag is zero for these kernels, stationary.py:360-361, static.py:27-31)
+ * D is that of the data set. The kernel is the evaluation's: a single kernel, or a composite of RBF .. Matern52, White
+ * (zero between test and training points) and Bias parts; the input-gradient rules are those of gpx_kern_grad_X.
+ *   gpx_predictive_gradients        : after gpx_exact_eval / _het / _multi. V = U (U^T K(X, Xnew)) with U = L^-T of the
+ *                                     stored factor, MAX_P = 8 test points per pair of triangular passes; K^-1 is never
+ *                                     formed. Launches: 2 + 3 ceil(M / 8) + R.
+ *   gpx_sparse_predictive_gradients : after gpx_sparse_eval / _het / _multi; X = Z, alpha = woodbury_vector and W =
+ *                                     woodbury_inv (var_dtc.py:207-210), formed as gpx_sparse_get(1) forms it, by the
+ *                                     first call after an evaluation only (kept for the later calls); V on the DMMA
+ *                                     GEMM. Launches: 8 + R for the first call after an evaluation, 3 + R after it.
+ * R = ceil((P + 1) / g) + 1 reduction launches, g = 4 channels per launch when the kernel's stacked active dims are
+ * <= 8, 2 when <= 16, else 1. Returns -2 without touching the posterior when there is no evaluation, M < 1, a pointer is
+ * null, the kernel has a RatQuad or StdPeriodic part (no device input gradient) or a communicator is attached
+ * (single-GPU). Nothing that gpx_get, gpx_sparse_get, gpx_predict or gpx_get_stats return changes. */
+int gpx_predictive_gradients(gpx_ctx* ctx, const double* Xnew, int64_t M, double* dmu, double* dvar);
+int gpx_sparse_predictive_gradients(gpx_ctx* ctx, const double* Xnew, int64_t M, double* dmu, double* dvar);
+
 /* Standalone kernel plugin calls (no context needed beyond a device; ctx may be NULL -> device 0 scratch context).
  * Replaces Stationary.K (stationary.py:105-168): out is N x M ROW-major (what Kern.K returns to NumPy callers).
  * out == NULL: build on the device only and report the kernel time via gpx_get_stats (kbuild_ms, kbuild_bytes). */
