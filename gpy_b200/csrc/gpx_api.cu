@@ -150,7 +150,7 @@ int gpx_destroy(gpx_ctx* c) {
   if (!c) return 0;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->st);
-  dist_free(c);
+  dist_destroy(c);
   sparse_free(c);
   free_data(c);
   for (auto e : c->ev) cudaEventDestroy(e);

@@ -96,7 +96,8 @@ int alloc_data(gpx_ctx* c, long NB);                         // those of them wh
 // multi-GPU hooks implemented in gpx_dist.cu
 int dist_set_data(gpx_ctx* c, int64_t N, int D, int P);      // (re)allocates the sharded layout for N points
 int dist_exact_eval(gpx_ctx* c, double extra_jitter);
-void dist_free(gpx_ctx* c);
+void dist_free(gpx_ctx* c);                                  // the sharded buffers; the communicator stays
+void dist_destroy(gpx_ctx* c);                               // the buffers, the communicator and its state
 int dist_get_L(gpx_ctx* c, double* out);                                       // collective: sharded woodbury_chol
 long dist_block(const gpx_ctx* c);
 const double* dist_U(const gpx_ctx* c, long* ld);                               // sharded: column-owned U storage                                             // NB of the sharded layout (0: none)

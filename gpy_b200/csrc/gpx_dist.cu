@@ -125,6 +125,21 @@ void dist_free(gpx_ctx* c) {
   d->Bc = d->Bc2 = d->blkpart = d->SU = nullptr;
 }
 
+// everything the communicator brought to the context: the sharded buffers, the NCCL communicators (and their device
+// memory and proxy threads), the reduction buffers and events; the context is single-GPU afterwards
+void dist_destroy(gpx_ctx* c) {
+  if (!c->dist) return;
+  DistState* d = c->dist;
+  dist_free(c);
+  if (d->comm2) g_nccl.CommDestroy(d->comm2);
+  if (d->comm) g_nccl.CommDestroy(d->comm);
+  if (d->raw) cudaFree(d->raw);
+  if (d->h_raw) cudaFreeHost(d->h_raw);
+  for (auto e : d->ev) cudaEventDestroy(e);
+  delete d;
+  c->dist = nullptr;
+}
+
 // Collective gpx_get(GPX_GET_L) on a sharded factor (Posterior.woodbury_chol, posterior.py:21-77): block row by block row the
 // owner extracts its rows of L into a staging block, broadcasts it, and every rank copies it into its own host matrix
 // (N x N column-major). N x NB doubles of device staging; nothing of size N^2 on any device.
@@ -273,9 +288,9 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
       GPX_CHECK(launch_assemble(Sblk, ld, (int)NB, Pb + pos_k * NB * NB, NB, Bc, ss));
       c->eval_launches++;
     }
-    if (d->nblk == 1) break;
-    GPX_NCCL(g_nccl.Broadcast(Bc, Bc, (size_t)NB * NB, ncclDouble, root, cs, ss));
-    {
+    // one block: there is no panel, and the owner's chunk already holds U_kk, which the copy-back files into SU
+    if (d->nblk > 1) {
+      GPX_NCCL(g_nccl.Broadcast(Bc, Bc, (size_t)NB * NB, ncclDouble, root, cs, ss));
       GemmParams pp = gemm_defaults();
       pp.mode = GEMM_PANEL;
       pp.A = c->S + o * ld; pp.lda = ld; pp.loc_A = 1;
@@ -286,8 +301,8 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
       pp.K = (int)NB; pp.nt = nt; pp.skip0 = kt0; pp.skip1 = kt1; pp.tri = 1;
       GPX_CHECK(launch_gemm(pp, dim3(nbt, nt - nbt), ss));
       c->eval_launches++;
+      GPX_NCCL(g_nccl.AllGather(Pb + (size_t)g * d->npr * NB * NB, Pb, (size_t)d->npr * NB * NB, ncclDouble, cs, ss));
     }
-    GPX_NCCL(g_nccl.AllGather(Pb + (size_t)g * d->npr * NB * NB, Pb, (size_t)d->npr * NB * NB, ncclDouble, cs, ss));
     GPX_CHECK(launch_copyback(c->S, ld, d->SU, Npad, Pb, NB, G, g, d->npr, k, nt, ss));
     c->eval_launches++;
     if (la) {
@@ -396,18 +411,28 @@ int gpx_comm_init(gpx_ctx* c, const char id[128], int rank, int nranks) {
   if (nranks < 1 || rank < 0 || rank >= nranks) { gpx::set_error("bad rank / nranks"); return -2; }
   GPX_CHECK(load_nccl());
   GPX_CUDA(cudaSetDevice(c->device));
-  if (!c->dist) c->dist = new DistState();
-  DistState* d = c->dist;
+  GPX_CUDA(cudaStreamSynchronize(c->st));
+  // a second call replaces the communicator: the earlier one is released, and the workspace (with any evaluation in it)
+  // goes with it, since its layout was that of the earlier attachment
+  dist_destroy(c);
+  free_data(c);
+  c->Npad = 0;   // the next gpx_set_data allocates the distributed layout
+  DistState* d = new DistState();
   ncclUniqueId uid;
   memcpy(uid.internal, id, 128);
-  GPX_NCCL(g_nccl.CommInitRank(&d->comm, nranks, uid, rank));
+  const ncclResult_t r = g_nccl.CommInitRank(&d->comm, nranks, uid, rank);
+  if (r != ncclSuccess) {   // the context stays single-GPU
+    delete d;
+    gpx::set_error(std::string("ncclCommInitRank failed: ") + g_nccl.GetErrorString(r));
+    return -4;
+  }
+  c->dist = d;
   d->rank = rank; d->G = nranks;
   if (g_nccl.CommSplit && nranks > 1 && !getenv("GPX_NO_DIST_LOOKAHEAD")) {
     if (g_nccl.CommSplit(d->comm, 0, rank, &d->comm2, nullptr) != ncclSuccess) d->comm2 = nullptr;
   }
   GPX_CUDA(cudaMalloc(&d->raw, (MAX_D + 8) * sizeof(double)));
   GPX_CUDA(cudaMallocHost(&d->h_raw, (MAX_D + 8) * sizeof(double)));
-  c->Npad = 0;   // force re-allocation in the distributed layout at the next gpx_set_data
   return 0;
 }
 

@@ -264,7 +264,10 @@ int gpx_set_option(gpx_ctx* ctx, const char* name, int64_t value);
 /* Multi-GPU (one process per GPU). The caller obtains a 128-byte NCCL unique id on rank 0 (gpx_comm_unique_id),
  * ships it to the other ranks with its own plumbing (torch.distributed broadcast), and every rank calls
  * gpx_comm_init. Afterwards gpx_set_data / gpx_exact_eval are collective: block rows are dealt block-cyclically
- * to the ranks, the inverted diagonal block is broadcast and the panel all-gathered (NCCL over NVLink), scalars all-reduced. */
+ * to the ranks, the inverted diagonal block is broadcast and the panel all-gathered (NCCL over NVLink), scalars all-reduced.
+ * nranks = 1 is supported: one process on one GPU then runs the same sharded layout and collectives. gpx_comm_init drops
+ * the context's data and evaluation (call gpx_set_data again); on a context that already has a communicator it releases
+ * that one first. gpx_destroy releases the communicator. */
 int gpx_comm_unique_id(char id_out[128]);
 int gpx_comm_init(gpx_ctx* ctx, const char id[128], int rank, int nranks);
 

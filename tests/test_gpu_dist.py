@@ -1,5 +1,6 @@
 """GPU test of the sharded (multi-GPU) evaluation: needs >= 2 devices, skipped otherwise (on a single H100 it skips;
-tools/dist_check.py is the same check for a multi-GPU session)."""
+tools/dist_check.py is the same check for a multi-GPU session). The sharded layout on one GPU, through a one-rank
+communicator, is tested in tests/test_gpu_sharded_single_rank.py."""
 import os
 import subprocess
 import sys
