@@ -81,6 +81,10 @@ EXPORTS = {
     "gpx_predict": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
     "gpx_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
     "gpx_sparse_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
+    "gpx_posterior_covariance": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, ctypes.c_int64, _dp]),
+    "gpx_posterior_samples": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
+    "gpx_sparse_posterior_samples": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, ctypes.c_int64, ctypes.c_int, _dp,
+                                                    _dp]),
     "gpx_kern_K": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64, _dp,
                                   ctypes.c_int64, ctypes.c_int, _dp]),
     "gpx_kern_Kdiag": (ctypes.c_int, [ctypes.c_int, ctypes.c_double, ctypes.c_int64, _dp]),
@@ -295,6 +299,44 @@ class Engine(object):
         """the same with the last sparse evaluation (predictive variable Z) -> (dmu (M, D, P), dvar (M, D))"""
         return self._pred_grads(self._L.gpx_sparse_predictive_gradients, "gpx_sparse_predictive_gradients", Xnew,
                                 self.sD, self.sP)
+
+    def posterior_covariance(self, X1, X2=None):
+        """Posterior.covariance_between_points (posterior.py:109-130) with the last exact evaluation -> (M1, M2)
+        K(X1, X2) - K(X1, X) Ky^-1 K(X, X2); X2 None: X2 = X1, exactly symmetric with zero distance on the diagonal"""
+        X1 = _f64(X1)
+        X2 = None if X2 is None else _f64(X2)
+        for A in (X1,) if X2 is None else (X1, X2):
+            if A.ndim != 2 or (self.D and A.shape[1] != self.D):
+                raise ValueError("test points must be M x %d" % self.D)
+        M1 = X1.shape[0]
+        M2 = M1 if X2 is None else X2.shape[0]
+        cov = np.empty((M1, M2))
+        check(self._L.gpx_posterior_covariance(self._h, _ptr(X1), M1, _ptr(X2), M2 if X2 is not None else 0, _ptr(cov)),
+              "gpx_posterior_covariance")
+        return cov
+
+    def _samples(self, fn, name, Xnew, z, max_tries, D, P):
+        Xnew, z = _f64(Xnew), _f64(z)
+        if Xnew.ndim != 2 or (D and Xnew.shape[1] != D):
+            raise ValueError("Xnew must be M x %d" % D)
+        M = Xnew.shape[0]
+        if z.ndim != 2 or z.shape[1] != M:
+            raise ValueError("z must be nz x %d (P S standard-normal vectors, output-major)" % M)
+        nz = z.shape[0]
+        f = np.empty((nz, M))
+        jit = ctypes.c_double()
+        check(fn(self._h, _ptr(Xnew), M, _ptr(z), nz, int(max_tries), _ptr(f), ctypes.byref(jit)), name)
+        return f, jit.value
+
+    def posterior_samples(self, Xnew, z, max_tries=5):
+        """joint samples of the latent function at Xnew from the last exact evaluation: z (P S, M) standard normals,
+        output-major -> (f (P S, M) in z's layout, f_j = mu[:, j // S] + chol(Sigma + jitter I) z_j, jitter used)"""
+        return self._samples(self._L.gpx_posterior_samples, "gpx_posterior_samples", Xnew, z, max_tries, self.D, self.P)
+
+    def sparse_posterior_samples(self, Xnew, z, max_tries=5):
+        """the same with the last sparse evaluation (predictive variable Z)"""
+        return self._samples(self._L.gpx_sparse_posterior_samples, "gpx_sparse_posterior_samples", Xnew, z, max_tries,
+                             self.sD, self.sP)
 
     def kern_K_device_only(self, kind, ARD, variance, lengthscale, X, X2=None):
         """build K(X, X2) on the device without bringing it back; -> (kernel ms, algorithmic GB/s)."""

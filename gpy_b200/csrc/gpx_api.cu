@@ -152,6 +152,7 @@ int gpx_destroy(gpx_ctx* c) {
   cudaStreamSynchronize(c->st);
   dist_destroy(c);
   sparse_free(c);
+  if (c->cJ) gpx_destroy(c->cJ);
   free_data(c);
   for (auto e : c->ev) cudaEventDestroy(e);
   for (auto e : c->sync_ev) cudaEventDestroy(e);
@@ -584,12 +585,6 @@ static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec) {
   if (rec) rec->end(h);
   c->eval_launches++;
   return 0;
-}
-
-// the kernel of the context's last evaluation, and its training points as build_Ky prepared them
-static Kern ctx_kern(const gpx_ctx* c) { return c->multi ? Kern(&c->mk) : Kern(&c->kp); }
-static Points train_points(const gpx_ctx* c) {
-  return c->multi ? Points{c->mXsT, c->msq, c->N, c->Npad} : Points{c->dXsT, c->dsq, c->N, c->Npad};
 }
 
 // Ky = K(X, X) + noise + jitter (+ the per-point noise) of the context's kernel into the workspace, training points

@@ -85,6 +85,8 @@ struct gpx_ctx {
   size_t mpart_cap = 0;        // doubles mpartials holds
   struct DistState* dist = nullptr;   // multi-GPU state (gpx_dist.cu), null on a single GPU
   struct SparseState* sparse = nullptr;   // sparse-GP (VarDTC) state (gpx_sparse.cu)
+  gpx_ctx* cJ = nullptr;       // child context holding the factor of the last sampled covariance (gpx_joint.cu), created on
+                               // first use: the caller's own factor, alpha and stats stay those of its evaluation
 };
 
 
@@ -164,6 +166,43 @@ int grad_X(gpx_ctx* c, Kern k, const GradFullParams& gp, int D, double* part, do
 int pred_grad_check(Kern k);
 int pred_grad(gpx_ctx* c, Kern k, const Points& test, const Points& train, const double* alpha, long lda, int P,
               const double* V, long ldv, int D, double* dmu, double* dvar);
+// the kernel of the context's last exact evaluation, and its training points as the evaluation prepared them
+inline Kern ctx_kern(const gpx_ctx* c) { return c->multi ? Kern(&c->mk) : Kern(&c->kp); }
+inline Points train_points(const gpx_ctx* c) {
+  return c->multi ? Points{c->mXsT, c->msq, c->N, c->Npad} : Points{c->dXsT, c->dsq, c->N, c->Npad};
+}
+
+// ---- joint posterior (gpx_joint.cu) ------------------------------------------------------------------------------------
+#define GPX_FAIL_DEVICE(what)                             \
+  do {                                                    \
+    gpx::set_error(std::string(what) + ": device failure"); \
+    return -1;                                            \
+  } while (0)
+// a stream-ordered temporary of doubles, released when it goes out of scope (or earlier, by release()); alloc reports an
+// exhausted pool as -1 with a message
+struct TmpBuf {
+  double* p = nullptr;
+  cudaStream_t st;
+  explicit TmpBuf(cudaStream_t s) : st(s) {}
+  ~TmpBuf() { release(); }
+  int alloc(size_t doubles);
+  void release() { GPX_TMP_FREE(p, st); p = nullptr; }
+};
+// C = A B^T on the plain DMMA GEMM (GEMM_PANEL entry): rows x cols (whole tiles), k-depth kdepth; plain 2: lower tiles only;
+// tri 1: B lower triangular, 2: A lower triangular. One launch, counted.
+int gemm_nt(gpx_ctx* c, const double* A, long lda, const double* B, long ldb, double* C, long ldc, long rows, long cols,
+            long kdepth, int plain, int tri);
+// out(a, b) = K(a, off2 + b) - prod(a, b) (prod's lower tiles mirrored when sym); out column-major (ldo) or row-major
+int joint_combine(gpx_ctx* c, const double* K, long ldk, long off2, const double* prod, long ldp, int sym, long M1, long M2,
+                  double* out, long ldo, int colmajor);
+// the argument checks of a sampling entry (-2 before anything is launched)
+int joint_check(const gpx_ctx* c, const double* X, int64_t M, const double* z, int64_t nz, const double* f,
+                const double* jitter_used, int P);
+// f = mu + L_Sigma z for the device matrix Sigma (M x M, leading dimension lds), factored with jitchol's ladder in the child
+// context c->cJ; mu [P][ldmu] (device), S vectors per output; z and f host, nz x M row-major
+int joint_sample(gpx_ctx* c, const double* Sig, long lds, long M, const double* mu, long ldmu, const double* z, long nz,
+                 long S, int max_tries, double* f, double* jitter_used);
+
 // the parts of a composite kernel -> mk (validated against Dfull columns of X), *kdiag_total = its Kdiag (gpx_api.cu)
 int fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Dfull, double* kdiag_total);
 }  // namespace gpx

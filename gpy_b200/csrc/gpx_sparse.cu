@@ -743,6 +743,26 @@ int gpx_sparse_get(gpx_ctx* c, int which, double* out) {
   return 0;
 }
 
+}  // extern "C"
+
+// woodbury_inv W of the current evaluation in mm[9], formed as gpx_sparse_get(1) forms it by the first caller after an
+// evaluation (predictive gradients or samples) and kept for the later ones: gpx_sparse_get(1) writes the same W into mm[9],
+// nothing else writes it
+static int woodbury_inv(gpx_ctx* c, double** W) {
+  SparseState* s = c->sparse;
+  double *Um = s->mm[1], *UB = s->mm[6], *T = s->mm[3], *DB = s->mm[8];
+  *W = s->mm[9];
+  if (!s->w_ready) {
+    GPX_CHECK(binv(c, UB, DB));
+    GPX_CHECK(combine(c, *W, s->Mpad, -1.0, DB, 0.0, nullptr, 1.0));
+    GPX_CHECK(sandwich(c, Um, *W, T, *W));
+    s->w_ready = true;
+  }
+  return 0;
+}
+
+extern "C" {
+
 /* predictive gradients of the last sparse evaluation (gp.py:438-474 with the predictive variable Z, sparse_gp.py:52-54):
  * woodbury_inv W as gpx_sparse_get(1) forms it, into the same scratch and once per evaluation (an optimiser asks for one
  * batch after another on the same posterior), then V = W K(Z, Xnew) on the DMMA GEMM and one fused Jacobian reduction */
@@ -759,13 +779,8 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
   const long Mpad = s->Mpad;
   PointSet pn;
   GPX_CHECK(upload_points(c, k, Xnew, Mn, s->D, pn));
-  double *Um = s->mm[1], *UB = s->mm[6], *T = s->mm[3], *W = s->mm[9], *DB = s->mm[8];
-  if (!s->w_ready) {   // once per evaluation: gpx_sparse_get(1) writes the same W into mm[9], nothing else writes it
-    GPX_CHECK(binv(c, UB, DB));
-    GPX_CHECK(combine(c, W, Mpad, -1.0, DB, 0.0, nullptr, 1.0));
-    GPX_CHECK(sandwich(c, Um, W, T, W));
-    s->w_ready = true;
-  }
+  double* W = nullptr;
+  GPX_CHECK(woodbury_inv(c, &W));
   // K(Xnew, Z) with element (m, a) at m + a * pn.ld (the GEMM's B operand, zero padded), V (Mpad x pn.ld) = W K(Xnew, Z)^T
   double *Kxz = nullptr, *V = nullptr;
   GPX_TMP_ALLOC(&Kxz, (size_t)pn.ld * Mpad * 8, st);
@@ -785,6 +800,46 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
   if (rc == 0) rc = pred_grad(c, k, pn, s->zpts(), s->Cm, Mpad, s->P, V, Mpad, s->D, dmu, dvar);
   GPX_TMP_FREE(Kxz, st); GPX_TMP_FREE(V, st);
   return rc;
+}
+
+/* joint samples of the latent function from the last sparse evaluation (posterior.py:238-270 with pred_var = Z, then
+ * gp.py:601-629): Sigma = K(Xnew) - K(Xnew, Z) W K(Z, Xnew) with W = woodbury_inv (shared with the predictive gradients),
+ * mu = K(Xnew, Z) woodbury_vector; V^T = K(Xnew, Z) W and the product term V^T K(Z, Xnew) on the DMMA GEMM */
+int gpx_sparse_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t Mn, const double* z, int64_t nz, int max_tries,
+                                 double* f, double* jitter_used) {
+  if (!c) GPX_FAIL("null argument");
+  if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to take the posterior from");
+  SparseState* s = c->sparse;
+  GPX_CHECK(joint_check(c, Xnew, Mn, z, nz, f, jitter_used, s->P));
+  const Kern k = s->kern();
+  GPX_CUDA(cudaSetDevice(c->device));
+  cudaStream_t st = c->st;
+  const long Mpad = s->Mpad;
+  PointSet pn;
+  GPX_CHECK(upload_points(c, k, Xnew, Mn, s->D, pn));
+  double* W = nullptr;
+  GPX_CHECK(woodbury_inv(c, &W));
+  const long L = pn.ld;
+  TmpBuf Kxz(st), Vt(st), prod(st), Kss(st), mu(st), part(st);
+  constexpr int RSPLIT = 64;
+  GPX_CHECK(Kxz.alloc((size_t)L * Mpad));
+  GPX_CHECK(Vt.alloc((size_t)L * Mpad));
+  GPX_CHECK(prod.alloc((size_t)L * L));
+  GPX_CHECK(Kss.alloc((size_t)L * L));
+  GPX_CHECK(mu.alloc((size_t)s->P * L));
+  GPX_CHECK(part.alloc((size_t)RSPLIT * s->P * L));
+  // K(Xnew, Z) with element (m, a) at m + a * L: test points thread-mapped, zero padded
+  GPX_CUDA(cudaMemsetAsync(Kxz.p, 0, (size_t)L * Mpad * 8, st));
+  GPX_CHECK(build_K(c, k, pn, s->zpts(), Kxz.p, L));
+  GPX_CHECK(launched(c));
+  GPX_CHECK(gemm_nt(c, Kxz.p, L, W, Mpad, Vt.p, L, L, Mpad, Mpad, 1, 0));          // V^T = K(Xnew, Z) W (W symmetric)
+  GPX_CHECK(gemm_nt(c, Vt.p, L, Kxz.p, L, prod.p, L, L, L, Mpad, 2, 0));           // V^T K(Z, Xnew), lower tiles
+  GPX_CHECK(launch_row_dot(Kxz.p, L, L, s->M, s->P, s->Cm, Mpad, RSPLIT, part.p, mu.p, st));   // mu = K(Xnew, Z) wv
+  GPX_CHECK(launched(c, 2));
+  GPX_CHECK(build_K(c, k, pn, pn, Kss.p, L));
+  GPX_CHECK(launched(c));
+  GPX_CHECK(joint_combine(c, Kss.p, L, 0, prod.p, L, 1, Mn, Mn, Kss.p, L, 1));      // Sigma in place of K(Xnew)
+  return joint_sample(c, Kss.p, L, Mn, mu.p, L, z, nz, nz / s->P, max_tries, f, jitter_used);
 }
 
 }  // extern "C"

@@ -67,5 +67,6 @@ def init_engine_comm(engine, group=None):
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     uid = exchange_unique_id(nccl_unique_id, group)
     _ffi.check(_ffi.lib().gpx_comm_init(engine._h, uid, rank, world), "gpx_comm_init")
+    engine.sharded = True   # the joint posterior (single-GPU on the device) takes the reference's host route
     engine.rank, engine.world = rank, world
     return engine

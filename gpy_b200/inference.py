@@ -40,6 +40,19 @@ class Gaussian(Parameterized):
             var = var + float(self.variance[0])
         return mu, var
 
+    def samples(self, gp, Y_metadata=None):
+        """gaussian.py:316-327: one draw N(f, variance) per entry of gp, in gp's flattened order. The reference loops with
+        np.random.normal(f_j, sqrt(variance), size=1); one vectorised call consumes numpy's legacy global stream in the
+        same order and gives the same values."""
+        gp = np.asarray(gp, dtype=np.float64)
+        scale = np.sqrt(np.asarray(self.variance.values, dtype=np.float64)).reshape(-1)
+        if scale.size != 1:
+            # HeteroscedasticGaussian inherits this method in the reference: normal(f_j, scale=sqrt(variance), size=1)
+            # with one variance per training point fails on the shape mismatch, and so does this restatement
+            raise ValueError("shape mismatch: Gaussian.samples draws with the whole variance vector (%d entries) as the "
+                             "scale of every entry" % scale.size)
+        return np.random.normal(gp.reshape(-1), scale[0], size=gp.size).reshape(gp.shape)
+
 
 class HeteroscedasticGaussian(Gaussian):
     """GPy.likelihoods.HeteroscedasticGaussian (gaussian.py:347-377): one noise variance per output index."""
@@ -107,6 +120,20 @@ class MixedNoise(Parameterized):
         if full_cov:
             return mu, var + np.eye(var.shape[0]) * _variance
         return mu, var + _variance.reshape(-1, 1)
+
+    def samples(self, gp, Y_metadata):
+        """mixed_noise.py:66-82: the rows of gp (N1 x N2) with output index j get N(f, variance_j) draws, group by group in
+        the order of np.unique, each group in its flattened order (the same stream as the reference's per-entry loop)"""
+        gp = np.asarray(gp, dtype=np.float64)
+        N1, N2 = gp.shape
+        Ysim = np.zeros((N1, N2))
+        ind = np.asarray(Y_metadata["output_index"]).flatten()
+        for j in np.unique(ind):
+            flt = ind == j
+            g = gp[flt, :]
+            scale = np.sqrt(float(self.likelihoods_list[j].variance[0]))
+            Ysim[flt, :] = np.random.normal(g.reshape(-1), scale, size=g.size).reshape(g.shape[0], N2)
+        return Ysim
 
     def predictive_variance(self, mu, sigma, Y_metadata):
         return self.gaussian_variance(Y_metadata) + sigma ** 2                                    # mixed_noise.py:52-54
@@ -178,6 +205,36 @@ class PosteriorExact(object):
             return HostPosterior(self.woodbury_chol, self.woodbury_vector, None)._raw_predict(kern, Xnew, pred_var, full_cov)
         self._check_fresh()
         return self._engine.predict(self._engine_X(kern, Xnew), full_cov=full_cov)
+
+    def _on_device(self, kern):
+        """the joint posterior of kern can come from the device: kern is the evaluated kernel (the mirror's, a plugin
+        kernel, or the reference's Add / Prod over plugin leaves, which the plugin keys by its flattened parts) and the
+        engine holds the whole factor (a sharded engine takes the reference's host route)"""
+        if getattr(self._engine, "sharded", False):
+            return False
+        if self._is_evaluated(kern):
+            return True
+        from .gpy_plugin import _composite_key
+        return not hasattr(kern, "_state_key") and _composite_key(kern) == self._kern_key
+
+    def covariance_between_points(self, kern, X, X1, X2):
+        """posterior.py:109-130: K(X1, X2) - K(X1, X) Ky^-1 K(X, X2). With the evaluated kernel one
+        gpx_posterior_covariance call (nothing of size N^2 reaches the host); another kernel, or a sharded engine, takes the
+        reference's formula on the fetched factor. An explicit X2 is built as kern.K(X1, X2) is, also when it equals X1;
+        X2 = None is the symmetric K(X1) form."""
+        if not self._on_device(kern):
+            return HostPosterior(self.woodbury_chol, self.woodbury_vector, None).covariance_between_points(kern, X, X1, X2)
+        self._check_fresh()
+        return self._engine.posterior_covariance(self._engine_X(kern, X1),
+                                                 None if X2 is None else self._engine_X(kern, X2))
+
+    def _posterior_samples(self, kern, Xnew, z):
+        """gp.py:601-629 on the device (gpx_posterior_samples): z (P S, M) standard normals, output-major -> f in z's
+        layout, or None when kern is not the evaluated kernel or the engine is sharded"""
+        if not self._on_device(kern):
+            return None
+        self._check_fresh()
+        return self._engine.posterior_samples(self._engine_X(kern, Xnew), z)[0]
 
     def _predictive_gradients(self, kern, Xnew):
         """gp.py:438-462 on the device (gpx_predictive_gradients) -> (dmu (M, D, P), dvar (M, D)) over the columns the
@@ -352,6 +409,14 @@ class HostPosterior(object):
         """posterior.py:183-203: (K + noise)^-1 from the factor (dpotri)"""
         from scipy.linalg import cho_solve
         return cho_solve((self.woodbury_chol, True), np.eye(self.woodbury_chol.shape[0]))
+
+    def covariance_between_points(self, kern, X, X1, X2):
+        """posterior.py:109-130 (two triangular solves with the factor)"""
+        from scipy.linalg import solve_triangular
+        X2 = X1 if X2 is None else X2
+        tmp1 = solve_triangular(self.woodbury_chol, kern.K(X, X1), lower=True)
+        tmp2 = solve_triangular(self.woodbury_chol, kern.K(X, X2), lower=True)
+        return kern.K(X1, X2) - tmp1.T.dot(tmp2)
 
     def _raw_predict(self, kern, Xnew, pred_var, full_cov=False):
         from scipy.linalg import solve_triangular

@@ -265,6 +265,104 @@ class GP(Parameterized):
         return mean_jac, var_jac
 
 
+    # ---- joint posterior: gp.py:601-652, 735-786 ---------------------------------------------------------------------
+    def _raw_posterior_covariance_between_points(self, X1, X2):
+        """gp.py:735-747: k(X1, X2) - k(X1, X) Ky^-1 k(X, X2), without normalizer or likelihood. On a device posterior with
+        the evaluated kernel this is one gpx_posterior_covariance call."""
+        return self.posterior.covariance_between_points(self.kern, self.X, np.asarray(X1, dtype=np.float64),
+                                                        np.asarray(X2, dtype=np.float64))
+
+    def posterior_covariance_between_points(self, X1, X2, Y_metadata=None, likelihood=None, include_likelihood=True):
+        """gp.py:750-786. include_likelihood: the covariance goes through likelihood.predictive_values(mean, cov,
+        full_cov=True) (a Gaussian adds its variance on the diagonal, which needs len(X1) == len(X2) as in the reference).
+        The mean handed over is that of _raw_predict(X1); the reference asks it for the full covariance as well and drops
+        it, here only the mean is computed. Normalizer: inverse_variance for one output, inverse_covariance (an output axis
+        appended) for several."""
+        cov = self._raw_posterior_covariance_between_points(X1, X2)
+        if include_likelihood:
+            mean, _ = self._raw_predict(np.asarray(X1, dtype=np.float64), full_cov=False)
+            if likelihood is None:
+                likelihood = self.likelihood
+            _, cov = likelihood.predictive_values(mean, cov, full_cov=True, Y_metadata=Y_metadata)
+        if self.normalizer is not None:
+            if self.output_dim > 1:
+                cov = self.normalizer.inverse_covariance(cov)
+            else:
+                cov = self.normalizer.inverse_variance(cov)
+        return cov
+
+    def posterior_samples_f(self, X, size=10, **predict_kwargs):
+        """gp.py:601-629: `size` joint samples of the latent function at X -> (Nnew, output_dim, size).
+
+        The standard normals come from numpy's legacy global RNG exactly as np.random.multivariate_normal(m, v, size)
+        draws them (one standard_normal((size, Nnew)) per output, in output order), so a seeded script consumes the same
+        stream as with the reference. With the evaluated kernel on a device posterior the rest is one
+        gpx_posterior_samples call: f = mu + chol(Sigma + jitter I) z, the jitter from jitchol's ladder (0 when Sigma
+        factors as it is). The reference uses numpy's SVD square root of Sigma instead; the samples have the same
+        distribution, not the same values. Another kern=, the generic inference path (mean function, K=) and a sharded
+        engine take the reference's host route (_raw_predict(full_cov=True), then np.random.multivariate_normal).
+
+        Normalizer: it is affine, so the device samples are mapped by inverse_mean, which equals sampling from
+        (inverse_mean(mu), std^2 Sigma). With several outputs the reference applies inverse_variance to the 2-D Nnew x Nnew
+        covariance, which broadcasts std^2 along its last axis: that raises ValueError unless Nnew == output_dim, and then
+        scales the columns of Sigma by the per-output variances, one output's std against another's. Here output d is drawn
+        with std_d^2 Sigma, the slice of inverse_covariance(Sigma) that posterior_covariance_between_points returns, on
+        both routes."""
+        X = np.asarray(X, dtype=np.float64)
+        M, P = X.shape[0], self.output_dim
+        kern = predict_kwargs.get("kern")
+        kern = self.kern if kern is None else kern
+        plain_kwargs = set(predict_kwargs) <= {"kern", "full_cov"}
+        if isinstance(self.posterior, PosteriorExact) and self.mean_function is None and plain_kwargs \
+                and self.posterior._on_device(kern):
+            z = draw_standard_normals(M, P, size)
+            f = self.posterior._posterior_samples(kern, X, z)
+            fsim = f.reshape(P, size, M).transpose(2, 0, 1)
+            if self.normalizer is not None:
+                fsim = self.normalizer.inverse_mean(fsim.transpose(0, 2, 1)).transpose(0, 2, 1)
+            return np.ascontiguousarray(fsim)
+        predict_kwargs["full_cov"] = True
+        m, v = self._raw_predict(X, **predict_kwargs)
+        return sample_normal(m, v, size, self.normalizer)
+
+    def posterior_samples(self, X, size=10, Y_metadata=None, likelihood=None, **predict_kwargs):
+        """gp.py:631-652: posterior_samples_f, then likelihood.samples per output (a Gaussian adds N(0, variance) per
+        entry) -> (Nnew, output_dim, size)"""
+        fsim = self.posterior_samples_f(X, size, **predict_kwargs)
+        return likelihood_samples(self.likelihood if likelihood is None else likelihood, fsim, Y_metadata)
+
+
+def draw_standard_normals(M, P, size):
+    """the standard normals np.random.multivariate_normal(m, v, size) draws for each of P outputs in turn (legacy global
+    RNG: one standard_normal((size, M)) per call) -> (P size, M), output-major"""
+    return np.concatenate([np.random.standard_normal((size, M)) for _ in range(P)], axis=0)
+
+
+def sample_normal(m, v, size, normalizer=None):
+    """gp.py:611-629 on the host: m (Nnew, P), v (Nnew, Nnew) -> (Nnew, P, size) with np.random.multivariate_normal; the
+    normalizer as GP.posterior_samples_f documents"""
+    m = np.asarray(m, dtype=np.float64)
+    P = m.shape[1]
+    if normalizer is not None:
+        m = normalizer.inverse_mean(m)
+        v = normalizer.inverse_variance(v) if P == 1 else normalizer.inverse_covariance(v)
+    fsim = np.empty((m.shape[0], P, size))
+    for d in range(P):
+        vd = v[:, :, d] if v.ndim == 3 else v
+        fsim[:, d, :] = np.random.multivariate_normal(m[:, d], vd, size).T
+    return fsim
+
+
+def likelihood_samples(likelihood, fsim, Y_metadata=None):
+    """gp.py:646-651: likelihood.samples on each output's Nnew x size slice"""
+    if fsim.ndim == 3:
+        for d in range(fsim.shape[1]):
+            fsim[:, d] = likelihood.samples(fsim[:, d], Y_metadata=Y_metadata)
+    else:
+        fsim = likelihood.samples(fsim, Y_metadata=Y_metadata)
+    return fsim
+
+
 def scatter_active_dims(kern, g, Q):
     """a single kernel's gradient over its active dims (axis 1) -> the full Q input columns, zero elsewhere, as
     Stationary.gradients_X scatters (kernel_slice_operations.py:138-150); a composite's already spans them"""

@@ -19,7 +19,8 @@ import numpy as np
 
 from . import _ffi
 from .inference import Gaussian, HeteroscedasticGaussian, _DataKey
-from .model import host_predictive_gradients, scatter_active_dims
+from .model import (draw_standard_normals, host_predictive_gradients, likelihood_samples, sample_normal,
+                    scatter_active_dims)
 from .kern import (RBF, RatQuad, StdPeriodic, Stationary, flatten_parts, part_descriptor, part_ngrad,
                    scatter_leaf_gradients, single_kernel)
 from .param import Logexp, Param, Parameterized
@@ -65,6 +66,12 @@ class LazySparsePosterior(object):
         if self._eng.sparse_serial != self._serial:
             raise RuntimeError("stale sparse posterior: the engine has evaluated other parameters since")
         return self._eng.sparse_predictive_gradients(Xnew)
+
+    def _posterior_samples(self, Xnew, z):
+        """gp.py:601-629 with the predictive variable Z on the device (gpx_sparse_posterior_samples) -> f in z's layout"""
+        if self._eng.sparse_serial != self._serial:
+            raise RuntimeError("stale sparse posterior: the engine has evaluated other parameters since")
+        return self._eng.sparse_posterior_samples(Xnew, z)[0]
 
     def materialise(self):
         for w in ("woodbury_vector", "woodbury_inv"):
@@ -311,6 +318,27 @@ class SparseGPRegression(Parameterized):
                                  "include_likelihood=False (gp_heteroscedastic_regression.py:13-15)")
             mu, var = self.likelihood.predictive_values(mu, var, full_cov, Y_metadata=Y_metadata)
         return mu, var
+
+    def posterior_samples_f(self, X, size=10, kern=None):
+        """gp.py:601-629 with the predictive variable Z (sparse_gp.py:52-54) -> (Nnew, output_dim, size). The standard
+        normals are drawn as GP.posterior_samples_f draws them; with the evaluated kernel the rest is one
+        gpx_sparse_posterior_samples call (Sigma = K(X) - K(X, Z) W K(Z, X) through its Cholesky factor and jitchol's
+        ladder), another kern= takes the reference's host route. posterior_covariance_between_points is not offered: the
+        reference raises for a sparse posterior (posterior.py:119-120)."""
+        X = np.asarray(X, dtype=np.float64)
+        if kern is None or kern is self.kern:
+            M, P = X.shape[0], self.Y.shape[1]
+            Xs = self.kern._slice_X(X) if single_kernel(self.kern) else np.ascontiguousarray(X)
+            z = draw_standard_normals(M, P, size)
+            f = self.posterior._posterior_samples(Xs, z)
+            return np.ascontiguousarray(f.reshape(P, size, M).transpose(2, 0, 1))
+        m, v = self.posterior._raw_predict(kern, X, self.Z.values, full_cov=True)
+        return sample_normal(m, v, size)
+
+    def posterior_samples(self, X, size=10, Y_metadata=None, likelihood=None, kern=None):
+        """gp.py:631-652: posterior_samples_f, then likelihood.samples per output"""
+        fsim = self.posterior_samples_f(X, size, kern=kern)
+        return likelihood_samples(self.likelihood if likelihood is None else likelihood, fsim, Y_metadata)
 
     def predictive_gradients(self, Xnew, kern=None):
         """gp.py:418-474 with the predictive variable Z (sparse_gp.py:52-54): with the evaluated kernel one

@@ -158,6 +158,51 @@ int gpx_predict(gpx_ctx* ctx, const double* Xnew, int64_t M, int full_cov, doubl
 int gpx_predictive_gradients(gpx_ctx* ctx, const double* Xnew, int64_t M, double* dmu, double* dvar);
 int gpx_sparse_predictive_gradients(gpx_ctx* ctx, const double* Xnew, int64_t M, double* dmu, double* dvar);
 
+/* The joint posterior of the last evaluation on the device (single-GPU; a context with a communicator attached gets -2).
+ *
+ * gpx_posterior_covariance : after gpx_exact_eval / _het / _multi. Posterior.covariance_between_points (posterior.py:109-130):
+ *   cov (M1 x M2 row-major) = K(X1, X2) - K(X1, X) Ky^-1 K(X, X2) with the evaluation's kernel and factor; X1 (M1 x D) and
+ *   X2 (M2 x D) row-major with the D of gpx_set_data. X2 == NULL means X2 = X1: cov is then exactly symmetric and K(X1, X1)
+ *   has the exact zero distance on its diagonal, as gpx_kern_K with X2 = NULL. An explicit X2, even one equal to X1, is
+ *   built the reference's way: kern.K(X1, X2) does not force coincident points to zero distance (this matters for
+ *   Exponential, whose k is first order in r, where |x|^2 + |x'|^2 - 2 x.x' leaves r ~ 1e-8 at coincident points).
+ *   Route: one K-build of K([X1; X2], X) (X2 stacked at a tile boundary), L^-1 = U^T extracted into a temporary,
+ *   T^T = K(X*, X) L^-T on the DMMA GEMM (B lower triangular, N^2 (M1 + M2) flops), T1^T T2 on the DMMA GEMM, one K-build
+ *   of K(X*, X*) and one combine. Launches: 7.
+ * gpx_posterior_samples / gpx_sparse_posterior_samples : after an exact (gpx_exact_eval / _het / _multi) or a sparse
+ *   (gpx_sparse_eval / _het / _multi) evaluation, every kernel either accepts. GP.posterior_samples_f (gp.py:601-629) with
+ *   the latent predictive covariance at Xnew (M x D row-major)
+ *     exact : Sigma = K(Xnew) - K(Xnew, X) Ky^-1 K(X, Xnew),  mu = K(Xnew, X) alpha          (posterior.py:273-302)
+ *     sparse: Sigma = K(Xnew) - K(Xnew, Z) W K(Z, Xnew),      mu = K(Xnew, Z) woodbury_vector (posterior.py:238-270)
+ *   with W = woodbury_inv, formed by the first of gpx_sparse_predictive_gradients / gpx_sparse_posterior_samples after an
+ *   evaluation and kept for both. Sigma is factored with jitchol's rules (util/linalg.py:56-75): first plain, then with
+ *   mean(diag) 1e-6 10^k added, k < max_tries; *jitter_used reports what was added. z holds nz = P S standard-normal
+ *   vectors of length M, row-major nz x M and ordered output-major (S vectors for output 0, then S for output 1, ...), as
+ *   numpy's legacy RNG draws them for np.random.multivariate_normal(m, v, S) once per output; f has the same layout:
+ *   f_j = mu[:, j / S] + L_Sigma z_j. The samples are drawn from N(mu, Sigma + jitter I) through the Cholesky factor; the
+ *   reference samples Sigma itself through numpy's SVD, with no jitter. Sigma is factored in a child context that the
+ *   calling context creates on first use and owns. Returns > 0 (the leading minor) when Sigma is not positive definite
+ *   after the ladder, as gpx_pdinv; -2 when there is no evaluation of the right kind, M < 1, nz < 1, nz is not a multiple
+ *   of P, a pointer is null or a communicator is attached.
+ *   Launches: exact 13 + F, sparse 12 + F, plus 5 on the first sparse call after an evaluation, which forms W. F is what
+ *   gpx_pdinv of an M x M matrix that returns no matrices launches on a fresh context, binding included; one fewer when
+ *   the child context holds an M x M workspace already.
+ * None of the three entries changes anything that gpx_get, gpx_sparse_get, gpx_predict, gpx_predictive_gradients,
+ * gpx_sparse_predictive_gradients or gpx_get_stats return, on success or failure; the evaluation's factor is only read.
+ * Temporaries are stream-ordered (the pool of gpx_predict); an exhausted device returns -1 with a message. Peak bytes of
+ * the temporaries, with Ls the test points padded to 128 (M1p + M2p for a cross-covariance, M1p = M1 padded), Np = N
+ * padded, Mz = the inducing points padded:
+ *   exact  : 8 (Np^2 + 2 Ls Np + 65 P Ls) while T^T is formed, then at most 8 (Ls Np + M1p M2p) and
+ *            8 (Ls^2 + M1p M2p + M1 M2); N = 32768 and M = 4096: 10.7 GB beside the evaluation's own workspace
+ *   sparse : 8 (2 Ls Mz + 2 Ls^2 + 65 P Ls)
+ *   sampling adds 8 (Ls^2 + 2 nzp Ls + 2 nz M) (nzp = nz padded) and, in the child context, the workspace gpx_set_data
+ *   allocates for M points. */
+int gpx_posterior_covariance(gpx_ctx* ctx, const double* X1, int64_t M1, const double* X2, int64_t M2, double* cov);
+int gpx_posterior_samples(gpx_ctx* ctx, const double* Xnew, int64_t M, const double* z, int64_t nz, int max_tries,
+                          double* f, double* jitter_used);
+int gpx_sparse_posterior_samples(gpx_ctx* ctx, const double* Xnew, int64_t M, const double* z, int64_t nz,
+                                 int max_tries, double* f, double* jitter_used);
+
 /* Standalone kernel plugin calls (no context needed beyond a device; ctx may be NULL -> device 0 scratch context).
  * Replaces Stationary.K (stationary.py:105-168): out is N x M ROW-major (what Kern.K returns to NumPy callers).
  * out == NULL: build on the device only and report the kernel time via gpx_get_stats (kbuild_ms, kbuild_bytes). */
