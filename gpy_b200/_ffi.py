@@ -100,6 +100,7 @@ EXPORTS = {
     "gpx_sparse_eval": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64,
                                        ctypes.c_double, _dp, _dp, _dp]),
     "gpx_sparse_get": (ctypes.c_int, [_vp, ctypes.c_int, _dp]),
+    "gpx_sparse_predict": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
     "gpx_sparse_eval_multi": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64,
                                              ctypes.c_double, _dp, _dp, _dp, _dp, _dp]),
     "gpx_sparse_eval_het": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64,
@@ -419,6 +420,20 @@ class Engine(object):
         out = np.empty((self.sM, self.sP)) if which == 0 else np.empty((self.sM, self.sM), order="F")
         check(self._L.gpx_sparse_get(self._h, which, _ptr(out)), "gpx_sparse_get")
         return out
+
+    def sparse_predict(self, Xnew, full_cov=False):
+        """Posterior._raw_predict (posterior.py:220-248) of the last sparse evaluation with the predictive variable Z ->
+        (mu (M, P), var (M, 1), clipped at 1e-15, or the full covariance (M, M)); the diagonal streams over chunks of
+        test points (gpx_sparse_predict)"""
+        Xnew = _f64(Xnew)
+        if Xnew.ndim != 2 or (self.sD and Xnew.shape[1] != self.sD):   # sD == 0: no data yet, the entry rejects the call
+            raise ValueError("Xnew must be M x %d" % self.sD)
+        M = Xnew.shape[0]
+        mu = np.empty((M, self.sP))
+        var = np.empty((M, M), order="F") if full_cov else np.empty(M)
+        check(self._L.gpx_sparse_predict(self._h, _ptr(Xnew), M, int(bool(full_cov)), _ptr(mu), _ptr(var)),
+              "gpx_sparse_predict")
+        return mu, (var if full_cov else var[:, None])
 
     def stats(self):
         s = GpxStats()

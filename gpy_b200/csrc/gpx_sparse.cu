@@ -746,8 +746,8 @@ int gpx_sparse_get(gpx_ctx* c, int which, double* out) {
 }  // extern "C"
 
 // woodbury_inv W of the current evaluation in mm[9], formed as gpx_sparse_get(1) forms it by the first caller after an
-// evaluation (predictive gradients or samples) and kept for the later ones: gpx_sparse_get(1) writes the same W into mm[9],
-// nothing else writes it
+// evaluation (predictive gradients, samples or predict) and kept for the later ones: gpx_sparse_get(1) writes the same W
+// into mm[9], nothing else writes it
 static int woodbury_inv(gpx_ctx* c, double** W) {
   SparseState* s = c->sparse;
   double *Um = s->mm[1], *UB = s->mm[6], *T = s->mm[3], *DB = s->mm[8];
@@ -802,25 +802,20 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
   return rc;
 }
 
-/* joint samples of the latent function from the last sparse evaluation (posterior.py:238-270 with pred_var = Z, then
- * gp.py:601-629): Sigma = K(Xnew) - K(Xnew, Z) W K(Z, Xnew) with W = woodbury_inv (shared with the predictive gradients),
- * mu = K(Xnew, Z) woodbury_vector; V^T = K(Xnew, Z) W and the product term V^T K(Z, Xnew) on the DMMA GEMM */
-int gpx_sparse_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t Mn, const double* z, int64_t nz, int max_tries,
-                                 double* f, double* jitter_used) {
-  if (!c) GPX_FAIL("null argument");
-  if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to take the posterior from");
+}  // extern "C"
+
+// The latent predictive covariance and mean of the last sparse evaluation at the prepared test points pn (posterior.py:
+// 220-238 with pred_var = Z): Sigma = K(Xnew) - K(Xnew, Z) W K(Z, Xnew) into Kss (pn.ld^2, column-major, exactly
+// symmetric: the lower tiles of the product term mirrored), mu = K(Xnew, Z) woodbury_vector into mu ([P][pn.ld]).
+// V^T = K(Xnew, Z) W and V^T K(Z, Xnew) run on the DMMA GEMM. Launches: 7, plus 5 when it forms W.
+static int sparse_joint(gpx_ctx* c, const PointSet& pn, TmpBuf& Kss, TmpBuf& mu) {
   SparseState* s = c->sparse;
-  GPX_CHECK(joint_check(c, Xnew, Mn, z, nz, f, jitter_used, s->P));
   const Kern k = s->kern();
-  GPX_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->st;
-  const long Mpad = s->Mpad;
-  PointSet pn;
-  GPX_CHECK(upload_points(c, k, Xnew, Mn, s->D, pn));
+  const long Mpad = s->Mpad, L = pn.ld;
   double* W = nullptr;
   GPX_CHECK(woodbury_inv(c, &W));
-  const long L = pn.ld;
-  TmpBuf Kxz(st), Vt(st), prod(st), Kss(st), mu(st), part(st);
+  TmpBuf Kxz(st), Vt(st), prod(st), part(st);
   constexpr int RSPLIT = 64;
   GPX_CHECK(Kxz.alloc((size_t)L * Mpad));
   GPX_CHECK(Vt.alloc((size_t)L * Mpad));
@@ -838,8 +833,123 @@ int gpx_sparse_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t Mn, con
   GPX_CHECK(launched(c, 2));
   GPX_CHECK(build_K(c, k, pn, pn, Kss.p, L));
   GPX_CHECK(launched(c));
-  GPX_CHECK(joint_combine(c, Kss.p, L, 0, prod.p, L, 1, Mn, Mn, Kss.p, L, 1));      // Sigma in place of K(Xnew)
-  return joint_sample(c, Kss.p, L, Mn, mu.p, L, z, nz, nz / s->P, max_tries, f, jitter_used);
+  return joint_combine(c, Kss.p, L, 0, prod.p, L, 1, pn.n, pn.n, Kss.p, L, 1);    // Sigma in place of K(Xnew)
+}
+
+// var[m] = max(kdiag - sum_{a < M} Vt(m, a) Kxz(m, a), 1e-15) for the n rows of one chunk (posterior.py:244-248: the
+// reference's rowsum((K(Xnew, Z) W) o K(Xnew, Z)) and its clip; a NaN stays NaN as under np.clip). Both operands are
+// column-major with leading dimension ld. A row's sum depends on M alone: 8 column slices of ceil(M / 8), each summed in
+// column order by one thread, then added in slice order, so a row gets the same bits in any chunk at any position.
+constexpr int VAR_ROWS = 32, VAR_SLICES = 8;
+__global__ void __launch_bounds__(VAR_ROWS * VAR_SLICES) sparse_var_kernel(const double* __restrict__ Kxz,
+                                                                           const double* __restrict__ Vt, long ld, long n,
+                                                                           long M, double kdiag, double* __restrict__ var) {
+  __shared__ double sh[VAR_SLICES][VAR_ROWS];
+  const long row = (long)blockIdx.x * VAR_ROWS + threadIdx.x;
+  const long chunk = (M + VAR_SLICES - 1) / VAR_SLICES, a0 = threadIdx.y * chunk;
+  const long a1 = a0 + chunk < M ? a0 + chunk : M;
+  double acc = 0.0;
+  if (row < n)
+    for (long a = a0; a < a1; a++) acc = fma(Vt[row + a * ld], Kxz[row + a * ld], acc);
+  sh[threadIdx.y][threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.y != 0 || row >= n) return;
+  double sum = sh[0][threadIdx.x];
+#pragma unroll
+  for (int q = 1; q < VAR_SLICES; q++) sum += sh[q][threadIdx.x];
+  const double v = kdiag - sum;
+  var[row] = v < 1e-15 ? 1e-15 : v;
+}
+
+namespace {
+// rows of one chunk of the diagonal prediction: the largest multiple of 128 whose temporaries, bounded by
+// 16 Mpad + 520 P + 1096 bytes per row (K(Xc, Z) and V^T, the mean's 64 partial sums, mean and variance, the uploaded and
+// prepared points at D, stacked dims and norms <= 64), fit in the 1 GiB the stream-ordered pool keeps cached (gpx_create);
+// never fewer than 128, never more than the test points padded to 128 (include/gpx.h states the same rule)
+long predict_chunk_rows(long Mpad, int P, long Mn) {
+  const long per_row = 16 * Mpad + 520 * (long)P + 1096;
+  const long Lc = std::max<long>(TILE, (1l << 30) / per_row / TILE * TILE);
+  return std::min<long>(Lc, (Mn + TILE - 1) / TILE * TILE);
+}
+}  // namespace
+
+extern "C" {
+
+/* joint samples of the latent function from the last sparse evaluation (posterior.py:238-270 with pred_var = Z, then
+ * gp.py:601-629): Sigma and mu from sparse_joint (W = woodbury_inv shared with the predictive gradients and predict) */
+int gpx_sparse_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t Mn, const double* z, int64_t nz, int max_tries,
+                                 double* f, double* jitter_used) {
+  if (!c) GPX_FAIL("null argument");
+  if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to take the posterior from");
+  SparseState* s = c->sparse;
+  GPX_CHECK(joint_check(c, Xnew, Mn, z, nz, f, jitter_used, s->P));
+  GPX_CUDA(cudaSetDevice(c->device));
+  PointSet pn;
+  GPX_CHECK(upload_points(c, s->kern(), Xnew, Mn, s->D, pn));
+  TmpBuf Kss(c->st), mu(c->st);
+  GPX_CHECK(sparse_joint(c, pn, Kss, mu));
+  return joint_sample(c, Kss.p, pn.ld, Mn, mu.p, pn.ld, z, nz, nz / s->P, max_tries, f, jitter_used);
+}
+
+/* SparseGP.predict's latent part (GPy/core/gp.py:303 -> posterior.py:220-248 with pred_var = Z): mu = K(Xnew, Z)
+ * woodbury_vector, and the diagonal variance (clipped at 1e-15), streamed over chunks of test points, or the full covariance
+ * in one pass. Every rank of a communicator holds the same posterior and predicts the points it is given, alone. */
+int gpx_sparse_predict(gpx_ctx* c, const double* Xnew, int64_t Mn, int full_cov, double* mu, double* var) {
+  if (!c || !Xnew || !mu || !var) GPX_FAIL("null argument");
+  if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to predict from");
+  if (Mn < 1) GPX_FAIL("empty Xnew");
+  SparseState* s = c->sparse;
+  const Kern k = s->kern();
+  const int P = s->P;
+  GPX_CUDA(cudaSetDevice(c->device));
+  cudaStream_t st = c->st;
+  if (full_cov) {
+    PointSet pn;
+    GPX_CHECK(upload_points(c, k, Xnew, Mn, s->D, pn));
+    TmpBuf Kss(st), mud(st);
+    GPX_CHECK(sparse_joint(c, pn, Kss, mud));
+    const long L = pn.ld;
+    std::vector<double> h((size_t)P * L);
+    GPX_CUDA(cudaMemcpyAsync(h.data(), mud.p, h.size() * 8, cudaMemcpyDeviceToHost, st));
+    GPX_CUDA(cudaMemcpy2DAsync(var, Mn * 8, Kss.p, L * 8, (size_t)Mn * 8, Mn, cudaMemcpyDeviceToHost, st));
+    if (cudaStreamSynchronize(st) != cudaSuccess) GPX_FAIL_DEVICE("gpx_sparse_predict");
+    for (long m = 0; m < Mn; m++)
+      for (int q = 0; q < P; q++) mu[m * P + q] = h[(size_t)q * L + m];
+    return 0;
+  }
+  const long Mpad = s->Mpad, Lc = predict_chunk_rows(Mpad, P, Mn);
+  double* W = nullptr;
+  GPX_CHECK(woodbury_inv(c, &W));
+  constexpr int RSPLIT = 64;
+  TmpBuf Kxz(st), Vt(st), part(st), red(st);   // red: [P][Lc] means, then [Lc] variances
+  GPX_CHECK(Kxz.alloc((size_t)Lc * Mpad));
+  GPX_CHECK(Vt.alloc((size_t)Lc * Mpad));
+  GPX_CHECK(part.alloc((size_t)RSPLIT * P * Lc));
+  GPX_CHECK(red.alloc((size_t)(P + 1) * Lc));
+  std::vector<double> h((size_t)P * Lc);
+  for (long m0 = 0; m0 < Mn; m0 += Lc) {
+    const long n = std::min<long>(Lc, Mn - m0);
+    PointSet pn;
+    GPX_CHECK(upload_points(c, k, Xnew + (size_t)m0 * s->D, n, s->D, pn));
+    const long L = pn.ld;   // this chunk's rows padded to 128 (<= Lc)
+    // K(Xc, Z) with element (m, a) at m + a * L, zero padded; V^T = K(Xc, Z) W
+    GPX_CUDA(cudaMemsetAsync(Kxz.p, 0, (size_t)L * Mpad * 8, st));
+    GPX_CHECK(build_K(c, k, pn, s->zpts(), Kxz.p, L));
+    GPX_CHECK(launched(c));
+    GPX_CHECK(gemm_nt(c, Kxz.p, L, W, Mpad, Vt.p, L, L, Mpad, Mpad, 1, 0));
+    GPX_CHECK(launch_row_dot(Kxz.p, L, L, s->M, P, s->Cm, Mpad, RSPLIT, part.p, red.p, st));   // mu ([P][L])
+    GPX_CHECK(launched(c, 2));
+    double* vd = red.p + (size_t)P * L;
+    sparse_var_kernel<<<(unsigned)(L / VAR_ROWS), dim3(VAR_ROWS, VAR_SLICES), 0, st>>>(Kxz.p, Vt.p, L, n, s->M, s->kdiag,
+                                                                                       vd);
+    GPX_CHECK(launched(c));
+    GPX_CUDA(cudaMemcpyAsync(h.data(), red.p, (size_t)P * L * 8, cudaMemcpyDeviceToHost, st));
+    GPX_CUDA(cudaMemcpyAsync(var + m0, vd, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    if (cudaStreamSynchronize(st) != cudaSuccess) GPX_FAIL_DEVICE("gpx_sparse_predict");
+    for (long m = 0; m < n; m++)
+      for (int q = 0; q < P; q++) mu[(m0 + m) * P + q] = h[(size_t)q * L + m];
+  }
+  return 0;
 }
 
 }  // extern "C"

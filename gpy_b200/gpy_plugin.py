@@ -354,7 +354,7 @@ def _make_vardtc(base, kernel_types, ffi):
             dlen = np.atleast_1d(gk[1:])
             knm = SparseDeviceGradient(key, "knm", (N, M), gk[0] - dL_dKdiag.sum(), dlen, dZ)
             kmm = SparseDeviceGradient(key, "kmm", (M, M), 0.0, np.zeros_like(dlen), np.zeros_like(dZ))
-            post = LazySparsePosterior(eng)
+            post = LazySparsePosterior(eng, key, Zs)
             return post, lml, {"dL_dKmm": kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": knm, "dL_dthetaL": dL_dthetaL,
                                "dL_dm": None}
 
@@ -391,8 +391,8 @@ def _make_vardtc(base, kernel_types, ffi):
             key = _composite_key(kern)
             h_knm = SparseDeviceGradient(key, "knm", (N, M), None, None, dZ, part_grads=knm)
             h_kmm = SparseDeviceGradient(key, "kmm", (M, M), None, None, np.zeros_like(dZ), part_grads=zeros)
-            return LazySparsePosterior(eng), lml, {"dL_dKmm": h_kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": h_knm,
-                                                   "dL_dthetaL": dL_dthetaL, "dL_dm": None}
+            return LazySparsePosterior(eng, key, Zs), lml, {"dL_dKmm": h_kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": h_knm,
+                                                           "dL_dthetaL": dL_dthetaL, "dL_dm": None}
 
     B200VarDTC.__name__ = B200VarDTC.__qualname__ = "VarDTC"
     return B200VarDTC

@@ -139,6 +139,17 @@ class MixedNoise(Parameterized):
         return self.gaussian_variance(Y_metadata) + sigma ** 2                                    # mixed_noise.py:52-54
 
 
+def evaluated_kernel(kern, key):
+    """kern is the kernel of the device evaluation keyed `key`: the mirror's or a plugin kernel by its own state key, the
+    reference's Add / Prod over plugin leaves by the key the plugin gives its flattened parts"""
+    own = kern._state_key() if hasattr(kern, "_state_key") else (
+        kern._gpx_state_key() if hasattr(kern, "_gpx_state_key") else composite_state_key(kern))
+    if own == key:
+        return True
+    from .gpy_plugin import _composite_key
+    return not hasattr(kern, "_state_key") and _composite_key(kern) == key
+
+
 class PosteriorExact(object):
     """Posterior whose big members live in HBM and are fetched lazily (posterior.py:21-77 constructor contract:
     woodbury_chol = L, woodbury_vector = alpha, K = noise-free kernel matrix)."""
@@ -207,15 +218,11 @@ class PosteriorExact(object):
         return self._engine.predict(self._engine_X(kern, Xnew), full_cov=full_cov)
 
     def _on_device(self, kern):
-        """the joint posterior of kern can come from the device: kern is the evaluated kernel (the mirror's, a plugin
-        kernel, or the reference's Add / Prod over plugin leaves, which the plugin keys by its flattened parts) and the
+        """the joint posterior of kern can come from the device: kern is the evaluated kernel (evaluated_kernel) and the
         engine holds the whole factor (a sharded engine takes the reference's host route)"""
         if getattr(self._engine, "sharded", False):
             return False
-        if self._is_evaluated(kern):
-            return True
-        from .gpy_plugin import _composite_key
-        return not hasattr(kern, "_state_key") and _composite_key(kern) == self._kern_key
+        return self._kern_key is None or evaluated_kernel(kern, self._kern_key)
 
     def covariance_between_points(self, kern, X, X1, X2):
         """posterior.py:109-130: K(X1, X2) - K(X1, X) Ky^-1 K(X, X2). With the evaluated kernel one

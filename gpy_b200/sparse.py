@@ -18,11 +18,11 @@ attached to a NCCL communicator, X and Y are this rank's rows (gpy_b200.dist.sha
 import numpy as np
 
 from . import _ffi
-from .inference import Gaussian, HeteroscedasticGaussian, _DataKey
+from .inference import Gaussian, HeteroscedasticGaussian, PosteriorExact, _DataKey, evaluated_kernel
 from .model import (draw_standard_normals, host_predictive_gradients, likelihood_samples, sample_normal,
                     scatter_active_dims)
-from .kern import (RBF, RatQuad, StdPeriodic, Stationary, flatten_parts, part_descriptor, part_ngrad,
-                   scatter_leaf_gradients, single_kernel)
+from .kern import (RBF, RatQuad, StdPeriodic, Stationary, composite_state_key, flatten_parts, part_descriptor,
+                   part_ngrad, scatter_leaf_gradients, single_kernel)
 from .param import Logexp, Param, Parameterized
 
 CONST_JITTER = 1e-8  # var_dtc.py:24
@@ -44,15 +44,22 @@ class SparsePosterior(object):
 
 
 class LazySparsePosterior(object):
-    """Posterior of the last gpx_sparse_eval; its arrays are produced on the device on first touch (var_dtc.py:201-214)."""
+    """Posterior of the last gpx_sparse_eval; its arrays are produced on the device on first touch (var_dtc.py:201-214).
+    kern_key and Z (as the evaluation sliced it) describe the evaluation, so that _raw_predict can tell when the device
+    holds what a prediction needs; without them every prediction takes the host route."""
 
-    def __init__(self, engine):
+    def __init__(self, engine, kern_key=None, Z=None):
         self._eng, self._serial, self._c = engine, engine.sparse_serial, {}
+        self._kern_key = kern_key
+        self._Z = None if Z is None else np.array(Z, dtype=np.float64, copy=True)
+
+    def _check_fresh(self):
+        if self._eng.sparse_serial != self._serial:
+            raise RuntimeError("stale sparse posterior: the engine has evaluated other parameters since")
 
     def _get(self, what):
         if what not in self._c:
-            if self._eng.sparse_serial != self._serial:
-                raise RuntimeError("stale sparse posterior: the engine has evaluated other parameters since")
+            self._check_fresh()
             self._c[what] = self._eng.sparse_get(what)
         return self._c[what]
 
@@ -63,14 +70,12 @@ class LazySparsePosterior(object):
 
     def _predictive_gradients(self, Xnew):
         """gp.py:438-462 with the predictive variable Z on the device (gpx_sparse_predictive_gradients)"""
-        if self._eng.sparse_serial != self._serial:
-            raise RuntimeError("stale sparse posterior: the engine has evaluated other parameters since")
+        self._check_fresh()
         return self._eng.sparse_predictive_gradients(Xnew)
 
     def _posterior_samples(self, Xnew, z):
         """gp.py:601-629 with the predictive variable Z on the device (gpx_sparse_posterior_samples) -> f in z's layout"""
-        if self._eng.sparse_serial != self._serial:
-            raise RuntimeError("stale sparse posterior: the engine has evaluated other parameters since")
+        self._check_fresh()
         return self._eng.sparse_posterior_samples(Xnew, z)[0]
 
     def materialise(self):
@@ -78,7 +83,21 @@ class LazySparsePosterior(object):
             self._get(w)
         return self
 
-    _raw_predict = SparsePosterior._raw_predict
+    def _on_device(self, kern, pred_var):
+        """the prediction can come from the device: kern is the evaluated kernel (inference.evaluated_kernel), pred_var
+        is the evaluated Z once sliced the same way, and the engine has gpx_sparse_predict"""
+        return (self._kern_key is not None and getattr(self._eng, "sparse_predict", None) is not None
+                and evaluated_kernel(kern, self._kern_key)
+                and np.array_equal(PosteriorExact._engine_X(kern, pred_var), self._Z))
+
+    def _raw_predict(self, kern, Xnew, pred_var, full_cov=False):
+        """posterior.py:220-248 with pred_var = Z (sparse_gp.py:52-54). With the evaluated kernel and Z one
+        gpx_sparse_predict call (the diagonal clipped at 1e-15 as the reference clips it); otherwise the formula on the
+        fetched woodbury arrays (SparsePosterior._raw_predict)."""
+        if not self._on_device(kern, pred_var):
+            return SparsePosterior._raw_predict(self, kern, Xnew, pred_var, full_cov)
+        self._check_fresh()
+        return self._eng.sparse_predict(PosteriorExact._engine_X(kern, Xnew), full_cov=full_cov)
 
 
 class VarDTC(object):
@@ -138,13 +157,13 @@ class VarDTC(object):
                     raise ValueError("one noise variance per data point expected")
                 lml, grad, dZ, dR = eng.sparse_eval_het(kind, ard, var, ls, Zs, gv.reshape(-1))
                 dL_dthetaL = likelihood.exact_inference_gradients(dR, Y_metadata)         # var_dtc.py:176
-                return LazySparsePosterior(eng), float(lml), {"dvariance": grad[0], "dlengthscale": grad[1:], "dZ": dZ,
-                                                              "dL_dthetaL": dL_dthetaL, "num_data": num_data}
+                return LazySparsePosterior(eng, kern._state_key(), Zs), float(lml), {
+                    "dvariance": grad[0], "dlengthscale": grad[1:], "dZ": dZ, "dL_dthetaL": dL_dthetaL, "num_data": num_data}
         elif np.size(precision) > 1:
             pv = np.asarray(precision, dtype=np.float64).reshape(-1)
             lml, grad, dZ, dR = eng.sparse_eval_het(kind, ard, var, ls, Zs, 1.0 / pv)
-            return LazySparsePosterior(eng), float(lml), {"dvariance": grad[0], "dlengthscale": grad[1:], "dZ": dZ,
-                                                          "dL_dthetaL": dR, "num_data": num_data}
+            return LazySparsePosterior(eng, kern._state_key(), Zs), float(lml), {
+                "dvariance": grad[0], "dlengthscale": grad[1:], "dZ": dZ, "dL_dthetaL": dR, "num_data": num_data}
         noise_var = None
         if precision is None:
             noise_var = float(np.squeeze(np.asarray(likelihood.gaussian_variance(Y_metadata))))
@@ -152,7 +171,7 @@ class VarDTC(object):
                                       self.const_jitter)                                   # var_dtc.py:79-80
         beta = float(precision)
         lml, grad, dZ = eng.sparse_eval(kind, ard, var, ls, Zs, noise_var if noise_var is not None else 1.0 / beta)
-        post = LazySparsePosterior(eng)
+        post = LazySparsePosterior(eng, kern._state_key(), Zs)
         return post, float(lml), {"dvariance": grad[0], "dlengthscale": grad[1:-1], "dZ": dZ,
                                   "dL_dthetaL": float(grad[-1]), "num_data": num_data}
 
@@ -187,8 +206,8 @@ class VarDTC(object):
             dL_dthetaL = likelihood.exact_inference_gradients(out[3], Y_metadata) if precision is None else out[3]
         else:
             dL_dthetaL = float(grad[-1])
-        return LazySparsePosterior(eng), float(lml), {"part_grads": blocks, "dZ": dZ, "dL_dthetaL": dL_dthetaL,
-                                                      "num_data": num_data}
+        return LazySparsePosterior(eng, composite_state_key(kern), Zs), float(lml), {
+            "part_grads": blocks, "dZ": dZ, "dL_dthetaL": dL_dthetaL, "num_data": num_data}
 
 
 class SparseGPRegression(Parameterized):
@@ -309,15 +328,22 @@ class SparseGPRegression(Parameterized):
         self.optimizer_array = x
         return ok
 
-    def predict(self, Xnew, full_cov=False, include_likelihood=True, Y_metadata=None):
-        """gp.py:290-365 with the sparse posterior (predictive variable = Z)."""
-        mu, var = self.posterior._raw_predict(self.kern, np.asarray(Xnew, dtype=np.float64), self.Z.values, full_cov)
+    def predict(self, Xnew, full_cov=False, include_likelihood=True, Y_metadata=None, kern=None, likelihood=None):
+        """gp.py:290-365 with the sparse posterior (predictive variable = Z). With the evaluated kernel the latent part is
+        one gpx_sparse_predict call; another kern= takes the reference's formula on the fetched woodbury arrays."""
+        kern = self.kern if kern is None else kern
+        mu, var = self.posterior._raw_predict(kern, np.asarray(Xnew, dtype=np.float64), self.Z.values, full_cov)
         if include_likelihood:
-            if isinstance(self.likelihood, HeteroscedasticGaussian) and Y_metadata is None:
+            likelihood = self.likelihood if likelihood is None else likelihood
+            if isinstance(likelihood, HeteroscedasticGaussian) and Y_metadata is None:
                 raise ValueError("a heteroscedastic likelihood needs Y_metadata (output_index) for the new points, or "
                                  "include_likelihood=False (gp_heteroscedastic_regression.py:13-15)")
-            mu, var = self.likelihood.predictive_values(mu, var, full_cov, Y_metadata=Y_metadata)
+            mu, var = likelihood.predictive_values(mu, var, full_cov, Y_metadata=Y_metadata)
         return mu, var
+
+    def predict_noiseless(self, Xnew, full_cov=False, Y_metadata=None, kern=None):
+        """gp.py:367-393: predict without the likelihood's variance"""
+        return self.predict(Xnew, full_cov, include_likelihood=False, Y_metadata=Y_metadata, kern=kern)
 
     def posterior_samples_f(self, X, size=10, kern=None):
         """gp.py:601-629 with the predictive variable Z (sparse_gp.py:52-54) -> (Nnew, output_dim, size). The standard

@@ -174,8 +174,8 @@ int gpx_sparse_predictive_gradients(gpx_ctx* ctx, const double* Xnew, int64_t M,
  *   the latent predictive covariance at Xnew (M x D row-major)
  *     exact : Sigma = K(Xnew) - K(Xnew, X) Ky^-1 K(X, Xnew),  mu = K(Xnew, X) alpha          (posterior.py:273-302)
  *     sparse: Sigma = K(Xnew) - K(Xnew, Z) W K(Z, Xnew),      mu = K(Xnew, Z) woodbury_vector (posterior.py:238-270)
- *   with W = woodbury_inv, formed by the first of gpx_sparse_predictive_gradients / gpx_sparse_posterior_samples after an
- *   evaluation and kept for both. Sigma is factored with jitchol's rules (util/linalg.py:56-75): first plain, then with
+ *   with W = woodbury_inv, formed by the first of gpx_sparse_predictive_gradients / gpx_sparse_posterior_samples /
+ *   gpx_sparse_predict after an evaluation and kept for all three. Sigma is factored with jitchol's rules (util/linalg.py:56-75): first plain, then with
  *   mean(diag) 1e-6 10^k added, k < max_tries; *jitter_used reports what was added. z holds nz = P S standard-normal
  *   vectors of length M, row-major nz x M and ordered output-major (S vectors for output 0, then S for output 1, ...), as
  *   numpy's legacy RNG draws them for np.random.multivariate_normal(m, v, S) once per output; f has the same layout:
@@ -247,6 +247,31 @@ int gpx_sparse_set_data(gpx_ctx* ctx, const double* X, int64_t N, int D, const d
 int gpx_sparse_eval(gpx_ctx* ctx, int kind, int ard, double variance, const double* lengthscale, const double* Z,
                     int64_t M, double noise_variance, double* lml, double* grad, double* dZ);
 int gpx_sparse_get(gpx_ctx* ctx, int which, double* out);
+/* SparseGP.predict's latent part on the device: Posterior._raw_predict (posterior.py:220-248) with pred_var = Z, the
+ * posterior VarDTC returns (var_dtc.py:213), after gpx_sparse_eval / _het / _multi, with that evaluation's kernel, Z,
+ * woodbury_vector and W = woodbury_inv. Xnew is M x D row-major with the D of gpx_sparse_set_data; mu is M x P row-major.
+ *   full_cov = 0: var (M) = Kdiag(Xnew) - rowsum((K(Xnew, Z) W) o K(Xnew, Z)), then clipped at 1e-15 as the reference
+ *                 clips it (posterior.py:248; a NaN stays NaN).
+ *   full_cov = 1: var (M x M column-major) = K(Xnew) - K(Xnew, Z) W K(Z, Xnew), exactly symmetric (the lower tiles of the
+ *                 product term mirrored), K(Xnew) with the exact zero distance on its diagonal; not clipped, as in the
+ *                 reference.
+ * W is formed by the first of gpx_sparse_predictive_gradients, gpx_sparse_posterior_samples and gpx_sparse_predict after an
+ * evaluation (5 launches) and kept for all three. V^T = K(Xnew, Z) W runs on the DMMA GEMM; W is used as the reference
+ * uses it, not in a factored form.
+ * The diagonal streams over chunks of Lc test points, so M is not bounded by device memory:
+ *   Lc = min(max(128, floor(2^30 / (16 Mz + 520 P + 1096) / 128) 128), M padded to 128), Mz = the inducing points padded
+ *   to 128 — the largest multiple of 128 whose temporaries stay within the 1 GiB the stream-ordered pool keeps cached
+ *   (Lc = 15872 at Mz = 4096, P = 1). Launches: 6 per chunk (upload, K-build, GEMM, 2 for the mean, 1 variance reduction).
+ *   Peak temporaries: 8 Lc (2 Mz + 65 P + 1) plus the chunk's points.
+ *   A row's mu and var do not depend on the chunking: every GEMM element has a fixed k-order and every reduction runs per
+ *   row in a fixed order, so a point predicted alone, in a block or inside a multi-chunk call gets the same bits.
+ * The full covariance is one pass: Launches: 8. Peak temporaries: those of gpx_sparse_posterior_samples before sampling,
+ *   8 (2 Ls Mz + 2 Ls^2 + 65 P Ls) with Ls = M padded to 128 (M = 4096, Mz = 4096: 539 MB).
+ * With a communicator attached every rank holds the same posterior and predicts the points it is given; there is no
+ * collective. Returns -2 without touching any state when there is no sparse evaluation, M < 1 or a pointer is null; -1 with
+ * a message when the device is out of memory. Nothing that gpx_sparse_get, gpx_sparse_predictive_gradients,
+ * gpx_sparse_posterior_samples or gpx_get_stats return changes, on success or failure. */
+int gpx_sparse_predict(gpx_ctx* ctx, const double* Xnew, int64_t M, int full_cov, double* mu, double* var);
 /* The same evaluation with ONE NOISE VARIANCE PER DATA POINT (HeteroscedasticGaussian, likelihoods/gaussian.py:347-362):
  * the `het_noise` branches of VarDTC.inference — tmp = Lm^-1 (psi1 sqrt(beta))^T (var_dtc.py:127-131), dL_dpsi1 += 2
  * (dL_dpsi2_beta (psi1 beta)^T)^T (:221-227), the bound with sum(log beta_n) and sum(beta_n |Y_n|^2) (:267-269) and the
