@@ -36,9 +36,10 @@ void gpx::free_data(gpx_ctx* c) {
   c->NBw = 0;
   c->have_eval = false;
   c->have_kinv = false;
-  for (double** mp : {&c->mXsT, &c->msq, &c->mpartials}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
-  c->m_cap = 0;
+  if (c->mpartials) cudaFree(c->mpartials);
+  c->mpartials = nullptr;
   c->mpart_cap = 0;
+  c->rows_cap = c->norm_cap = 0;
   oz_planes_free(c->ozp[0]);
   oz_planes_free(c->ozp[1]);
   oz_planes_free(c->ozpA);
@@ -56,6 +57,7 @@ int gpx::alloc_data(gpx_ctx* c, long NB) {
   GPX_CUDA(cudaMalloc(&c->dX, (size_t)Npad * c->D * 8));
   GPX_CUDA(cudaMalloc(&c->dXsT, (size_t)Npad * c->D * 8));
   GPX_CUDA(cudaMalloc(&c->dsq, (size_t)Npad * 8));
+  c->rows_cap = c->D; c->norm_cap = 1;
   GPX_CUDA(cudaMalloc(&c->dY, (size_t)Npad * c->P * 8));
   GPX_CUDA(cudaMalloc(&c->dT, (size_t)Npad * c->P * 8));
   GPX_CUDA(cudaMalloc(&c->dAlpha, (size_t)Npad * c->P * 8));
@@ -85,21 +87,6 @@ static long choose_nb(const gpx_ctx* c) {
 }
 // the outer block of the allocated workspace, fixed until the next allocation
 static long pick_nb(const gpx_ctx* c) { return c->NBw > 0 ? c->NBw : choose_nb(c); }
-
-int gpx::fill_kp(KernParams& kp, int kind, int ard, int D, double variance, const double* ls) {
-  if (kind < 0 || kind > 3) GPX_FAIL("unknown kernel kind");
-  if (D < 1 || D > MAX_D) GPX_FAIL("input dimension must be in [1, 64]");
-  if (!(variance > 0)) GPX_FAIL("variance must be positive");
-  kp.kind = kind; kp.ard = ard ? 1 : 0; kp.D = D; kp.variance = variance;
-  const int nl = ard ? D : 1;
-  for (int q = 0; q < nl; q++) {
-    if (!(ls[q] > 0)) GPX_FAIL("lengthscale must be positive");
-    kp.ls[q] = ls[q];
-  }
-  for (int q = nl; q < MAX_D; q++) kp.ls[q] = 1.0;
-  kp.inv_ls_iso = ard ? 1.0 : 1.0 / ls[0];
-  return 0;
-}
 
 extern "C" {
 
@@ -554,10 +541,10 @@ static int run_sweep_chain(gpx_ctx* c, Recorder& rec, cudaEvent_t first_rows) {
 }
 
 // K^-1 = U U^T on gemm_lauum_kernel, in one of two modes:
-//   fused (kinv_out == nullptr): the epilogue reduces dL_dK straight into the gradient partials of the context's single
-//     kernel (and diag(dL_dK) for per-point noise); K^-1 is not stored
+//   fused (kinv_out == nullptr): the epilogue reduces dL_dK straight into the gradient partials of the single kernel kp
+//     (and diag(dL_dK) for per-point noise); K^-1 is not stored
 //   plain store: the lower tiles of K^-1 go to kinv_out (leading dimension Npad); no reductions
-static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec) {
+static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec, const KernParams* kp = nullptr) {
   const long ld = c->Npad;
   const int nt = (int)(c->Npad / TILE);
   GemmParams pl = gemm_defaults();
@@ -570,13 +557,13 @@ static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec) {
     pl.kinv_out = kinv_out;
     pl.kp.D = 1; pl.P = 1;   // the smallest epilogue staging: the plain store does not use it
   } else {
-    const int nl = c->kp.ard ? c->D : 1;
+    const int nl = kp->ard ? c->D : 1;
     GPX_CUDA(cudaMemsetAsync(c->partials, 0, (size_t)nt * nt * (nl + 2) * 8, c->st));
     pl.XsT = c->dXsT; pl.sq = c->dsq; pl.alpha = c->dAlpha; pl.ldx = c->Npad;
     pl.N = (int)c->N; pl.P = c->P;
     pl.partials = c->partials;
     pl.dnoise_out = c->het ? c->dDnoise : nullptr;
-    pl.kp = c->kp;
+    pl.kp = *kp;
   }
   double flops = 0;
   for (int r = 0; r < nt; r++) flops += (double)(r + 1) * 2.0 * TILE * TILE * (double)(c->Npad - (long)r * TILE);
@@ -590,16 +577,16 @@ static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec) {
 // Ky = K(X, X) + noise + jitter (+ the per-point noise) of the context's kernel into the workspace, training points
 // prepared first. On the int8 sweep a single kernel's first block row goes first and *first_rows is the event after it, so
 // that the factorisation of the first diagonal block runs beside the rest of the build; otherwise *first_rows = nullptr.
-static int build_Ky(gpx_ctx* c, double extra_jitter, bool int8, Recorder& rec, cudaEvent_t* first_rows) {
+static int build_Ky(gpx_ctx* c, double extra_jitter, bool single, bool int8, Recorder& rec, cudaEvent_t* first_rows) {
   const int nt = (int)(c->Npad / TILE);
   *first_rows = nullptr;
-  if (c->multi && c->m_cap != c->Npad) {
-    for (double** mp : {&c->mXsT, &c->msq}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
-    GPX_CUDA(cudaMalloc(&c->mXsT, (size_t)MAX_D * c->Npad * 8));
-    GPX_CUDA(cudaMalloc(&c->msq, (size_t)MAX_PARTS * c->Npad * 8));
-    c->m_cap = c->Npad;
+  if (c->mk.sumD > c->rows_cap || c->mk.nparts > c->norm_cap) {   // a composite that stacks more rows than D and 1
+    for (double** mp : {&c->dXsT, &c->dsq}) { if (*mp) cudaFree(*mp); *mp = nullptr; }
+    c->rows_cap = std::max(c->rows_cap, c->mk.sumD); c->norm_cap = std::max(c->norm_cap, c->mk.nparts);
+    GPX_CUDA(cudaMalloc(&c->dXsT, (size_t)c->rows_cap * c->Npad * 8));
+    GPX_CUDA(cudaMalloc(&c->dsq, (size_t)c->norm_cap * c->Npad * 8));
   }
-  if (c->multi) {   // the parts' reduction partials, sized by the parts of this evaluation
+  if (!single) {   // the parts' reduction partials, sized by the parts of this evaluation
     size_t need = 0;
     for (int q = 0; q < c->mk.nparts; q++) need += (size_t)nt * nt * part_nred(c->mk.part[q]);
     if (need > c->mpart_cap) {
@@ -611,20 +598,20 @@ static int build_Ky(gpx_ctx* c, double extra_jitter, bool int8, Recorder& rec, c
     }
   }
   const Points tr = train_points(c);
-  GPX_CHECK(prep_points(c, ctx_kern(c), c->dX, c->N, c->D, c->Npad, tr.xT, tr.sq));
+  GPX_CHECK(prep_points(c, c->mk, c->dX, c->N, c->D, c->Npad, tr.xT, tr.sq));
   c->eval_launches++;
   const KyDiag ky{((c->het ? 0.0 : c->noise) + c->jitter) + extra_jitter, c->het ? c->dNoiseVec : nullptr};
   const int h = rec.begin(PH_KBUILD);
-  if (int8 && !c->multi) {
+  if (int8 && single) {
     const int nbt0 = (int)(pick_nb(c) / TILE);
-    GPX_CHECK(build_K(c, &c->kp, tr, tr, c->S, c->Npad, &ky, 0, nbt0));
+    GPX_CHECK(build_K(c, c->mk, c->D, tr, tr, c->S, c->Npad, &ky, 0, nbt0));
     if (!c->ev_kfirst) GPX_CUDA(cudaEventCreateWithFlags(&c->ev_kfirst, cudaEventDisableTiming));
     GPX_CUDA(cudaEventRecord(c->ev_kfirst, c->st));
     *first_rows = c->ev_kfirst;
-    GPX_CHECK(build_K(c, &c->kp, tr, tr, c->S, c->Npad, &ky, nbt0, nt - nbt0));
+    GPX_CHECK(build_K(c, c->mk, c->D, tr, tr, c->S, c->Npad, &ky, nbt0, nt - nbt0));
     c->eval_launches++;
   } else {
-    GPX_CHECK(build_K(c, ctx_kern(c), tr, tr, c->S, c->Npad, &ky));
+    GPX_CHECK(build_K(c, c->mk, c->D, tr, tr, c->S, c->Npad, &ky));
   }
   rec.end(h);
   c->eval_launches++;
@@ -646,13 +633,15 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
   cudaStream_t st = c->st;
   const long ld = c->Npad;
   const int nt = (int)(c->Npad / TILE);
-  const int nl = c->kp.ard ? c->D : 1;
+  KernParams kp;
+  const bool single = as_single(c->mk, c->D, &kp);
+  const int ngrad = kern_ngrad(c->mk), nl = ngrad - 1;   // nl: the single kernel's lengthscales
   const bool int8 = oz_wanted(c);
-  const KinvRoute route = int8 ? KINV_SWEEP : c->multi ? KINV_PLAIN : nt <= 8 ? KINV_FINE : KINV_FUSED;
+  const KinvRoute route = int8 ? KINV_SWEEP : !single ? KINV_PLAIN : nt <= 8 ? KINV_FINE : KINV_FUSED;
   *kinv_stored = route != KINV_FUSED;
   GPX_CUDA(cudaMemsetAsync(c->info, 0, sizeof(int), st));
   cudaEvent_t first_rows;
-  GPX_CHECK(build_Ky(c, extra_jitter, int8, rec, &first_rows));
+  GPX_CHECK(build_Ky(c, extra_jitter, single, int8, rec, &first_rows));
   if (*kinv_stored) GPX_CHECK(ensure_kinv(c));
   if (int8) GPX_CHECK(oz_prepare(c));
   {
@@ -676,7 +665,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
   };
   long grad_tiles = (long)nt * nt;
   if (route == KINV_FUSED) {
-    GPX_CHECK(run_lauum(c, nullptr, &rec));
+    GPX_CHECK(run_lauum(c, nullptr, &rec, &kp));
   } else {
     if (route == KINV_PLAIN) GPX_CHECK(run_lauum(c, c->Kinv, &rec));
     const int h = rec.begin(PH_LAUUM, 0.0);
@@ -689,12 +678,12 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
       GPX_CHECK(launch_fine(fl, st));
       c->eval_launches++;
     }
-    if (c->multi) {   // one reduction pass per part
+    if (!single) {   // one reduction pass per part
       for (int q = 0; q < c->mk.nparts; q++) {
         GPX_CUDA(cudaMemsetAsync(mpart(q), 0, (size_t)nt * nt * part_nred(c->mk.part[q]) * 8, st));
         GradKinvMultiParams gm;
         memset(&gm, 0, sizeof(gm));
-        gm.Kinv = c->Kinv; gm.ld = ld; gm.XsT = c->mXsT; gm.sq = c->msq; gm.ldx = c->Npad; gm.alpha = c->dAlpha;
+        gm.Kinv = c->Kinv; gm.ld = ld; gm.XsT = c->dXsT; gm.sq = c->dsq; gm.ldx = c->Npad; gm.alpha = c->dAlpha;
         gm.N = c->N; gm.P = c->P; gm.nt = nt; gm.part = q; gm.want_noise = q == 0; gm.partials = mpart(q); gm.mk = c->mk;
         GPX_CHECK(launch_grad_kinv_multi(gm, st));
         c->eval_launches++;
@@ -711,13 +700,13 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
       gk.N = c->N; gk.P = c->P; gk.nt = nt;
       gk.partials = c->partials;
       gk.dnoise_out = c->het ? c->dDnoise : nullptr;
-      gk.kp = c->kp;
+      gk.kp = kp;
       GPX_CHECK(launch_grad_kinv(gk, st));
       c->eval_launches++;
     }
     rec.end(h);
   }
-  if (c->multi) {
+  if (!single) {
     FinalizeMultiParams fm;
     memset(&fm, 0, sizeof(fm));
     for (int q = 0; q < c->mk.nparts; q++) fm.partials[q] = mpart(q);
@@ -730,17 +719,12 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
     f.partials = c->partials; f.ntiles = grad_tiles; f.nl = nl;
     f.logdet_part = c->logdet_part; f.nt = nt;
     f.T = T; f.ld = ld; f.N = c->N; f.P = c->P;
-    f.kp = c->kp;
+    f.kp = kp;
     f.res = c->res;
     GPX_CHECK(launch_finalize(f, st));
   }
   c->eval_launches++;
-  size_t nres = nl + 5;
-  if (c->multi) {
-    nres = 4;
-    for (int q = 0; q < c->mk.nparts; q++) nres += part_ngrad(c->mk.part[q]);
-  }
-  GPX_CUDA(cudaMemcpyAsync(c->h_res, c->res, nres * sizeof(double), cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(c->h_res, c->res, (4 + ngrad) * sizeof(double), cudaMemcpyDeviceToHost, st));
   GPX_CUDA(cudaMemcpyAsync(c->h_info, c->info, sizeof(int), cudaMemcpyDeviceToHost, st));
   return 0;
 }
@@ -802,7 +786,7 @@ static int eval_args(const gpx_ctx* c, const void* kern, const double* lml, cons
 
 // One evaluation of the validated kernel k (Kdiag = kdiag), which becomes the context's kernel. noise_vec == nullptr:
 // homoscedastic (`noise`); else N per-point variances (`noise` = their mean, used by the ladder)
-static int exact_eval_impl(gpx_ctx* c, Kern k, double kdiag, double noise, const double* noise_vec, double jitter,
+static int exact_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, double noise, const double* noise_vec, double jitter,
                            int max_tries, double* lml, double* grad, double* dnoise, double* jitter_used) {
   GPX_CUDA(cudaSetDevice(c->device));
   c->het = noise_vec != nullptr;
@@ -819,14 +803,12 @@ static int exact_eval_impl(gpx_ctx* c, Kern k, double kdiag, double noise, const
     }
     GPX_CUDA(cudaMemcpyAsync(c->dNoiseVec, noise_vec, (size_t)c->N * 8, cudaMemcpyHostToDevice, c->st));
   }
-  c->multi = k.mk != nullptr;
-  if (c->multi) c->mk = *k.mk; else c->kp = *k.kp;
+  c->mk = k;
   c->kdiag = kdiag;
   c->noise = noise;
   c->jitter = jitter;
   c->have_eval = false;
   c->have_kinv = false;
-  const int nl = c->kp.ard ? c->D : 1;
   memset(&c->stats, 0, sizeof(c->stats));
   c->eval_launches = 0;
   Recorder rec{c};
@@ -879,13 +861,12 @@ static int exact_eval_impl(gpx_ctx* c, Kern k, double kdiag, double noise, const
     return info;
   }
   *lml = c->h_res[0];
-  if (c->multi) {
-    int n = 0;
-    for (int p = 0; p < c->mk.nparts; p++) n += part_ngrad(c->mk.part[p]);
-    for (int q = 0; q < n; q++) grad[q] = c->h_res[4 + q];
-    grad[n] = c->h_res[3];
-  } else
-  for (int q = 0; q < nl + 2; q++) grad[q] = c->h_res[1 + q];
+  // the kernel's gradient block and d/d noise: [lml, block, noise, ..] from finalize_kernel, [lml, .., noise, block] from
+  // finalize_multi_kernel
+  const bool single = as_single(c->mk, c->D, nullptr);
+  const int n = kern_ngrad(c->mk);
+  for (int q = 0; q < n; q++) grad[q] = c->h_res[(single ? 1 : 4) + q];
+  grad[n] = c->h_res[single ? 1 + n : 3];
   if (c->het) {
     GPX_CUDA(cudaMemcpyAsync(dnoise, c->dDnoise, (size_t)c->N * 8, cudaMemcpyDeviceToHost, c->st));
     GPX_CUDA(cudaStreamSynchronize(c->st));
@@ -900,9 +881,9 @@ extern "C" {
 int gpx_exact_eval(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, double noise,
                    double jitter, int max_tries, double* lml, double* grad, double* jitter_used) {
   GPX_CHECK(eval_args(c, lengthscale, lml, grad, noise));
-  KernParams kp{};
-  GPX_CHECK(fill_kp(kp, kind, ard, c->D, variance, lengthscale));
-  return exact_eval_impl(c, &kp, variance, noise, nullptr, jitter, max_tries, lml, grad, nullptr, jitter_used);
+  MultiKern mk;
+  GPX_CHECK(fill_single(mk, kind, ard, c->D, variance, lengthscale));
+  return exact_eval_impl(c, mk, variance, noise, nullptr, jitter, max_tries, lml, grad, nullptr, jitter_used);
 }
 
 int gpx_exact_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, double noise, double jitter, int max_tries,
@@ -912,7 +893,7 @@ int gpx_exact_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, dou
   MultiKern mk;
   double kdiag;
   GPX_CHECK(fill_mk(mk, parts, nparts, c->D, &kdiag));
-  return exact_eval_impl(c, &mk, kdiag, noise, nullptr, jitter, max_tries, lml, grad, nullptr, jitter_used);
+  return exact_eval_impl(c, mk, kdiag, noise, nullptr, jitter, max_tries, lml, grad, nullptr, jitter_used);
 }
 
 int gpx_exact_eval_het(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale,
@@ -926,9 +907,9 @@ int gpx_exact_eval_het(gpx_ctx* c, int kind, int ard, double variance, const dou
   }
   mean /= (double)std::max<int64_t>(c->N, 1);
   GPX_CHECK(eval_args(c, lengthscale, lml, grad, mean));
-  KernParams kp{};
-  GPX_CHECK(fill_kp(kp, kind, ard, c->D, variance, lengthscale));
-  return exact_eval_impl(c, &kp, variance, mean, noise_variances, jitter, max_tries, lml, grad, dnoise, jitter_used);
+  MultiKern mk;
+  GPX_CHECK(fill_single(mk, kind, ard, c->D, variance, lengthscale));
+  return exact_eval_impl(c, mk, variance, mean, noise_variances, jitter, max_tries, lml, grad, dnoise, jitter_used);
 }
 
 int gpx_measure_fp64_peak(gpx_ctx* c, double* tflops) {
@@ -973,7 +954,7 @@ int gpx_get(gpx_ctx* c, int which, double* out) {
   GPX_CHECK(ensure_staging(c));
   if (which == GPX_GET_K) {
     const Points tr = train_points(c);
-    GPX_CHECK(build_K(c, ctx_kern(c), tr, tr, c->staging, N));
+    GPX_CHECK(build_K(c, c->mk, c->D, tr, tr, c->staging, N));
     c->total_launches++;
   } else if (which == GPX_GET_L || which == GPX_GET_LINV) {
     GPX_CHECK(launch_extract(which, c->S, ld, c->Ldiag, nullptr, nullptr, 0, N, c->staging, st));
@@ -1001,8 +982,8 @@ int gpx_get(gpx_ctx* c, int which, double* out) {
 
 // ---------------------------------------------------------------------------------------------------------------
 // stand-alone kernel calls: K and update_gradients_full of a single kernel (kinds 0-3) or of one composite part (kinds 0-3,
-// 6, 7: the K-build and the per-pair gradient terms of the composite evaluation), gradients_X of a single kernel. Each works
-// with the kernel it is given; the context's own (that of its last evaluation) is left alone.
+// 6, 7), gradients_X of a single kernel. Each works with the kernel it is given; the context's own (that of its last
+// evaluation) is left alone.
 // ---------------------------------------------------------------------------------------------------------------
 static std::mutex g_scratch_mu;
 static gpx_ctx* g_scratch = nullptr;
@@ -1027,10 +1008,21 @@ static int fill_one_part(const gpx_kern_part* part, int D, MultiKern& mk) {
   return fill_mk(mk, &one, 1, D, &kdiag);
 }
 
+int gpx::fill_single(MultiKern& mk, int kind, int ard, int D, double variance, const double* ls) {
+  if (kind < GPX_RBF || kind > GPX_MATERN52) GPX_FAIL("unknown kernel kind");
+  if (D < 1 || D > MAX_D) GPX_FAIL("input dimension must be in [1, 64]");
+  int dims[MAX_D];
+  for (int q = 0; q < D; q++) dims[q] = q;
+  gpx_kern_part part{};
+  part.kind = kind; part.ard = ard; part.ndims = D; part.dims = dims; part.variance = variance; part.lengthscale = ls;
+  double kdiag;
+  return fill_mk(mk, &part, 1, D, &kdiag);
+}
+
 // K(X, X2) of k into out (N x M row-major; X2 == NULL: K(X, X)) on c (NULL: the scratch context), timed into c's kbuild_ms /
 // kbuild_bytes. out == NULL: built on the device only (the result is dropped) -- used to measure the rectangular K(X, Z)
 // build of the sparse model at full size.
-static int kern_K(gpx_ctx* c, Kern k, const double* X, int64_t N, const double* X2, int64_t M, int D, double* out,
+static int kern_K(gpx_ctx* c, const MultiKern& k, const double* X, int64_t N, const double* X2, int64_t M, int D, double* out,
                   const char* what) {
   if (!c) GPX_CHECK(scratch_ctx(&c));
   GPX_CUDA(cudaSetDevice(c->device));
@@ -1044,7 +1036,7 @@ static int kern_K(gpx_ctx* c, Kern k, const double* X, int64_t N, const double* 
   int rc = ev_get(c, 0, &e0) || ev_get(c, 1, &e1);
   if (rc == 0) {
     cudaEventRecord(e0, c->st);
-    rc = build_K(c, k, pj, p1, dout, M);
+    rc = build_K(c, k, D, pj, p1, dout, M);
     cudaEventRecord(e1, c->st);
   }
   c->total_launches++;
@@ -1059,7 +1051,7 @@ static int kern_K(gpx_ctx* c, Kern k, const double* X, int64_t N, const double* 
 }
 
 // update_gradients_full of k for a caller's dL_dK (N x M row-major) on c (NULL: the scratch context) -> k's gradient block
-static int kern_grad_full(gpx_ctx* c, Kern k, const double* X, int64_t N, const double* X2, int64_t M, int D,
+static int kern_grad_full(gpx_ctx* c, const MultiKern& k, const double* X, int64_t N, const double* X2, int64_t M, int D,
                           const double* dL_dK, double* grad) {
   if (!c) GPX_CHECK(scratch_ctx(&c));
   GPX_CUDA(cudaSetDevice(c->device));
@@ -1068,10 +1060,10 @@ static int kern_grad_full(gpx_ctx* c, Kern k, const double* X, int64_t N, const 
   if (X2) GPX_CHECK(upload_points(c, k, X2, M, D, p2));
   double *dd = nullptr, *dpart = nullptr;
   GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
-  const GradFullParams gp = grad_params(k, p1, X2 ? p2 : p1, dd, 0);
-  GPX_TMP_ALLOC(&dpart, grad_full_doubles(k, gp) * 8, c->st);
+  const GradFullParams gp = grad_params(k, D, p1, X2 ? p2 : p1, dd, 0);
+  GPX_TMP_ALLOC(&dpart, grad_full_doubles(k, D, gp) * 8, c->st);
   GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
-  const int rc = grad_full_sum(c, k, gp, dpart, grad);
+  const int rc = grad_full_sum(c, k, D, gp, dpart, grad);
   GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
   return rc;
 }
@@ -1081,11 +1073,11 @@ extern "C" {
 int gpx_kern_K(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
                const double* X2, int64_t M, int D, double* out) {
   if (!X || !lengthscale) GPX_FAIL("null argument");
-  KernParams kp{};
-  GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
+  MultiKern mk;
+  GPX_CHECK(fill_single(mk, kind, ard, D, variance, lengthscale));
   if (!X2) M = N;
   if (N < 1 || M < 1) GPX_FAIL("empty input");
-  return kern_K(c, &kp, X, N, X2, M, D, out, "gpx_kern_K");
+  return kern_K(c, mk, X, N, X2, M, D, out, "gpx_kern_K");
 }
 
 int gpx_kern_part_K(gpx_ctx* c, const gpx_kern_part* part, const double* X, int64_t N, const double* X2, int64_t M, int D,
@@ -1095,7 +1087,7 @@ int gpx_kern_part_K(gpx_ctx* c, const gpx_kern_part* part, const double* X, int6
   GPX_CHECK(fill_one_part(part, D, mk));
   if (!X2) M = N;
   if (N < 1 || M < 1) GPX_FAIL("empty input");
-  return kern_K(c, &mk, X, N, X2, M, D, out, "gpx_kern_part_K");
+  return kern_K(c, mk, X, N, X2, M, D, out, "gpx_kern_part_K");
 }
 
 int gpx_kern_Kdiag(int kind, double variance, int64_t N, double* out) {
@@ -1109,13 +1101,13 @@ int gpx_kern_grad_full(gpx_ctx* c, int kind, int ard, double variance, const dou
                        int64_t N, const double* X2, int64_t M, int D, const double* dL_dK, double* dvariance,
                        double* dlengthscale) {
   if (!X || !dL_dK || !lengthscale || !dvariance || !dlengthscale) GPX_FAIL("null argument");
-  KernParams kp{};
-  GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
+  MultiKern mk;
+  GPX_CHECK(fill_single(mk, kind, ard, D, variance, lengthscale));
   if (!X2) M = N;
   double g[MAX_D + 1];
-  GPX_CHECK(kern_grad_full(c, &kp, X, N, X2, M, D, dL_dK, g));
+  GPX_CHECK(kern_grad_full(c, mk, X, N, X2, M, D, dL_dK, g));
   *dvariance = g[0];
-  for (int q = 0; q < (kp.ard ? D : 1); q++) dlengthscale[q] = g[1 + q];
+  for (int q = 0; q < (ard ? D : 1); q++) dlengthscale[q] = g[1 + q];
   return 0;
 }
 
@@ -1126,7 +1118,7 @@ int gpx_kern_part_grad_full(gpx_ctx* c, const gpx_kern_part* part, const double*
   GPX_CHECK(fill_one_part(part, D, mk));
   if (!X2) M = N;
   if (N < 1 || M < 1) GPX_FAIL("empty input");
-  return kern_grad_full(c, &mk, X, N, X2, M, D, dL_dK, grad);
+  return kern_grad_full(c, mk, X, N, X2, M, D, dL_dK, grad);
 }
 
 int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* X, int64_t N,
@@ -1134,18 +1126,18 @@ int gpx_kern_grad_X(gpx_ctx* c, int kind, int ard, double variance, const double
   if (!X || !dL_dK || !lengthscale || !grad) GPX_FAIL("null argument");
   if (!c) GPX_CHECK(scratch_ctx(&c));
   GPX_CUDA(cudaSetDevice(c->device));
-  KernParams kp;
-  GPX_CHECK(fill_kp(kp, kind, ard, D, variance, lengthscale));
+  MultiKern mk;
+  GPX_CHECK(fill_single(mk, kind, ard, D, variance, lengthscale));
   if (!X2) M = N;
   PointSet p1, p2;
-  GPX_CHECK(upload_points(c, &kp, X, N, D, p1));
-  if (X2) GPX_CHECK(upload_points(c, &kp, X2, M, D, p2));
+  GPX_CHECK(upload_points(c, mk, X, N, D, p1));
+  if (X2) GPX_CHECK(upload_points(c, mk, X2, M, D, p2));
   double *dd = nullptr, *dpart = nullptr;
   GPX_TMP_ALLOC(&dd, (size_t)N * M * 8, c->st);
-  const GradFullParams gp = grad_params(&kp, p1, X2 ? p2 : p1, dd, 0);
-  GPX_TMP_ALLOC(&dpart, grad_X_doubles(c, &kp, gp, D) * 8, c->st);
+  const GradFullParams gp = grad_params(mk, D, p1, X2 ? p2 : p1, dd, 0);
+  GPX_TMP_ALLOC(&dpart, grad_X_doubles(c, mk, gp, D) * 8, c->st);
   GPX_CUDA(cudaMemcpyAsync(dd, dL_dK, (size_t)N * M * 8, cudaMemcpyHostToDevice, c->st));
-  const int rc = grad_X(c, &kp, gp, D, dpart, grad);
+  const int rc = grad_X(c, mk, gp, D, dpart, grad);
   GPX_TMP_FREE(dd, c->st); GPX_TMP_FREE(dpart, c->st);
   return rc;
 }
@@ -1278,14 +1270,14 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
   cudaStream_t st = c->st;
   const long ld = c->Npad, N = c->N;
   PointSet pn;
-  GPX_CHECK(upload_points(c, ctx_kern(c), Xnew, M, c->D, pn));
+  GPX_CHECK(upload_points(c, c->mk, Xnew, M, c->D, pn));
   // Kx as [M][ld] (each new point one zero-padded column of length ld): thread-mapped operand = training points
   double* Kx = nullptr; double* Tx = nullptr;
   GPX_TMP_ALLOC(&Kx, (size_t)pn.ld * ld * 8, c->st);
   GPX_TMP_ALLOC(&Tx, (size_t)pn.ld * ld * 8, c->st);
   GPX_CUDA(cudaMemsetAsync(Kx, 0, (size_t)pn.ld * ld * 8, st));
   if (dG > 1) GPX_CUDA(cudaMemsetAsync(Tx, 0, (size_t)pn.ld * ld * 8, st));   // columns of other ranks stay zero
-  int rc = build_K(c, ctx_kern(c), train_points(c), pn, Kx, ld);
+  int rc = build_K(c, c->mk, c->D, train_points(c), pn, Kx, ld);
   c->total_launches++;
   // tmp = L^-1 Kx = U^T Kx, MAX_P columns per pass
   for (long m0 = 0; rc == 0 && m0 < M; m0 += MAX_P) {
@@ -1355,7 +1347,7 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
   std::vector<double> kxx((size_t)M * M);
   double* dk = nullptr;
   GPX_TMP_ALLOC(&dk, (size_t)M * M * 8, c->st);
-  rc = build_K(c, ctx_kern(c), pn, pn, dk, M);
+  rc = build_K(c, c->mk, c->D, pn, pn, dk, M);
   c->total_launches++;
   if (rc == 0 && cudaMemcpyAsync(kxx.data(), dk, (size_t)M * M * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) rc = -1;
   if (cudaStreamSynchronize(st) != cudaSuccess) { gpx::set_error("gpx_predict: device failure"); rc = -1; }
@@ -1375,7 +1367,7 @@ int gpx_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t M, double* 
   if (!c->have_eval) GPX_FAIL("no successful gpx_exact_eval to differentiate the prediction of");
   if (M < 1) GPX_FAIL("empty Xnew");
   if (c->dist) GPX_FAIL("predictive gradients are single-GPU");
-  const Kern k = ctx_kern(c);
+  const MultiKern& k = c->mk;
   GPX_CHECK(pred_grad_check(k));
   GPX_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->st;
@@ -1389,7 +1381,7 @@ int gpx_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t M, double* 
   GPX_TMP_ALLOC(&uvp, (size_t)KSPLIT * MAX_P * ld * 8, st);
   int rc = 0;
   if (cudaMemsetAsync(Kx, 0, (size_t)pn.ld * ld * 8, st) != cudaSuccess) { gpx::set_error("gpx_predictive_gradients: device failure"); rc = -1; }
-  if (rc == 0) rc = build_K(c, k, train_points(c), pn, Kx, ld);
+  if (rc == 0) rc = build_K(c, k, c->D, train_points(c), pn, Kx, ld);
   c->total_launches++;
   for (long m0 = 0; rc == 0 && m0 < M; m0 += MAX_P) {
     const int pc = (int)std::min<long>(MAX_P, M - m0);

@@ -23,8 +23,9 @@ struct gpx_ctx {
   long N = 0, Npad = 0;
   int D = 0, P = 0;
   double* dX = nullptr;      // N x D row-major (as given)
-  double* dXsT = nullptr;    // [D][Npad] scaled SoA
-  double* dsq = nullptr;     // [Npad]
+  double* dXsT = nullptr;    // [rows_cap][Npad] scaled SoA of the training points, stacked as the kernel needs them
+  double* dsq = nullptr;     // [norm_cap][Npad] their squared norms
+  int rows_cap = 0, norm_cap = 0;   // rows dXsT and dsq hold: D and 1 from alloc_data, grown by a kernel that needs more
   double* dY = nullptr;      // [P][Npad]
   double* dT = nullptr;      // [P][Npad]  L^-1 y
   double* dAlpha = nullptr;  // [P][Npad]
@@ -50,8 +51,8 @@ struct gpx_ctx {
   // last evaluation
   bool have_eval = false;
   bool have_kinv = false;    // c->Kinv holds K^-1 of the last evaluation (its route stored it, or gpx_get made it)
-  gpx::KernParams kp{};      // the single kernel of the last evaluation (unused after a composite one: see `multi`)
-  double kdiag = 0;          // Kdiag of the last evaluation's kernel (jitter ladder, gpx_predict)
+  gpx::MultiKern mk{};       // the kernel of the last evaluation
+  double kdiag = 0;          // its Kdiag (jitter ladder, gpx_predict)
   double noise = 0, jitter = 0, jitter_extra = 0;
   // heteroscedastic evaluation (gpx_exact_eval_het): per-point noise variances in, diag(dL_dK) out
   bool het = false;
@@ -76,12 +77,7 @@ struct gpx_ctx {
   using OzStep = gpx::OzStep;
   std::vector<OzStep> oz_steps;
   // ---- composite kernels (gpx_multi.cu) ---------------------------------------------------------------------------------
-  bool multi = false;          // the last evaluation used gpx_exact_eval_multi: K-builds use mk, mXsT and msq
-  gpx::MultiKern mk{};
-  double* mXsT = nullptr;      // [sumD][Npad] stacked scaled inputs of the parts
-  double* msq = nullptr;       // [nparts][Npad]
   double* mpartials = nullptr; // per part p in turn: [nt*nt][part_nred(p)]
-  long m_cap = 0;              // Npad mXsT and msq were sized for
   size_t mpart_cap = 0;        // doubles mpartials holds
   struct DistState* dist = nullptr;   // multi-GPU state (gpx_dist.cu), null on a single GPU
   struct SparseState* sparse = nullptr;   // sparse-GP (VarDTC) state (gpx_sparse.cu)
@@ -108,7 +104,6 @@ int dist_allreduce_sum(gpx_ctx* c, double* buf, size_t count, cudaStream_t st); 
 void sparse_free(gpx_ctx* c);
 int factor_device(gpx_ctx* c, const double* dA, long lda, long N, double jitter0, int max_tries, double* logdet,
                   double* jitter_used);
-int fill_kp(KernParams& kp, int kind, int ard, int D, double variance, const double* ls);
 
 // ---- point sets, K-builds and kernel-gradient reductions (gpx_points.cu) ----------------------------------------------
 // Temporaries of the stand-alone kernel calls and of gpx_predict: stream-ordered allocations from the device's default memory
@@ -118,16 +113,13 @@ int fill_kp(KernParams& kp, int kind, int ard, int D, double variance, const dou
 #define GPX_TMP_ALLOC(ptr, bytes, st) GPX_CUDA(cudaMallocAsync((void**)(ptr), (bytes), (st)))
 #define GPX_TMP_FREE(p, st) do { if (p) cudaFreeAsync((p), (st)); } while (0)
 
-// The covariance function a helper below works with: a single stationary kernel or a composite one (exactly one is set)
-struct Kern {
-  const KernParams* kp = nullptr;
-  const MultiKern* mk = nullptr;
-  Kern(const KernParams* k) : kp(k) {}
-  Kern(const MultiKern* m) : mk(m) {}
-  int coord_rows() const { return kp ? kp->D : mk->sumD; }   // rows of a point set's stacked coordinates
-  int norm_rows() const { return kp ? 1 : mk->nparts; }      // rows of its squared norms
-};
-// n points prepared for a kernel: scaled coordinates xT, SoA [coord_rows][ld], and their squared norms sq, [norm_rows][ld]
+// Every helper below works with the kernel description k it is given, for host points with D columns (k's dims index them),
+// and never falls back on the context's own. as_single is the one place that picks the specialised kernels: true iff k is a
+// single stationary kernel, one part of kind RBF .. Matern52 on the dims 0 .. D-1 in order; then *kp (if given) is its
+// KernParams, the launch parameter of those kernels. Every other description takes the composite kernels.
+bool as_single(const MultiKern& k, int D, KernParams* kp);
+int kern_ngrad(const MultiKern& k);   // entries of k's gradient block: every part's block in turn
+// n points prepared for a kernel: scaled coordinates xT, SoA [k.sumD][ld], and their squared norms sq, [k.nparts][ld]
 struct Points { double* xT = nullptr; double* sq = nullptr; long n = 0, ld = 0; };
 struct PointSet : Points {   // host points uploaded and prepared in temporaries it owns
   double* raw = nullptr;
@@ -138,39 +130,35 @@ struct KyDiag { double add; const double* vec; };   // added to the diagonal of 
 
 // The K-build and prep launches are counted by the caller (into eval_launches inside an exact evaluation); the other
 // helpers count theirs into c->total_launches.
-// X: n points, row-major with D columns (a single kernel's D; a composite's dims index them)
-int prep_points(gpx_ctx* c, Kern k, const double* X, long n, int D, long ld, double* xT, double* sq);
-int upload_points(gpx_ctx* c, Kern k, const double* X, long n, int D, PointSet& ps);
+// X: n points, row-major with D columns
+int prep_points(gpx_ctx* c, const MultiKern& k, const double* X, long n, int D, long ld, double* xT, double* sq);
+int upload_points(gpx_ctx* c, const MultiKern& k, const double* X, long n, int D, PointSet& ps);
 // K(rows, cols) into out[i + j * ld] (i: row point, j: column point), row tiles [rt0, rt0 + nrt) (nrt = 0: all of them;
 // a part of the rows: single kernel only). ky != nullptr: the factor workspace form of Ky (lower tiles, zero upper tiles,
 // identity padding, ky's diagonal terms).
-int build_K(gpx_ctx* c, Kern k, const Points& rows, const Points& cols, double* out, long ld, const KyDiag* ky = nullptr,
-            int rt0 = 0, int nrt = 0);
+int build_K(gpx_ctx* c, const MultiKern& k, int D, const Points& rows, const Points& cols, double* out, long ld,
+            const KyDiag* ky = nullptr, int rt0 = 0, int nrt = 0);
 // dL_dK (device; element (i, j) of rows x cols at dL_dK[i * ldd + j], ldd = 0: cols.n) for the reductions below. The caller
 // may add the rank-P term (ci, cj, cP) and, for gradients_X, the transposed read.
-GradFullParams grad_params(Kern k, const Points& rows, const Points& cols, const double* dL_dK, long ldd);
-// update_gradients_full: one reduction launch per part (a single kernel: one) writes a row of partial sums per tile into
-// `part` (grad_full_doubles); they are summed on the host in tile order and mapped to k's gradient block in paramz order
-// into grad (a single kernel: variance, lengthscale(s); a composite: every part's block in turn, as part_grad_entry maps it)
-size_t grad_full_doubles(Kern k, const GradFullParams& gp);
-int grad_full_sum(gpx_ctx* c, Kern k, GradFullParams gp, double* part, double* grad);
-// gradients_X w.r.t. the row points (D: columns of their host X; a single kernel's own D): chunk partials and the N x D
-// result in `part` (grad_X_doubles); the result is copied to `out` on the host. A composite's RatQuad / StdPeriodic parts
-// have no device gradients_X (rc -2).
-size_t grad_X_doubles(const gpx_ctx* c, Kern k, const GradFullParams& gp, int D);
-int grad_X(gpx_ctx* c, Kern k, const GradFullParams& gp, int D, double* part, double* out);
+GradFullParams grad_params(const MultiKern& k, int D, const Points& rows, const Points& cols, const double* dL_dK, long ldd);
+// update_gradients_full: one reduction launch per part writes a row of partial sums per tile into `part`
+// (grad_full_doubles); they are summed on the host in tile order and mapped to k's gradient block in paramz order into grad
+// (every part's block in turn, as part_grad_entry maps it)
+size_t grad_full_doubles(const MultiKern& k, int D, const GradFullParams& gp);
+int grad_full_sum(gpx_ctx* c, const MultiKern& k, int D, GradFullParams gp, double* part, double* grad);
+// gradients_X w.r.t. the row points: chunk partials and the N x D result in `part` (grad_X_doubles); the result is copied
+// to `out` on the host. RatQuad / StdPeriodic parts have no device gradients_X (rc -2).
+size_t grad_X_doubles(const gpx_ctx* c, const MultiKern& k, const GradFullParams& gp, int D);
+int grad_X(gpx_ctx* c, const MultiKern& k, const GradFullParams& gp, int D, double* part, double* out);
 // predictive gradients (gp.py:438-474) of k at the prepared test points against `train`, for the woodbury vector alpha
 // ([P][lda], device) and V = woodbury_inv K(train, test) (V[n + m * ldv], device): dmu (n x D x P) and dvar (n x D), host,
-// row-major, D the columns of the host X. pred_grad_check: -2 for a kernel without a device input gradient (RatQuad /
-// StdPeriodic parts), before anything is launched.
-int pred_grad_check(Kern k);
-int pred_grad(gpx_ctx* c, Kern k, const Points& test, const Points& train, const double* alpha, long lda, int P,
+// row-major. pred_grad_check: -2 for a kernel without a device input gradient (RatQuad / StdPeriodic parts), before
+// anything is launched.
+int pred_grad_check(const MultiKern& k);
+int pred_grad(gpx_ctx* c, const MultiKern& k, const Points& test, const Points& train, const double* alpha, long lda, int P,
               const double* V, long ldv, int D, double* dmu, double* dvar);
-// the kernel of the context's last exact evaluation, and its training points as the evaluation prepared them
-inline Kern ctx_kern(const gpx_ctx* c) { return c->multi ? Kern(&c->mk) : Kern(&c->kp); }
-inline Points train_points(const gpx_ctx* c) {
-  return c->multi ? Points{c->mXsT, c->msq, c->N, c->Npad} : Points{c->dXsT, c->dsq, c->N, c->Npad};
-}
+// the training points of the context's last exact evaluation, as it prepared them for c->mk
+inline Points train_points(const gpx_ctx* c) { return Points{c->dXsT, c->dsq, c->N, c->Npad}; }
 
 // ---- joint posterior (gpx_joint.cu) ------------------------------------------------------------------------------------
 #define GPX_FAIL_DEVICE(what)                             \
@@ -205,4 +193,7 @@ int joint_sample(gpx_ctx* c, const double* Sig, long lds, long M, const double* 
 
 // the parts of a composite kernel -> mk (validated against Dfull columns of X), *kdiag_total = its Kdiag (gpx_api.cu)
 int fill_mk(MultiKern& mk, const gpx_kern_part* parts, int nparts, int Dfull, double* kdiag_total);
+// the single stationary kernel of the single-kernel entries (kind, ard, variance, lengthscale on all D columns) -> its
+// one-part description mk, checked with those entries' messages; its Kdiag is the variance (gpx_api.cu)
+int fill_single(MultiKern& mk, int kind, int ard, int D, double variance, const double* ls);
 }  // namespace gpx

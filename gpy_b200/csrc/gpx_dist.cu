@@ -233,10 +233,12 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
   const long ld = d->ldl, Npad = c->Npad, NB = d->NB;   // ld: leading dimension of the row-owned workspace
   const int nt = (int)(Npad / TILE), nbt = (int)(NB / TILE);
   const int G = d->G, g = d->rank;
-  const int nl = c->kp.ard ? c->D : 1, nred = nl + 2;
+  KernParams kp;   // the single-kernel entries alone reach a sharded context
+  if (!as_single(c->mk, c->D, &kp)) GPX_FAIL("internal: the sharded evaluation takes a single kernel");
+  const int nl = kp.ard ? c->D : 1, nred = nl + 2;
   GPX_CUDA(cudaMemsetAsync(c->info, 0, sizeof(int), st));
   GPX_CUDA(cudaMemsetAsync(c->logdet_part, 0, (size_t)nt * 8, st));
-  GPX_CHECK(launch_prep_x(c->dX, c->N, Npad, c->kp, c->dXsT, c->dsq, st));
+  GPX_CHECK(launch_prep_x(c->dX, c->N, Npad, kp, c->dXsT, c->dsq, st));
   c->eval_launches++;
   {
     KBuildParams kb;
@@ -246,7 +248,7 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
     kb.out = c->S; kb.ld = ld; kb.nrows = c->N; kb.ncols = c->N; kb.sym = 1; kb.same = 1;
     kb.diag_add = (c->noise + c->jitter) + extra_jitter;
     kb.own_G = G; kb.own_g = g; kb.own_blk = nbt; kb.loc_rows = 1;
-    kb.kp = c->kp;
+    kb.kp = kp;
     GPX_CHECK(launch_kbuild(kb, nt, nt, st));
     c->eval_launches++;
   }
@@ -358,7 +360,7 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
     pl.XsT = c->dXsT; pl.sq = c->dsq; pl.alpha = c->dAlpha; pl.ldx = Npad;
     pl.N = (int)c->N; pl.P = c->P; pl.partials = c->partials; pl.kinv_out = nullptr;
     pl.k_G = G; pl.k_g = g; pl.k_blk = nbt;
-    pl.kp = c->kp;
+    pl.kp = kp;
     GPX_CHECK(launch_gemm(pl, dim3(1, 1), st));
     c->eval_launches++;
   }
@@ -367,7 +369,7 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
     memset(&f, 0, sizeof(f));
     f.partials = c->partials; f.ntiles = (long)nt * nt; f.nl = nl;
     f.logdet_part = c->logdet_part; f.nt = nt;
-    f.T = c->dT; f.ld = Npad; f.N = c->N; f.P = c->P; f.kp = c->kp; f.res = d->raw;
+    f.T = c->dT; f.ld = Npad; f.N = c->N; f.P = c->P; f.kp = kp; f.res = d->raw;
     GPX_CHECK(launch_finalize_raw(f, st));
     c->eval_launches++;
   }
@@ -382,11 +384,7 @@ int dist_exact_eval(gpx_ctx* c, double extra_jitter) {
   const double log2pi = 1.8378770664093453;
   c->h_res[0] = 0.5 * (-(double)c->N * c->P * log2pi - (double)c->P * logdet - quad);
   c->h_res[1] = tot[0];
-  if (c->kp.ard) {
-    for (int q = 0; q < nl; q++) c->h_res[2 + q] = -tot[1 + q] / c->kp.ls[q];
-  } else {
-    c->h_res[2] = -tot[1] / c->kp.ls[0];
-  }
+  for (int q = 0; q < nl; q++) c->h_res[2 + q] = -tot[1 + q] / kp.ls[q];
   c->h_res[2 + nl] = tot[nred - 1];
   c->h_res[3 + nl] = logdet;
   c->h_res[4 + nl] = quad;

@@ -164,7 +164,6 @@ int joint_sample(gpx_ctx* c, const double* Sig, long lds, long M, const double* 
 static int exact_joint(gpx_ctx* c, const Points& ps, long M1, long off2, long M2, int sym, TmpBuf& Kss, TmpBuf& prod,
                        TmpBuf* mu) {
   cudaStream_t st = c->st;
-  const Kern k = ctx_kern(c);
   const long Ls = ps.ld, Npad = c->Npad, M1pad = (M1 + TILE - 1) / TILE * TILE, M2pad = (M2 + TILE - 1) / TILE * TILE;
   {
     TmpBuf Ks(st), Li(st), Tt(st);
@@ -172,7 +171,7 @@ static int exact_joint(gpx_ctx* c, const Points& ps, long M1, long off2, long M2
     GPX_CHECK(Li.alloc((size_t)Npad * Npad));
     GPX_CHECK(Tt.alloc((size_t)Ls * Npad));
     GPX_CUDA(cudaMemsetAsync(Ks.p, 0, (size_t)Ls * Npad * 8, st));
-    GPX_CHECK(build_K(c, k, ps, train_points(c), Ks.p, Ls));   // K(X*, X): test points thread-mapped, m-contiguous
+    GPX_CHECK(build_K(c, c->mk, c->D, ps, train_points(c), Ks.p, Ls));   // K(X*, X): test points thread-mapped, m-contiguous
     c->total_launches++;
     joint_extract_kernel<<<dim3((unsigned)(Npad / 256 + 1), grid_y(Npad)), 256, 0, st>>>(0, c->S, Npad, c->Ldiag, c->N,
                                                                                           Li.p, Npad);
@@ -193,7 +192,7 @@ static int exact_joint(gpx_ctx* c, const Points& ps, long M1, long off2, long M2
     GPX_CHECK(gemm_nt(c, Tt.p, Ls, Tt.p + off2, Ls, prod.p, M1pad, M1pad, sym ? M1pad : M2pad, Npad, sym ? 2 : 1, 0));
   }
   GPX_CHECK(Kss.alloc((size_t)Ls * Ls));
-  GPX_CHECK(build_K(c, k, ps, ps, Kss.p, Ls));   // one point set on both sides: exact zero distance on its diagonal only
+  GPX_CHECK(build_K(c, c->mk, c->D, ps, ps, Kss.p, Ls));   // one point set on both sides: exact zero distance on its diagonal only
   c->total_launches++;
   return 0;
 }
@@ -230,7 +229,7 @@ int gpx_posterior_covariance(gpx_ctx* c, const double* X1, int64_t M1, const dou
     Xs = hx.data();
   }
   PointSet ps;
-  GPX_CHECK(upload_points(c, ctx_kern(c), Xs, ns, (int)D, ps));
+  GPX_CHECK(upload_points(c, c->mk, Xs, ns, (int)D, ps));
   TmpBuf Kss(c->st), prod(c->st), out(c->st);
   GPX_CHECK(exact_joint(c, ps, M1, off2, M2, sym, Kss, prod, nullptr));
   GPX_CHECK(out.alloc((size_t)M1 * M2));
@@ -247,7 +246,7 @@ int gpx_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t M, const doubl
   GPX_CHECK(joint_check(c, Xnew, M, z, nz, f, jitter_used, c->P));
   GPX_CUDA(cudaSetDevice(c->device));
   PointSet ps;
-  GPX_CHECK(upload_points(c, ctx_kern(c), Xnew, M, c->D, ps));
+  GPX_CHECK(upload_points(c, c->mk, Xnew, M, c->D, ps));
   TmpBuf Kss(c->st), prod(c->st), mu(c->st);
   GPX_CHECK(exact_joint(c, ps, M, 0, M, 1, Kss, prod, &mu));
   GPX_CHECK(joint_combine(c, Kss.p, ps.ld, 0, prod.p, ps.ld, 1, M, M, Kss.p, ps.ld, 1));   // Sigma in place of K(X*, X*)

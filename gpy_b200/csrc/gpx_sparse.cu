@@ -35,17 +35,14 @@ struct SparseState {
   double *Gm = nullptr, *W2 = nullptr, *Cm = nullptr;   // Mpad x Mpad, Mpad x Mpad, [P][Mpad]
   double *part = nullptr; size_t part_cap = 0;
   int rows_cap = 0, norm_cap = 0;          // stacked coordinate rows of XsT / ZsT, squared-norm rows of sqX / sqZ
-  // the kernel of the last evaluation: a single stationary kernel (kp) or a composite (mk), and its Kdiag (psi0 per point)
-  KernParams kp{};
-  MultiKern mk{};
-  bool multi = false;
-  double kdiag = 0.0;
+  MultiKern mk{};          // the kernel of the last evaluation
+  double kdiag = 0.0;      // its Kdiag (psi0 per point)
   // full-device evaluation (gpx_sparse_eval)
   gpx_ctx *cK = nullptr, *cB = nullptr;             // child contexts holding the factors of Kmm and of B = I + A
   double *mm[10] = {nullptr};                        // Mpad x Mpad work matrices
   double *vec = nullptr;                             // [8][P][Mpad] small vectors
   double *red = nullptr; double *h_red = nullptr;    // scalar reductions
-  double *gsum = nullptr;                            // [1 + nl + M*D] gradient pieces summed over ranks
+  double *gsum = nullptr;                            // [kernel gradient entries + M*D] gradient pieces summed over ranks
   double *hb = nullptr;                              // het noise: [2][Npad] sqrt(beta_n), beta_n
   double *hs = nullptr;                              // het noise: [2 + P][Npad] column reductions s1, s2, r (see eval)
   double trYYT = 0.0;
@@ -53,7 +50,6 @@ struct SparseState {
   bool w_ready = false;                              // mm[9] holds woodbury_inv of the current evaluation (formed by
                                                      // gpx_sparse_predictive_gradients, kept for its later calls)
   double noise = 0.0;
-  Kern kern() const { return multi ? Kern(&mk) : Kern(&kp); }
   Points xpts() const { return Points{XsT, sqX, N, Npad}; }   // this rank's data points, prepared
   Points zpts() const { return Points{ZsT, sqZ, M, Mpad}; }   // the inducing points, prepared
 };
@@ -164,8 +160,8 @@ int launched(gpx_ctx* c, int n = 1) {
 }
 // XsT / ZsT hold rows_cap stacked coordinate rows and sqX / sqZ norm_cap rows: grown when kernel k needs more (a composite
 // stacks every part's active dims, which can exceed D when parts share columns, and keeps one norm row per part)
-int ensure_rows(gpx_ctx* c, SparseState* s, Kern k) {
-  const int rows = std::max(s->rows_cap, std::max(1, k.coord_rows())), norms = std::max(s->norm_cap, k.norm_rows());
+int ensure_rows(gpx_ctx* c, SparseState* s, const MultiKern& k) {
+  const int rows = std::max(s->rows_cap, std::max(1, k.sumD)), norms = std::max(s->norm_cap, k.nparts);
   if (rows == s->rows_cap && norms == s->norm_cap) return 0;
   GPX_CUDA(cudaStreamSynchronize(c->st));
   double** ptrs[] = {&s->XsT, &s->sqX, &s->ZsT, &s->sqZ};
@@ -248,7 +244,7 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
 static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
-  const Kern k = s->kern();
+  const MultiKern& k = s->mk;
   GPX_CHECK(ensure_rows(c, s, k));
   const long Mpad = (M + TILE - 1) / TILE * TILE, Npad = s->Npad, N = s->N;
   if (Mpad != s->Mpad) {
@@ -279,8 +275,8 @@ static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
   GPX_CHECK(prep_points(c, k, s->X, N, s->D, Npad, s->XsT, s->sqX));
   GPX_CHECK(prep_points(c, k, s->Z, M, s->D, Mpad, s->ZsT, s->sqZ));
   GPX_CHECK(launched(c, 2));
-  GPX_CHECK(build_K(c, k, s->zpts(), s->xpts(), s->Kuf, Mpad));   // psi1^T: thread-mapped operand = inducing points
-  GPX_CHECK(build_K(c, k, s->xpts(), s->zpts(), s->Kfu, Npad));   // psi1: thread-mapped operand = data points
+  GPX_CHECK(build_K(c, k, s->D, s->zpts(), s->xpts(), s->Kuf, Mpad));   // psi1^T: thread-mapped operand = inducing points
+  GPX_CHECK(build_K(c, k, s->D, s->xpts(), s->zpts(), s->Kfu, Npad));   // psi1: thread-mapped operand = data points
   return launched(c, 2);
 }
 
@@ -316,18 +312,19 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
     GPX_CHECK(launched(c));
   }
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
-  const Kern k = s->kern();
-  if (s->multi) {
+  const MultiKern& k = s->mk;
+  const bool single = as_single(k, s->D, nullptr);
+  if (!single) {
     add_rank_p_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(s->dLt, Mpad, s->M, N, s->Cm, s->Yb, Npad, P);
     GPX_CHECK(launched(c));
   }
-  const int cP = s->multi ? 0 : P;
-  GradFullParams gp = grad_params(k, s->xpts(), s->zpts(), s->dLt, Mpad);
+  const int cP = single ? P : 0;
+  GradFullParams gp = grad_params(k, s->D, s->xpts(), s->zpts(), s->dLt, Mpad);
   gp.ci = s->Yb; gp.ldci = Npad; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = cP;
-  GPX_CHECK(ensure_part(s, grad_full_doubles(k, gp) * 8));
-  GPX_CHECK(grad_full_sum(c, k, gp, s->part, grad));
+  GPX_CHECK(ensure_part(s, grad_full_doubles(k, s->D, gp) * 8));
+  GPX_CHECK(grad_full_sum(c, k, s->D, gp, s->part, grad));
   // dL/dZ: gradients_X(dL_dKnm^T, Z, X): rows = inducing points, columns = data points, dL read transposed
-  GradFullParams gx = grad_params(k, s->zpts(), s->xpts(), s->dLt, Mpad);
+  GradFullParams gx = grad_params(k, s->D, s->zpts(), s->xpts(), s->dLt, Mpad);
   gx.transposed = 1; gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = s->Yb; gx.ldcj = Npad; gx.cP = cP;
   GPX_CHECK(ensure_part(s, grad_X_doubles(c, k, gx, s->D) * 8));
   return grad_X(c, k, gx, s->D, s->part, dZ);
@@ -372,7 +369,7 @@ static int binv(gpx_ctx* c, const double* UB, double* out) {
 static int build_Kmm(gpx_ctx* c, double* Kd) {
   SparseState* s = c->sparse;
   GPX_CUDA(cudaMemsetAsync(Kd, 0, (size_t)s->Mpad * s->Mpad * 8, c->st));
-  GPX_CHECK(build_K(c, s->kern(), s->zpts(), s->zpts(), Kd, s->Mpad));
+  GPX_CHECK(build_K(c, s->mk, s->D, s->zpts(), s->zpts(), Kd, s->Mpad));
   return launched(c);
 }
 // factor-and-invert the M x M matrix A (written on c's stream) on the child context ch, then U (clean upper) and
@@ -409,11 +406,6 @@ static int sparse_args(const gpx_ctx* c, const void* kern, const double* Z, int6
 // (prod.py:386-394, Kdiag = variance for every leaf kind); only the variance entry of a block depends on Kdiag.
 static void kern_grads(const SparseState* s, double ddiag, const std::vector<double>& g_knm, const std::vector<double>& g_kmm,
                        double* grad) {
-  if (!s->multi) {
-    grad[0] = ddiag + g_knm[0] + g_kmm[0];
-    for (size_t q = 1; q < g_knm.size(); q++) grad[q] = g_knm[q] + g_kmm[q];
-    return;
-  }
   const MultiKern& mk = s->mk;
   int g = 0;
   for (int p = 0; p < mk.nparts; p++) {
@@ -421,7 +413,7 @@ static void kern_grads(const SparseState* s, double ddiag, const std::vector<dou
     for (int q = 0; q < mk.nparts; q++)
       if (q != p && mk.part[q].term == mk.part[p].term) other *= mk.part[q].variance;
     const int n = part_ngrad(mk.part[p]);
-    for (int t = 0; t < n; t++) grad[g + t] = (t == 0 ? ddiag * other : 0.0) + g_knm[g + t] + g_kmm[g + t];
+    for (int t = 0; t < n; t++) grad[g + t] = (t == 0 ? ddiag * other + g_knm[g] : g_knm[g + t]) + g_kmm[g + t];
     g += n;
   }
 }
@@ -430,7 +422,7 @@ static void kern_grads(const SparseState* s, double ddiag, const std::vector<dou
 // noise_vec == nullptr: scalar noise variance `noise` (grad = [k's gradient block, noise variance]);
 // noise_vec (host, one variance per row held by this rank): grad = [k's gradient block], dL_dR (host, N x P row-major).
 // k's block: a single kernel's [variance, lengthscale..]; a composite's part blocks in order (part_ngrad entries each).
-static int sparse_eval_impl(gpx_ctx* c, Kern k, double kdiag, const double* Z, int64_t M, double noise,
+static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const double* Z, int64_t M, double noise,
                             const double* noise_vec, double* lml, double* grad, double* dZ, double* dL_dR_out) {
   const bool het = noise_vec != nullptr;
   GPX_CUDA(cudaSetDevice(c->device));
@@ -438,8 +430,7 @@ static int sparse_eval_impl(gpx_ctx* c, Kern k, double kdiag, const double* Z, i
   cudaStream_t st = c->st;
   s->have_eval = false;
   s->w_ready = false;
-  s->multi = k.mk != nullptr;
-  if (s->multi) s->mk = *k.mk; else s->kp = *k.kp;
+  s->mk = k;
   s->kdiag = kdiag;
   memset(&c->stats, 0, sizeof(c->stats));   // filled below: Kmm's attempts, the trailing updates of both factorisations
   // per-point precisions beta_n = 1 / max(variance_n, const_jitter) (var_dtc.py:79-84) and the sums over n the bound needs
@@ -465,14 +456,7 @@ static int sparse_eval_impl(gpx_ctx* c, Kern k, double kdiag, const double* Z, i
   GPX_CHECK(psi_device(c, Z, M));
   const long Mpad = s->Mpad, N = s->Ntot, Npad = s->Npad;
   const int D = s->D, P = s->P, mt = (int)(Mpad / TILE);
-  // entries of the kernel's gradient block (a single kernel: variance and nl lengthscales; the row-shard all-reduce below
-  // is single-kernel only)
-  const int nl = s->kp.ard ? D : 1;
-  int ngk = 1 + nl;
-  if (s->multi) {
-    ngk = 0;
-    for (int p = 0; p < s->mk.nparts; p++) ngk += part_ngrad(s->mk.part[p]);
-  }
+  const int ngk = kern_ngrad(s->mk);   // entries of the kernel's gradient block
   constexpr int RSPLIT = 64;
   if (!s->mm[0]) {
     for (auto& p : s->mm) GPX_CUDA(cudaMalloc(&p, (size_t)Mpad * Mpad * 8));
@@ -587,24 +571,24 @@ static int sparse_eval_impl(gpx_ctx* c, Kern k, double kdiag, const double* Z, i
     int rank = 0, G = 1;
     dist_world(c, &rank, &G);
     if (G > 1) {   // sums over this rank's data points -> totals
-      std::vector<double> h((size_t)1 + nl + (size_t)M * D);
-      memcpy(h.data(), g_knm.data(), (size_t)(1 + nl) * 8);
-      memcpy(h.data() + 1 + nl, dZ, (size_t)M * D * 8);
+      std::vector<double> h((size_t)ngk + (size_t)M * D);
+      memcpy(h.data(), g_knm.data(), (size_t)ngk * 8);
+      memcpy(h.data() + ngk, dZ, (size_t)M * D * 8);
       GPX_CUDA(cudaMemcpyAsync(s->gsum, h.data(), h.size() * 8, cudaMemcpyHostToDevice, st));
       GPX_CHECK(dist_allreduce_sum(c, s->gsum, h.size(), st));
       GPX_CUDA(cudaMemcpyAsync(h.data(), s->gsum, h.size() * 8, cudaMemcpyDeviceToHost, st));
       GPX_CUDA(cudaStreamSynchronize(st));
-      memcpy(g_knm.data(), h.data(), (size_t)(1 + nl) * 8);
-      memcpy(dZ, h.data() + 1 + nl, (size_t)M * D * 8);
+      memcpy(g_knm.data(), h.data(), (size_t)ngk * 8);
+      memcpy(dZ, h.data() + ngk, (size_t)M * D * 8);
     }
   }
   // Kmm part: kern.update_gradients_full(dL_dKmm, Z) and kern.gradients_X(dL_dKmm, Z)  (sparse_gp.py:114,117)
-  const GradFullParams gk = grad_params(s->kern(), s->zpts(), s->zpts(), Kd, Mpad);
+  const GradFullParams gk = grad_params(s->mk, D, s->zpts(), s->zpts(), Kd, Mpad);
   std::vector<double> g_kmm(ngk, 0.0), hz((size_t)M * D);
-  GPX_CHECK(ensure_part(s, grad_full_doubles(s->kern(), gk) * 8));
-  GPX_CHECK(grad_full_sum(c, s->kern(), gk, s->part, g_kmm.data()));
-  GPX_CHECK(ensure_part(s, grad_X_doubles(c, s->kern(), gk, D) * 8));
-  GPX_CHECK(grad_X(c, s->kern(), gk, D, s->part, hz.data()));
+  GPX_CHECK(ensure_part(s, grad_full_doubles(s->mk, D, gk) * 8));
+  GPX_CHECK(grad_full_sum(c, s->mk, D, gk, s->part, g_kmm.data()));
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, s->mk, gk, D) * 8));
+  GPX_CHECK(grad_X(c, s->mk, gk, D, s->part, hz.data()));
   for (size_t i = 0; i < hz.size(); i++) dZ[i] += hz[i];
   // ---- scalars on the host (var_dtc.py:237-276, homoscedastic) -----------------------------------------------------
   double trAr = 0.0, sumAD = 0.0, data_fit = 0.0;
@@ -673,18 +657,18 @@ extern "C" {
 int gpx_sparse_eval(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* Z, int64_t M,
                     double noise, double* lml, double* grad, double* dZ) {
   GPX_CHECK(sparse_args(c, lengthscale, Z, M, lml, grad, dZ, false, nullptr));
-  KernParams kp{};
-  GPX_CHECK(fill_kp(kp, kind, ard, c->sparse->D, variance, lengthscale));
-  return sparse_eval_impl(c, &kp, variance, Z, M, noise, nullptr, lml, grad, dZ, nullptr);
+  MultiKern mk;
+  GPX_CHECK(fill_single(mk, kind, ard, c->sparse->D, variance, lengthscale));
+  return sparse_eval_impl(c, mk, variance, Z, M, noise, nullptr, lml, grad, dZ, nullptr);
 }
 
 int gpx_sparse_eval_het(gpx_ctx* c, int kind, int ard, double variance, const double* lengthscale, const double* Z,
                         int64_t M, const double* noise_variances, double* lml, double* grad, double* dZ, double* dL_dR) {
   if (!noise_variances) GPX_FAIL("null argument");
   GPX_CHECK(sparse_args(c, lengthscale, Z, M, lml, grad, dZ, true, dL_dR));
-  KernParams kp{};
-  GPX_CHECK(fill_kp(kp, kind, ard, c->sparse->D, variance, lengthscale));
-  return sparse_eval_impl(c, &kp, variance, Z, M, 0.0, noise_variances, lml, grad, dZ, dL_dR);
+  MultiKern mk;
+  GPX_CHECK(fill_single(mk, kind, ard, c->sparse->D, variance, lengthscale));
+  return sparse_eval_impl(c, mk, variance, Z, M, 0.0, noise_variances, lml, grad, dZ, dL_dR);
 }
 
 int gpx_sparse_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
@@ -699,7 +683,7 @@ int gpx_sparse_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, co
   for (int p = 0; p < mk.nparts; p++)   // dL/dZ needs every part's gradients_X
     if (mk.part[p].kind == GPX_RATQUAD || mk.part[p].kind == GPX_STDPERIODIC)
       GPX_FAIL("RatQuad and StdPeriodic parts are not on the sparse evaluation (no device gradients_X)");
-  return sparse_eval_impl(c, &mk, kdiag, Z, M, het ? 0.0 : noise_variance, noise_variances, lml, grad, dZ, dL_dR);
+  return sparse_eval_impl(c, mk, kdiag, Z, M, het ? 0.0 : noise_variance, noise_variances, lml, grad, dZ, dL_dR);
 }
 
 /* which: 0 woodbury_vector (M x P row-major), 1 woodbury_inv (M x M), 2 Kmm (+1e-8 I), 3 Lm (lower, col-major) */
@@ -772,7 +756,7 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
   if (Mn < 1) GPX_FAIL("empty Xnew");
   if (c->dist) GPX_FAIL("predictive gradients are single-GPU");
   SparseState* s = c->sparse;
-  const Kern k = s->kern();
+  const MultiKern& k = s->mk;
   GPX_CHECK(pred_grad_check(k));
   GPX_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->st;
@@ -787,7 +771,7 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
   GPX_TMP_ALLOC(&V, (size_t)Mpad * pn.ld * 8, st);
   int rc = 0;
   if (cudaMemsetAsync(Kxz, 0, (size_t)pn.ld * Mpad * 8, st) != cudaSuccess) { gpx::set_error("gpx_sparse_predictive_gradients: device failure"); rc = -1; }
-  if (rc == 0) rc = build_K(c, k, pn, s->zpts(), Kxz, pn.ld);
+  if (rc == 0) rc = build_K(c, k, s->D, pn, s->zpts(), Kxz, pn.ld);
   if (rc == 0) rc = launched(c);
   if (rc == 0) {
     GemmParams pg = gemm_defaults();
@@ -810,7 +794,6 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
 // V^T = K(Xnew, Z) W and V^T K(Z, Xnew) run on the DMMA GEMM. Launches: 7, plus 5 when it forms W.
 static int sparse_joint(gpx_ctx* c, const PointSet& pn, TmpBuf& Kss, TmpBuf& mu) {
   SparseState* s = c->sparse;
-  const Kern k = s->kern();
   cudaStream_t st = c->st;
   const long Mpad = s->Mpad, L = pn.ld;
   double* W = nullptr;
@@ -825,13 +808,13 @@ static int sparse_joint(gpx_ctx* c, const PointSet& pn, TmpBuf& Kss, TmpBuf& mu)
   GPX_CHECK(part.alloc((size_t)RSPLIT * s->P * L));
   // K(Xnew, Z) with element (m, a) at m + a * L: test points thread-mapped, zero padded
   GPX_CUDA(cudaMemsetAsync(Kxz.p, 0, (size_t)L * Mpad * 8, st));
-  GPX_CHECK(build_K(c, k, pn, s->zpts(), Kxz.p, L));
+  GPX_CHECK(build_K(c, s->mk, s->D, pn, s->zpts(), Kxz.p, L));
   GPX_CHECK(launched(c));
   GPX_CHECK(gemm_nt(c, Kxz.p, L, W, Mpad, Vt.p, L, L, Mpad, Mpad, 1, 0));          // V^T = K(Xnew, Z) W (W symmetric)
   GPX_CHECK(gemm_nt(c, Vt.p, L, Kxz.p, L, prod.p, L, L, L, Mpad, 2, 0));           // V^T K(Z, Xnew), lower tiles
   GPX_CHECK(launch_row_dot(Kxz.p, L, L, s->M, s->P, s->Cm, Mpad, RSPLIT, part.p, mu.p, st));   // mu = K(Xnew, Z) wv
   GPX_CHECK(launched(c, 2));
-  GPX_CHECK(build_K(c, k, pn, pn, Kss.p, L));
+  GPX_CHECK(build_K(c, s->mk, s->D, pn, pn, Kss.p, L));
   GPX_CHECK(launched(c));
   return joint_combine(c, Kss.p, L, 0, prod.p, L, 1, pn.n, pn.n, Kss.p, L, 1);    // Sigma in place of K(Xnew)
 }
@@ -885,7 +868,7 @@ int gpx_sparse_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t Mn, con
   GPX_CHECK(joint_check(c, Xnew, Mn, z, nz, f, jitter_used, s->P));
   GPX_CUDA(cudaSetDevice(c->device));
   PointSet pn;
-  GPX_CHECK(upload_points(c, s->kern(), Xnew, Mn, s->D, pn));
+  GPX_CHECK(upload_points(c, s->mk, Xnew, Mn, s->D, pn));
   TmpBuf Kss(c->st), mu(c->st);
   GPX_CHECK(sparse_joint(c, pn, Kss, mu));
   return joint_sample(c, Kss.p, pn.ld, Mn, mu.p, pn.ld, z, nz, nz / s->P, max_tries, f, jitter_used);
@@ -899,7 +882,7 @@ int gpx_sparse_predict(gpx_ctx* c, const double* Xnew, int64_t Mn, int full_cov,
   if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to predict from");
   if (Mn < 1) GPX_FAIL("empty Xnew");
   SparseState* s = c->sparse;
-  const Kern k = s->kern();
+  const MultiKern& k = s->mk;
   const int P = s->P;
   GPX_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->st;
@@ -934,7 +917,7 @@ int gpx_sparse_predict(gpx_ctx* c, const double* Xnew, int64_t Mn, int full_cov,
     const long L = pn.ld;   // this chunk's rows padded to 128 (<= Lc)
     // K(Xc, Z) with element (m, a) at m + a * L, zero padded; V^T = K(Xc, Z) W
     GPX_CUDA(cudaMemsetAsync(Kxz.p, 0, (size_t)L * Mpad * 8, st));
-    GPX_CHECK(build_K(c, k, pn, s->zpts(), Kxz.p, L));
+    GPX_CHECK(build_K(c, k, s->D, pn, s->zpts(), Kxz.p, L));
     GPX_CHECK(launched(c));
     GPX_CHECK(gemm_nt(c, Kxz.p, L, W, Mpad, Vt.p, L, L, Mpad, Mpad, 1, 0));
     GPX_CHECK(launch_row_dot(Kxz.p, L, L, s->M, P, s->Cm, Mpad, RSPLIT, part.p, red.p, st));   // mu ([P][L])

@@ -99,7 +99,9 @@ int gpx_exact_eval_het(gpx_ctx* ctx, int kind, int ard, double variance, const d
  *           StdPeriodic       [variance, period (1 or ndims), lengthscale (1 or ndims)] (standard_periodic.py:94)
  *         A StdPeriodic part keeps one sum per active dim for its period and one for its lengthscale: 2 ndims <= 64, else
  *         the call fails with -2 (the reduction does not fit).
- * gpx_get / gpx_predict afterwards use the composite kernel. Single-GPU. */
+ * gpx_get / gpx_predict afterwards use the composite kernel. Single-GPU. A one-part description equal to a single
+ * stationary kernel (RBF .. Matern52 on the columns 0 .. D-1 in order) takes the single-kernel route, here and in every
+ * other entry that takes parts: the same bits and launches as the single-kernel entry. */
 typedef struct {
   int kind;                  /* GPX_RBF .. GPX_MATERN52, GPX_WHITE, GPX_BIAS, GPX_RATQUAD, GPX_STDPERIODIC */
   int ard;                   /* lengthscale: 0 -> points at 1 double, 1 -> at ndims doubles (StdPeriodic: GPy's ARD2) */

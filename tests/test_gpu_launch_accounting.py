@@ -77,12 +77,15 @@ def test_sparse_calls_count_every_launch():
         e.close()
 
 
-def test_kernel_calls_pdinv_and_exact_evaluation_count_every_launch():
+def test_kernel_and_part_calls_pdinv_and_exact_evaluation_count_every_launch():
+    """the part calls on the single kernel as one part (its columns in order) run the kernels of the single-kernel calls;
+    on the same covariance with the columns in reverse order they keep the composite kernels"""
     rng, X, Y = _problem(1100, 3, 1, 3)
     X2 = rng.uniform(-3, 3, (260, 3))
     ls = np.array([1.2, 1.6, 2.1])
-    part, keep = _ffi.GpxKernPart(), []   # the same kernel as one composite part
-    _ffi._fill_part(part, ("matern52", True, 0, [0, 1, 2], 1.3, ls), keep)
+    single, part, keep = _ffi.GpxKernPart(), _ffi.GpxKernPart(), []
+    _ffi._fill_part(single, ("matern52", True, 0, [0, 1, 2], 1.3, ls), keep)
+    _ffi._fill_part(part, ("matern52", True, 0, [2, 1, 0], 1.3, ls[::-1].copy()), keep)
     e = _ffi.Engine(0)
     L, h, p = _ffi.lib(), e._h, _ffi._ptr
     try:
@@ -96,17 +99,24 @@ def test_kernel_calls_pdinv_and_exact_evaluation_count_every_launch():
                 "kern_grad_full": lambda: L.gpx_kern_grad_full(h, 3, 1, 1.3, p(ls), p(X), 1100, p(x2), M, 3, p(dL), p(dv),
                                                                p(dl)),
                 "kern_grad_X": lambda: L.gpx_kern_grad_X(h, 3, 1, 1.3, p(ls), p(X), 1100, p(x2), M, 3, p(dL), p(gx)),
+                "single_part_K": lambda: L.gpx_kern_part_K(h, ctypes.byref(single), p(X), 1100, p(x2), M, 3, p(out)),
+                "single_part_grad_full": lambda: L.gpx_kern_part_grad_full(h, ctypes.byref(single), p(X), 1100, p(x2), M, 3,
+                                                                           p(dL), p(g)),
                 "kern_part_K": lambda: L.gpx_kern_part_K(h, ctypes.byref(part), p(X), 1100, p(x2), M, 3, p(out)),
                 "kern_part_grad_full": lambda: L.gpx_kern_part_grad_full(h, ctypes.byref(part), p(X), 1100, p(x2), M, 3, p(dL),
                                                                          p(g)),
             }
+            seen = {}
             for name, call in calls.items():
                 assert call() == 0
                 rc = []
-                names = _counted(e, lambda: rc.append(call()), "%s X2=%s" % (name, x2 is not None))
+                seen[name] = _counted(e, lambda: rc.append(call()), "%s X2=%s" % (name, x2 is not None))
                 assert rc == [0]
-                if name.startswith("kern_part"):   # a part of kind 0-3 runs the composite kernels
-                    assert all("multi" in k for k in names), names
+            assert sorted(seen["single_part_K"]) == sorted(seen["kern_K"]), seen
+            assert sorted(seen["single_part_grad_full"]) == sorted(seen["kern_grad_full"]), seen
+            assert not any("multi" in k for k in seen["kern_K"] + seen["kern_grad_full"]), seen
+            for name in ("kern_part_K", "kern_part_grad_full"):
+                assert all("multi" in k for k in seen[name]), seen[name]
         e.set_data(X, Y)
         e.exact_eval("matern32", True, 1.3, ls, 0.05)
         _counted(e, lambda: e.exact_eval("rbf", True, 1.3, ls, 0.05), "exact_eval (5 blocks)")
