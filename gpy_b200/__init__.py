@@ -12,6 +12,6 @@ from .kern import (RBF, Exponential, Matern32, Matern52, RatQuad, StdPeriodic, S
 from .inference import (ExactGaussianInference, Gaussian, HeteroscedasticGaussian, MixedNoise,  # noqa: F401
                         PosteriorExact)
 from .model import GP, GPHeteroscedasticRegression, GPRegression  # noqa: F401
-from .sparse import SparseGPRegression, VarDTC  # noqa: F401
+from .sparse import FITC, SparseGPRegression, VarDTC  # noqa: F401
 
 __version__ = "0.1.0"

@@ -105,6 +105,8 @@ EXPORTS = {
                                              ctypes.c_double, _dp, _dp, _dp, _dp, _dp]),
     "gpx_sparse_eval_het": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_double, _dp, _dp, ctypes.c_int64,
                                            _dp, _dp, _dp, _dp, _dp]),
+    "gpx_sparse_eval_fitc": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64,
+                                            ctypes.c_double, _dp, _dp, _dp, _dp]),
     "gpx_pdinv": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
     "gpx_get_stats": (ctypes.c_int, [_vp, ctypes.POINTER(GpxStats)]),
     "gpx_total_launches": (ctypes.c_int64, [_vp]),
@@ -412,6 +414,30 @@ class Engine(object):
         self.sM = M
         self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
         return (lml.value, grad, dZ, dR) if het else (lml.value, grad, dZ)
+
+    def sparse_eval_fitc(self, parts, Z, noise):
+        """one FITC evaluation (fitc.py:19-88 with the gradient wiring of sparse_gp.py:108-118) with the kernel described
+        by parts (as sparse_eval_multi takes them; a single kernel is one part on all columns) and a scalar noise variance
+        -> (lml, grad [every part's block, noise], dZ (M x D), dL_dKdiag (N)). A non-positive effective noise raises
+        numpy.linalg.LinAlgError naming the data point."""
+        Z = _f64(Z)
+        M = Z.shape[0]
+        arr = (GpxKernPart * len(parts))()
+        keep, ngrad = [], 0
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
+        lml = ctypes.c_double()
+        grad = np.zeros(ngrad + 1)
+        dZ = np.empty((M, self.sD))
+        dR = np.empty(self.sN)
+        rc = self._L.gpx_sparse_eval_fitc(self._h, arr, len(parts), _ptr(Z), M, float(noise), ctypes.byref(lml),
+                                          _ptr(grad), _ptr(dZ), _ptr(dR))
+        if rc > 0:
+            raise np.linalg.LinAlgError(self._L.gpx_last_error().decode())
+        check(rc, "gpx_sparse_eval_fitc")
+        self.sM = M
+        self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
+        return lml.value, grad, dZ, dR
 
     SPARSE_GET = {"woodbury_vector": 0, "woodbury_inv": 1, "Kmm": 2, "Lm": 3}
 

@@ -50,13 +50,16 @@ struct SparseState {
   bool w_ready = false;                              // mm[9] holds woodbury_inv of the current evaluation (formed by
                                                      // gpx_sparse_predictive_gradients, kept for its later calls)
   double noise = 0.0;
+  double jitter = 1e-8;                              // const_jitter of the last evaluation (VarDTC 1e-8, FITC 1e-6)
+  double *F2 = nullptr, *G = nullptr;                // FITC: Mpad x Npad, Kmm^-1 psi1^T and its columns scaled by dL_dR
   Points xpts() const { return Points{XsT, sqX, N, Npad}; }   // this rank's data points, prepared
   Points zpts() const { return Points{ZsT, sqZ, M, Mpad}; }   // the inducing points, prepared
 };
 
 namespace {
 void free_m(SparseState* s) {
-  double** ptrs[] = {&s->Z, &s->ZsT, &s->sqZ, &s->Kuf, &s->Kfu, &s->dLt, &s->Gm, &s->W2, &s->Cm, &s->vec, &s->gsum};
+  double** ptrs[] = {&s->Z, &s->ZsT, &s->sqZ, &s->Kuf, &s->Kfu, &s->dLt, &s->Gm, &s->W2, &s->Cm, &s->vec, &s->gsum,
+                     &s->F2, &s->G};
   for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
   for (auto& p : s->mm) { if (p) cudaFree(p); p = nullptr; }
   s->have_eval = false;
@@ -291,6 +294,8 @@ static int mul_psi1T(gpx_ctx* c, const double* A, double* C, int tri) {
   return launched(c);
 }
 
+static int knm_reduce(gpx_ctx* c, double* grad, double* dZ);
+
 // dL_dKnm^T = W2 psi1^T (+ rank-P term: on the fly for a single kernel, added in one pass for a composite) reduced to
 // kernel-parameter gradients and dL/dZ; W2 (device, s->W2) and C (device, s->Cm as [P][Mpad]) must be in place. Results on
 // the host.
@@ -311,6 +316,16 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
     scale_cols_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(s->dLt, Mpad, N, bvec);
     GPX_CHECK(launched(c));
   }
+  return knm_reduce(c, grad, dZ);
+}
+
+// dL_dKnm^T = dLt + sum_q C[q] (Yb[q])^T reduced to kernel-parameter gradients and dL/dZ (results on the host): dLt
+// (s->dLt), C (s->Cm, [P][Mpad]) and Yb (s->Yb, [P][Npad]) must be in place
+static int knm_reduce(gpx_ctx* c, double* grad, double* dZ) {
+  SparseState* s = c->sparse;
+  cudaStream_t st = c->st;
+  const long Mpad = s->Mpad, N = s->N, Npad = s->Npad;
+  const int P = s->P;
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
   const MultiKern& k = s->mk;
   const bool single = as_single(k, s->D, nullptr);
@@ -432,6 +447,7 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   s->w_ready = false;
   s->mk = k;
   s->kdiag = kdiag;
+  s->jitter = 1e-8;
   memset(&c->stats, 0, sizeof(c->stats));   // filled below: Kmm's attempts, the trailing updates of both factorisations
   // per-point precisions beta_n = 1 / max(variance_n, const_jitter) (var_dtc.py:79-84) and the sums over n the bound needs
   std::vector<double> hbeta, hsb;
@@ -686,7 +702,8 @@ int gpx_sparse_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, co
   return sparse_eval_impl(c, mk, kdiag, Z, M, het ? 0.0 : noise_variance, noise_variances, lml, grad, dZ, dL_dR);
 }
 
-/* which: 0 woodbury_vector (M x P row-major), 1 woodbury_inv (M x M), 2 Kmm (+1e-8 I), 3 Lm (lower, col-major) */
+/* which: 0 woodbury_vector (M x P row-major), 1 woodbury_inv (M x M), 2 Kmm (+ the evaluation's const_jitter I: 1e-8
+ * VarDTC, 1e-6 FITC), 3 Lm (lower, col-major) */
 int gpx_sparse_get(gpx_ctx* c, int which, double* out) {
   if (!c || !c->sparse || !c->sparse->have_eval || !out) GPX_FAIL("no sparse evaluation to fetch from");
   GPX_CUDA(cudaSetDevice(c->device));
@@ -712,7 +729,7 @@ int gpx_sparse_get(gpx_ctx* c, int which, double* out) {
   } else if (which == 2) {   // Kmm, rebuilt by the kernel build, + const_jitter
     src = s->mm[3];
     GPX_CHECK(build_Kmm(c, src));
-    GPX_CHECK(combine(c, src, M, 1.0, src, 0.0, nullptr, 1e-8));
+    GPX_CHECK(combine(c, src, M, 1.0, src, 0.0, nullptr, s->jitter));
   } else if (which == 3) {   // Lm, extracted from the child context's factor
     src = s->mm[3];
     GPX_CUDA(cudaStreamSynchronize(st));
@@ -933,6 +950,250 @@ int gpx_sparse_predict(gpx_ctx* c, const double* Xnew, int64_t Mn, int full_cov,
       for (int q = 0; q < P; q++) mu[(m0 + m) * P + q] = h[(size_t)q * L + m];
   }
   return 0;
+}
+
+}  // extern "C"
+
+// =================================================================================================================
+// FITC (fitc.py:19-88, Snelson & Ghahramani's SPGP) with the gradient wiring of sparse_gp.py:108-118: the per-point-noise
+// VarDTC pipeline with the effective noise sigma*_n = Kdiag + sigma^2 - s1_n (s1_n = |Lm^-1 psi1_n^T|^2) formed on the
+// device, no trace term, and the chain rule through sigma* in the gradients. The posterior has VarDTC's form
+// (woodbury_inv = Um (I - B^-1) Um^T, woodbury_vector = v = Lm^-T LB^-T b), so the sparse predict, predictive gradients and
+// samples serve it unchanged. Every N M^2 product runs on the DMMA GEMM; the per-point work is three kernels below, each
+// with a fixed reduction order.
+// =================================================================================================================
+namespace {
+constexpr int FITC_RED_BLOCKS = 256;   // partial sums of the bound: one pair per CTA, added on the host in CTA order
+// n < N: sigma*_n = kdiag + noise - s1_n (fitc.py:43), beta*_n = 1 / sigma*_n (no floor, :44), sqrt(beta*_n), Yb_n =
+// sqrt(beta*_n) y_n and the CTA's partial sums of log(beta*_n) and beta*_n y_n^2 (:60-64); the padding columns get
+// beta* = 0. bad: the first n with sigma*_n <= 0 or NaN (atomicMin: the same index whatever the schedule)
+__global__ void __launch_bounds__(256) fitc_beta_kernel(const double* __restrict__ s1, long N, long Npad, double kdiag,
+                                                        double noise, const double* __restrict__ Y, double* __restrict__ sb,
+                                                        double* __restrict__ b, double* __restrict__ Yb,
+                                                        double* __restrict__ part, int* __restrict__ bad) {
+  __shared__ double sh[2][256];
+  double slog = 0.0, sby2 = 0.0;
+  for (long n = (long)blockIdx.x * 256 + threadIdx.x; n < Npad; n += (long)gridDim.x * 256) {
+    if (n >= N) { sb[n] = 0.0; b[n] = 0.0; Yb[n] = 0.0; continue; }
+    const double sig = kdiag + noise - s1[n];
+    if (!(sig > 0.0)) atomicMin(bad, (int)n);
+    const double be = 1.0 / sig, y = Y[n];
+    sb[n] = sqrt(be); b[n] = be; Yb[n] = sqrt(be) * y;
+    slog += log(be);
+    sby2 += be * y * y;
+  }
+  sh[0][threadIdx.x] = slog; sh[1][threadIdx.x] = sby2;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) { sh[0][threadIdx.x] += sh[0][threadIdx.x + o]; sh[1][threadIdx.x] += sh[1][threadIdx.x + o]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) { part[2 * blockIdx.x] = sh[0][0]; part[2 * blockIdx.x + 1] = sh[1][0]; }
+}
+__device__ __forceinline__ double fitc_warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+// one warp per column n (8 per CTA), lanes over the M rows in a fixed order: s2_n = psi1_n P psi1_n^T = sum_a Kuf(a, n)
+// F1(a, n) with F1 = P psi1^T, (Uv)_n = sum_a Kuf(a, n) v_a, then dL_dR_n (fitc.py:67) and the rank-1 factor of dL_dKnm^T,
+// Yb_n = beta*_n (y_n - (Uv)_n) (:77-79); the padding columns get 0
+__global__ void __launch_bounds__(256) fitc_dldr_kernel(const double* __restrict__ Kuf, const double* __restrict__ F1,
+                                                        long ld, long M, long N, long Npad, const double* __restrict__ v,
+                                                        const double* __restrict__ Y, const double* __restrict__ b,
+                                                        double* __restrict__ dLdR, double* __restrict__ Yb) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long n = (long)blockIdx.x * 8 + warp;
+  if (n >= Npad) return;
+  if (n >= N) {
+    if (lane == 0) { dLdR[n] = 0.0; Yb[n] = 0.0; }
+    return;
+  }
+  const double *k = Kuf + n * ld, *f = F1 + n * ld;
+  double s2 = 0.0, uv = 0.0;
+  for (long a = lane; a < M; a += 32) {
+    const double ka = k[a];
+    s2 = fma(ka, f[a], s2);
+    uv = fma(ka, v[a], uv);
+  }
+  s2 = fitc_warp_sum(s2);
+  uv = fitc_warp_sum(uv);
+  if (lane != 0) return;
+  const double be = b[n], y = Y[n];
+  dLdR[n] = 0.5 * (s2 - 1.0 / be + y * y - 2.0 * uv * y + uv * uv) * (be * be);
+  Yb[n] = (y - uv) * be;
+}
+// dL_dKnm^T without its rank-1 term, in place of F1: -F1 diag(beta*) - 2 F2 diag(dL_dR) (fitc.py:78-80), and G = F2
+// diag(dL_dR) for the Kmm term F2 diag(dL_dR) F2^T (:73-74), over all Npad columns (the GEMM reads G to k-depth Npad);
+// rows a >= M and columns n >= N are zeroed in both
+__global__ void fitc_assemble_kernel(double* __restrict__ dLt, const double* __restrict__ F2, double* __restrict__ G,
+                                     long ld, long M, long N, long Npad, const double* __restrict__ b,
+                                     const double* __restrict__ dLdR) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ld * Npad) return;
+  const long a = i % ld, n = i / ld;
+  if (a >= M || n >= N) { dLt[i] = 0.0; G[i] = 0.0; return; }
+  const double r = dLdR[n], f2 = F2[i];
+  dLt[i] = -b[n] * dLt[i] - 2.0 * r * f2;
+  G[i] = r * f2;
+}
+}  // namespace
+
+// One FITC evaluation of the validated kernel k (Kdiag = kdiag): grad = [k's gradient block, d/d noise variance],
+// dZ (M x D), dL_dKdiag (N, or null) = dL_dR. Route (NT GEMMs over column-major operands; k-depth M reads psi1 as Kfu,
+// k-depth N reads M x N operands M-contiguous):
+//   Kmm + 1e-6 I -> Um, Lmi;  tmp = Lmi psi1^T;  s1;  sigma*, beta*;  tmp diag(sqrt beta*);  A = tmp tmp^T;  B = I + A
+//   -> UB, LBi;  t = tmp (sqrt(beta*) y);  b = LBi t, v = Lmi^T LBi^T b;  P = Um B^-1 Um^T;  Kmm^-1 = Um Um^T;
+//   F1 = P psi1^T, F2 = Kmm^-1 psi1^T;  s2, Uv, dL_dR;  dL_dKmm = 1/2 (Kmm^-1 - v v^T - P) + F2 diag(dL_dR) F2^T;
+//   dL_dKnm^T = -F1 diag(beta*) - 2 F2 diag(dL_dR) + v (beta* (y - Uv))^T;  the reductions of VarDTC
+static int fitc_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const double* Z, int64_t M, double noise,
+                          double* lml, double* grad, double* dZ, double* dL_dKdiag) {
+  GPX_CUDA(cudaSetDevice(c->device));
+  SparseState* s = c->sparse;
+  cudaStream_t st = c->st;
+  s->have_eval = false;
+  s->w_ready = false;
+  s->mk = k;
+  s->kdiag = kdiag;
+  s->jitter = 1e-6;                                                                     // fitc.py:18
+  s->noise = noise;
+  memset(&c->stats, 0, sizeof(c->stats));
+  GPX_CHECK(psi_device(c, Z, M));
+  const long Mpad = s->Mpad, N = s->N, Npad = s->Npad;
+  const int D = s->D;
+  const int ngk = kern_ngrad(s->mk);
+  constexpr int RSPLIT = 64;
+  if (!s->mm[0]) {
+    for (auto& p : s->mm) GPX_CUDA(cudaMalloc(&p, (size_t)Mpad * Mpad * 8));
+    GPX_CUDA(cudaMalloc(&s->vec, (size_t)(8 + RSPLIT) * Mpad * 8));
+  }
+  if (!s->red) {
+    GPX_CUDA(cudaMalloc(&s->red, 4096 * 8));
+    GPX_CUDA(cudaMallocHost(&s->h_red, 4096 * 8));
+  }
+  if (!s->hb) {
+    GPX_CUDA(cudaMalloc(&s->hb, (size_t)2 * Npad * 8));
+    GPX_CUDA(cudaMalloc(&s->hs, (size_t)(2 + s->P) * Npad * 8));
+  }
+  if (!s->F2) {
+    GPX_CUDA(cudaMalloc(&s->F2, (size_t)Mpad * Npad * 8));
+    GPX_CUDA(cudaMalloc(&s->G, (size_t)Mpad * Npad * 8));
+  }
+  if (!s->cK) { GPX_CHECK(gpx_create(c->device, &s->cK)); GPX_CHECK(gpx_create(c->device, &s->cB)); }
+  for (gpx_ctx* ch : {s->cK, s->cB})
+    if (ch->NB != c->NB) GPX_CHECK(gpx_set_option(ch, "nb", c->NB));
+  double *Kd = s->mm[0], *Um = s->mm[1], *Lmi = s->mm[2], *T = s->mm[3], *Ki = s->mm[4], *Bd = s->mm[5], *UB = s->mm[6],
+         *LBi = s->mm[7], *Pm = s->mm[8], *E = s->mm[9];
+  double *tv = s->vec, *vv = tv + Mpad, *Cv = vv + Mpad, *wv = Cv + Mpad, *rpart = s->vec + (size_t)8 * Mpad;
+  double *sbv = s->hb, *bv = s->hb + Npad, *s1 = s->hs, *dLdR = s->hs + Npad;
+  double* Tuf = s->dLt;   // tmp, then F1, then dL_dKnm^T
+  // Kmm + const_jitter, factored with jitchol's ladder as pdinv does (fitc.py:38-39, linalg.py:193-214)
+  GPX_CHECK(build_Kmm(c, Kd));
+  GPX_CHECK(factor_child(c, s->cK, Kd, 1e-6, nullptr, Um, Lmi));
+  c->stats.tries = s->cK->stats.tries;
+  // tmp = Li U^T (:42), s1 = its column norms, sigma*, beta* and the bound's sums over n (:43-44)
+  GPX_CHECK(mul_psi1T(c, Lmi, Tuf, 2));
+  GPX_CHECK(launch_col_sqnorm(Tuf, Mpad, M, N, s1, st));
+  GPX_CHECK(launched(c));
+  int* bad = reinterpret_cast<int*>(s->red + 2 * FITC_RED_BLOCKS);
+  GPX_CUDA(cudaMemsetAsync(bad, 0x7f, sizeof(int), st));
+  fitc_beta_kernel<<<FITC_RED_BLOCKS, 256, 0, st>>>(s1, N, Npad, kdiag, noise, s->Y, sbv, bv, s->Yb, s->red, bad);
+  GPX_CHECK(launched(c));
+  GPX_CUDA(cudaMemcpyAsync(s->h_red, s->red, (2 * FITC_RED_BLOCKS + 1) * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaStreamSynchronize(st));
+  {
+    int first;
+    memcpy(&first, s->h_red + 2 * FITC_RED_BLOCKS, sizeof(int));
+    if (first < N) {
+      gpx::set_error("FITC: the effective noise Kdiag + noise variance - Qdiag of data point " + std::to_string(first) +
+                     " is not positive (or is NaN)");
+      return 1 + first;
+    }
+  }
+  double sum_log_beta = 0.0, sum_bY2 = 0.0;
+  for (int i = 0; i < FITC_RED_BLOCKS; i++) { sum_log_beta += s->h_red[2 * i]; sum_bY2 += s->h_red[2 * i + 1]; }
+  // A = tdot(tmp diag(sqrt beta*)) + I, factored with jitchol's ladder (:47-48)
+  scale_cols_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(Tuf, Mpad, N, sbv);
+  GPX_CHECK(launched(c));
+  GPX_CHECK(gemm_nt(c, Tuf, Mpad, Tuf, Mpad, Kd, Mpad, Mpad, Mpad, Npad, 2, 0));   // A_raw, lower tiles (Kd is free)
+  GPX_CHECK(launch_row_dot(Tuf, Mpad, Mpad, N, 1, s->Yb, Npad, RSPLIT, rpart, tv, st));   // t = Li U^T diag(beta*) y
+  GPX_CHECK(launched(c, 2));
+  {
+    dim3 grid((unsigned)((Mpad + 255) / 256), (unsigned)Mpad);
+    mirror_tiles_kernel<<<grid, 256, 0, st>>>(Kd, Mpad, Mpad);
+    GPX_CHECK(launched(c));
+  }
+  GPX_CHECK(combine(c, Bd, Mpad, 1.0, Kd, 0.0, nullptr, 1.0));
+  double logdetB = 0.0;
+  GPX_CHECK(factor_child(c, s->cB, Bd, 0.0, &logdetB, UB, LBi));
+  // b = LA^-1 Li U^T beta* y, v = Li^T LA^-T b (:51-55)
+  GPX_CHECK(launch_col_dot(UB, Mpad, Mpad, Mpad, 1, tv, Mpad, vv, Mpad, st));             // b = UB^T t = LBi t
+  GPX_CHECK(launch_col_dot(LBi, Mpad, Mpad, Mpad, 1, vv, Mpad, wv, Mpad, st));            // LBi^T b
+  GPX_CHECK(launch_col_dot(Lmi, Mpad, Mpad, Mpad, 1, wv, Mpad, Cv, Mpad, st));            // v = Lmi^T LBi^T b
+  GPX_CHECK(launched(c, 3));
+  std::vector<double> hb((size_t)M);
+  GPX_CUDA(cudaMemcpyAsync(hb.data(), vv, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
+  // P = Li^T LA^-T LA^-1 Li = Um B^-1 Um^T (:56-57), Kmm^-1 = Um Um^T (pdinv), both exactly symmetric
+  GPX_CHECK(binv(c, UB, Pm));
+  GPX_CHECK(sandwich(c, Um, Pm, T, Pm));
+  GPX_CHECK(binv(c, Um, Ki));
+  // F1 = P U^T, F2 = Kmm^-1 U^T; s2, Uv, dL_dR (:66-67) and Yb = beta* (y - Uv)
+  GPX_CHECK(mul_psi1T(c, Pm, Tuf, 0));
+  GPX_CHECK(mul_psi1T(c, Ki, s->F2, 0));
+  fitc_dldr_kernel<<<(unsigned)((Npad + 7) / 8), 256, 0, st>>>(s->Kuf, Tuf, Mpad, M, N, Npad, Cv, s->Y, bv, dLdR, s->Yb);
+  GPX_CHECK(launched(c));
+  fitc_assemble_kernel<<<(unsigned)((Mpad * Npad + 255) / 256), 256, 0, st>>>(Tuf, s->F2, s->G, Mpad, M, N, Npad, bv,
+                                                                              dLdR);
+  GPX_CHECK(launched(c));
+  std::vector<double> hr((size_t)N);
+  GPX_CUDA(cudaMemcpyAsync(hr.data(), dLdR, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  // dL_dKmm = 1/2 (Kmm^-1 - v v^T - P) + F2 diag(dL_dR) F2^T (:71-74), the last term lower tiles mirrored
+  GPX_CHECK(gemm_nt(c, s->F2, Mpad, s->G, Mpad, Bd, Mpad, Mpad, Mpad, Npad, 2, 0));
+  {
+    dim3 grid((unsigned)((Mpad + 255) / 256), (unsigned)Mpad);
+    mirror_tiles_kernel<<<grid, 256, 0, st>>>(Bd, Mpad, Mpad);
+    GPX_CHECK(launched(c));
+  }
+  GPX_CHECK(combine(c, E, Mpad, 0.5, Ki, -0.5, Pm, 0.0, -0.5, Cv, 1));
+  GPX_CHECK(combine(c, Kd, Mpad, 1.0, E, 1.0, Bd, 0.0));
+  // the Knm reductions with the rank-1 term v (beta* (y - Uv))^T (:76-78), then the Kmm ones (sparse_gp.py:114,117)
+  GPX_CUDA(cudaMemcpyAsync(s->Cm, Cv, (size_t)Mpad * 8, cudaMemcpyDeviceToDevice, st));
+  std::vector<double> g_knm(ngk, 0.0), g_kmm(ngk, 0.0), hz((size_t)M * D);
+  GPX_CHECK(knm_reduce(c, g_knm.data(), dZ));
+  const GradFullParams gk = grad_params(s->mk, D, s->zpts(), s->zpts(), Kd, Mpad);
+  GPX_CHECK(ensure_part(s, grad_full_doubles(s->mk, D, gk) * 8));
+  GPX_CHECK(grad_full_sum(c, s->mk, D, gk, s->part, g_kmm.data()));
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, s->mk, gk, D) * 8));
+  GPX_CHECK(grad_X(c, s->mk, gk, D, s->part, hz.data()));
+  for (size_t i = 0; i < hz.size(); i++) dZ[i] += hz[i];
+  GPX_CUDA(cudaStreamSynchronize(st));
+  // the bound (:60-64); the Kdiag share and the noise gradient are sum(dL_dR) (sparse_gp.py:110, gaussian.py:78-79)
+  double data_fit = 0.0, sum_dR = 0.0;
+  for (long i = 0; i < M; i++) data_fit += hb[i] * hb[i];
+  for (long n = 0; n < N; n++) sum_dR += hr[n];
+  const double log2pi = 1.8378770664093453;
+  *lml = -0.5 * (double)N * log2pi - 0.5 * logdetB + 0.5 * sum_log_beta - 0.5 * sum_bY2 + 0.5 * data_fit;
+  kern_grads(s, sum_dR, g_knm, g_kmm, grad);
+  grad[ngk] = sum_dR;
+  if (dL_dKdiag) memcpy(dL_dKdiag, hr.data(), (size_t)N * 8);
+  s->have_eval = true;
+  return 0;
+}
+
+extern "C" {
+
+int gpx_sparse_eval_fitc(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
+                         double noise_variance, double* lml, double* grad, double* dZ, double* dL_dKdiag) {
+  GPX_CHECK(sparse_args(c, parts, Z, M, lml, grad, dZ, false, nullptr));
+  if (c->dist) GPX_FAIL("FITC is single-GPU");
+  if (c->sparse->P != 1) GPX_FAIL("FITC takes one output column (fitc.py reshapes v to a column)");
+  MultiKern mk;
+  double kdiag;
+  GPX_CHECK(fill_mk(mk, parts, nparts, c->sparse->D, &kdiag));
+  for (int p = 0; p < mk.nparts; p++)   // dL/dZ needs every part's gradients_X
+    if (mk.part[p].kind == GPX_RATQUAD || mk.part[p].kind == GPX_STDPERIODIC)
+      GPX_FAIL("RatQuad and StdPeriodic parts are not on the sparse evaluation (no device gradients_X)");
+  return fitc_eval_impl(c, mk, kdiag, Z, M, noise_variance, lml, grad, dZ, dL_dKdiag);
 }
 
 }  // extern "C"

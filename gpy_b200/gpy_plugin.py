@@ -21,6 +21,8 @@ The sparse model is a drop-in the same way — the reference's own `GPy.core.Spa
 handles carrying the gradients the device already reduced; `SparseGP._update_gradients` (core/sparse_gp.py:108-119) then
 calls the kernel's `update_gradients_diag / update_gradients_full / gradients_X` exactly as written there and gets those
 numbers back (the N x M matrix dL_dKnm never exists).
+`B.FITC` (over GPy's own `FITC`) does the same with ONE `gpx_sparse_eval_fitc`, and hands back the real N-vector
+`dL_dKdiag` beside the handles.
 
 The methods `K`, `Kdiag`, `update_gradients_full`, `update_gradients_diag`, `gradients_X` are defined in the class bodies on purpose:
 `KernCallsViaSlicerMeta` only wraps names it finds in the class dict (GPy/kern/src/kernel_slice_operations.py:14-57), and
@@ -375,33 +377,107 @@ def _make_vardtc(base, kernel_types, ffi):
             if Z_tilde is not None:
                 lml += Z_tilde                                     # var_dtc.py:166-170
             dL_dKdiag = -0.5 * P * beta                            # _compute_dL_dpsi: dL_dpsi0 (:218)
-            diag = dL_dKdiag.sum()
-            knm, zeros, i = [], [], 0
-            for j, (leaf, t) in enumerate(leaves):
-                n = _leaf_ngrad(leaf)
-                g = np.array(grad[i:i + n], dtype=np.float64)
-                other = 1.0
-                for q, (l2, t2) in enumerate(leaves):
-                    if q != j and t2 == t:
-                        other *= float(np.asarray(l2.variance).reshape(-1)[0])
-                g[0] -= diag * other
-                knm.append(g)
-                zeros.append(np.zeros(n))
-                i += n
-            key = _composite_key(kern)
-            h_knm = SparseDeviceGradient(key, "knm", (N, M), None, None, dZ, part_grads=knm)
-            h_kmm = SparseDeviceGradient(key, "kmm", (M, M), None, None, np.zeros_like(dZ), part_grads=zeros)
-            return LazySparsePosterior(eng, key, Zs), lml, {"dL_dKmm": h_kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": h_knm,
-                                                           "dL_dthetaL": dL_dthetaL, "dL_dm": None}
+            h_knm, h_kmm = _composite_handles(kern, leaves, grad, dL_dKdiag.sum(), dZ, N, M)
+            return LazySparsePosterior(eng, h_knm._key, Zs), lml, {"dL_dKmm": h_kmm, "dL_dKdiag": dL_dKdiag,
+                                                                  "dL_dKnm": h_knm, "dL_dthetaL": dL_dthetaL,
+                                                                  "dL_dm": None}
 
     B200VarDTC.__name__ = B200VarDTC.__qualname__ = "VarDTC"
     return B200VarDTC
 
 
+def _composite_handles(kern, leaves, grad, diag, dZ, N, M):
+    """the dL_dKnm / dL_dKmm handles of a fused composite sparse evaluation. GPy's stock update_gradients_diag runs first
+    (sparse_gp.py:110) and gives each leaf sum(dL_dKdiag) = diag times the other variances of its term (add.py:79-80,
+    prod.py:386-394); the dL_dKnm handle carries each leaf's total minus that share, the dL_dKmm handle zeros."""
+    knm, zeros, i = [], [], 0
+    for j, (leaf, t) in enumerate(leaves):
+        n = _leaf_ngrad(leaf)
+        g = np.array(grad[i:i + n], dtype=np.float64)
+        other = 1.0
+        for q, (l2, t2) in enumerate(leaves):
+            if q != j and t2 == t:
+                other *= float(np.asarray(l2.variance).reshape(-1)[0])
+        g[0] -= diag * other
+        knm.append(g)
+        zeros.append(np.zeros(n))
+        i += n
+    key = _composite_key(kern)
+    return (SparseDeviceGradient(key, "knm", (N, M), None, None, dZ, part_grads=knm),
+            SparseDeviceGradient(key, "kmm", (M, M), None, None, np.zeros_like(dZ), part_grads=zeros))
+
+
+def _make_fitc(base, kernel_types, ffi):
+    from .sparse import LazySparsePosterior
+
+    class B200FITC(base):
+        """GPy.inference.latent_function_inference.FITC with the whole evaluation on the device (gpx_sparse_eval_fitc) for
+        a plugin stationary kernel or a B.Add / B.Prod over plugin stationary leaves and GPy's own White / Bias, Gaussian
+        noise, one output column and no mean function; anything else goes to the stock method (fitc.py:19-88), which
+        raises what the reference raises. The grad dict has the stock keys: dL_dKnm / dL_dKmm are handles of the
+        gradients the device already reduced (as B.VarDTC returns them), dL_dKdiag is the real N-vector dL_dR (:67)."""
+
+        def __init__(self, device=0, engine=None):
+            super(B200FITC, self).__init__()
+            self.device, self._engine, self._data_key = device, engine, _DataKey()
+
+        @property
+        def engine(self):
+            if self._engine is None:
+                self._engine = ffi.Engine(self.device)
+            return self._engine
+
+        def invalidate_data(self):
+            self._data_key.invalidate()
+
+        def __getstate__(self):
+            d = dict(self.__dict__)
+            d["_engine"], d["_data_key"] = None, _DataKey()
+            return d
+
+        def inference(self, kern, X, Z, likelihood, Y, mean_function=None, Y_metadata=None):
+            leaves = _flatten(kern) if hasattr(kern, "_gpx_is_prod") else None
+            if leaves is not None and any(not (hasattr(l, "_gpx_kind") or type(l).__name__ in ("White", "Bias"))
+                                          for l, _ in leaves):
+                leaves = None                                      # RatQuad / StdPeriodic: no device gradients_X
+            variance = np.asarray(likelihood.gaussian_variance(Y_metadata), dtype=np.float64).reshape(-1)
+            if ((leaves is None and not isinstance(kern, kernel_types)) or not isinstance(X, np.ndarray)
+                    or mean_function is not None or variance.size > 1 or np.shape(Y)[1] != 1):
+                return super(B200FITC, self).inference(kern, X, Z, likelihood, Y, mean_function, Y_metadata)
+            Xs = np.ascontiguousarray(kern._slice_X(np.asarray(X)), dtype=np.float64)
+            Zs = np.ascontiguousarray(kern._slice_X(np.asarray(Z)), dtype=np.float64)
+            Yc = np.ascontiguousarray(Y, dtype=np.float64)
+            N, M = Yc.shape[0], Zs.shape[0]
+            eng = self.engine
+            if not self._data_key.matches(Xs, Yc):
+                eng.sparse_set_data(Xs, Yc)
+                self._data_key.remember(Xs, Yc)
+            if leaves is not None:
+                parts = [_leaf_descriptor(l, t) for (l, t) in leaves]
+            else:
+                k, ard, var, ls = kern._gpx_theta()
+                parts = [(k, ard, 0, list(range(Xs.shape[1])), var, ls)]
+            lml, grad, dZ, dL_dR = eng.sparse_eval_fitc(parts, Zs, float(variance[0]))
+            dL_dthetaL = likelihood.exact_inference_gradients(dL_dR, Y_metadata)          # fitc.py:82
+            if leaves is not None:
+                knm, kmm = _composite_handles(kern, leaves, grad, dL_dR.sum(), dZ, N, M)
+                key = knm._key
+            else:
+                key = kern._gpx_state_key()
+                dlen = np.atleast_1d(grad[1:-1])
+                knm = SparseDeviceGradient(key, "knm", (N, M), grad[0] - dL_dR.sum(), dlen, dZ)
+                kmm = SparseDeviceGradient(key, "kmm", (M, M), 0.0, np.zeros_like(dlen), np.zeros_like(dZ))
+            return LazySparsePosterior(eng, key, Zs), lml, {"dL_dKmm": kmm, "dL_dKdiag": dL_dR, "dL_dKnm": knm,
+                                                           "dL_dthetaL": dL_dthetaL}
+
+    B200FITC.__name__ = B200FITC.__qualname__ = "FITC"
+    return B200FITC
+
+
 def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None,
-         RatQuad=None, StdPeriodic=None):
-    """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC
-    optional: the sparse model; RatQuad / StdPeriodic optional: leaves the composite evaluation knows, alone or inside
+         RatQuad=None, StdPeriodic=None, FITC=None):
+    """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC /
+    FITC optional: the sparse model; RatQuad / StdPeriodic optional: leaves the composite evaluation knows, alone or inside
     Add / Prod)."""
     kernels = {n: _make_kernel(b, _KINDS[n], ffi) for n, b in
                (("RBF", RBF), ("Exponential", Exponential), ("Matern32", Matern32), ("Matern52", Matern52))}
@@ -498,6 +574,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
     extra = {}
     if VarDTC is not None:
         extra["VarDTC"] = _make_vardtc(VarDTC, kernel_types, ffi)
+    if FITC is not None:
+        extra["FITC"] = _make_fitc(FITC, kernel_types, ffi)
     return types.SimpleNamespace(ExactGaussianInference=B200ExactGaussianInference, **kernels, **extra)
 
 
@@ -510,6 +588,7 @@ def _returns_tuple(kern, X):
 def load():
     """Plugin classes over an installed GPy."""
     import GPy
-    from GPy.inference.latent_function_inference import ExactGaussianInference, VarDTC
+    from GPy.inference.latent_function_inference import FITC, ExactGaussianInference, VarDTC
     return make(GPy.kern.RBF, GPy.kern.Exponential, GPy.kern.Matern32, GPy.kern.Matern52, ExactGaussianInference,
-                Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic)
+                Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic,
+                FITC=FITC)

@@ -1,7 +1,8 @@
-"""Host-side mirror of GPy's sparse GP regression (VarDTC), computing the N-dependent work on the H100.
+"""Host-side mirror of GPy's sparse GP regression (VarDTC and FITC), computing the N-dependent work on the H100.
 
 Mirrors:
     GPy.inference.latent_function_inference.VarDTC.inference   GPy/inference/latent_function_inference/var_dtc.py:66-215
+    GPy.inference.latent_function_inference.FITC.inference     GPy/inference/latent_function_inference/fitc.py:19-88
     GPy.core.SparseGP.parameters_changed / _update_gradients   GPy/core/sparse_gp.py:76-119
     GPy.models.SparseGPRegression                              GPy/models/sparse_gp_regression.py:33-59
 (Gaussian likelihood, certain inputs, no mean function — BASELINE.json configs[4]; scalar noise through gpx_sparse_eval,
@@ -210,6 +211,79 @@ class VarDTC(object):
             "part_grads": blocks, "dZ": dZ, "dL_dthetaL": dL_dthetaL, "num_data": num_data}
 
 
+class FITC(object):
+    """Drop-in for GPy's FITC (fitc.py:11-88, Snelson & Ghahramani's SPGP): inference(kern, X, Z, likelihood, Y,
+    mean_function=None, Y_metadata=None) -> (posterior, log_marginal, grad_dict), with the reference's argument order and
+    exceptions. ONE gpx_sparse_eval_fitc call does the whole evaluation and the gradient reductions of sparse_gp.py:108-118;
+    the grad dict has VarDTC's shape (`dvariance` / `dlengthscale` or `part_grads`, `dZ`, `dL_dthetaL`) plus the N-vector
+    `dL_dKdiag`. The posterior (woodbury_inv = Kmm^-1 - P, woodbury_vector = v, fitc.py:86) serves predict, predictive
+    gradients and samples on the device like VarDTC's. Select it as the reference's tests do (GPy/testing/fitc.py:31):
+    `m.inference_method = gpy_b200.FITC()`."""
+
+    const_jitter = 1e-6  # fitc.py:18
+
+    def __init__(self, device=0, engine=None):
+        self.device, self._engine, self._data_key = device, engine, _DataKey()
+
+    @property
+    def engine(self):
+        if self._engine is None:
+            self._engine = _ffi.Engine(self.device)
+        return self._engine
+
+    def on_optimization_start(self):
+        pass
+
+    def on_optimization_end(self):
+        pass
+
+    def invalidate_data(self):
+        self._data_key.invalidate()
+
+    def inference(self, kern, X, Z, likelihood, Y, mean_function=None, Y_metadata=None):
+        assert mean_function is None, "inference with a mean function not implemented"                 # fitc.py:21
+        sigma_n = np.asarray(likelihood.gaussian_variance(Y_metadata), dtype=np.float64)
+        if sigma_n.size > 1:                                                                               # :27-29
+            raise NotImplementedError("no hetero noise with this implementation of FITC")
+        Y = np.ascontiguousarray(Y, dtype=np.float64)
+        num_data, output_dim = Y.shape
+        if output_dim != 1:   # the reference fails on tdot(v.reshape(-1, 1)) + P (:71) with a broadcasting ValueError
+            raise ValueError("FITC takes one output column (fitc.py:71 reshapes v to a column); Y has %d" % output_dim)
+        leaves = None if single_kernel(kern) else flatten_parts(kern)
+        for k in ([kern] if leaves is None else [q for q, _ in leaves]):
+            if isinstance(k, (RatQuad, StdPeriodic)):
+                raise NotImplementedError("gpy_b200.FITC: %s is not on the device's sparse evaluation (RBF, Exponential, "
+                                          "Matern32, Matern52, White, Bias and their sums and products are)"
+                                          % type(k).__name__)
+        if leaves is None and not isinstance(kern, Stationary):
+            raise TypeError("gpy_b200.FITC accelerates gpy_b200.kern stationary kernels and sums / products of them "
+                            "with White and Bias")
+        if leaves is None:
+            Xs, Zs = kern._slice_X(X), kern._slice_X(Z)
+            kind, ard, var, ls = kern._theta()
+            parts, key = [(kind, ard, 0, list(range(Xs.shape[1])), var, ls)], kern._state_key()
+        else:
+            Xs, Zs = X, Z
+            parts, key = [part_descriptor(k, t) for k, t in leaves], composite_state_key(kern)
+        Xs = np.ascontiguousarray(Xs, dtype=np.float64)
+        Zs = np.ascontiguousarray(Zs, dtype=np.float64)
+        eng = self.engine
+        if not self._data_key.matches(Xs, Y):
+            eng.sparse_set_data(Xs, Y)
+            self._data_key.remember(Xs, Y)
+        lml, grad, dZ, dR = eng.sparse_eval_fitc(parts, Zs, float(np.squeeze(sigma_n)))
+        gd = {"dZ": dZ, "dL_dKdiag": dR, "dL_dthetaL": float(grad[-1]), "num_data": num_data}
+        if leaves is None:
+            gd["dvariance"], gd["dlengthscale"] = grad[0], grad[1:-1]
+        else:
+            blocks, i = [], 0
+            for k, _ in leaves:
+                blocks.append(grad[i:i + part_ngrad(k)])
+                i += part_ngrad(k)
+            gd["part_grads"] = blocks
+        return LazySparsePosterior(eng, key, Zs), float(lml), gd
+
+
 class SparseGPRegression(Parameterized):
     """GPy.models.SparseGPRegression (sparse_gp_regression.py:33-59) / GPy.core.SparseGP (sparse_gp.py:38-119).
     Parameter (and gradient) order as in the reference: [inducing inputs, the kernel's parameters in link order (a single
@@ -248,7 +322,7 @@ class SparseGPRegression(Parameterized):
     def parameters_changed(self):
         Z = self.Z.values
         self.posterior, self._log_marginal_likelihood, gd = self.inference_method.inference(
-            self.kern, self.X, Z, self.likelihood, self.Y, self.Y_metadata)
+            self.kern, self.X, Z, self.likelihood, self.Y, Y_metadata=self.Y_metadata)
         self.grad_dict = gd
         self.likelihood.update_gradients(gd["dL_dthetaL"])                                     # :84
         if "part_grads" in gd:                                                 # :110-115 summed on the device, per leaf

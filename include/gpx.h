@@ -296,6 +296,23 @@ int gpx_sparse_eval_het(gpx_ctx* ctx, int kind, int ard, double variance, const 
 int gpx_sparse_eval_multi(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
                           double noise_variance, const double* noise_variances, double* lml, double* grad, double* dZ,
                           double* dL_dR);
+/* FITC sparse GP regression (Snelson & Ghahramani's SPGP): FITC.inference
+ * (GPy/inference/latent_function_inference/fitc.py:19-88) + SparseGP._update_gradients (core/sparse_gp.py:108-118) +
+ * Gaussian.update_gradients, for the data of gpx_sparse_set_data (P = 1) and any kernel gpx_sparse_eval_multi takes (a
+ * single RBF .. Matern52 on all columns in order runs the single-kernel kernels). Kmm + 1e-6 I is factored with jitchol's
+ * ladder as pdinv does; the effective noise sigma*_n = Kdiag + noise_variance - |Lm^-1 psi1_n^T|^2 is formed on the
+ * device, beta*_n = 1 / sigma*_n without a floor, B = I + tmp diag(beta*) tmp^T factored with the ladder. Every N M^2
+ * product runs on the DMMA GEMM (about 7 N M^2 flops, VarDTC about 4 N M^2); five M x N buffers (40 N Mz bytes, Mz = M
+ * padded to 128) are kept on the context; launches do not depend on N.
+ *   grad: the kernel's block (part blocks in order, part_ngrad entries each), then d/d noise variance = sum(dL_dR);
+ *   dZ: M x D row-major; dL_dKdiag: N values of dL_dR (fitc.py:67), or NULL.
+ * gpx_sparse_get(0..3) then return v, Kmm^-1 - P, Kmm + 1e-6 I and Lm (fitc.py:86), and gpx_sparse_predict /
+ * _predictive_gradients / _posterior_samples serve this posterior. Returns 1 + n (numpy.linalg.LinAlgError in the Python
+ * layer) with a message naming data point n when sigma*_n <= 0 or NaN, the first such n; >0 as well when a factorisation
+ * fails after the ladder. Rejected with -2: P != 1, RatQuad / StdPeriodic parts, a context with a communicator attached
+ * (single-GPU), null pointers, M < 1, no data. */
+int gpx_sparse_eval_fitc(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
+                         double noise_variance, double* lml, double* grad, double* dZ, double* dL_dKdiag);
 
 /* Measurement hooks (bench.py): device time of the last eval between CUDA events on the launching stream, the number
  * of kernels this library launched since creation, and per-phase accounting of the last eval. */
