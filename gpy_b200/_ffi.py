@@ -107,6 +107,10 @@ EXPORTS = {
                                            _dp, _dp, _dp, _dp, _dp]),
     "gpx_sparse_eval_fitc": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64,
                                             ctypes.c_double, _dp, _dp, _dp, _dp]),
+    "gpx_laplace_begin": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int]),
+    "gpx_laplace_matvec": (ctypes.c_int, [_vp, _dp, _dp]),
+    "gpx_laplace_newton": (ctypes.c_int, [_vp, _dp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp]),
+    "gpx_laplace_finish": (ctypes.c_int, [_vp, _dp, _dp, _dp, ctypes.c_int, _dp, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
     "gpx_pdinv": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
     "gpx_get_stats": (ctypes.c_int, [_vp, ctypes.POINTER(GpxStats)]),
     "gpx_total_launches": (ctypes.c_int64, [_vp]),
@@ -438,6 +442,58 @@ class Engine(object):
         self.sM = M
         self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
         return lml.value, grad, dZ, dR
+
+    # ---- Laplace approximation (laplace.py:122-353) -----------------------------------------------------------------
+    def _vec(self, v, what):
+        v = _f64(np.asarray(v, dtype=np.float64).reshape(-1))
+        if v.size != self.N:
+            raise ValueError("%s must have one value per data point (%d given, N = %d)" % (what, v.size, self.N))
+        return v
+
+    def laplace_begin(self, parts):
+        """K(X, X) of the kernel described by parts (as exact_eval_multi takes them) into the buffer kept for the Laplace
+        evaluation; -> the number of kernel gradient entries"""
+        arr = (GpxKernPart * len(parts))()
+        keep, ngrad = [], 0
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
+        self.eval_serial += 1
+        check(self._L.gpx_laplace_begin(self._h, arr, len(parts)), "gpx_laplace_begin")
+        self._lap_ngrad = ngrad
+        return ngrad
+
+    def laplace_matvec(self, v):
+        """K v with the kept K -> (N, 1)"""
+        v = self._vec(v, "v")
+        out = np.empty(self.N)
+        check(self._L.gpx_laplace_matvec(self._h, _ptr(v), _ptr(out)), "gpx_laplace_matvec")
+        return out[:, None]
+
+    def laplace_newton(self, W, b, Ki_f, max_tries=5):
+        """one Newton direction (laplace.py:184-199) -> (dKi_f (N, 1), K dKi_f (N, 1), jitter); a B that stays not positive
+        definite raises numpy.linalg.LinAlgError as jitchol does"""
+        W, b, Ki_f = self._vec(W, "W"), self._vec(b, "b"), self._vec(Ki_f, "Ki_f")
+        d, Kd, jit = np.empty(self.N), np.empty(self.N), ctypes.c_double()
+        rc = self._L.gpx_laplace_newton(self._h, _ptr(W), _ptr(b), _ptr(Ki_f), int(max_tries), _ptr(d), _ptr(Kd),
+                                        ctypes.byref(jit))
+        self.eval_serial += 1
+        check(rc, "gpx_laplace_newton")
+        return d[:, None], Kd[:, None], jit.value
+
+    def laplace_finish(self, W, Ki_f, dW_df, dlik_grad_dthetaL=None, max_tries=5):
+        """the mode computations (laplace.py:243-306) -> (logdet_I_KW, diag(Ki_W_i) (N,), kernel gradient block,
+        dL_dthetaL_imp (nlik,), jitter). dlik_grad_dthetaL: nlik x N (or None)"""
+        W, Ki_f, dW_df = self._vec(W, "W"), self._vec(Ki_f, "Ki_f"), self._vec(dW_df, "dW_df")
+        g = None if dlik_grad_dthetaL is None else _f64(np.asarray(dlik_grad_dthetaL, dtype=np.float64).reshape(-1, self.N))
+        nlik = 0 if g is None else g.shape[0]
+        logdet, jit = ctypes.c_double(), ctypes.c_double()
+        diag, kgrad, imp = np.empty(self.N), np.zeros(getattr(self, "_lap_ngrad", 0)), np.zeros(nlik)
+        rc = self._L.gpx_laplace_finish(self._h, _ptr(W), _ptr(Ki_f), _ptr(dW_df), nlik, _ptr(g) if nlik else None,
+                                        int(max_tries), ctypes.byref(logdet), _ptr(diag), _ptr(kgrad),
+                                        _ptr(imp) if nlik else None, ctypes.byref(jit))
+        self.eval_serial += 1
+        check(rc, "gpx_laplace_finish")
+        return logdet.value, diag, kgrad, imp, jit.value
 
     SPARSE_GET = {"woodbury_vector": 0, "woodbury_inv": 1, "Kmm": 2, "Lm": 3}
 

@@ -139,6 +139,7 @@ int gpx_destroy(gpx_ctx* c) {
   cudaStreamSynchronize(c->st);
   dist_destroy(c);
   sparse_free(c);
+  laplace_free(c);
   if (c->cJ) gpx_destroy(c->cJ);
   free_data(c);
   for (auto e : c->ev) cudaEventDestroy(e);
@@ -198,6 +199,7 @@ int gpx_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y,
   c->N = N;
   c->have_eval = false;
   c->have_kinv = false;
+  laplace_release(c);
   // X: keep the caller's row-major layout on device; Y: SoA [P][Npad] zero padded (staged through dT)
   GPX_CUDA(cudaMemcpyAsync(c->dX, X, (size_t)N * D * 8, cudaMemcpyHostToDevice, c->st));
   GPX_CUDA(cudaMemcpyAsync(c->dT, Y, (size_t)N * P * 8, cudaMemcpyHostToDevice, c->st));
@@ -574,6 +576,16 @@ static int run_lauum(gpx_ctx* c, double* kinv_out, Recorder* rec, const KernPara
   return 0;
 }
 
+int gpx::sweep_workspace(gpx_ctx* c) {
+  Recorder rec{c};
+  return run_sweep(c, rec);
+}
+
+int gpx::lauum_store(gpx_ctx* c) {
+  GPX_CHECK(ensure_kinv(c));
+  return run_lauum(c, c->Kinv, nullptr);
+}
+
 // Ky = K(X, X) + noise + jitter (+ the per-point noise) of the context's kernel into the workspace, training points
 // prepared first. On the int8 sweep a single kernel's first block row goes first and *first_rows is the event after it, so
 // that the factorisation of the first diagonal block runs beside the rest of the build; otherwise *first_rows = nullptr.
@@ -805,6 +817,7 @@ static int exact_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, double 
   }
   c->mk = k;
   c->kdiag = kdiag;
+  laplace_release(c);
   c->noise = noise;
   c->jitter = jitter;
   c->have_eval = false;
@@ -940,6 +953,8 @@ int gpx_get(gpx_ctx* c, int which, double* out) {
     memset(out, 0, (size_t)c->N * c->N * 8);
     return dist_get_L(c, out);
   }
+  if (c->lap_post && which == GPX_GET_DLDK)
+    GPX_FAIL("the Laplace posterior keeps no dL_dK: its kernel gradient was reduced by gpx_laplace_finish");
   if (c->dist && which != GPX_GET_ALPHA)
     GPX_FAIL("sharded mode: alpha and L (collective) can be fetched; K^-1 / dL_dK / K stay distributed or are rebuilt by the caller");
   cudaStream_t st = c->st;
@@ -1163,6 +1178,7 @@ int gpx::factor_device(gpx_ctx* c, const double* dA, long lda, long N, double ji
   GPX_CHECK(bind_dummy_data(c, N));
   c->have_eval = false;
   c->have_kinv = false;
+  c->lap_begun = c->lap_post = false;
   cudaStream_t st = c->st;
   const long ld = c->Npad;
   Recorder rec{c};

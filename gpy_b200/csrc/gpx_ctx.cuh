@@ -83,6 +83,13 @@ struct gpx_ctx {
   struct SparseState* sparse = nullptr;   // sparse-GP (VarDTC) state (gpx_sparse.cu)
   gpx_ctx* cJ = nullptr;       // child context holding the factor of the last sampled covariance (gpx_joint.cu), created on
                                // first use: the caller's own factor, alpha and stats stay those of its evaluation
+  // ---- Laplace approximation (gpx_laplace.cu) ---------------------------------------------------------------------------
+  double* lapK = nullptr;      // K(X, X) of gpx_laplace_begin, Npad x Npad column-major, zero padded, kept for the evaluation
+  double* lapV = nullptr;      // the vectors of the Newton steps and of the finish, [LAP_NV][Npad]
+  long lap_cap = 0;            // Npad the two are sized for
+  bool lap_begun = false;      // lapK holds K of c->mk on the current data (released by laplace_release)
+  bool lap_post = false;       // the last evaluation is a Laplace one (gpx_laplace_finish): no dL_dK to fetch
+  std::vector<cudaEvent_t> lap_ev;
 };
 
 
@@ -104,6 +111,16 @@ int dist_allreduce_sum(gpx_ctx* c, double* buf, size_t count, cudaStream_t st); 
 void sparse_free(gpx_ctx* c);
 int factor_device(gpx_ctx* c, const double* dA, long lda, long N, double jitter0, int max_tries, double* logdet,
                   double* jitter_used);
+// the DMMA factor-and-invert sweep over the matrix a caller wrote into S (factor workspace form); the caller zeroes c->info
+// first and reads it afterwards. Launches are counted into c->eval_launches (gpx_api.cu)
+int sweep_workspace(gpx_ctx* c);
+// the plain LAUUM: U U^T of the factor in S into the lower tiles of c->Kinv (allocated on first use), one launch counted
+// into c->eval_launches (gpx_api.cu)
+int lauum_store(gpx_ctx* c);
+void laplace_free(gpx_ctx* c);     // the Laplace buffers and events (gpx_laplace.cu)
+void laplace_release(gpx_ctx* c);  // the Laplace buffers (K and the vectors, 8 Npad (Npad + 17) bytes) and flags: called by
+                                   // gpx_set_data, gpx_sparse_set_data and every exact evaluation, so that the device memory
+                                   // of a finished Laplace evaluation does not stay with the context
 
 // ---- point sets, K-builds and kernel-gradient reductions (gpx_points.cu) ----------------------------------------------
 // Temporaries of the stand-alone kernel calls and of gpx_predict: stream-ordered allocations from the device's default memory

@@ -195,6 +195,7 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
   if (!c || !X || !Y) GPX_FAIL("null argument");
   if (N < 1 || D < 1 || D > MAX_D || P < 1 || P > MAX_P) GPX_FAIL("bad shape (D <= 64, P <= 8)");
   GPX_CUDA(cudaSetDevice(c->device));
+  laplace_release(c);
   if (!c->sparse) c->sparse = new SparseState();
   SparseState* s = c->sparse;
   const long Npad = (N + TILE - 1) / TILE * TILE;

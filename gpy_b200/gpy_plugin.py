@@ -474,11 +474,69 @@ def _make_fitc(base, kernel_types, ffi):
     return B200FITC
 
 
+def _make_laplace(base, kernel_types, ffi):
+    from .laplace import Laplace as _DeviceLaplace
+
+    class B200Laplace(base):
+        """GPy.inference.latent_function_inference.Laplace with the N^2 / N^3 work on the device (gpx_laplace_*), for a
+        plugin stationary kernel or a B.Add / B.Prod over plugin leaves and GPy's own White / Bias, any GPy likelihood (its
+        own per-point terms are used), one output column and no mean function; anything else goes to the stock method
+        (laplace.py:122-146), which raises what the reference raises. dL_dK is a handle of the gradient the device already
+        reduced, as B.ExactGaussianInference returns it."""
+
+        def __init__(self, device=0, engine=None):
+            super(B200Laplace, self).__init__()
+            self.device, self._engine = device, engine
+            self._dev = None
+
+        @property
+        def engine(self):
+            if self._engine is None:
+                self._engine = ffi.Engine(self.device)
+            return self._engine
+
+        def invalidate_data(self):
+            if self._dev is not None:
+                self._dev.invalidate_data()
+
+        def __getstate__(self):
+            d = dict(self.__dict__)
+            d["_engine"], d["_dev"] = None, None
+            return d
+
+        def inference(self, kern, X, likelihood, Y, mean_function=None, Y_metadata=None):
+            leaves = None
+            if not isinstance(kern, kernel_types):
+                leaves = _flatten(kern) if hasattr(kern, "_gpx_is_prod") or hasattr(kern, "_gpx_part_kind") else None
+            if ((leaves is None and not isinstance(kern, kernel_types)) or not isinstance(X, np.ndarray)
+                    or mean_function is not None or np.ndim(Y) != 2 or np.shape(Y)[1] != 1):
+                return super(B200Laplace, self).inference(kern, X, likelihood, Y, mean_function, Y_metadata)
+            if self._dev is None:
+                self._dev = _DeviceLaplace(engine=self.engine)
+            dev = self._dev
+            dev.bad_fhat = self.bad_fhat
+            if leaves is not None:
+                parts = [_leaf_descriptor(l, t) for (l, t) in leaves]
+                Xs, key, ngrads, single = X, _composite_key(kern), [_leaf_ngrad(l) for l, _ in leaves], False
+            else:
+                Xs = kern._slice_X(X)[0] if _returns_tuple(kern, X) else kern._slice_X(X)
+                k, ard, var, ls = kern._gpx_theta()
+                parts = [(k, ard, 0, list(range(np.shape(Xs)[1])), var, ls)]
+                key, ngrads, single = kern._gpx_state_key(), [1 + np.size(ls)], True
+            out = dev.device_inference(Xs, Y, likelihood, Y_metadata, parts, key, ngrads, single)
+            self.bad_fhat, self.first_run = dev.bad_fhat, False
+            self.f_hat, self.W, self._previous_Ki_fhat = dev.f_hat, dev.W, dev._previous_Ki_fhat   # laplace.py:302-305
+            return out
+
+    B200Laplace.__name__ = B200Laplace.__qualname__ = "Laplace"
+    return B200Laplace
+
+
 def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None,
-         RatQuad=None, StdPeriodic=None, FITC=None):
+         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None):
     """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC /
-    FITC optional: the sparse model; RatQuad / StdPeriodic optional: leaves the composite evaluation knows, alone or inside
-    Add / Prod)."""
+    FITC optional: the sparse model; Laplace optional: non-Gaussian likelihoods; RatQuad / StdPeriodic optional: leaves
+    the composite evaluation knows, alone or inside Add / Prod)."""
     kernels = {n: _make_kernel(b, _KINDS[n], ffi) for n, b in
                (("RBF", RBF), ("Exponential", Exponential), ("Matern32", Matern32), ("Matern52", Matern52))}
     kernel_types = tuple(kernels.values())      # the single-kernel evaluations (exact and VarDTC) take these only
@@ -576,6 +634,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
         extra["VarDTC"] = _make_vardtc(VarDTC, kernel_types, ffi)
     if FITC is not None:
         extra["FITC"] = _make_fitc(FITC, kernel_types, ffi)
+    if Laplace is not None:
+        extra["Laplace"] = _make_laplace(Laplace, kernel_types, ffi)
     return types.SimpleNamespace(ExactGaussianInference=B200ExactGaussianInference, **kernels, **extra)
 
 
@@ -588,7 +648,7 @@ def _returns_tuple(kern, X):
 def load():
     """Plugin classes over an installed GPy."""
     import GPy
-    from GPy.inference.latent_function_inference import FITC, ExactGaussianInference, VarDTC
+    from GPy.inference.latent_function_inference import FITC, ExactGaussianInference, Laplace, VarDTC
     return make(GPy.kern.RBF, GPy.kern.Exponential, GPy.kern.Matern32, GPy.kern.Matern52, ExactGaussianInference,
                 Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic,
-                FITC=FITC)
+                FITC=FITC, Laplace=Laplace)

@@ -314,6 +314,53 @@ int gpx_sparse_eval_multi(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, 
 int gpx_sparse_eval_fitc(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
                          double noise_variance, double* lml, double* grad, double* dZ, double* dL_dKdiag);
 
+/* The Laplace approximation for a non-Gaussian likelihood (GPy/inference/latent_function_inference/laplace.py:122-353), one
+ * output column (gpx_set_data with P = 1) and no mean function. The likelihood's per-point terms stay with the caller (they
+ * are O(N)); the N^2 / N^3 work of Rasmussen's mode finding (rasm_mode, :148-231) and of the mode computations (:233-306)
+ * runs here. Every entry returns -2 with nothing touched for a null pointer, a communicator (single-GPU), P != 1, and (all
+ * but begin) no gpx_laplace_begin on the current data; > 0 (the leading minor) when B stays not positive definite after
+ * jitchol's ladder (util/linalg.py:56-75: first as it is, then mean(diag B) 1e-6 10^k added, k < max_tries; *jitter_used
+ * reports it). Launch counts below exclude F, the factor-and-invert sweep of an N x N matrix (that of gpx_pdinv), once per
+ * attempt of the ladder; none of them depends on N. gpx_get_stats afterwards: launches, tries, and per-phase times
+ * (profile option): kbuild_ms (the K-build), sweep_ms (B-build + sweep), update_ms (finish's GEMM), lauum_ms (finish's
+ * LAUUM), solve_ms (mat-vecs and their glue), total_ms.
+ *
+ * gpx_laplace_begin : kern.K(X) (:128) with the kernel of the parts (every kernel gpx_exact_eval_multi takes) into an
+ *   N x N buffer kept for the whole evaluation (8 Npad^2 bytes beside the factor workspace; it and the Newton vectors
+ *   are released by the next gpx_set_data, gpx_sparse_set_data or exact evaluation on the context). The kernel becomes
+ *   the context's kernel and the posterior of any earlier evaluation is gone. Launches: 2.
+ * gpx_laplace_matvec : Kv = K v (N values each), np.dot(K, Ki_f) of :170,:210. Launches: 2.
+ * gpx_laplace_newton : one Newton direction of rasm_mode (:184-199). W: N values clipped as the caller's likelihood clips them
+ *   for B (:319-321); b = W f + dlogpdf_df with the unclipped W (:191-193); Ki_f the current iterate. B = I + (w_i K_ij) w_j,
+ *   w = sqrt(W), is formed from the kept K in one pass and factored; a = b - w o (U U^T (w o K b)) with U = L_B^-T (the
+ *   reference forms K_Wi_i, C, Ki_W_i and I_KW_i, four N x N products, on every step; only the factor is formed here);
+ *   out: dKi_f = a - Ki_f and Kd = K dKi_f (N values each). Launches: 11 + F (+ 1 + F per extra attempt).
+ * gpx_laplace_finish : the mode computations at f_hat (:243-306) with the clipped W, Ki_f = Ki_f_hat and
+ *   dW_df = -d3logpdf_df3 (N values each):
+ *     logdet_I_KW = 2 sum log diag(L_B) (:352);
+ *     U~ = diag(w) U_B in place, so that gpx_get(LINV) returns LiW12 = L_B^-1 diag(w) (:331) and gpx_get(L) L_B;
+ *     alpha = Ki_f_hat (gpx_get(ALPHA), woodbury_vector);
+ *     diag_Ki_W_i (N) = diag(K) - the squared column norms of C = LiW12 K, C on the DMMA GEMM with A lower triangular (:347-348);
+ *     dL_dfhat = -1/2 diag_Ki_W_i o dW_df (:258);
+ *     K_Wi_i = U~ U~^T (woodbury_inv, :332) by the plain LAUUM; gpx_get(KINV) returns it;
+ *     v = dL_dfhat - K_Wi_i K dL_dfhat (= I_KW_i^T dL_dfhat);
+ *     kgrad: the kernel's gradient block (as gpx_exact_eval_multi's, without the noise entry) for dL_dK = 1/2 a a^T + a v^T
+ *       - 1/2 K_Wi_i (:267-272, a = Ki_f_hat), whose symmetric part 1/2 [(a + v)(a + v)^T - (K_Wi_i + v v^T)] is reduced from
+ *       the stored K_Wi_i + v v^T and alpha' = a + v by the exact evaluation's per-part reduction;
+ *     dL_dthetaL_imp (nlik) = dL_dfhat^T I_KW_i K g_t = (K v)^T g_t for each row g_t of dlik_grad_dthetaL (nlik x N
+ *       row-major; :293-295): one mat-vec whatever nlik.
+ *   Afterwards gpx_get(K / ALPHA / KINV / L / LINV) return K, Ki_f_hat, K_Wi_i, L_B and LiW12, gpx_get(DLDK) returns -2, and
+ *   gpx_predict, gpx_predictive_gradients, gpx_posterior_covariance and gpx_posterior_samples serve the Laplace posterior
+ *   (woodbury_vector Ki_f_hat, woodbury_inv K_Wi_i; gpx_predict does not clip the variance). Launches: 16 + nparts + F.
+ *   Peak temporaries: 16 Npad^2 bytes (LiW12 and C; 17.2 GB at N = 32768) beside the factor workspace, K^-1 and K. */
+int gpx_laplace_begin(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts);
+int gpx_laplace_matvec(gpx_ctx* ctx, const double* v, double* Kv);
+int gpx_laplace_newton(gpx_ctx* ctx, const double* W, const double* b, const double* Ki_f, int max_tries, double* dKi_f,
+                       double* Kd, double* jitter_used);
+int gpx_laplace_finish(gpx_ctx* ctx, const double* W, const double* Ki_f, const double* dW_df, int nlik,
+                       const double* dlik_grad_dthetaL, int max_tries, double* logdet_I_KW, double* diag_Ki_W_i, double* kgrad,
+                       double* dL_dthetaL_imp, double* jitter_used);
+
 /* Measurement hooks (bench.py): device time of the last eval between CUDA events on the launching stream, the number
  * of kernels this library launched since creation, and per-phase accounting of the last eval. */
 typedef struct {
