@@ -111,6 +111,11 @@ EXPORTS = {
     "gpx_laplace_matvec": (ctypes.c_int, [_vp, _dp, _dp]),
     "gpx_laplace_newton": (ctypes.c_int, [_vp, _dp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp]),
     "gpx_laplace_finish": (ctypes.c_int, [_vp, _dp, _dp, _dp, ctypes.c_int, _dp, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
+    "gpx_ep_begin": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int]),
+    "gpx_ep_start": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _dp]),
+    "gpx_ep_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_double, ctypes.c_double, ctypes.c_int,
+                                    ctypes.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
+    "gpx_ep_finish": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
     "gpx_pdinv": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
     "gpx_get_stats": (ctypes.c_int, [_vp, ctypes.POINTER(GpxStats)]),
     "gpx_total_launches": (ctypes.c_int64, [_vp]),
@@ -494,6 +499,59 @@ class Engine(object):
         self.eval_serial += 1
         check(rc, "gpx_laplace_finish")
         return logdet.value, diag, kgrad, imp, jit.value
+
+    # ---- expectation propagation (expectation_propagation.py:187-434) ----------------------------------------------
+    def ep_begin(self, parts):
+        """K(X, X) of the kernel described by parts (as laplace_begin) for EP with the probit Bernoulli likelihood; the
+        labels of set_data must be in {-1, 0, 1}. -> the number of kernel gradient entries"""
+        arr = (GpxKernPart * len(parts))()
+        keep, ngrad = [], 0
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
+        self.eval_serial += 1
+        check(self._L.gpx_ep_begin(self._h, arr, len(parts)), "gpx_ep_begin")
+        self._lap_ngrad = ngrad
+        return ngrad
+
+    def ep_start(self, tau_tilde=None, v_tilde=None, parallel=False, max_tries=5):
+        """_init_approximations (:312-328): cold without sites, warm (the recompute from them) with -> jitter"""
+        warm = tau_tilde is not None
+        t = self._vec(tau_tilde, "tau_tilde") if warm else None
+        v = self._vec(v_tilde, "v_tilde") if warm else None
+        jit = ctypes.c_double()
+        rc = self._L.gpx_ep_start(self._h, _ptr(t) if warm else None, _ptr(v) if warm else None, int(warm),
+                                  int(bool(parallel)), int(max_tries), ctypes.byref(jit))
+        self.eval_serial += 1
+        check(rc, "gpx_ep_start")
+        return jit.value
+
+    def ep_sweep(self, order, tau_tilde, v_tilde, eta=1., delta=1., parallel=False, max_tries=5):
+        """one sweep of the sites in the given order, then the recompute -> (tau_tilde, v_tilde, cav_tau, cav_v, Z_hat,
+        mu_hat, sigma2_hat, jitter), N values each but the jitter"""
+        order = np.ascontiguousarray(np.asarray(order).reshape(-1), dtype=np.int64)
+        if order.size != self.N:
+            raise ValueError("order must hold N = %d entries (%d given)" % (self.N, order.size))
+        t, v = self._vec(tau_tilde, "tau_tilde").copy(), self._vec(v_tilde, "v_tilde").copy()
+        outs = [np.empty(self.N) for _ in range(5)]
+        jit = ctypes.c_double()
+        rc = self._L.gpx_ep_sweep(self._h, order.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), float(eta), float(delta),
+                                  int(bool(parallel)), int(max_tries), _ptr(t), _ptr(v), *[_ptr(o) for o in outs],
+                                  ctypes.byref(jit))
+        self.eval_serial += 1
+        check(rc, "gpx_ep_sweep")
+        return (t, v, *outs, jit.value)
+
+    def ep_finish(self, tau_tilde, v_tilde, max_tries=5):
+        """_ep_marginal + _inference (:363-395) -> (logdet_B, v~^T Sigma v~, diag(dL_dK) (N,), kernel gradient block,
+        jitter); the posterior stays for get / predict"""
+        t, v = self._vec(tau_tilde, "tau_tilde"), self._vec(v_tilde, "v_tilde")
+        logdet, vsv, jit = ctypes.c_double(), ctypes.c_double(), ctypes.c_double()
+        diag, kgrad = np.empty(self.N), np.zeros(getattr(self, "_lap_ngrad", 0))
+        rc = self._L.gpx_ep_finish(self._h, _ptr(t), _ptr(v), int(max_tries), ctypes.byref(logdet), ctypes.byref(vsv),
+                                   _ptr(diag), _ptr(kgrad), ctypes.byref(jit))
+        self.eval_serial += 1
+        check(rc, "gpx_ep_finish")
+        return logdet.value, vsv.value, diag, kgrad, jit.value
 
     SPARSE_GET = {"woodbury_vector": 0, "woodbury_inv": 1, "Kmm": 2, "Lm": 3}
 

@@ -88,8 +88,16 @@ struct gpx_ctx {
   double* lapV = nullptr;      // the vectors of the Newton steps and of the finish, [LAP_NV][Npad]
   long lap_cap = 0;            // Npad the two are sized for
   bool lap_begun = false;      // lapK holds K of c->mk on the current data (released by laplace_release)
-  bool lap_post = false;       // the last evaluation is a Laplace one (gpx_laplace_finish): no dL_dK to fetch
+  bool lap_post = false;       // the last evaluation is a Laplace or EP one (gpx_laplace_finish, gpx_ep_finish): no dL_dK
   std::vector<cudaEvent_t> lap_ev;
+  // ---- expectation propagation (gpx_laplace.cu, on the kept K above) ----------------------------------------------------
+  double* epSig = nullptr;     // Sigma of the sequential updates, Npad x Npad, lower tiles (diagonal tiles whole), zero padded
+  double* epBlk = nullptr;     // one block of sites: S, S diag(c) (Npad x TILE each), the chain's G (TILE x TILE), c, g
+  int* epOrd = nullptr;        // the update order of a sweep (N entries)
+  bool ep_begun = false;       // gpx_ep_begin checked the labels and built K (released with the Laplace buffers)
+  bool ep_ready = false;       // mu (and Sigma or its diagonal) of gpx_ep_start / gpx_ep_sweep are on the device
+  bool ep_labels = false;      // the labels of the current data were checked by gpx_ep_begin (cleared with the buffers)
+  bool ep_full = false;        // epSig holds the whole Sigma (else only its diagonal, in the vector slot, is kept)
 };
 
 
@@ -118,7 +126,8 @@ int sweep_workspace(gpx_ctx* c);
 // into c->eval_launches (gpx_api.cu)
 int lauum_store(gpx_ctx* c);
 void laplace_free(gpx_ctx* c);     // the Laplace buffers and events (gpx_laplace.cu)
-void laplace_release(gpx_ctx* c);  // the Laplace buffers (K and the vectors, 8 Npad (Npad + 17) bytes) and flags: called by
+void laplace_release(gpx_ctx* c);  // the Laplace / EP buffers (K and the vectors, 8 Npad (Npad + 28) bytes, EP's Sigma and
+                                   // block) and flags: called by
                                    // gpx_set_data, gpx_sparse_set_data and every exact evaluation, so that the device memory
                                    // of a finished Laplace evaluation does not stay with the context
 

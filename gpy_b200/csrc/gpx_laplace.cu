@@ -1,5 +1,6 @@
 // gpx_laplace.cu — the Laplace approximation for non-Gaussian likelihoods on the device (GPy's Laplace,
-// GPy/inference/latent_function_inference/laplace.py:122-353), for one output column and no mean function.
+// GPy/inference/latent_function_inference/laplace.py:122-353), for one output column and no mean function, and expectation
+// propagation for the probit Bernoulli likelihood on the same kept K (the second half of this file).
 //
 // The likelihood's per-point quantities (W, its derivatives, the gradient terms of its parameters) are O(N) and come from the
 // caller; everything N^2 and N^3 runs here:
@@ -25,7 +26,9 @@ namespace gpx {
 
 // vectors of lapV ([LAP_NV][Npad], zero padded)
 enum { LV_W = 0, LV_SW, LV_B, LV_KIF, LV_DWDF, LV_T1, LV_Y, LV_U, LV_A, LV_D, LV_KD, LV_CSQ, LV_DIAG, LV_DLDF, LV_V,
-       LV_AP, LV_KV, LAP_NV };
+       LV_AP, LV_KV,
+       // expectation propagation: sites, their sign, cavities and moments, mu, diag(Sigma), diag(dL_dK)
+       LV_TT, LV_VT, LV_SGN, LV_CT, LV_CV, LV_ZH, LV_MH, LV_S2, LV_MU, LV_SD, LV_DL, LAP_NV };
 // the small vector glue, one thread per entry i < n (entries N <= i < n are zero on output)
 enum { LG_SQRTW = 0, LG_MULW = 1, LG_NEWTON = 2, LG_DIAG = 3, LG_V = 4 };
 
@@ -110,9 +113,12 @@ __global__ void __launch_bounds__(256) laplace_rank1_kernel(double* __restrict__
 static unsigned lap_grid_y(long n) { return (unsigned)std::max<long>(1, std::min<long>(n, 65535)); }
 
 void laplace_release(gpx_ctx* c) {
-  for (double** p : {&c->lapK, &c->lapV}) { if (*p) cudaFree(*p); *p = nullptr; }
+  for (double** p : {&c->lapK, &c->lapV, &c->epSig, &c->epBlk}) { if (*p) cudaFree(*p); *p = nullptr; }
+  if (c->epOrd) cudaFree(c->epOrd);
+  c->epOrd = nullptr;
   c->lap_cap = 0;
   c->lap_begun = c->lap_post = false;
+  c->ep_begun = c->ep_ready = c->ep_full = c->ep_labels = false;
 }
 
 void laplace_free(gpx_ctx* c) {
@@ -268,11 +274,11 @@ int gpx_laplace_begin(gpx_ctx* c, const gpx_kern_part* parts, int nparts) {
   GPX_CUDA(cudaSetDevice(c->device));
   lap_start(c);
   c->lap_begun = false;
+  c->ep_begun = c->ep_ready = false;
   c->het = false;
   const long ld = c->Npad;
   if (c->lap_cap != ld) {
-    for (double** p : {&c->lapK, &c->lapV}) { if (*p) cudaFree(*p); *p = nullptr; }
-    c->lap_cap = 0;
+    laplace_release(c);
     GPX_CUDA(cudaMalloc(&c->lapK, (size_t)ld * ld * 8));
     GPX_CUDA(cudaMalloc(&c->lapV, (size_t)LAP_NV * ld * 8));
     c->lap_cap = ld;
@@ -451,6 +457,540 @@ int gpx_laplace_finish(gpx_ctx* c, const double* W, const double* Ki_f, const do
   }
   c->have_eval = true;
   c->have_kinv = false;   // the stored matrix is K_Wi_i + v v^T: gpx_get(KINV) forms U~ U~^T again
+  c->lap_post = true;
+  return 0;
+}
+
+}  // extern "C"
+
+// ==== expectation propagation (GPy/inference/latent_function_inference/expectation_propagation.py:187-434) ===============
+// EP for the probit Bernoulli likelihood on the kept K of gpx_laplace_begin. A sequential sweep is a chain of N rank-1
+// updates of Sigma (:101-105); it runs here in blocks of TILE sites of the update order: the block's chain on its TILE x TILE
+// part G = Sigma[I, I] in one CTA (ep_chain_kernel), S = Sigma[:, I] (I + U)^-1 row by row (ep_solve_kernel, U[l, j] =
+// c_l s_l[j] for l < j), then Sigma -= S diag(c) S^T as one rank-TILE update on the DMMA GEMM's GEMM_UPDATE mode and
+// mu -= S g. That is the chain of rank-1 updates regrouped, not an approximation of it. _recompute (:129-143) is the Laplace
+// factor with tau~ in place of W.
+namespace gpx {
+
+// W. J. Cody's rational approximations (Math. Comp. 23, 1969) in the form util/univariate_Gaussian.py:26-158 evaluates
+// them, with its branch points: erfc for x / sqrt(2) >= 4 (P1, Q1), 0.469 <= x / sqrt(2) < 4 (P2, Q2), erf below (P3, Q3)
+__constant__ double EP_P1[6] = {3.05326634961232344e-1, 3.60344899949804439e-1, 1.25781726111229246e-1,
+                                1.60837851487422766e-2, 6.58749161529837803e-4, 1.63153871373020978e-2};
+__constant__ double EP_Q1[5] = {2.56852019228982242e+0, 1.87295284992346047e+0, 5.27905102951428412e-1,
+                                6.05183413124413191e-2, 2.33520497626869185e-3};
+__constant__ double EP_P2[9] = {5.64188496988670089e-1, 8.88314979438837594e+0, 6.61191906371416295e+1,
+                                2.98635138197400131e+2, 8.81952221241769090e+2, 1.71204761263407058e+3,
+                                2.05107837782607147e+3, 1.23033935479799725e+3, 2.15311535474403846e-8};
+__constant__ double EP_Q2[8] = {1.57449261107098347e+1, 1.17693950891312499e+2, 5.37181101862009858e+2,
+                                1.62138957456669019e+3, 3.29079923573345963e+3, 4.36261909014324716e+3,
+                                3.43936767414372164e+3, 1.23033935480374942e+3};
+__constant__ double EP_P3[5] = {3.16112374387056560e+0, 1.13864154151050156e+2, 3.77485237685302021e+2,
+                                3.20937758913846947e+3, 1.85777706184603153e-1};
+__constant__ double EP_Q3[4] = {2.36012909523441209e+1, 2.44024637934444173e+2, 1.28261652607737228e+3,
+                                2.84423683343917062e+3};
+constexpr double EP_LIMIT1 = 0.6629, EP_LIMIT2 = 5.6569;
+constexpr double EP_LN2PI = 1.83787706640934533908193770913, EP_LN2 = 0.69314718055994530941723212146;
+constexpr double EP_SQRTPI = 1.77245385090551602729816748334, EP_SQRT2 = 1.41421356237309504880168872421;
+
+__device__ __forceinline__ double ep_log_pdf(double z) { return -0.5 * (EP_LN2PI + z * z); }
+
+__device__ double ep_erf_r3(double y) {   // _erfRationalHelperR3
+  double nom = y * EP_P3[4], den = y;
+  for (int i = 0; i <= 2; i++) {
+    nom = (nom + EP_P3[i]) * y;
+    den = (den + EP_Q3[i]) * y;
+  }
+  return (nom + EP_P3[3]) / (den + EP_Q3[3]);
+}
+
+__device__ double ep_erf_helper(double x) {   // _erfRationalHelper: Q(x), x > 0
+  if (x >= EP_LIMIT2) {
+    const double y = 2.0 / (x * x);
+    double res = y * EP_P1[5], den = y;
+    for (int i = 0; i <= 3; i++) {
+      res = (res + EP_P1[i]) * y;
+      den = (den + EP_Q1[i]) * y;
+    }
+    return 1.0 - EP_SQRTPI * y * (res + EP_P1[4]) / (den + EP_Q1[4]);
+  }
+  const double y = x / EP_SQRT2;
+  double res = y * EP_P2[8], den = y;
+  for (int i = 0; i <= 6; i++) {
+    res = (res + EP_P2[i]) * y;
+    den = (den + EP_Q2[i]) * y;
+  }
+  return EP_SQRTPI * y * (res + EP_P2[7]) / (den + EP_Q2[7]);
+}
+
+__device__ double ep_log_cdf(double z) {   // logCdfNormal
+  if (fabs(z) < EP_LIMIT1) return log1p((z / EP_SQRT2) * ep_erf_r3(0.5 * z * z)) - EP_LN2;
+  if (z < 0.0) return ep_log_pdf(z) - log(-z) + log(ep_erf_helper(-z));
+  return log1p(-(exp(ep_log_pdf(z))) * ep_erf_helper(z) / z);
+}
+
+__device__ double ep_dlog_cdf(double z) {   // derivLogCdfNormal
+  if (fabs(z) < EP_LIMIT1) return 2.0 * exp(ep_log_pdf(z)) / (1.0 + (z / EP_SQRT2) * ep_erf_r3(0.5 * z * z));
+  if (z < 0.0) return -z / ep_erf_helper(-z);
+  const double t = exp(ep_log_pdf(z));
+  return t / (1.0 - t * ep_erf_helper(z) / z);
+}
+
+// the site outputs of a sweep (vectors of lapV)
+struct EpSites {
+  double *tt, *vt;                      // tau~, v~ (in / out)
+  double *ct, *cv, *zh, *mh, *s2;       // cavity tau and v, Z_hat, mu_hat, sigma2_hat
+  const double* sgn;                    // +1 for y = 1, -1 for y in {0, -1}
+  double eta, delta;
+};
+
+// site i of _local_updates (:333-351) at Sigma_ii = Sii and mu_i = mui: the cavity (:27-29), the probit moments
+// (bernoulli.py:59-92), the site update with tau~ clipped at machine epsilon (:52-68). -> the rank-1 update's
+// c = dtau / (1 + dtau Sii) and g = c (mu_i + Sii dv) - dv (:101-105: mu -= g s, Sigma -= c s s^T)
+__device__ void ep_site(const EpSites& e, long i, double Sii, double mui, double* c_out, double* g_out) {
+  const double tau = 1.0 / Sii - e.eta * e.tt[i];
+  const double v = mui / Sii - e.eta * e.vt[i];
+  const double sgn = e.sgn[i];
+  const double q = sqrt(tau * tau + tau);
+  const double z = sgn * v / q;
+  const double r = ep_dlog_cdf(z);
+  const double lz = ep_log_cdf(z);
+  const double mh = v / tau + sgn * r / q;
+  const double s2 = 1.0 / tau - (r / (tau * tau + tau)) * (z + r);
+  const double de = e.delta / e.eta;
+  double dtau = de * (1.0 / s2 - 1.0 / Sii);
+  const double dv = de * (mh / s2 - mui / Sii);
+  const double prev = e.tt[i];
+  double t = prev + dtau;
+  if (t < 2.220446049250313e-16) {
+    t = 2.220446049250313e-16;
+    dtau = t - prev;
+  }
+  e.tt[i] = t;
+  e.vt[i] += dv;
+  e.ct[i] = tau; e.cv[i] = v; e.zh[i] = exp(lz); e.mh[i] = mh; e.s2[i] = s2;
+  const double c = dtau / (1.0 + dtau * Sii);
+  *c_out = c;
+  *g_out = c * (mui + Sii * dv) - dv;
+}
+
+// Sigma(p, q) of the stored lower tiles (diagonal tiles whole)
+__device__ __forceinline__ double ep_sym(const double* __restrict__ S, long ld, long p, long q) {
+  return (p / TILE >= q / TILE) ? S[p + q * ld] : S[q + p * ld];
+}
+
+constexpr int EP_CHAIN_THREADS = 1024;
+constexpr int EP_SOLVE_ROWS = 64;
+constexpr int EP_CHAIN_SMEM = (TILE * TILE + 2 * TILE + 2) * 8;
+constexpr int EP_SOLVE_SMEM = (TILE * TILE + 2 * TILE + TILE * EP_SOLVE_ROWS) * 8;
+
+// the site chain of one block of m <= TILE sites I (one CTA): G = Sigma[I, I] (lower part, row-major in shared memory),
+// mu_I; for j = 0 .. m-1 the site update at (G_jj, mu_I[j]), then mu_I -= g s and G -= c s s^T on the trailing part
+// (s = G[:, j]). Column l of G keeps s_l below the diagonal (the later steps touch columns > l only): Gout = G, cg = (c, g),
+// zero beyond m.
+__global__ void __launch_bounds__(EP_CHAIN_THREADS, 1) ep_chain_kernel(const double* __restrict__ Sig, long ld,
+                                                                       const int* __restrict__ I, int m,
+                                                                       const double* __restrict__ mu, EpSites e,
+                                                                       double* __restrict__ Gout, double* __restrict__ cg) {
+  extern __shared__ double ep_sm[];
+  double* G = ep_sm;
+  double* s = G + TILE * TILE;
+  double* muI = s + TILE;
+  double* cgs = muI + TILE;
+  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
+  for (int a = ty; a < TILE; a += 32)
+    for (int b = tx; b < TILE; b += 32) G[a * TILE + b] = (a < m && b <= a) ? ep_sym(Sig, ld, I[a], I[b]) : 0.0;
+  if (tid < TILE) muI[tid] = tid < m ? mu[I[tid]] : 0.0;
+  __syncthreads();
+  for (int j = 0; j < m; j++) {
+    if (tid == 0) {
+      double c, g;
+      ep_site(e, I[j], G[j * TILE + j], muI[j], &c, &g);
+      cgs[0] = c; cgs[1] = g;
+      cg[j] = c; cg[TILE + j] = g;
+    }
+    if (tid > j && tid < m) s[tid] = G[tid * TILE + j];
+    __syncthreads();
+    const double c = cgs[0], g = cgs[1];
+    for (int a = j + 1 + ty; a < m; a += 32) {
+      const double ca = c * s[a];
+      for (int b = j + 1 + tx; b <= a; b += 32) G[a * TILE + b] -= ca * s[b];
+    }
+    if (tid > j && tid < m) muI[tid] -= g * s[tid];
+    __syncthreads();
+  }
+  for (int k = tid; k < TILE * TILE; k += EP_CHAIN_THREADS) Gout[k] = G[k];
+  if (tid >= m && tid < TILE) { cg[tid] = 0.0; cg[TILE + tid] = 0.0; }
+}
+
+// S = Sigma[:, I] (I + U)^-1, one thread per row r (forward substitution in the fixed order l = 0 .. j-1):
+// x_j = Sigma(r, I_j) - sum_l (x_l c_l) s_l[j]; out Sx = S, Sc = S diag(c) (Npad x TILE each, zero beyond m) and
+// mu_r -= sum_j x_j g_j. G, c and g are those of ep_chain_kernel.
+__global__ void __launch_bounds__(EP_SOLVE_ROWS) ep_solve_kernel(const double* __restrict__ Sig, long ld,
+                                                                 const int* __restrict__ I, int m,
+                                                                 const double* __restrict__ Gin,
+                                                                 const double* __restrict__ cg, double* __restrict__ Sx,
+                                                                 double* __restrict__ Sc, double* __restrict__ mu) {
+  extern __shared__ double ep_sm[];
+  double* G = ep_sm;
+  double* cc = G + TILE * TILE;
+  double* gg = cc + TILE;
+  double* xs = gg + TILE;   // [TILE][EP_SOLVE_ROWS]: x_l c_l of this CTA's rows
+  const int t = threadIdx.x;
+  for (int k = t; k < TILE * TILE; k += EP_SOLVE_ROWS) G[k] = Gin[k];
+  for (int k = t; k < 2 * TILE; k += EP_SOLVE_ROWS) cc[k] = cg[k];
+  __syncthreads();
+  for (long r = (long)blockIdx.x * EP_SOLVE_ROWS + t; r < ld; r += (long)gridDim.x * EP_SOLVE_ROWS) {
+    double dot = 0.0;
+    for (int j = 0; j < m; j++) {
+      double acc = ep_sym(Sig, ld, r, I[j]);
+      const double* Gj = G + j * TILE;
+      for (int l = 0; l < j; l++) acc = fma(-xs[l * EP_SOLVE_ROWS + t], Gj[l], acc);
+      const double xc = acc * cc[j];
+      xs[j * EP_SOLVE_ROWS + t] = xc;
+      Sx[r + j * ld] = acc;
+      Sc[r + j * ld] = xc;
+      dot = fma(acc, gg[j], dot);
+    }
+    for (int j = m; j < TILE; j++) { Sx[r + j * ld] = 0.0; Sc[r + j * ld] = 0.0; }
+    mu[r] -= dot;
+  }
+}
+
+// parallel_updates=True: every site from the same diag(Sigma) and mu, no rank-1 updates
+__global__ void __launch_bounds__(256) ep_parallel_kernel(long N, const double* __restrict__ sd,
+                                                          const double* __restrict__ mu, EpSites e) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  double c, g;
+  ep_site(e, i, sd[i], mu[i], &c, &g);
+}
+
+// the EP vector glue, one thread per entry i < n (entries N <= i < n of o are zero)
+enum { EV_SUB = 0, EV_DIAG = 1, EV_DLDK = 2, EV_ADDDIAG = 3, EV_SIGN = 4 };
+__global__ void __launch_bounds__(256) ep_vec_kernel(int mode, long N, long n, const double* __restrict__ x,
+                                                     const double* __restrict__ y, double* __restrict__ A, long ld,
+                                                     double add, double* __restrict__ o) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const bool in = i < N;
+  switch (mode) {
+    case EV_SUB: o[i] = in ? x[i] - y[i] : 0.0; break;                              // alpha = v~ - U~ U~^T K v~ (:139-140)
+    case EV_DIAG: o[i] = in ? (A[i + i * ld] - (x ? x[i] : 0.0)) + add : 0.0; break; // diag(K - V^T V) (+ 1e-7, :319,:326)
+    case EV_DLDK: o[i] = in ? 0.5 * (x[i] * x[i] - A[i + i * ld]) : 0.0; break;      // diag(dL_dK) (:393)
+    case EV_ADDDIAG: if (in) A[i + i * ld] += add; break;                            // diag.add(Sigma, 1e-7)
+    default: o[i] = in ? (x[i] == 1.0 ? 1.0 : -1.0) : 0.0;                          // bernoulli.py:67-70
+  }
+}
+
+}  // namespace gpx
+
+namespace {
+
+int ep_vec(gpx_ctx* c, int mode, const double* x, const double* y, double* A, double add, double* o) {
+  ep_vec_kernel<<<(unsigned)((c->Npad + 255) / 256), 256, 0, c->st>>>(mode, c->N, c->Npad, x, y, A, c->Npad, add, o);
+  c->eval_launches++;
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+EpSites ep_sites(gpx_ctx* c, double eta, double delta) {
+  EpSites e;
+  e.tt = lv(c, LV_TT); e.vt = lv(c, LV_VT); e.ct = lv(c, LV_CT); e.cv = lv(c, LV_CV); e.zh = lv(c, LV_ZH);
+  e.mh = lv(c, LV_MH); e.s2 = lv(c, LV_S2); e.sgn = lv(c, LV_SGN); e.eta = eta; e.delta = delta;
+  return e;
+}
+
+// the sweep buffers (and Sigma for sequential updates), kept until laplace_release
+int ep_alloc(gpx_ctx* c, bool full) {
+  const long ld = c->Npad;
+  if (!c->epBlk) GPX_CUDA(cudaMalloc(&c->epBlk, ((size_t)2 * ld * TILE + TILE * TILE + 2 * TILE) * 8));
+  if (!c->epOrd) GPX_CUDA(cudaMalloc(&c->epOrd, (size_t)ld * sizeof(int)));
+  if (full && !c->epSig) GPX_CUDA(cudaMalloc(&c->epSig, (size_t)ld * ld * 8));
+  return 0;
+}
+
+int ep_args(const gpx_ctx* c) {
+  if (c->dist) GPX_FAIL("expectation propagation is single-GPU");
+  if (!c->ep_begun || !c->lap_begun) GPX_FAIL("gpx_ep_begin has not been called on this data");
+  return 0;
+}
+
+// posteriorParams._recompute (:129-143) from the sites in LV_TT / LV_VT (tt: tau~ on the host, for the jitter ladder's mean):
+// B = I + S~^1/2 K S~^1/2 factored, U~ = diag(sqrt tau~) U_B, then Sigma = K - D D^T with D = K U~ (the Laplace factor with
+// tau~ for W; ep_full) or only diag(Sigma) = diag(K) - |columns of U~^T K|^2 (parallel updates); `add` on its diagonal;
+// alpha = v~ - U~ U~^T K v~ and mu = K alpha
+int ep_recompute(gpx_ctx* c, LapTimer& tm, const double* tt, int max_tries, double* jitter_used, double add) {
+  cudaStream_t st = c->st;
+  const long ld = c->Npad, N = c->N;
+  GPX_CHECK(vec(c, LG_SQRTW, nullptr, lv(c, LV_TT), nullptr, nullptr, lv(c, LV_SW)));
+  const int info = lap_factor(c, tt, max_tries, jitter_used);
+  if (info) return info;
+  GPX_CHECK(tm.mark(PH_FACTOR));
+  {
+    TmpBuf Li(st), Dm(st);
+    GPX_CHECK(Li.alloc((size_t)ld * ld));
+    GPX_CHECK(Dm.alloc((size_t)ld * ld));
+    laplace_scale_u_kernel<<<dim3((unsigned)(ld / 32), (unsigned)(ld / 32)), 256, 0, st>>>(c->S, ld, lv(c, LV_SW), N, Li.p);
+    c->eval_launches++;
+    GPX_CUDA(cudaGetLastError());
+    if (c->ep_full) {
+      GPX_CHECK(gemm_nt(c, c->lapK, ld, Li.p, ld, Dm.p, ld, ld, ld, ld, 1, 1));    // D = K Li^T, Li lower triangular
+      Li.release();
+      GPX_CUDA(cudaMemcpyAsync(c->epSig, c->lapK, (size_t)ld * ld * 8, cudaMemcpyDeviceToDevice, st));
+      GemmParams pu = gemm_defaults();
+      pu.mode = GEMM_UPDATE;
+      pu.A = Dm.p; pu.lda = ld; pu.B = Dm.p; pu.ldb = ld; pu.C = c->epSig; pu.ldc = ld;
+      pu.K = (int)ld; pu.nt = (int)(ld / TILE); pu.c0 = 0; pu.ncols = 0; pu.rlow = 0;
+      GPX_CHECK(launch_gemm(pu, dim3(1, 1), st));
+      c->eval_launches++;
+      if (add != 0.0) GPX_CHECK(ep_vec(c, EV_ADDDIAG, nullptr, nullptr, c->epSig, add, nullptr));
+    } else {
+      GPX_CHECK(gemm_nt(c, Li.p, ld, c->lapK, ld, Dm.p, ld, ld, ld, ld, 1, 2));    // C = Li K, Li lower triangular
+      GPX_CHECK(launch_col_sqnorm(Dm.p, ld, ld, N, lv(c, LV_CSQ), st));
+      c->eval_launches++;
+      GPX_CHECK(ep_vec(c, EV_DIAG, lv(c, LV_CSQ), nullptr, c->lapK, add, lv(c, LV_SD)));
+    }
+  }
+  GPX_CHECK(tm.mark(PH_GEMM));
+  GPX_CHECK(kmv(c, lv(c, LV_VT), lv(c, LV_KV)));
+  GPX_CHECK(uut_mv(c, lv(c, LV_KV), lv(c, LV_U)));
+  GPX_CHECK(ep_vec(c, EV_SUB, lv(c, LV_VT), lv(c, LV_U), nullptr, 0.0, lv(c, LV_A)));
+  GPX_CHECK(kmv(c, lv(c, LV_A), lv(c, LV_MU)));
+  GPX_CHECK(tm.mark(PH_MV));
+  return 0;
+}
+
+int ep_download(gpx_ctx* c, int slot, double* h) {
+  GPX_CUDA(cudaMemcpyAsync(h, lv(c, slot), (size_t)c->N * 8, cudaMemcpyDeviceToHost, c->st));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int gpx_ep_begin(gpx_ctx* c, const gpx_kern_part* parts, int nparts) {
+  if (!c || !parts) GPX_FAIL("null argument");
+  if (!c->S) GPX_FAIL("gpx_set_data has not been called");
+  if (c->dist) GPX_FAIL("expectation propagation is single-GPU");
+  if (c->P != 1) GPX_FAIL("expectation propagation takes one output column (P = 1)");
+  GPX_CUDA(cudaSetDevice(c->device));
+  if (!c->ep_labels) {   // once per data set: gpx_set_data releases the Laplace / EP state and with it this flag
+    std::vector<double> y((size_t)c->N);
+    GPX_CUDA(cudaMemcpy(y.data(), c->dY, (size_t)c->N * 8, cudaMemcpyDeviceToHost));
+    for (double v : y)
+      if (!(v == 1.0 || v == 0.0 || v == -1.0)) GPX_FAIL("bad value for Bernoulli observation (0, 1)");
+  }
+  GPX_CHECK(gpx_laplace_begin(c, parts, nparts));
+  c->ep_labels = true;
+  c->eval_launches = 0;
+  GPX_CHECK(ep_vec(c, EV_SIGN, c->dY, nullptr, nullptr, 0.0, lv(c, LV_SGN)));
+  if (cudaStreamSynchronize(c->st) != cudaSuccess) GPX_FAIL_DEVICE("gpx_ep_begin");
+  c->total_launches += c->eval_launches;
+  c->stats.launches += c->eval_launches;
+  c->ep_begun = true;
+  return 0;
+}
+
+int gpx_ep_start(gpx_ctx* c, const double* tau_tilde, const double* v_tilde, int warm, int parallel, int max_tries,
+                 double* jitter_used) {
+  if (!c || !jitter_used || (warm && (!tau_tilde || !v_tilde))) GPX_FAIL("null argument");
+  GPX_CHECK(ep_args(c));
+  GPX_CUDA(cudaSetDevice(c->device));
+  lap_start(c);
+  c->ep_ready = false;
+  c->ep_full = !parallel;
+  GPX_CHECK(ep_alloc(c, c->ep_full));
+  const long ld = c->Npad;
+  const int64_t l0 = c->total_launches;
+  LapTimer tm{c};
+  GPX_CHECK(tm.mark(-1));
+  *jitter_used = 0.0;
+  if (!warm) {   // _init_approximations, cold (:315-321): sites 0, Sigma = K + 1e-7 I, mu = 0
+    GPX_CUDA(cudaMemsetAsync(lv(c, LV_TT), 0, (size_t)ld * 8, c->st));
+    GPX_CUDA(cudaMemsetAsync(lv(c, LV_VT), 0, (size_t)ld * 8, c->st));
+    GPX_CUDA(cudaMemsetAsync(lv(c, LV_MU), 0, (size_t)ld * 8, c->st));
+    if (c->ep_full) {
+      GPX_CUDA(cudaMemcpyAsync(c->epSig, c->lapK, (size_t)ld * ld * 8, cudaMemcpyDeviceToDevice, c->st));
+      GPX_CHECK(ep_vec(c, EV_ADDDIAG, nullptr, nullptr, c->epSig, 1e-7, nullptr));
+    } else {
+      GPX_CHECK(ep_vec(c, EV_DIAG, nullptr, nullptr, c->lapK, 1e-7, lv(c, LV_SD)));
+    }
+  } else {       // warm (:322-326): _recompute from the kept sites, then 1e-7 on Sigma's diagonal
+    GPX_CHECK(upload(c, LV_TT, tau_tilde));
+    GPX_CHECK(upload(c, LV_VT, v_tilde));
+    const int info = ep_recompute(c, tm, tau_tilde, max_tries, jitter_used, 1e-7);
+    if (info) { lap_end(c, tm, l0); return info; }
+  }
+  GPX_CHECK(lap_end(c, tm, l0));
+  c->ep_ready = true;
+  return 0;
+}
+
+int gpx_ep_sweep(gpx_ctx* c, const int64_t* order, double eta, double delta, int parallel, int max_tries,
+                 double* tau_tilde, double* v_tilde, double* cav_tau, double* cav_v, double* Z_hat, double* mu_hat,
+                 double* sigma2_hat, double* jitter_used) {
+  if (!c || !order || !tau_tilde || !v_tilde || !cav_tau || !cav_v || !Z_hat || !mu_hat || !sigma2_hat || !jitter_used)
+    GPX_FAIL("null argument");
+  GPX_CHECK(ep_args(c));
+  if (!c->ep_ready) GPX_FAIL("gpx_ep_start has not been called since gpx_ep_begin");
+  if (!parallel != c->ep_full) GPX_FAIL("parallel must be the value gpx_ep_start was given");
+  const long N = c->N, ld = c->Npad;
+  std::vector<int> ord((size_t)N);
+  {
+    std::vector<char> seen((size_t)N, 0);
+    for (long k = 0; k < N; k++) {
+      const int64_t i = order[k];
+      if (i < 0 || i >= N || seen[(size_t)i]) GPX_FAIL("order is not a permutation of 0 .. N-1");
+      seen[(size_t)i] = 1;
+      ord[(size_t)k] = (int)i;
+    }
+  }
+  GPX_CUDA(cudaSetDevice(c->device));
+  lap_start(c);
+  cudaStream_t st = c->st;
+  const int64_t l0 = c->total_launches;
+  LapTimer tm{c};
+  GPX_CHECK(tm.mark(-1));
+  GPX_CHECK(upload(c, LV_TT, tau_tilde));
+  GPX_CHECK(upload(c, LV_VT, v_tilde));
+  const EpSites e = ep_sites(c, eta, delta);
+  if (!parallel) {   // _local_updates with the rank-1 updates (:333-351), one block of TILE sites at a time
+    GPX_CUDA(cudaMemcpyAsync(c->epOrd, ord.data(), (size_t)N * sizeof(int), cudaMemcpyHostToDevice, st));
+    GPX_CUDA(cudaFuncSetAttribute(ep_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EP_CHAIN_SMEM));
+    GPX_CUDA(cudaFuncSetAttribute(ep_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EP_SOLVE_SMEM));
+    double* Sx = c->epBlk;
+    double* Sc = Sx + (size_t)ld * TILE;
+    double* Gb = Sc + (size_t)ld * TILE;
+    double* cg = Gb + TILE * TILE;
+    const unsigned solve_grid = (unsigned)std::min<long>(ld / EP_SOLVE_ROWS, c->num_sms);
+    for (long k0 = 0; k0 < N; k0 += TILE) {
+      const int m = (int)std::min<long>(TILE, N - k0);
+      const int* I = c->epOrd + k0;
+      ep_chain_kernel<<<1, EP_CHAIN_THREADS, EP_CHAIN_SMEM, st>>>(c->epSig, ld, I, m, lv(c, LV_MU), e, Gb, cg);
+      ep_solve_kernel<<<solve_grid, EP_SOLVE_ROWS, EP_SOLVE_SMEM, st>>>(c->epSig, ld, I, m, Gb, cg, Sx, Sc, lv(c, LV_MU));
+      GPX_CUDA(cudaGetLastError());
+      GemmParams pu = gemm_defaults();   // Sigma -= S diag(c) S^T over the lower tiles, k-depth TILE
+      pu.mode = GEMM_UPDATE;
+      pu.A = Sc; pu.lda = ld; pu.B = Sx; pu.ldb = ld; pu.C = c->epSig; pu.ldc = ld;
+      pu.K = TILE; pu.nt = (int)(ld / TILE); pu.c0 = 0; pu.ncols = 0; pu.rlow = 0;
+      GPX_CHECK(launch_gemm(pu, dim3(1, 1), st));
+      c->eval_launches += 3;
+    }
+  } else {           // parallel_updates: every site from the same diag(Sigma) and mu
+    ep_parallel_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(N, lv(c, LV_SD), lv(c, LV_MU), e);
+    c->eval_launches++;
+    GPX_CUDA(cudaGetLastError());
+  }
+  GPX_CHECK(tm.mark(PH_OTHER));
+  GPX_CHECK(ep_download(c, LV_TT, tau_tilde));
+  GPX_CHECK(ep_download(c, LV_VT, v_tilde));
+  GPX_CHECK(ep_download(c, LV_CT, cav_tau));
+  GPX_CHECK(ep_download(c, LV_CV, cav_v));
+  GPX_CHECK(ep_download(c, LV_ZH, Z_hat));
+  GPX_CHECK(ep_download(c, LV_MH, mu_hat));
+  GPX_CHECK(ep_download(c, LV_S2, sigma2_hat));
+  if (cudaStreamSynchronize(st) != cudaSuccess) GPX_FAIL_DEVICE("gpx_ep_sweep");
+  c->ep_ready = false;   // Sigma and mu are those of the updates until the recompute below has run
+  const int info = ep_recompute(c, tm, tau_tilde, max_tries, jitter_used, 0.0);
+  if (info) { lap_end(c, tm, l0); return info; }
+  GPX_CHECK(lap_end(c, tm, l0));
+  c->ep_ready = true;
+  return 0;
+}
+
+int gpx_ep_finish(gpx_ctx* c, const double* tau_tilde, const double* v_tilde, int max_tries, double* logdet_B,
+                  double* vSv, double* diag_dL_dK, double* kgrad, double* jitter_used) {
+  if (!c || !tau_tilde || !v_tilde || !logdet_B || !vSv || !diag_dL_dK || !kgrad || !jitter_used)
+    GPX_FAIL("null argument");
+  GPX_CHECK(ep_args(c));
+  GPX_CUDA(cudaSetDevice(c->device));
+  lap_start(c);
+  cudaStream_t st = c->st;
+  const long ld = c->Npad, N = c->N;
+  const int nt = (int)(ld / TILE);
+  const MultiKern& mk = c->mk;
+  size_t need = 0;
+  for (int q = 0; q < mk.nparts; q++) need += (size_t)nt * nt * part_nred(mk.part[q]);
+  if (need > c->mpart_cap) {
+    if (c->mpartials) cudaFree(c->mpartials);
+    c->mpartials = nullptr;
+    c->mpart_cap = 0;
+    GPX_CUDA(cudaMalloc(&c->mpartials, need * 8));
+    c->mpart_cap = need;
+  }
+  const int64_t l0 = c->total_launches;
+  LapTimer tm{c};
+  GPX_CHECK(tm.mark(-1));
+  GPX_CHECK(upload(c, LV_TT, tau_tilde));
+  GPX_CHECK(upload(c, LV_VT, v_tilde));
+  GPX_CHECK(vec(c, LG_SQRTW, nullptr, lv(c, LV_TT), nullptr, nullptr, lv(c, LV_SW)));
+  // _ep_marginal (:363-377): B at the sites, B_logdet = 2 sum log diag(L) from the per-tile partials
+  const int info = lap_factor(c, tau_tilde, max_tries, jitter_used);
+  if (info) { lap_end(c, tm, l0); return info; }
+  std::vector<double> ldp(nt);
+  GPX_CUDA(cudaMemcpyAsync(ldp.data(), c->logdet_part, (size_t)nt * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CHECK(tm.mark(PH_FACTOR));
+  {
+    TmpBuf Li(st);
+    GPX_CHECK(Li.alloc((size_t)ld * ld));
+    laplace_scale_u_kernel<<<dim3((unsigned)(ld / 32), (unsigned)(ld / 32)), 256, 0, st>>>(c->S, ld, lv(c, LV_SW), N, Li.p);
+    c->eval_launches++;
+    GPX_CUDA(cudaGetLastError());
+  }
+  // alpha = v~ - U~ U~^T K v~ (:386-387); c->dT keeps U~^T K v~ for v~^T Sigma v~ = v~^T K v~ - |U~^T K v~|^2
+  GPX_CHECK(kmv(c, lv(c, LV_VT), lv(c, LV_KV)));
+  GPX_CHECK(uut_mv(c, lv(c, LV_KV), lv(c, LV_U)));
+  GPX_CHECK(ep_vec(c, EV_SUB, lv(c, LV_VT), lv(c, LV_U), nullptr, 0.0, c->dAlpha));
+  std::vector<double> kv((size_t)N), t((size_t)N);
+  GPX_CUDA(cudaMemcpyAsync(kv.data(), lv(c, LV_KV), (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(t.data(), c->dT, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CHECK(tm.mark(PH_MV));
+  // Wi = U~ U~^T (:389-391) into the lower tiles of c->Kinv
+  GPX_CHECK(lauum_store(c));
+  GPX_CHECK(tm.mark(PH_LAUUM));
+  // the kernel gradient of dL_dK = 1/2 (alpha alpha^T - Wi) (:393), one reduction per part, and diag(dL_dK)
+  size_t off = 0;
+  for (int q = 0; q < mk.nparts; q++) {
+    GPX_CUDA(cudaMemsetAsync(c->mpartials + off, 0, (size_t)nt * nt * part_nred(mk.part[q]) * 8, st));
+    GradKinvMultiParams gm;
+    memset(&gm, 0, sizeof(gm));
+    gm.Kinv = c->Kinv; gm.ld = ld; gm.XsT = c->dXsT; gm.sq = c->dsq; gm.ldx = ld; gm.alpha = c->dAlpha;
+    gm.N = N; gm.P = 1; gm.nt = nt; gm.part = q; gm.want_noise = 0; gm.partials = c->mpartials + off; gm.mk = mk;
+    GPX_CHECK(launch_grad_kinv_multi(gm, st));
+    c->eval_launches++;
+    off += (size_t)nt * nt * part_nred(mk.part[q]);
+  }
+  GPX_CHECK(ep_vec(c, EV_DLDK, c->dAlpha, nullptr, c->Kinv, 0.0, lv(c, LV_DL)));
+  GPX_CHECK(tm.mark(PH_OTHER));
+  std::vector<double> hp(off);
+  GPX_CUDA(cudaMemcpyAsync(hp.data(), c->mpartials, off * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CHECK(ep_download(c, LV_DL, diag_dL_dK));
+  GPX_CHECK(lap_end(c, tm, l0));
+  double s = 0.0;
+  for (int i = 0; i < nt; i++) s += ldp[i];
+  *logdet_B = s;
+  double a = 0.0, b = 0.0;
+  for (long i = 0; i < N; i++) {
+    a += v_tilde[i] * kv[i];
+    b += t[i] * t[i];
+  }
+  *vSv = a - b;
+  off = 0;
+  int g = 0;
+  for (int p = 0; p < mk.nparts; p++) {   // tile order, as grad_full_sum
+    const int nred = part_nred(mk.part[p]);
+    std::vector<double> tot(nred, 0.0);
+    for (size_t k = 0; k < (size_t)nt * nt; k++)
+      for (int q = 0; q < nred; q++) tot[q] += hp[off + k * nred + q];
+    double v;
+    for (int q = 0; q < nred; q++)
+      if (part_grad_entry(mk, p, q, tot[q], &v)) kgrad[g + q] = v;
+    g += part_ngrad(mk.part[p]);
+    off += (size_t)nt * nt * nred;
+  }
+  c->have_eval = true;
+  c->have_kinv = true;   // c->Kinv holds Wi = U~ U~^T as it is
   c->lap_post = true;
   return 0;
 }

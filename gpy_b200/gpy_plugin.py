@@ -532,10 +532,87 @@ def _make_laplace(base, kernel_types, ffi):
     return B200Laplace
 
 
+def _make_ep(base, kernel_types, ffi):
+    import sys
+    from .ep import EP as _DeviceEP
+    ref = sys.modules[base.__module__]   # the reference's gaussianApproximation, so that the stock method continues
+
+    class B200EP(base):
+        """GPy.inference.latent_function_inference.EP with the sweeps and the marginal on the device (gpx_ep_*), for a
+        plugin stationary kernel or a B.Add / B.Prod over plugin leaves and GPy's own White / Bias, GPy's Bernoulli with
+        the probit link, ndarray X, one output column and no mean function; anything else goes to the stock method
+        (expectation_propagation.py:246-277). Both keep the sites in ga_approx_old as the reference's
+        gaussianApproximation and the approximation in _ep_approximation, so either continues from the other's sites.
+        dL_dK is a handle of the gradient the device already reduced, as B.ExactGaussianInference returns it."""
+
+        def __init__(self, epsilon=1e-6, eta=1., delta=1., always_reset=False, max_iters=np.inf, ep_mode="alternated",
+                     parallel_updates=False, loading=False, device=0, engine=None):
+            super(B200EP, self).__init__(epsilon=epsilon, eta=eta, delta=delta, always_reset=always_reset,
+                                         max_iters=max_iters, ep_mode=ep_mode, parallel_updates=parallel_updates,
+                                         loading=loading)
+            self.device, self._engine = device, engine
+            self._dev = None
+
+        @property
+        def engine(self):
+            if self._engine is None:
+                self._engine = ffi.Engine(self.device)
+            return self._engine
+
+        def invalidate_data(self):
+            if self._dev is not None:
+                self._dev.invalidate_data()
+
+        def __getstate__(self):
+            d = dict(self.__dict__)
+            d["_engine"], d["_dev"] = None, None
+            return d
+
+        def _on_device(self, kern, X, likelihood, Y, mean_function, K):
+            link = getattr(likelihood, "gp_link", None)
+            return (isinstance(X, np.ndarray) and mean_function is None and K is None and np.ndim(Y) == 2
+                    and np.shape(Y)[1] == 1 and type(likelihood).__name__ == "Bernoulli"
+                    and type(link).__name__ == "Probit"
+                    and (isinstance(kern, kernel_types) or hasattr(kern, "_gpx_is_prod")
+                         or hasattr(kern, "_gpx_part_kind")))
+
+        def inference(self, kern, X, likelihood, Y, mean_function=None, Y_metadata=None, precision=None, K=None):
+            leaves = None
+            if self._on_device(kern, X, likelihood, Y, mean_function, K) and not isinstance(kern, kernel_types):
+                leaves = _flatten(kern)
+            if not self._on_device(kern, X, likelihood, Y, mean_function, K) or (
+                    leaves is None and not isinstance(kern, kernel_types)):
+                return super(B200EP, self).inference(kern, X, likelihood, Y, mean_function=mean_function,
+                                                     Y_metadata=Y_metadata, precision=precision, K=K)
+            if self._dev is None:
+                self._dev = _DeviceEP(engine=self.engine)
+            dev = self._dev
+            for name in ("epsilon", "eta", "delta", "always_reset", "max_iters", "ep_mode", "parallel_updates",
+                         "loading", "ga_approx_old", "_ep_approximation"):
+                setattr(dev, name, getattr(self, name, None))
+            if leaves is not None:
+                parts = [_leaf_descriptor(l, t) for (l, t) in leaves]
+                Xs, key, ngrads, single = X, _composite_key(kern), [_leaf_ngrad(l) for l, _ in leaves], False
+            else:
+                Xs = kern._slice_X(X)[0] if _returns_tuple(kern, X) else kern._slice_X(X)
+                k, ard, var, ls = kern._gpx_theta()
+                parts = [(k, ard, 0, list(range(np.shape(Xs)[1])), var, ls)]
+                key, ngrads, single = kern._gpx_state_key(), [1 + np.size(ls)], True
+            try:
+                return dev.device_inference(Xs, np.asarray(Y), likelihood, Y_metadata, parts, key, ngrads, single)
+            finally:
+                old = dev.ga_approx_old
+                self.ga_approx_old = None if old is None else ref.gaussianApproximation(old.v, old.tau)
+                self._ep_approximation, self.loading = dev._ep_approximation, dev.loading
+
+    B200EP.__name__ = B200EP.__qualname__ = "EP"
+    return B200EP
+
+
 def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None,
-         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None):
+         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None, EP=None):
     """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC /
-    FITC optional: the sparse model; Laplace optional: non-Gaussian likelihoods; RatQuad / StdPeriodic optional: leaves
+    FITC optional: the sparse model; Laplace / EP optional: non-Gaussian likelihoods; RatQuad / StdPeriodic optional: leaves
     the composite evaluation knows, alone or inside Add / Prod)."""
     kernels = {n: _make_kernel(b, _KINDS[n], ffi) for n, b in
                (("RBF", RBF), ("Exponential", Exponential), ("Matern32", Matern32), ("Matern52", Matern52))}
@@ -636,6 +713,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
         extra["FITC"] = _make_fitc(FITC, kernel_types, ffi)
     if Laplace is not None:
         extra["Laplace"] = _make_laplace(Laplace, kernel_types, ffi)
+    if EP is not None:
+        extra["EP"] = _make_ep(EP, kernel_types, ffi)
     return types.SimpleNamespace(ExactGaussianInference=B200ExactGaussianInference, **kernels, **extra)
 
 
@@ -648,7 +727,7 @@ def _returns_tuple(kern, X):
 def load():
     """Plugin classes over an installed GPy."""
     import GPy
-    from GPy.inference.latent_function_inference import FITC, ExactGaussianInference, Laplace, VarDTC
+    from GPy.inference.latent_function_inference import EP, FITC, ExactGaussianInference, Laplace, VarDTC
     return make(GPy.kern.RBF, GPy.kern.Exponential, GPy.kern.Matern32, GPy.kern.Matern52, ExactGaussianInference,
                 Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic,
-                FITC=FITC, Laplace=Laplace)
+                FITC=FITC, Laplace=Laplace, EP=EP)

@@ -132,6 +132,10 @@ class Bernoulli(Parameterized):
     def predictive_variance(self, mu, variance, pred_mean, Y_metadata=None):
         return np.nan
 
+    def ep_gradients(self, Y, cav_tau, cav_v, dL_dKdiag, Y_metadata=None, quad_mode='gk', boost_grad=1.):
+        """likelihood.py:273-309 for a likelihood without parameters"""
+        return np.zeros(0)
+
     def predictive_values(self, mu, var, full_cov=False, Y_metadata=None):
         """likelihood.py:734-755"""
         pred_mean = self.predictive_mean(mu, var, Y_metadata=Y_metadata)
@@ -268,6 +272,11 @@ class PosteriorLaplace(PosteriorExact):
         X2 = X1 if X2 is None else X2
         return kern.K(X1, X2) - kern.K(X1, X).dot(self.woodbury_inv).dot(kern.K(X, X2))
 
+    _var_floor = 1e-15   # the clip of the diagonal variance (posterior.py:245); PosteriorEP has none
+
+    def _floor(self, var):
+        return var if self._var_floor is None else np.clip(var, self._var_floor, np.inf)
+
     def _raw_predict(self, kern, Xnew, pred_var=None, full_cov=False):
         if not self._is_evaluated(kern):
             Kx = kern.K(pred_var, Xnew)
@@ -275,10 +284,10 @@ class PosteriorLaplace(PosteriorExact):
             if full_cov:
                 return mu, kern.K(Xnew) - np.dot(Kx.T, np.dot(self.woodbury_inv, Kx))
             var = kern.Kdiag(Xnew) - np.sum(np.dot(self.woodbury_inv, Kx) * Kx, 0)
-            return mu, np.clip(var, 1e-15, np.inf)[:, None]
+            return mu, self._floor(var)[:, None]
         self._check_fresh()
         mu, var = self._engine.predict(self._engine_X(kern, Xnew), full_cov=full_cov)
-        return mu, (var if full_cov else np.clip(var, 1e-15, np.inf))
+        return mu, (var if full_cov else self._floor(var))
 
 
 def _kernel_parts(kern):

@@ -361,6 +361,45 @@ int gpx_laplace_finish(gpx_ctx* ctx, const double* W, const double* Ki_f, const 
                        const double* dlik_grad_dthetaL, int max_tries, double* logdet_I_KW, double* diag_Ki_W_i, double* kgrad,
                        double* dL_dthetaL_imp, double* jitter_used);
 
+/* Expectation propagation for GP classification (GPy/inference/latent_function_inference/expectation_propagation.py:187-434,
+ * the EP class) with the probit Bernoulli likelihood (likelihoods/bernoulli.py:59-92), one output column and no mean
+ * function. The sites, the stopping rule, log Z~ and the update order (np.random.permutation, one per sweep) stay with the
+ * caller; the N^2 / N^3 work runs here on the K kept as gpx_laplace_begin keeps it (the same buffer and release rules).
+ * Every entry returns -2 with nothing touched for a null pointer, a communicator, P != 1 and (all but begin) no gpx_ep_begin
+ * on the current data; > 0 (the leading minor) when B = I + S~^1/2 K S~^1/2 stays not positive definite after jitchol's
+ * ladder (as gpx_laplace_newton). Launch counts exclude F, the factor sweep of B, once per attempt of the ladder.
+ *
+ * gpx_ep_begin : K(X, X) of the parts as gpx_laplace_begin builds it (:258-259). -2 also for labels outside {-1, 0, 1}
+ *   ("bad value for Bernoulli observation (0, 1)", bernoulli.py:67-72), checked once per data set. Launches: 3.
+ * gpx_ep_start : _init_approximations (:312-328). warm = 0: Sigma = K + 1e-7 I, mu = 0, the sites zero (tau_tilde and v_tilde
+ *   are not read); warm = 1: _recompute (:129-143) from the given sites (N values each), then 1e-7 on Sigma's diagonal.
+ *   parallel: the sweeps that follow update in parallel (parallel_updates=True): only diag(Sigma) is kept; otherwise the
+ *   whole Sigma (8 Npad^2 bytes beside K). Launches: 1 cold; 14 + F warm.
+ * gpx_ep_sweep : one pass of EP's loop (:296-306): _local_updates in the given order (a permutation of 0 .. N-1, else -2),
+ *   then _recompute. parallel must be the value gpx_ep_start was given. tau_tilde, v_tilde: the sites, in and out; out:
+ *   the cavity parameters cav_tau, cav_v and the moments Z_hat (= exp log Z_hat), mu_hat, sigma2_hat (N values each).
+ *   Sequential updates run in blocks of 128 sites of the order: the block's chain of rank-1 updates on Sigma[I, I] in one
+ *   CTA, S = Sigma[:, I] (I + U)^-1 with U[l, j] = c_l s_l[j] (l < j), then Sigma -= S diag(c) S^T on the DMMA GEMM
+ *   (GEMM_UPDATE, k-depth 128) and mu -= S g: the reference's chain of DSYR calls, regrouped. _recompute is the Laplace
+ *   factor with tau~ in place of W; Sigma = K - D D^T with D = K U~ (sequential) or diag(Sigma) = diag(K) - the squared
+ *   column norms of U~^T K (parallel). Launches: 3 per block + 13 + F (sequential), 15 + F (parallel).
+ *   gpx_get_stats: solve_ms holds the site updates (chains, solves, rank-128 updates), sweep_ms the factor, update_ms the
+ *   recompute's two GEMMs.
+ * gpx_ep_finish : _ep_marginal and _inference (:363-395) at the given sites: logdet_B = 2 sum log diag(L_B),
+ *   vSv = v~^T Sigma v~ = v~^T K v~ - |U~^T K v~|^2 (Sigma itself is not formed), alpha = v~ - U~ U~^T K v~ (gpx_get(ALPHA),
+ *   woodbury_vector), Wi = U~ U~^T (woodbury_inv, gpx_get(KINV)) by the plain LAUUM, diag_dL_dK (N) and kgrad, the
+ *   kernel's gradient block (as gpx_laplace_finish's) for dL_dK = 1/2 (alpha alpha^T - Wi). Afterwards gpx_get(DLDK)
+ *   returns -2 and gpx_predict, gpx_predictive_gradients, gpx_posterior_covariance and gpx_posterior_samples serve the EP
+ *   posterior (gpx_predict does not clip the variance). Launches: 11 + nparts + F. */
+int gpx_ep_begin(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts);
+int gpx_ep_start(gpx_ctx* ctx, const double* tau_tilde, const double* v_tilde, int warm, int parallel, int max_tries,
+                 double* jitter_used);
+int gpx_ep_sweep(gpx_ctx* ctx, const int64_t* order, double eta, double delta, int parallel, int max_tries,
+                 double* tau_tilde, double* v_tilde, double* cav_tau, double* cav_v, double* Z_hat, double* mu_hat,
+                 double* sigma2_hat, double* jitter_used);
+int gpx_ep_finish(gpx_ctx* ctx, const double* tau_tilde, const double* v_tilde, int max_tries, double* logdet_B,
+                  double* vSv, double* diag_dL_dK, double* kgrad, double* jitter_used);
+
 /* Measurement hooks (bench.py): device time of the last eval between CUDA events on the launching stream, the number
  * of kernels this library launched since creation, and per-phase accounting of the last eval. */
 typedef struct {
