@@ -14,6 +14,6 @@ from .inference import (ExactGaussianInference, Gaussian, HeteroscedasticGaussia
 from .model import GP, GPHeteroscedasticRegression, GPRegression  # noqa: F401
 from .sparse import FITC, SparseGPRegression, VarDTC  # noqa: F401
 from .laplace import Bernoulli, Laplace, PosteriorLaplace, StudentT  # noqa: F401
-from .ep import EP, GPClassification, PosteriorEP  # noqa: F401
+from .ep import EP, EPDTC, GPClassification, PosteriorEP, SparseGPClassification  # noqa: F401
 
 __version__ = "0.1.0"

@@ -116,6 +116,11 @@ EXPORTS = {
     "gpx_ep_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_double, ctypes.c_double, ctypes.c_int,
                                     ctypes.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     "gpx_ep_finish": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
+    "gpx_epdtc_begin": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64]),
+    "gpx_epdtc_start": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _dp, _dp, _dp]),
+    "gpx_epdtc_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_double, ctypes.c_double,
+                                       ctypes.c_int, ctypes.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
+    "gpx_epdtc_finish": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp, _dp]),
     "gpx_pdinv": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
     "gpx_get_stats": (ctypes.c_int, [_vp, ctypes.POINTER(GpxStats)]),
     "gpx_total_launches": (ctypes.c_int64, [_vp]),
@@ -552,6 +557,77 @@ class Engine(object):
         self.eval_serial += 1
         check(rc, "gpx_ep_finish")
         return logdet.value, vsv.value, diag, kgrad, jit.value
+
+    # ---- sparse expectation propagation (EPDTC, expectation_propagation.py:436-611) -----------------------------------
+    def _svec(self, v, what):
+        v = _f64(np.asarray(v, dtype=np.float64).reshape(-1))
+        if v.size != self.sN:
+            raise ValueError("%s must have one value per data point (%d given, N = %d)" % (what, v.size, self.sN))
+        return v
+
+    def epdtc_begin(self, parts, Z):
+        """Kmm, Kmn and jitchol(Kmm) of the kernel described by parts (as sparse_eval_multi takes them) at the inducing
+        inputs Z, for sparse EP with the probit Bernoulli likelihood on the data of sparse_set_data (labels in {-1, 0, 1})
+        -> the number of kernel gradient entries"""
+        Z = _f64(Z)
+        M = Z.shape[0]
+        arr = (GpxKernPart * len(parts))()
+        keep, ngrad = [], 0
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
+        rc = self._L.gpx_epdtc_begin(self._h, arr, len(parts), _ptr(Z), M)
+        if rc > 0:
+            raise np.linalg.LinAlgError(self._L.gpx_last_error().decode())
+        check(rc, "gpx_epdtc_begin")
+        self.sM = M
+        self._epdtc_ngrad = ngrad
+        return ngrad
+
+    def epdtc_start(self, tau_tilde=None, v_tilde=None, parallel=False, max_tries=5):
+        """_init_approximations (:522-551): cold without sites, warm (the recompute from them) with ->
+        (jitter, mu, Sigma_diag)"""
+        warm = tau_tilde is not None
+        t = self._svec(tau_tilde, "tau_tilde") if warm else None
+        v = self._svec(v_tilde, "v_tilde") if warm else None
+        jit, mu, sd = ctypes.c_double(), np.empty(self.sN), np.empty(self.sN)
+        rc = self._L.gpx_epdtc_start(self._h, _ptr(t) if warm else None, _ptr(v) if warm else None, int(warm),
+                                     int(bool(parallel)), int(max_tries), ctypes.byref(jit), _ptr(mu), _ptr(sd))
+        if rc > 0:
+            raise np.linalg.LinAlgError(self._L.gpx_last_error().decode())
+        check(rc, "gpx_epdtc_start")
+        return jit.value, mu, sd
+
+    def epdtc_sweep(self, order, tau_tilde, v_tilde, eta=1., delta=1., parallel=False, max_tries=5):
+        """one sweep of the sites in the given order, then the recompute -> (tau_tilde, v_tilde, cav_tau, cav_v, Z_hat,
+        mu_hat, sigma2_hat, jitter, mu, Sigma_diag)"""
+        order = np.ascontiguousarray(np.asarray(order).reshape(-1), dtype=np.int64)
+        if order.size != self.sN:
+            raise ValueError("order must hold N = %d entries (%d given)" % (self.sN, order.size))
+        t, v = self._svec(tau_tilde, "tau_tilde").copy(), self._svec(v_tilde, "v_tilde").copy()
+        outs = [np.empty(self.sN) for _ in range(5)]
+        mu, sd = np.empty(self.sN), np.empty(self.sN)
+        jit = ctypes.c_double()
+        rc = self._L.gpx_epdtc_sweep(self._h, order.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), float(eta),
+                                     float(delta), int(bool(parallel)), int(max_tries), _ptr(t), _ptr(v),
+                                     *[_ptr(o) for o in outs], ctypes.byref(jit), _ptr(mu), _ptr(sd))
+        if rc > 0:
+            raise np.linalg.LinAlgError(self._L.gpx_last_error().decode())
+        check(rc, "gpx_epdtc_sweep")
+        return (t, v, *outs, jit.value, mu, sd)
+
+    def epdtc_finish(self, tau_tilde, v_tilde, max_tries=5):
+        """VarDTC at Y = v~ / tau~ and precision tau~ (:474-482) without log Z~ -> (lml, kernel gradient block,
+        dZ (M x D), jitter); the posterior stays for sparse_get / sparse_predict"""
+        t, v = self._svec(tau_tilde, "tau_tilde"), self._svec(v_tilde, "v_tilde")
+        lml, jit = ctypes.c_double(), ctypes.c_double()
+        grad, dZ = np.zeros(getattr(self, "_epdtc_ngrad", 0)), np.empty((self.sM, self.sD))
+        rc = self._L.gpx_epdtc_finish(self._h, _ptr(t), _ptr(v), int(max_tries), ctypes.byref(lml), _ptr(grad), _ptr(dZ),
+                                      ctypes.byref(jit))
+        if rc > 0:
+            raise np.linalg.LinAlgError(self._L.gpx_last_error().decode())
+        check(rc, "gpx_epdtc_finish")
+        self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
+        return lml.value, grad, dZ, jit.value
 
     SPARSE_GET = {"woodbury_vector": 0, "woodbury_inv": 1, "Kmm": 2, "Lm": 3}
 

@@ -20,6 +20,7 @@
 
 #include "gpx_common.cuh"
 #include "gpx_ctx.cuh"
+#include "gpx_ep.cuh"
 #include "gpx_kernels.cuh"
 
 namespace gpx {
@@ -535,20 +536,13 @@ __device__ double ep_dlog_cdf(double z) {   // derivLogCdfNormal
   return t / (1.0 - t * ep_erf_helper(z) / z);
 }
 
-// the site outputs of a sweep (vectors of lapV)
-struct EpSites {
-  double *tt, *vt;                      // tau~, v~ (in / out)
-  double *ct, *cv, *zh, *mh, *s2;       // cavity tau and v, Z_hat, mu_hat, sigma2_hat
-  const double* sgn;                    // +1 for y = 1, -1 for y in {0, -1}
-  double eta, delta;
-};
-
-// site i of _local_updates (:333-351) at Sigma_ii = Sii and mu_i = mui: the cavity (:27-29), the probit moments
-// (bernoulli.py:59-92), the site update with tau~ clipped at machine epsilon (:52-68). -> the rank-1 update's
-// c = dtau / (1 + dtau Sii) and g = c (mu_i + Sii dv) - dv (:101-105: mu -= g s, Sigma -= c s s^T)
-__device__ void ep_site(const EpSites& e, long i, double Sii, double mui, double* c_out, double* g_out) {
-  const double tau = 1.0 / Sii - e.eta * e.tt[i];
-  const double v = mui / Sii - e.eta * e.vt[i];
+// site i of _local_updates (:333-351) at mu_i = mui: the cavity (:27-29) and the site update with tau~ clipped at machine
+// epsilon (:52-68) read the diagonal the caller holds, Sd; the probit moments (bernoulli.py:59-92). -> the rank-1 update's
+// c = dtau / (1 + dtau Sii) and g = c (mu_i + Sii dv) - dv (:101-105: mu -= g s, Sigma -= c s s^T) with Sii the diagonal of
+// the Sigma being updated. Dense EP holds Sd = Sii; the DTC form holds a clipped copy (:149-156).
+__device__ void ep_site(const EpSites& e, long i, double Sd, double Sii, double mui, double* c_out, double* g_out) {
+  const double tau = 1.0 / Sd - e.eta * e.tt[i];
+  const double v = mui / Sd - e.eta * e.vt[i];
   const double sgn = e.sgn[i];
   const double q = sqrt(tau * tau + tau);
   const double z = sgn * v / q;
@@ -557,8 +551,8 @@ __device__ void ep_site(const EpSites& e, long i, double Sii, double mui, double
   const double mh = v / tau + sgn * r / q;
   const double s2 = 1.0 / tau - (r / (tau * tau + tau)) * (z + r);
   const double de = e.delta / e.eta;
-  double dtau = de * (1.0 / s2 - 1.0 / Sii);
-  const double dv = de * (mh / s2 - mui / Sii);
+  double dtau = de * (1.0 / s2 - 1.0 / Sd);
+  const double dv = de * (mh / s2 - mui / Sd);
   const double prev = e.tt[i];
   double t = prev + dtau;
   if (t < 2.220446049250313e-16) {
@@ -578,19 +572,17 @@ __device__ __forceinline__ double ep_sym(const double* __restrict__ S, long ld, 
   return (p / TILE >= q / TILE) ? S[p + q * ld] : S[q + p * ld];
 }
 
-constexpr int EP_CHAIN_THREADS = 1024;
-constexpr int EP_SOLVE_ROWS = 64;
-constexpr int EP_CHAIN_SMEM = (TILE * TILE + 2 * TILE + 2) * 8;
-constexpr int EP_SOLVE_SMEM = (TILE * TILE + 2 * TILE + TILE * EP_SOLVE_ROWS) * 8;
-
 // the site chain of one block of m <= TILE sites I (one CTA): G = Sigma[I, I] (lower part, row-major in shared memory),
 // mu_I; for j = 0 .. m-1 the site update at (G_jj, mu_I[j]), then mu_I -= g s and G -= c s s^T on the trailing part
 // (s = G[:, j]). Column l of G keeps s_l below the diagonal (the later steps touch columns > l only): Gout = G, cg = (c, g),
-// zero beyond m.
+// zero beyond m. dtc: G and mu_I as gpx_ep.cuh describes, and the cavity of site j reads max(G_jj, eps) (sd0[I[0]] for
+// the first site of a run), the reference's Sigma_diag, while c and g use G_jj itself.
 __global__ void __launch_bounds__(EP_CHAIN_THREADS, 1) ep_chain_kernel(const double* __restrict__ Sig, long ld,
                                                                        const int* __restrict__ I, int m,
                                                                        const double* __restrict__ mu, EpSites e,
-                                                                       double* __restrict__ Gout, double* __restrict__ cg) {
+                                                                       double* __restrict__ Gout, double* __restrict__ cg,
+                                                                       const double* __restrict__ muadd,
+                                                                       const double* __restrict__ sd0, int dtc) {
   extern __shared__ double ep_sm[];
   double* G = ep_sm;
   double* s = G + TILE * TILE;
@@ -598,13 +590,16 @@ __global__ void __launch_bounds__(EP_CHAIN_THREADS, 1) ep_chain_kernel(const dou
   double* cgs = muI + TILE;
   const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
   for (int a = ty; a < TILE; a += 32)
-    for (int b = tx; b < TILE; b += 32) G[a * TILE + b] = (a < m && b <= a) ? ep_sym(Sig, ld, I[a], I[b]) : 0.0;
-  if (tid < TILE) muI[tid] = tid < m ? mu[I[tid]] : 0.0;
+    for (int b = tx; b < TILE; b += 32)
+      G[a * TILE + b] = (a < m && b <= a) ? (dtc ? Sig[a + b * ld] : ep_sym(Sig, ld, I[a], I[b])) : 0.0;
+  if (tid < TILE) muI[tid] = tid < m ? (dtc ? mu[I[tid]] + muadd[tid] : mu[I[tid]]) : 0.0;
   __syncthreads();
   for (int j = 0; j < m; j++) {
     if (tid == 0) {
       double c, g;
-      ep_site(e, I[j], G[j * TILE + j], muI[j], &c, &g);
+      const double Gjj = G[j * TILE + j];
+      const double Sd = !dtc ? Gjj : (j == 0 && sd0) ? sd0[I[0]] : fmax(Gjj, 2.220446049250313e-16);
+      ep_site(e, I[j], Sd, Gjj, muI[j], &c, &g);
       cgs[0] = c; cgs[1] = g;
       cg[j] = c; cg[TILE + j] = g;
     }
@@ -624,12 +619,12 @@ __global__ void __launch_bounds__(EP_CHAIN_THREADS, 1) ep_chain_kernel(const dou
 
 // S = Sigma[:, I] (I + U)^-1, one thread per row r (forward substitution in the fixed order l = 0 .. j-1):
 // x_j = Sigma(r, I_j) - sum_l (x_l c_l) s_l[j]; out Sx = S, Sc = S diag(c) (Npad x TILE each, zero beyond m) and
-// mu_r -= sum_j x_j g_j. G, c and g are those of ep_chain_kernel.
+// mu_r -= sum_j x_j g_j. G, c and g are those of ep_chain_kernel. dtc: Sigma(r, I_j) is P(r, j), read from P^T in Sig.
 __global__ void __launch_bounds__(EP_SOLVE_ROWS) ep_solve_kernel(const double* __restrict__ Sig, long ld,
                                                                  const int* __restrict__ I, int m,
                                                                  const double* __restrict__ Gin,
                                                                  const double* __restrict__ cg, double* __restrict__ Sx,
-                                                                 double* __restrict__ Sc, double* __restrict__ mu) {
+                                                                 double* __restrict__ Sc, double* __restrict__ mu, int dtc) {
   extern __shared__ double ep_sm[];
   double* G = ep_sm;
   double* cc = G + TILE * TILE;
@@ -642,7 +637,7 @@ __global__ void __launch_bounds__(EP_SOLVE_ROWS) ep_solve_kernel(const double* _
   for (long r = (long)blockIdx.x * EP_SOLVE_ROWS + t; r < ld; r += (long)gridDim.x * EP_SOLVE_ROWS) {
     double dot = 0.0;
     for (int j = 0; j < m; j++) {
-      double acc = ep_sym(Sig, ld, r, I[j]);
+      double acc = dtc ? Sig[j + r * TILE] : ep_sym(Sig, ld, r, I[j]);
       const double* Gj = G + j * TILE;
       for (int l = 0; l < j; l++) acc = fma(-xs[l * EP_SOLVE_ROWS + t], Gj[l], acc);
       const double xc = acc * cc[j];
@@ -662,11 +657,10 @@ __global__ void __launch_bounds__(256) ep_parallel_kernel(long N, const double* 
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   double c, g;
-  ep_site(e, i, sd[i], mu[i], &c, &g);
+  ep_site(e, i, sd[i], sd[i], mu[i], &c, &g);
 }
 
 // the EP vector glue, one thread per entry i < n (entries N <= i < n of o are zero)
-enum { EV_SUB = 0, EV_DIAG = 1, EV_DLDK = 2, EV_ADDDIAG = 3, EV_SIGN = 4 };
 __global__ void __launch_bounds__(256) ep_vec_kernel(int mode, long N, long n, const double* __restrict__ x,
                                                      const double* __restrict__ y, double* __restrict__ A, long ld,
                                                      double add, double* __restrict__ o) {
@@ -867,8 +861,10 @@ int gpx_ep_sweep(gpx_ctx* c, const int64_t* order, double eta, double delta, int
     for (long k0 = 0; k0 < N; k0 += TILE) {
       const int m = (int)std::min<long>(TILE, N - k0);
       const int* I = c->epOrd + k0;
-      ep_chain_kernel<<<1, EP_CHAIN_THREADS, EP_CHAIN_SMEM, st>>>(c->epSig, ld, I, m, lv(c, LV_MU), e, Gb, cg);
-      ep_solve_kernel<<<solve_grid, EP_SOLVE_ROWS, EP_SOLVE_SMEM, st>>>(c->epSig, ld, I, m, Gb, cg, Sx, Sc, lv(c, LV_MU));
+      ep_chain_kernel<<<1, EP_CHAIN_THREADS, EP_CHAIN_SMEM, st>>>(c->epSig, ld, I, m, lv(c, LV_MU), e, Gb, cg, nullptr,
+                                                                  nullptr, 0);
+      ep_solve_kernel<<<solve_grid, EP_SOLVE_ROWS, EP_SOLVE_SMEM, st>>>(c->epSig, ld, I, m, Gb, cg, Sx, Sc, lv(c, LV_MU),
+                                                                        0);
       GPX_CUDA(cudaGetLastError());
       GemmParams pu = gemm_defaults();   // Sigma -= S diag(c) S^T over the lower tiles, k-depth TILE
       pu.mode = GEMM_UPDATE;

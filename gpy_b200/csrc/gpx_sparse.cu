@@ -19,6 +19,7 @@
 #include "gpx_common.cuh"
 #include "gpx_ctx.cuh"
 #include "gpx_kernels.cuh"
+#include "gpx_ep.cuh"
 
 using namespace gpx;
 
@@ -52,6 +53,17 @@ struct SparseState {
   double noise = 0.0;
   double jitter = 1e-8;                              // const_jitter of the last evaluation (VarDTC 1e-8, FITC 1e-6)
   double *F2 = nullptr, *G = nullptr;                // FITC: Mpad x Npad, Kmm^-1 psi1^T and its columns scaled by dL_dR
+  // sparse EP (gpx_epdtc_*): Kmm, A = LLT^-1 (whole, symmetric) and A at the sites zero (Mpad x Mpad each); one block of
+  // sites (epb); the site vectors ([EDV_N][Npad]); the update order; the inducing inputs of gpx_epdtc_begin on the host
+  double *eK = nullptr, *eA = nullptr, *eA0 = nullptr, *epb = nullptr;
+  double *ev = nullptr;
+  int* eord = nullptr;
+  std::vector<double> eZ;
+  bool ep_begun = false;    // gpx_epdtc_begin built Kmm, Kmn and A0 for the current data and Z (psi_device clears it)
+  bool ep_ready = false;    // mu0, u and the held diagonal of gpx_epdtc_start / _sweep are on the device
+  bool ep_labels = false;   // the labels of the current data were checked
+  bool ep_seq = false;      // the sites run sequentially (A is updated)
+  bool ep_first = false;    // the next site is the first of a run: its cavity reads the held diagonal of the start
   Points xpts() const { return Points{XsT, sqX, N, Npad}; }   // this rank's data points, prepared
   Points zpts() const { return Points{ZsT, sqZ, M, Mpad}; }   // the inducing points, prepared
 };
@@ -59,18 +71,20 @@ struct SparseState {
 namespace {
 void free_m(SparseState* s) {
   double** ptrs[] = {&s->Z, &s->ZsT, &s->sqZ, &s->Kuf, &s->Kfu, &s->dLt, &s->Gm, &s->W2, &s->Cm, &s->vec, &s->gsum,
-                     &s->F2, &s->G};
+                     &s->F2, &s->G, &s->eK, &s->eA, &s->eA0, &s->epb};
   for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
   for (auto& p : s->mm) { if (p) cudaFree(p); p = nullptr; }
   s->have_eval = false;
   s->w_ready = false;
+  s->ep_begun = s->ep_ready = false;
   s->M = s->Mpad = 0;
   s->Nw = s->Mw = 0;
 }
 void free_all(SparseState* s) {
   free_m(s);
-  double** ptrs[] = {&s->X, &s->XsT, &s->sqX, &s->Y, &s->Yb, &s->part, &s->red, &s->hb, &s->hs};
+  double** ptrs[] = {&s->X, &s->XsT, &s->sqX, &s->Y, &s->Yb, &s->part, &s->red, &s->hb, &s->hs, &s->ev};
   for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
+  if (s->eord) { cudaFree(s->eord); s->eord = nullptr; }
   if (s->h_red) { cudaFreeHost(s->h_red); s->h_red = nullptr; }
   if (s->cK) { gpx_destroy(s->cK); s->cK = nullptr; }
   if (s->cB) { gpx_destroy(s->cB); s->cB = nullptr; }
@@ -213,6 +227,7 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
   s->N = N;
   s->have_eval = false;
   s->w_ready = false;
+  s->ep_begun = s->ep_ready = s->ep_labels = false;
   {   // trYYT = sum(Y .* Y) (var_dtc.py:37,90); with row shards: summed over the ranks, like num_data
     double t = 0.0;
     for (int64_t i = 0; i < N * (int64_t)P; i++) t += Y[i] * Y[i];
@@ -270,6 +285,7 @@ static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
     GPX_CUDA(cudaMemsetAsync(s->Kfu, 0, (size_t)Mpad * Npad * 8, st));   // are ever written
   }
   s->M = M;
+  s->ep_begun = s->ep_ready = false;   // Kmn changes: a sparse EP run has to begin again
   if (N < s->Nw || M < s->Mw) {   // fewer points than last time inside the same padded extents: stale entries must go
     GPX_CUDA(cudaMemsetAsync(s->Kuf, 0, (size_t)Mpad * Npad * 8, st));
     GPX_CUDA(cudaMemsetAsync(s->Kfu, 0, (size_t)Mpad * Npad * 8, st));
@@ -389,13 +405,15 @@ static int build_Kmm(gpx_ctx* c, double* Kd) {
   return launched(c);
 }
 // factor-and-invert the M x M matrix A (written on c's stream) on the child context ch, then U (clean upper) and
-// Linv = U^T out of its factor; the child's launches count on c as well, its trailing updates in c's stats
-static int factor_child(gpx_ctx* c, gpx_ctx* ch, const double* A, double jitter, double* logdet, double* U, double* Linv) {
+// Linv = U^T out of its factor; the child's launches count on c as well, its trailing updates in c's stats. jitchol's ladder
+// with max_tries; *jitter_used (if given): what the ladder added beyond `jitter`
+static int factor_child(gpx_ctx* c, gpx_ctx* ch, const double* A, double jitter, double* logdet, double* U, double* Linv,
+                        double* jitter_used = nullptr, int max_tries = 5) {
   const long Mpad = c->sparse->Mpad;
   GPX_CUDA(cudaStreamSynchronize(c->st));
   const int64_t l0 = ch->total_launches;
   const int32_t u0 = ch->stats.update_launches;
-  const int rc = factor_device(ch, A, Mpad, c->sparse->M, jitter, 5, logdet, nullptr);
+  const int rc = factor_device(ch, A, Mpad, c->sparse->M, jitter, max_tries, logdet, jitter_used);
   c->total_launches += ch->total_launches - l0;
   c->stats.update_launches += ch->stats.update_launches - u0;
   if (rc) return rc;
@@ -438,9 +456,12 @@ static void kern_grads(const SparseState* s, double ddiag, const std::vector<dou
 // noise_vec == nullptr: scalar noise variance `noise` (grad = [k's gradient block, noise variance]);
 // noise_vec (host, one variance per row held by this rank): grad = [k's gradient block], dL_dR (host, N x P row-major).
 // k's block: a single kernel's [variance, lengthscale..]; a composite's part blocks in order (part_ngrad entries each).
+// precision (host, one per row; sparse EP's marginal): the per-point form with beta_n = precision_n as given (no floor) and
+// Kmm factored with jitchol's ladder (max_tries) and no const_jitter; *jitter_used: what the ladder added.
 static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const double* Z, int64_t M, double noise,
-                            const double* noise_vec, double* lml, double* grad, double* dZ, double* dL_dR_out) {
-  const bool het = noise_vec != nullptr;
+                            const double* noise_vec, double* lml, double* grad, double* dZ, double* dL_dR_out,
+                            const double* precision = nullptr, int max_tries = 5, double* jitter_used = nullptr) {
+  const bool het = noise_vec != nullptr || precision != nullptr;
   GPX_CUDA(cudaSetDevice(c->device));
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
@@ -448,7 +469,7 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   s->w_ready = false;
   s->mk = k;
   s->kdiag = kdiag;
-  s->jitter = 1e-8;
+  s->jitter = precision ? 0.0 : 1e-8;
   memset(&c->stats, 0, sizeof(c->stats));   // filled below: Kmm's attempts, the trailing updates of both factorisations
   // per-point precisions beta_n = 1 / max(variance_n, const_jitter) (var_dtc.py:79-84) and the sums over n the bound needs
   std::vector<double> hbeta, hsb;
@@ -457,8 +478,8 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
     const long Nl = s->N, Npd = s->Npad;
     hbeta.assign((size_t)Npd, 0.0); hsb.assign((size_t)Npd, 0.0);
     for (long n = 0; n < Nl; n++) {
-      if (!(noise_vec[n] == noise_vec[n])) GPX_FAIL("noise variance is NaN");
-      const double b = 1.0 / std::max(noise_vec[n], 1e-8);
+      if (precision ? !(precision[n] == precision[n]) : !(noise_vec[n] == noise_vec[n])) GPX_FAIL("noise variance is NaN");
+      const double b = precision ? precision[n] : 1.0 / std::max(noise_vec[n], 1e-8);
       hbeta[n] = b; hsb[n] = sqrt(b);
       sum_log_beta += log(b); sum_beta += b;
     }
@@ -498,7 +519,15 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   const double *sbv = het ? s->hb : nullptr, *bvec = het ? s->hb + Npad : nullptr;
   // Kmm (dense, zero padded), factor-and-invert with const_jitter (var_dtc.py:93-95)
   GPX_CHECK(build_Kmm(c, Kd));
-  GPX_CHECK(factor_child(c, s->cK, Kd, 1e-8, nullptr, Um, Lmi));                      // Um (clean upper), Lmi = Um^T
+  if (precision) {   // var_dtc.py:96-98 with Lm = jitchol(Kmm) of the caller: Kmm = Lm Lm^T
+    double jit = 0.0;
+    const int rc = factor_child(c, s->cK, Kd, 0.0, nullptr, Um, Lmi, &jit, max_tries);
+    if (rc) return rc;
+    s->jitter = jit;
+    if (jitter_used) *jitter_used = jit;
+  } else {
+    GPX_CHECK(factor_child(c, s->cK, Kd, 1e-8, nullptr, Um, Lmi));                    // Um (clean upper), Lmi = Um^T
+  }
   c->stats.tries = s->cK->stats.tries;
   // tmp = Lm^-1 psi1^T (M x N; var_dtc.py:131,139 dtrtrs) as a product with the triangular inverse, k-range <= row tile.
   // A = tmp tmp^T is then formed from O(1) entries. (Forming G = psi1^T psi1 first and sandwiching it, Lm^-1 G Lm^-T,
@@ -1195,6 +1224,341 @@ int gpx_sparse_eval_fitc(gpx_ctx* c, const gpx_kern_part* parts, int nparts, con
     if (mk.part[p].kind == GPX_RATQUAD || mk.part[p].kind == GPX_STDPERIODIC)
       GPX_FAIL("RatQuad and StdPeriodic parts are not on the sparse evaluation (no device gradients_X)");
   return fitc_eval_impl(c, mk, kdiag, Z, M, noise_variance, lml, grad, dZ, dL_dKdiag);
+}
+
+}  // extern "C"
+
+// =================================================================================================================
+// Sparse EP (EPDTC, expectation_propagation.py:436-611) for the probit Bernoulli likelihood, in M-space.
+// The posterior of the sites is Sigma = Knm A Kmn with A = LLT^-1, LLT = Kmm + Kmn diag(tau~) Knm (M x M), and
+// mu = mu0 + Knm u, mu0 that of the last recompute. A sequential sweep runs in blocks of TILE sites I of the order:
+//   KbT = Kmn[:, I]^T (gather), P^T = KbT A, G = KbT P = Sigma[I, I] (DMMA GEMMs), mu_I = mu0[I] + KbT u;
+//   the site chain of dense EP on G (ep_chain_kernel, dtc form: the cavity reads the clipped diagonal the reference holds);
+//   Y = P (I + U)^-1 over the M rows (ep_solve_kernel, dtc form), u -= Y g; A -= Y diag(c) Y^T (GEMM_UPDATE), mirrored.
+// Sigma -= S diag(c) S^T with S = Knm Y is dense EP's update, which regroups the reference's chain of rank-1 updates; here
+// it is carried by A, so nothing of size N x N or N x TILE is formed. _recompute (:175-185): LLT from the GEMM with k-depth
+// N, jitchol's ladder on the factor-and-invert sweep, A = U U^T, V = L^-1 Kmn, Sigma_diag = |V[:, n]|^2 and mu = V^T (V v~).
+// =================================================================================================================
+namespace {
+// the site vectors of the sparse EP, s->ev + k * Npad
+enum { ED_TT = 0, ED_VT, ED_SGN, ED_CT, ED_CV, ED_ZH, ED_MH, ED_S2, ED_MU0, ED_SD, ED_SDT, ED_QNN, ED_Y, ED_DRIFT, EDV_N };
+constexpr int EP_RSPLIT = 64;
+double* edv(SparseState* s, int k) { return s->ev + (size_t)k * s->Npad; }
+// one block of sites, inside s->epb
+struct EpBlock { double *KbT, *PT, *Sx, *Sc, *G, *Gb, *cg, *ku, *u, *t, *part; };
+EpBlock ep_block(SparseState* s) {
+  const size_t Mp = (size_t)s->Mpad;
+  EpBlock b;
+  b.KbT = s->epb; b.PT = b.KbT + TILE * Mp; b.Sx = b.PT + TILE * Mp; b.Sc = b.Sx + TILE * Mp; b.G = b.Sc + TILE * Mp;
+  b.Gb = b.G + TILE * TILE; b.cg = b.Gb + TILE * TILE; b.ku = b.cg + 2 * TILE; b.u = b.ku + TILE; b.t = b.u + Mp;
+  b.part = b.t + Mp;
+  return b;
+}
+size_t ep_block_doubles(long Mpad) { return (size_t)4 * TILE * Mpad + 2 * TILE * TILE + 3 * TILE + (2 + EP_RSPLIT) * Mpad; }
+
+// KbT (TILE x Mpad, ld TILE) = rows I of Kfu, zero beyond m
+__global__ void epdtc_gather_kernel(const double* __restrict__ Kfu, long ldk, const int* __restrict__ I, int m, long Mpad,
+                                    double* __restrict__ KbT) {
+  const long k = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= (long)TILE * Mpad) return;
+  const int j = (int)(k % TILE);
+  const long a = k / TILE;
+  KbT[k] = j < m ? Kfu[I[j] + a * ldk] : 0.0;
+}
+// o_i = max(x_i, eps) (clip = 1) or x_i + add, for i < N; zero for N <= i < n
+__global__ void epdtc_vec_kernel(int clip, long N, long n, const double* __restrict__ x, double add, double* __restrict__ o) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  o[i] = i < N ? (clip ? fmax(x[i], 2.220446049250313e-16) : x[i] + add) : 0.0;
+}
+
+// o_n = sum_a K[a, n] W[a, n] over the M rows (diag(Knm A Kmn) with W = A Kmn), one thread per column, fixed order
+__global__ void epdtc_coldot_kernel(const double* __restrict__ K, const double* __restrict__ W, long ld, long M, long N,
+                                    double* __restrict__ o) {
+  const long n = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  double d = 0.0;
+  for (long a = 0; a < M; a++) d = fma(K[a + n * ld], W[a + n * ld], d);
+  o[n] = d;
+}
+
+int ep_vecop(gpx_ctx* c, int clip, const double* x, double add, double* o) {
+  SparseState* s = c->sparse;
+  epdtc_vec_kernel<<<(unsigned)((s->Npad + 255) / 256), 256, 0, c->st>>>(clip, s->N, s->Npad, x, add, o);
+  return launched(c);
+}
+
+int epdtc_args(gpx_ctx* c) {
+  if (!c) GPX_FAIL("null argument");
+  if (c->dist) GPX_FAIL("sparse expectation propagation is single-GPU");
+  if (!c->sparse || !c->sparse->X) GPX_FAIL("gpx_sparse_set_data has not been called");
+  if (!c->sparse->ep_begun) GPX_FAIL("gpx_epdtc_begin has not been called on this data, kernel and Z");
+  return 0;
+}
+
+int epdtc_upload(gpx_ctx* c, int slot, const double* h) {
+  GPX_CUDA(cudaMemcpyAsync(edv(c->sparse, slot), h, (size_t)c->sparse->N * 8, cudaMemcpyHostToDevice, c->st));
+  return 0;
+}
+int epdtc_download(gpx_ctx* c, int slot, double* h) {
+  if (h) GPX_CUDA(cudaMemcpyAsync(h, edv(c->sparse, slot), (size_t)c->sparse->N * 8, cudaMemcpyDeviceToHost, c->st));
+  return 0;
+}
+
+// posteriorParamsDTC._recompute (:175-185) from the sites in ED_TT / ED_VT: A = LLT^-1, the true diagonal in ED_SDT,
+// mu0 in ED_MU0, u = 0. -> 0 or the failing minor of LLT after the ladder
+int epdtc_recompute(gpx_ctx* c, int max_tries, double* jitter_used) {
+  SparseState* s = c->sparse;
+  cudaStream_t st = c->st;
+  const long Mpad = s->Mpad, Npad = s->Npad, N = s->N, M = s->M;
+  double *R = s->mm[3], *LLT = s->mm[4], *U = s->mm[1], *Linv = s->mm[2];
+  const EpBlock b = ep_block(s);
+  // LLT = Kmm + (Kmn diag(tau~)) Knm: the scaled copy in the dL_dKnm^T buffer, the product's lower tiles, mirrored
+  GPX_CUDA(cudaMemcpyAsync(s->dLt, s->Kuf, (size_t)Mpad * Npad * 8, cudaMemcpyDeviceToDevice, st));
+  scale_cols_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(s->dLt, Mpad, N, edv(s, ED_TT));
+  GPX_CHECK(launched(c));
+  {
+    GemmParams pg = gemm_defaults();
+    pg.mode = GEMM_PANEL; pg.plain = 2;
+    pg.A = s->dLt; pg.lda = Mpad; pg.B = s->Kuf; pg.ldb = Mpad; pg.C = R; pg.ldc = Mpad;
+    pg.K = (int)Npad; pg.nt = (int)(Mpad / TILE); pg.ncols = (int)(Mpad / TILE);
+    GPX_CHECK(launch_gemm(pg, dim3(1, 1), st));
+    GPX_CHECK(launched(c));
+  }
+  mirror_tiles_kernel<<<dim3((unsigned)((Mpad + 255) / 256), (unsigned)Mpad), 256, 0, st>>>(R, Mpad, Mpad);
+  GPX_CHECK(launched(c));
+  GPX_CHECK(combine(c, LLT, M, 1.0, s->eK, 1.0, R, 0.0));
+  const int rc = factor_child(c, s->cK, LLT, 0.0, nullptr, U, Linv, jitter_used, max_tries);
+  if (rc) return rc;
+  GPX_CHECK(binv(c, U, s->eA));                                                          // A = U U^T = LLT^-1
+  GPX_CHECK(mul_psi1T(c, Linv, s->dLt, 2));                                              // V = L^-1 Kmn
+  GPX_CHECK(launch_col_sqnorm(s->dLt, Mpad, M, N, edv(s, ED_SDT), st));
+  GPX_CHECK(launch_row_dot(s->dLt, Mpad, Mpad, N, 1, edv(s, ED_VT), Npad, EP_RSPLIT, b.part, b.t, st));   // t = V v~
+  GPX_CHECK(launch_col_dot(s->dLt, Mpad, M, N, 1, b.t, Mpad, edv(s, ED_MU0), Npad, st));                   // mu0 = V^T t
+  GPX_CHECK(launched(c, 4));
+  GPX_CUDA(cudaMemsetAsync(b.u, 0, (size_t)Mpad * 8, st));
+  return 0;
+}
+
+int epdtc_end(gpx_ctx* c, const char* what) {
+  if (cudaStreamSynchronize(c->st) != cudaSuccess) GPX_FAIL_DEVICE(what);
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int gpx_epdtc_begin(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M) {
+  if (!c || !parts || !Z) GPX_FAIL("null argument");
+  if (c->dist) GPX_FAIL("sparse expectation propagation is single-GPU");
+  if (!c->sparse || !c->sparse->X) GPX_FAIL("gpx_sparse_set_data has not been called");
+  SparseState* s = c->sparse;
+  if (s->P != 1) GPX_FAIL("sparse expectation propagation takes one output column (P = 1)");
+  if (M < 1) GPX_FAIL("M must be positive");
+  MultiKern mk;
+  double kdiag;
+  GPX_CHECK(fill_mk(mk, parts, nparts, s->D, &kdiag));
+  for (int p = 0; p < mk.nparts; p++)
+    if (mk.part[p].kind == GPX_RATQUAD || mk.part[p].kind == GPX_STDPERIODIC)
+      GPX_FAIL("RatQuad and StdPeriodic parts are not on the sparse evaluation (no device gradients_X)");
+  GPX_CUDA(cudaSetDevice(c->device));
+  cudaStream_t st = c->st;
+  const long N = s->N, Npad = s->Npad;
+  if (!s->ep_labels) {   // once per data set: gpx_sparse_set_data clears the flag
+    std::vector<double> y((size_t)N);
+    GPX_CUDA(cudaMemcpy(y.data(), s->Y, (size_t)N * 8, cudaMemcpyDeviceToHost));
+    for (double v : y)
+      if (!(v == 1.0 || v == 0.0 || v == -1.0)) GPX_FAIL("bad value for Bernoulli observation (0, 1)");
+  }
+  s->have_eval = s->w_ready = false;
+  s->mk = mk;
+  s->kdiag = kdiag;
+  memset(&c->stats, 0, sizeof(c->stats));
+  GPX_CHECK(psi_device(c, Z, M));
+  const long Mpad = s->Mpad;
+  if (!s->mm[0]) {
+    for (auto& p : s->mm) GPX_CUDA(cudaMalloc(&p, (size_t)Mpad * Mpad * 8));
+    GPX_CUDA(cudaMalloc(&s->vec, (size_t)(8 + 64) * s->P * Mpad * 8));
+  }
+  if (!s->red) {
+    GPX_CUDA(cudaMalloc(&s->red, 4096 * 8));
+    GPX_CUDA(cudaMallocHost(&s->h_red, 4096 * 8));
+  }
+  if (!s->cK) { GPX_CHECK(gpx_create(c->device, &s->cK)); GPX_CHECK(gpx_create(c->device, &s->cB)); }
+  for (gpx_ctx* ch : {s->cK, s->cB})
+    if (ch->NB != c->NB) GPX_CHECK(gpx_set_option(ch, "nb", c->NB));
+  if (!s->eK) {
+    for (double** p : {&s->eK, &s->eA, &s->eA0}) GPX_CUDA(cudaMalloc(p, (size_t)Mpad * Mpad * 8));
+    GPX_CUDA(cudaMalloc(&s->epb, ep_block_doubles(Mpad) * 8));
+    GPX_CUDA(cudaMemsetAsync(s->epb, 0, ep_block_doubles(Mpad) * 8, st));
+  }
+  if (!s->ev) {
+    GPX_CUDA(cudaMalloc(&s->ev, (size_t)EDV_N * Npad * 8));
+    GPX_CUDA(cudaMemsetAsync(s->ev, 0, (size_t)EDV_N * Npad * 8, st));
+    GPX_CUDA(cudaMalloc(&s->eord, (size_t)Npad * sizeof(int)));
+  }
+  s->eZ.assign(Z, Z + (size_t)M * s->D);
+  // Kmm (LLT0, no jitter), Lm = jitchol(Kmm); A0 = Kmm^-1 and diag(Knm Kmm^-1 Kmn) for the cold start (:522-535)
+  GPX_CHECK(build_Kmm(c, s->eK));
+  double jit = 0.0;
+  const int rc = factor_child(c, s->cK, s->eK, 0.0, nullptr, s->mm[1], s->mm[2], &jit, 5);
+  if (rc) return rc;
+  GPX_CHECK(binv(c, s->mm[1], s->eA0));
+  GPX_CHECK(mul_psi1T(c, s->mm[2], s->dLt, 2));
+  GPX_CHECK(launch_col_sqnorm(s->dLt, Mpad, M, N, edv(s, ED_QNN), st));
+  GPX_CHECK(launched(c));
+  ep_vec_kernel<<<(unsigned)((Npad + 255) / 256), 256, 0, st>>>(EV_SIGN, N, Npad, s->Y, nullptr, nullptr, 0, 0.0,
+                                                                edv(s, ED_SGN));
+  GPX_CHECK(launched(c));
+  GPX_CHECK(epdtc_end(c, "gpx_epdtc_begin"));
+  s->ep_labels = true;
+  s->ep_begun = true;
+  s->ep_ready = false;
+  return 0;
+}
+
+int gpx_epdtc_start(gpx_ctx* c, const double* tau_tilde, const double* v_tilde, int warm, int parallel, int max_tries,
+                    double* jitter_used, double* mu, double* sigma_diag) {
+  if (!c || !jitter_used || (warm && (!tau_tilde || !v_tilde))) GPX_FAIL("null argument");
+  GPX_CHECK(epdtc_args(c));
+  GPX_CUDA(cudaSetDevice(c->device));
+  SparseState* s = c->sparse;
+  cudaStream_t st = c->st;
+  const long Mpad = s->Mpad, Npad = s->Npad;
+  s->ep_ready = false;
+  s->ep_seq = !parallel;
+  memset(&c->stats, 0, sizeof(c->stats));
+  *jitter_used = 0.0;
+  const EpBlock b = ep_block(s);
+  if (!warm) {   // cold (:536-544): sites 0, LLT = Kmm, mu = 0, Sigma_diag = diag(Knm Kmm^-1 Kmn) + 1e-8
+    for (int k : {ED_TT, ED_VT, ED_MU0}) GPX_CUDA(cudaMemsetAsync(edv(s, k), 0, (size_t)Npad * 8, st));
+    GPX_CUDA(cudaMemsetAsync(b.u, 0, (size_t)Mpad * 8, st));
+    GPX_CUDA(cudaMemcpyAsync(s->eA, s->eA0, (size_t)Mpad * Mpad * 8, cudaMemcpyDeviceToDevice, st));
+    GPX_CHECK(ep_vecop(c, 0, edv(s, ED_QNN), 1e-8, edv(s, ED_SD)));
+  } else {       // warm (:545-549): the recompute from the kept sites, then 1e-8 on Sigma_diag (no clip)
+    GPX_CHECK(epdtc_upload(c, ED_TT, tau_tilde));
+    GPX_CHECK(epdtc_upload(c, ED_VT, v_tilde));
+    const int rc = epdtc_recompute(c, max_tries, jitter_used);
+    if (rc) { epdtc_end(c, "gpx_epdtc_start"); return rc; }
+    GPX_CHECK(ep_vecop(c, 0, edv(s, ED_SDT), 1e-8, edv(s, ED_SD)));
+  }
+  GPX_CHECK(epdtc_download(c, ED_MU0, mu));
+  GPX_CHECK(epdtc_download(c, ED_SD, sigma_diag));
+  GPX_CHECK(epdtc_end(c, "gpx_epdtc_start"));
+  s->ep_first = true;
+  s->ep_ready = true;
+  return 0;
+}
+
+int gpx_epdtc_sweep(gpx_ctx* c, const int64_t* order, double eta, double delta, int parallel, int max_tries,
+                    double* tau_tilde, double* v_tilde, double* cav_tau, double* cav_v, double* Z_hat, double* mu_hat,
+                    double* sigma2_hat, double* jitter_used, double* mu, double* sigma_diag) {
+  if (!c || !order || !tau_tilde || !v_tilde || !cav_tau || !cav_v || !Z_hat || !mu_hat || !sigma2_hat || !jitter_used)
+    GPX_FAIL("null argument");
+  GPX_CHECK(epdtc_args(c));
+  SparseState* s = c->sparse;
+  if (!s->ep_ready) GPX_FAIL("gpx_epdtc_start has not been called since gpx_epdtc_begin");
+  if (!parallel != s->ep_seq) GPX_FAIL("parallel must be the value gpx_epdtc_start was given");
+  const long N = s->N, Npad = s->Npad, Mpad = s->Mpad;
+  std::vector<int> ord((size_t)N);
+  {
+    std::vector<char> seen((size_t)N, 0);
+    for (long k = 0; k < N; k++) {
+      const int64_t i = order[k];
+      if (i < 0 || i >= N || seen[(size_t)i]) GPX_FAIL("order is not a permutation of 0 .. N-1");
+      seen[(size_t)i] = 1;
+      ord[(size_t)k] = (int)i;
+    }
+  }
+  GPX_CUDA(cudaSetDevice(c->device));
+  cudaStream_t st = c->st;
+  memset(&c->stats, 0, sizeof(c->stats));
+  GPX_CHECK(epdtc_upload(c, ED_TT, tau_tilde));
+  GPX_CHECK(epdtc_upload(c, ED_VT, v_tilde));
+  EpSites e;
+  e.tt = edv(s, ED_TT); e.vt = edv(s, ED_VT); e.ct = edv(s, ED_CT); e.cv = edv(s, ED_CV); e.zh = edv(s, ED_ZH);
+  e.mh = edv(s, ED_MH); e.s2 = edv(s, ED_S2); e.sgn = edv(s, ED_SGN); e.eta = eta; e.delta = delta;
+  if (!parallel) {   // _local_updates with posteriorParamsDTC._update_rank1 (:553-572), one block of TILE sites at a time
+    GPX_CUDA(cudaMemcpyAsync(s->eord, ord.data(), (size_t)N * sizeof(int), cudaMemcpyHostToDevice, st));
+    GPX_CUDA(cudaFuncSetAttribute(ep_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EP_CHAIN_SMEM));
+    GPX_CUDA(cudaFuncSetAttribute(ep_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EP_SOLVE_SMEM));
+    const EpBlock b = ep_block(s);
+    const unsigned solve_grid = (unsigned)std::min<long>(Mpad / EP_SOLVE_ROWS, c->num_sms);
+    const unsigned gather_grid = (unsigned)((TILE * Mpad + 255) / 256);
+    for (long k0 = 0; k0 < N; k0 += TILE) {
+      const int m = (int)std::min<long>(TILE, N - k0);
+      const int* I = s->eord + k0;
+      epdtc_gather_kernel<<<gather_grid, 256, 0, st>>>(s->Kfu, Npad, I, m, Mpad, b.KbT);
+      GPX_CHECK(launched(c));
+      GPX_CHECK(gemm_nt(c, b.KbT, TILE, s->eA, Mpad, b.PT, TILE, TILE, Mpad, Mpad, 1, 0));   // P^T = KbT A
+      GPX_CHECK(gemm_nt(c, b.KbT, TILE, b.PT, TILE, b.G, TILE, TILE, TILE, Mpad, 1, 0));    // G = KbT P
+      GPX_CHECK(launch_row_dot(b.KbT, TILE, TILE, Mpad, 1, b.u, Mpad, EP_RSPLIT, b.part, b.ku, st));   // KbT u
+      GPX_CHECK(launched(c, 2));
+      ep_chain_kernel<<<1, EP_CHAIN_THREADS, EP_CHAIN_SMEM, st>>>(b.G, TILE, I, m, edv(s, ED_MU0), e, b.Gb, b.cg, b.ku,
+                                                                  s->ep_first ? edv(s, ED_SD) : nullptr, 1);
+      ep_solve_kernel<<<solve_grid, EP_SOLVE_ROWS, EP_SOLVE_SMEM, st>>>(b.PT, Mpad, I, m, b.Gb, b.cg, b.Sx, b.Sc, b.u, 1);
+      GPX_CHECK(launched(c, 2));
+      s->ep_first = false;
+      GemmParams pu = gemm_defaults();   // A -= Y diag(c) Y^T over the lower tiles, k-depth TILE, then mirrored
+      pu.mode = GEMM_UPDATE;
+      pu.A = b.Sc; pu.lda = Mpad; pu.B = b.Sx; pu.ldb = Mpad; pu.C = s->eA; pu.ldc = Mpad;
+      pu.K = TILE; pu.nt = (int)(Mpad / TILE); pu.c0 = 0; pu.ncols = 0; pu.rlow = 0;
+      GPX_CHECK(launch_gemm(pu, dim3(1, 1), st));
+      GPX_CHECK(launched(c));
+      mirror_tiles_kernel<<<dim3((unsigned)((Mpad + 255) / 256), (unsigned)Mpad), 256, 0, st>>>(s->eA, Mpad, Mpad);
+      GPX_CHECK(launched(c));
+    }
+  } else {           // parallel_updates: every site from the same Sigma_diag and mu
+    ep_parallel_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(N, edv(s, ED_SD), edv(s, ED_MU0), e);
+    GPX_CHECK(launched(c));
+  }
+  const bool drift = c->epdtc_drift && !parallel;
+  if (drift) {   // the measurement option: diag(Knm A Kmn) of the downdated A, before the recompute replaces it
+    GPX_CHECK(mul_psi1T(c, s->eA, s->dLt, 0));
+    epdtc_coldot_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(s->Kuf, s->dLt, Mpad, s->M, N, edv(s, ED_DRIFT));
+    GPX_CHECK(launched(c));
+  }
+  GPX_CHECK(epdtc_download(c, ED_TT, tau_tilde));
+  GPX_CHECK(epdtc_download(c, ED_VT, v_tilde));
+  GPX_CHECK(epdtc_download(c, ED_CT, cav_tau));
+  GPX_CHECK(epdtc_download(c, ED_CV, cav_v));
+  GPX_CHECK(epdtc_download(c, ED_ZH, Z_hat));
+  GPX_CHECK(epdtc_download(c, ED_MH, mu_hat));
+  GPX_CHECK(epdtc_download(c, ED_S2, sigma2_hat));
+  GPX_CHECK(epdtc_end(c, "gpx_epdtc_sweep"));
+  s->ep_ready = false;   // A, mu0 and u are those of the updates until the recompute has run
+  s->ep_first = false;
+  const int rc = epdtc_recompute(c, max_tries, jitter_used);
+  if (rc) { epdtc_end(c, "gpx_epdtc_sweep"); return rc; }
+  GPX_CHECK(ep_vecop(c, 1, edv(s, ED_SDT), 0.0, edv(s, ED_SD)));                      // np.maximum(Sigma_diag, eps)
+  GPX_CHECK(epdtc_download(c, ED_MU0, mu));
+  GPX_CHECK(epdtc_download(c, drift ? ED_DRIFT : ED_SD, sigma_diag));
+  GPX_CHECK(epdtc_end(c, "gpx_epdtc_sweep"));
+  s->ep_ready = true;
+  return 0;
+}
+
+int gpx_epdtc_finish(gpx_ctx* c, const double* tau_tilde, const double* v_tilde, int max_tries, double* lml, double* grad,
+                     double* dZ, double* jitter_used) {
+  if (!c || !tau_tilde || !v_tilde || !lml || !grad || !dZ || !jitter_used) GPX_FAIL("null argument");
+  GPX_CHECK(epdtc_args(c));
+  GPX_CUDA(cudaSetDevice(c->device));
+  SparseState* s = c->sparse;
+  const long N = s->N;
+  // VarDTC.inference at Y = v~ / tau~ and precision = tau~ as they are (:474-482), Lm = jitchol(Kmm)
+  std::vector<double> y((size_t)N), dR((size_t)N);
+  for (long n = 0; n < N; n++) y[(size_t)n] = v_tilde[n] / tau_tilde[n];
+  double* yd = edv(s, ED_Y);
+  GPX_CUDA(cudaMemcpyAsync(yd, y.data(), (size_t)N * 8, cudaMemcpyHostToDevice, c->st));
+  GPX_CUDA(cudaStreamSynchronize(c->st));
+  const std::vector<double> Z = s->eZ;
+  double* labels = s->Y;
+  s->Y = yd;
+  *jitter_used = 0.0;
+  const int rc = sparse_eval_impl(c, s->mk, s->kdiag, Z.data(), s->M, 0.0, nullptr, lml, grad, dZ, dR.data(), tau_tilde,
+                                  max_tries, jitter_used);
+  s->Y = labels;
+  return rc;
 }
 
 }  // extern "C"

@@ -609,10 +609,118 @@ def _make_ep(base, kernel_types, ffi):
     return B200EP
 
 
+def _make_epdtc(base, kernel_types, ffi):
+    import sys
+    from .ep import EPDTC as _DeviceEPDTC
+    ref = sys.modules[base.__module__]   # the reference's gaussianApproximation / posteriorParamsDTC
+
+    class B200EPDTC(base):
+        """GPy.inference.latent_function_inference.EPDTC with the sweeps (in M-space) and the marginal on the device
+        (gpx_epdtc_*), for a plugin stationary kernel or a B.Add / B.Prod over plugin stationary leaves and GPy's own White /
+        Bias, GPy's Bernoulli with the probit link, ndarray X, one output column, no mean function and no precomputed Lm,
+        dL_dKmm or psi statistics; anything else goes to the stock method (expectation_propagation.py:437-482). Both keep
+        the sites in ga_approx_old as the reference's gaussianApproximation and _ep_approximation as the reference's
+        3-tuple (posteriorParamsDTC, gaussianApproximation, log_Z_tilde), so either continues from the other's sites. The
+        grad dict is B.VarDTC's: dL_dKnm / dL_dKmm are handles of the gradients the device already reduced."""
+
+        def __init__(self, epsilon=1e-6, eta=1., delta=1., always_reset=False, max_iters=np.inf, ep_mode="alternated",
+                     parallel_updates=False, loading=False, device=0, engine=None):
+            super(B200EPDTC, self).__init__(epsilon=epsilon, eta=eta, delta=delta, always_reset=always_reset,
+                                            max_iters=max_iters, ep_mode=ep_mode, parallel_updates=parallel_updates,
+                                            loading=loading)
+            self.device, self._engine = device, engine
+            self._dev = None
+
+        @property
+        def engine(self):
+            if self._engine is None:
+                self._engine = ffi.Engine(self.device)
+            return self._engine
+
+        def invalidate_data(self):
+            if self._dev is not None:
+                self._dev.invalidate_data()
+
+        def __getstate__(self):
+            d = dict(self.__dict__)
+            d["_engine"], d["_dev"] = None, None
+            return d
+
+        def __setstate__(self, state):
+            self.__dict__.update(state)
+
+        def _leaves(self, kern, X, likelihood, Y, mean_function, extra):
+            """-> None (the stock method), False (a single plugin kernel) or the leaves of a plugin sum / product"""
+            link = getattr(likelihood, "gp_link", None)
+            if not (isinstance(X, np.ndarray) and mean_function is None and all(a is None for a in extra)
+                    and np.ndim(Y) == 2 and np.shape(Y)[1] == 1 and type(likelihood).__name__ == "Bernoulli"
+                    and type(link).__name__ == "Probit"):
+                return None
+            if isinstance(kern, kernel_types):
+                return False
+            if not hasattr(kern, "_gpx_is_prod"):
+                return None
+            leaves = _flatten(kern)
+            if leaves is None or any(not (hasattr(l, "_gpx_kind") or type(l).__name__ in ("White", "Bias"))
+                                     for l, _ in leaves):
+                return None                                        # RatQuad / StdPeriodic: no device gradients_X
+            return leaves
+
+        def inference(self, kern, X, Z, likelihood, Y, mean_function=None, Y_metadata=None, Lm=None, dL_dKmm=None,
+                      psi0=None, psi1=None, psi2=None):
+            leaves = self._leaves(kern, X, likelihood, Y, mean_function, (Lm, dL_dKmm, psi0, psi1, psi2))
+            if leaves is None:
+                return super(B200EPDTC, self).inference(kern, X, Z, likelihood, Y, mean_function=mean_function,
+                                                        Y_metadata=Y_metadata, Lm=Lm, dL_dKmm=dL_dKmm, psi0=psi0,
+                                                        psi1=psi1, psi2=psi2)
+            if self._dev is None:
+                self._dev = _DeviceEPDTC(engine=self.engine)
+            dev = self._dev
+            for name in ("epsilon", "eta", "delta", "always_reset", "max_iters", "ep_mode", "parallel_updates",
+                         "loading", "ga_approx_old", "_ep_approximation"):
+                setattr(dev, name, getattr(self, name, None))
+            if leaves:
+                parts = [_leaf_descriptor(l, t) for (l, t) in leaves]
+                Xs, Zs, key, ngrads = np.asarray(X), np.asarray(Z), _composite_key(kern), [_leaf_ngrad(l) for l, _ in leaves]
+            else:
+                Xs = kern._slice_X(X)[0] if _returns_tuple(kern, X) else kern._slice_X(X)
+                Zs = kern._slice_X(Z)[0] if _returns_tuple(kern, Z) else kern._slice_X(Z)
+                k, ard, var, ls = kern._gpx_theta()
+                parts = [(k, ard, 0, list(range(np.shape(Xs)[1])), var, ls)]
+                key, ngrads = kern._gpx_state_key(), [1 + np.size(ls)]
+            try:
+                post, lml, gd = dev.device_inference(Xs, Zs, np.asarray(Y), parts, key, ngrads, not leaves)
+            finally:
+                old = dev.ga_approx_old
+                self.ga_approx_old = None if old is None else ref.gaussianApproximation(old.v, old.tau)
+                app = dev._ep_approximation
+                if app is not None:
+                    pp, ga, logZ = app
+                    app = (ref.posteriorParamsDTC(pp.mu, pp.Sigma_diag), ref.gaussianApproximation(ga.v, ga.tau), logZ)
+                self._ep_approximation, self.loading = app, dev.loading
+            N, M = np.shape(Y)[0], np.shape(Zs)[0]
+            tau = np.asarray(self._ep_approximation[1].tau, dtype=np.float64)
+            dL_dKdiag = -0.5 * tau                                 # _compute_dL_dpsi: dL_dpsi0 at precision tau~ (:218)
+            dL_dthetaL = likelihood.exact_inference_gradients(np.zeros((N, 1)), Y_metadata)   # var_dtc.py:176
+            dZ = gd["dZ"]
+            if leaves:
+                h_knm, h_kmm = _composite_handles(kern, leaves, np.concatenate(gd["part_grads"]), dL_dKdiag.sum(), dZ,
+                                                  N, M)
+            else:
+                dlen = np.atleast_1d(gd["dlengthscale"])
+                h_knm = SparseDeviceGradient(key, "knm", (N, M), gd["dvariance"] - dL_dKdiag.sum(), dlen, dZ)
+                h_kmm = SparseDeviceGradient(key, "kmm", (M, M), 0.0, np.zeros_like(dlen), np.zeros_like(dZ))
+            return post, lml, {"dL_dKmm": h_kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": h_knm, "dL_dthetaL": dL_dthetaL,
+                               "dL_dm": None}
+
+    B200EPDTC.__name__ = B200EPDTC.__qualname__ = "EPDTC"
+    return B200EPDTC
+
+
 def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None,
-         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None, EP=None):
+         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None, EP=None, EPDTC=None):
     """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC /
-    FITC optional: the sparse model; Laplace / EP optional: non-Gaussian likelihoods; RatQuad / StdPeriodic optional: leaves
+    FITC optional: the sparse model; Laplace / EP / EPDTC optional: non-Gaussian likelihoods; RatQuad / StdPeriodic optional: leaves
     the composite evaluation knows, alone or inside Add / Prod)."""
     kernels = {n: _make_kernel(b, _KINDS[n], ffi) for n, b in
                (("RBF", RBF), ("Exponential", Exponential), ("Matern32", Matern32), ("Matern52", Matern52))}
@@ -715,6 +823,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
         extra["Laplace"] = _make_laplace(Laplace, kernel_types, ffi)
     if EP is not None:
         extra["EP"] = _make_ep(EP, kernel_types, ffi)
+    if EPDTC is not None:
+        extra["EPDTC"] = _make_epdtc(EPDTC, kernel_types, ffi)
     return types.SimpleNamespace(ExactGaussianInference=B200ExactGaussianInference, **kernels, **extra)
 
 
@@ -728,6 +838,7 @@ def load():
     """Plugin classes over an installed GPy."""
     import GPy
     from GPy.inference.latent_function_inference import EP, FITC, ExactGaussianInference, Laplace, VarDTC
+    from GPy.inference.latent_function_inference.expectation_propagation import EPDTC
     return make(GPy.kern.RBF, GPy.kern.Exponential, GPy.kern.Matern32, GPy.kern.Matern52, ExactGaussianInference,
                 Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic,
-                FITC=FITC, Laplace=Laplace, EP=EP)
+                FITC=FITC, Laplace=Laplace, EP=EP, EPDTC=EPDTC)

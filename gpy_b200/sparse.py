@@ -290,7 +290,7 @@ class SparseGPRegression(Parameterized):
     kernel: variance, lengthscale), the likelihood's]."""
 
     def __init__(self, X, Y, kernel=None, Z=None, num_inducing=10, device=0, engine=None, name="sparse_gp", likelihood=None,
-                 Y_metadata=None):
+                 Y_metadata=None, inference_method=None):
         super(SparseGPRegression, self).__init__(name)
         X = np.asarray(X, dtype=np.float64)
         Y = np.asarray(Y, dtype=np.float64)
@@ -312,7 +312,7 @@ class SparseGPRegression(Parameterized):
         self.Z.values = np.array(Z, dtype=np.float64)                          # keep the M x D shape
         self.Z.gradient = np.zeros_like(self.Z.values)
         self.num_inducing = self.Z.values.shape[0]
-        self.inference_method = VarDTC(device=device, engine=engine)
+        self.inference_method = VarDTC(device=device, engine=engine) if inference_method is None else inference_method
         self.link_parameter(self.Z)                                            # sparse_gp.py:61 (index 0)
         self.link_parameter(self.kern)
         self.link_parameter(self.likelihood)
@@ -368,6 +368,7 @@ class SparseGPRegression(Parameterized):
     def optimize(self, max_iters=1000, messages=False):
         from scipy.optimize import fmin_l_bfgs_b
         self.n_evals = 0
+        self.inference_method.on_optimization_start()                          # gp.py:677
 
         def fg(x):
             self.n_evals += 1

@@ -400,6 +400,40 @@ int gpx_ep_sweep(gpx_ctx* ctx, const int64_t* order, double eta, double delta, i
 int gpx_ep_finish(gpx_ctx* ctx, const double* tau_tilde, const double* v_tilde, int max_tries, double* logdet_B,
                   double* vSv, double* diag_dL_dK, double* kgrad, double* jitter_used);
 
+/* Sparse expectation propagation (GPy's EPDTC, expectation_propagation.py:436-611) for the probit Bernoulli likelihood, after
+ * gpx_sparse_set_data(X, labels) with P = 1. The sweeps run in M-space: Sigma = Knm A Kmn with A = LLT^-1 (M x M) and
+ * mu = mu0 + Knm u, so nothing of size N x N is formed. The kernels are those gpx_sparse_eval_multi takes.
+ *   gpx_epdtc_begin  : Kmm (no const jitter), Kmn, Lm = jitchol(Kmm), A0 = Kmm^-1 and diag(Knm Kmm^-1 Kmn); checks the
+ *                      labels once per data set ("bad value for Bernoulli observation (0, 1)").
+ *   gpx_epdtc_start  : _init_approximations: cold (sites 0, A = A0, Sigma_diag = diag(Qnn) + 1e-8) or warm (the recompute
+ *                      from tau_tilde / v_tilde, then + 1e-8). mu / sigma_diag (N each, NULL allowed) receive the
+ *                      posteriorParamsDTC the reference holds.
+ *   gpx_epdtc_sweep  : one _local_updates pass in the given order, then _recompute (LLT, jitchol's ladder, A, V = L^-1 Kmn,
+ *                      Sigma_diag clipped at eps, mu = V^T V v~); arguments as gpx_ep_sweep, plus mu / sigma_diag as above.
+ *                      The cavity of a site reads the clipped diagonal the reference holds; the rank-1 algebra the true one.
+ *                      Launches: 9 per block of 128 sites (gather, two GEMMs for A Kb and G, a row dot (2), the site chain,
+ *                      the solve, GEMM_UPDATE of A, its mirror); 1 per parallel sweep; then 12 for the recompute beyond
+ *                      the factor sweep of LLT, and 1 for the clip.
+ *   gpx_epdtc_finish : VarDTC at Y = v~ / tau~ and precision tau~ as given (no floor), Kmm = Lm Lm^T from the ladder
+ *                      (jitter_used), without log Z~ (the caller adds it): lml, grad (the part blocks in order), dZ (M x D,
+ *                      row-major). Afterwards gpx_sparse_get(0..3) and gpx_sparse_predict / _predictive_gradients /
+ *                      _posterior_samples serve this posterior.
+ * The posterior a sweep updates (A, mu0, u) is that of the sites of the last gpx_epdtc_start or sweep on the context:
+ * tau_tilde / v_tilde passed to a sweep must be those sites (the outputs of the previous call, or the warm start's input);
+ * the entries do not compare them. finish reads only the sites it is given.
+ * Option "epdtc_drift" (gpx_set_option, default 0): a sequential sweep returns diag(Knm A Kmn) of the downdated A after its
+ * last block in sigma_diag instead of the recompute's diagonal (2 more launches and M^2 N flops; a measurement of the drift).
+ * -2: a communicator attached, P != 1, a null pointer, M < 1, RatQuad / StdPeriodic parts, a call before begin (or a sweep
+ * before start). A value > 0 is the leading minor that failed after jitchol's ladder. */
+int gpx_epdtc_begin(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M);
+int gpx_epdtc_start(gpx_ctx* ctx, const double* tau_tilde, const double* v_tilde, int warm, int parallel, int max_tries,
+                    double* jitter_used, double* mu, double* sigma_diag);
+int gpx_epdtc_sweep(gpx_ctx* ctx, const int64_t* order, double eta, double delta, int parallel, int max_tries,
+                    double* tau_tilde, double* v_tilde, double* cav_tau, double* cav_v, double* Z_hat, double* mu_hat,
+                    double* sigma2_hat, double* jitter_used, double* mu, double* sigma_diag);
+int gpx_epdtc_finish(gpx_ctx* ctx, const double* tau_tilde, const double* v_tilde, int max_tries, double* lml,
+                     double* grad, double* dZ, double* jitter_used);
+
 /* Measurement hooks (bench.py): device time of the last eval between CUDA events on the launching stream, the number
  * of kernels this library launched since creation, and per-phase accounting of the last eval. */
 typedef struct {
