@@ -121,6 +121,9 @@ EXPORTS = {
     "gpx_epdtc_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_double, ctypes.c_double,
                                        ctypes.c_int, ctypes.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     "gpx_epdtc_finish": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp, _dp]),
+    "gpx_svgp_begin": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64, _dp, _dp,
+                                      ctypes.c_int64, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp, _dp]),
+    "gpx_svgp_finish": (ctypes.c_int, [_vp, _dp, _dp, _dp, _dp, _dp, _dp]),
     "gpx_pdinv": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
     "gpx_get_stats": (ctypes.c_int, [_vp, ctypes.POINTER(GpxStats)]),
     "gpx_total_launches": (ctypes.c_int64, [_vp]),
@@ -628,6 +631,49 @@ class Engine(object):
         check(rc, "gpx_epdtc_finish")
         self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
         return lml.value, grad, dZ, jit.value
+
+    # ---- stochastic variational sparse GP (SVGP, svgp.py:10-118) -------------------------------------------------------
+    def svgp_begin(self, parts, Z, q_m, q_L, row0, nb, max_tries=5):
+        """the marginals of q(f) on the rows [row0, row0 + nb) of the data of sparse_set_data (P = 1) for the kernel
+        described by parts (as sparse_eval_multi takes them), inducing inputs Z, q(u) = N(q_m, q_L q_L^T) (q_L: M x M lower
+        triangular) -> (mu (nb,), v (nb,), KL, jitter)"""
+        Z = _f64(Z)
+        M = Z.shape[0]
+        m = _f64(np.asarray(q_m, dtype=np.float64).reshape(-1))
+        L = _f64(q_L)
+        if m.size != M or L.shape != (M, M):
+            raise ValueError("q_m must hold M = %d values and q_L be M x M" % M)
+        arr = (GpxKernPart * len(parts))()
+        keep, ngrad = [], 0
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
+        nb = int(nb)
+        mu, v = np.empty(max(nb, 0)), np.empty(max(nb, 0))
+        kl, jit = ctypes.c_double(), ctypes.c_double()
+        rc = self._L.gpx_svgp_begin(self._h, arr, len(parts), _ptr(Z), M, _ptr(m), _ptr(L), int(row0), nb, int(max_tries),
+                                    _ptr(mu), _ptr(v), ctypes.byref(kl), ctypes.byref(jit))
+        if rc > 0:
+            raise np.linalg.LinAlgError(self._L.gpx_last_error().decode())
+        check(rc, "gpx_svgp_begin")
+        self.sM = M
+        self._svgp_ngrad, self._svgp_nb = ngrad, nb
+        return mu, v, kl.value, jit.value
+
+    def svgp_finish(self, dF_dmu, dF_dv):
+        """the gradients of the bound for the batch-scaled dF_dmu, dF_dv of the last svgp_begin's batch -> (kernel gradient
+        block, dZ (M x D), dL_dm (M,), dL_dchol (M x M, lower triangular)); the posterior stays for sparse_get / predict"""
+        nb = getattr(self, "_svgp_nb", 0)
+        a = _f64(np.asarray(dF_dmu, dtype=np.float64).reshape(-1))
+        b = _f64(np.asarray(dF_dv, dtype=np.float64).reshape(-1))
+        if a.size != nb or b.size != nb:
+            raise ValueError("dF_dmu and dF_dv must hold one value per row of the last batch (%d)" % nb)
+        M = self.sM
+        grad, dZ = np.zeros(getattr(self, "_svgp_ngrad", 0)), np.empty((M, self.sD))
+        dm, dchol = np.empty(M), np.empty((M, M))
+        check(self._L.gpx_svgp_finish(self._h, _ptr(a), _ptr(b), _ptr(grad), _ptr(dZ), _ptr(dm), _ptr(dchol)),
+              "gpx_svgp_finish")
+        self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
+        return grad, dZ, dm, dchol
 
     SPARSE_GET = {"woodbury_vector": 0, "woodbury_inv": 1, "Kmm": 2, "Lm": 3}
 

@@ -64,6 +64,15 @@ struct SparseState {
   bool ep_labels = false;   // the labels of the current data were checked
   bool ep_seq = false;      // the sites run sequentially (A is updated)
   bool ep_first = false;    // the next site is the first of a run: its cavity reads the held diagonal of the start
+  // SVGP (gpx_svgp_*): M x M work matrices beyond mm (Mpad x Mpad each); small vectors ([SV_MV][Mpad]); one allocation per
+  // batch capacity sv_cap (padded rows) holding the four Mpad x sv_cap batch buffers, four sv_cap vectors and the batch's
+  // prepared points (svgp_batch)
+  double *svm[8] = {nullptr};
+  double *svv = nullptr, *svb = nullptr;
+  long sv_cap = 0, sv_row0 = 0, sv_nb = 0;
+  double sv_jit = 0.0;      // what jitchol's ladder added to Kmm in the last gpx_svgp_begin
+  bool sv_begun = false;    // gpx_svgp_begin ran on the current data, kernel and Z (psi_device and set_data clear it)
+  bool w_own = false;       // mm[9] is the posterior's own woodbury_inv (SVGP), not formed from B's factor
   Points xpts() const { return Points{XsT, sqX, N, Npad}; }   // this rank's data points, prepared
   Points zpts() const { return Points{ZsT, sqZ, M, Mpad}; }   // the inducing points, prepared
 };
@@ -74,6 +83,10 @@ void free_m(SparseState* s) {
                      &s->F2, &s->G, &s->eK, &s->eA, &s->eA0, &s->epb};
   for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
   for (auto& p : s->mm) { if (p) cudaFree(p); p = nullptr; }
+  for (auto& p : s->svm) { if (p) cudaFree(p); p = nullptr; }
+  for (double** p : {&s->svv, &s->svb}) { if (*p) cudaFree(*p); *p = nullptr; }
+  s->sv_cap = 0;
+  s->sv_begun = s->w_own = false;
   s->have_eval = false;
   s->w_ready = false;
   s->ep_begun = s->ep_ready = false;
@@ -228,6 +241,7 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
   s->have_eval = false;
   s->w_ready = false;
   s->ep_begun = s->ep_ready = s->ep_labels = false;
+  s->sv_begun = s->w_own = false;
   {   // trYYT = sum(Y .* Y) (var_dtc.py:37,90); with row shards: summed over the ranks, like num_data
     double t = 0.0;
     for (int64_t i = 0; i < N * (int64_t)P; i++) t += Y[i] * Y[i];
@@ -266,7 +280,7 @@ static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
   const MultiKern& k = s->mk;
   GPX_CHECK(ensure_rows(c, s, k));
   const long Mpad = (M + TILE - 1) / TILE * TILE, Npad = s->Npad, N = s->N;
-  if (Mpad != s->Mpad) {
+  if (Mpad != s->Mpad || !s->Kuf) {   // (gpx_svgp_begin sets up Z without psi1)
     GPX_CUDA(cudaStreamSynchronize(st));
     free_m(s);
     s->Mpad = Mpad;
@@ -286,6 +300,7 @@ static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
   }
   s->M = M;
   s->ep_begun = s->ep_ready = false;   // Kmn changes: a sparse EP run has to begin again
+  s->sv_begun = s->w_own = false;
   if (N < s->Nw || M < s->Mw) {   // fewer points than last time inside the same padded extents: stale entries must go
     GPX_CUDA(cudaMemsetAsync(s->Kuf, 0, (size_t)Mpad * Npad * 8, st));
     GPX_CUDA(cudaMemsetAsync(s->Kfu, 0, (size_t)Mpad * Npad * 8, st));
@@ -336,30 +351,35 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
   return knm_reduce(c, grad, dZ);
 }
 
-// dL_dKnm^T = dLt + sum_q C[q] (Yb[q])^T reduced to kernel-parameter gradients and dL/dZ (results on the host): dLt
-// (s->dLt), C (s->Cm, [P][Mpad]) and Yb (s->Yb, [P][Npad]) must be in place
-static int knm_reduce(gpx_ctx* c, double* grad, double* dZ) {
+// dL_dKnm^T = dLt + sum_q C[q] (Yb[q])^T reduced to kernel-parameter gradients and dL/dZ (results on the host) for the
+// data points xp: dLt (Mpad x xp.ld, column-major), C (s->Cm, [P][Mpad]) and Yb ([P][ldy]) must be in place
+static int knm_reduce_at(gpx_ctx* c, const Points& xp, double* dLt, const double* Yb, long ldy, double* grad, double* dZ) {
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
-  const long Mpad = s->Mpad, N = s->N, Npad = s->Npad;
+  const long Mpad = s->Mpad, N = xp.n;
   const int P = s->P;
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
   const MultiKern& k = s->mk;
   const bool single = as_single(k, s->D, nullptr);
   if (!single) {
-    add_rank_p_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(s->dLt, Mpad, s->M, N, s->Cm, s->Yb, Npad, P);
+    add_rank_p_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(dLt, Mpad, s->M, N, s->Cm, Yb, ldy, P);
     GPX_CHECK(launched(c));
   }
   const int cP = single ? P : 0;
-  GradFullParams gp = grad_params(k, s->D, s->xpts(), s->zpts(), s->dLt, Mpad);
-  gp.ci = s->Yb; gp.ldci = Npad; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = cP;
+  GradFullParams gp = grad_params(k, s->D, xp, s->zpts(), dLt, Mpad);
+  gp.ci = Yb; gp.ldci = ldy; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = cP;
   GPX_CHECK(ensure_part(s, grad_full_doubles(k, s->D, gp) * 8));
   GPX_CHECK(grad_full_sum(c, k, s->D, gp, s->part, grad));
   // dL/dZ: gradients_X(dL_dKnm^T, Z, X): rows = inducing points, columns = data points, dL read transposed
-  GradFullParams gx = grad_params(k, s->D, s->zpts(), s->xpts(), s->dLt, Mpad);
-  gx.transposed = 1; gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = s->Yb; gx.ldcj = Npad; gx.cP = cP;
+  GradFullParams gx = grad_params(k, s->D, s->zpts(), xp, dLt, Mpad);
+  gx.transposed = 1; gx.ci = s->Cm; gx.ldci = Mpad; gx.cj = Yb; gx.ldcj = ldy; gx.cP = cP;
   GPX_CHECK(ensure_part(s, grad_X_doubles(c, k, gx, s->D) * 8));
   return grad_X(c, k, gx, s->D, s->part, dZ);
+}
+// the same for the data of gpx_sparse_set_data with dL_dKnm^T in s->dLt and the rank-P factor in s->Yb
+static int knm_reduce(gpx_ctx* c, double* grad, double* dZ) {
+  SparseState* s = c->sparse;
+  return knm_reduce_at(c, s->xpts(), s->dLt, s->Yb, s->Npad, grad, dZ);
 }
 
 // =================================================================================================================
@@ -750,7 +770,9 @@ int gpx_sparse_get(gpx_ctx* c, int which, double* out) {
     return 0;
   }
   double* src = nullptr;
-  if (which == 1) {   // woodbury_inv = Um (I - B^-1) Um^T   (var_dtc.py:207-210); B^-1 is rebuilt from UB
+  if (which == 1 && s->w_own) {   // SVGP: Kmm^-1 - Kmm^-1 S Kmm^-1, formed by gpx_svgp_finish
+    src = s->mm[9];
+  } else if (which == 1) {   // woodbury_inv = Um (I - B^-1) Um^T   (var_dtc.py:207-210); B^-1 is rebuilt from UB
     double *Um = s->mm[1], *UB = s->mm[6], *T = s->mm[3], *E = s->mm[9], *DB = s->mm[8];
     GPX_CHECK(binv(c, UB, DB));
     GPX_CHECK(combine(c, E, Mpad, -1.0, DB, 0.0, nullptr, 1.0));
@@ -1559,6 +1581,313 @@ int gpx_epdtc_finish(gpx_ctx* c, const double* tau_tilde, const double* v_tilde,
                                   max_tries, jitter_used);
   s->Y = labels;
   return rc;
+}
+
+}  // extern "C"
+
+// =================================================================================================================
+// SVGP (svgp.py:10-118, Hensman et al. 2013 / 2015) with one output column, one latent function and no mean function, on
+// the rows [row0, row0 + nb) of the data of gpx_sparse_set_data. The likelihood's quadrature stays on the host between the
+// two entries. Layouts: "M-major" is Mpad x NBp column-major ((a, n) at a + n Mpad), "N-major" NBp x Mpad ((n, a) at
+// n + a NBp); every product is the NT DMMA GEMM (C = X Y^T), which reads its Y operand N-major when the contraction runs
+// over M and both operands M-major when it runs over the batch. Lmi = Lm^-1, Um = Lm^-T from the factor-and-invert sweep.
+//   begin:  Knm (N-major), Kmn (M-major);  Vt = Knm Lmi^T (= (Lm^-1 Kmn)^T, B lower triangular);  A = Um Vt^T
+//           (= Kmm^-1 Kmn: dpotrs's two triangular solves, svgp.py:45);  Wt = q_L^T Um;  Bq = Wt Vt^T (= q_L^T A);
+//           mu = A^T m, v = colsum(Bq^2) + (Kdiag - colsum(A o Kmn)) (:46-52);  KL (:55) with tr(Kmm^-1 S) = |Wt|_F^2
+//   finish: Ki = Um Um^T, S = q_L q_L^T, Tt = Ki S (= T^T, T = S Ki);  Adv = A diag(dF_dv), Vd = diag(dF_dv) Vt;
+//           AdvA = Adv A^T (lower tiles, mirrored);  R = AdvA T;  KSK = Ki S Ki;  dL_dKmm (:81-83,60 symmetrised);
+//           dL_dKmn^T = (2 (Tt - I) Um) Vd^T + Kmm^-1 m dF_dmu^T (:85-90; the rank-1 term added by the reductions);
+//           dL_dchol = 2 tril((AdvA - Ki / 2) q_L) + diag(1 / q_L,ii) (:113-114: S^-1 q_L = q_L^-T is upper triangular,
+//           so the reference's dpotri (Si, :22) is not formed); posterior: woodbury_vector = Kmm^-1 m, woodbury_inv =
+//           Ki - KSK (posterior.py:166-196 with K = Kmm, cov = S).
+// Products of M^2 NBp: Vt (1 M^2 NBp multiply-adds, triangular), A, Bq, dL_dKmn^T (2 each), AdvA (1, lower tiles): 8 M^2 NBp
+// flops; of M^3 (Mpad^3 multiply-adds): Wt, Tt, R, KSK, GU, H (2 each) and Ki, S (1 each, lower tiles), 28 M^3 flops, plus
+// the factor-and-invert sweep of Kmm.
+// =================================================================================================================
+namespace {
+enum { SV_M = 0, SV_LMM, SV_ADMU, SV_RPART, SV_MV = SV_RPART + 64 };   // [SV_MV][Mpad] vectors of s->svv
+enum { SB_MU = 0, SB_V, SB_DMU, SB_DV };                              // [4][sv_cap] vectors of s->svb
+constexpr int SV_RB = 64;                                             // CTAs of trace_dot_kernel
+// one batch's device buffers inside s->svb: b[0..3] Mpad x ld each, vec[4][ld], prepared points
+struct SvBatch { double* b[4]; double* vec[4]; Points x; };
+SvBatch sv_batch(SparseState* s) {
+  const size_t cap = (size_t)s->sv_cap, Mp = (size_t)s->Mpad;
+  const long ld = (s->sv_nb + TILE - 1) / TILE * TILE;
+  SvBatch b;
+  for (int k = 0; k < 4; k++) b.b[k] = s->svb + k * Mp * cap;
+  for (int k = 0; k < 4; k++) b.vec[k] = s->svb + 4 * Mp * cap + k * cap;
+  b.x = Points{s->svb + (4 * Mp + 4) * cap, s->svb + (4 * Mp + 4 + MAX_D) * cap, s->sv_nb, ld};
+  return b;
+}
+size_t sv_batch_doubles(long Mpad, long cap) { return (size_t)(4 * Mpad + 4 + MAX_D + MAX_PARTS) * cap; }
+
+// mu_n = sum_a A(a, n) m_a and v_n = sum_a Bq(a, n)^2 + (kdiag - sum_a A(a, n) Kmn(a, n)) over the M rows of M-major
+// operands (svgp.py:46-52): one warp per column, lanes over the rows in a fixed order, then the warp's fixed tree
+__global__ void __launch_bounds__(256) svgp_marg_kernel(const double* __restrict__ A, const double* __restrict__ K,
+                                                        const double* __restrict__ Bq, long ld, long M, long nb,
+                                                        const double* __restrict__ m, double kdiag, double* __restrict__ mu,
+                                                        double* __restrict__ v) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long n = (long)blockIdx.x * 8 + warp;
+  if (n >= nb) return;
+  const double *a = A + n * ld, *k = K + n * ld, *b = Bq + n * ld;
+  double am = 0.0, ak = 0.0, bb = 0.0;
+  for (long i = lane; i < M; i += 32) {
+    const double ai = a[i], bi = b[i];
+    am = fma(ai, m[i], am);
+    ak = fma(ai, k[i], ak);
+    bb = fma(bi, bi, bb);
+  }
+  am = fitc_warp_sum(am);
+  ak = fitc_warp_sum(ak);
+  bb = fitc_warp_sum(bb);
+  if (lane == 0) { mu[n] = am; v[n] = bb + (kdiag - ak); }
+}
+// out = in diag(d) (M-major in: the column index scales) or diag(d) in (N-major in: the row index scales), `total` entries,
+// leading dimension ld (svgp.py:72 Adv = A dF_dv)
+__global__ void svgp_scale_kernel(const double* __restrict__ in, long ld, long total, int rows, const double* __restrict__ d,
+                                  double* __restrict__ out) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  out[i] = in[i] * d[rows ? i % ld : i / ld];
+}
+// dL_dKmm = dF_dKmm - dKL_dKmm (svgp.py:60,81-83,116) with dF_dKmm = sym(-Admu Kmmim^T + AdvA - R - R^T), sym(X) =
+// (X + X^T) / 2, and dKL_dKmm = Ki / 2 - KSK / 2 - Kmmim Kmmim^T / 2; zero outside the M x M block
+__global__ void svgp_dkmm_kernel(const double* __restrict__ AdvA, const double* __restrict__ R, const double* __restrict__ Ki,
+                                 const double* __restrict__ KSK, const double* __restrict__ admu,
+                                 const double* __restrict__ kim, long ld, long M, double* __restrict__ out) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y;
+  if (i >= ld) return;
+  if (i >= M || j >= M) { out[i + j * ld] = 0.0; return; }
+  const long ij = i + j * ld, ji = j + i * ld;
+  const double r = R[ij] + R[ji];
+  const double x = -admu[i] * kim[j] + AdvA[ij] - r, xt = -admu[j] * kim[i] + AdvA[ji] - r;
+  const double dF = 0.5 * (x + xt);
+  const double dKL = 0.5 * Ki[ij] - 0.5 * KSK[ij] - 0.5 * kim[i] * kim[j];
+  out[ij] = dF - dKL;
+}
+// dL_dchol (M x M row-major, the lower triangle; svgp.py:113): 2 H(i, j) + [i == j] / L_ii for j <= i with
+// H = (AdvA - Ki / 2) q_L, zero above the diagonal; L_ii read from Lt = q_L^T (column-major, ld)
+__global__ void svgp_dchol_kernel(const double* __restrict__ H, const double* __restrict__ Lt, long ld, long M,
+                                  double* __restrict__ out) {
+  const long j = (long)blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
+  if (j >= M) return;
+  double v = 0.0;
+  if (j <= i) v = 2.0 * H[i + j * ld] + (i == j ? 1.0 / Lt[i + i * ld] : 0.0);
+  out[i * M + j] = v;
+}
+
+int svgp_end(gpx_ctx* c, const char* what) {
+  if (cudaStreamSynchronize(c->st) != cudaSuccess) GPX_FAIL_DEVICE(what);
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int gpx_svgp_begin(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M, const double* q_m,
+                   const double* q_L, int64_t row0, int64_t nb, int max_tries, double* mu, double* var, double* kl,
+                   double* jitter_used) {
+  if (!c || !parts || !Z || !q_m || !q_L || !mu || !var || !kl || !jitter_used) GPX_FAIL("null argument");
+  if (c->dist) GPX_FAIL("SVGP is single-GPU");
+  if (!c->sparse || !c->sparse->X) GPX_FAIL("gpx_sparse_set_data has not been called");
+  SparseState* s = c->sparse;
+  if (s->P != 1) GPX_FAIL("SVGP takes one output column and one latent function (P = 1)");
+  if (M < 1) GPX_FAIL("M must be positive");
+  if (row0 < 0 || nb < 1 || row0 > s->N - nb) GPX_FAIL("the batch rows [row0, row0 + nb) are not inside the data");
+  MultiKern mk;
+  double kdiag;
+  GPX_CHECK(fill_mk(mk, parts, nparts, s->D, &kdiag));
+  for (int p = 0; p < mk.nparts; p++)
+    if (mk.part[p].kind == GPX_RATQUAD || mk.part[p].kind == GPX_STDPERIODIC)
+      GPX_FAIL("RatQuad and StdPeriodic parts are not on the sparse evaluation (no device gradients_X)");
+  GPX_CUDA(cudaSetDevice(c->device));
+  cudaStream_t st = c->st;
+  const int D = s->D;
+  s->have_eval = s->w_ready = s->w_own = s->sv_begun = false;
+  s->mk = mk;
+  s->kdiag = kdiag;
+  memset(&c->stats, 0, sizeof(c->stats));
+  // Z and its prepared points without psi1 (psi_device's set-up; psi_device allocates psi1 when it next runs)
+  GPX_CHECK(ensure_rows(c, s, mk));
+  const long Mpad = (M + TILE - 1) / TILE * TILE;
+  if (Mpad != s->Mpad) {
+    GPX_CUDA(cudaStreamSynchronize(st));
+    free_m(s);
+    s->Mpad = Mpad;
+    GPX_CUDA(cudaMalloc(&s->Z, (size_t)Mpad * D * 8));
+    GPX_CUDA(cudaMalloc(&s->ZsT, (size_t)Mpad * s->rows_cap * 8));
+    GPX_CUDA(cudaMalloc(&s->sqZ, (size_t)Mpad * s->norm_cap * 8));
+    GPX_CUDA(cudaMalloc(&s->Cm, (size_t)Mpad * s->P * 8));
+  }
+  s->M = M;
+  if (!s->mm[0]) {   // as the other sparse entries allocate them (they expect vec with mm)
+    for (auto& p : s->mm) GPX_CUDA(cudaMalloc(&p, (size_t)Mpad * Mpad * 8));
+    GPX_CUDA(cudaMalloc(&s->vec, (size_t)(8 + 64) * s->P * Mpad * 8));
+  }
+  if (!s->svm[0]) {
+    for (auto& p : s->svm) GPX_CUDA(cudaMalloc(&p, (size_t)Mpad * Mpad * 8));
+    GPX_CUDA(cudaMalloc(&s->svv, (size_t)SV_MV * Mpad * 8));
+  }
+  if (!s->red) {
+    GPX_CUDA(cudaMalloc(&s->red, 4096 * 8));
+    GPX_CUDA(cudaMallocHost(&s->h_red, 4096 * 8));
+  }
+  if (!s->cK) { GPX_CHECK(gpx_create(c->device, &s->cK)); GPX_CHECK(gpx_create(c->device, &s->cB)); }
+  for (gpx_ctx* ch : {s->cK, s->cB})
+    if (ch->NB != c->NB) GPX_CHECK(gpx_set_option(ch, "nb", c->NB));
+  const long L = (nb + TILE - 1) / TILE * TILE;   // the batch's padded rows
+  if (L > s->sv_cap) {
+    GPX_CUDA(cudaStreamSynchronize(st));
+    if (s->svb) cudaFree(s->svb);
+    s->svb = nullptr;
+    s->sv_cap = 0;
+    if (cudaMalloc(&s->svb, sv_batch_doubles(Mpad, L) * 8) != cudaSuccess) {
+      cudaGetLastError();
+      gpx::set_error("gpx_svgp_begin: out of device memory for the batch buffers (" +
+                     std::to_string(sv_batch_doubles(Mpad, L) * 8) + " bytes)");
+      return -1;
+    }
+    s->sv_cap = L;
+  }
+  s->sv_row0 = row0;
+  s->sv_nb = nb;
+  const SvBatch b = sv_batch(s);
+  // q_L^T and q_L live in svm[6..7], which no other entry writes (gpx_sparse_get uses mm[3] as scratch)
+  double *Kd = s->mm[0], *Um = s->mm[1], *Lmi = s->mm[2], *QLt = s->svm[6], *QL = s->svm[7], *Wt = s->mm[5];
+  double *vm = s->svv + (size_t)SV_M * Mpad, *lmm = s->svv + (size_t)SV_LMM * Mpad;
+  // inputs: Z, m, q_L^T (q_L row-major read as column-major) and q_L (its transpose on the device)
+  GPX_CUDA(cudaMemcpyAsync(s->Z, Z, (size_t)M * D * 8, cudaMemcpyHostToDevice, st));
+  GPX_CUDA(cudaMemsetAsync(vm, 0, (size_t)Mpad * 8, st));
+  GPX_CUDA(cudaMemcpyAsync(vm, q_m, (size_t)M * 8, cudaMemcpyHostToDevice, st));
+  GPX_CUDA(cudaMemsetAsync(QLt, 0, (size_t)Mpad * Mpad * 8, st));
+  GPX_CUDA(cudaMemcpy2DAsync(QLt, Mpad * 8, q_L, M * 8, M * 8, M, cudaMemcpyHostToDevice, st));
+  GPX_CHECK(launch_transpose_pad(QLt, Mpad, (int)Mpad, Mpad, QL, st));
+  GPX_CHECK(launched(c));
+  // prepared points: Z and the batch rows of X
+  GPX_CHECK(prep_points(c, mk, s->Z, M, D, Mpad, s->ZsT, s->sqZ));
+  GPX_CHECK(prep_points(c, mk, s->X + (size_t)row0 * D, nb, D, L, b.x.xT, b.x.sq));
+  GPX_CHECK(launched(c, 2));
+  // Kmm and Lm = jitchol(Kmm) with logdet Kmm (svgp.py:38-42)
+  GPX_CHECK(build_Kmm(c, Kd));
+  double logdetK = 0.0, jit = 0.0;
+  *jitter_used = 0.0;
+  const int rc = factor_child(c, s->cK, Kd, 0.0, &logdetK, Um, Lmi, &jit, max_tries);
+  if (rc) return rc;
+  c->stats.tries = s->cK->stats.tries;
+  s->jitter = 0.0;   // the posterior's K is Kmm itself (svgp.py:118); Lm (gpx_sparse_get(3)) carries the ladder's jitter
+  s->sv_jit = jit;
+  *jitter_used = jit;
+  // Knm (N-major) and Kmn (M-major) of the batch, zero padded
+  GPX_CUDA(cudaMemsetAsync(b.b[0], 0, (size_t)L * Mpad * 8, st));
+  GPX_CUDA(cudaMemsetAsync(b.b[1], 0, (size_t)Mpad * L * 8, st));
+  GPX_CHECK(build_K(c, mk, D, b.x, s->zpts(), b.b[0], L));
+  GPX_CHECK(build_K(c, mk, D, s->zpts(), b.x, b.b[1], Mpad));
+  GPX_CHECK(launched(c, 2));
+  GPX_CHECK(gemm_nt(c, b.b[0], L, Lmi, Mpad, b.b[2], L, L, Mpad, Mpad, 1, 1));      // Vt = Knm Lmi^T
+  GPX_CHECK(gemm_nt(c, Um, Mpad, b.b[2], L, b.b[3], Mpad, Mpad, L, Mpad, 1, 0));    // A = Um Vt^T
+  GPX_CHECK(mm_nt(c, QLt, Lmi, Wt));                                                // Wt = q_L^T Um
+  GPX_CHECK(gemm_nt(c, Wt, Mpad, b.b[2], L, b.b[0], Mpad, Mpad, L, Mpad, 1, 0));    // Bq = q_L^T A (Knm is done)
+  svgp_marg_kernel<<<(unsigned)((nb + 7) / 8), 256, 0, st>>>(b.b[3], b.b[1], b.b[0], Mpad, M, nb, vm, kdiag,
+                                                             b.vec[SB_MU], b.vec[SB_V]);
+  GPX_CHECK(launched(c));
+  // KL (svgp.py:55): Kmm^-1 m = Lmi^T (Lmi m) (the woodbury vector, into Cm), tr(Kmm^-1 S) = |Wt|_F^2
+  GPX_CHECK(launch_col_dot(Um, Mpad, M, M, 1, vm, Mpad, lmm, Mpad, st));            // Lmi m = Um^T m
+  GPX_CHECK(launch_col_dot(Lmi, Mpad, M, M, 1, lmm, Mpad, s->Cm, Mpad, st));        // Kmm^-1 m = Lmi^T (Lmi m)
+  trace_dot_kernel<<<SV_RB, 256, 0, st>>>(Wt, Wt, Mpad, M, s->red);
+  GPX_CHECK(launched(c, 3));
+  std::vector<double> kim((size_t)M);
+  GPX_CUDA(cudaMemcpyAsync(kim.data(), s->Cm, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(s->h_red, s->red, 2 * SV_RB * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(mu, b.vec[SB_MU], (size_t)nb * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(var, b.vec[SB_V], (size_t)nb * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CHECK(svgp_end(c, "gpx_svgp_begin"));
+  double logdetS = 0.0, trKS = 0.0, mKm = 0.0;
+  for (long i = 0; i < M; i++) logdetS += log(fabs(q_L[i * M + i]));
+  logdetS *= 2.0;
+  for (int r = 0; r < SV_RB; r++) trKS += s->h_red[2 * r + 1];
+  for (long i = 0; i < M; i++) mKm += q_m[i] * kim[(size_t)i];
+  *kl = -0.5 * logdetS - 0.5 * (double)M + 0.5 * logdetK + 0.5 * trKS + 0.5 * mKm;
+  s->sv_begun = true;
+  return 0;
+}
+
+int gpx_svgp_finish(gpx_ctx* c, const double* dF_dmu, const double* dF_dv, double* grad, double* dZ, double* dL_dm,
+                    double* dL_dchol) {
+  if (!c || !dF_dmu || !dF_dv || !grad || !dZ || !dL_dm || !dL_dchol) GPX_FAIL("null argument");
+  if (!c->sparse || !c->sparse->sv_begun) GPX_FAIL("gpx_svgp_begin has not been called on this data, kernel and Z");
+  GPX_CUDA(cudaSetDevice(c->device));
+  SparseState* s = c->sparse;
+  cudaStream_t st = c->st;
+  const long Mpad = s->Mpad, M = s->M, nb = s->sv_nb;
+  const int D = s->D;
+  const SvBatch b = sv_batch(s);
+  const long L = b.x.ld;
+  double *Kd = s->mm[0], *Um = s->mm[1], *Lmi = s->mm[2], *QLt = s->svm[6], *QL = s->svm[7], *Ki = s->mm[5], *S = s->mm[6],
+         *Tt = s->mm[7], *AdvA = s->mm[8], *W = s->mm[9];
+  double *R = s->svm[0], *KSK = s->svm[1], *G = s->svm[2], *GU = s->svm[3], *Eh = s->svm[4], *H = s->svm[5];
+  double *admu = s->svv + (size_t)SV_ADMU * Mpad, *rpart = s->svv + (size_t)SV_RPART * Mpad;
+  s->have_eval = s->w_ready = s->w_own = false;
+  GPX_CUDA(cudaMemsetAsync(b.vec[SB_DMU], 0, (size_t)2 * s->sv_cap * 8, st));
+  GPX_CUDA(cudaMemcpyAsync(b.vec[SB_DMU], dF_dmu, (size_t)nb * 8, cudaMemcpyHostToDevice, st));
+  GPX_CUDA(cudaMemcpyAsync(b.vec[SB_DV], dF_dv, (size_t)nb * 8, cudaMemcpyHostToDevice, st));
+  GPX_CHECK(binv(c, Um, Ki));                                                        // Kmm^-1 = Um Um^T
+  GPX_CHECK(binv(c, QL, S));                                                         // S = q_L q_L^T
+  GPX_CHECK(mm_nt(c, Ki, S, Tt));                                                    // Tt = Kmm^-1 S = T^T
+  svgp_scale_kernel<<<(unsigned)((Mpad * L + 255) / 256), 256, 0, st>>>(b.b[3], Mpad, Mpad * L, 0, b.vec[SB_DV], b.b[0]);
+  svgp_scale_kernel<<<(unsigned)((Mpad * L + 255) / 256), 256, 0, st>>>(b.b[2], L, Mpad * L, 1, b.vec[SB_DV], b.b[1]);
+  GPX_CHECK(launched(c, 2));
+  GPX_CHECK(gemm_nt(c, b.b[0], Mpad, b.b[3], Mpad, AdvA, Mpad, Mpad, Mpad, L, 2, 0));   // AdvA = Adv A^T, lower tiles
+  mirror_tiles_kernel<<<dim3((unsigned)((Mpad + 255) / 256), (unsigned)Mpad), 256, 0, st>>>(AdvA, Mpad, Mpad);
+  GPX_CHECK(launched(c));
+  GPX_CHECK(launch_row_dot(b.b[3], Mpad, Mpad, nb, 1, b.vec[SB_DMU], L, 64, rpart, admu, st));   // Admu = A dF_dmu
+  GPX_CHECK(launched(c, 2));
+  GPX_CHECK(mm_nt(c, AdvA, Tt, R));                                                  // R = AdvA S Kmm^-1
+  GPX_CHECK(mm_nt(c, Tt, Ki, KSK));                                                  // KSK = Kmm^-1 S Kmm^-1
+  svgp_dkmm_kernel<<<dim3((unsigned)((Mpad + 255) / 256), (unsigned)Mpad), 256, 0, st>>>(AdvA, R, Ki, KSK, admu, s->Cm,
+                                                                                         Mpad, M, Kd);
+  GPX_CHECK(launched(c));
+  // dL_dKmn^T = 2 (Tt - I) Adv = (2 (Tt - I) Um) Vd^T, into the Adv buffer (AdvA is formed)
+  GPX_CHECK(combine(c, G, Mpad, 2.0, Tt, 0.0, nullptr, -2.0));
+  GPX_CHECK(mm_nt(c, G, Lmi, GU));                                                   // GU = G Um
+  GPX_CHECK(gemm_nt(c, GU, Mpad, b.b[1], L, b.b[0], Mpad, Mpad, L, Mpad, 1, 0));
+  // dL_dchol and the posterior's woodbury_inv
+  GPX_CHECK(combine(c, Eh, Mpad, 1.0, AdvA, -0.5, Ki, 0.0));
+  GPX_CHECK(mm_nt(c, Eh, QLt, H));                                                   // H = (AdvA - Ki / 2) q_L
+  svgp_dchol_kernel<<<dim3((unsigned)((M + 255) / 256), (unsigned)M), 256, 0, st>>>(H, QLt, Mpad, M, Eh);
+  GPX_CHECK(launched(c));
+  // woodbury_inv = Lm^-T Lm^-1 (Kmm - S) Lm^-T Lm^-1 (posterior.py:187-191 with K = Kmm and K_chol = Lm): Ki - KSK, less
+  // j Ki^2 when the ladder factored Kmm + j I (Ki Kmm Ki = Ki - j Ki Ki)
+  GPX_CUDA(cudaMemsetAsync(W, 0, (size_t)Mpad * Mpad * 8, st));
+  if (s->sv_jit > 0.0) {
+    GPX_CHECK(mm_nt(c, Ki, Ki, R));                                                  // R is free: Ki Ki
+    GPX_CHECK(combine(c, W, M, 1.0, Ki, -s->sv_jit, R, 0.0));
+    GPX_CHECK(combine(c, W, M, 1.0, W, -1.0, KSK, 0.0));
+  } else {
+    GPX_CHECK(combine(c, W, M, 1.0, Ki, -1.0, KSK, 0.0));
+  }
+  std::vector<double> hadmu((size_t)M), hkim((size_t)M);
+  GPX_CUDA(cudaMemcpyAsync(dL_dchol, Eh, (size_t)M * M * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(hadmu.data(), admu, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(hkim.data(), s->Cm, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
+  // the kernel's gradient block: the Kmn reductions with the rank-1 term Kmm^-1 m dF_dmu^T, then the Kmm ones
+  const int ngk = kern_ngrad(s->mk);
+  std::vector<double> g_knm(ngk, 0.0), g_kmm(ngk, 0.0), hz((size_t)M * D);
+  GPX_CHECK(knm_reduce_at(c, b.x, b.b[0], b.vec[SB_DMU], L, g_knm.data(), dZ));
+  const GradFullParams gk = grad_params(s->mk, D, s->zpts(), s->zpts(), Kd, Mpad);
+  GPX_CHECK(ensure_part(s, grad_full_doubles(s->mk, D, gk) * 8));
+  GPX_CHECK(grad_full_sum(c, s->mk, D, gk, s->part, g_kmm.data()));
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, s->mk, gk, D) * 8));
+  GPX_CHECK(grad_X(c, s->mk, gk, D, s->part, hz.data()));
+  GPX_CHECK(svgp_end(c, "gpx_svgp_finish"));
+  for (size_t i = 0; i < hz.size(); i++) dZ[i] += hz[i];
+  double ddiag = 0.0;   // dL_dKdiag = dF_dv through update_gradients_diag (core/svgp.py:60)
+  for (long n = 0; n < nb; n++) ddiag += dF_dv[n];
+  kern_grads(s, ddiag, g_knm, g_kmm, grad);
+  for (long i = 0; i < M; i++) dL_dm[i] = hadmu[(size_t)i] - hkim[(size_t)i];   // dF_dm - dKL_dm (:97,116)
+  s->w_ready = s->w_own = true;
+  s->have_eval = true;
+  return 0;
 }
 
 }  // extern "C"

@@ -717,10 +717,102 @@ def _make_epdtc(base, kernel_types, ffi):
     return B200EPDTC
 
 
+def _make_svgp(base, kernel_types, ffi):
+    from .svgp import SVGPInference, q_triangle
+
+    class B200SVGP(base):
+        """GPy.inference.latent_function_inference.SVGP with Kmm, Kmn, A = Kmm^-1 Kmn, the marginals, the KL term and every
+        gradient on the device (gpx_svgp_begin / _finish) around the likelihood's own variational_expectations on the
+        host, for a plugin stationary kernel or a B.Add / B.Prod over plugin stationary leaves and GPy's own White / Bias,
+        any likelihood, ndarray X, one output column and one latent function, no mean function; anything else goes to the
+        stock method (svgp.py:12-118). The grad dict has the stock keys: dL_dKmn / dL_dKmm are handles of the gradients the
+        device already reduced (GPy's unchanged SVGP.parameters_changed passes them to update_gradients_full and
+        gradients_X, core/svgp.py:53-62), dL_dKdiag, dL_dm, dL_dchol (flat) and dL_dthetaL are the real arrays."""
+
+        def __init__(self, device=0, engine=None):
+            super(B200SVGP, self).__init__()
+            self.device, self._engine = device, engine
+            self._dev = None
+
+        @property
+        def engine(self):
+            if self._engine is None:
+                self._engine = ffi.Engine(self.device)
+            return self._engine
+
+        def invalidate_data(self):
+            if self._dev is not None:
+                self._dev.invalidate_data()
+
+        def __getstate__(self):
+            d = dict(self.__dict__)
+            d["_engine"], d["_dev"] = None, None
+            return d
+
+        def _leaves(self, kern, X, Y, q_u_mean, mean_function):
+            """-> None (the stock method), False (a single plugin kernel) or the leaves of a plugin sum / product"""
+            if not (isinstance(X, np.ndarray) and mean_function is None and np.ndim(Y) == 2 and np.shape(Y)[1] == 1
+                    and np.ndim(q_u_mean) == 2 and np.shape(q_u_mean)[1] == 1):
+                return None
+            if isinstance(kern, kernel_types):
+                return False
+            if not hasattr(kern, "_gpx_is_prod"):
+                return None
+            leaves = _flatten(kern)
+            if leaves is None or any(not (hasattr(l, "_gpx_kind") or type(l).__name__ in ("White", "Bias"))
+                                     for l, _ in leaves):
+                return None                                        # RatQuad / StdPeriodic: no device gradients_X
+            return leaves
+
+        def inference(self, q_u_mean, q_u_chol, kern, X, Z, likelihood, Y, mean_function=None, Y_metadata=None,
+                      KL_scale=1.0, batch_scale=1.0):
+            leaves = self._leaves(kern, X, Y, q_u_mean, mean_function)
+            if leaves is None:
+                return super(B200SVGP, self).inference(q_u_mean, q_u_chol, kern, X, Z, likelihood, Y, mean_function,
+                                                       Y_metadata, KL_scale, batch_scale)
+            if self._dev is None:
+                self._dev = SVGPInference(engine=self.engine)
+            dev = self._dev
+            if leaves:
+                parts = [_leaf_descriptor(l, t) for (l, t) in leaves]
+                Xs, Zs, key = np.asarray(X), np.asarray(Z), _composite_key(kern)
+            else:
+                Xs = kern._slice_X(X)[0] if _returns_tuple(kern, X) else kern._slice_X(X)
+                Zs = kern._slice_X(Z)[0] if _returns_tuple(kern, Z) else kern._slice_X(Z)
+                k, ard, var, ls = kern._gpx_theta()
+                parts = [(k, ard, 0, list(range(np.shape(Xs)[1])), var, ls)]
+                key = kern._gpx_state_key()
+            Xs = np.ascontiguousarray(Xs, dtype=np.float64)
+            Zs = np.ascontiguousarray(Zs, dtype=np.float64)
+            Yc = np.ascontiguousarray(Y, dtype=np.float64)
+            q_m = np.asarray(q_u_mean, dtype=np.float64)
+            L = q_triangle(q_m, np.asarray(q_u_chol, dtype=np.float64), Zs.shape[0])
+            eng = self.engine
+            if not dev._data_key.matches(Xs, Yc):
+                eng.sparse_set_data(Xs, Yc)
+                dev._data_key.remember(Xs, Yc)
+            N, M = Yc.shape[0], Zs.shape[0]
+            post, lml, grad, gd = dev.device_inference(q_m, L, parts, key, Zs, likelihood, Yc, 0, N, Y_metadata,
+                                                       batch_scale)
+            dL_dKdiag, dZ = gd["dL_dKdiag"], gd["dZ"]
+            if leaves:
+                h_knm, h_kmm = _composite_handles(kern, leaves, grad, dL_dKdiag.sum(), dZ, N, M)
+            else:
+                dlen = np.atleast_1d(grad[1:])
+                h_knm = SparseDeviceGradient(key, "knm", (N, M), grad[0] - dL_dKdiag.sum(), dlen, dZ)
+                h_kmm = SparseDeviceGradient(key, "kmm", (M, M), 0.0, np.zeros_like(dlen), np.zeros_like(dZ))
+            return post, lml, {"dL_dKmm": h_kmm, "dL_dKmn": h_knm.T, "dL_dKdiag": dL_dKdiag, "dL_dm": gd["dL_dm"],
+                               "dL_dchol": gd["dL_dchol"], "dL_dthetaL": gd["dL_dthetaL"]}
+
+    B200SVGP.__name__ = B200SVGP.__qualname__ = "SVGP"
+    return B200SVGP
+
+
 def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None,
-         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None, EP=None, EPDTC=None):
+         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None, EP=None, EPDTC=None, SVGP=None):
     """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC /
-    FITC optional: the sparse model; Laplace / EP / EPDTC optional: non-Gaussian likelihoods; RatQuad / StdPeriodic optional: leaves
+    FITC optional: the sparse model; Laplace / EP / EPDTC optional: non-Gaussian likelihoods; SVGP optional: the
+    stochastic variational sparse GP; RatQuad / StdPeriodic optional: leaves
     the composite evaluation knows, alone or inside Add / Prod)."""
     kernels = {n: _make_kernel(b, _KINDS[n], ffi) for n, b in
                (("RBF", RBF), ("Exponential", Exponential), ("Matern32", Matern32), ("Matern52", Matern52))}
@@ -825,6 +917,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
         extra["EP"] = _make_ep(EP, kernel_types, ffi)
     if EPDTC is not None:
         extra["EPDTC"] = _make_epdtc(EPDTC, kernel_types, ffi)
+    if SVGP is not None:
+        extra["SVGP"] = _make_svgp(SVGP, kernel_types, ffi)
     return types.SimpleNamespace(ExactGaussianInference=B200ExactGaussianInference, **kernels, **extra)
 
 
@@ -839,6 +933,7 @@ def load():
     import GPy
     from GPy.inference.latent_function_inference import EP, FITC, ExactGaussianInference, Laplace, VarDTC
     from GPy.inference.latent_function_inference.expectation_propagation import EPDTC
+    from GPy.inference.latent_function_inference.svgp import SVGP
     return make(GPy.kern.RBF, GPy.kern.Exponential, GPy.kern.Matern32, GPy.kern.Matern52, ExactGaussianInference,
                 Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic,
-                FITC=FITC, Laplace=Laplace, EP=EP, EPDTC=EPDTC)
+                FITC=FITC, Laplace=Laplace, EP=EP, EPDTC=EPDTC, SVGP=SVGP)

@@ -33,6 +33,16 @@ class Gaussian(Parameterized):
     def exact_inference_gradients(self, dL_dKdiag, Y_metadata=None):
         return np.asarray(dL_dKdiag).sum()
 
+    def variational_expectations(self, Y, m, v, gh_points=None, Y_metadata=None):
+        """gaussian.py:336-345 (identity link): E_q[log p(y | f)] for q(f) = N(m, v) in closed form -> (F, dF_dmu, dF_dv,
+        dF_dtheta (1, N, P))"""
+        lik_var = np.asarray(self.variance.values, dtype=np.float64).item()
+        F = -0.5 * np.log(2 * np.pi) - 0.5 * np.log(lik_var) - 0.5 * (np.square(Y) + np.square(m) + v - 2 * m * Y) / lik_var
+        dF_dmu = (Y - m) / lik_var
+        dF_dv = np.ones_like(v) * (-0.5 / lik_var)
+        dF_dtheta = -0.5 / lik_var + 0.5 * (np.square(Y) + np.square(m) + v - 2 * m * Y) / (lik_var ** 2)
+        return F, dF_dmu, dF_dv, dF_dtheta.reshape(1, Y.shape[0], Y.shape[1])
+
     def predictive_values(self, mu, var, full_cov=False, Y_metadata=None):
         if full_cov:
             var = var + np.eye(var.shape[0]) * float(self.variance[0])

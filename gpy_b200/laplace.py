@@ -58,6 +58,37 @@ def _chain_3(d3f_dg3, dg_dx, d2f_dg2, d2g_dx2, df_dg, d3g_dx3):
     return d3f_dg3 * dg_dx_3 + 3 * d2f_dg2 * dg_dx * d2g_dx2 + df_dg * d3g_dx3
 
 
+def _gh_points(T=20):
+    """likelihood.py:268-271: the T-point Gauss-Hermite rule"""
+    return np.polynomial.hermite.hermgauss(T)
+
+
+def quadrature_expectations(lik, Y, m, v, dlogpdf_dtheta=None, gh=None):
+    """Likelihood.variational_expectations (likelihood.py:358-411): E_q[log p(y | f)] and its derivatives in m and v for
+    q(f) = N(m, v) by Gauss-Hermite quadrature on lik's logpdf, dlogpdf_df and d2logpdf_df2; dlogpdf_dtheta(f, y) -> the
+    (size, N, T) parameter derivatives on the grid, or None for a likelihood without parameters. -> (F, dF_dm, dF_dv,
+    dF_dtheta (size, N, P) or None)"""
+    gh_x, gh_w = _gh_points() if gh is None else gh
+    shape = m.shape
+    m, v, Y = m.flatten(), v.flatten(), Y.flatten()
+    X = gh_x[None, :] * np.sqrt(2. * v[:, None]) + m[:, None]
+    logp = lik.logpdf(X, Y[:, None])
+    dlogp_dx = lik.dlogpdf_df(X, Y[:, None])
+    d2logp_dx2 = lik.d2logpdf_df2(X, Y[:, None])
+    F = np.dot(logp, gh_w) / np.sqrt(np.pi)
+    dF_dm = np.dot(dlogp_dx, gh_w) / np.sqrt(np.pi)
+    dF_dv = np.dot(d2logp_dx2, gh_w) / np.sqrt(np.pi)
+    dF_dv /= 2.
+    if not (np.all(np.isfinite(dF_dv)) and np.all(np.isfinite(dF_dm))):
+        # the reference stops on an undefined name here (likelihood.py:400-403)
+        raise NameError("name 'stop' is not defined")
+    dF_dtheta = None
+    if dlogpdf_dtheta is not None:
+        dt = np.dot(dlogpdf_dtheta(X, Y[:, None]), gh_w) / np.sqrt(np.pi)
+        dF_dtheta = dt.reshape(dt.shape[0], shape[0], shape[1])
+    return F.reshape(*shape), dF_dm.reshape(*shape), dF_dv.reshape(*shape), dF_dtheta
+
+
 class Bernoulli(Parameterized):
     """GPy.likelihoods.Bernoulli with its default probit link (bernoulli.py; link_functions.py:109-126): y in {0, 1},
     p(y = 1 | f) = Phi(f). Log-concave, no parameters."""
@@ -117,6 +148,24 @@ class Bernoulli(Parameterized):
         g = self._transf(f)
         return _chain_3(self.d3logpdf_dlink3(g, y), std_norm_pdf(f), self.d2logpdf_dlink2(g, y), -f * std_norm_pdf(f),
                         self.dlogpdf_dlink(g, y), self._d3transf(f))
+
+    def variational_expectations(self, Y, m, v, gh_points=None, Y_metadata=None):
+        """bernoulli.py:94-115 (probit): the 20-point Gauss-Hermite rule on log Phi(y_sign f), p clipped to [1e-9, 1 - 1e-9]
+        -> (F, dF_dmu, dF_dv, None)"""
+        gh_x, gh_w = _gh_points() if gh_points is None else gh_points
+        gh_w = gh_w / np.sqrt(np.pi)
+        shape = m.shape
+        m, v, Y = m.flatten(), v.flatten(), Y.flatten()
+        Ysign = np.where(Y == 1, 1, -1)
+        X = gh_x[None, :] * np.sqrt(2. * v[:, None]) + (m * Ysign)[:, None]
+        p = ndtr(X)
+        p = np.clip(p, 1e-9, 1. - 1e-9)
+        N = std_norm_pdf(X)
+        F = np.log(p).dot(gh_w)
+        NoverP = N / p
+        dF_dm = (NoverP * Ysign[:, None]).dot(gh_w)
+        dF_dv = -0.5 * (NoverP ** 2 + NoverP * X).dot(gh_w)
+        return F.reshape(*shape), dF_dm.reshape(*shape), dF_dv.reshape(*shape), None
 
     def _laplace_gradients(self, f, y, Y_metadata=None):
         """likelihood.py:722-733 for a likelihood without parameters: three (0, N, 1) arrays"""
@@ -201,6 +250,11 @@ class StudentT(Parameterized):
         e2_s2v = e ** 2 + s2 * df
         d2v = (-s2 * (df + 1) + e2 - s2 * df) / e2_s2v ** 2 - 2 * s2 * (df + 1) * (e2 - s2 * df) / e2_s2v ** 3
         return np.array((dvar, dv)), np.array((d1var, d1v)), np.array((d2var, d2v))
+
+    def variational_expectations(self, Y, m, v, gh_points=None, Y_metadata=None):
+        """likelihood.py:358-411 (the generic quadrature; student_t.py has no closed form) -> (F, dF_dmu, dF_dv,
+        dF_dtheta (2, N, P): t_scale2, deg_free)"""
+        return quadrature_expectations(self, Y, m, v, lambda f, y: self._laplace_gradients(f, y)[0], gh_points)
 
     def predictive_mean(self, mu, sigma, Y_metadata=None):
         return mu                                                                  # the identity link (student_t.py)

@@ -434,6 +434,41 @@ int gpx_epdtc_sweep(gpx_ctx* ctx, const int64_t* order, double eta, double delta
 int gpx_epdtc_finish(gpx_ctx* ctx, const double* tau_tilde, const double* v_tilde, int max_tries, double* lml,
                      double* grad, double* dZ, double* jitter_used);
 
+/* Stochastic variational sparse GP (GPy's SVGP, svgp.py:10-118 with the gradient wiring of core/svgp.py:53-66) with one
+ * output column, one latent function and no mean function, for any likelihood: the host evaluates the likelihood's
+ * variational expectations (F, dF_dmu, dF_dv) between the two entries. The batch is the rows [row0, row0 + nb) of the data
+ * of gpx_sparse_set_data (P = 1), so a step uploads only Z, theta, m and q_L. The kernels are those gpx_sparse_eval_multi
+ * takes.
+ *   gpx_svgp_begin  : Kmm (no const jitter), Lm = jitchol(Kmm) with max_tries (jitter_used: what the ladder added) and
+ *                     logdet Kmm (:38-42); Kmn of the batch; A = Kmm^-1 Kmn as the two triangular products of dpotrs (:45);
+ *                     mu = A^T m and var = colsum((q_L^T A)^2) + Kdiag - colsum(A o Kmn) (:46-52), nb each; kl, the KL term
+ *                     (:55). q_m: M values; q_L: M x M row-major, read on and below the diagonal (the host expands GPy's
+ *                     flat q_u_chol with np.tril_indices(M)); a zero on its diagonal gives kl = +inf and infinite dL_dchol
+ *                     entries (the reference's Si). Launches: 14 + F (F: the factor-and-invert sweep of Kmm).
+ *   gpx_svgp_finish : the gradients of F.sum() - KL for the batch-scaled dF_dmu and dF_dv (nb each) of the last begin
+ *                     (:60-116): grad, the kernel's gradient block (the Kmm, Kmn and Kdiag shares, as gpx_sparse_eval_multi
+ *                     orders it); dZ (M x D, row-major); dL_dm (M); dL_dchol (M x M row-major, zero above the diagonal) =
+ *                     2 tril((AdvA - Kmm^-1 / 2) q_L) + diag(1 / q_L,ii), which is 2 tril(dL_dS q_L) without forming S^-1.
+ *                     It publishes the posterior (woodbury_vector = Kmm^-1 m, woodbury_inv = Kmm^-1 - Kmm^-1 S Kmm^-1
+ *                     with Kmm^-1 from the ladder's factor, less j Kmm^-2 when the ladder added j (two more launches),
+ *                     posterior.py:166-196 with K = Kmm): afterwards gpx_sparse_get(0..3), gpx_sparse_predict,
+ *                     _predictive_gradients and _posterior_samples serve it (gpx_sparse_get(2) is Kmm without the
+ *                     ladder's jitter, as the reference's Posterior holds it). It may be repeated with other dF_dmu / dF_dv.
+ *                     Launches: 27 for a single kernel, 26 + 2 nparts for a composite.
+ * Flops: 8 M^2 NBp on the DMMA GEMM (NBp = nb padded to 128) and 28 M^3 plus the factor sweep (M: padded to 128).
+ * Device memory held between the calls: 8 NBp (4 Mpad + 76) bytes for the batch (Kmn in both layouts, A in both layouts
+ * and the temporaries that reuse them, four vectors, the prepared points), grown to the largest batch seen, plus
+ * 18 Mpad^2 doubles (144 Mpad^2 bytes) of M x M work matrices. Launch counts do not depend on nb. -1 with a message when
+ * the batch buffers do not fit.
+ * -2, with nothing touched: a null pointer, M < 1, P != 1, a communicator attached, RatQuad / StdPeriodic parts, a row range
+ * outside the data, a finish without a begin on the current data, kernel and Z. A value > 0 is the leading minor of Kmm
+ * that failed after jitchol's ladder. */
+int gpx_svgp_begin(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M, const double* q_m,
+                   const double* q_L, int64_t row0, int64_t nb, int max_tries, double* mu, double* var, double* kl,
+                   double* jitter_used);
+int gpx_svgp_finish(gpx_ctx* ctx, const double* dF_dmu, const double* dF_dv, double* grad, double* dZ, double* dL_dm,
+                    double* dL_dchol);
+
 /* Measurement hooks (bench.py): device time of the last eval between CUDA events on the launching stream, the number
  * of kernels this library launched since creation, and per-phase accounting of the last eval. */
 typedef struct {
