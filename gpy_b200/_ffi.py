@@ -80,6 +80,7 @@ EXPORTS = {
     "gpx_get": (ctypes.c_int, [_vp, ctypes.c_int, _dp]),
     "gpx_predict": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
     "gpx_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
+    "gpx_exact_grad_X": (ctypes.c_int, [_vp, _dp]),
     "gpx_sparse_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
     "gpx_posterior_covariance": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, ctypes.c_int64, _dp]),
     "gpx_posterior_samples": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
@@ -236,10 +237,10 @@ class Engine(object):
         X, Y = _f64(X), _f64(Y)
         if X.ndim != 2 or Y.ndim != 2 or X.shape[0] != Y.shape[0]:
             raise ValueError("X must be N x D and Y N x P")
-        self.N, self.D = X.shape
-        self.P = Y.shape[1]
+        (N, D), P = X.shape, Y.shape[1]
         self.eval_serial += 1
-        check(self._L.gpx_set_data(self._h, _ptr(X), self.N, self.D, _ptr(Y), self.P), "gpx_set_data")
+        check(self._L.gpx_set_data(self._h, _ptr(X), N, D, _ptr(Y), P), "gpx_set_data")
+        self.N, self.D, self.P = N, D, P      # a rejected data set leaves the engine's shapes as they were
 
     def exact_eval(self, kind, ARD, variance, lengthscale, noise, jitter=1e-8, max_tries=5):
         """-> (log_marginal, gradient[variance, lengthscale.., noise], extra_jitter_used)"""
@@ -314,6 +315,12 @@ class Engine(object):
     def predictive_gradients(self, Xnew):
         """GP.predictive_gradients (gp.py:418-474) with the last exact evaluation -> (dmu (M, D, P), dvar (M, D))"""
         return self._pred_grads(self._L.gpx_predictive_gradients, "gpx_predictive_gradients", Xnew, self.D, self.P)
+
+    def exact_grad_X(self):
+        """kern.gradients_X(dL_dK, X, None) of the last exact evaluation (gplvm.py:47-49) at the data it holds -> (N, D)"""
+        dX = np.empty((self.N, self.D))
+        check(self._L.gpx_exact_grad_X(self._h, _ptr(dX)), "gpx_exact_grad_X")
+        return dX
 
     def sparse_predictive_gradients(self, Xnew):
         """the same with the last sparse evaluation (predictive variable Z) -> (dmu (M, D, P), dvar (M, D))"""

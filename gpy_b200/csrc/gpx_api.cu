@@ -27,7 +27,7 @@ using namespace gpx;
 
 void gpx::free_data(gpx_ctx* c) {
   double** ptrs[] = {&c->dX, &c->dXsT, &c->dsq, &c->dY, &c->dT, &c->dAlpha, &c->dUvPart, &c->S, &c->Pbuf, &c->Tm,
-                     &c->Ldiag, &c->Dinv, &c->logdet_part, &c->partials, &c->Kinv, &c->staging};
+                     &c->Ldiag, &c->Dinv, &c->logdet_part, &c->partials, &c->Kinv, &c->staging, &c->dTt};
   for (auto p : ptrs) {
     if (*p) cudaFree(*p);
     *p = nullptr;
@@ -58,9 +58,11 @@ int gpx::alloc_data(gpx_ctx* c, long NB) {
   GPX_CUDA(cudaMalloc(&c->dXsT, (size_t)Npad * c->D * 8));
   GPX_CUDA(cudaMalloc(&c->dsq, (size_t)Npad * 8));
   c->rows_cap = c->D; c->norm_cap = 1;
-  GPX_CUDA(cudaMalloc(&c->dY, (size_t)Npad * c->P * 8));
-  GPX_CUDA(cudaMalloc(&c->dT, (size_t)Npad * c->P * 8));
-  GPX_CUDA(cudaMalloc(&c->dAlpha, (size_t)Npad * c->P * 8));
+  const long Pc = c->P > MAX_P ? c->Ppad : c->P;   // the wide route keeps whole tiles of outputs
+  GPX_CUDA(cudaMalloc(&c->dY, (size_t)Npad * Pc * 8));
+  GPX_CUDA(cudaMalloc(&c->dT, (size_t)Npad * Pc * 8));
+  GPX_CUDA(cudaMalloc(&c->dAlpha, (size_t)Npad * Pc * 8));
+  if (c->P > MAX_P) GPX_CUDA(cudaMalloc(&c->dTt, (size_t)Npad * Pc * 8));
   GPX_CUDA(cudaMalloc(&c->Tm, (size_t)NB * NB * 8));
   GPX_CUDA(cudaMalloc(&c->Ldiag, (size_t)Npad * TILE * 8));
   GPX_CUDA(cudaMalloc(&c->Dinv, (size_t)Npad * TILE * 8));
@@ -181,7 +183,8 @@ int gpx_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y,
   if (!c || !X || !Y) GPX_FAIL("null argument");
   if (N < 1) GPX_FAIL("N must be positive");
   if (D < 1 || D > MAX_D) GPX_FAIL("input dimension must be in [1, 64]");
-  if (P < 1 || P > MAX_P) GPX_FAIL("number of output columns must be in [1, 8]");
+  if (P < 1 || P > GPX_MAX_OUTPUTS) GPX_FAIL("number of output columns must be in [1, 1024]");
+  if (P > MAX_P && c->dist) GPX_FAIL("more than 8 output columns are single-GPU");
   GPX_CUDA(cudaSetDevice(c->device));
   const long Npad = (N + TILE - 1) / TILE * TILE;
   if (c->dist) {
@@ -189,11 +192,11 @@ int gpx_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y,
   } else if (Npad != c->Npad || D != c->D || P != c->P) {
     GPX_CUDA(cudaStreamSynchronize(c->st));
     free_data(c);
-    c->Npad = Npad; c->D = D; c->P = P;
+    c->Npad = Npad; c->D = D; c->P = P; c->Ppad = (P + TILE - 1) / TILE * TILE;
     const long NB = choose_nb(c);
     c->NBw = NB;
     GPX_CHECK(alloc_data(c, NB));
-    GPX_CUDA(cudaMalloc(&c->dUvPart, (size_t)KSPLIT * Npad * P * 8));
+    if (P <= MAX_P) GPX_CUDA(cudaMalloc(&c->dUvPart, (size_t)KSPLIT * Npad * P * 8));
     GPX_CUDA(cudaMalloc(&c->S, (size_t)Npad * Npad * 8));
     GPX_CUDA(cudaMalloc(&c->Pbuf, (size_t)2 * Npad * NB * 8));   // double-buffered for the look-ahead
   }
@@ -203,9 +206,14 @@ int gpx_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y,
   laplace_release(c);
   // X: keep the caller's row-major layout on device; Y: SoA [P][Npad] zero padded (staged through dT)
   GPX_CUDA(cudaMemcpyAsync(c->dX, X, (size_t)N * D * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CUDA(cudaMemcpyAsync(c->dT, Y, (size_t)N * P * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(launch_transpose_pad(c->dT, N, P, c->Npad, c->dY, c->st));
-  c->total_launches += 1;
+  if (P > MAX_P) {   // the wide route's GEMM operand: Y row-major with rows of Ppad, zero padded
+    GPX_CUDA(cudaMemsetAsync(c->dY, 0, (size_t)c->Npad * c->Ppad * 8, c->st));
+    GPX_CUDA(cudaMemcpy2DAsync(c->dY, (size_t)c->Ppad * 8, Y, (size_t)P * 8, (size_t)P * 8, N, cudaMemcpyHostToDevice, c->st));
+  } else {
+    GPX_CUDA(cudaMemcpyAsync(c->dT, Y, (size_t)N * P * 8, cudaMemcpyHostToDevice, c->st));
+    GPX_CHECK(launch_transpose_pad(c->dT, N, P, c->Npad, c->dY, c->st));
+    c->total_launches += 1;
+  }
   GPX_CUDA(cudaStreamSynchronize(c->st));
   return 0;
 }
@@ -278,7 +286,7 @@ static bool oz_wanted(const gpx_ctx* c) {
   // off by default: on the H100 the fp64 DMMA.16x8x4 GEMMs are faster than the int8 digit split (140 vs 183 ms at
   // N = 16384, H100 80GB HBM3 at a 400 W power limit, profiles/h100_bench_*); option "ozaki" = 1 or GPX_OZAKI=1 selects it
   if (on < 0) { const char* e = getenv("GPX_OZAKI"); on = e ? atoi(e) : 0; }
-  if (!on) return false;
+  if (!on || c->P > MAX_P) return false;   // the int8 sweep's forward substitution carries at most 8 columns
   const long NB = pick_nb(c);
   // wherever there are at least two panels; a single-block matrix has no panel and stays on the DMMA path
   return c->Npad >= 2 * NB && NB % OZ_KC == 0;
@@ -631,6 +639,32 @@ static int build_Ky(gpx_ctx* c, double extra_jitter, bool single, bool int8, Rec
   return 0;
 }
 
+// the single-kernel kernels serve the evaluation (its reductions and result layout): a single stationary kernel and at most
+// MAX_P output columns; above that a single kernel runs as its one-part description through the composite pass
+static bool single_route(const gpx_ctx* c, KernParams* kp) { return as_single(c->mk, c->D, kp) && c->P <= MAX_P; }
+
+// The wide route's solves on the DMMA GEMM (C = A B^T, column-major operands): T^T = Y^T (L^-1)^T with L^-1 lower (T into
+// dTt, [Npad][Ppad]), then alpha = U T with U = L^-T extracted with zeros below the diagonal (full k range), and T once more
+// as [Ppad][Npad] for the LML's quadratic term. L^-1 and U pass through c->Kinv, which the LAUUM overwrites afterwards.
+static int solve_wide(gpx_ctx* c) {
+  const long Npad = c->Npad, Ppad = c->Ppad;
+  GPX_CHECK(extract_inverse_factor(c, 0, c->Kinv));
+  GemmParams g = gemm_defaults();
+  g.mode = GEMM_PANEL; g.plain = 1; g.tri = 1;
+  g.A = c->dY; g.lda = Ppad; g.B = c->Kinv; g.ldb = Npad; g.C = c->dTt; g.ldc = Ppad;
+  g.K = (int)Npad; g.nt = (int)(Ppad / TILE); g.ncols = (int)(Npad / TILE);
+  GPX_CHECK(launch_gemm(g, dim3(1, 1), c->st));
+  GPX_CHECK(extract_inverse_factor(c, 1, c->Kinv));
+  g = gemm_defaults();
+  g.mode = GEMM_PANEL; g.plain = 1; g.tri = 0;
+  g.A = c->Kinv; g.lda = Npad; g.B = c->dTt; g.ldb = Ppad; g.C = c->dAlpha; g.ldc = Npad;
+  g.K = (int)Npad; g.nt = (int)(Npad / TILE); g.ncols = (int)(Ppad / TILE);
+  GPX_CHECK(launch_gemm(g, dim3(1, 1), c->st));
+  GPX_CHECK(launch_transpose_pad(c->dTt, Npad, (int)Ppad, Npad, c->dT, c->st));
+  c->eval_launches += 5;
+  return 0;
+}
+
 // Where K^-1 of one evaluation comes from; the gradient reductions follow from it
 enum KinvRoute {
   KINV_FUSED,   // DMMA sweep, single kernel, nt > 8: the fused LAUUM epilogue reduces it, nothing is stored
@@ -647,7 +681,7 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
   const long ld = c->Npad;
   const int nt = (int)(c->Npad / TILE);
   KernParams kp;
-  const bool single = as_single(c->mk, c->D, &kp);
+  const bool single = single_route(c, &kp), wide = c->P > MAX_P;
   const int ngrad = kern_ngrad(c->mk), nl = ngrad - 1;   // nl: the single kernel's lengthscales
   const bool int8 = oz_wanted(c);
   const KinvRoute route = int8 ? KINV_SWEEP : !single ? KINV_PLAIN : nt <= 8 ? KINV_FINE : KINV_FUSED;
@@ -666,10 +700,14 @@ static int eval_once(gpx_ctx* c, double extra_jitter, Recorder& rec, bool* kinv_
   const double* T = int8 ? c->dTfw : c->dT;
   {
     const int h = rec.begin(PH_SOLVE);
-    if (!int8) GPX_CHECK(launch_utv(c->S, ld, c->Npad, c->P, c->dY, c->dT, st));
-    GPX_CHECK(launch_uv(c->S, ld, c->Npad, c->P, T, KSPLIT, c->dUvPart, c->dAlpha, st));
+    if (wide) {
+      GPX_CHECK(solve_wide(c));
+    } else {
+      if (!int8) GPX_CHECK(launch_utv(c->S, ld, c->Npad, c->P, c->dY, c->dT, st));
+      GPX_CHECK(launch_uv(c->S, ld, c->Npad, c->P, T, KSPLIT, c->dUvPart, c->dAlpha, st));
+      c->eval_launches += int8 ? 2 : 3;
+    }
     rec.end(h);
-    c->eval_launches += int8 ? 2 : 3;
   }
   auto mpart = [&](int q) {
     size_t off = 0;
@@ -877,7 +915,7 @@ static int exact_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, double 
   *lml = c->h_res[0];
   // the kernel's gradient block and d/d noise: [lml, block, noise, ..] from finalize_kernel, [lml, .., noise, block] from
   // finalize_multi_kernel
-  const bool single = as_single(c->mk, c->D, nullptr);
+  const bool single = single_route(c, nullptr);
   const int n = kern_ngrad(c->mk);
   for (int q = 0; q < n; q++) grad[q] = c->h_res[(single ? 1 : 4) + q];
   grad[n] = c->h_res[single ? 1 + n : 3];
@@ -914,6 +952,7 @@ int gpx_exact_eval_het(gpx_ctx* c, int kind, int ard, double variance, const dou
                        const double* noise_variances, double jitter, int max_tries, double* lml, double* grad,
                        double* dnoise, double* jitter_used) {
   if (!c || !noise_variances) GPX_FAIL("null argument");
+  if (c->P > MAX_P) GPX_FAIL("the heteroscedastic evaluation serves at most 8 output columns");
   double mean = 0.0;
   for (int64_t i = 0; i < c->N; i++) {
     if (!(noise_variances[i] >= 0)) GPX_FAIL("noise variances must be non-negative");
@@ -961,10 +1000,13 @@ int gpx_get(gpx_ctx* c, int which, double* out) {
   cudaStream_t st = c->st;
   const long N = c->N, ld = c->Npad;
   if (which == GPX_GET_ALPHA) {
-    GPX_CHECK(launch_untranspose(c->dAlpha, N, c->P, ld, c->dUvPart, st));
+    double* tmp = c->dUvPart;   // the wide route has no dUvPart: a temporary of N P doubles
+    if (c->P > MAX_P) GPX_TMP_ALLOC(&tmp, (size_t)N * c->P * 8, st);
+    GPX_CHECK(launch_untranspose(c->dAlpha, N, c->P, ld, tmp, st));
     c->total_launches++;
-    GPX_CUDA(cudaMemcpyAsync(out, c->dUvPart, (size_t)N * c->P * 8, cudaMemcpyDeviceToHost, st));
+    GPX_CUDA(cudaMemcpyAsync(out, tmp, (size_t)N * c->P * 8, cudaMemcpyDeviceToHost, st));
     GPX_CUDA(cudaStreamSynchronize(st));
+    if (tmp != c->dUvPart) GPX_TMP_FREE(tmp, st);
     return 0;
   }
   GPX_CHECK(ensure_staging(c));
@@ -1309,10 +1351,13 @@ int gpx_predict(gpx_ctx* c, const double* Xnew, int64_t M, int full_cov, double*
     // diagonal variance: everything reduces on the device; only M (P + 1) doubles come back
     double* red = nullptr;   // [P][M] means, then [M] sums of squares
     if (rc == 0 && cudaMallocAsync((void**)&red, (size_t)(c->P + 1) * M * 8, c->st) != cudaSuccess) { gpx::set_error("gpx_predict: out of memory"); rc = -1; }
-    if (rc == 0) rc = launch_col_dot(Kx, ld, N, M, c->P, c->dAlpha, ld, red, M, st);              // mu = Kx^T alpha
+    for (int q0 = 0; rc == 0 && q0 < c->P; q0 += MAX_P) {   // mu = Kx^T alpha, MAX_P outputs per launch
+      rc = launch_col_dot(Kx, ld, N, M, std::min(MAX_P, c->P - q0), c->dAlpha + (size_t)q0 * ld, ld, red + (size_t)q0 * M, M, st);
+      c->total_launches++;
+    }
     if (rc == 0) rc = launch_col_sqnorm(Tx, ld, c->Npad, M, red + (size_t)c->P * M, st);          // sum_i tmp_i^2
     if (rc == 0 && dG > 1) rc = dist_allreduce_sum(c, red + (size_t)c->P * M, (size_t)M, st);
-    c->total_launches += 2;
+    c->total_launches++;
     std::vector<double> h((size_t)(c->P + 1) * M);
     if (rc == 0 && cudaMemcpyAsync(h.data(), red, h.size() * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) rc = -1;
     if (cudaStreamSynchronize(st) != cudaSuccess) { gpx::set_error("gpx_predict: device failure"); rc = -1; }
@@ -1384,6 +1429,7 @@ int gpx_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t M, double* 
   if (!c->have_eval) GPX_FAIL("no successful gpx_exact_eval to differentiate the prediction of");
   if (M < 1) GPX_FAIL("empty Xnew");
   if (c->dist) GPX_FAIL("predictive gradients are single-GPU");
+  if (c->P > MAX_P) GPX_FAIL("predictive gradients serve at most 8 output columns");
   const MultiKern& k = c->mk;
   GPX_CHECK(pred_grad_check(k));
   GPX_CUDA(cudaSetDevice(c->device));
@@ -1409,6 +1455,29 @@ int gpx_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t M, double* 
   if (rc == 0) rc = pred_grad(c, k, pn, train_points(c), c->dAlpha, ld, c->P, Kx, ld, c->D, dmu, dvar);
   GPX_TMP_FREE(Kx, st); GPX_TMP_FREE(Tx, st); GPX_TMP_FREE(uvp, st);
   return rc;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// the input gradient of the last exact evaluation (GPy/models/gplvm.py:47-49): kern.gradients_X(dL_dK, X, None) from the
+// stored K^-1 and alpha. The fused route did not store K^-1: the plain LAUUM stores it first, as gpx_get(KINV) does.
+// ---------------------------------------------------------------------------------------------------------------
+int gpx_exact_grad_X(gpx_ctx* c, double* dX) {
+  if (!c || !dX) GPX_FAIL("null argument");
+  if (!c->have_eval) GPX_FAIL("no successful exact evaluation to differentiate");
+  if (c->lap_post) GPX_FAIL("a Laplace / EP posterior: its dL_dK is not 1/2 (alpha alpha^T - P K^-1)");
+  if (c->het) GPX_FAIL("the input gradient of a heteroscedastic evaluation is not served");
+  if (c->dist) GPX_FAIL("the input gradient of the exact evaluation is single-GPU");
+  GPX_CHECK(pred_grad_check(c->mk));
+  GPX_CUDA(cudaSetDevice(c->device));
+  if (!c->have_kinv) {
+    GPX_CHECK(ensure_kinv(c));
+    const int64_t keep = c->eval_launches;
+    GPX_CHECK(run_lauum(c, c->Kinv, nullptr));
+    c->total_launches += c->eval_launches - keep;
+    c->eval_launches = keep;
+    c->have_kinv = true;
+  }
+  return exact_grad_X(c, dX);
 }
 
 }  // extern "C"

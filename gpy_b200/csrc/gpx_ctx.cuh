@@ -29,7 +29,11 @@ struct gpx_ctx {
   double* dY = nullptr;      // [P][Npad]
   double* dT = nullptr;      // [P][Npad]  L^-1 y
   double* dAlpha = nullptr;  // [P][Npad]
-  double* dUvPart = nullptr; // [KSPLIT][P][Npad]
+  double* dUvPart = nullptr; // [KSPLIT][P][Npad]; not allocated for P > MAX_P
+  // P > MAX_P (the wide route): dY holds Y as [Npad][Ppad] (row-major, zero padded), dT and dAlpha are [Ppad][Npad], and
+  // dTt holds T = L^-1 Y as [Npad][Ppad]; Ppad = P padded to 128
+  long Ppad = 0;
+  double* dTt = nullptr;
   // workspace
   double* S = nullptr;       // Npad x Npad column-major: lower L, upper U
   double* Pbuf = nullptr;    // Npad x NB
@@ -178,6 +182,9 @@ int grad_full_sum(gpx_ctx* c, const MultiKern& k, int D, GradFullParams gp, doub
 // to `out` on the host. RatQuad / StdPeriodic parts have no device gradients_X (rc -2).
 size_t grad_X_doubles(const gpx_ctx* c, const MultiKern& k, const GradFullParams& gp, int D);
 int grad_X(gpx_ctx* c, const MultiKern& k, const GradFullParams& gp, int D, double* part, double* out);
+// gradients_X of the last exact evaluation's kernel at its training points for its dL_dK, from the stored K^-1 (c->Kinv must
+// hold it) and alpha: out (host) N x D row-major. Two launches, counted; temporaries from the stream-ordered pool.
+int exact_grad_X(gpx_ctx* c, double* out);
 // predictive gradients (gp.py:438-474) of k at the prepared test points against `train`, for the woodbury vector alpha
 // ([P][lda], device) and V = woodbury_inv K(train, test) (V[n + m * ldv], device): dmu (n x D x P) and dvar (n x D), host,
 // row-major. pred_grad_check: -2 for a kernel without a device input gradient (RatQuad / StdPeriodic parts), before
@@ -204,6 +211,9 @@ struct TmpBuf {
   int alloc(size_t doubles);
   void release() { GPX_TMP_FREE(p, st); p = nullptr; }
 };
+// L^-1 (upper = 0: lower, as gpx_get(LINV) reads it) or U = L^-T (upper = 1) of the factor in S into out (Npad x Npad
+// column-major, zero elsewhere and in the padding). One launch, not counted.
+int extract_inverse_factor(gpx_ctx* c, int upper, double* out);
 // C = A B^T on the plain DMMA GEMM (GEMM_PANEL entry): rows x cols (whole tiles), k-depth kdepth; plain 2: lower tiles only;
 // tri 1: B lower triangular, 2: A lower triangular. One launch, counted.
 int gemm_nt(gpx_ctx* c, const double* A, long lda, const double* B, long ldb, double* C, long ldc, long rows, long cols,

@@ -89,6 +89,25 @@ int TmpBuf::alloc(size_t doubles) {
   return 0;
 }
 
+// U = L^-T of the factor in S (its upper triangle, U(i, j) = S[i + j ld] for i <= j) column-major with zeros below the
+// diagonal and in the padding
+__global__ void __launch_bounds__(256) extract_u_kernel(const double* __restrict__ S, long ld, long N, double* __restrict__ out) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ld) return;
+  for (long j = blockIdx.y; j < ld; j += gridDim.y) out[i + j * ld] = (i <= j && j < N) ? S[i + j * ld] : 0.0;
+}
+
+int extract_inverse_factor(gpx_ctx* c, int upper, double* out) {
+  const long Npad = c->Npad;
+  if (upper)
+    extract_u_kernel<<<dim3((unsigned)(Npad / 256 + 1), grid_y(Npad)), 256, 0, c->st>>>(c->S, Npad, c->N, out);
+  else
+    joint_extract_kernel<<<dim3((unsigned)(Npad / 256 + 1), grid_y(Npad)), 256, 0, c->st>>>(0, c->S, Npad, c->Ldiag, c->N,
+                                                                                             out, Npad);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int gemm_nt(gpx_ctx* c, const double* A, long lda, const double* B, long ldb, double* C, long ldc, long rows, long cols,
             long kdepth, int plain, int tri) {
   GemmParams pg = gemm_defaults();
@@ -212,6 +231,7 @@ extern "C" {
 int gpx_posterior_covariance(gpx_ctx* c, const double* X1, int64_t M1, const double* X2, int64_t M2, double* cov) {
   if (!c || !X1 || !cov) GPX_FAIL("null argument");
   GPX_CHECK(exact_args(c));
+  if (c->P > MAX_P) GPX_FAIL("the joint posterior serves at most 8 output columns");
   if (M1 < 1 || (X2 && M2 < 1)) GPX_FAIL("empty point set");
   GPX_CUDA(cudaSetDevice(c->device));
   const int sym = X2 == nullptr;
@@ -243,6 +263,7 @@ int gpx_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t M, const doubl
                           double* jitter_used) {
   if (!c) GPX_FAIL("null argument");
   GPX_CHECK(exact_args(c));
+  if (c->P > MAX_P) GPX_FAIL("the joint posterior serves at most 8 output columns");
   GPX_CHECK(joint_check(c, Xnew, M, z, nz, f, jitter_used, c->P));
   GPX_CUDA(cudaSetDevice(c->device));
   PointSet ps;

@@ -457,6 +457,32 @@ __device__ __forceinline__ double gx_part_r(const PartDev& pd, int p, const doub
   return sqrt(fmax(r2, 0.0)) * pd.inv_ls_iso;
 }
 
+// one pair (row point il, chunk column point mm) with weight dl into the row point's stacked-row sums acc
+template <int DREG>
+__device__ __forceinline__ void gx_pair(const MultiKern& mk, const double* sR, const double* sC, const double* sSr,
+                                        const double* sSc, int il, int mm, bool samept, double dl, double (&acc)[DREG]) {
+  for (int pi = 0; pi < mk.nparts; pi++) {
+    const PartDev& pd = mk.part[pi];
+    if (!is_stationary(pd.kind)) continue;
+    const double rr = gx_part_r(pd, pi, sR, sC, sSr, sSc, il, mm, samept);
+    if (rr == 0.0) continue;
+    double kk, dk;
+    k_dk_of_r_unit(pd.kind, rr, kk, dk);
+    double t = pd.variance * dk * dl / rr;
+    for (int q = 0; q < mk.nparts; q++) {          // the other factors of this part's term
+      const PartDev& o = mk.part[q];
+      if (q == pi || o.term != pd.term) continue;
+      const double v = o.kind == GPX_BIAS ? 1.0
+                       : o.kind == GPX_WHITE ? (samept ? 1.0 : 0.0)
+                       : k_of_r_unit(o.kind, gx_part_r(o, q, sR, sC, sSr, sSc, il, mm, samept));
+      t *= o.variance * v;
+    }
+#pragma unroll
+    for (int q = 0; q < DREG; q++)
+      if (q >= pd.xoff && q < pd.xoff + pd.D) acc[q] = fma(t, sR[q * TILE + il] - sC[q * 32 + mm], acc[q]);
+  }
+}
+
 template <int DREG>
 __global__ void __launch_bounds__(TILE) gradx_multi_kernel(GradXMultiParams p, long mchunk, double* __restrict__ part) {
   extern __shared__ __align__(128) unsigned char gxm_smem[];
@@ -508,26 +534,7 @@ __global__ void __launch_bounds__(TILE) gradx_multi_kernel(GradXMultiParams p, l
         const bool samept = p.same && n == gm;
         double dl = sdl[tid][mm];
         if (p.same) dl += p.dL[gm * p.ldd + n];                  // tmp + tmp^T (stationary.py:334-336)
-        for (int pi = 0; pi < mk.nparts; pi++) {
-          const PartDev& pd = mk.part[pi];
-          if (!is_stationary(pd.kind)) continue;
-          const double rr = gx_part_r(pd, pi, sR, sC, sSr, sSc, tid, mm, samept);
-          if (rr == 0.0) continue;
-          double kk, dk;
-          k_dk_of_r_unit(pd.kind, rr, kk, dk);
-          double t = pd.variance * dk * dl / rr;
-          for (int q = 0; q < mk.nparts; q++) {          // the other factors of this part's term
-            const PartDev& o = mk.part[q];
-            if (q == pi || o.term != pd.term) continue;
-            const double v = o.kind == GPX_BIAS ? 1.0
-                             : o.kind == GPX_WHITE ? (samept ? 1.0 : 0.0)
-                             : k_of_r_unit(o.kind, gx_part_r(o, q, sR, sC, sSr, sSc, tid, mm, samept));
-            t *= o.variance * v;
-          }
-#pragma unroll
-          for (int q = 0; q < DREG; q++)
-            if (q >= pd.xoff && q < pd.xoff + pd.D) acc[q] = fma(t, sR[q * TILE + tid] - sC[q * 32 + mm], acc[q]);
-        }
+        gx_pair<DREG>(mk, sR, sC, sSr, sSc, tid, mm, samept, dl, acc);
       }
     }
   }
@@ -535,6 +542,82 @@ __global__ void __launch_bounds__(TILE) gradx_multi_kernel(GradXMultiParams p, l
 #pragma unroll
     for (int q = 0; q < DREG; q++)
       if (q < mk.sumD) part[((long)blockIdx.y * p.nrows + n) * mk.sumD + q] = acc[q];
+  }
+}
+
+// gradients_X of the exact evaluation's kernel at its own training points (gpx_exact_grad_X): gradx_multi_kernel's layout
+// and rules with the symmetric weight W = dL_dK + dL_dK^T = alpha alpha^T - P K^-1 formed per 128 x 32 tile in shared
+// memory. The K^-1 tile comes from the stored lower tiles (a column tile right of the row tile is read transposed, 32
+// contiguous doubles per warp); alpha of the chunk's 32 points is staged in slabs of 32 outputs, so any P fits, and each
+// thread adds alpha[c][n] alpha[c][m] to its own row of the tile in output order.
+template <int DREG>
+__global__ void __launch_bounds__(TILE, 1) exact_gradx_kernel(ExactGradXParams p, long mchunk, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char egx_smem[];
+  const MultiKern& mk = p.mk;
+  double (*sw)[33] = reinterpret_cast<double (*)[33]>(egx_smem);    // [128][33] W tile
+  double* sA = reinterpret_cast<double*>(egx_smem) + TILE * 33;     // [32][32] alpha slab: [output][chunk point]
+  double* sR = sA + 32 * 32;                                        // [sumD][128] row points
+  double* sSr = sR + (size_t)mk.sumD * TILE;                        // [nparts][128]
+  double* sC = sSr + (size_t)mk.nparts * TILE;                      // [sumD][32] column chunk
+  double* sSc = sC + (size_t)mk.sumD * 32;                          // [nparts][32]
+  const int tid = threadIdx.x;
+  const long r0 = (long)blockIdx.x * TILE, n = r0 + tid;
+  const long m_beg = (long)blockIdx.y * mchunk;
+  const long m_end = m_beg + mchunk < p.N ? m_beg + mchunk : p.N;
+  const double negP = -(double)p.P;
+  for (int q = 0; q < mk.sumD; q++) sR[q * TILE + tid] = p.XsT[(long)q * p.ldx + n];
+  for (int q = 0; q < mk.nparts; q++) sSr[q * TILE + tid] = p.sq[(long)q * p.ldx + n];
+  double acc[DREG];
+#pragma unroll
+  for (int q = 0; q < DREG; q++) acc[q] = 0.0;
+  for (long m0 = m_beg; m0 < m_end; m0 += 32) {
+    __syncthreads();
+    if (m0 / TILE <= (long)blockIdx.x) {   // stored tile: element (n, m) at Kinv[n + m ld], row n thread-contiguous
+      for (int mm = 0; mm < 32; mm++) {
+        const long gm = m0 + mm;
+        sw[tid][mm] = (n < p.N && gm < m_end) ? negP * p.Kinv[n + gm * p.ld] : 0.0;
+      }
+    } else {                               // above the diagonal tiles: element (m, n) of the stored tile
+      for (int rr = tid >> 5; rr < TILE; rr += TILE / 32) {
+        const long gn = r0 + rr, gm = m0 + (tid & 31);
+        sw[rr][tid & 31] = (gn < p.N && gm < m_end) ? negP * p.Kinv[gm + gn * p.ld] : 0.0;
+      }
+    }
+    for (int idx = tid; idx < mk.sumD * 32; idx += TILE) {
+      const int q = idx >> 5, mm = idx & 31;
+      sC[idx] = (m0 + mm < p.N) ? p.XsT[(long)q * p.ldx + m0 + mm] : 0.0;
+    }
+    for (int idx = tid; idx < mk.nparts * 32; idx += TILE) {
+      const int q = idx >> 5, mm = idx & 31;
+      sSc[idx] = (m0 + mm < p.N) ? p.sq[(long)q * p.ldx + m0 + mm] : 0.0;
+    }
+    for (int c0 = 0; c0 < p.P; c0 += 32) {
+      __syncthreads();                     // the tile is written and the previous slab consumed
+      for (int idx = tid; idx < 32 * 32; idx += TILE) {
+        const int c = c0 + (idx >> 5), mm = idx & 31;
+        sA[idx] = (c < p.P && m0 + mm < m_end) ? p.alpha[(long)c * p.ldx + m0 + mm] : 0.0;
+      }
+      __syncthreads();
+      if (n < p.N) {
+        const int cl = p.P - c0 < 32 ? p.P - c0 : 32;
+        for (int c = 0; c < cl; c++) {
+          const double an = p.alpha[(long)(c0 + c) * p.ldx + n];
+          for (int mm = 0; mm < 32; mm++) sw[tid][mm] = fma(an, sA[c * 32 + mm], sw[tid][mm]);
+        }
+      }
+    }
+    if (n < p.N) {
+      const int mlim = (int)((m_end - m0) < 32 ? (m_end - m0) : 32);
+      for (int mm = 0; mm < mlim; mm++) {
+        const long gm = m0 + mm;
+        gx_pair<DREG>(mk, sR, sC, sSr, sSc, tid, mm, n == gm, sw[tid][mm], acc);
+      }
+    }
+  }
+  if (n < p.N) {
+#pragma unroll
+    for (int q = 0; q < DREG; q++)
+      if (q < mk.sumD) part[((long)blockIdx.y * p.N + n) * mk.sumD + q] = acc[q];
   }
 }
 
@@ -588,6 +671,36 @@ int launch_gradx_multi(const GradXMultiParams& p, int nchunk, long mchunk, doubl
   if (rc) return rc;
   gradx_multi_reduce_kernel<<<(unsigned)((p.nrows * p.Dfull + 255) / 256), 256, 0, st>>>(part, p.nrows, nchunk, p.Dfull, mk,
                                                                                          out);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <int DREG>
+static int launch_egx_t(const ExactGradXParams& p, dim3 grid, size_t smem, long mchunk, double* part, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    const int mx = (TILE * 33 + 32 * 32 + (MAX_D + MAX_PARTS) * (TILE + 32)) * 8;
+    GPX_CUDA(cudaFuncSetAttribute(exact_gradx_kernel<DREG>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx));
+    attr_set = true;
+  }
+  exact_gradx_kernel<DREG><<<grid, TILE, smem, st>>>(p, mchunk, part);
+  GPX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int launch_exact_gradx(const ExactGradXParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st) {
+  const MultiKern& mk = p.mk;
+  if (has_ext(mk)) { set_error("gradients_X: RatQuad / StdPeriodic parts have no input gradient on the device"); return -2; }
+  const size_t smem = (size_t)(TILE * 33 + 32 * 32 + (mk.sumD + mk.nparts) * (TILE + 32)) * 8;
+  const dim3 grid((unsigned)((p.N + TILE - 1) / TILE), nchunk);
+  const int D = mk.sumD;
+  int rc;
+  if (D <= 8) rc = launch_egx_t<8>(p, grid, smem, mchunk, part, st);
+  else if (D <= 16) rc = launch_egx_t<16>(p, grid, smem, mchunk, part, st);
+  else if (D <= 32) rc = launch_egx_t<32>(p, grid, smem, mchunk, part, st);
+  else rc = launch_egx_t<64>(p, grid, smem, mchunk, part, st);
+  if (rc) return rc;
+  gradx_multi_reduce_kernel<<<(unsigned)((p.N * p.Dfull + 255) / 256), 256, 0, st>>>(part, p.N, nchunk, p.Dfull, mk, out);
   GPX_CUDA(cudaGetLastError());
   return 0;
 }

@@ -103,6 +103,16 @@ struct GradXMultiParams {
   MultiKern mk;
 };
 
+// gradients_X of the exact evaluation's kernel at its N training points with dL_dK = 1/2 (alpha alpha^T - P K^-1) from the
+// stored K^-1 (GPy/models/gplvm.py:47-49): the rules of GradXMultiParams with X2 = None
+struct ExactGradXParams {
+  const double* Kinv; long ld;                                 // lower tiles of K^-1 (diagonal tiles whole), column-major
+  const double* alpha; int P;                                  // [P][ldx]
+  const double* XsT; const double* sq; long ldx; long N;       // the training points as the evaluation prepared them
+  int Dfull;
+  MultiKern mk;
+};
+
 // predictive gradients (GPy/core/gp.py:438-474) at the row points (the test points) against the column points (training
 // or inducing points), with gradx_multi_kernel's rules: channel c < P weights a pair by alpha[c * lda + n] (the mean
 // Jacobian of output c), channel P by V[m * ldv + n] with V = W K(X, X*) (the variance Jacobian's Schur term).
@@ -129,6 +139,8 @@ int launch_grad_kinv_multi(const GradKinvMultiParams& p, cudaStream_t st);
 int launch_grad_full_multi(const GradFullMultiParams& p, int row_tiles, int col_tiles, cudaStream_t st);
 // two launches: chunk partials [nchunk][nrows][sumD] into part, then their fixed-order sum into out (device, nrows x Dfull)
 int launch_gradx_multi(const GradXMultiParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st);
+// the same two launches for ExactGradXParams: partials [nchunk][N][sumD], then out (device, N x Dfull)
+int launch_exact_gradx(const ExactGradXParams& p, int nchunk, long mchunk, double* part, double* out, cudaStream_t st);
 int launch_finalize_multi(const FinalizeMultiParams& f, cudaStream_t st);
 // one reduction launch per group of channels (as many channels per group as the accumulators allow), partials
 // [P + 1][nchunk][nrows][sumD] into part, then their fixed-order sum into out (device): dmu (nrows x Dfull x P row-major),

@@ -175,6 +175,31 @@ int grad_X(gpx_ctx* c, const MultiKern& k, const GradFullParams& gp, int D, doub
   return 0;
 }
 
+int exact_grad_X(gpx_ctx* c, double* out) {
+  GradFullParams gp;   // only its extents: training points x training points
+  memset(&gp, 0, sizeof(gp));
+  gp.N = gp.M = c->N;
+  int nchunk;
+  long mchunk;
+  gradx_chunks(c, gp, &nchunk, &mchunk);
+  ExactGradXParams ep;
+  memset(&ep, 0, sizeof(ep));
+  ep.Kinv = c->Kinv; ep.ld = c->Npad;
+  ep.alpha = c->dAlpha; ep.P = c->P;
+  ep.XsT = c->dXsT; ep.sq = c->dsq; ep.ldx = c->Npad; ep.N = c->N;
+  ep.Dfull = c->D; ep.mk = c->mk;
+  const size_t npart = (size_t)nchunk * c->N * std::max(1, c->mk.sumD), nout = (size_t)c->N * c->D;
+  double* buf = nullptr;
+  GPX_TMP_ALLOC(&buf, (npart + nout) * 8, c->st);
+  int rc = launch_exact_gradx(ep, nchunk, mchunk, buf, buf + npart, c->st);
+  if (rc == 0) c->total_launches += 2;   // counted only when both launches were issued
+  if (rc == 0 && cudaMemcpyAsync(out, buf + npart, nout * 8, cudaMemcpyDeviceToHost, c->st) != cudaSuccess) rc = -1;
+  if (cudaStreamSynchronize(c->st) != cudaSuccess && rc == 0) rc = -1;
+  GPX_TMP_FREE(buf, c->st);
+  if (rc == -1) set_error("gpx_exact_grad_X: device failure");
+  return rc;
+}
+
 int pred_grad_check(const MultiKern& k) {
   for (int p = 0; p < k.nparts; p++)
     if (k.part[p].kind == GPX_RATQUAD || k.part[p].kind == GPX_STDPERIODIC)

@@ -119,6 +119,10 @@ def _make_kernel(base, kind, ffi):
                 if not dL_dK.matches(self._gpx_state_key()):
                     raise ValueError("stale gradient handle: the kernel parameters changed since the sparse evaluation")
                 return dL_dK.dZ
+            if isinstance(dL_dK, DeviceGradient) and X2 is None:   # gplvm.py:49 on the exact evaluation of this kernel on X
+                g = dL_dK.grad_X(self._gpx_state_key(), X)
+                if g is not None:
+                    return g
             k, ard, var, ls = self._gpx_theta()
             return ffi.kern_grad_X(k, ard, var, ls, np.asarray(X, dtype=np.float64), np.asarray(dL_dK, dtype=np.float64),
                                    None if X2 is None else np.asarray(X2, dtype=np.float64))
@@ -233,6 +237,12 @@ def _make_combination(base, is_prod):
             if isinstance(dL_dK, SparseDeviceGradient):
                 _check_sparse_handle(self, dL_dK)
                 return dL_dK.dZ
+            if isinstance(dL_dK, DeviceGradient) and X2 is None:   # one gpx_exact_grad_X for the whole combination
+                leaves = _flatten(self)
+                if leaves is not None and not any(hasattr(l, "_gpx_part_kind") for l, _ in leaves):
+                    g = dL_dK.grad_X(_composite_key(self), X)
+                    if g is not None:
+                        return g
             return super(B200Combination, self).gradients_X(dL_dK, X, X2)
 
     B200Combination.__name__ = B200Combination.__qualname__ = base.__name__
@@ -882,7 +892,7 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
                     i += n
                 key = _composite_key(kern)
                 post = PosteriorExact(self.engine, Yc.shape[0], Yc.shape[1], key)
-                dL_dK = DeviceGradient(self.engine, key, None, None, Yc.shape[0], part_grads=pg)
+                dL_dK = DeviceGradient(self.engine, key, None, None, Yc.shape[0], part_grads=pg, X=self._data_key._X)
                 return post, lml, {"dL_dK": dL_dK, "dL_dthetaL": grad[-1], "dL_dm": _LazyAlpha(post)}
             noise = None if het else float(nvec[0])
             Xs = np.ascontiguousarray(kern._slice_X(X)[0] if _returns_tuple(kern, X) else kern._slice_X(X),
@@ -902,7 +912,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
                 lml += Z_tilde
             post = PosteriorExact(self.engine, Yc.shape[0], Yc.shape[1], kern._gpx_state_key())
             dlen = grad[1:-1] if ard else grad[1]
-            dL_dK = DeviceGradient(self.engine, kern._gpx_state_key(), grad[0], dlen, Yc.shape[0])
+            dL_dK = DeviceGradient(self.engine, kern._gpx_state_key(), grad[0], dlen, Yc.shape[0],
+                                   X=None if het else self._data_key._X)
             return post, lml, {"dL_dK": dL_dK, "dL_dthetaL": dL_dthetaL, "dL_dm": _LazyAlpha(post)}
 
     B200ExactGaussianInference.__name__ = B200ExactGaussianInference.__qualname__ = "ExactGaussianInference"

@@ -363,7 +363,7 @@ class ExactGaussianInference(object):
             lml += Z_tilde
         N, P = Y.shape
         post = PosteriorExact(self.engine, N, P, kern._state_key())
-        dL_dK = DeviceGradient(self.engine, kern._state_key(), grad[0], grad[1:-1], N)
+        dL_dK = DeviceGradient(self.engine, kern._state_key(), grad[0], grad[1:-1], N, X=self._data_key._X)
         grad_dict = {"dL_dK": dL_dK, "dL_dthetaL": grad[-1], "dL_dm": _LazyAlpha(post)}
         return post, lml, grad_dict
 
@@ -386,7 +386,7 @@ class ExactGaussianInference(object):
         N, P = Y.shape
         key = composite_state_key(kern)
         post = PosteriorExact(self.engine, N, P, key)
-        dL_dK = DeviceGradient(self.engine, key, None, None, N, part_grads=part_grads)
+        dL_dK = DeviceGradient(self.engine, key, None, None, N, part_grads=part_grads, X=self._data_key._X)
         return post, lml, {"dL_dK": dL_dK, "dL_dthetaL": grad[-1], "dL_dm": _LazyAlpha(post)}
 
     def _generic_inference(self, kern, X, Y, noise, mean_function, K, Z_tilde, likelihood=None, Y_metadata=None):

@@ -23,7 +23,7 @@ class DeviceGradient(object):
     the kernel's parameter gradients; this handle carries them (keyed by the kernel state they were computed for)
     and only materialises the matrix (2 GiB at N=16384) if somebody treats it as an ndarray."""
 
-    def __init__(self, engine, key, dvariance, dlengthscale, N, part_grads=None):
+    def __init__(self, engine, key, dvariance, dlengthscale, N, part_grads=None, X=None):
         self._engine, self._key = engine, key
         self.dvariance, self.dlengthscale = dvariance, dlengthscale
         self.part_grads = part_grads          # composite kernels: one [variance, lengthscale..] array per flattened part
@@ -31,9 +31,25 @@ class DeviceGradient(object):
         self.ndim = 2
         self.dtype = np.dtype(np.float64)
         self._host = None
+        self._X = X                           # a private copy of the inputs the engine evaluated on (None: unknown)
+        self._serial = getattr(engine, "eval_serial", None)
+        self._dX = None
 
     def matches(self, key):
         return self._key == key
+
+    def grad_X(self, key, X):
+        """kern.gradients_X(dL_dK, X, None) from the device (gpx_exact_grad_X, fetched once per handle) when this is the
+        dL_dK of the engine's current evaluation of the kernel keyed `key` on exactly these inputs X (the kernel's columns
+        as the engine holds them); None otherwise"""
+        if self._X is None or not self.matches(key) or getattr(self._engine, "eval_serial", None) != self._serial:
+            return None
+        X = np.asarray(X)
+        if X.shape != self._X.shape or not np.array_equal(X, self._X):
+            return None
+        if self._dX is None:
+            self._dX = self._engine.exact_grad_X()
+        return self._dX
 
     def __array__(self, dtype=None, copy=None):
         if self._host is None:
@@ -158,11 +174,15 @@ class Stationary(Kern):
         self.lengthscale.gradient = np.atleast_1d(dl)
 
     def gradients_X(self, dL_dK, X, X2=None):
-        """stationary.py:245-252 -> gpx_kern_grad_X (needed by inducing-point / latent-variable models)."""
+        """stationary.py:245-252 -> gpx_kern_grad_X (needed by inducing-point / latent-variable models). The DeviceGradient of
+        this kernel's exact evaluation on X is reduced on the device from what the evaluation stored (gpx_exact_grad_X):
+        dL_dK is never formed on the host."""
         Xs = self._slice_X(X)
         X2s = None if X2 is None else self._slice_X(X2)
-        kind, ard, var, ls = self._theta()
-        g = _ffi.kern_grad_X(kind, ard, var, ls, Xs, np.asarray(dL_dK, dtype=np.float64), X2s)
+        g = device_grad_X(self, dL_dK, Xs, X2, self._state_key())
+        if g is None:
+            kind, ard, var, ls = self._theta()
+            g = _ffi.kern_grad_X(kind, ard, var, ls, Xs, np.asarray(dL_dK, dtype=np.float64), X2s)
         if Xs.shape[1] == np.asarray(X).shape[1]:
             return g
         full = np.zeros(np.asarray(X).shape)       # kernel_slice_operations.py:138-150: scatter into the full X
@@ -420,6 +440,18 @@ def composite_state_key(kern):
                   tuple(k.active_dims.tolist())) + ((k._state_key(),) if isinstance(k, _PartKern) else ()) for (k, t) in fl)
 
 
+def device_grad_X(kern, dL_dK, X, X2, key):
+    """kern.gradients_X(dL_dK, X, X2) from the device, or None: only X2 = None with the DeviceGradient of the engine's
+    current exact evaluation of kern (state key `key`) on exactly X, and only for leaves with a device input gradient
+    (RatQuad / StdPeriodic have none)"""
+    if X2 is not None or not isinstance(dL_dK, DeviceGradient):
+        return None
+    leaves = flatten_parts(kern)
+    if leaves is None or any(isinstance(k, _PartKern) for k, _ in leaves):
+        return None
+    return dL_dK.grad_X(key, X)
+
+
 def scatter_part_gradients(kern, dL_dK):
     """hand the per-part gradients of a fused composite evaluation to the leaves (what Add / Prod.update_gradients_full do
     with a dense dL_dK); -> False if the handle does not belong to this kernel state"""
@@ -488,6 +520,10 @@ class Add(CombinationKernel):
             p.update_gradients_diag(dL_dKdiag, X)
 
     def gradients_X(self, dL_dK, X, X2=None):
+        """add.py:88-100; the DeviceGradient of this kernel's exact evaluation on X: one gpx_exact_grad_X for the sum"""
+        g = device_grad_X(self, dL_dK, X, X2, composite_state_key(self))
+        if g is not None:
+            return g
         return sum(p.gradients_X(dL_dK, X, X2) for p in self.parts)
 
     def gradients_X_diag(self, dL_dKdiag, X):
@@ -535,6 +571,10 @@ class Prod(CombinationKernel):
             p.update_gradients_full(dL_dK * other if other is not None else dL_dK, X, X2)
 
     def gradients_X(self, dL_dK, X, X2=None):
+        """prod.py:397-407; the DeviceGradient of this kernel's exact evaluation on X: one gpx_exact_grad_X"""
+        g = device_grad_X(self, dL_dK, X, X2, composite_state_key(self))
+        if g is not None:
+            return g
         dL_dK = np.asarray(dL_dK, dtype=np.float64)
         Ks = [p.K(X, X2) for p in self.parts]
         out = 0.0

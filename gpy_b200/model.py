@@ -134,15 +134,18 @@ class GP(Parameterized):
     def _free(self):
         return [p for p in self.flattened_parameters() if not p.is_fixed]
 
+    # every parameter through Logexp, except an unconstrained one (transform None: GPLVM's latent_mean)
     @property
     def optimizer_array(self):
-        return np.concatenate([Logexp.finv(p.values).reshape(-1) for p in self._free()])
+        return np.concatenate([(p.values if p.transform is None else Logexp.finv(p.values)).reshape(-1)
+                               for p in self._free()])
 
     @optimizer_array.setter
     def optimizer_array(self, x):
         i = 0
         for p in self._free():
-            p.values[...] = Logexp.f(x[i:i + p.size]).reshape(p.values.shape)
+            v = x[i:i + p.size]
+            p.values[...] = (v if p.transform is None else Logexp.f(v)).reshape(p.values.shape)
             i += p.size
         self.parameters_changed()
 
@@ -157,7 +160,8 @@ class GP(Parameterized):
     def _grads_transformed(self):
         g = []
         for p in self._free():
-            g.append(np.asarray(p.gradient, dtype=np.float64).reshape(-1) * Logexp.gradfactor(p.values).reshape(-1))
+            gp = np.asarray(p.gradient, dtype=np.float64).reshape(-1)
+            g.append(gp if p.transform is None else gp * Logexp.gradfactor(p.values).reshape(-1))
         return -np.concatenate(g)
 
     def _objective_and_grad(self, x):

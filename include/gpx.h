@@ -41,6 +41,19 @@ enum { GPX_RBF = 0, GPX_EXPONENTIAL = 1, GPX_MATERN32 = 2, GPX_MATERN52 = 3,
        GPX_RATQUAD = 6,              /* RatQuad (stationary.py:747-802), composite parts and gpx_kern_part_* only */
        GPX_STDPERIODIC = 7 };        /* StdPeriodic (standard_periodic.py:56-94,125-139,501-548), likewise */
 
+/* Output columns P of gpx_set_data: 1 .. GPX_MAX_OUTPUTS. Up to 8 every route below is open. Above 8 (the wide route) the
+ * exact evaluation always stores K^-1 and runs on the fp64 DMMA path whatever option "ozaki" says; its solves are two
+ * GEMMs, T = L^-1 Y (lower-triangular operand, N^2 Ppad flops) and alpha = U T (U = L^-T extracted with zeros below the
+ * diagonal, 2 N^2 Ppad flops, Ppad = P padded to 128), the quadratic term of the LML is ||T||_F^2, and every part's gradient
+ * (a single kernel's too) is reduced by the composite pass; gradients and LML come back in the layout of the entry called.
+ * It keeps 32 Npad Ppad bytes of Y, T (twice) and alpha beside the N x N workspace; an allocation that does not fit returns
+ * -1 with a message. For P > 8:
+ *   served : gpx_exact_eval, gpx_exact_eval_multi, gpx_get (every selector), gpx_predict, gpx_exact_grad_X;
+ *   -2     : gpx_exact_eval_het, gpx_predictive_gradients, gpx_posterior_covariance, gpx_posterior_samples, the Laplace and
+ *            EP entries (P = 1 only), a context with a communicator attached (gpx_set_data);
+ *   sparse : gpx_sparse_set_data keeps its limit of 8. */
+enum { GPX_MAX_OUTPUTS = 1024 };
+
 /* gpx_get selectors */
 enum {
   GPX_GET_L = 0,     /* woodbury_chol: lower Cholesky factor of K + (noise+jitter) I, N x N col-major, zeros above diag
@@ -159,6 +172,24 @@ int gpx_predict(gpx_ctx* ctx, const double* Xnew, int64_t M, int full_cov, doubl
  * (single-GPU). Nothing that gpx_get, gpx_sparse_get, gpx_predict or gpx_get_stats return changes. */
 int gpx_predictive_gradients(gpx_ctx* ctx, const double* Xnew, int64_t M, double* dmu, double* dvar);
 int gpx_sparse_predictive_gradients(gpx_ctx* ctx, const double* Xnew, int64_t M, double* dmu, double* dvar);
+
+/* The input gradient of the last exact evaluation, what GPy's GPLVM adds to an evaluation (GPy/models/gplvm.py:47-49:
+ * X.gradient = kern.gradients_X(dL_dK, X, None)). After gpx_exact_eval or gpx_exact_eval_multi, dX (N x D row-major, the D
+ * of gpx_set_data) receives
+ *   dX[n, d] = sum_m W[n, m] dk(x_n, x_m)/dx_n,d,   W = dL_dK + dL_dK^T = alpha alpha^T - P Ky^-1,
+ * Stationary.gradients_X with X2 = None (stationary.py:245-252,325-345) summed over the parts as Add.gradients_X does
+ * (add.py:88-100); a product's factor sees the other factors (prod.py:397-407); White and Bias enter only as factors; each
+ * part's sums land on the data columns of its active dims. The kernel is that of the evaluation (a single kernel runs as
+ * its one-part description through the same kernel). W is formed per 128 x 32 tile from the stored K^-1 and alpha, so
+ * nothing of size N^2 is written: N^2 pairs x (P + per-part work) FMAs plus 8 N^2 bytes of K^-1 read.
+ * Launches: 2, plus 1 when the evaluation took the fused single-kernel route (a single kernel with more than 8 tiles of
+ * 128 points on the DMMA path), which does not store K^-1: the plain LAUUM stores it first, exactly as gpx_get(KINV) does,
+ * and later calls reuse it. Returns -2 with nothing touched when there is no evaluation, the last one is a Laplace or EP
+ * posterior (gpx_laplace_finish, gpx_ep_finish: their dL_dK is another), it is heteroscedastic (gpx_exact_eval_het), a
+ * communicator is attached (single-GPU), the kernel has a RatQuad or StdPeriodic part (no device input gradient) or dX is
+ * null. Nothing that gpx_get, gpx_predict or gpx_get_stats return changes. Temporaries: 8 N (nchunk sumD + D) bytes from
+ * the stream-ordered pool (nchunk: the column chunks of gpx_kern_grad_X, sumD: the parts' stacked active dims). */
+int gpx_exact_grad_X(gpx_ctx* ctx, double* dX);
 
 /* The joint posterior of the last evaluation on the device (single-GPU; a context with a communicator attached gets -2).
  *
