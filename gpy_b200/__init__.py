@@ -17,5 +17,6 @@ from .laplace import Bernoulli, Laplace, PosteriorLaplace, StudentT  # noqa: F40
 from .ep import EP, EPDTC, GPClassification, PosteriorEP, SparseGPClassification  # noqa: F401
 from .svgp import SVGP, SVGPInference  # noqa: F401
 from .gplvm import GPLVM  # noqa: F401
+from .vargauss import GPVariationalGaussianApproximation, VarGauss  # noqa: F401
 
 __version__ = "0.1.0"

@@ -117,6 +117,9 @@ EXPORTS = {
     "gpx_ep_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_double, ctypes.c_double, ctypes.c_int,
                                     ctypes.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     "gpx_ep_finish": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp, _dp, _dp]),
+    "gpx_vargauss_begin": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, _dp, ctypes.c_int, _dp,
+                                          _dp, _dp, _dp]),
+    "gpx_vargauss_finish": (ctypes.c_int, [_vp, _dp, _dp, _dp, _dp, _dp]),
     "gpx_epdtc_begin": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64]),
     "gpx_epdtc_start": (ctypes.c_int, [_vp, _dp, _dp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _dp, _dp, _dp]),
     "gpx_epdtc_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_double, ctypes.c_double,
@@ -567,6 +570,35 @@ class Engine(object):
         self.eval_serial += 1
         check(rc, "gpx_ep_finish")
         return logdet.value, vsv.value, diag, kgrad, jit.value
+
+    # ---- variational Gaussian approximation (var_gauss.py:34-69) -----------------------------------------------------
+    def vargauss_begin(self, parts, alpha, beta, max_tries=5):
+        """K of the kernel described by parts (as laplace_begin takes them) kept on the device, m = K alpha and the
+        factor of A = I + B K B, B = diag(beta) -> (m (N,), var = diag(Sigma) (N,), KL, jitter). A beta entry that is zero
+        or not finite raises GpxArgumentError; an A that stays not positive definite numpy.linalg.LinAlgError"""
+        a, b = self._vec(alpha, "alpha"), self._vec(beta, "beta")
+        arr = (GpxKernPart * len(parts))()
+        keep, ngrad = [], 0
+        for i, desc in enumerate(parts):
+            ngrad += _fill_part(arr[i], desc, keep, i)
+        m, var = np.empty(self.N), np.empty(self.N)
+        kl, jit = ctypes.c_double(), ctypes.c_double()
+        rc = self._L.gpx_vargauss_begin(self._h, arr, len(parts), _ptr(a), _ptr(b), int(max_tries), _ptr(m), _ptr(var),
+                                        ctypes.byref(kl), ctypes.byref(jit))
+        self.eval_serial += 1
+        check(rc, "gpx_vargauss_begin")
+        self._lap_ngrad = ngrad
+        return m, var, kl.value, jit.value
+
+    def vargauss_finish(self, dF_dm, dF_dv):
+        """the gradients of F.sum() - KL for the likelihood's dF_dm and dF_dv at the last vargauss_begin's (m, var) ->
+        (dalpha (N,), dbeta (N,), kernel gradient block); the posterior stays for get / predict"""
+        g, dv = self._vec(dF_dm, "dF_dm"), self._vec(dF_dv, "dF_dv")
+        da, db, kgrad = np.empty(self.N), np.empty(self.N), np.zeros(getattr(self, "_lap_ngrad", 0))
+        rc = self._L.gpx_vargauss_finish(self._h, _ptr(g), _ptr(dv), _ptr(da), _ptr(db), _ptr(kgrad))
+        self.eval_serial += 1
+        check(rc, "gpx_vargauss_finish")
+        return da, db, kgrad
 
     # ---- sparse expectation propagation (EPDTC, expectation_propagation.py:436-611) -----------------------------------
     def _svec(self, v, what):

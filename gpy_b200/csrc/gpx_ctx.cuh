@@ -104,6 +104,11 @@ struct gpx_ctx {
   bool ep_full = false;        // epSig holds the whole Sigma (else only its diagonal, in the vector slot, is kept)
   int epdtc_drift = 0;         // option "epdtc_drift": gpx_epdtc_sweep returns diag(Knm A Kmn) after its last block (the
                                // downdated A) in sigma_diag instead of the recompute's diagonal
+  // ---- variational Gaussian approximation (gpx_laplace.cu, on the kept K above) ----------------------------------------
+  std::vector<double> vg_alpha, vg_beta, vg_m;   // alpha, beta and m = K alpha of the last gpx_vargauss_begin (N each)
+  bool vg_begun = false;       // lapK, alpha and beta of gpx_vargauss_begin are current (every other Laplace / EP call clears it)
+  bool vg_factored = false;    // S holds the factor of A = I + B K B of that begin (gpx_vargauss_finish scales it in place)
+  int vg_max_tries = 0;        // the ladder's max_tries of that begin, for a finish that factors A again
 };
 
 

@@ -1,6 +1,7 @@
 // gpx_laplace.cu — the Laplace approximation for non-Gaussian likelihoods on the device (GPy's Laplace,
 // GPy/inference/latent_function_inference/laplace.py:122-353), for one output column and no mean function, and expectation
-// propagation for the probit Bernoulli likelihood on the same kept K (the second half of this file).
+// propagation for the probit Bernoulli likelihood on the same kept K (the second half of this file), and the variational
+// Gaussian approximation for any likelihood on it (the last part).
 //
 // The likelihood's per-point quantities (W, its derivatives, the gradient terms of its parameters) are O(N) and come from the
 // caller; everything N^2 and N^3 runs here:
@@ -214,6 +215,7 @@ void lap_start(gpx_ctx* c) {
   c->have_eval = false;
   c->have_kinv = false;
   c->lap_post = false;
+  c->vg_begun = c->vg_factored = false;
   memset(&c->stats, 0, sizeof(c->stats));
   c->eval_launches = 0;
 }
@@ -988,6 +990,332 @@ int gpx_ep_finish(gpx_ctx* c, const double* tau_tilde, const double* v_tilde, in
   c->have_eval = true;
   c->have_kinv = true;   // c->Kinv holds Wi = U~ U~^T as it is
   c->lap_post = true;
+  return 0;
+}
+
+}  // extern "C"
+
+// ==== the variational Gaussian approximation (GPy/inference/latent_function_inference/var_gauss.py:34-69) =================
+// Opper & Archambeau's q(f) = N(m, Sigma) with m = K alpha and Sigma = (K^-1 + B^2)^-1, B = diag(beta), on the kept K of
+// gpx_laplace_begin. A = I + B K B is factored by the Laplace ladder with w = beta itself (BKB depends on the signs), so
+// that Ai = A^-1 = U U^T with U = L_A^-T and Sigma = B^-2 - B^-1 Ai B^-1 (:40). begin needs only the row norms of U for
+// diag(Sigma) and tr Ai; finish forms Ai (LAUUM), H = Ai diag(c) Ai (one DMMA GEMM, lower tiles) and one fused pass over
+// the lower tiles of Ai and H for the beta gradient and S = B (Ai - H) B + r r^T, the matrix whose -1/2 S + 1/2 g g^T is the
+// symmetric part of dL_dK.
+namespace gpx {
+
+// partial squared row norms of U (the upper and diagonal tiles of S, zeros below the diagonal inside a diagonal tile):
+// part[k * ld + i] = sum of U(i, c)^2 over the columns c < N of chunk k (KSPLIT chunks), zero for rows i >= N
+__global__ void __launch_bounds__(256) vargauss_rownorm_kernel(const double* __restrict__ S, long ld, long N,
+                                                               double* __restrict__ part) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ld) return;
+  const long chunk = (ld + gridDim.y - 1) / gridDim.y;
+  const long ce = (long)(blockIdx.y + 1) * chunk, c1 = ce < N ? ce : N;
+  const long cs = (long)blockIdx.y * chunk, ct = (i / TILE) * TILE;
+  double s = 0.0;
+  if (i < N)
+    for (long c = cs > ct ? cs : ct; c < c1; c++) s = fma(S[i + c * ld], S[i + c * ld], s);
+  part[(long)blockIdx.y * ld + i] = s;
+}
+
+// Ai_ii = the row norms summed over the chunks in order, var_i = Sigma_ii = beta_i^-2 - (Ai_ii / beta_i) / beta_i
+__global__ void __launch_bounds__(256) vargauss_var_kernel(const double* __restrict__ part, int nsplit, long ld, long N,
+                                                           const double* __restrict__ beta, double* __restrict__ aii,
+                                                           double* __restrict__ var) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ld) return;
+  double s = 0.0;
+  for (int k = 0; k < nsplit; k++) s += part[(long)k * ld + i];
+  const double b = i < N ? beta[i] : 1.0;
+  aii[i] = i < N ? s : 0.0;
+  var[i] = i < N ? 1.0 / (b * b) - (s / b) / b : 0.0;
+}
+
+// Sc = Ai diag(cv) (whole, cv_j = 0 for j >= N) and the upper tiles of Ai mirrored from its lower tiles, so that H = Sc Ai^T
+// runs on the plain DMMA GEMM. 32 x 32 blocks; an upper block reads its transpose through shared memory.
+__global__ void __launch_bounds__(256) vargauss_colscale_kernel(double* __restrict__ Ai, long ld, long N,
+                                                                const double* __restrict__ cv, double* __restrict__ Sc) {
+  __shared__ double t[32][33];
+  const long r0 = (long)blockIdx.x * 32, c0 = (long)blockIdx.y * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  if (r0 / TILE >= c0 / TILE) {
+    for (int k = ty; k < 32; k += 8) {
+      const long col = c0 + k;
+      Sc[r0 + tx + col * ld] = Ai[r0 + tx + col * ld] * (col < N ? cv[col] : 0.0);
+    }
+    return;
+  }
+  for (int k = ty; k < 32; k += 8) t[k][tx] = Ai[(c0 + tx) + (r0 + k) * ld];   // Ai(c0 + tx, r0 + k), a lower tile
+  __syncthreads();
+  for (int k = ty; k < 32; k += 8) {
+    const long col = c0 + k;
+    const double v = t[tx][k];                                                  // Ai(c0 + k, r0 + tx) = Ai(r0 + tx, col)
+    Ai[r0 + tx + col * ld] = v;
+    Sc[r0 + tx + col * ld] = v * (col < N ? cv[col] : 0.0);
+  }
+}
+
+// The fused pass of gpx_vargauss_finish, one CTA of TILE threads per lower tile (ti >= tj), thread t on row i = ti TILE + t.
+// Per element (i, j), with Sigma_ij = delta_ij beta_i^-2 - (Ai_ij / beta_i) / beta_j:
+//   F  : Sigma_ij^2 dF_dv_i for column j (and Sigma_ij^2 dF_dv_j for column i off the diagonal tiles), var_gauss.py:52;
+//   KL : (delta_ij - Ai_ij)^2 + jit Ai_ij^2 - delta_ij jit Ai_ij, whose column sums times 1 / beta_j are
+//        diag(KB^T (Ai - Ai^2)) (:57) because B K B = A - (1 + jit) I;
+//   Ai_ij is replaced by S_ij = beta_i beta_j (Ai_ij - H_ij) + r_i r_j (zero outside N x N).
+// part[(q nt + t) ld + col], q = 0 (F) / 1 (KL): the sum over the rows of tile t of column col, written by exactly one CTA
+// (t >= col's tile: its own column; t < col's tile: the mirror). Column sums are fixed-order shuffle trees.
+__global__ void __launch_bounds__(TILE) vargauss_pass_kernel(double* __restrict__ Ai, const double* __restrict__ H, long ld,
+                                                             long N, int nt, const double* __restrict__ beta,
+                                                             const double* __restrict__ dv, const double* __restrict__ r,
+                                                             double jit, double* __restrict__ part) {
+  const int ti = blockIdx.x, tj = blockIdx.y;
+  if (ti < tj) return;
+  __shared__ double sF[TILE / 32][TILE], sK[TILE / 32][TILE];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const long i = (long)ti * TILE + t;
+  const bool irow = i < N;
+  const double bi = irow ? beta[i] : 1.0, dvi = irow ? dv[i] : 0.0, ri = irow ? r[i] : 0.0;
+  double rowF = 0.0, rowK = 0.0;
+  for (int jj = 0; jj < TILE; jj++) {
+    const long j = (long)tj * TILE + jj;
+    const bool in = irow && j < N;
+    double f = 0.0, k = 0.0;
+    if (in) {
+      const double bj = beta[j];
+      const double a = Ai[i + j * ld], h = H[i + j * ld];
+      const bool d = i == j;
+      const double sig = (d ? 1.0 / (bi * bi) : 0.0) - (a / bi) / bj;
+      const double s2 = sig * sig;
+      f = s2 * dvi;
+      const double e = (d ? 1.0 : 0.0) - a;
+      k = e * e + jit * (a * a) - (d ? jit * a : 0.0);
+      Ai[i + j * ld] = (bi * bj) * (a - h) + ri * r[j];
+      rowF = fma(s2, dv[j], rowF);
+      rowK += k;
+    } else {
+      Ai[i + j * ld] = 0.0;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      f += __shfl_down_sync(0xffffffffu, f, o);
+      k += __shfl_down_sync(0xffffffffu, k, o);
+    }
+    if (lane == 0) { sF[warp][jj] = f; sK[warp][jj] = k; }
+  }
+  __syncthreads();
+  double cf = 0.0, ck = 0.0;
+  for (int w = 0; w < TILE / 32; w++) { cf += sF[w][t]; ck += sK[w][t]; }
+  const long col = (long)tj * TILE + t;
+  part[((long)ti) * ld + col] = cf;
+  part[((long)nt + ti) * ld + col] = ck;
+  if (ti > tj) {
+    part[((long)tj) * ld + i] = rowF;
+    part[((long)nt + tj) * ld + i] = rowK;
+  }
+}
+
+// dbeta_j = dF_dbeta_j - dKL_dbeta_j = -2 beta_j sum_t F(t, j) - sum_t KL(t, j) / beta_j (tile order), zero for j >= N
+__global__ void __launch_bounds__(256) vargauss_dbeta_kernel(const double* __restrict__ part, int nt, long ld, long N,
+                                                             const double* __restrict__ beta, double* __restrict__ dbeta) {
+  const long j = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= ld) return;
+  double f = 0.0, k = 0.0;
+  for (int t = 0; t < nt; t++) {
+    f += part[(long)t * ld + j];
+    k += part[((long)nt + t) * ld + j];
+  }
+  dbeta[j] = j < N ? -2.0 * f * beta[j] - k / beta[j] : 0.0;
+}
+
+}  // namespace gpx
+
+namespace {
+
+// beta from the caller: every entry finite and non-zero (B and B^-2 are formed from it)
+int vg_beta_ok(const double* beta, long N) {
+  for (long i = 0; i < N; i++)
+    if (!std::isfinite(beta[i]) || beta[i] == 0.0) GPX_FAIL("beta must be finite and non-zero");
+  return 0;
+}
+
+// A = I + B K B with the ladder (the diagonal's mean is 1 + beta_i^2 Kdiag), beta in LV_SW -> 0 or the failing minor
+int vg_factor(gpx_ctx* c, int max_tries, double* jitter_used) {
+  std::vector<double> b2(c->vg_beta.size());
+  for (size_t i = 0; i < b2.size(); i++) b2[i] = c->vg_beta[i] * c->vg_beta[i];
+  const int info = lap_factor(c, b2.data(), max_tries, jitter_used);
+  if (info) gpx::set_error("VarGauss: A = I + B K B is not positive definite, even with jitter.");
+  return info;
+}
+
+}  // namespace
+
+extern "C" {
+
+int gpx_vargauss_begin(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const double* alpha, const double* beta,
+                       int max_tries, double* m, double* var, double* kl, double* jitter_used) {
+  if (!c || !parts || !alpha || !beta || !m || !var || !kl || !jitter_used) GPX_FAIL("null argument");
+  if (!c->S) GPX_FAIL("gpx_set_data has not been called");
+  if (c->dist) GPX_FAIL("the variational Gaussian approximation is single-GPU");
+  if (c->P != 1) GPX_FAIL("the variational Gaussian approximation takes one output column (P = 1)");
+  GPX_CHECK(vg_beta_ok(beta, c->N));
+  GPX_CHECK(gpx_laplace_begin(c, parts, nparts));   // K into lapK (kbuild_ms, 2 launches)
+  const gpx_stats kst = c->stats;
+  cudaStream_t st = c->st;
+  const long ld = c->Npad, N = c->N;
+  c->vg_alpha.assign(alpha, alpha + N);
+  c->vg_beta.assign(beta, beta + N);
+  c->eval_launches = 0;
+  const int64_t l0 = c->total_launches;
+  LapTimer tm{c};
+  GPX_CHECK(tm.mark(-1));
+  GPX_CHECK(upload(c, LV_T1, alpha));
+  GPX_CHECK(upload(c, LV_SW, beta));
+  GPX_CHECK(kmv(c, lv(c, LV_T1), lv(c, LV_KV)));                                 // m = K alpha (:37)
+  GPX_CHECK(tm.mark(PH_MV));
+  double jit = 0.0;
+  const int info = vg_factor(c, max_tries, &jit);
+  *jitter_used = jit;
+  if (info) {
+    lap_end(c, tm, l0);
+    return info;
+  }
+  std::vector<double> ldp(ld / TILE);
+  GPX_CUDA(cudaMemcpyAsync(ldp.data(), c->logdet_part, ldp.size() * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CHECK(tm.mark(PH_FACTOR));
+  // diag(Ai) from the row norms of U, var = diag(Sigma) (:40-41)
+  vargauss_rownorm_kernel<<<dim3((unsigned)((ld + 255) / 256), KSPLIT), 256, 0, st>>>(c->S, ld, N, c->dUvPart);
+  vargauss_var_kernel<<<(unsigned)((ld + 255) / 256), 256, 0, st>>>(c->dUvPart, KSPLIT, ld, N, lv(c, LV_SW), lv(c, LV_DIAG),
+                                                                    lv(c, LV_U));
+  c->eval_launches += 2;
+  GPX_CUDA(cudaGetLastError());
+  GPX_CHECK(tm.mark(PH_OTHER));
+  std::vector<double> aii((size_t)N);
+  c->vg_m.resize((size_t)N);
+  GPX_CUDA(cudaMemcpyAsync(c->vg_m.data(), lv(c, LV_KV), (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(var, lv(c, LV_U), (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(aii.data(), lv(c, LV_DIAG), (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CHECK(lap_end(c, tm, l0));
+  c->stats.total_ms += kst.total_ms;
+  c->stats.launches += kst.launches;
+  // KL = 1/2 (log|A| + tr Ai - N + alpha^T m) (:55), each sum in index order
+  double logdet = 0.0, tr = 0.0, am = 0.0;
+  for (double v : ldp) logdet += v;
+  for (long i = 0; i < N; i++) { tr += aii[i]; am += c->vg_m[i] * alpha[i]; }
+  *kl = 0.5 * (logdet + tr - (double)N + am);
+  std::memcpy(m, c->vg_m.data(), (size_t)N * 8);
+  c->vg_max_tries = max_tries;
+  c->vg_begun = c->vg_factored = true;
+  return 0;
+}
+
+int gpx_vargauss_finish(gpx_ctx* c, const double* dF_dm, const double* dF_dv, double* dalpha, double* dbeta, double* kgrad) {
+  if (!c || !dF_dm || !dF_dv || !dalpha || !dbeta || !kgrad) GPX_FAIL("null argument");
+  if (c->dist) GPX_FAIL("the variational Gaussian approximation is single-GPU");
+  if (!c->vg_begun || !c->lap_begun) GPX_FAIL("gpx_vargauss_begin has not been called on this data and kernel");
+  GPX_CUDA(cudaSetDevice(c->device));
+  const bool factored = c->vg_factored;
+  lap_start(c);
+  cudaStream_t st = c->st;
+  const long ld = c->Npad, N = c->N;
+  const int nt = (int)(ld / TILE);
+  const MultiKern& mk = c->mk;
+  size_t need = 0;
+  for (int q = 0; q < mk.nparts; q++) need += (size_t)nt * nt * part_nred(mk.part[q]);
+  if (need > c->mpart_cap) {
+    if (c->mpartials) cudaFree(c->mpartials);
+    c->mpartials = nullptr;
+    c->mpart_cap = 0;
+    GPX_CUDA(cudaMalloc(&c->mpartials, need * 8));
+    c->mpart_cap = need;
+  }
+  // the O(N) terms: c = 1 + 2 dF_dv / beta^2, r = alpha - dF_dm
+  std::vector<double> cv((size_t)N), rv((size_t)N);
+  for (long i = 0; i < N; i++) {
+    const double b = c->vg_beta[i];
+    cv[i] = 1.0 + 2.0 * dF_dv[i] / (b * b);
+    rv[i] = c->vg_alpha[i] - dF_dm[i];
+  }
+  const int64_t l0 = c->total_launches;
+  LapTimer tm{c};
+  GPX_CHECK(tm.mark(-1));
+  GPX_CHECK(upload(c, LV_SW, c->vg_beta.data()));
+  GPX_CHECK(upload(c, LV_B, dF_dm));
+  GPX_CHECK(upload(c, LV_W, dF_dv));
+  GPX_CHECK(upload(c, LV_T1, cv.data()));
+  GPX_CHECK(upload(c, LV_Y, rv.data()));
+  GPX_CUDA(cudaMemcpyAsync(c->dAlpha, c->vg_alpha.data(), (size_t)N * 8, cudaMemcpyHostToDevice, st));
+  double jit = c->jitter_extra;
+  if (!factored) {   // a finish after a finish: the last one scaled the factor in place
+    const int info = vg_factor(c, c->vg_max_tries, &jit);
+    if (info) {
+      lap_end(c, tm, l0);
+      return info;
+    }
+    GPX_CHECK(tm.mark(PH_FACTOR));
+  }
+  // 1. Ai = U U^T into the lower tiles of c->Kinv
+  GPX_CHECK(lauum_store(c));
+  GPX_CHECK(tm.mark(PH_LAUUM));
+  {
+    TmpBuf Sc(st), H(st);
+    GPX_CHECK(Sc.alloc((size_t)ld * ld));
+    GPX_CHECK(H.alloc((size_t)ld * ld));
+    // 2. H = Ai diag(c) Ai: the scaled copy and the mirrored Ai, then one GEMM over the lower tiles
+    vargauss_colscale_kernel<<<dim3((unsigned)(ld / 32), (unsigned)(ld / 32)), 256, 0, st>>>(c->Kinv, ld, N, lv(c, LV_T1),
+                                                                                            Sc.p);
+    c->eval_launches++;
+    GPX_CUDA(cudaGetLastError());
+    GPX_CHECK(tm.mark(PH_OTHER));
+    GPX_CHECK(gemm_nt(c, Sc.p, ld, c->Kinv, ld, H.p, ld, ld, ld, ld, 2, 0));
+    GPX_CHECK(tm.mark(PH_GEMM));
+    // 3. the fused pass: beta-gradient partials (into Sc, free after the GEMM) and S over Ai
+    vargauss_pass_kernel<<<dim3((unsigned)nt, (unsigned)nt), TILE, 0, st>>>(c->Kinv, H.p, ld, N, nt, lv(c, LV_SW),
+                                                                            lv(c, LV_W), lv(c, LV_Y), jit, Sc.p);
+    vargauss_dbeta_kernel<<<(unsigned)((ld + 255) / 256), 256, 0, st>>>(Sc.p, nt, ld, N, lv(c, LV_SW), lv(c, LV_U));
+    c->eval_launches += 2;
+    GPX_CUDA(cudaGetLastError());
+    // 4. the kernel gradient of dL_dK's symmetric part 1/2 (g g^T - S), g = dF_dm, one reduction per part
+    size_t off = 0;
+    for (int q = 0; q < mk.nparts; q++) {
+      GPX_CUDA(cudaMemsetAsync(c->mpartials + off, 0, (size_t)nt * nt * part_nred(mk.part[q]) * 8, st));
+      GradKinvMultiParams gm;
+      memset(&gm, 0, sizeof(gm));
+      gm.Kinv = c->Kinv; gm.ld = ld; gm.XsT = c->dXsT; gm.sq = c->dsq; gm.ldx = ld; gm.alpha = lv(c, LV_B);
+      gm.N = N; gm.P = 1; gm.nt = nt; gm.part = q; gm.want_noise = 0; gm.partials = c->mpartials + off; gm.mk = mk;
+      GPX_CHECK(launch_grad_kinv_multi(gm, st));
+      c->eval_launches++;
+      off += (size_t)nt * nt * part_nred(mk.part[q]);
+    }
+    GPX_CHECK(tm.mark(PH_OTHER));
+    // 5. K dF_dm; 6. the posterior: U~ = diag(beta) U_A in place (Li = U~^T into H, free now), woodbury_vector = alpha
+    GPX_CHECK(kmv(c, lv(c, LV_B), lv(c, LV_KV)));
+    laplace_scale_u_kernel<<<dim3((unsigned)(ld / 32), (unsigned)(ld / 32)), 256, 0, st>>>(c->S, ld, lv(c, LV_SW), N, H.p);
+    c->eval_launches++;
+    GPX_CUDA(cudaGetLastError());
+    GPX_CHECK(tm.mark(PH_MV));
+  }
+  std::vector<double> hp(need), kg((size_t)N);
+  GPX_CUDA(cudaMemcpyAsync(hp.data(), c->mpartials, need * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(kg.data(), lv(c, LV_KV), (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CUDA(cudaMemcpyAsync(dbeta, lv(c, LV_U), (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+  GPX_CHECK(lap_end(c, tm, l0));
+  for (long i = 0; i < N; i++) dalpha[i] = kg[i] - c->vg_m[i];                  // dF_da - dKL_da (:43,:56)
+  size_t off = 0;
+  int g = 0;
+  for (int p = 0; p < mk.nparts; p++) {   // tile order, as grad_full_sum
+    const int nred = part_nred(mk.part[p]);
+    std::vector<double> tot(nred, 0.0);
+    for (size_t k = 0; k < (size_t)nt * nt; k++)
+      for (int q = 0; q < nred; q++) tot[q] += hp[off + k * nred + q];
+    double v;
+    for (int q = 0; q < nred; q++)
+      if (part_grad_entry(mk, p, q, tot[q], &v)) kgrad[g + q] = v;
+    g += part_ngrad(mk.part[p]);
+    off += (size_t)nt * nt * nred;
+  }
+  c->have_eval = true;
+  c->have_kinv = false;   // the stored matrix is S: gpx_get(KINV) forms U~ U~^T = B Ai B again
+  c->lap_post = true;
+  c->vg_begun = true;     // K, alpha and beta stay; the factor is scaled, so the next finish factors A again
   return 0;
 }
 

@@ -818,11 +818,71 @@ def _make_svgp(base, kernel_types, ffi):
     return B200SVGP
 
 
+def _make_vargauss(base, kernel_types, ffi):
+    from .vargauss import VarGauss as _DeviceVarGauss
+
+    class B200VarGauss(base):
+        """GPy.inference.latent_function_inference.VarGauss with the N^2 / N^3 work on the device (gpx_vargauss_*), for a
+        plugin stationary kernel or a B.Add / B.Prod over plugin leaves and GPy's own White / Bias, any GPy likelihood
+        with variational_expectations, ndarray X, one output column, no mean function and a finite, non-zero beta;
+        anything else goes to the stock method (var_gauss.py:34-69), which raises what the reference raises. Under GPy's
+        own model: m.inference_method = B.VarGauss(m.alpha, m.beta). dL_dK is a handle of the gradient the device
+        already reduced; it is the derivative of the bound, where the stock method's dF_dK scales the wrong side
+        (var_gauss.py:66) unless dF_dv is constant."""
+
+        def __init__(self, alpha, beta, device=0, engine=None):
+            super(B200VarGauss, self).__init__(alpha, beta)
+            self.device, self._engine = device, engine
+            self._dev = None
+
+        @property
+        def engine(self):
+            if self._engine is None:
+                self._engine = ffi.Engine(self.device)
+            return self._engine
+
+        def invalidate_data(self):
+            if self._dev is not None:
+                self._dev.invalidate_data()
+
+        def __getstate__(self):
+            d = dict(self.__dict__)
+            d["_engine"], d["_dev"] = None, None
+            return d
+
+        def inference(self, kern, X, likelihood, Y, mean_function=None, Y_metadata=None, Z=None):
+            leaves = None
+            if not isinstance(kern, kernel_types):
+                leaves = _flatten(kern) if hasattr(kern, "_gpx_is_prod") or hasattr(kern, "_gpx_part_kind") else None
+            b = np.asarray(self.beta, dtype=np.float64)
+            if ((leaves is None and not isinstance(kern, kernel_types)) or not isinstance(X, np.ndarray)
+                    or mean_function is not None or np.ndim(Y) != 2 or np.shape(Y)[1] != 1
+                    or not np.all(np.isfinite(b)) or np.any(b == 0)):
+                return super(B200VarGauss, self).inference(kern, X, likelihood, Y, mean_function, Y_metadata, Z)
+            if self._dev is None:
+                self._dev = _DeviceVarGauss(self.alpha, self.beta, engine=self.engine)
+            dev = self._dev
+            dev.alpha, dev.beta = self.alpha, self.beta
+            if leaves is not None:
+                parts = [_leaf_descriptor(l, t) for (l, t) in leaves]
+                Xs, key, ngrads, single = X, _composite_key(kern), [_leaf_ngrad(l) for l, _ in leaves], False
+            else:
+                Xs = kern._slice_X(X)[0] if _returns_tuple(kern, X) else kern._slice_X(X)
+                k, ard, var, ls = kern._gpx_theta()
+                parts = [(k, ard, 0, list(range(np.shape(Xs)[1])), var, ls)]
+                key, ngrads, single = kern._gpx_state_key(), [1 + np.size(ls)], True
+            return dev.device_inference(Xs, Y, likelihood, Y_metadata, parts, key, ngrads, single)
+
+    B200VarGauss.__name__ = B200VarGauss.__qualname__ = "VarGauss"
+    return B200VarGauss
+
+
 def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi, Add=None, Prod=None, VarDTC=None,
-         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None, EP=None, EPDTC=None, SVGP=None):
+         RatQuad=None, StdPeriodic=None, FITC=None, Laplace=None, EP=None, EPDTC=None, SVGP=None,
+         VarGauss=None):
     """Build the plugin classes on top of the given GPy base classes (Add / Prod optional: composite kernels; VarDTC /
     FITC optional: the sparse model; Laplace / EP / EPDTC optional: non-Gaussian likelihoods; SVGP optional: the
-    stochastic variational sparse GP; RatQuad / StdPeriodic optional: leaves
+    stochastic variational sparse GP; VarGauss optional: the variational Gaussian approximation; RatQuad / StdPeriodic optional: leaves
     the composite evaluation knows, alone or inside Add / Prod)."""
     kernels = {n: _make_kernel(b, _KINDS[n], ffi) for n, b in
                (("RBF", RBF), ("Exponential", Exponential), ("Matern32", Matern32), ("Matern52", Matern52))}
@@ -930,6 +990,8 @@ def make(RBF, Exponential, Matern32, Matern52, ExactGaussianInference, ffi=_ffi,
         extra["EPDTC"] = _make_epdtc(EPDTC, kernel_types, ffi)
     if SVGP is not None:
         extra["SVGP"] = _make_svgp(SVGP, kernel_types, ffi)
+    if VarGauss is not None:
+        extra["VarGauss"] = _make_vargauss(VarGauss, kernel_types, ffi)
     return types.SimpleNamespace(ExactGaussianInference=B200ExactGaussianInference, **kernels, **extra)
 
 
@@ -942,9 +1004,9 @@ def _returns_tuple(kern, X):
 def load():
     """Plugin classes over an installed GPy."""
     import GPy
-    from GPy.inference.latent_function_inference import EP, FITC, ExactGaussianInference, Laplace, VarDTC
+    from GPy.inference.latent_function_inference import EP, FITC, ExactGaussianInference, Laplace, VarDTC, VarGauss
     from GPy.inference.latent_function_inference.expectation_propagation import EPDTC
     from GPy.inference.latent_function_inference.svgp import SVGP
     return make(GPy.kern.RBF, GPy.kern.Exponential, GPy.kern.Matern32, GPy.kern.Matern52, ExactGaussianInference,
                 Add=GPy.kern.Add, Prod=GPy.kern.Prod, VarDTC=VarDTC, RatQuad=GPy.kern.RatQuad, StdPeriodic=GPy.kern.StdPeriodic,
-                FITC=FITC, Laplace=Laplace, EP=EP, EPDTC=EPDTC, SVGP=SVGP)
+                FITC=FITC, Laplace=Laplace, EP=EP, EPDTC=EPDTC, SVGP=SVGP, VarGauss=VarGauss)

@@ -431,6 +431,48 @@ int gpx_ep_sweep(gpx_ctx* ctx, const int64_t* order, double eta, double delta, i
 int gpx_ep_finish(gpx_ctx* ctx, const double* tau_tilde, const double* v_tilde, int max_tries, double* logdet_B,
                   double* vSv, double* diag_dL_dK, double* kgrad, double* jitter_used);
 
+/* The variational Gaussian approximation (GPy's VarGauss, Opper & Archambeau 2009,
+ * GPy/inference/latent_function_inference/var_gauss.py:34-69) for any likelihood, one output column and no mean function:
+ * q(f) = N(m, Sigma) with m = K alpha and Sigma = (K^-1 + B^2)^-1, B = diag(beta), alpha and beta (N values each) the
+ * variational parameters; beta may be negative. The host evaluates the likelihood's variational expectations (F, dF_dm,
+ * dF_dv) at (m, var) between the two entries. The K is kept as gpx_laplace_begin keeps it (the same buffer and release
+ * rules). With A = I + B K B factored by jitchol's ladder (the mean of its diagonal is 1 + beta_i^2 Kdiag; jitter_used
+ * reports the j it added) and Ai = (A + j I)^-1 = U U^T, U = L_A^-T:
+ *
+ * gpx_vargauss_begin : K of the parts (every kernel gpx_laplace_begin takes), m = K alpha, A formed from K in one pass with
+ *   w = beta and factored; var_i = Sigma_ii = (1 - Ai_ii) / beta_i^2 with Ai_ii the squared norm of row i of U, and
+ *   kl = 1/2 (log|A| + tr Ai - N + alpha^T m) (:55). Launches: 7 + F.
+ * gpx_vargauss_finish : for dF_dm and dF_dv (N values each) of the last begin: Ai = U U^T by the plain LAUUM;
+ *   H = Ai diag(c) Ai, c_i = 1 + 2 dF_dv_i / beta_i^2, on the DMMA GEMM (lower tiles) from a column-scaled copy of Ai; one
+ *   fused pass over the lower tiles of Ai and H that sums, per column j, dF_dbeta_j = -2 beta_j sum_i Sigma_ij^2 dF_dv_i and
+ *   dKL_dbeta_j = (|e_j - Ai_:j|^2 + j (|Ai_:j|^2 - Ai_jj)) / beta_j (= diag(KB^T (Ai - Ai^2))_j, :57, since
+ *   B K B = A - (1 + j) I), and writes S = B (Ai - H) B + r r^T over Ai, r = alpha - dF_dm. Out:
+ *     dalpha = K dF_dm - m (:43,:56);
+ *     dbeta = dF_dbeta - dKL_dbeta;
+ *     kgrad, the kernel's gradient block (as gpx_laplace_finish's) for the symmetric part 1/2 (g g^T - S) of dL_dK,
+ *       g = dF_dm, reduced by the exact evaluation's per-part reduction with alpha = g and K^-1 = S. That is the derivative
+ *       of the bound. The reference's dF_dK (:66) scales the rows of tmp by dF_dv where the columns belong
+ *       (B Ai diag(dF_dv / beta^2) Ai B); the two agree when dF_dv is constant, as for the Gaussian likelihood.
+ *   It publishes the posterior: U~ = diag(beta) U in place, woodbury_vector = alpha and woodbury_inv = B Ai B =
+ *   (K + B^-2)^-1, which equal the reference's Posterior(mean = m, cov = Sigma, K) in exact arithmetic. Afterwards
+ *   gpx_get(K / ALPHA / KINV / L / LINV) return K, alpha, B Ai B, L_A and L_A^-1 B, gpx_get(DLDK) returns -2, and
+ *   gpx_predict (it does not clip the variance), gpx_predictive_gradients, gpx_posterior_covariance and
+ *   gpx_posterior_samples serve it. finish may be repeated with other dF_dm / dF_dv; as the last one scaled the factor, a
+ *   repeated finish factors A again (1 + F more launches). Launches: 8 + nparts.
+ * Launch counts exclude F, the factor-and-invert sweep of A, once per attempt of the ladder; none depends on N. Flops: the
+ * sweep, N^3 / 3 for the LAUUM and N^3 for the GEMM (N: padded to 128). Peak device memory: five Npad^2 buffers (K, the
+ * factor workspace, Ai / S, the scaled copy of Ai and H; 40 Npad^2 bytes, 43 GB at N = 32768); nothing of size N^2 crosses
+ * PCIe. gpx_get_stats afterwards: launches, tries, and per-phase times (profile option): kbuild_ms (begin's K-build),
+ * sweep_ms (A-build + sweep), update_ms (finish's GEMM), lauum_ms (finish's LAUUM), solve_ms (mat-vecs and the scaling of
+ * U), total_ms (the whole call).
+ * -2, with nothing touched: a null pointer, a communicator attached, P != 1, a beta entry that is zero or not finite
+ * (begin), a finish without a begin on the current data and kernel (any other Laplace or EP call in between counts as
+ * another kernel). A value > 0 is A's failing minor after the ladder. */
+int gpx_vargauss_begin(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* alpha, const double* beta,
+                       int max_tries, double* m, double* var, double* kl, double* jitter_used);
+int gpx_vargauss_finish(gpx_ctx* ctx, const double* dF_dm, const double* dF_dv, double* dalpha, double* dbeta,
+                        double* kgrad);
+
 /* Sparse expectation propagation (GPy's EPDTC, expectation_propagation.py:436-611) for the probit Bernoulli likelihood, after
  * gpx_sparse_set_data(X, labels) with P = 1. The sweeps run in M-space: Sigma = Knm A Kmn with A = LLT^-1 (M x M) and
  * mu = mu0 + Knm u, so nothing of size N x N is formed. The kernels are those gpx_sparse_eval_multi takes.
