@@ -16,7 +16,7 @@ from .sparse import FITC, SparseGPRegression, VarDTC  # noqa: F401
 from .laplace import Bernoulli, Laplace, PosteriorLaplace, StudentT  # noqa: F401
 from .ep import EP, EPDTC, GPClassification, PosteriorEP, SparseGPClassification  # noqa: F401
 from .svgp import SVGP, SVGPInference  # noqa: F401
-from .gplvm import GPLVM  # noqa: F401
+from .gplvm import GPLVM, SparseGPLVM  # noqa: F401
 from .vargauss import GPVariationalGaussianApproximation, VarGauss  # noqa: F401
 
 __version__ = "0.1.0"

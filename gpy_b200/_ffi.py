@@ -81,6 +81,7 @@ EXPORTS = {
     "gpx_predict": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
     "gpx_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
     "gpx_exact_grad_X": (ctypes.c_int, [_vp, _dp]),
+    "gpx_sparse_grad_X": (ctypes.c_int, [_vp, _dp]),
     "gpx_sparse_predictive_gradients": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, _dp]),
     "gpx_posterior_covariance": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, ctypes.c_int64, _dp]),
     "gpx_posterior_samples": (ctypes.c_int, [_vp, _dp, ctypes.c_int64, _dp, ctypes.c_int64, ctypes.c_int, _dp, _dp]),
@@ -379,9 +380,15 @@ class Engine(object):
     # ---- sparse GP regression (VarDTC) building blocks ---------------------------------------------------------
     def sparse_set_data(self, X, Y):
         X, Y = _f64(X), _f64(Y)
-        self.sN, self.sD = X.shape
-        self.sP = Y.shape[1]
-        check(self._L.gpx_sparse_set_data(self._h, _ptr(X), self.sN, self.sD, _ptr(Y), self.sP), "gpx_sparse_set_data")
+        (N, D), P = X.shape, Y.shape[1]
+        check(self._L.gpx_sparse_set_data(self._h, _ptr(X), N, D, _ptr(Y), P), "gpx_sparse_set_data")
+        self.sN, self.sD, self.sP = N, D, P   # a rejected data set leaves the engine's shapes as they were
+
+    def sparse_grad_X(self):
+        """kern.gradients_X(dL_dKnm, X, Z) of the last VarDTC evaluation (sparse_gplvm.py:34) at the data it holds -> (N, D)"""
+        dX = np.empty((self.sN, self.sD))
+        check(self._L.gpx_sparse_grad_X(self._h, _ptr(dX)), "gpx_sparse_grad_X")
+        return dX
 
     def sparse_eval(self, kind, ARD, variance, lengthscale, Z, noise_variance):
         """one whole VarDTC evaluation on the device -> (lml, grad [variance, lengthscale.., noise], dZ (M x D))"""

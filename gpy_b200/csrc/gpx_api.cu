@@ -175,6 +175,7 @@ int gpx_set_option(gpx_ctx* c, const char* name, int64_t value) {
   }
   if (!strcmp(name, "profile")) { c->profile = (int)value; return 0; }
   if (!strcmp(name, "epdtc_drift")) { c->epdtc_drift = value ? 1 : 0; return 0; }
+  if (!strcmp(name, "sparse_wide")) { c->sparse_wide = value ? 1 : 0; return 0; }
   if (!strcmp(name, "ozaki")) { c->ozaki = value < 0 ? -1 : (value ? 1 : 0); return 0; }
   GPX_FAIL("unknown option");
 }

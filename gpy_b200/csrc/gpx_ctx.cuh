@@ -102,6 +102,7 @@ struct gpx_ctx {
   bool ep_ready = false;       // mu (and Sigma or its diagonal) of gpx_ep_start / gpx_ep_sweep are on the device
   bool ep_labels = false;      // the labels of the current data were checked by gpx_ep_begin (cleared with the buffers)
   bool ep_full = false;        // epSig holds the whole Sigma (else only its diagonal, in the vector slot, is kept)
+  int sparse_wide = 0;         // option "sparse_wide": gpx_sparse_set_data takes up to GPX_MAX_OUTPUTS columns, not 8
   int epdtc_drift = 0;         // option "epdtc_drift": gpx_epdtc_sweep returns diag(Knm A Kmn) after its last block (the
                                // downdated A) in sigma_diag instead of the recompute's diagonal
   // ---- variational Gaussian approximation (gpx_laplace.cu, on the kept K above) ----------------------------------------

@@ -28,12 +28,14 @@ struct SparseState {
   long Ntot = 0;                           // rows over all ranks (var_dtc.py num_data)
   long Nw = 0, Mw = 0;                     // extents of psi1 written last time (a smaller N or M must re-zero the padding)
   int D = 0, P = 0;
-  double *X = nullptr, *XsT = nullptr, *sqX = nullptr, *Y = nullptr, *Yb = nullptr;   // Y: [P][Npad]
+  long Ppad = 0;                           // P > MAX_P (the wide route): P padded to whole tiles of outputs
+  double *X = nullptr, *XsT = nullptr, *sqX = nullptr, *Y = nullptr, *Yb = nullptr;   // Y: [P][Npad] ([Ppad][Npad] wide)
+  double* YT = nullptr;                    // wide route: Y as [Npad][Ppad] (row-major, zero padded), the GEMM operand of t
   double *Z = nullptr, *ZsT = nullptr, *sqZ = nullptr;
   double *Kuf = nullptr;   // Mpad x Npad column-major: (a, n) at a + n*Mpad
-  double *Kfu = nullptr;   // Npad x Mpad column-major: (n, a) at n + a*Npad
+  double *Kfu = nullptr;   // Npad x Mpad column-major: (n, a) at n + a*Npad; wide route: Ppad more columns, beta Y
   double *dLt = nullptr;   // Mpad x Npad: dL_dKnm^T
-  double *Gm = nullptr, *W2 = nullptr, *Cm = nullptr;   // Mpad x Mpad, Mpad x Mpad, [P][Mpad]
+  double *Gm = nullptr, *W2 = nullptr, *Cm = nullptr;   // Mpad x Mpad (wide: Ppad more columns, C), Mpad x Mpad, [P][Mpad]
   double *part = nullptr; size_t part_cap = 0;
   int rows_cap = 0, norm_cap = 0;          // stacked coordinate rows of XsT / ZsT, squared-norm rows of sqX / sqZ
   MultiKern mk{};          // the kernel of the last evaluation
@@ -48,6 +50,8 @@ struct SparseState {
   double *hs = nullptr;                              // het noise: [2 + P][Npad] column reductions s1, s2, r (see eval)
   double trYYT = 0.0;
   bool have_eval = false;
+  bool dl_ready = false;                             // dLt, Yb and Cm hold the dL_dKnm^T of the last VarDTC evaluation
+                                                     // (gpx_sparse_grad_X reads them; every other writer clears it)
   bool w_ready = false;                              // mm[9] holds woodbury_inv of the current evaluation (formed by
                                                      // gpx_sparse_predictive_gradients, kept for its later calls)
   double noise = 0.0;
@@ -88,6 +92,7 @@ void free_m(SparseState* s) {
   s->sv_cap = 0;
   s->sv_begun = s->w_own = false;
   s->have_eval = false;
+  s->dl_ready = false;
   s->w_ready = false;
   s->ep_begun = s->ep_ready = false;
   s->M = s->Mpad = 0;
@@ -95,7 +100,7 @@ void free_m(SparseState* s) {
 }
 void free_all(SparseState* s) {
   free_m(s);
-  double** ptrs[] = {&s->X, &s->XsT, &s->sqX, &s->Y, &s->Yb, &s->part, &s->red, &s->hb, &s->hs, &s->ev};
+  double** ptrs[] = {&s->X, &s->XsT, &s->sqX, &s->Y, &s->Yb, &s->YT, &s->part, &s->red, &s->hb, &s->hs, &s->ev};
   for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
   if (s->eord) { cudaFree(s->eord); s->eord = nullptr; }
   if (s->h_red) { cudaFreeHost(s->h_red); s->h_red = nullptr; }
@@ -103,7 +108,7 @@ void free_all(SparseState* s) {
   if (s->cB) { gpx_destroy(s->cB); s->cB = nullptr; }
   s->part_cap = 0;
   s->rows_cap = s->norm_cap = 0;
-  s->N = s->Npad = 0;
+  s->N = s->Npad = s->Ppad = 0;
 }
 int ensure_part(SparseState* s, size_t bytes) {
   if (s->part_cap >= bytes) return 0;
@@ -182,6 +187,19 @@ __global__ void __launch_bounds__(256) trace_dot_kernel(const double* __restrict
   }
   if (threadIdx.x == 0) { r[2 * blockIdx.x] = sh[0][0]; r[2 * blockIdx.x + 1] = sh[1][0]; }
 }
+// r[b] = partial sum of a[i]^2 over the i = b, b + 256 gridDim.x, ... < n of CTA b, in a fixed order
+__global__ void __launch_bounds__(256) sumsq_kernel(const double* __restrict__ a, long n, double* __restrict__ r) {
+  __shared__ double sh[256];
+  double acc = 0.0;
+  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long)gridDim.x * 256) acc = fma(a[i], a[i], acc);
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) r[blockIdx.x] = sh[0];
+}
 // n kernels just issued for context c (on its stream or on a child context's): counted on c, a launch error surfaced
 int launched(gpx_ctx* c, int n = 1) {
   c->total_launches += n;
@@ -220,25 +238,35 @@ extern "C" {
 
 int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const double* Y, int P) {
   if (!c || !X || !Y) GPX_FAIL("null argument");
-  if (N < 1 || D < 1 || D > MAX_D || P < 1 || P > MAX_P) GPX_FAIL("bad shape (D <= 64, P <= 8)");
+  if (N < 1 || D < 1 || D > MAX_D || P < 1 || P > (c->sparse_wide ? GPX_MAX_OUTPUTS : MAX_P))
+    GPX_FAIL(c->sparse_wide ? "bad shape (D <= 64, P <= 1024)" : "bad shape (D <= 64, P <= 8; option \"sparse_wide\" takes 1024)");
+  if (P > MAX_P && c->dist) GPX_FAIL("more than 8 output columns are single-GPU");
   GPX_CUDA(cudaSetDevice(c->device));
   laplace_release(c);
   if (!c->sparse) c->sparse = new SparseState();
   SparseState* s = c->sparse;
   const long Npad = (N + TILE - 1) / TILE * TILE;
+  const bool wide = P > MAX_P;
+  const long Ppad = wide ? (P + TILE - 1) / TILE * TILE : 0;
   if (Npad != s->Npad || D != s->D || P != s->P) {
     GPX_CUDA(cudaStreamSynchronize(c->st));
     free_all(s);
-    s->Npad = Npad; s->D = D; s->P = P;
+    s->Npad = Npad; s->D = D; s->P = P; s->Ppad = Ppad;
     GPX_CUDA(cudaMalloc(&s->X, (size_t)Npad * D * 8));
     GPX_CUDA(cudaMalloc(&s->XsT, (size_t)Npad * D * 8));
     GPX_CUDA(cudaMalloc(&s->sqX, (size_t)Npad * 8));
     s->rows_cap = D; s->norm_cap = 1;
-    GPX_CUDA(cudaMalloc(&s->Y, (size_t)Npad * P * 8));
-    GPX_CUDA(cudaMalloc(&s->Yb, (size_t)Npad * P * 8));
+    if (wide) {   // no Yb: the wide route adds the rank-P term of dL_dKnm^T inside its GEMM (knm_grads_device)
+      GPX_CUDA(cudaMalloc(&s->Y, (size_t)Npad * Ppad * 8));
+      GPX_CUDA(cudaMalloc(&s->YT, (size_t)Npad * Ppad * 8));
+    } else {
+      GPX_CUDA(cudaMalloc(&s->Y, (size_t)Npad * P * 8));
+      GPX_CUDA(cudaMalloc(&s->Yb, (size_t)Npad * P * 8));
+    }
   }
   s->N = N;
   s->have_eval = false;
+  s->dl_ready = false;
   s->w_ready = false;
   s->ep_begun = s->ep_ready = s->ep_labels = false;
   s->sv_begun = s->w_own = false;
@@ -264,8 +292,14 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
     }
   }
   GPX_CUDA(cudaMemcpyAsync(s->X, X, (size_t)N * D * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CUDA(cudaMemcpyAsync(s->Yb, Y, (size_t)N * P * 8, cudaMemcpyHostToDevice, c->st));
-  GPX_CHECK(launch_transpose_pad(s->Yb, N, P, Npad, s->Y, c->st));
+  if (wide) {   // YT: rows of Ppad, zero padded; Y = its transpose, [Ppad][Npad]
+    GPX_CUDA(cudaMemsetAsync(s->YT, 0, (size_t)Npad * Ppad * 8, c->st));
+    GPX_CUDA(cudaMemcpy2DAsync(s->YT, Ppad * 8, Y, (size_t)P * 8, (size_t)P * 8, N, cudaMemcpyHostToDevice, c->st));
+    GPX_CHECK(launch_transpose_pad(s->YT, N, (int)Ppad, Npad, s->Y, c->st));
+  } else {
+    GPX_CUDA(cudaMemcpyAsync(s->Yb, Y, (size_t)N * P * 8, cudaMemcpyHostToDevice, c->st));
+    GPX_CHECK(launch_transpose_pad(s->Yb, N, P, Npad, s->Y, c->st));
+  }
   c->total_launches++;
   GPX_CUDA(cudaStreamSynchronize(c->st));
   return 0;
@@ -280,18 +314,20 @@ static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
   const MultiKern& k = s->mk;
   GPX_CHECK(ensure_rows(c, s, k));
   const long Mpad = (M + TILE - 1) / TILE * TILE, Npad = s->Npad, N = s->N;
+  s->dl_ready = false;
   if (Mpad != s->Mpad || !s->Kuf) {   // (gpx_svgp_begin sets up Z without psi1)
     GPX_CUDA(cudaStreamSynchronize(st));
     free_m(s);
     s->Mpad = Mpad;
+    const long Mk = Mpad + s->Ppad;   // k-depth of dL_dKnm^T = [W2 | C] [psi1 | beta Y]^T on the wide route
     GPX_CUDA(cudaMalloc(&s->Z, (size_t)Mpad * s->D * 8));
     GPX_CUDA(cudaMalloc(&s->ZsT, (size_t)Mpad * s->rows_cap * 8));
     GPX_CUDA(cudaMalloc(&s->sqZ, (size_t)Mpad * s->norm_cap * 8));
     GPX_CUDA(cudaMalloc(&s->Kuf, (size_t)Mpad * Npad * 8));
-    GPX_CUDA(cudaMalloc(&s->Kfu, (size_t)Mpad * Npad * 8));
+    GPX_CUDA(cudaMalloc(&s->Kfu, (size_t)Mk * Npad * 8));
     GPX_CUDA(cudaMalloc(&s->dLt, (size_t)Mpad * Npad * 8));
     GPX_CUDA(cudaMalloc(&s->Gm, (size_t)Mpad * Mpad * 8));
-    GPX_CUDA(cudaMalloc(&s->W2, (size_t)Mpad * Mpad * 8));
+    GPX_CUDA(cudaMalloc(&s->W2, (size_t)Mpad * Mk * 8));
     GPX_CUDA(cudaMalloc(&s->Cm, (size_t)Mpad * s->P * 8));
     GPX_CUDA(cudaMalloc(&s->gsum, (size_t)(MAX_D + 2 + Mpad * s->D) * 8));
     GPX_CUDA(cudaMemsetAsync(s->Gm, 0, (size_t)Mpad * Mpad * 8, st));
@@ -328,9 +364,16 @@ static int mul_psi1T(gpx_ctx* c, const double* A, double* C, int tri) {
 
 static int knm_reduce(gpx_ctx* c, double* grad, double* dZ);
 
-// dL_dKnm^T = W2 psi1^T (+ rank-P term: on the fly for a single kernel, added in one pass for a composite) reduced to
-// kernel-parameter gradients and dL/dZ; W2 (device, s->W2) and C (device, s->Cm as [P][Mpad]) must be in place. Results on
-// the host.
+// output columns of the rank-P term C (beta Y)^T that the Knm reductions add on the fly: a single kernel's up to MAX_P
+// columns; a composite's term is added to dL_dKnm^T in one pass first, and the wide route's by its GEMM
+static int rank_p_cols(const SparseState* s) {
+  return as_single(s->mk, s->D, nullptr) && s->P <= MAX_P ? s->P : 0;
+}
+
+// dL_dKnm^T = W2 psi1^T (+ rank-P term: on the fly for a single kernel, added in one pass for a composite, and for P > MAX_P
+// by the GEMM itself as [W2 | C] [psi1 | beta Y]^T) reduced to kernel-parameter gradients and dL/dZ; W2 (device, s->W2) and
+// C (device, s->Cm as [P][Mpad]; wide route: also as [Ppad][Mpad] in the columns of s->W2 after W2) must be in place.
+// Results on the host.
 // bvec (device, [Npad], per-point precisions) selects the heteroscedastic form: VVT_factor = beta_n Y_n and the columns of
 // W2 psi1^T scaled by beta_n (var_dtc.py:226); W2 is then 2 dL_dpsi2_beta without the scalar beta.
 static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double* grad, double* dZ) {
@@ -338,6 +381,14 @@ static int knm_grads_device(gpx_ctx* c, double beta, const double* bvec, double*
   cudaStream_t st = c->st;
   const long Mpad = s->Mpad, N = s->N, Npad = s->Npad;
   const int P = s->P;
+  if (P > MAX_P) {   // scalar noise only: beta Y into the columns of Kfu after psi1, k-depth Mpad + Ppad
+    const long Ppad = s->Ppad;
+    scale_kernel<<<(unsigned)((Npad * Ppad + 255) / 256), 256, 0, st>>>(s->Y, beta, Npad * Ppad, s->Kfu + (size_t)Npad * Mpad);
+    GPX_CHECK(launched(c));
+    GPX_CHECK(gemm_nt(c, s->W2, Mpad, s->Kfu, Npad, s->dLt, Mpad, Mpad, Npad, Mpad + Ppad, 1, 0));
+    GPX_CUDA(cudaGetLastError());
+    return knm_reduce(c, grad, dZ);
+  }
   if (bvec)
     ymul_kernel<<<(unsigned)((Npad * P + 255) / 256), 256, 0, st>>>(s->Y, bvec, Npad, P, s->Yb);
   else
@@ -361,11 +412,11 @@ static int knm_reduce_at(gpx_ctx* c, const Points& xp, double* dLt, const double
   // kernel-parameter gradients of sum(dL_dKnm * K(X, Z)): rows i = data points, columns j = inducing points
   const MultiKern& k = s->mk;
   const bool single = as_single(k, s->D, nullptr);
-  if (!single) {
+  if (!single && P <= MAX_P) {
     add_rank_p_kernel<<<(unsigned)((Mpad * N + 255) / 256), 256, 0, st>>>(dLt, Mpad, s->M, N, s->Cm, Yb, ldy, P);
     GPX_CHECK(launched(c));
   }
-  const int cP = single ? P : 0;
+  const int cP = rank_p_cols(s);
   GradFullParams gp = grad_params(k, s->D, xp, s->zpts(), dLt, Mpad);
   gp.ci = Yb; gp.ldci = ldy; gp.cj = s->Cm; gp.ldcj = Mpad; gp.cP = cP;
   GPX_CHECK(ensure_part(s, grad_full_doubles(k, s->D, gp) * 8));
@@ -486,6 +537,7 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
   s->have_eval = false;
+  s->dl_ready = false;
   s->w_ready = false;
   s->mk = k;
   s->kdiag = kdiag;
@@ -516,9 +568,13 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   const int D = s->D, P = s->P, mt = (int)(Mpad / TILE);
   const int ngk = kern_ngrad(s->mk);   // entries of the kernel's gradient block
   constexpr int RSPLIT = 64;
+  // P > MAX_P (scalar noise): every P-column product on the DMMA GEMM, the vectors held transposed as [Mpad][Ppad]
+  const bool wide = P > MAX_P;
+  const long Ppad = s->Ppad;
   if (!s->mm[0]) {
     for (auto& p : s->mm) GPX_CUDA(cudaMalloc(&p, (size_t)Mpad * Mpad * 8));
-    GPX_CUDA(cudaMalloc(&s->vec, (size_t)(8 + RSPLIT) * P * Mpad * 8));
+    if (wide) GPX_CUDA(cudaMalloc(&s->vec, (size_t)6 * Ppad * Mpad * 8));
+    else GPX_CUDA(cudaMalloc(&s->vec, (size_t)(8 + RSPLIT) * P * Mpad * 8));
   }
   if (!s->red) {
     GPX_CUDA(cudaMalloc(&s->red, 4096 * 8));
@@ -532,6 +588,9 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
          *LBi = s->mm[7], *DB = s->mm[8], *E = s->mm[9];
   double *tv = s->vec, *vv = tv + (size_t)P * Mpad, *Cv = vv + (size_t)P * Mpad, *wv = Cv + (size_t)P * Mpad,
          *xv = wv + (size_t)P * Mpad, *rpart = s->vec + (size_t)8 * P * Mpad;
+  // wide route: t^T, (beta t)^T, v^T, w^T, C^T ([Mpad][Ppad] each) and w ([Ppad][Mpad])
+  double *tT = s->vec, *xT = tT + (size_t)Ppad * Mpad, *vT = xT + (size_t)Ppad * Mpad, *wT = vT + (size_t)Ppad * Mpad,
+         *CT = wT + (size_t)Ppad * Mpad, *wq = CT + (size_t)Ppad * Mpad;
   // scalar noise: beta multiplies A, psi1Vf and dL_dpsi2 as a number; per-point noise: it is inside tmp, Y and the columns
   // of dL_dKnm^T already, and the same formulas run with beta = 1
   const double beta = het ? 1.0 : 1.0 / std::max(noise, 1e-8);                           // var_dtc.py:79-80
@@ -573,8 +632,13 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
     GPX_CHECK(launch_gemm(pg, dim3(1, 1), st));
     GPX_CHECK(launched(c));
   }
-  GPX_CHECK(launch_row_dot(Tuf, Mpad, Mpad, s->N, P, Yrow, Npad, RSPLIT, rpart, tv, st));   // t = tmp Y  ([P][Mpad])
-  GPX_CHECK(launched(c, 2));
+  if (wide) {
+    GPX_CHECK(gemm_nt(c, s->YT, Ppad, Tuf, Mpad, tT, Ppad, Ppad, Mpad, Npad, 1, 0));     // t^T = Y^T tmp^T
+    GPX_CUDA(cudaGetLastError());
+  } else {
+    GPX_CHECK(launch_row_dot(Tuf, Mpad, Mpad, s->N, P, Yrow, Npad, RSPLIT, rpart, tv, st));   // t = tmp Y  ([P][Mpad])
+    GPX_CHECK(launched(c, 2));
+  }
   // row shards: A_raw and t are sums over data points -> one M x M and one M x P all-reduce
   // (the pattern of var_dtc_parallel.py:113-131 with NCCL instead of mpi4py)
   GPX_CHECK(dist_allreduce_sum(c, Ar, (size_t)Mpad * Mpad, st));
@@ -589,12 +653,21 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   double logdetB = 0.0;
   GPX_CHECK(factor_child(c, s->cB, Bd, 0.0, &logdetB, UB, LBi));
   // v = LB^-1 (beta t) (:139-141) ; w = LB^-T v ; C = Lm^-T w (:142-143)   [col_dot(A, y) = A^T y]
-  scale_kernel<<<(unsigned)((Mpad * P + 255) / 256), 256, 0, st>>>(tv, beta, Mpad * P, xv);
-  GPX_CHECK(launched(c));
-  GPX_CHECK(launch_col_dot(UB, Mpad, Mpad, Mpad, P, xv, Mpad, vv, Mpad, st));           // v = UB^T x = LBi x
-  GPX_CHECK(launch_col_dot(LBi, Mpad, Mpad, Mpad, P, vv, Mpad, wv, Mpad, st));          // w = LBi^T v
-  GPX_CHECK(launch_col_dot(Lmi, Mpad, Mpad, Mpad, P, wv, Mpad, Cv, Mpad, st));          // C = Lmi^T w
-  GPX_CHECK(launched(c, 3));
+  if (wide) {   // transposed: v^T = x^T LBi^T, w^T = v^T LBi, C^T = w^T Lmi; GEMM operand B(j, k) = LBi(j, k), UB(j, k), Um(j, k)
+    scale_kernel<<<(unsigned)((Mpad * Ppad + 255) / 256), 256, 0, st>>>(tT, beta, Mpad * Ppad, xT);
+    GPX_CHECK(launched(c));
+    GPX_CHECK(gemm_nt(c, xT, Ppad, LBi, Mpad, vT, Ppad, Ppad, Mpad, Mpad, 1, 1));
+    GPX_CHECK(gemm_nt(c, vT, Ppad, UB, Mpad, wT, Ppad, Ppad, Mpad, Mpad, 1, 0));
+    GPX_CHECK(gemm_nt(c, wT, Ppad, Um, Mpad, CT, Ppad, Ppad, Mpad, Mpad, 1, 0));
+    GPX_CUDA(cudaGetLastError());
+  } else {
+    scale_kernel<<<(unsigned)((Mpad * P + 255) / 256), 256, 0, st>>>(tv, beta, Mpad * P, xv);
+    GPX_CHECK(launched(c));
+    GPX_CHECK(launch_col_dot(UB, Mpad, Mpad, Mpad, P, xv, Mpad, vv, Mpad, st));           // v = UB^T x = LBi x
+    GPX_CHECK(launch_col_dot(LBi, Mpad, Mpad, Mpad, P, vv, Mpad, wv, Mpad, st));          // w = LBi^T v
+    GPX_CHECK(launch_col_dot(Lmi, Mpad, Mpad, Mpad, P, wv, Mpad, Cv, Mpad, st));          // C = Lmi^T w
+    GPX_CHECK(launched(c, 3));
+  }
   std::vector<double> hstat, hY;
   if (het) {
     // _compute_dL_dR, het_noise (var_dtc.py:241-257): per data point
@@ -614,14 +687,29 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   }
   // DBi = P B^-1 + w w^T
   GPX_CHECK(binv(c, UB, DB));
-  GPX_CHECK(combine(c, DB, Mpad, (double)P, DB, 0.0, nullptr, 0.0, 1.0, wv, P));
+  if (wide) {   // w w^T with k-depth Ppad: lower tiles, mirrored (T is free), then added
+    GPX_CHECK(launch_transpose_pad(wT, Mpad, (int)Ppad, Mpad, wq, st));
+    GPX_CHECK(launched(c));
+    GPX_CHECK(gemm_nt(c, wq, Mpad, wq, Mpad, T, Mpad, Mpad, Mpad, Ppad, 2, 0));
+    mirror_tiles_kernel<<<dim3((unsigned)((Mpad + 255) / 256), (unsigned)Mpad), 256, 0, st>>>(T, Mpad, Mpad);
+    GPX_CHECK(launched(c));
+    GPX_CHECK(combine(c, DB, Mpad, (double)P, DB, 1.0, T, 0.0));
+  } else {
+    GPX_CHECK(combine(c, DB, Mpad, (double)P, DB, 0.0, nullptr, 0.0, 1.0, wv, P));
+  }
   // scalars: trace(A_raw), sum(A_raw .* DBi), |v|^2
   const int RB = 64;
   trace_dot_kernel<<<RB, 256, 0, st>>>(Ar, DB, Mpad, M, s->red);
   GPX_CHECK(launched(c));
   GPX_CUDA(cudaMemcpyAsync(s->h_red, s->red, 2 * RB * 8, cudaMemcpyDeviceToHost, st));
-  std::vector<double> hv((size_t)P * Mpad);
-  GPX_CUDA(cudaMemcpyAsync(hv.data(), vv, hv.size() * 8, cudaMemcpyDeviceToHost, st));
+  std::vector<double> hv(wide ? (size_t)RB : (size_t)P * Mpad);
+  if (wide) {   // |v|^2 over v^T, whose padding is zero: RB partial sums
+    sumsq_kernel<<<RB, 256, 0, st>>>(vT, Mpad * Ppad, s->red + 2 * RB);
+    GPX_CHECK(launched(c));
+    GPX_CUDA(cudaMemcpyAsync(hv.data(), s->red + 2 * RB, RB * 8, cudaMemcpyDeviceToHost, st));
+  } else {
+    GPX_CUDA(cudaMemcpyAsync(hv.data(), vv, hv.size() * 8, cudaMemcpyDeviceToHost, st));
+  }
   // dL_dKmm = Um (-0.5 DBi - 0.5 P B + P I) Um^T   (var_dtc.py:152-156)
   GPX_CHECK(combine(c, E, Mpad, -0.5, DB, -0.5 * P, Bd, (double)P));
   GPX_CHECK(sandwich(c, Um, E, T, Kd));                                                   // Kd now holds dL_dKmm
@@ -629,8 +717,15 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   GPX_CHECK(combine(c, E, Mpad, -1.0, DB, 0.0, nullptr, (double)P));
   GPX_CHECK(sandwich(c, Um, E, T, E));
   GPX_CHECK(combine(c, s->W2, Mpad, beta, E, 0.0, nullptr, 0.0));
-  // Knm part: needs C in s->Cm
-  GPX_CUDA(cudaMemcpyAsync(s->Cm, Cv, (size_t)P * Mpad * 8, cudaMemcpyDeviceToDevice, st));
+  // Knm part: needs C in s->Cm (wide route: and as [Ppad][Mpad] in the columns of W2 after W2)
+  if (wide) {
+    double* Cext = s->W2 + (size_t)Mpad * Mpad;
+    GPX_CHECK(launch_transpose_pad(CT, Mpad, (int)Ppad, Mpad, Cext, st));
+    GPX_CHECK(launched(c));
+    GPX_CUDA(cudaMemcpyAsync(s->Cm, Cext, (size_t)P * Mpad * 8, cudaMemcpyDeviceToDevice, st));
+  } else {
+    GPX_CUDA(cudaMemcpyAsync(s->Cm, Cv, (size_t)P * Mpad * 8, cudaMemcpyDeviceToDevice, st));
+  }
   std::vector<double> g_knm(ngk, 0.0);
   GPX_CHECK(knm_grads_device(c, beta, bvec, g_knm.data(), dZ));                         // dZ <- Knm part
   {
@@ -659,8 +754,11 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   // ---- scalars on the host (var_dtc.py:237-276, homoscedastic) -----------------------------------------------------
   double trAr = 0.0, sumAD = 0.0, data_fit = 0.0;
   for (int b = 0; b < RB; b++) { trAr += s->h_red[2 * b]; sumAD += s->h_red[2 * b + 1]; }
-  for (int q = 0; q < P; q++)
-    for (long i = 0; i < M; i++) data_fit += hv[(size_t)q * Mpad + i] * hv[(size_t)q * Mpad + i];
+  if (wide)
+    for (int b = 0; b < RB; b++) data_fit += hv[b];
+  else
+    for (int q = 0; q < P; q++)
+      for (long i = 0; i < M; i++) data_fit += hv[(size_t)q * Mpad + i] * hv[(size_t)q * Mpad + i];
   const double trA = beta * trAr, sumADB = beta * sumAD;
   const double variance = s->kdiag;                                                           // psi0 per point
   const double psi0_sum = variance * (double)N;
@@ -701,6 +799,7 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
     *lml = lik_1h + lik_2h + lik_3 + lik_4;
     kern_grads(s, -0.5 * od * sums[1], g_knm, g_kmm, grad);                                 // update_gradients_diag (:110)
     s->have_eval = true;
+    s->dl_ready = !precision;
     return 0;
   }
   const double lik_1 = -0.5 * nd * od * (log2pi - log(beta)) - 0.5 * beta * s->trYYT;
@@ -715,6 +814,7 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   kern_grads(s, dvar_diag, g_knm, g_kmm, grad);
   grad[ngk] = dL_dR;
   s->have_eval = true;
+  s->dl_ready = !precision;
   return 0;
 }
 
@@ -732,6 +832,7 @@ int gpx_sparse_eval_het(gpx_ctx* c, int kind, int ard, double variance, const do
                         int64_t M, const double* noise_variances, double* lml, double* grad, double* dZ, double* dL_dR) {
   if (!noise_variances) GPX_FAIL("null argument");
   GPX_CHECK(sparse_args(c, lengthscale, Z, M, lml, grad, dZ, true, dL_dR));
+  if (c->sparse->P > MAX_P) GPX_FAIL("the heteroscedastic sparse evaluation serves at most 8 output columns");
   MultiKern mk;
   GPX_CHECK(fill_single(mk, kind, ard, c->sparse->D, variance, lengthscale));
   return sparse_eval_impl(c, mk, variance, Z, M, 0.0, noise_variances, lml, grad, dZ, dL_dR);
@@ -743,6 +844,7 @@ int gpx_sparse_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, co
   const bool het = noise_variances != nullptr;
   GPX_CHECK(sparse_args(c, parts, Z, M, lml, grad, dZ, het, dL_dR));
   if (c->dist) GPX_FAIL("composite kernels are single-GPU");
+  if (het && c->sparse->P > MAX_P) GPX_FAIL("the heteroscedastic sparse evaluation serves at most 8 output columns");
   MultiKern mk;
   double kdiag;
   GPX_CHECK(fill_mk(mk, parts, nparts, c->sparse->D, &kdiag));
@@ -824,6 +926,7 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
   if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to differentiate the prediction of");
   if (Mn < 1) GPX_FAIL("empty Xnew");
   if (c->dist) GPX_FAIL("predictive gradients are single-GPU");
+  if (c->sparse->P > MAX_P) GPX_FAIL("predictive gradients serve at most 8 output columns");
   SparseState* s = c->sparse;
   const MultiKern& k = s->mk;
   GPX_CHECK(pred_grad_check(k));
@@ -857,6 +960,20 @@ int gpx_sparse_predictive_gradients(gpx_ctx* c, const double* Xnew, int64_t Mn, 
 
 }  // extern "C"
 
+// mu ([P][L]) = K(Xnew, Z) woodbury_vector for the L padded rows of Kxz (column-major, leading dimension L): MAX_P outputs
+// per launch_row_dot; part holds RSPLIT min(P, MAX_P) L doubles
+constexpr int MEAN_RSPLIT = 64;
+static int sparse_mean(gpx_ctx* c, const double* Kxz, long L, double* part, double* mu) {
+  SparseState* s = c->sparse;
+  for (int q0 = 0; q0 < s->P; q0 += MAX_P) {
+    const int pc = std::min(MAX_P, s->P - q0);
+    GPX_CHECK(launch_row_dot(Kxz, L, L, s->M, pc, s->Cm + (size_t)q0 * s->Mpad, s->Mpad, MEAN_RSPLIT, part,
+                             mu + (size_t)q0 * L, c->st));
+    GPX_CHECK(launched(c, 2));
+  }
+  return 0;
+}
+
 // The latent predictive covariance and mean of the last sparse evaluation at the prepared test points pn (posterior.py:
 // 220-238 with pred_var = Z): Sigma = K(Xnew) - K(Xnew, Z) W K(Z, Xnew) into Kss (pn.ld^2, column-major, exactly
 // symmetric: the lower tiles of the product term mirrored), mu = K(Xnew, Z) woodbury_vector into mu ([P][pn.ld]).
@@ -868,21 +985,19 @@ static int sparse_joint(gpx_ctx* c, const PointSet& pn, TmpBuf& Kss, TmpBuf& mu)
   double* W = nullptr;
   GPX_CHECK(woodbury_inv(c, &W));
   TmpBuf Kxz(st), Vt(st), prod(st), part(st);
-  constexpr int RSPLIT = 64;
   GPX_CHECK(Kxz.alloc((size_t)L * Mpad));
   GPX_CHECK(Vt.alloc((size_t)L * Mpad));
   GPX_CHECK(prod.alloc((size_t)L * L));
   GPX_CHECK(Kss.alloc((size_t)L * L));
   GPX_CHECK(mu.alloc((size_t)s->P * L));
-  GPX_CHECK(part.alloc((size_t)RSPLIT * s->P * L));
+  GPX_CHECK(part.alloc((size_t)MEAN_RSPLIT * std::min(s->P, MAX_P) * L));
   // K(Xnew, Z) with element (m, a) at m + a * L: test points thread-mapped, zero padded
   GPX_CUDA(cudaMemsetAsync(Kxz.p, 0, (size_t)L * Mpad * 8, st));
   GPX_CHECK(build_K(c, s->mk, s->D, pn, s->zpts(), Kxz.p, L));
   GPX_CHECK(launched(c));
   GPX_CHECK(gemm_nt(c, Kxz.p, L, W, Mpad, Vt.p, L, L, Mpad, Mpad, 1, 0));          // V^T = K(Xnew, Z) W (W symmetric)
   GPX_CHECK(gemm_nt(c, Vt.p, L, Kxz.p, L, prod.p, L, L, L, Mpad, 2, 0));           // V^T K(Z, Xnew), lower tiles
-  GPX_CHECK(launch_row_dot(Kxz.p, L, L, s->M, s->P, s->Cm, Mpad, RSPLIT, part.p, mu.p, st));   // mu = K(Xnew, Z) wv
-  GPX_CHECK(launched(c, 2));
+  GPX_CHECK(sparse_mean(c, Kxz.p, L, part.p, mu.p));                                // mu = K(Xnew, Z) wv
   GPX_CHECK(build_K(c, s->mk, s->D, pn, pn, Kss.p, L));
   GPX_CHECK(launched(c));
   return joint_combine(c, Kss.p, L, 0, prod.p, L, 1, pn.n, pn.n, Kss.p, L, 1);    // Sigma in place of K(Xnew)
@@ -915,11 +1030,12 @@ __global__ void __launch_bounds__(VAR_ROWS * VAR_SLICES) sparse_var_kernel(const
 
 namespace {
 // rows of one chunk of the diagonal prediction: the largest multiple of 128 whose temporaries, bounded by
-// 16 Mpad + 520 P + 1096 bytes per row (K(Xc, Z) and V^T, the mean's 64 partial sums, mean and variance, the uploaded and
-// prepared points at D, stacked dims and norms <= 64), fit in the 1 GiB the stream-ordered pool keeps cached (gpx_create);
-// never fewer than 128, never more than the test points padded to 128 (include/gpx.h states the same rule)
+// 16 Mpad + 512 min(P, 8) + 8 P + 1096 bytes per row (K(Xc, Z) and V^T, the mean's 64 partial sums of one slab of at most
+// 8 outputs, mean and variance, the uploaded and prepared points at D, stacked dims and norms <= 64), fit in the 1 GiB the
+// stream-ordered pool keeps cached (gpx_create); never fewer than 128, never more than the test points padded to 128
+// (include/gpx.h states the same rule)
 long predict_chunk_rows(long Mpad, int P, long Mn) {
-  const long per_row = 16 * Mpad + 520 * (long)P + 1096;
+  const long per_row = 16 * Mpad + 512 * (long)std::min(P, MAX_P) + 8 * (long)P + 1096;
   const long Lc = std::max<long>(TILE, (1l << 30) / per_row / TILE * TILE);
   return std::min<long>(Lc, (Mn + TILE - 1) / TILE * TILE);
 }
@@ -933,6 +1049,7 @@ int gpx_sparse_posterior_samples(gpx_ctx* c, const double* Xnew, int64_t Mn, con
                                  double* f, double* jitter_used) {
   if (!c) GPX_FAIL("null argument");
   if (!c->sparse || !c->sparse->have_eval) GPX_FAIL("no sparse evaluation to take the posterior from");
+  if (c->sparse->P > MAX_P) GPX_FAIL("the joint posterior serves at most 8 output columns");
   SparseState* s = c->sparse;
   GPX_CHECK(joint_check(c, Xnew, Mn, z, nz, f, jitter_used, s->P));
   GPX_CUDA(cudaSetDevice(c->device));
@@ -972,11 +1089,10 @@ int gpx_sparse_predict(gpx_ctx* c, const double* Xnew, int64_t Mn, int full_cov,
   const long Mpad = s->Mpad, Lc = predict_chunk_rows(Mpad, P, Mn);
   double* W = nullptr;
   GPX_CHECK(woodbury_inv(c, &W));
-  constexpr int RSPLIT = 64;
   TmpBuf Kxz(st), Vt(st), part(st), red(st);   // red: [P][Lc] means, then [Lc] variances
   GPX_CHECK(Kxz.alloc((size_t)Lc * Mpad));
   GPX_CHECK(Vt.alloc((size_t)Lc * Mpad));
-  GPX_CHECK(part.alloc((size_t)RSPLIT * P * Lc));
+  GPX_CHECK(part.alloc((size_t)MEAN_RSPLIT * std::min(P, MAX_P) * Lc));
   GPX_CHECK(red.alloc((size_t)(P + 1) * Lc));
   std::vector<double> h((size_t)P * Lc);
   for (long m0 = 0; m0 < Mn; m0 += Lc) {
@@ -989,8 +1105,7 @@ int gpx_sparse_predict(gpx_ctx* c, const double* Xnew, int64_t Mn, int full_cov,
     GPX_CHECK(build_K(c, k, s->D, pn, s->zpts(), Kxz.p, L));
     GPX_CHECK(launched(c));
     GPX_CHECK(gemm_nt(c, Kxz.p, L, W, Mpad, Vt.p, L, L, Mpad, Mpad, 1, 0));
-    GPX_CHECK(launch_row_dot(Kxz.p, L, L, s->M, P, s->Cm, Mpad, RSPLIT, part.p, red.p, st));   // mu ([P][L])
-    GPX_CHECK(launched(c, 2));
+    GPX_CHECK(sparse_mean(c, Kxz.p, L, part.p, red.p));                                   // mu ([P][L])
     double* vd = red.p + (size_t)P * L;
     sparse_var_kernel<<<(unsigned)(L / VAR_ROWS), dim3(VAR_ROWS, VAR_SLICES), 0, st>>>(Kxz.p, Vt.p, L, n, s->M, s->kdiag,
                                                                                        vd);
@@ -1704,7 +1819,7 @@ int gpx_svgp_begin(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const dou
   GPX_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->st;
   const int D = s->D;
-  s->have_eval = s->w_ready = s->w_own = s->sv_begun = false;
+  s->have_eval = s->dl_ready = s->w_ready = s->w_own = s->sv_begun = false;
   s->mk = mk;
   s->kdiag = kdiag;
   memset(&c->stats, 0, sizeof(c->stats));
@@ -1827,7 +1942,7 @@ int gpx_svgp_finish(gpx_ctx* c, const double* dF_dmu, const double* dF_dv, doubl
          *Tt = s->mm[7], *AdvA = s->mm[8], *W = s->mm[9];
   double *R = s->svm[0], *KSK = s->svm[1], *G = s->svm[2], *GU = s->svm[3], *Eh = s->svm[4], *H = s->svm[5];
   double *admu = s->svv + (size_t)SV_ADMU * Mpad, *rpart = s->svv + (size_t)SV_RPART * Mpad;
-  s->have_eval = s->w_ready = s->w_own = false;
+  s->have_eval = s->dl_ready = s->w_ready = s->w_own = false;
   GPX_CUDA(cudaMemsetAsync(b.vec[SB_DMU], 0, (size_t)2 * s->sv_cap * 8, st));
   GPX_CUDA(cudaMemcpyAsync(b.vec[SB_DMU], dF_dmu, (size_t)nb * 8, cudaMemcpyHostToDevice, st));
   GPX_CUDA(cudaMemcpyAsync(b.vec[SB_DV], dF_dv, (size_t)nb * 8, cudaMemcpyHostToDevice, st));
@@ -1888,6 +2003,26 @@ int gpx_svgp_finish(gpx_ctx* c, const double* dF_dmu, const double* dF_dv, doubl
   s->w_ready = s->w_own = true;
   s->have_eval = true;
   return 0;
+}
+
+}  // extern "C"
+
+extern "C" {
+
+/* gradients_X(dL_dKnm, X, Z) of the last VarDTC evaluation's kernel at its data points (sparse_gplvm.py:34), reduced from
+ * the dL_dKnm^T the evaluation left on the device: rows = data points, columns = inducing points, read untransposed with
+ * its rank-P term added as the evaluation's dL/dZ reduction added it. Launches: 2. */
+int gpx_sparse_grad_X(gpx_ctx* c, double* dX) {
+  if (!c || !dX) GPX_FAIL("null argument");
+  if (c->dist) GPX_FAIL("the sparse input gradient is single-GPU");
+  if (!c->sparse || !c->sparse->dl_ready)
+    GPX_FAIL("no VarDTC evaluation whose dL_dKnm is still on the device (gpx_sparse_eval, _het or _multi first)");
+  GPX_CUDA(cudaSetDevice(c->device));
+  SparseState* s = c->sparse;
+  GradFullParams gp = grad_params(s->mk, s->D, s->xpts(), s->zpts(), s->dLt, s->Mpad);
+  gp.ci = s->Yb; gp.ldci = s->Npad; gp.cj = s->Cm; gp.ldcj = s->Mpad; gp.cP = rank_p_cols(s);
+  GPX_CHECK(ensure_part(s, grad_X_doubles(c, s->mk, gp, s->D) * 8));
+  return grad_X(c, s->mk, gp, s->D, s->part, dX);
 }
 
 }  // extern "C"

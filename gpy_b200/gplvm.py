@@ -8,6 +8,11 @@ An evaluation is the exact evaluation of GPRegression plus the input gradient X.
 (gplvm.py:47-49), which the kernels take from the device (gpx_exact_grad_X) because dL_dK is the evaluation's
 DeviceGradient: nothing of size N^2 reaches the host. The latent inputs are a parameter without a transform, linked first,
 so the gradient and the optimizer space are ordered [latent_mean, kernel.., noise] as in the reference.
+
+    GPy.models.SparseGPLVM                  GPy/models/sparse_gplvm.py:9-34
+is the sparse model (VarDTC) with the latent inputs as a parameter: X.gradient = kern.gradients_X(dL_dKnm, X, Z)
+(sparse_gplvm.py:34) is reduced on the device from the dL_dKnm the evaluation left there (gpx_sparse_grad_X); the
+gradients_X_diag term of :33 is zero for every kernel the sparse evaluation takes.
 """
 import warnings
 
@@ -17,6 +22,7 @@ from .inference import Gaussian
 from .kern import RBF, Bias
 from .model import GP
 from .param import Param
+from .sparse import SparseGPRegression
 
 
 class PCA(object):
@@ -115,3 +121,35 @@ class GPLVM(GP):
         self.X = self.latent_mean.values
         super(GPLVM, self).parameters_changed()
         self.latent_mean.gradient = self.kern.gradients_X(self.grad_dict["dL_dK"], self.X, None)
+
+
+class SparseGPLVM(SparseGPRegression):
+    """GPy.models.SparseGPLVM (sparse_gplvm.py:9-34): SparseGPRegression of Y on latent inputs X that are themselves a
+    parameter ('latent space', linked first, no transform). The seeded draws follow the reference: initialize_latent's,
+    then SparseGPRegression's permutation for Z. The default kernel is SparseGPRegression's RBF(input_dim), isotropic.
+    Gradient and optimizer order: [latent space, inducing inputs, kernel.., noise]."""
+
+    def __init__(self, Y, input_dim, X=None, kernel=None, init="PCA", num_inducing=10, device=0, engine=None):
+        if X is None:
+            X, fracs = initialize_latent(init, input_dim, np.asarray(Y, dtype=np.float64))
+        X = np.array(X, dtype=np.float64)
+        self.latent_space = Param("latent space", X, transform=None)
+        self.latent_space.values = X                                   # keep the N x Q shape
+        self.latent_space.gradient = np.zeros_like(X)
+        super(SparseGPLVM, self).__init__(X, Y, kernel=kernel, num_inducing=num_inducing, device=device, engine=engine)
+        self._links.insert(0, self.latent_space)                      # link_parameter(self.X, 0)
+        self.latent_space._observers.append(self._child_changed)
+
+    def _free(self):
+        return [self.latent_space, self.Z]
+
+    def parameters_changed(self):
+        """sparse_gplvm.py:29-34: the sparse evaluation on the current latent inputs, then their gradient"""
+        self.X = self.latent_space.values
+        super(SparseGPLVM, self).parameters_changed()
+        dX = self.inference_method.engine.sparse_grad_X()
+        if "part_grads" not in self.grad_dict:                        # a lone kernel saw its active dims only
+            full = np.zeros_like(self.X)
+            full[:, self.kern.active_dims] = dX
+            dX = full
+        self.latent_space.gradient = dX

@@ -44,15 +44,22 @@ class SparseDeviceGradient(object):
     """Stand-in for `grad_dict['dL_dKnm']` (N x M) / `grad_dict['dL_dKmm']` (M x M) of VarDTC.inference
     (var_dtc.py:178-188). The device evaluation has already reduced both to d/d(variance, lengthscale) and dL/dZ
     (core/sparse_gp.py:110-118); the handle carries its share, keyed by the kernel state and the inducing inputs they were
-    computed for. `.T` is the same handle (SparseGP passes `dL_dKnm.T` to `gradients_X`, :118). It cannot turn into an
-    ndarray: the N x M matrix is never formed. A composite kernel's handle carries one gradient block per flattened leaf
-    (`part_grads`) instead of dvariance / dlengthscale."""
+    computed for. `.T` flips `transposed` (the shape cannot tell the orientation when N = M): SparseGP passes
+    `dL_dKnm.T` to `gradients_X` for dL/dZ (:118), SparseGPLVM the untransposed `dL_dKnm` for dL/dX (sparse_gplvm.py:34),
+    which a VarDTC handle (`engine`, `X`, `Z` given) reduces on the device from what the evaluation left there
+    (gpx_sparse_grad_X, once per handle). It cannot turn into an ndarray: the N x M matrix is never formed. A composite
+    kernel's handle carries one gradient block per flattened leaf (`part_grads`) instead of dvariance / dlengthscale."""
 
-    def __init__(self, key, role, shape, dvariance, dlengthscale, dZ, part_grads=None):
+    def __init__(self, key, role, shape, dvariance, dlengthscale, dZ, part_grads=None, engine=None, X=None, Z=None,
+                 transposed=False):
         self._key, self.role, self.shape = key, role, shape
         self.dvariance, self.dlengthscale, self.dZ = dvariance, dlengthscale, dZ
         self.part_grads = part_grads
         self.ndim, self.dtype = 2, np.dtype(np.float64)
+        self.transposed = transposed
+        self._engine, self._X, self._Z = engine, X, Z
+        self._serial = getattr(engine, "sparse_serial", None)
+        self._dX = [None]                     # shared with the .T views
 
     def matches(self, key):
         return self._key == key
@@ -60,8 +67,27 @@ class SparseDeviceGradient(object):
     @property
     def T(self):
         h = SparseDeviceGradient(self._key, self.role, self.shape[::-1], self.dvariance, self.dlengthscale, self.dZ,
-                                 self.part_grads)
+                                 self.part_grads, transposed=not self.transposed)
+        h._engine, h._X, h._Z, h._serial, h._dX = self._engine, self._X, self._Z, self._serial, self._dX
         return h
+
+    def wants_dX(self):
+        """True for dL_dKnm as VarDTC returned it (rows = data points): gradients_X then asks for dL/dX"""
+        return self.role == "knm" and not self.transposed
+
+    def grad_X(self, X, X2):
+        """kern.gradients_X(dL_dKnm, X, Z) from the device, for the X and Z the evaluation ran on"""
+        if self._engine is None:
+            raise ValueError("gradients_X of dL_dKnm: this evaluation keeps no input gradient on the device (VarDTC does)")
+        if getattr(self._engine, "sparse_serial", None) != self._serial:
+            raise ValueError("stale gradient handle: the device has evaluated again since")
+        X = np.asarray(X)
+        if X.shape != self._X.shape or not np.array_equal(X, self._X) or \
+                (X2 is not None and not np.array_equal(np.asarray(X2), self._Z)):
+            raise ValueError("gradients_X of dL_dKnm takes the inputs and inducing inputs of the evaluation")
+        if self._dX[0] is None:
+            self._dX[0] = self._engine.sparse_grad_X()
+        return self._dX[0]
 
     def __array__(self, dtype=None, copy=None):
         raise TypeError("%s of the device VarDTC evaluation is a handle to already-reduced gradients; the matrix itself is "
@@ -114,11 +140,12 @@ def _make_kernel(base, kind, ffi):
 
         def gradients_X(self, dL_dK, X, X2=None):
             """stationary.py:245-252,348-366 (gpx_kern_grad_X); with a handle of the device VarDTC evaluation: the dL/dZ
-            it already holds (core/sparse_gp.py:117-118)."""
+            it already holds (core/sparse_gp.py:117-118), or for the untransposed dL_dKnm dL/dX from the device
+            (sparse_gplvm.py:34)."""
             if isinstance(dL_dK, SparseDeviceGradient):
                 if not dL_dK.matches(self._gpx_state_key()):
                     raise ValueError("stale gradient handle: the kernel parameters changed since the sparse evaluation")
-                return dL_dK.dZ
+                return dL_dK.grad_X(X, X2) if dL_dK.wants_dX() else dL_dK.dZ
             if isinstance(dL_dK, DeviceGradient) and X2 is None:   # gplvm.py:49 on the exact evaluation of this kernel on X
                 g = dL_dK.grad_X(self._gpx_state_key(), X)
                 if g is not None:
@@ -234,9 +261,9 @@ def _make_combination(base, is_prod):
             return super(B200Combination, self).update_gradients_full(np.asarray(dL_dK, dtype=np.float64), X, X2)
 
         def gradients_X(self, dL_dK, X, X2=None):
-            if isinstance(dL_dK, SparseDeviceGradient):
+            if isinstance(dL_dK, SparseDeviceGradient):   # one gpx_sparse_grad_X for the whole combination
                 _check_sparse_handle(self, dL_dK)
-                return dL_dK.dZ
+                return dL_dK.grad_X(X, X2) if dL_dK.wants_dX() else dL_dK.dZ
             if isinstance(dL_dK, DeviceGradient) and X2 is None:   # one gpx_exact_grad_X for the whole combination
                 leaves = _flatten(self)
                 if leaves is not None and not any(hasattr(l, "_gpx_part_kind") for l, _ in leaves):
@@ -344,10 +371,13 @@ def _make_vardtc(base, kernel_types, ffi):
             M = Zs.shape[0]
             eng = self.engine
             if not self._data_key.matches(Xs, Yc):
+                if P > 8:
+                    eng.set_option("sparse_wide", 1)               # the sparse state's wide route (P <= 1024)
                 eng.sparse_set_data(Xs, Yc)
                 self._data_key.remember(Xs, Yc)
             if leaves is not None:
-                return self._inference_multi(eng, kern, leaves, Zs, likelihood, variance, N, P, M, Y_metadata, Z_tilde)
+                return self._inference_multi(eng, kern, leaves, Xs, Zs, likelihood, variance, N, P, M, Y_metadata,
+                                             Z_tilde)
             k, ard, var, ls = kern._gpx_theta()
             if variance.size > 1:                                  # het_noise (var_dtc.py:82-84)
                 lml, grad, dZ, dR = eng.sparse_eval_het(k, ard, var, ls, Zs, variance)
@@ -364,13 +394,13 @@ def _make_vardtc(base, kernel_types, ffi):
             dL_dKdiag = -0.5 * P * beta                            # _compute_dL_dpsi: dL_dpsi0 (:218)
             key = kern._gpx_state_key()
             dlen = np.atleast_1d(gk[1:])
-            knm = SparseDeviceGradient(key, "knm", (N, M), gk[0] - dL_dKdiag.sum(), dlen, dZ)
+            knm = SparseDeviceGradient(key, "knm", (N, M), gk[0] - dL_dKdiag.sum(), dlen, dZ, engine=eng, X=Xs, Z=Zs)
             kmm = SparseDeviceGradient(key, "kmm", (M, M), 0.0, np.zeros_like(dlen), np.zeros_like(dZ))
             post = LazySparsePosterior(eng, key, Zs)
             return post, lml, {"dL_dKmm": kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": knm, "dL_dthetaL": dL_dthetaL,
                                "dL_dm": None}
 
-        def _inference_multi(self, eng, kern, leaves, Zs, likelihood, variance, N, P, M, Y_metadata, Z_tilde):
+        def _inference_multi(self, eng, kern, leaves, Xs, Zs, likelihood, variance, N, P, M, Y_metadata, Z_tilde):
             """a sum / product kernel: ONE gpx_sparse_eval_multi. GPy's stock update_gradients_diag runs first
             (sparse_gp.py:110) and gives each leaf sum(dL_dKdiag) times the other variances of its term (add.py:79-80,
             prod.py:386-394); the dL_dKnm handle carries each leaf's total minus that share, the dL_dKmm handle zeros."""
@@ -387,7 +417,7 @@ def _make_vardtc(base, kernel_types, ffi):
             if Z_tilde is not None:
                 lml += Z_tilde                                     # var_dtc.py:166-170
             dL_dKdiag = -0.5 * P * beta                            # _compute_dL_dpsi: dL_dpsi0 (:218)
-            h_knm, h_kmm = _composite_handles(kern, leaves, grad, dL_dKdiag.sum(), dZ, N, M)
+            h_knm, h_kmm = _composite_handles(kern, leaves, grad, dL_dKdiag.sum(), dZ, N, M, engine=eng, X=Xs, Z=Zs)
             return LazySparsePosterior(eng, h_knm._key, Zs), lml, {"dL_dKmm": h_kmm, "dL_dKdiag": dL_dKdiag,
                                                                   "dL_dKnm": h_knm, "dL_dthetaL": dL_dthetaL,
                                                                   "dL_dm": None}
@@ -396,7 +426,7 @@ def _make_vardtc(base, kernel_types, ffi):
     return B200VarDTC
 
 
-def _composite_handles(kern, leaves, grad, diag, dZ, N, M):
+def _composite_handles(kern, leaves, grad, diag, dZ, N, M, engine=None, X=None, Z=None):
     """the dL_dKnm / dL_dKmm handles of a fused composite sparse evaluation. GPy's stock update_gradients_diag runs first
     (sparse_gp.py:110) and gives each leaf sum(dL_dKdiag) = diag times the other variances of its term (add.py:79-80,
     prod.py:386-394); the dL_dKnm handle carries each leaf's total minus that share, the dL_dKmm handle zeros."""
@@ -413,7 +443,7 @@ def _composite_handles(kern, leaves, grad, diag, dZ, N, M):
         zeros.append(np.zeros(n))
         i += n
     key = _composite_key(kern)
-    return (SparseDeviceGradient(key, "knm", (N, M), None, None, dZ, part_grads=knm),
+    return (SparseDeviceGradient(key, "knm", (N, M), None, None, dZ, part_grads=knm, engine=engine, X=X, Z=Z),
             SparseDeviceGradient(key, "kmm", (M, M), None, None, np.zeros_like(dZ), part_grads=zeros))
 
 

@@ -146,6 +146,8 @@ class VarDTC(object):
         Zs = kern._slice_X(Z)
         Y = np.ascontiguousarray(Y, dtype=np.float64)
         if not self._data_key.matches(Xs, Y):
+            if Y.shape[1] > 8:
+                eng.set_option("sparse_wide", 1)                   # the sparse state's wide route (P <= 1024)
             eng.sparse_set_data(Xs, Y)
             self._data_key.remember(Xs, Y)
         num_data, output_dim = Y.shape
@@ -183,6 +185,8 @@ class VarDTC(object):
         Zs = np.ascontiguousarray(Z, dtype=np.float64)
         Y = np.ascontiguousarray(Y, dtype=np.float64)
         if not self._data_key.matches(Xs, Y):
+            if Y.shape[1] > 8:
+                eng.set_option("sparse_wide", 1)                   # the sparse state's wide route (P <= 1024)
             eng.sparse_set_data(Xs, Y)
             self._data_key.remember(Xs, Y)
         num_data = Y.shape[0]
@@ -342,26 +346,34 @@ class SparseGPRegression(Parameterized):
     def _flat(self):
         return self.flattened_parameters()      # Z, then the kernel's and the likelihood's parameters in link order
 
+    def _free(self):
+        """the leading parameters without a transform"""
+        return [self.Z]
+
     @property
     def optimizer_array(self):
-        out = [self.Z.values.reshape(-1)]
-        for p in self._flat()[1:]:
+        free = self._free()
+        out = [p.values.reshape(-1) for p in free]
+        for p in self._flat()[len(free):]:
             out.append(Logexp.finv(p.values).reshape(-1))
         return np.concatenate(out)
 
     @optimizer_array.setter
     def optimizer_array(self, x):
-        nz = self.Z.values.size
-        self.Z.values[...] = x[:nz].reshape(self.Z.values.shape)
-        i = nz
-        for p in self._flat()[1:]:
+        free = self._free()
+        i = 0
+        for p in free:
+            p.values[...] = x[i:i + p.values.size].reshape(p.values.shape)
+            i += p.values.size
+        for p in self._flat()[len(free):]:
             p.values[...] = Logexp.f(x[i:i + p.size]).reshape(p.values.shape)
             i += p.size
         self.parameters_changed()
 
     def _grads_transformed(self):
-        g = [np.asarray(self.Z.gradient).reshape(-1)]
-        for p in self._flat()[1:]:
+        free = self._free()
+        g = [np.asarray(p.gradient).reshape(-1) for p in free]
+        for p in self._flat()[len(free):]:
             g.append(np.asarray(p.gradient, dtype=np.float64).reshape(-1) * Logexp.gradfactor(p.values).reshape(-1))
         return -np.concatenate(g)
 
@@ -381,11 +393,12 @@ class SparseGPRegression(Parameterized):
         return d
 
     def checkgrad(self, step=1e-6, tolerance=1e-3, sample=12, seed=0):
-        """finite differences on the kernel / noise parameters and on a random sample of inducing-point coordinates."""
+        """finite differences on the kernel / noise parameters and on a random sample of the unconstrained coordinates
+        (inducing inputs, and latent inputs in the sparse GPLVM)."""
         x = self.optimizer_array.copy()
         self.optimizer_array = x
         g = self._grads_transformed()
-        nz = self.Z.values.size
+        nz = sum(p.values.size for p in self._free())
         rng = np.random.default_rng(seed)
         idx = np.concatenate([rng.choice(nz, size=min(sample, nz), replace=False), np.arange(nz, x.size)])
         ok = True

@@ -50,8 +50,18 @@ enum { GPX_RBF = 0, GPX_EXPONENTIAL = 1, GPX_MATERN32 = 2, GPX_MATERN52 = 3,
  * -1 with a message. For P > 8:
  *   served : gpx_exact_eval, gpx_exact_eval_multi, gpx_get (every selector), gpx_predict, gpx_exact_grad_X;
  *   -2     : gpx_exact_eval_het, gpx_predictive_gradients, gpx_posterior_covariance, gpx_posterior_samples, the Laplace and
- *            EP entries (P = 1 only), a context with a communicator attached (gpx_set_data);
- *   sparse : gpx_sparse_set_data keeps its limit of 8. */
+ *            EP entries (P = 1 only), a context with a communicator attached (gpx_set_data).
+ * Output columns P of gpx_sparse_set_data: 1 .. 8, or 1 .. GPX_MAX_OUTPUTS once the context's option "sparse_wide" is 1
+ * (gpx_set_option; a context that never sets it keeps the limit of 8 it always had), more than 8 single-GPU only. Up to 8
+ * every sparse route is as it was. Above 8 the VarDTC evaluation with scalar noise runs every P-column product on the fp64 DMMA GEMM
+ * with Y held padded to whole tiles of outputs (Ppad): t^T = Y^T tmp^T (k-depth N), v, w and C against the triangular
+ * factors, w w^T (k-depth Ppad), and dL_dKnm^T = [W2 | C] [psi1 | beta Y]^T in one GEMM of k-depth Mpad + Ppad; data_fit
+ * = ||v||_F^2 is reduced on the device. Its launches depend on neither N nor P. It keeps 16 Npad Ppad bytes of Y (both
+ * layouts) and 8 Npad Ppad more beside psi1. For P > 8:
+ *   served : gpx_sparse_eval, gpx_sparse_eval_multi (scalar noise), gpx_sparse_get (every selector), gpx_sparse_predict
+ *            (8 outputs per mean launch), gpx_sparse_grad_X;
+ *   -2     : gpx_sparse_eval_het, gpx_sparse_eval_multi with per-point noise, gpx_sparse_predictive_gradients,
+ *            gpx_sparse_posterior_samples, FITC, EPDTC and SVGP (P = 1 only), a context with a communicator attached. */
 enum { GPX_MAX_OUTPUTS = 1024 };
 
 /* gpx_get selectors */
@@ -292,10 +302,11 @@ int gpx_sparse_get(gpx_ctx* ctx, int which, double* out);
  * evaluation (5 launches) and kept for all three. V^T = K(Xnew, Z) W runs on the DMMA GEMM; W is used as the reference
  * uses it, not in a factored form.
  * The diagonal streams over chunks of Lc test points, so M is not bounded by device memory:
- *   Lc = min(max(128, floor(2^30 / (16 Mz + 520 P + 1096) / 128) 128), M padded to 128), Mz = the inducing points padded
- *   to 128 — the largest multiple of 128 whose temporaries stay within the 1 GiB the stream-ordered pool keeps cached
- *   (Lc = 15872 at Mz = 4096, P = 1). Launches: 6 per chunk (upload, K-build, GEMM, 2 for the mean, 1 variance reduction).
- *   Peak temporaries: 8 Lc (2 Mz + 65 P + 1) plus the chunk's points.
+ *   Lc = min(max(128, floor(2^30 / (16 Mz + 512 min(P, 8) + 8 P + 1096) / 128) 128), M padded to 128), Mz = the inducing
+ *   points padded to 128 — the largest multiple of 128 whose temporaries stay within the 1 GiB the stream-ordered pool keeps
+ *   cached (Lc = 15872 at Mz = 4096, P = 1). Launches: 6 per chunk (upload, K-build, GEMM, 2 for the mean, 1 variance
+ *   reduction), with 2 more for the mean per further slab of 8 outputs when P > 8.
+ *   Peak temporaries: 8 Lc (2 Mz + 64 min(P, 8) + P + 1) plus the chunk's points.
  *   A row's mu and var do not depend on the chunking: every GEMM element has a fixed k-order and every reduction runs per
  *   row in a fixed order, so a point predicted alone, in a block or inside a multi-chunk call gets the same bits.
  * The full covariance is one pass: Launches: 8. Peak temporaries: those of gpx_sparse_posterior_samples before sampling,
@@ -327,6 +338,16 @@ int gpx_sparse_eval_het(gpx_ctx* ctx, int kind, int ard, double variance, const 
 int gpx_sparse_eval_multi(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* Z, int64_t M,
                           double noise_variance, const double* noise_variances, double* lml, double* grad, double* dZ,
                           double* dL_dR);
+/* The latent-input gradient of the sparse bound (SparseGPLVM, GPy/models/sparse_gplvm.py:33-34): after gpx_sparse_eval,
+ * _het or _multi, at any P that evaluation took, dX (N x D row-major, host) = sum_a dL_dKnm[n, a] dk(x_n, z_a)/dx_n, i.e.
+ * kern.gradients_X(dL_dKnm, X, Z) of the evaluation's kernel. The gradients_X_diag term is zero for every kernel the sparse
+ * evaluation takes (stationary.py:360-361, static.py:30-31) and is not added. It reads the dL_dKnm^T (M x N) the
+ * evaluation left on the device, with its rank-P term added as the evaluation's own dL/dZ reduction added it; nothing of
+ * size N x M crosses PCIe. Launches: 2. gpx_sparse_get, gpx_sparse_predict, gpx_sparse_predictive_gradients and
+ * gpx_sparse_posterior_samples leave it intact. Returns -2 with nothing touched when there is no such evaluation, when a
+ * FITC evaluation, EPDTC, SVGP or a new gpx_sparse_set_data has run since, with a communicator attached, or for a null
+ * pointer. */
+int gpx_sparse_grad_X(gpx_ctx* ctx, double* dX);
 /* FITC sparse GP regression (Snelson & Ghahramani's SPGP): FITC.inference
  * (GPy/inference/latent_function_inference/fitc.py:19-88) + SparseGP._update_gradients (core/sparse_gp.py:108-118) +
  * Gaussian.update_gradients, for the data of gpx_sparse_set_data (P = 1) and any kernel gpx_sparse_eval_multi takes (a
@@ -574,7 +595,9 @@ int gpx_measure_fp64_peak(gpx_ctx* ctx, double* tflops);
  *             allocation. The sparse evaluation factors Kmm and B = I + A with the same option,
  *   "profile" 1 (default) = per-phase times in gpx_stats, 0 = total_ms only,
  *   "ozaki"   0 = fp64 DMMA only, 1 = trailing update and K^-1 on the wgmma int8 path where applicable,
- *             -1 = default: env GPX_OZAKI, else 0.
+ *             -1 = default: env GPX_OZAKI, else 0,
+ *   "sparse_wide" 1 = gpx_sparse_set_data takes up to GPX_MAX_OUTPUTS output columns (the sparse wide route), 0 (default)
+ *             = at most 8; read by gpx_sparse_set_data only.
  * Any other name fails with "unknown option". */
 int gpx_set_option(gpx_ctx* ctx, const char* name, int64_t value);
 
