@@ -17,6 +17,7 @@ from .laplace import Bernoulli, Laplace, PosteriorLaplace, StudentT  # noqa: F40
 from .ep import EP, EPDTC, GPClassification, PosteriorEP, SparseGPClassification  # noqa: F401
 from .svgp import SVGP, SVGPInference  # noqa: F401
 from .gplvm import GPLVM, SparseGPLVM  # noqa: F401
+from .bgplvm import BayesianGPLVM  # noqa: F401
 from .vargauss import GPVariationalGaussianApproximation, VarGauss  # noqa: F401
 
 __version__ = "0.1.0"

@@ -109,6 +109,12 @@ EXPORTS = {
                                            _dp, _dp, _dp, _dp, _dp]),
     "gpx_sparse_eval_fitc": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, ctypes.c_int64,
                                             ctypes.c_double, _dp, _dp, _dp, _dp]),
+    "gpx_psi_stats": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), _dp, _dp, ctypes.c_int64, _dp, ctypes.c_int64,
+                                     ctypes.c_int, _dp, _dp]),
+    "gpx_psi_grads": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), _dp, _dp, ctypes.c_int64, _dp, ctypes.c_int64,
+                                     ctypes.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
+    "gpx_sparse_eval_psi": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int, _dp, _dp, ctypes.c_int64,
+                                           ctypes.c_double, _dp, _dp, _dp, _dp, _dp]),
     "gpx_laplace_begin": (ctypes.c_int, [_vp, ctypes.POINTER(GpxKernPart), ctypes.c_int]),
     "gpx_laplace_matvec": (ctypes.c_int, [_vp, _dp, _dp]),
     "gpx_laplace_newton": (ctypes.c_int, [_vp, _dp, _dp, _dp, ctypes.c_int, _dp, _dp, _dp]),
@@ -448,6 +454,56 @@ class Engine(object):
         self.sM = M
         self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
         return (lml.value, grad, dZ, dR) if het else (lml.value, grad, dZ)
+
+    def sparse_eval_psi(self, rbf, S, Z, noise):
+        """VarDTC with uncertain inputs q(X) = N(X, diag(S)) (var_dtc.py:107-123, sparse_gp.py:88-107) for the X of
+        sparse_set_data, the RBF part `rbf` (a part description on the columns 0 .. D-1) and a scalar noise variance ->
+        (lml without the KL term, grad [variance, lengthscale.., noise], dZ (M x D), dmu (N x D), dS (N x D))"""
+        Z, S = _f64(Z), _f64(S)
+        M = Z.shape[0]
+        if S.shape != (self.sN, self.sD):
+            raise ValueError("S must be N x D (%d x %d)" % (self.sN, self.sD))
+        arr = (GpxKernPart * 1)()
+        keep = []
+        ngrad = _fill_part(arr[0], rbf, keep)
+        lml = ctypes.c_double()
+        grad = np.zeros(ngrad + 1)
+        dZ = np.empty((M, self.sD))
+        dmu, dS = np.empty((self.sN, self.sD)), np.empty((self.sN, self.sD))
+        check(self._L.gpx_sparse_eval_psi(self._h, arr, 1, _ptr(S), _ptr(Z), M, float(noise), ctypes.byref(lml),
+                                          _ptr(grad), _ptr(dZ), _ptr(dmu), _ptr(dS)), "gpx_sparse_eval_psi")
+        self.sM = M
+        self.sparse_serial = getattr(self, "sparse_serial", 0) + 1
+        return lml.value, grad, dZ, dmu, dS
+
+    def psi_stats(self, rbf, mu, S, Z):
+        """the RBF psi-statistics (rbf_psi_comp.py:8-51) -> (psi0 (N,), psi1 (N x M), psi2 = sum_n psi2_n (M x M))"""
+        mu, S, Z = _f64(mu), _f64(S), _f64(Z)
+        (N, Q), M = mu.shape, Z.shape[0]
+        arr = (GpxKernPart * 1)()
+        keep = []
+        _fill_part(arr[0], rbf, keep)
+        psi1, psi2 = np.empty((N, M)), np.empty((M, M))
+        check(self._L.gpx_psi_stats(self._h, arr, _ptr(mu), _ptr(S), N, _ptr(Z), M, Q, _ptr(psi1), _ptr(psi2)),
+              "gpx_psi_stats")
+        return np.full(N, float(rbf[4])), psi1, psi2
+
+    def psi_grads(self, rbf, mu, S, Z, dL_dpsi0, dL_dpsi1, dL_dpsi2):
+        """psiDerivativecomputations (rbf_psi_comp.py:53-73) for an (M x M) dL_dpsi2 -> (grad [variance, lengthscale..],
+        dZ (M x Q), dmu (N x Q), dS (N x Q))"""
+        mu, S, Z = _f64(mu), _f64(S), _f64(Z)
+        (N, Q), M = mu.shape, Z.shape[0]
+        d0 = _f64(np.broadcast_to(np.asarray(dL_dpsi0, dtype=np.float64).reshape(-1), (N,)))
+        d1, d2 = _f64(dL_dpsi1), _f64(dL_dpsi2)
+        if d1.shape != (N, M) or d2.shape != (M, M):
+            raise ValueError("dL_dpsi1 must be N x M and dL_dpsi2 M x M")
+        arr = (GpxKernPart * 1)()
+        keep = []
+        ngrad = _fill_part(arr[0], rbf, keep)
+        grad, dZ, dmu, dS = np.zeros(ngrad), np.empty((M, Q)), np.empty((N, Q)), np.empty((N, Q))
+        check(self._L.gpx_psi_grads(self._h, arr, _ptr(mu), _ptr(S), N, _ptr(Z), M, Q, _ptr(d0), _ptr(d1), _ptr(d2),
+                                    _ptr(grad), _ptr(dZ), _ptr(dmu), _ptr(dS)), "gpx_psi_grads")
+        return grad, dZ, dmu, dS
 
     def sparse_eval_fitc(self, parts, Z, noise):
         """one FITC evaluation (fitc.py:19-88 with the gradient wiring of sparse_gp.py:108-118) with the kernel described
@@ -834,3 +890,24 @@ def kern_grad_full(kind, ARD, variance, lengthscale, X, dL_dK, X2=None):
     check(lib().gpx_kern_grad_full(None, k, a, float(variance), _ptr(ls), _ptr(X), N, _ptr(X2), M, D, _ptr(dL_dK),
                                    ctypes.byref(dv), _ptr(dl)), "gpx_kern_grad_full")
     return dv.value, dl
+
+
+_psi_engine = None
+
+
+def _scratch():
+    """the context of the stand-alone psi entries outside an evaluation (created on first use, device 0)"""
+    global _psi_engine
+    if _psi_engine is None:
+        _psi_engine = Engine()
+    return _psi_engine
+
+
+def psi_stats(rbf, mu, S, Z):
+    """the RBF psi-statistics of an RBF part description (Engine.psi_stats) on a context of their own"""
+    return _scratch().psi_stats(rbf, mu, S, Z)
+
+
+def psi_grads(rbf, mu, S, Z, dL_dpsi0, dL_dpsi1, dL_dpsi2):
+    """psiDerivativecomputations (Engine.psi_grads) on a context of their own"""
+    return _scratch().psi_grads(rbf, mu, S, Z, dL_dpsi0, dL_dpsi1, dL_dpsi2)

@@ -20,6 +20,7 @@
 #include "gpx_ctx.cuh"
 #include "gpx_kernels.cuh"
 #include "gpx_ep.cuh"
+#include "gpx_psi.cuh"
 
 using namespace gpx;
 
@@ -147,6 +148,15 @@ __global__ void add_rank_p_kernel(double* __restrict__ dLt, long ld, long M, lon
   double v = dLt[i];
   for (int q = 0; q < P; q++) v = fma(C[(long)q * ld + a], Yb[(long)q * ldy + n], v);
   dLt[i] = v;
+}
+// uncertain inputs: dL_dpsi1 (n, a) = beta sum_q Y[q][n] C[q][a] (var_dtc.py:218), written at n + a ld (psi1's layout)
+__global__ void dl_dpsi1_kernel(const double* __restrict__ Y, long ldy, const double* __restrict__ C, long ldc, int P,
+                                double beta, long N, double* __restrict__ out, long ld) {
+  const long n = (long)blockIdx.x * blockDim.x + threadIdx.x, a = blockIdx.y;
+  if (n >= N) return;
+  double v = 0.0;
+  for (int q = 0; q < P; q++) v = fma(Y[(long)q * ldy + n], C[(long)q * ldc + a], v);
+  out[n + a * ld] = beta * v;
 }
 // out = a X + b Y + cdiag I + d sum_p u_p u_p^T   (n x n, leading dimension ld; X, Y, U may be null)
 __global__ void combine_kernel(double* __restrict__ out, long ld, long n, double a, const double* __restrict__ X, double b,
@@ -307,8 +317,10 @@ int gpx_sparse_set_data(gpx_ctx* c, const double* X, int64_t N, int D, const dou
 
 }  // extern "C"
 
-// psi1 = K(X, Z) of the state's kernel in both layouts (Kuf: M x N, Kfu: N x M), left on the device
-static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
+// psi1 = K(X, Z) of the state's kernel in both layouts (Kuf: M x N, Kfu: N x M), left on the device. build = false (the
+// uncertain-input evaluation, which writes its own psi1 into Kfu): Z and the points are set up, no K(X, Z) is built and
+// Kuf is not written; FITC and EPDTC, its only readers, build it again before they read it.
+static int psi_device(gpx_ctx* c, const double* Z, int64_t M, bool build = true) {
   SparseState* s = c->sparse;
   cudaStream_t st = c->st;
   const MultiKern& k = s->mk;
@@ -346,6 +358,7 @@ static int psi_device(gpx_ctx* c, const double* Z, int64_t M) {
   GPX_CHECK(prep_points(c, k, s->X, N, s->D, Npad, s->XsT, s->sqX));
   GPX_CHECK(prep_points(c, k, s->Z, M, s->D, Mpad, s->ZsT, s->sqZ));
   GPX_CHECK(launched(c, 2));
+  if (!build) return 0;
   GPX_CHECK(build_K(c, k, s->D, s->zpts(), s->xpts(), s->Kuf, Mpad));   // psi1^T: thread-mapped operand = inducing points
   GPX_CHECK(build_K(c, k, s->D, s->xpts(), s->zpts(), s->Kfu, Npad));   // psi1: thread-mapped operand = data points
   return launched(c, 2);
@@ -523,15 +536,25 @@ static void kern_grads(const SparseState* s, double ddiag, const std::vector<dou
   }
 }
 
+// uncertain inputs q(X) = N(X, diag(S)) of gpx_sparse_eval_psi: the lone RBF part, S on the host, dmu / dS out (host)
+struct PsiCall {
+  PsiParams pp;
+  const double* S;
+  double *dmu, *dS;
+};
+
 // One evaluation of the validated kernel k (Kdiag = kdiag, psi0 of every data point), which becomes the state's kernel.
 // noise_vec == nullptr: scalar noise variance `noise` (grad = [k's gradient block, noise variance]);
 // noise_vec (host, one variance per row held by this rank): grad = [k's gradient block], dL_dR (host, N x P row-major).
 // k's block: a single kernel's [variance, lengthscale..]; a composite's part blocks in order (part_ngrad entries each).
 // precision (host, one per row; sparse EP's marginal): the per-point form with beta_n = precision_n as given (no floor) and
 // Kmm factored with jitchol's ladder (max_tries) and no const_jitter; *jitter_used: what the ladder added.
+// psi (scalar noise only): the uncertain-input branches (var_dtc.py:107-123, sparse_gp.py:88-107): psi1 replaces Knm in
+// Kfu, A_raw = Lm^-1 psi2 Lm^-T, and the psi gradient passes replace the Knm reductions.
 static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const double* Z, int64_t M, double noise,
                             const double* noise_vec, double* lml, double* grad, double* dZ, double* dL_dR_out,
-                            const double* precision = nullptr, int max_tries = 5, double* jitter_used = nullptr) {
+                            const double* precision = nullptr, int max_tries = 5, double* jitter_used = nullptr,
+                            const PsiCall* psi = nullptr) {
   const bool het = noise_vec != nullptr || precision != nullptr;
   GPX_CUDA(cudaSetDevice(c->device));
   SparseState* s = c->sparse;
@@ -563,9 +586,19 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
     GPX_CUDA(cudaMemcpyAsync(s->hb + Npd, hbeta.data(), (size_t)Npd * 8, cudaMemcpyHostToDevice, st));
     GPX_CUDA(cudaStreamSynchronize(st));   // the host vectors are pageable
   }
-  GPX_CHECK(psi_device(c, Z, M));
+  GPX_CHECK(psi_device(c, Z, M, psi == nullptr));
   const long Mpad = s->Mpad, N = s->Ntot, Npad = s->Npad;
   const int D = s->D, P = s->P, mt = (int)(Mpad / TILE);
+  TmpBuf psiS(st), psiPre(st);
+  PsiDev pd;
+  if (psi) {   // psi1 (rbf_psi_comp.py:22-34) in Kfu, the layout every consumer of psi1 reads
+    GPX_CHECK(psiS.alloc((size_t)s->N * D));
+    GPX_CHECK(psiPre.alloc((size_t)s->N * (2 * D + 2)));
+    GPX_CUDA(cudaMemcpyAsync(psiS.p, psi->S, (size_t)s->N * D * 8, cudaMemcpyHostToDevice, st));
+    pd.mu = s->X; pd.S = psiS.p; pd.Z = s->Z; pd.pre = psiPre.p;
+    GPX_CHECK(psi_prep(c, psi->pp, pd));
+    GPX_CHECK(psi1_build(c, psi->pp, pd, s->Kfu, 1, Npad));
+  }
   const int ngk = kern_ngrad(s->mk);   // entries of the kernel's gradient block
   constexpr int RSPLIT = 64;
   // P > MAX_P (scalar noise): every P-column product on the DMMA GEMM, the vectors held transposed as [Mpad][Ppad]
@@ -624,7 +657,10 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
     GPX_CHECK(launched(c));
     Yrow = s->Yb;
   }
-  {
+  if (psi) {   // A_raw = Lm^-1 psi2 Lm^-T (var_dtc.py:119-121), psi2 summed over the points into Bd (free until B)
+    GPX_CHECK(psi2_build(c, psi->pp, pd, Bd, Mpad, Mpad));
+    GPX_CHECK(sandwich(c, Lmi, Bd, T, Ar));
+  } else {
     GemmParams pg = gemm_defaults();   // A_raw = tmp tmp^T (lower tiles), k-depth = Npad
     pg.mode = GEMM_PANEL; pg.plain = 2;
     pg.A = Tuf; pg.lda = Mpad; pg.B = Tuf; pg.ldb = Mpad; pg.C = Ar; pg.ldc = Mpad;
@@ -727,7 +763,15 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
     GPX_CUDA(cudaMemcpyAsync(s->Cm, Cv, (size_t)P * Mpad * 8, cudaMemcpyDeviceToDevice, st));
   }
   std::vector<double> g_knm(ngk, 0.0);
-  GPX_CHECK(knm_grads_device(c, beta, bvec, g_knm.data(), dZ));                         // dZ <- Knm part
+  if (psi) {   // dL_dpsi1 = beta Y C^T, dL_dpsi2 = beta dL_dpsi2_beta (var_dtc.py:218-229) -> the psi gradient passes
+    dl_dpsi1_kernel<<<dim3((unsigned)((s->N + 255) / 256), (unsigned)M), 256, 0, st>>>(s->Y, Npad, s->Cm, Mpad, P, beta,
+                                                                                       s->N, s->dLt, Npad);
+    GPX_CHECK(launched(c));
+    GPX_CHECK(combine(c, E, Mpad, 0.5 * beta, E, 0.0, nullptr, 0.0));
+    GPX_CHECK(psi_grads(c, psi->pp, pd, s->Kfu, s->dLt, 1, Npad, E, Mpad, g_knm.data(), dZ, psi->dmu, psi->dS));
+  } else {
+    GPX_CHECK(knm_grads_device(c, beta, bvec, g_knm.data(), dZ));                       // dZ <- Knm part
+  }
   {
     int rank = 0, G = 1;
     dist_world(c, &rank, &G);
@@ -814,7 +858,7 @@ static int sparse_eval_impl(gpx_ctx* c, const MultiKern& k, double kdiag, const 
   kern_grads(s, dvar_diag, g_knm, g_kmm, grad);
   grad[ngk] = dL_dR;
   s->have_eval = true;
-  s->dl_ready = !precision;
+  s->dl_ready = !precision && !psi;
   return 0;
 }
 
@@ -852,6 +896,23 @@ int gpx_sparse_eval_multi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, co
     if (mk.part[p].kind == GPX_RATQUAD || mk.part[p].kind == GPX_STDPERIODIC)
       GPX_FAIL("RatQuad and StdPeriodic parts are not on the sparse evaluation (no device gradients_X)");
   return sparse_eval_impl(c, mk, kdiag, Z, M, het ? 0.0 : noise_variance, noise_variances, lml, grad, dZ, dL_dR);
+}
+
+int gpx_sparse_eval_psi(gpx_ctx* c, const gpx_kern_part* parts, int nparts, const double* S, const double* Z, int64_t M,
+                        double noise_variance, double* lml, double* grad, double* dZ, double* dmu, double* dS) {
+  GPX_CHECK(sparse_args(c, parts, Z, M, lml, grad, dZ, false, nullptr));
+  if (!S || !dmu || !dS) GPX_FAIL("null argument");
+  if (c->dist) GPX_FAIL("the uncertain-input evaluation is single-GPU");
+  SparseState* s = c->sparse;
+  PsiCall pc{};
+  GPX_CHECK(psi_params(parts, nparts, s->D, &pc.pp));
+  GPX_CHECK(psi_check_S(S, s->N, s->D));
+  pc.pp.N = s->N; pc.pp.M = M;
+  pc.S = S; pc.dmu = dmu; pc.dS = dS;
+  MultiKern mk;
+  double kdiag;
+  GPX_CHECK(fill_mk(mk, parts, nparts, s->D, &kdiag));
+  return sparse_eval_impl(c, mk, kdiag, Z, M, noise_variance, nullptr, lml, grad, dZ, nullptr, nullptr, 5, nullptr, &pc);
 }
 
 /* which: 0 woodbury_vector (M x P row-major), 1 woodbury_inv (M x M), 2 Kmm (+ the evaluation's const_jitter I: 1e-8

@@ -95,6 +95,45 @@ class SparseDeviceGradient(object):
                             "dL_dKnm" if self.role == "knm" else "dL_dKmm"))
 
 
+class PsiDeviceGradient(object):
+    """Stand-in for `grad_dict['dL_dpsi1']` (N x M) / `grad_dict['dL_dpsi2']` (M x M) of VarDTC.inference with uncertain
+    inputs (var_dtc.py:178-183). The device evaluation (gpx_sparse_eval_psi) has already reduced them, with dL_dpsi0 and
+    dL_dKmm, to the kernel's gradient, dZ and the gradients of q(X)'s mean and variance; the plugin RBF's
+    update_gradients_expectations, gradients_Z_expectations and gradients_qX_expectations (sparse_gp.py:95-107,
+    bayesian_gplvm.py:92-97) hand those back when given this handle for the kernel state, Z and q(X) it was computed for,
+    while the engine holds that evaluation."""
+
+    def __init__(self, key, role, shape, grad, dZ, dmu, dS, engine, mu, S, Z):
+        self._key, self.role, self.shape = key, role, shape
+        self.grad, self.dZ, self.dmu, self.dS = grad, dZ, dmu, dS
+        self.ndim, self.dtype = 2, np.dtype(np.float64)
+        self._engine, self._mu, self._S, self._Z = engine, mu, S, Z
+        self._serial = getattr(engine, "sparse_serial", None)
+
+    def sibling(self, role, shape):
+        h = PsiDeviceGradient(self._key, role, shape, self.grad, self.dZ, self.dmu, self.dS, self._engine, self._mu,
+                              self._S, self._Z)
+        h._serial = self._serial
+        return h
+
+    def check(self, key, Z, qX):
+        """ValueError unless the handle belongs to this kernel state, Z, q(X) and the engine's last evaluation"""
+        if key != self._key or getattr(self._engine, "sparse_serial", None) != self._serial:
+            raise ValueError("stale gradient handle: the device has evaluated other parameters since")
+        if not (np.array_equal(np.asarray(Z), self._Z) and np.array_equal(np.asarray(qX.mean), self._mu)
+                and np.array_equal(np.asarray(qX.variance), self._S)):
+            raise ValueError("the psi gradient handle takes the inducing inputs and q(X) of its evaluation")
+
+    def __array__(self, dtype=None, copy=None):
+        raise TypeError("dL_d%s of the device evaluation is a handle to already-reduced gradients; the matrix itself is "
+                        "never materialised (use the gpy_plugin RBF, or the stock VarDTC)" % self.role)
+
+
+def _normal_posterior(qX):
+    """q(X) is a NormalPosterior (not a spike-and-slab one): the device's psi-statistics apply"""
+    return type(qX).__name__ == "NormalPosterior" and hasattr(qX, "mean") and hasattr(qX, "variance")
+
+
 def _make_kernel(base, kind, ffi):
     class B200Kernel(base):
         _gpx_kind = kind
@@ -153,6 +192,68 @@ def _make_kernel(base, kind, ffi):
             k, ard, var, ls = self._gpx_theta()
             return ffi.kern_grad_X(k, ard, var, ls, np.asarray(X, dtype=np.float64), np.asarray(dL_dK, dtype=np.float64),
                                    None if X2 is None else np.asarray(X2, dtype=np.float64))
+
+        if kind == "rbf":
+            # the expectations under q(X) = N(mu, diag(S)) (rbf.py:344-367): the device's psi-statistics for a
+            # NormalPosterior on up to 16 latent columns; a spike-and-slab posterior and psi2n stay the reference's
+            def _gpx_psi_ok(self, qX):
+                return _normal_posterior(qX) and 1 <= np.asarray(qX.mean).shape[1] <= 16
+
+            def _gpx_psi_desc(self, Q):
+                k, ard, var, ls = self._gpx_theta()
+                return ("rbf", ard, 0, list(range(Q)), var, ls)
+
+            def _gpx_psi_args(self, Z, qX):
+                mu = np.ascontiguousarray(qX.mean, dtype=np.float64)
+                S = np.ascontiguousarray(qX.variance, dtype=np.float64)
+                return self._gpx_psi_desc(mu.shape[1]), mu, S, np.ascontiguousarray(Z, dtype=np.float64)
+
+            def psi0(self, Z, variational_posterior):
+                if not self._gpx_psi_ok(variational_posterior):
+                    return super(B200Kernel, self).psi0(Z, variational_posterior)
+                return np.full(np.asarray(variational_posterior.mean).shape[0], self._gpx_theta()[2])
+
+            def psi1(self, Z, variational_posterior):
+                if not self._gpx_psi_ok(variational_posterior):
+                    return super(B200Kernel, self).psi1(Z, variational_posterior)
+                return ffi.psi_stats(*self._gpx_psi_args(Z, variational_posterior))[1]
+
+            def psi2(self, Z, variational_posterior):
+                if not self._gpx_psi_ok(variational_posterior):
+                    return super(B200Kernel, self).psi2(Z, variational_posterior)
+                return ffi.psi_stats(*self._gpx_psi_args(Z, variational_posterior))[2]
+
+            def _gpx_psi_derivs(self, dL_dpsi0, dL_dpsi1, dL_dpsi2, Z, qX):
+                """(grad [variance, lengthscale..], dZ, dmu, dS): from the handle of the device evaluation, or from
+                gpx_psi_grads for host arrays; None when the reference's method applies"""
+                if isinstance(dL_dpsi1, PsiDeviceGradient):
+                    dL_dpsi1.check(self._gpx_state_key(), Z, qX)
+                    return dL_dpsi1.grad, dL_dpsi1.dZ, dL_dpsi1.dmu, dL_dpsi1.dS
+                if not self._gpx_psi_ok(qX) or np.ndim(dL_dpsi2) != 2:
+                    return None
+                return ffi.psi_grads(*self._gpx_psi_args(Z, qX), dL_dpsi0, dL_dpsi1, dL_dpsi2)
+
+            def update_gradients_expectations(self, dL_dpsi0, dL_dpsi1, dL_dpsi2, Z, variational_posterior):
+                r = self._gpx_psi_derivs(dL_dpsi0, dL_dpsi1, dL_dpsi2, Z, variational_posterior)
+                if r is None:
+                    return super(B200Kernel, self).update_gradients_expectations(dL_dpsi0, dL_dpsi1, dL_dpsi2, Z,
+                                                                                 variational_posterior)
+                self.variance.gradient = r[0][0]
+                self.lengthscale.gradient = r[0][1:] if self.ARD else r[0][1]
+
+            def gradients_Z_expectations(self, dL_dpsi0, dL_dpsi1, dL_dpsi2, Z, variational_posterior):
+                r = self._gpx_psi_derivs(dL_dpsi0, dL_dpsi1, dL_dpsi2, Z, variational_posterior)
+                if r is None:
+                    return super(B200Kernel, self).gradients_Z_expectations(dL_dpsi0, dL_dpsi1, dL_dpsi2, Z,
+                                                                            variational_posterior)
+                return r[1]
+
+            def gradients_qX_expectations(self, dL_dpsi0, dL_dpsi1, dL_dpsi2, Z, variational_posterior):
+                r = self._gpx_psi_derivs(dL_dpsi0, dL_dpsi1, dL_dpsi2, Z, variational_posterior)
+                if r is None:
+                    return super(B200Kernel, self).gradients_qX_expectations(dL_dpsi0, dL_dpsi1, dL_dpsi2, Z,
+                                                                             variational_posterior)
+                return r[2], r[3]
 
     B200Kernel.__name__ = B200Kernel.__qualname__ = base.__name__
     return B200Kernel
@@ -351,6 +452,9 @@ def _make_vardtc(base, kernel_types, ffi):
 
         def inference(self, kern, X, Z, likelihood, Y, Y_metadata=None, mean_function=None, precision=None, Lm=None,
                       dL_dKmm=None, psi0=None, psi1=None, psi2=None, Z_tilde=None):
+            if self._psi_route(kern, X, likelihood, Y_metadata, mean_function, precision, Lm, dL_dKmm, psi0, psi1,
+                               psi2):
+                return self._inference_psi(kern, X, Z, likelihood, Y, Y_metadata, Z_tilde)
             plain_X = isinstance(X, np.ndarray)                    # a VariationalPosterior is not an ndarray subclass
             leaves = _flatten(kern) if hasattr(kern, "_gpx_is_prod") else None
             if leaves is not None and any(not (hasattr(l, "_gpx_kind") or type(l).__name__ in ("White", "Bias"))
@@ -399,6 +503,49 @@ def _make_vardtc(base, kernel_types, ffi):
             post = LazySparsePosterior(eng, key, Zs)
             return post, lml, {"dL_dKmm": kmm, "dL_dKdiag": dL_dKdiag, "dL_dKnm": knm, "dL_dthetaL": dL_dthetaL,
                                "dL_dm": None}
+
+        def _psi_route(self, kern, X, likelihood, Y_metadata, mean_function, precision, Lm, dL_dKmm, psi0, psi1, psi2):
+            """uncertain inputs on the device: a NormalPosterior X on up to 16 columns, a lone plugin RBF on all of them in
+            order, a scalar Gaussian noise, no mean function and nothing precomputed"""
+            if not _normal_posterior(X) or getattr(kern, "_gpx_kind", None) != "rbf":
+                return False
+            if mean_function is not None or precision is not None or any(
+                    a is not None for a in (Lm, dL_dKmm, psi0, psi1, psi2)):
+                return False
+            Q = np.asarray(X.mean).shape[1]
+            if not (1 <= Q <= 16) or not np.array_equal(np.atleast_1d(kern.active_dims), np.arange(Q)):
+                return False
+            return np.asarray(likelihood.gaussian_variance(Y_metadata)).size == 1
+
+        def _inference_psi(self, kern, X, Z, likelihood, Y, Y_metadata, Z_tilde):
+            """ONE gpx_sparse_eval_psi (var_dtc.py:66-215 with uncertain inputs, sparse_gp.py:88-107); dL_dpsi0 is the
+            real N-vector (:218), dL_dpsi1 / dL_dpsi2 are handles carrying the reduced gradients, dL_dKmm a handle of
+            zeros (its share is inside the expectations' gradients)"""
+            mu = np.ascontiguousarray(X.mean, dtype=np.float64)
+            S = np.ascontiguousarray(X.variance, dtype=np.float64)
+            Zs = np.ascontiguousarray(Z, dtype=np.float64)
+            Yc = np.ascontiguousarray(Y, dtype=np.float64)
+            N, P = Yc.shape
+            M = Zs.shape[0]
+            eng = self.engine
+            if not self._data_key.matches(mu, Yc):
+                if P > 8:
+                    eng.set_option("sparse_wide", 1)
+                eng.sparse_set_data(mu, Yc)
+                self._data_key.remember(mu, Yc)
+            noise = float(np.asarray(likelihood.gaussian_variance(Y_metadata)).reshape(-1)[0])
+            k, ard, var, ls = kern._gpx_theta()
+            lml, grad, dZ, dmu, dS = eng.sparse_eval_psi(("rbf", ard, 0, list(range(mu.shape[1])), var, ls), S, Zs, noise)
+            if Z_tilde is not None:
+                lml += Z_tilde                                     # var_dtc.py:166-170
+            beta = 1.0 / max(noise, self.const_jitter)
+            key = kern._gpx_state_key()
+            h1 = PsiDeviceGradient(key, "psi1", (N, M), grad[:-1], dZ, dmu, dS, eng, mu, S, Zs)
+            kmm = SparseDeviceGradient(key, "kmm", (M, M), 0.0, np.zeros(grad.size - 2), np.zeros_like(dZ))
+            dL_dthetaL = likelihood.exact_inference_gradients(np.atleast_1d(grad[-1]), Y_metadata)
+            return LazySparsePosterior(eng, key, Zs), lml, {
+                "dL_dKmm": kmm, "dL_dpsi0": np.full(N, -0.5 * P * beta), "dL_dpsi1": h1,
+                "dL_dpsi2": h1.sibling("psi2", (M, M)), "dL_dthetaL": dL_dthetaL}
 
         def _inference_multi(self, eng, kern, leaves, Xs, Zs, likelihood, variance, N, P, M, Y_metadata, Z_tilde):
             """a sum / product kernel: ONE gpx_sparse_eval_multi. GPy's stock update_gradients_diag runs first

@@ -563,6 +563,35 @@ int gpx_svgp_begin(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const d
 int gpx_svgp_finish(gpx_ctx* ctx, const double* dF_dmu, const double* dF_dv, double* grad, double* dZ, double* dL_dm,
                     double* dL_dchol);
 
+/* Uncertain inputs (Bayesian GPLVM, GPy/models/bayesian_gplvm.py:20-101): the RBF psi-statistics of q(x_n) =
+ * N(mu_n, diag(S_n)) (GPy/kern/src/psi_comp/rbf_psi_comp.py:8-136) on the device. The kernel is one RBF part (`parts`,
+ * isotropic or ARD) on the latent columns 0 .. Q-1 in order, 1 <= Q <= 16; mu and S are N x Q row-major, S > 0 and
+ * finite; Z is M x Q row-major. psi2 is summed over the points; nothing of size N x M x M is formed. Every sum runs in a
+ * fixed order, so repeated calls give the same bits. Each entry returns -2 for another kernel, Q out of range, S <= 0 or
+ * non-finite, or a null pointer.
+ *   gpx_psi_stats : psi1 (N x M row-major, rbf_psi_comp.py:22-34) and psi2 = sum_n psi2_n (M x M, exactly symmetric,
+ *                   :36-51); psi0 is the variance. Launches: 4.
+ *   gpx_psi_grads : psiDerivativecomputations (:53-136) for dL_dpsi0 (N), dL_dpsi1 (N x M row-major) and dL_dpsi2 (M x M,
+ *                   symmetrised as the reference does): grad = [variance, lengthscale (1 or Q)], dZ (M x Q), dmu and dS
+ *                   (N x Q), row-major. Launches: 6.
+ *   gpx_sparse_eval_psi : VarDTC.inference with uncertain inputs (var_dtc.py:66-215: A = Lm^-1 psi2 Lm^-T beta,
+ *                   dL_dpsi0 = -P beta / 2, dL_dpsi1 = beta Y C^T, dL_dpsi2 = beta dL_dpsi2_beta, the homoscedastic
+ *                   dL_dR of :258-262) with SparseGP._update_gradients' uncertain branch (core/sparse_gp.py:88-107) and
+ *                   gradients_qX_expectations, for the data of gpx_sparse_set_data: its X is mu (D = Q), S is N x Q.
+ *                   lml: the bound without the KL term; grad: [variance, lengthscale.., noise variance] with the Kmm part;
+ *                   dZ: gradients_X(dL_dKmm, Z) + gradients_Z_expectations (M x Q); dmu, dS: N x Q, without the KL
+ *                   gradient. Any P of gpx_sparse_set_data (the wide route above 8). Only O(N Q + M Q) values cross PCIe.
+ *                   Afterwards gpx_sparse_get, gpx_sparse_predict, gpx_sparse_predictive_gradients and
+ *                   gpx_sparse_posterior_samples serve its posterior at certain test inputs; gpx_sparse_grad_X returns -2.
+ *                   Also -2 with a communicator attached or before gpx_sparse_set_data. Launches do not depend on N. */
+int gpx_psi_stats(gpx_ctx* ctx, const gpx_kern_part* part, const double* mu, const double* S, int64_t N, const double* Z,
+                  int64_t M, int Q, double* psi1, double* psi2);
+int gpx_psi_grads(gpx_ctx* ctx, const gpx_kern_part* part, const double* mu, const double* S, int64_t N, const double* Z,
+                  int64_t M, int Q, const double* dL_dpsi0, const double* dL_dpsi1, const double* dL_dpsi2, double* grad,
+                  double* dZ, double* dmu, double* dS);
+int gpx_sparse_eval_psi(gpx_ctx* ctx, const gpx_kern_part* parts, int nparts, const double* S, const double* Z, int64_t M,
+                        double noise_variance, double* lml, double* grad, double* dZ, double* dmu, double* dS);
+
 /* Measurement hooks (bench.py): device time of the last eval between CUDA events on the launching stream, the number
  * of kernels this library launched since creation, and per-phase accounting of the last eval. */
 typedef struct {
